@@ -59,6 +59,8 @@ extern "C" {
 #define PBB_WEIGHT_CONST 1    /* -2: constant 1/K */
 #define PBB_WEIGHT_TIED_TIME 2 /* (-3,): frequency-tied weights, one per (class, frame): array (K, T) */
 #define PBB_WEIGHT_TIED 3     /* (-3, -1): frequency-tied, one per class: array (K) */
+#define PBB_WEIGHT_FRAME 4    /* one weight per (bin, frame), the same for every class: array (F, T); only
+                                 pbb_log_pdf_to_affiliation (GMM / VMFMM weight_constant_axis (-2,)) */
 
 const char* pbb_last_error(void);
 int pbb_version(void);
@@ -231,6 +233,51 @@ int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
  * weight[f][k] = sum_t m[f][k][t] / sum_k sum_t m[f][k][t]. */
 int pbb_class_weight(const double* masked_affiliation, int F, int K, int T, double* weight,
                      void* stream);
+
+/* ------------------------------------------------------------------------
+ * Embedding mixture models with independent leading dims (pb_bss/distribution/gmm.py, vmfmm.py): B independent
+ * models of K classes over N embeddings of dimension E each.  embedding (B, N, E), weights / log pdfs (B, K, N).
+ * E <= 64, K <= 6 (the posterior, pbb_log_pdf_to_affiliation with F = B, T = N). */
+
+/* Gaussian.log_pdf (gaussian.py:36-56) with full covariance: mean (B, K, E), precision_cholesky U (B, K, E, E) (only
+ * the upper triangle is read), log_det (B, K) -> log_pdf (B, K, N).  The reference contracts sklearn's
+ * upper-triangular precision Cholesky factor with the einsum '...dD,...nD->...nd', i.e. white = U d, where sklearn's
+ * own density uses U^T d; the quadratic form is therefore d^T U^T U d and not d^T Sigma^-1 d (they agree for a
+ * diagonal Sigma only).  A drop-in returns what the reference returns, so this evaluates U d. */
+int pbb_gaussian_full_log_pdf(const double* embedding, const double* mean, const double* precision_cholesky,
+                              const double* log_det, int B, int N, int E, int K, double* log_pdf, void* stream);
+
+/* GaussianTrainer._fit (gaussian.py:152-193), covariance_type 'full', per (b, k) with the weights weight (B, K, N):
+ * mean (B, K, E) = sum w x / max(sum w, tiny), covariance (B, K, E, E) = sum w (x - mean)(x - mean)^T / that
+ * denominator.  Two passes; the N axis is split into chunks whose partial sums are added in chunk order (the chunking
+ * depends on B, N, K only), so results are bit-reproducible.  scratch: pbb_gaussian_full_fit_scratch_doubles. */
+size_t pbb_gaussian_full_fit_scratch_doubles(int B, int N, int E, int K);
+int pbb_gaussian_full_fit(const double* embedding, const double* weight, int B, int N, int E, int K, double* mean,
+                          double* covariance, double* scratch, void* stream);
+
+/* sklearn's _compute_precision_cholesky(covariance, 'full') and _compute_log_det_cholesky (Gaussian.__post_init__,
+ * gaussian.py:26-34) for M matrices covariance (M, E, E) (lower triangle read): L = cholesky(Sigma),
+ * precision_cholesky = (L^-1)^T (M, E, E), log_det = sum log diag (M).  *status (reset by the call) = 1 + index of the
+ * first matrix that is not positive definite (sklearn raises ValueError there). */
+int pbb_precision_cholesky(const double* covariance, int M, int E, double* precision_cholesky, double* log_det,
+                           int* status, void* stream);
+
+/* VonMisesFisher.log_pdf (von_mises_fisher.py:65-79): mean (B, K, E), concentration / log_norm (B, K) ->
+ * log_pdf (B, K, N) = concentration <mean, x / max(||x||, tiny)> - log_norm. */
+int pbb_vmf_log_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
+                    int B, int N, int E, int K, double* log_pdf, void* stream);
+
+/* The sums of VonMisesFisherTrainer._fit (von_mises_fisher.py:122-137) over x / max(||x||, tiny): resultant (B, K, E)
+ * = sum_n w x, total (B, K) = sum_n w; the rest (B*K*E numbers, scipy's ive) is host math.  Same chunked fixed-order
+ * reduction and scratch size as pbb_gaussian_full_fit. */
+int pbb_vmf_resultant(const double* embedding, const double* weight, int B, int N, int E, int K, double* resultant,
+                      double* total, double* scratch, void* stream);
+
+/* estimate_mixture_weight with weight_constant_axis (-2,) and a saliency (mixture_model_utils.py:178-201): the tuple
+ * is not caught by the reference's int test, so the masked affiliations (B, K, N) are summed over the classes and
+ * L1-normalised over that singleton axis: weight (B, N) = s / |s|, 0 where s == 0.  Feed it to
+ * pbb_log_pdf_to_affiliation as PBB_WEIGHT_FRAME. */
+int pbb_frame_weight(const double* masked_affiliation, int B, int K, int N, double* weight, void* stream);
 
 /* ------------------------------------------------------------------------
  * Complex Watson mixture model (pb_bss/distribution/cwmm.py, complex_watson.py).

@@ -12,7 +12,7 @@ LIB_PATH = os.environ.get('PBB_LIB') or os.path.join(_HERE, 'libpbb.so')
 
 PBB_C64, PBB_C128 = 0, 1
 NORM_NONE, NORM_EIGENVALUE, NORM_TRACE = 0, 1, 2
-WEIGHT_TIME, WEIGHT_CONST, WEIGHT_TIED_TIME, WEIGHT_TIED = 0, 1, 2, 3
+WEIGHT_TIME, WEIGHT_CONST, WEIGHT_TIED_TIME, WEIGHT_TIED, WEIGHT_FRAME = 0, 1, 2, 3, 4
 
 
 class CacgmmOptions(ctypes.Structure):
@@ -72,6 +72,13 @@ SIGNATURES = {
     'pbb_gaussian_fit': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_log_pdf_to_affiliation': (_i, [_vp, _vp, _d, _d, _vp, _i, _vp, _d, _i, _i, _i, _i, _vp, _vp, _vp]),
     'pbb_class_weight': (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    'pbb_gaussian_full_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    'pbb_gaussian_full_fit_scratch_doubles': (_sz, [_i, _i, _i, _i]),
+    'pbb_gaussian_full_fit': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_precision_cholesky': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_vmf_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    'pbb_vmf_resultant': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_frame_weight': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'pbb_dhtv_mapping': (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i), _i, _vp, _vp, _vp, _vp]),
     'pbb_dhtv_mapping_ex': (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i), _i, _vp, _vp, _vp, _i, _i, _vp]),
     'pbb_apply_mapping': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),

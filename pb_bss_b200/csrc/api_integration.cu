@@ -8,6 +8,11 @@
 //   pbb_log_pdf_to_affiliation    softmax * weight, clip (mixture_model_utils.py:7-55), optionally after the
 //                                 per-bin search over the K! pairings of spatial and spectral classes (:58-130)
 //   pbb_class_weight              L1-normalised sums of the masked affiliations  (gcacgmm.py:283-291)
+// and the batched pieces of the embedding mixture models GMM / VMFMM (gmm.py, vmfmm.py), B independent models:
+//   pbb_gaussian_full_log_pdf     full-covariance Gaussian, the reference's U d form (gaussian.py:36-56)
+//   pbb_gaussian_full_fit         weighted mean + full scatter, N split over CTAs (gaussian.py:152-193)
+//   pbb_precision_cholesky        sklearn's precision Cholesky + log det, one warp per matrix
+//   pbb_vmf_log_pdf / pbb_vmf_resultant / pbb_frame_weight
 // All reductions run in a fixed order (bit-reproducible).
 #include <cstring>
 
@@ -145,6 +150,7 @@ __device__ __forceinline__ double weight_of(const double* __restrict__ w, int mo
     case PBB_WEIGHT_CONST: return 1.0 / K;
     case PBB_WEIGHT_TIED_TIME: return w[(size_t)k * T + t];
     case PBB_WEIGHT_TIED: return w[k];
+    case PBB_WEIGHT_FRAME: return w[(size_t)f * T + t];
     default: return w[(size_t)f * K + k];
   }
 }
@@ -234,6 +240,266 @@ __global__ void class_weight_kernel(const double* __restrict__ m, int F, int K, 
   }
 }
 
+// ---- embedding mixture models with independent leading dims: B models, each (K, E[, E]) over N observations ----
+
+// Full-covariance Gaussian.log_pdf (gaussian.py:36-56) with the reference's einsum '...dD,...nD->...nd': white = U d
+// (sklearn's own log pdf uses U^T d), so the quadratic form is d^T U^T U d.  One thread per observation; the centred
+// row d lives in EM registers, U_k (upper triangle, the rest is zero) and mean_k are staged in shared memory per class.
+template <int EM>
+__global__ void __launch_bounds__(128) gaussian_full_log_pdf_kernel(
+    const double* __restrict__ x, const double* __restrict__ mean, const double* __restrict__ U,
+    const double* __restrict__ log_det, int N, int E, int K, double* __restrict__ out) {
+  extern __shared__ double sm[];  // U_k [E][E], mean_k [E]
+  double* us = sm;
+  double* ms = sm + E * E;
+  const int b = blockIdx.y, n = blockIdx.x * blockDim.x + threadIdx.x;
+  const double c0 = -0.5 * (double)E * log(2.0 * 3.14159265358979323846);
+  const double* __restrict__ xr = x + ((size_t)b * N + (n < N ? n : 0)) * E;
+  for (int k = 0; k < K; ++k) {
+    const size_t bk = (size_t)b * K + k;
+    __syncthreads();
+    for (int i = threadIdx.x; i < E * E; i += blockDim.x) us[i] = U[bk * E * E + i];
+    for (int i = threadIdx.x; i < E; i += blockDim.x) ms[i] = mean[bk * E + i];
+    __syncthreads();
+    if (n >= N) continue;
+    double d[EM];
+#pragma unroll
+    for (int j = 0; j < EM; ++j) d[j] = j < E ? xr[j] - ms[j] : 0.0;
+    double s = 0.0;
+    for (int i = 0; i < E; ++i) {
+      double w = 0.0;
+#pragma unroll
+      for (int j = 0; j < EM; ++j)
+        if (j >= i && j < E) w += us[i * E + j] * d[j];
+      s += w * w;
+    }
+    out[bk * N + n] = c0 + log_det[bk] - 0.5 * s;
+  }
+}
+
+constexpr int kFitTileN = 32;       // observations staged in shared memory per step
+constexpr int kFitThreads = 256;
+constexpr int kFitMaxAcc = (kIntMaxE * (kIntMaxE + 1) / 2 + kFitThreads - 1) / kFitThreads;
+constexpr int kFitTargetCtas = 528;  // 4 per SM of a 132-SM H100; the chunking depends on the shape only
+
+__host__ __device__ inline int fit_entries(int E) { return E * (E + 1) / 2 > E + 1 ? E * (E + 1) / 2 : E + 1; }
+
+// Weighted moments of one chunk of observations for one (b, k); xs holds the staged rows plus a column E of ones, so
+// both passes are acc += w * xs[n][i] * xs[n][j]:
+//   pass 0: entry e < E: (i, j) = (e, E) -> sum w x_e;  entry E: (E, E) -> sum w.  normalize != 0 stages the rows as
+//           x / max(||x||, tiny) (the von Mises-Fisher trainer's observations, von_mises_fisher.py:106-109)
+//   pass 1: entry p = packed upper triangle (i <= j, row-major): sum w (x_i - mean_i)(x_j - mean_j)
+// partial[c][bk][entry].  Every chunk has a fixed range of observations and a fixed thread order: bit-reproducible.
+__global__ void __launch_bounds__(kFitThreads, 1) gaussian_full_partial_kernel(
+    const double* __restrict__ x, const double* __restrict__ w, const double* __restrict__ mean, int N, int E, int K,
+    int chunk_len, int pass, int normalize, double* __restrict__ partial) {
+  __shared__ double xs[kFitTileN][kIntMaxE + 1];
+  __shared__ double ws[kFitTileN];
+  const int c = blockIdx.x, bk = blockIdx.y, b = bk / K, tid = threadIdx.x;
+  const int P = pass == 0 ? E + 1 : E * (E + 1) / 2;
+  int ij[kFitMaxAcc];  // i | j << 8
+  double acc[kFitMaxAcc];
+#pragma unroll
+  for (int r = 0; r < kFitMaxAcc; ++r) {
+    const int p = tid + r * kFitThreads;
+    acc[r] = 0.0;
+    ij[r] = 0;
+    if (p < P) {
+      if (pass == 0) ij[r] = p | E << 8;
+      else {
+        int i = 0, off = 0;
+        while (off + (E - i) <= p) { off += E - i; ++i; }
+        ij[r] = i | (i + (p - off)) << 8;
+      }
+    }
+  }
+  const double* __restrict__ xb = x + (size_t)b * N * E;
+  const double* __restrict__ wb = w + (size_t)bk * N;
+  const int n_begin = c * chunk_len, n_end = min(N, n_begin + chunk_len);
+  for (int n0 = n_begin; n0 < n_end; n0 += kFitTileN) {
+    const int rows = min(kFitTileN, n_end - n0);
+    __syncthreads();
+    for (int idx = tid; idx < kFitTileN * E; idx += kFitThreads) {
+      const int r = idx / E, e = idx - r * E;
+      double v = r < rows ? xb[(size_t)(n0 + r) * E + e] : 0.0;
+      if (pass == 1) v -= mean[(size_t)bk * E + e];
+      xs[r][e] = v;
+    }
+    if (tid < kFitTileN) { xs[tid][E] = 1.0; ws[tid] = tid < rows ? wb[n0 + tid] : 0.0; }
+    __syncthreads();
+    if (normalize) {
+      if (tid < kFitTileN) {
+        double n2 = 0.0;
+        for (int e = 0; e < E; ++e) n2 += xs[tid][e] * xs[tid][e];
+        const double nrm = fmax(sqrt(n2), kTiny);
+        for (int e = 0; e < E; ++e) xs[tid][e] /= nrm;
+      }
+      __syncthreads();
+    }
+    for (int r = 0; r < rows; ++r) {
+      const double wr = ws[r];
+#pragma unroll
+      for (int a = 0; a < kFitMaxAcc; ++a)
+        if (tid + a * kFitThreads < P) acc[a] += wr * xs[r][ij[a] & 255] * xs[r][ij[a] >> 8];
+    }
+  }
+  const size_t BK = gridDim.y;
+#pragma unroll
+  for (int a = 0; a < kFitMaxAcc; ++a) {
+    const int p = tid + a * kFitThreads;
+    if (p < P) partial[((size_t)c * BK + bk) * P + p] = acc[a];
+  }
+}
+
+// Sums the chunks in chunk order.  pass 0: denom[bk] = max(sum w, tiny), mean = sum w x / denom (if mean != null);
+// resultant = sum w x and total = sum w unscaled (if resultant != null).  pass 1: covariance[bk] = scatter / denom,
+// both triangles.
+__global__ void __launch_bounds__(kFitThreads) gaussian_full_reduce_kernel(
+    const double* __restrict__ partial, int nchunks, int E, int pass, double* __restrict__ denom,
+    double* __restrict__ mean, double* __restrict__ resultant, double* __restrict__ total,
+    double* __restrict__ covariance) {
+  __shared__ double den;
+  const int bk = blockIdx.x, BK = gridDim.x, tid = threadIdx.x;
+  const int P = pass == 0 ? E + 1 : E * (E + 1) / 2;
+  for (int p0 = 0; p0 < P; p0 += kFitThreads) {
+    const int p = p0 + tid;
+    double s = 0.0;
+    if (p < P)
+      for (int c = 0; c < nchunks; ++c) s += partial[((size_t)c * BK + bk) * P + p];
+    if (pass == 0) {  // P = E + 1 <= 65: a single round
+      if (p == E) {
+        den = fmax(s, kTiny);
+        denom[bk] = den;
+        if (total) total[bk] = s;
+      }
+      __syncthreads();
+      if (p < E) {
+        if (mean) mean[(size_t)bk * E + p] = s / den;
+        if (resultant) resultant[(size_t)bk * E + p] = s;
+      }
+    } else if (p < P) {
+      int i = 0, off = 0;
+      while (off + (E - i) <= p) { off += E - i; ++i; }
+      const int j = i + (p - off);
+      const double v = s / denom[bk];
+      covariance[((size_t)bk * E + i) * E + j] = v;
+      covariance[((size_t)bk * E + j) * E + i] = v;
+    }
+  }
+}
+
+// sklearn's _compute_precision_cholesky(covariance, 'full') (gaussian.py:26-34): L = cholesky(Sigma) (lower triangle
+// read, LAPACK potrf order), U = (L^-1)^T, log_det = sum log diag U.  One warp per matrix, L in shared memory; lane j
+// solves column j of L^-1 and keeps it in row j of U.  A pivot that is not > 0 (or NaN) stops the matrix and records
+// 1 + its index in *status (the smallest failing index wins).
+__global__ void __launch_bounds__(32) precision_cholesky_kernel(const double* __restrict__ cov, int E,
+                                                                double* __restrict__ U, double* __restrict__ log_det,
+                                                                int* __restrict__ status) {
+  extern __shared__ double L[];  // [E][E]
+  const int m = blockIdx.x, lane = threadIdx.x;
+  const double* __restrict__ A = cov + (size_t)m * E * E;
+  double* __restrict__ Um = U + (size_t)m * E * E;
+  for (int i = lane; i < E * E; i += 32) L[i] = A[i];
+  __syncwarp();
+  for (int j = 0; j < E; ++j) {
+    double djj = L[j * E + j];
+    for (int k = 0; k < j; ++k) djj -= L[j * E + k] * L[j * E + k];
+    if (!(djj > 0.0)) {
+      if (lane == 0) {
+        int old = atomicCAS(status, 0, m + 1);
+        while (old != 0 && old > m + 1) {
+          const int seen = atomicCAS(status, old, m + 1);
+          if (seen == old) break;
+          old = seen;
+        }
+        log_det[m] = NAN;
+      }
+      for (int i = lane; i < E * E; i += 32) Um[i] = NAN;
+      return;
+    }
+    const double ljj = sqrt(djj);
+    for (int i = j + 1 + lane; i < E; i += 32) {
+      double v = L[i * E + j];
+      for (int k = 0; k < j; ++k) v -= L[i * E + k] * L[j * E + k];
+      L[i * E + j] = v / ljj;
+    }
+    __syncwarp();
+    if (lane == 0) L[j * E + j] = ljj;
+    __syncwarp();
+  }
+  for (int j = lane; j < E; j += 32) {  // column j of X = L^-1 (forward substitution on e_j) -> row j of U
+    double* __restrict__ uj = Um + (size_t)j * E;
+    for (int i = 0; i < j; ++i) uj[i] = 0.0;
+    for (int i = j; i < E; ++i) {
+      double v = i == j ? 1.0 : 0.0;
+      for (int k = j; k < i; ++k) v -= L[i * E + k] * uj[k];
+      uj[i] = v / L[i * E + i];
+    }
+  }
+  __syncwarp();
+  if (lane == 0) {
+    double s = 0.0;
+    for (int i = 0; i < E; ++i) s += log(Um[(size_t)i * E + i]);
+    log_det[m] = s;
+  }
+}
+
+// VonMisesFisher.log_pdf (von_mises_fisher.py:65-79) for B models: out[b][k][n] = concentration[b][k]
+// <mean[b][k], x / max(||x||, tiny)> - log_norm[b][k].
+__global__ void __launch_bounds__(128) vmf_log_pdf_kernel(const double* __restrict__ x, const double* __restrict__ mean,
+                                                          const double* __restrict__ concentration,
+                                                          const double* __restrict__ log_norm, int N, int E, int K,
+                                                          double* __restrict__ out) {
+  __shared__ double ms[kIntMaxK * kIntMaxE];
+  const int b = blockIdx.y, n = blockIdx.x * blockDim.x + threadIdx.x;
+  for (int i = threadIdx.x; i < K * E; i += blockDim.x) ms[i] = mean[(size_t)b * K * E + i];
+  __syncthreads();
+  if (n >= N) return;
+  const double* __restrict__ xr = x + ((size_t)b * N + n) * E;
+  double dot[kIntMaxK], n2 = 0.0;
+#pragma unroll
+  for (int k = 0; k < kIntMaxK; ++k) dot[k] = 0.0;
+  for (int e = 0; e < E; ++e) {
+    const double v = xr[e];
+    n2 += v * v;
+#pragma unroll
+    for (int k = 0; k < kIntMaxK; ++k)
+      if (k < K) dot[k] += v * ms[k * E + e];
+  }
+  const double nrm = fmax(sqrt(n2), kTiny);
+#pragma unroll
+  for (int k = 0; k < kIntMaxK; ++k)
+    if (k < K) {
+      const size_t bk = (size_t)b * K + k;
+      out[bk * N + n] = concentration[bk] * (dot[k] / nrm) - log_norm[bk];
+    }
+}
+
+// Mixture weight of weight_constant_axis=(-2,) with a saliency (mixture_model_utils.py:191-201): the sum over the
+// classes, L1-normalised over its singleton class axis -> s / |s|, and 0 where s == 0 (eps_style 'where').
+__global__ void frame_weight_kernel(const double* __restrict__ m, int K, int N, double* __restrict__ w) {
+  const int b = blockIdx.y, n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  double s = 0.0;
+  for (int k = 0; k < K; ++k) s += m[((size_t)b * K + k) * N + n];
+  const double nrm = fabs(s);
+  w[(size_t)b * N + n] = s / (nrm == 0.0 ? 1e-10 : nrm);
+}
+
+struct FullFitChunks { int nchunks, chunk_len; };
+inline FullFitChunks full_fit_chunks(int B, int N, int K) {
+  const long long BK = (long long)B * K;
+  const int tiles = (N + kFitTileN - 1) / kFitTileN;
+  long long want = (kFitTargetCtas + BK - 1) / BK;
+  if (want > tiles) want = tiles;
+  if (want < 1) want = 1;
+  const int per = (int)((tiles + want - 1) / want);
+  FullFitChunks c;
+  c.chunk_len = per * kFitTileN;
+  c.nchunks = (N + c.chunk_len - 1) / c.chunk_len;
+  return c;
+}
+
 }  // namespace pbb
 
 using namespace pbb;
@@ -295,7 +561,7 @@ int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
                                void* stream) {
   PBB_CHECK_ARG(log_pdf_a != nullptr, 1, "log pdf is null");
   PBB_CHECK_ARG(weight != nullptr || weight_mode == PBB_WEIGHT_CONST, 5, "weight is null");
-  PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_TIED, 6, "bad weight_mode");
+  PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_FRAME, 6, "bad weight_mode");
   PBB_CHECK_ARG(F > 0 && T > 0, 10, "bad shape");
   PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 11, "need 0 < K <= 6 (K! pairings per bin)");
   PBB_CHECK_ARG(!inline_pa || log_pdf_b != nullptr, 9, "the inline alignment pairs TWO log pdfs");
@@ -315,6 +581,122 @@ int pbb_class_weight(const double* masked_affiliation, int F, int K, int T, doub
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   LaunchScope ls("class_weight_kernel", st);
   class_weight_kernel<<<F, 256, 0, st>>>(masked_affiliation, F, K, T, weight);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_gaussian_full_log_pdf(const double* embedding, const double* mean, const double* precision_cholesky,
+                              const double* log_det, int B, int N, int E, int K, double* log_pdf, void* stream) {
+  PBB_CHECK_ARG(embedding && mean && precision_cholesky && log_det, 1, "input is null");
+  PBB_CHECK_ARG(B > 0 && B <= 65535 && N > 0, 5, "bad shape");
+  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 7, "need 0 < E <= 64");
+  PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 8, "need 0 < K <= 6");
+  PBB_CHECK_ARG(log_pdf != nullptr, 9, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid((N + 127) / 128, B);
+  const size_t smem = (size_t)(E * E + E) * sizeof(double);
+  LaunchScope ls("gaussian_full_log_pdf_kernel", st);
+  if (E <= 8)
+    gaussian_full_log_pdf_kernel<8><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
+  else if (E <= 16)
+    gaussian_full_log_pdf_kernel<16><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
+  else if (E <= 32)
+    gaussian_full_log_pdf_kernel<32><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
+  else
+    gaussian_full_log_pdf_kernel<64><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+size_t pbb_gaussian_full_fit_scratch_doubles(int B, int N, int E, int K) {
+  if (B <= 0 || N <= 0 || E <= 0 || K <= 0) return 0;
+  const FullFitChunks c = full_fit_chunks(B, N, K);
+  return (size_t)c.nchunks * B * K * fit_entries(E) + (size_t)B * K;
+}
+
+int pbb_gaussian_full_fit(const double* embedding, const double* weight, int B, int N, int E, int K, double* mean,
+                          double* covariance, double* scratch, void* stream) {
+  PBB_CHECK_ARG(embedding && weight, 1, "input is null");
+  PBB_CHECK_ARG(B > 0 && N > 0, 3, "bad shape");
+  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 5, "need 0 < E <= 64");
+  PBB_CHECK_ARG(K > 0 && (long long)B * K <= 65535, 6, "need 0 < K and B * K <= 65535");
+  PBB_CHECK_ARG(mean && covariance && scratch, 7, "output / scratch is null (pbb_gaussian_full_fit_scratch_doubles)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const FullFitChunks c = full_fit_chunks(B, N, K);
+  const int BK = B * K;
+  double* partial = scratch;
+  double* denom = scratch + (size_t)c.nchunks * BK * fit_entries(E);
+  LaunchScope ls("gaussian_full_fit_kernels", st);
+  gaussian_full_partial_kernel<<<dim3(c.nchunks, BK), kFitThreads, 0, st>>>(embedding, weight, nullptr, N, E, K,
+                                                                             c.chunk_len, 0, 0, partial);
+  gaussian_full_reduce_kernel<<<BK, kFitThreads, 0, st>>>(partial, c.nchunks, E, 0, denom, mean, nullptr, nullptr,
+                                                          nullptr);
+  gaussian_full_partial_kernel<<<dim3(c.nchunks, BK), kFitThreads, 0, st>>>(embedding, weight, mean, N, E, K,
+                                                                             c.chunk_len, 1, 0, partial);
+  gaussian_full_reduce_kernel<<<BK, kFitThreads, 0, st>>>(partial, c.nchunks, E, 1, denom, nullptr, nullptr, nullptr,
+                                                          covariance);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_precision_cholesky(const double* covariance, int M, int E, double* precision_cholesky, double* log_det,
+                           int* status, void* stream) {
+  PBB_CHECK_ARG(covariance != nullptr, 1, "input is null");
+  PBB_CHECK_ARG(M > 0, 2, "bad shape");
+  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 3, "need 0 < E <= 64");
+  PBB_CHECK_ARG(precision_cholesky && log_det && status, 4, "output / status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("precision_cholesky_kernel", st);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  precision_cholesky_kernel<<<M, 32, (size_t)E * E * sizeof(double), st>>>(covariance, E, precision_cholesky, log_det,
+                                                                           status);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_vmf_log_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
+                    int B, int N, int E, int K, double* log_pdf, void* stream) {
+  PBB_CHECK_ARG(embedding && mean && concentration && log_norm, 1, "input is null");
+  PBB_CHECK_ARG(B > 0 && B <= 65535 && N > 0, 5, "bad shape");
+  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 7, "need 0 < E <= 64");
+  PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 8, "need 0 < K <= 6");
+  PBB_CHECK_ARG(log_pdf != nullptr, 9, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("vmf_log_pdf_kernel", st);
+  vmf_log_pdf_kernel<<<dim3((N + 127) / 128, B), 128, 0, st>>>(embedding, mean, concentration, log_norm, N, E, K,
+                                                                log_pdf);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_vmf_resultant(const double* embedding, const double* weight, int B, int N, int E, int K, double* resultant,
+                      double* total, double* scratch, void* stream) {
+  PBB_CHECK_ARG(embedding && weight, 1, "input is null");
+  PBB_CHECK_ARG(B > 0 && N > 0, 3, "bad shape");
+  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 5, "need 0 < E <= 64");
+  PBB_CHECK_ARG(K > 0 && (long long)B * K <= 65535, 6, "need 0 < K and B * K <= 65535");
+  PBB_CHECK_ARG(resultant && total && scratch, 7, "output / scratch is null (pbb_gaussian_full_fit_scratch_doubles)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const FullFitChunks c = full_fit_chunks(B, N, K);
+  const int BK = B * K;
+  double* partial = scratch;
+  double* denom = scratch + (size_t)c.nchunks * BK * fit_entries(E);
+  LaunchScope ls("vmf_resultant_kernels", st);
+  gaussian_full_partial_kernel<<<dim3(c.nchunks, BK), kFitThreads, 0, st>>>(embedding, weight, nullptr, N, E, K,
+                                                                             c.chunk_len, 0, 1, partial);
+  gaussian_full_reduce_kernel<<<BK, kFitThreads, 0, st>>>(partial, c.nchunks, E, 0, denom, nullptr, resultant, total,
+                                                          nullptr);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_frame_weight(const double* masked_affiliation, int B, int K, int N, double* weight, void* stream) {
+  PBB_CHECK_ARG(masked_affiliation != nullptr, 1, "input is null");
+  PBB_CHECK_ARG(B > 0 && B <= 65535 && K > 0 && N > 0, 2, "bad shape");
+  PBB_CHECK_ARG(weight != nullptr, 5, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("frame_weight_kernel", st);
+  frame_weight_kernel<<<dim3((N + 255) / 256, B), 256, 0, st>>>(masked_affiliation, K, N, weight);
   PBB_CUDA(cudaGetLastError());
   return 0;
 }

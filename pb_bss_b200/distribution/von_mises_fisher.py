@@ -1,7 +1,9 @@
-"""von Mises-Fisher distribution over real embedding vectors (pb_bss/distribution/von_mises_fisher.py:31-144), tied
-over all (bin, frame) observations, as the integrated model vmfcacgmm.py uses it.  The K x E parameters and the
-normaliser (scipy's exponentially scaled Bessel function on K scalars) stay on the host; the F*T embeddings are only
-touched by the device kernels."""
+"""von Mises-Fisher distribution over real embedding vectors (pb_bss/distribution/von_mises_fisher.py:31-144): tied
+over all (bin, frame) observations, as the integrated model vmfcacgmm.py uses it (``log_pdf_fkt``), and with any
+number of independent leading dims (``log_pdf``, ``VonMisesFisherTrainer``, the VMFMM).  The normaliser (scipy's
+exponentially scaled Bessel function on one scalar per model) and the final K x E parameter math stay on the host;
+the observations are only touched by the device kernels."""
+import math
 from dataclasses import dataclass
 
 import numpy as np
@@ -9,6 +11,7 @@ import torch
 from scipy.special import ive
 
 from .. import _device, _lib
+from .gaussian import _dev, _is_real, _np, batched_layout, check_embedding_dim
 from .utils import _ProbabilisticModel
 
 
@@ -23,6 +26,23 @@ class VonMisesFisher(_ProbabilisticModel):
         kappa = np.asarray(self.concentration)
         return ((D / 2) * np.log(2 * np.pi) + np.log(ive(D / 2 - 1, kappa))
                 + (np.abs(kappa) - (D / 2 - 1) * np.log(kappa)))
+
+    def log_pdf(self, y):
+        """y (..., N, E) (any norm: normalised inside) -> (..., N), broadcast against the model dims
+        (von_mises_fisher.py:65-79)."""
+        like_numpy = not _device.is_tensor(y)
+        yd = _dev(y)
+        E = yd.shape[-1]
+        check_embedding_dim(E)
+        mean = _np(self.mean)
+        kappa = _np(self.concentration)
+        x, B, K, L = batched_layout(yd, mean.shape[:-1])
+        log_norm = VonMisesFisher(mean=mean, concentration=kappa).log_norm()
+        m = _dev(np.broadcast_to(mean, L + (E,)).reshape(B, K, E))
+        kap = _dev(np.broadcast_to(kappa, L).reshape(B, K))
+        ln = _dev(np.broadcast_to(log_norm, L).reshape(B, K))
+        out = vmf_log_pdf_bkn(x, m, kap, ln)
+        return _device.to_host(out.reshape(L + (yd.shape[-2],)), like_numpy)
 
     def log_pdf_fkt(self, embedding):
         """embedding (F, T, E) CUDA tensor (any norm: normalised inside, von_mises_fisher.py:75-77) -> (F, K, T)."""
@@ -59,3 +79,60 @@ def vmf_fit_fkt(embedding, weight_fkt, min_concentration, max_concentration):
     concentration = (r_bar * E - r_bar ** 3) / (1 - r_bar ** 2)               # eq. 4.4
     concentration = np.clip(concentration, min_concentration, max_concentration)
     return VonMisesFisher(mean=direction, concentration=concentration)
+
+
+def vmf_log_pdf_bkn(x, mean, concentration, log_norm):
+    """x (B, N, E), mean (B, K, E), concentration / log_norm (B, K) device -> (B, K, N)."""
+    B, N, E = x.shape
+    K = mean.shape[1]
+    out = _device.empty((B, K, N), torch.float64)
+    lib = _lib.load()
+    _lib.check(lib.pbb_vmf_log_pdf(_device.ptr(x), _device.ptr(mean), _device.ptr(concentration),
+                                   _device.ptr(log_norm), B, N, E, K, _device.ptr(out), _device.stream_ptr()),
+               'pbb_vmf_log_pdf')
+    return out
+
+
+def vmf_fit_bkn(x, weight, min_concentration, max_concentration):
+    """VonMisesFisherTrainer._fit (von_mises_fisher.py:122-144) of x (B, N, E) (normalised by the kernel) with weights
+    (B, K, N) device -> host mean (B, K, E), concentration (B, K)."""
+    B, N, E = x.shape
+    K = weight.shape[1]
+    check_embedding_dim(E)
+    lib = _lib.load()
+    r = _device.empty((B, K, E), torch.float64)
+    total = _device.empty((B, K), torch.float64)
+    scratch = _device.empty((int(lib.pbb_gaussian_full_fit_scratch_doubles(B, N, E, K)),), torch.float64)
+    _lib.check(lib.pbb_vmf_resultant(_device.ptr(x), _device.ptr(weight), B, N, E, K, _device.ptr(r),
+                                     _device.ptr(total), _device.ptr(scratch), _device.stream_ptr()),
+               'pbb_vmf_resultant')
+    r, total = r.cpu().numpy(), total.cpu().numpy()
+    norm = np.linalg.norm(r, axis=-1)                                                 # Banerjee2005vMF eq. 2.4
+    mean = r / np.maximum(norm, np.finfo(np.float64).tiny)[..., None]
+    r_bar = norm / total                                                              # eq. 2.5
+    concentration = (r_bar * E - r_bar ** 3) / (1 - r_bar ** 2)                       # eq. 4.4
+    concentration = np.clip(concentration, min_concentration, max_concentration)
+    return mean, concentration
+
+
+class VonMisesFisherTrainer:
+    def fit(self, y, saliency=None, min_concentration=1e-10, max_concentration=500) -> VonMisesFisher:
+        """von_mises_fisher.py:93-120: y (..., N, E), saliency (..., N) or None."""
+        assert _is_real(y), y.dtype
+        if saliency is not None:
+            ys, ss = tuple(y.shape[:-1]), tuple(saliency.shape)
+            assert all(len({a, b} | {1}) <= 2 for a, b in zip(ys[::-1], ss[::-1])), (y.shape, saliency.shape)
+        like_numpy = not _device.is_tensor(y)
+        yd = _dev(y)
+        N, E = yd.shape[-2:]
+        sal = None if saliency is None else _dev(saliency)
+        lead = tuple(yd.shape[:-2]) if sal is None else tuple(np.broadcast_shapes(yd.shape[:-2], sal.shape[:-1]))
+        B = math.prod(lead)
+        x = yd.expand(lead + (N, E)).reshape(B, N, E).contiguous()
+        w = (torch.ones((B, 1, N), dtype=torch.float64, device=x.device) if sal is None
+             else sal.expand(lead + (N,)).reshape(B, 1, N).contiguous())
+        mean, concentration = vmf_fit_bkn(x, w, min_concentration, max_concentration)
+        mean, concentration = mean.reshape(lead + (E,)), concentration.reshape(lead)
+        if not like_numpy:
+            mean, concentration = _dev(mean), _dev(concentration)
+        return VonMisesFisher(mean=mean, concentration=concentration)
