@@ -311,6 +311,79 @@ int pbb_cwmm_predict(const void* y, int dtype, int F, int T, int D, int K,
                      void* stream);
 
 /* ------------------------------------------------------------------------
+ * Complex Bingham mixture model (pb_bss/distribution/cbmm.py, complex_bingham.py).
+ *
+ * Device model: eigenvectors (F, K, D, D) complex128 (columns, ascending scatter
+ * eigenvalues, like np.linalg.eigh), eigenvalues (F, K, D) = the Bingham parameters
+ * lambda (largest 0), weight (F, K) = CBMM.weight / complex_bingham.covariance_eigenvectors /
+ * .covariance_eigenvalues.  D is limited to 2..6, the reference's domain
+ * (complex_bingham_utils.py:342-348; D = 7 raises KeyError there).
+ *
+ * Normaliser c(lambda) = 2 pi^D exp[lambda_1..lambda_D], the divided difference of exp
+ * (complex_bingham.py:153-164), evaluated as an entry of exp() of the bidiagonal Opitz
+ * matrix by scaling and squaring; the E-step first applies the reference's gap rule
+ * (sorted neighbours at least 1e-8 apart, :167-203, norm()'s default eps).
+ *
+ * Parameter solve (find_eigenvalues_v3, :304-425): grad log c(lambda) = s in the differences
+ * of neighbouring sorted lambda, bounds [-max_concentration, -1e-8], start -diff(-1 / s),
+ * by projected Gauss-Newton with the analytic Jacobian, to max |residual| <= 1e-12 (or until
+ * the residual stops decreasing in fp64).  The reference's scipy least_squares stops at
+ * residuals of ~1e-7, so its lambda differ from these by up to ~2e-4 relative.
+ *
+ * Status word (int, 0 = ok): ((2^29 - 1 - index) << 2) | (4 - kind), index = f * K + k of the
+ * first failing (bin, class) (of the problem for pbb_bingham_parameters); at one index the
+ * smallest kind is kept (the cause, not the non-finite values a failed class leaves for the
+ * later iterations); kind
+ *   1: a scatter eigenvalue is negative or numerically zero, i.e. not above 1e-12 times
+ *      the largest (the reference asserts >= 0, complex_bingham.py:584; LAPACK and the
+ *      Jacobi solver round the zero eigenvalues of a rank-deficient scatter differently)
+ *      -> AssertionError;
+ *   2: infeasible start of the solve (a zero or negative scatter eigenvalue makes
+ *      x0 = -inf or > -1e-8, :378-408) -> ValueError;
+ *   3: non-finite scatter, parameters or normaliser -> AssertionError. */
+size_t pbb_cbmm_workspace_bytes(int F, int T, int D, int K);
+
+/* CBMMTrainer.fit / _fit / _m_step (cbmm.py:79-237, complex_bingham.py:567-594).
+ * init_aff (F, K, T) is required (cbmm.py:120-126 draws it on the host); saliency (F, T)
+ * or null (ones, cbmm.py:128-129); weight_mode PBB_WEIGHT_TIME or PBB_WEIGHT_CONST;
+ * affiliation_eps clips the posteriors of iterations 2.. to [eps, 1 - eps] (cbmm.py:189).
+ * All iterations are enqueued on `stream` without host synchronisation. */
+int pbb_cbmm_fit(const void* y, int dtype, int F, int T, int D, int K,
+                 const double* init_aff, const double* saliency, int iterations,
+                 int weight_mode, double affiliation_eps, double eigenvalue_eps,
+                 double max_concentration, void* eigenvectors, double* eigenvalues,
+                 double* weight, void* workspace, size_t workspace_bytes,
+                 int* status, void* stream);
+
+/* CBMM.predict (cbmm.py:26-55): normalises y, affiliation (F, K, T) out.  weight as for
+ * pbb_cwmm_predict (every PBB_WEIGHT_* layout but PBB_WEIGHT_FRAME). */
+int pbb_cbmm_predict(const void* y, int dtype, int F, int T, int D, int K,
+                     const void* eigenvectors, const double* eigenvalues,
+                     const double* weight, int weight_mode, double affiliation_eps,
+                     double* affiliation, void* workspace, size_t workspace_bytes,
+                     int* status, void* stream);
+
+/* ComplexBinghamTrainer.find_eigenvalues_v3 (complex_bingham.py:304-425), batched:
+ * scatter_eigenvalues (n, D) in any order -> eigenvalues (n, D) in the same order.
+ * eps: the trainer's eignevalue_eps; max_concentration may be +inf. */
+int pbb_bingham_parameters(const double* scatter_eigenvalues, int n, int D, double eps,
+                           double max_concentration, double* eigenvalues, int* status,
+                           void* stream);
+
+/* ComplexBingham.log_norm (complex_bingham.py:80-164): log c of eigenvalues (n, D);
+ * eps > 0 applies the gap rule with that eps first, eps <= 0 does not
+ * (remove_duplicate_eigenvalues=False; repeated eigenvalues need no special case here). */
+int pbb_bingham_log_norm(const double* eigenvalues, int n, int D, double eps,
+                         double* log_norm, void* stream);
+
+/* ComplexBingham.log_pdf (complex_bingham.py:59-78): log_pdf (M, T) = Re(y^H B y) - log_norm,
+ * B = V diag(lambda) V^H, for y (M, T, D) as given (not normalised), eigenvectors V (M, D, D)
+ * complex128, eigenvalues lambda (M, D), log_norm (M). */
+int pbb_bingham_log_pdf(const void* y, int dtype, int M, int T, int D, const void* eigenvectors,
+                        const double* eigenvalues, const double* log_norm, double* log_pdf,
+                        void* stream);
+
+/* ------------------------------------------------------------------------
  * Batched Hermitian eigendecomposition, ascending eigenvalues
  * (np.linalg.eigh as used in complex_angular_central_gaussian.py:95 and
  * pb_bss/utils.py:154).  a: (n, D, D) complex128 (only read), w: (n, D),

@@ -57,6 +57,13 @@ SIGNATURES = {
     'pbb_cwmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _d,
                           _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
     'pbb_cwmm_predict': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_cbmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
+    'pbb_cbmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _d, _d, _d,
+                          _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_cbmm_predict': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _d, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_bingham_parameters': (_i, [_vp, _i, _i, _d, _d, _vp, _vp, _vp]),
+    'pbb_bingham_log_norm': (_i, [_vp, _i, _i, _d, _vp, _vp]),
+    'pbb_bingham_log_pdf': (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'pbb_heig_batched': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_psd_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'pbb_power_spectral_density': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),

@@ -15,6 +15,7 @@
 #include "em_ws.cuh"
 #include "em_ls.cuh"
 #include "em_sticky.cuh"
+#include "bingham.cuh"
 #include "prof.cuh"
 
 #ifndef PBB_CTA_FPL
@@ -636,6 +637,58 @@ static int launch_cw_update(CwUpdArgs u, cudaStream_t st) {
   return 0;
 }
 
+// complex Bingham kernels are instantiated for D = 2..6, the reference's domain (complex_bingham_utils.py:342-348)
+template <template <int> class Launch, typename... Args>
+static int bingham_dispatch(int D, Args... args) {
+  switch (D) {
+    case 2: return Launch<2>::run(args...);
+    case 3: return Launch<3>::run(args...);
+    case 4: return Launch<4>::run(args...);
+    case 5: return Launch<5>::run(args...);
+    case 6: return Launch<6>::run(args...);
+    default: set_error("complex Bingham: D = %d, need 2 <= D <= 6", D); return -5;
+  }
+}
+template <int D> struct CbUpdateLaunch {
+  static int run(CbUpdArgs u, cudaStream_t st) {
+    LaunchScope ls("cb_update_kernel", st);
+    cb_update_kernel<D><<<u.F, 32 * kCbWarps, 0, st>>>(u);
+    PBB_CUDA(cudaGetLastError());
+    return 0;
+  }
+};
+template <int D> struct CbFromModelLaunch {
+  static int run(CbFromModelArgs u, cudaStream_t st) {
+    LaunchScope ls("cb_from_model_kernel", st);
+    cb_from_model_kernel<D><<<u.F, 32 * kCbWarps, 0, st>>>(u);
+    PBB_CUDA(cudaGetLastError());
+    return 0;
+  }
+};
+template <int D> struct BinghamParametersLaunch {
+  static int run(const double* s, int n, double eps, double mc, double* lam, int* status, cudaStream_t st) {
+    LaunchScope ls("bingham_parameters_kernel", st);
+    bingham_parameters_kernel<D><<<(n + 3) / 4, 128, 0, st>>>(s, n, eps, mc, lam, status);
+    PBB_CUDA(cudaGetLastError());
+    return 0;
+  }
+};
+template <int D> struct BinghamLogNormLaunch {
+  static int run(const double* lam, int n, double eps, double* out, cudaStream_t st) {
+    LaunchScope ls("bingham_log_norm_kernel", st);
+    bingham_log_norm_kernel<D><<<(n + 127) / 128, 128, 0, st>>>(lam, n, eps, out);
+    PBB_CUDA(cudaGetLastError());
+    return 0;
+  }
+};
+
+static int check_cbmm_shape(int F, int T, int D, int K, int dtype) {
+  if (int r = check_shape(F, T, D, K, dtype)) return r;
+  PBB_CHECK_ARG(D >= 2 && D <= 6, 5, "complex Bingham: need 2 <= D <= 6 (complex_bingham_utils.py:342-348)");
+  PBB_CHECK_ARG((long long)F * K <= kCbMaxIndex, 6, "F * K too large for the status word");
+  return 0;
+}
+
 }  // namespace pbb
 
 using namespace pbb;
@@ -1125,6 +1178,139 @@ int pbb_cwmm_predict(const void* y, int dtype, int F, int T, int D, int K, const
   a.aff_out = affiliation;
   int nch = launch_em(a, dtype, 0, st);
   return nch > 0 ? 0 : (nch ? nch : 1);
+}
+
+size_t pbb_cbmm_workspace_bytes(int F, int T, int D, int K) { return pbb_cacgmm_workspace_bytes(F, T, D, K); }
+
+int pbb_cbmm_fit(const void* y, int dtype, int F, int T, int D, int K, const double* init_aff,
+                 const double* saliency, int iterations, int weight_mode, double affiliation_eps,
+                 double eigenvalue_eps, double max_concentration, void* eigenvectors, double* eigenvalues,
+                 double* weight, void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  if (int r = check_cbmm_shape(F, T, D, K, dtype)) return r;
+  PBB_CHECK_ARG(init_aff != nullptr, 7, "initial affiliations are null (cbmm.py:120-126)");
+  PBB_CHECK_ARG(iterations > 0, 9, "iterations must be positive");
+  PBB_CHECK_ARG(weight_mode == PBB_WEIGHT_TIME || weight_mode == PBB_WEIGHT_CONST, 10, "bad weight_mode");
+  PBB_CHECK_ARG(affiliation_eps >= 0.0 && affiliation_eps < 0.5, 11, "need 0 <= affiliation_eps < 0.5");
+  PBB_CHECK_ARG(max_concentration > 0.0, 13, "max_concentration must be positive (complex_bingham.py:221)");
+  PBB_CHECK_ARG(eigenvectors && eigenvalues && weight, 14, "model output is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 17,
+                "workspace too small (pbb_cbmm_workspace_bytes)");
+  PBB_CHECK_ARG(status != nullptr, 19, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
+                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
+  if (r) return r;
+  EmArgs a;
+  memset(&a, 0, sizeof(a));
+  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  a.model_kind = 1;  // lp = ew q - ld with ew = -1, q = y^H (-B) y
+  a.coef = ws.coef; a.ld = ws.ld; a.w = weight; a.ew = ws.ew;
+  a.saliency = saliency; a.part = ws.part; a.aff_eps = affiliation_eps;
+  CbUpdArgs u;
+  memset(&u, 0, sizeof(u));
+  u.F = F; u.T = T; u.K = K;
+  u.part = ws.part; u.weight_mode = weight_mode;
+  u.eigenvalue_eps = eigenvalue_eps; u.max_concentration = max_concentration;
+  u.evec = reinterpret_cast<double2*>(eigenvectors); u.eval = eigenvalues; u.weight = weight;
+  u.coef = ws.coef; u.ld = ws.ld; u.ew = ws.ew; u.status = status;
+  for (int it = 0; it < iterations; ++it) {
+    // iteration 0: M-step from the initial affiliations; then E-step (predict) + M-step (cbmm.py:186-203)
+    if (it == 0) { a.mode = kModeM; a.aff_in = init_aff; a.q_in = nullptr; }
+    else { a.mode = kModeEM; a.aff_in = nullptr; }
+    const int nch = launch_em(a, dtype, 0, st);
+    if (nch <= 0) return nch ? nch : 1;
+    u.nch = nch;
+    u.coef = it + 1 < iterations ? ws.coef : nullptr;  // nobody reads the E-step form of the final model
+    if ((r = bingham_dispatch<CbUpdateLaunch>(D, u, st))) return r;
+  }
+  return 0;
+}
+
+int pbb_cbmm_predict(const void* y, int dtype, int F, int T, int D, int K, const void* eigenvectors,
+                     const double* eigenvalues, const double* weight, int weight_mode, double affiliation_eps,
+                     double* affiliation, void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  if (int r = check_cbmm_shape(F, T, D, K, dtype)) return r;
+  PBB_CHECK_ARG(eigenvectors && eigenvalues, 7, "model is null");
+  PBB_CHECK_ARG(weight != nullptr || weight_mode == PBB_WEIGHT_CONST, 9, "weight is null");
+  PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_TIED, 10, "bad weight_mode");
+  PBB_CHECK_ARG(affiliation_eps >= 0.0 && affiliation_eps < 0.5, 11, "need 0 <= affiliation_eps < 0.5");
+  PBB_CHECK_ARG(affiliation != nullptr, 12, "affiliation output is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 13,
+                "workspace too small (pbb_cbmm_workspace_bytes)");
+  PBB_CHECK_ARG(status != nullptr, 15, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
+                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
+  if (r) return r;
+  const bool tied = weight_mode == PBB_WEIGHT_TIED_TIME || weight_mode == PBB_WEIGHT_TIED;
+  CbFromModelArgs fm;
+  fm.F = F; fm.K = K;
+  fm.evec = reinterpret_cast<const double2*>(eigenvectors); fm.eval = eigenvalues;
+  fm.weight = (tied || weight_mode == PBB_WEIGHT_CONST) ? nullptr : weight;
+  fm.coef = ws.coef; fm.ld = ws.ld; fm.ew = ws.ew; fm.w = ws.w;
+  if ((r = bingham_dispatch<CbFromModelLaunch>(D, fm, st))) return r;
+  EmArgs a;
+  memset(&a, 0, sizeof(a));
+  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  a.mode = kModeE; a.model_kind = 1;
+  a.coef = ws.coef; a.ld = ws.ld; a.w = ws.w; a.ew = ws.ew;
+  if (tied) { a.w_time = weight; a.w_time_st = weight_mode == PBB_WEIGHT_TIED_TIME ? 1 : 0; }
+  a.aff_eps = affiliation_eps;
+  a.aff_out = affiliation;
+  const int nch = launch_em(a, dtype, 0, st);
+  return nch > 0 ? 0 : (nch ? nch : 1);
+}
+
+int pbb_bingham_parameters(const double* scatter_eigenvalues, int n, int D, double eps, double max_concentration,
+                           double* eigenvalues, int* status, void* stream) {
+  PBB_CHECK_ARG(scatter_eigenvalues != nullptr, 1, "scatter eigenvalues are null");
+  PBB_CHECK_ARG(n > 0 && n <= kCbMaxIndex, 2, "need 0 < n < 2^29");
+  PBB_CHECK_ARG(D >= 2 && D <= 6, 3, "complex Bingham: need 2 <= D <= 6 (complex_bingham_utils.py:342-348)");
+  PBB_CHECK_ARG(max_concentration > 0.0, 5, "max_concentration must be positive (complex_bingham.py:221)");
+  PBB_CHECK_ARG(eigenvalues != nullptr, 6, "output is null");
+  PBB_CHECK_ARG(status != nullptr, 7, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  return bingham_dispatch<BinghamParametersLaunch>(D, scatter_eigenvalues, n, eps, max_concentration, eigenvalues,
+                                                   status, st);
+}
+
+int pbb_bingham_log_norm(const double* eigenvalues, int n, int D, double eps, double* log_norm, void* stream) {
+  PBB_CHECK_ARG(eigenvalues != nullptr, 1, "eigenvalues are null");
+  PBB_CHECK_ARG(n > 0, 2, "n must be positive");
+  PBB_CHECK_ARG(D >= 2 && D <= 6, 3, "complex Bingham: need 2 <= D <= 6 (complex_bingham_utils.py:342-348)");
+  PBB_CHECK_ARG(log_norm != nullptr, 5, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  return bingham_dispatch<BinghamLogNormLaunch>(D, eigenvalues, n, eps, log_norm, st);
+}
+
+int pbb_bingham_log_pdf(const void* y, int dtype, int M, int T, int D, const void* eigenvectors,
+                        const double* eigenvalues, const double* log_norm, double* log_pdf, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(M > 0 && T > 0, 3, "empty shape");
+  PBB_CHECK_ARG(D >= 1 && D < 256, 5, "bad D");
+  PBB_CHECK_ARG(eigenvectors != nullptr && eigenvalues != nullptr && log_norm != nullptr, 6, "model is null");
+  PBB_CHECK_ARG(log_pdf != nullptr, 9, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long long n = (long long)M * T;
+  const unsigned blocks = (unsigned)((n + 127) / 128);
+  const double2* V = static_cast<const double2*>(eigenvectors);
+  LaunchScope ls("bingham_log_pdf_kernel", st);
+  if (dtype == PBB_C128)
+    bingham_log_pdf_kernel<double2><<<blocks, 128, 0, st>>>(static_cast<const double2*>(y), V, eigenvalues, log_norm,
+                                                            M, T, D, log_pdf);
+  else
+    bingham_log_pdf_kernel<float2><<<blocks, 128, 0, st>>>(static_cast<const float2*>(y), V, eigenvalues, log_norm,
+                                                           M, T, D, log_pdf);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 int pbb_mixture_weight_over_bins(const double* affiliation, int F, int K, int T, int flags, double* weight_kt,

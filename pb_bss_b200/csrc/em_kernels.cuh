@@ -90,10 +90,11 @@ __device__ __forceinline__ void em_softmax(const double (&q)[K], const double* _
 // (complex_watson.py:73-87), then the same softmax (mixture_model_utils.py:7-55,
 // affiliation_eps = 0, cwmm.py:161).  q[k] = |m_k^H z|^2 arrives as the slot-form
 // quadratic form of the rank-1 matrix m m^H.
+// A non-zero eps clips the posterior to [eps, 1 - eps] (CBMM, cbmm.py:41-55).
 template <int K>
 __device__ __forceinline__ void watson_softmax(const double (&q)[K], const double* __restrict__ lognorm,
                                                const double* __restrict__ w, const double* __restrict__ kappa,
-                                               double (&gam)[K]) {
+                                               double eps, double (&gam)[K]) {
   double lp[K];
   double m = -INFINITY;
 #pragma unroll
@@ -109,7 +110,10 @@ __device__ __forceinline__ void watson_softmax(const double (&q)[K], const doubl
   }
   const double inv = 1.0 / fmax(den, kTiny);
 #pragma unroll
-  for (int k = 0; k < K; ++k) gam[k] *= inv;
+  for (int k = 0; k < K; ++k) {
+    gam[k] *= inv;
+    if (eps != 0.0) gam[k] = fmin(fmax(gam[k], eps), 1.0 - eps);
+  }
 }
 
 // --------------------------------------------------------------------------
@@ -211,9 +215,9 @@ __device__ __forceinline__ void em_fast_group(const EmArgs& a, EmFastSmem<D, K>&
           double wl[K];
 #pragma unroll
           for (int k = 0; k < K; ++k) wl[k] = a.w_time[(size_t)k * (a.w_time_st ? T : 1) + (a.w_time_st && valid ? t : 0)];
-          watson_softmax<K>(q, sm.ld, wl, sm.ew, gam);
+          watson_softmax<K>(q, sm.ld, wl, sm.ew, a.aff_eps, gam);
         } else {
-          watson_softmax<K>(q, sm.ld, sm.w, sm.ew, gam);
+          watson_softmax<K>(q, sm.ld, sm.w, sm.ew, a.aff_eps, gam);
         }
 #pragma unroll
         for (int k = 0; k < K; ++k) invq[k] = 1.0;

@@ -4,6 +4,8 @@ from .complex_angular_central_gaussian import (  # noqa: F401
     normalize_observation,
 )
 from .cacgmm import CACGMM, CACGMMTrainer  # noqa: F401
+from .cbmm import CBMM, CBMMTrainer  # noqa: F401
+from .complex_bingham import ComplexBingham, ComplexBinghamTrainer  # noqa: F401
 from .complex_watson import ComplexWatson, ComplexWatsonTrainer  # noqa: F401
 from .cwmm import CWMM, CWMMTrainer  # noqa: F401
 from .gaussian import DiagonalGaussian, Gaussian, GaussianTrainer, SphericalGaussian  # noqa: F401
