@@ -458,6 +458,104 @@ int pbb_apply_beamforming_vector(const void* vector, const void* mix, int dtype,
 int pbb_apply_beamforming_vector_shared(const void* vector, const void* mix, int dtype,
                                         int B, int F, int D, int T, void* out, void* stream);
 
+/* Plain np.linalg.solve without the lstsq fallback (get_mvdr_vector_merl,
+ * beamformer.py:277): a (n, D, D), b (n, D, R) -> x (n, D, R).  status must not be
+ * NULL; it is set to 1 + the index of an exactly singular matrix (a zero pivot,
+ * where NumPy raises LinAlgError), whose x is then undefined. */
+int pbb_solve_batched_strict(const void* a, const void* b, int n, int D, int R,
+                             void* x, int* status, void* stream);
+
+/* get_lcmv_vector (beamformer.py:414-456): atf (K, F, D), response (K)
+ * complex128 on the device, noise_psd (F, D, D) -> w (F, D).  X = solve(noise, H)
+ * with the K ATFs as right-hand sides, y = solve(H^H X, r), w = X y; both solves
+ * with stable_solve semantics (pbb_solve_batched).  Like the reference (:444), r is
+ * rounded to complex64 first, so a response of 1e-3 is met as float32(1e-3).
+ * When any bin's K x K system is exactly singular, y of every bin is rounded to
+ * complex64, as the reference's stable_solve does there (it writes into
+ * zeros_like(r), math/solve.py:107-113).  scratch: F (2 D K + K K + 2 K) + 1
+ * complex128.  status = 1 + a bin whose system is singular with D > 40 or K > 40
+ * (no minimum-norm fallback there). */
+int pbb_lcmv(const void* atf, const void* response, const void* noise_psd, int K,
+             int F, int D, void* w, void* scratch, int* status, void* stream);
+
+/* The filter of get_wmwf_vector (beamformer.py:701-742): phi = stable_solve(noise,
+ * target), lambda = trace(phi) (complex, not clamped); filter = phi / (mu + lambda)
+ * or, frequency_dependent != 0, phi / sqrt(target[0][0] lambda) (principal root).
+ * target_psd, noise_psd, filter (n, D, D); scratch: n D D complex128.  status as
+ * pbb_solve_batched.  The caller selects a column or calls pbb_weighted_channel_sum. */
+int pbb_wmwf(const void* target_psd, const void* noise_psd, int n, int D,
+             int frequency_dependent, double distortion_weight, void* filter,
+             void* scratch, int* status, void* stream);
+
+/* out[m][r] = sum_c filter[m][r][c] * weight[m][r][c]: the channel_selection_vector
+ * sum of get_wmwf_vector (beamformer.py:743-745).  filter, weight (n, D, D). */
+int pbb_weighted_channel_sum(const void* filter, const void* weight, int n, int D,
+                             void* out, void* stream);
+
+/* The SNR terms of get_optimal_reference_channel (beamformer.py:601-624) for
+ * w_mat (n, D, D): num[m][R] = w_R^H target w_R, den[m][R] = w_R^H noise w_R with
+ * w_R = w_mat[m][:, R] (n, D), and their sums over the n bins in bin order
+ * (num_sum, den_sum: D complex128).  The same quadratic forms as pbb_souden. */
+int pbb_reference_channel_snr(const void* w_mat, const void* target_psd,
+                              const void* noise_psd, int n, int D, void* num,
+                              void* den, void* num_sum, void* den_sum, void* stream);
+
+/* get_mvdr_vector_merl (beamformer.py:263-289): G = solve(noise, target) with
+ * np.linalg.solve (no fallback: status = 1 + a singular bin, the reference raises
+ * LinAlgError), w = (G / trace G)[:, 0].  The reference's SNR is summed over the
+ * channel axis as well (np.sum of an einsum that keeps only 'c'), so its argmax is
+ * always 0 and w is column 0 -- the WMWF filter with mu = 0; no SNR is computed.
+ * target_psd, noise_psd (n, D, D), w (n, D), scratch n D D complex128. */
+int pbb_mvdr_merl(const void* target_psd, const void* noise_psd, int n, int D,
+                  void* w, void* scratch, int* status, void* stream);
+
+/* condition_covariance (beamformer.py:563-569): (x + gamma trace(x) / D I) /
+ * (1 + gamma) with the complex trace; x, out (n, D, D). */
+int pbb_condition_covariance(const void* x, int n, int D, double gamma, void* out,
+                             void* stream);
+
+/* distortionless_normalization (beamformer.py:491-499): out = N w w^H a / (w^H N w);
+ * vector, atf, out (n, D), noise_psd (n, D, D). */
+int pbb_distortionless_normalization(const void* vector, const void* atf,
+                                     const void* noise_psd, int n, int D,
+                                     void* out, void* stream);
+
+/* mvdr_snr_postfilter (beamformer.py:502-509): out[m] = (w^H T w) / (w^H N w);
+ * vector (n, D), target_psd, noise_psd (n, D, D), out (n). */
+int pbb_mvdr_snr_postfilter(const void* vector, const void* target_psd,
+                            const void* noise_psd, int n, int D, void* out,
+                            void* stream);
+
+/* zero_degree_normalization (beamformer.py:512-514): out = w exp(-i angle(w[ref]))
+ * per row; vector, out (n, D). */
+int pbb_zero_degree_normalization(const void* vector, int n, int D,
+                                  int reference_channel, void* out, void* stream);
+
+/* phase_correction (beamformer.py:517-560): bin f >= 1 is multiplied by the
+ * cumulative product of exp(i angle(sum_d conj(w_f[d]) w_{f-1}[d])) along the
+ * reference's AXIS 0 OF THE WHOLE ARRAY.  scan_bins = 1 (A = M = 1): a 2-D (F, D)
+ * input, axis 0 is the bin axis and the product runs over the bins.  scan_bins = 0:
+ * an (A, M, F, D) input (A = axis 0, M = the dims between), and the product runs
+ * over A for every (m, f) on its own -- for a (K, F, D) input over the K vectors,
+ * not over the bins.  This is the reference's behaviour and is kept.  Row f = 0 is
+ * copied; out must not alias vector. */
+int pbb_phase_correction(const void* vector, int A, int M, int F, int D,
+                         int scan_bins, void* out, void* stream);
+
+/* apply_online_beamforming_vector (beamformer.py:586-598): time-varying filters,
+ * out[b][f][t] = sum_d conj(v[t][f][d]) mix[b][f][d][t]; vector complex128,
+ * mix complex64 or complex128 (dtype), out (B, F, T) complex128.  Strides in
+ * elements: the vector's d stride is 1, frame / bin strides as given (bin stride 0
+ * broadcasts one vector bin); the mix's d / t strides are T / 1, batch / bin
+ * strides as given (0 broadcasts).  The vector is read once for all B. */
+int pbb_apply_online_beamforming_vector(const void* vector, const void* mix,
+                                        int dtype, int B, int F, int D, int T,
+                                        long long vector_frame_stride,
+                                        long long vector_bin_stride,
+                                        long long mix_batch_stride,
+                                        long long mix_bin_stride, void* out,
+                                        void* stream);
+
 /* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */

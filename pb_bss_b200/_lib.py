@@ -96,6 +96,19 @@ SIGNATURES = {
     'pbb_matvec_batched': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     'pbb_apply_beamforming_vector': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'pbb_apply_beamforming_vector_shared': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    'pbb_solve_batched_strict': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
+    'pbb_lcmv': (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_wmwf': (_i, [_vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp]),
+    'pbb_weighted_channel_sum': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
+    'pbb_reference_channel_snr': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    'pbb_mvdr_merl': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_condition_covariance': (_i, [_vp, _i, _i, _d, _vp, _vp]),
+    'pbb_distortionless_normalization': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
+    'pbb_mvdr_snr_postfilter': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
+    'pbb_zero_degree_normalization': (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    'pbb_phase_correction': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    'pbb_apply_online_beamforming_vector': (_i, [_vp, _vp, _i, _i, _i, _i, _i, ctypes.c_longlong, ctypes.c_longlong,
+                                                 ctypes.c_longlong, ctypes.c_longlong, _vp, _vp]),
 }
 
 _lib = None

@@ -5,6 +5,7 @@
 #include "em_args.cuh"
 #include "heig.cuh"
 #include "linalg_kernels.cuh"
+#include "extraction.cuh"
 #include "prof.cuh"
 
 namespace pbb {
@@ -56,6 +57,21 @@ static int warps_for(size_t per_warp_bytes) {
   return w;
 }
 
+static int solve_launch(const void* a, const void* b, int n, int D, int R, int hermitize, void* x, int* status,
+                        int strict, cudaStream_t st, int* fallback = nullptr) {
+  const size_t per = solve_smem_per_warp(D, R);
+  const int warps = warps_for(per);
+  PBB_CUDA(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  LaunchScope ls("solve_kernel", st);
+  solve_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
+      reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), n, D, R, hermitize,
+      reinterpret_cast<double2*>(x), status, warps, strict, fallback);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+static unsigned blocks_for(size_t count, int threads) { return (unsigned)((count + threads - 1) / threads); }
+
 }  // namespace pbb
 
 using namespace pbb;
@@ -106,16 +122,18 @@ int pbb_solve_batched(const void* a, const void* b, int n, int D, int R, int her
   PBB_CHECK_ARG(D > 0 && D <= 64, 4, "need 0 < D <= 64");
   PBB_CHECK_ARG(R > 0 && R <= 64, 5, "need 0 < R <= 64");
   PBB_CHECK_ARG(x != nullptr, 7, "x is null");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t per = solve_smem_per_warp(D, R);
-  const int warps = warps_for(per);
-  PBB_CUDA(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  LaunchScope ls("solve_kernel", st);
-  solve_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
-      reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), n, D, R, hermitize,
-      reinterpret_cast<double2*>(x), status, warps);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return solve_launch(a, b, n, D, R, hermitize, x, status, 0, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pbb_solve_batched_strict(const void* a, const void* b, int n, int D, int R, void* x, int* status, void* stream) {
+  PBB_CHECK_ARG(a != nullptr, 1, "a is null");
+  PBB_CHECK_ARG(b != nullptr, 2, "b is null");
+  PBB_CHECK_ARG(n > 0, 3, "n must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= 64, 4, "need 0 < D <= 64");
+  PBB_CHECK_ARG(R > 0 && R <= 64, 5, "need 0 < R <= 64");
+  PBB_CHECK_ARG(x != nullptr, 6, "x is null");
+  PBB_CHECK_ARG(status != nullptr, 7, "status is null");
+  return solve_launch(a, b, n, D, R, 0, x, status, 1, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pbb_mvdr(const void* atf, const void* noise_psd, int n, int D, void* w, void* scratch, int* status,
@@ -253,6 +271,216 @@ int pbb_power_spectral_density(const void* observation, int dtype, int F, int D,
   const int scale = mask == nullptr ? 2 : (normalize ? 1 : 0);
   LaunchScope ls("psd_finalize_kernel", st);
   psd_finalize_kernel<<<dim3(F, K), 64, 0, st>>>(a.part, nch, F, K, D, T, scale, reinterpret_cast<double2*>(psd));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- multi-source beamformers and vector post-processing (csrc/extraction.cuh) ----------------------------------
+
+int pbb_lcmv(const void* atf, const void* response, const void* noise_psd, int K, int F, int D, void* w,
+             void* scratch, int* status, void* stream) {
+  PBB_CHECK_ARG(atf != nullptr, 1, "atf is null");
+  PBB_CHECK_ARG(response != nullptr, 2, "response is null");
+  PBB_CHECK_ARG(noise_psd != nullptr, 3, "noise PSD is null");
+  PBB_CHECK_ARG(K > 0 && K <= 64, 4, "need 0 < K <= 64");
+  PBB_CHECK_ARG(F > 0, 5, "F must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= 64, 6, "need 0 < D <= 64");
+  PBB_CHECK_ARG(w != nullptr, 7, "w is null");
+  PBB_CHECK_ARG(scratch != nullptr, 8, "scratch (F * (2 * D * K + K * K + 2 * K) + 1 complex128) is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  double2* H = reinterpret_cast<double2*>(scratch);
+  double2* X = H + (size_t)F * D * K;
+  double2* G = X + (size_t)F * D * K;
+  double2* rhs = G + (size_t)F * K * K;
+  double2* y = rhs + (size_t)F * K;
+  int* fallback = reinterpret_cast<int*>(y + (size_t)F * K);
+  PBB_CUDA(cudaMemsetAsync(fallback, 0, sizeof(int), st));
+  {
+    LaunchScope ls("lcmv_rhs_kernel", st);
+    lcmv_rhs_kernel<<<blocks_for((size_t)K * F * D, 256), 256, 0, st>>>(reinterpret_cast<const double2*>(atf), K, F,
+                                                                        D, H);
+    PBB_CUDA(cudaGetLastError());
+  }
+  int r = solve_launch(noise_psd, H, F, D, K, 0, X, status, 0, st);  // Phi_N X = H, stable_solve (:432-435)
+  if (r) return r;
+  {
+    LaunchScope ls("lcmv_gram_kernel", st);
+    lcmv_gram_kernel<<<blocks_for((size_t)F * K * K, 128), 128, 0, st>>>(
+        reinterpret_cast<const double2*>(atf), X, reinterpret_cast<const double2*>(response), K, F, D, G, rhs);
+    PBB_CUDA(cudaGetLastError());
+  }
+  r = solve_launch(G, rhs, F, K, 1, 0, y, status, 0, st, fallback);  // (H^H Phi_N^-1 H) y = r (:446-449)
+  if (r) return r;
+  LaunchScope ls("lcmv_combine_kernel", st);
+  lcmv_combine_kernel<<<blocks_for((size_t)F * D, 128), 128, 0, st>>>(X, y, fallback, K, F, D,
+                                                                      reinterpret_cast<double2*>(w));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_wmwf(const void* target_psd, const void* noise_psd, int n, int D, int frequency_dependent,
+             double distortion_weight, void* filter, void* scratch, int* status, void* stream) {
+  PBB_CHECK_ARG(target_psd != nullptr, 1, "target PSD is null");
+  PBB_CHECK_ARG(noise_psd != nullptr, 2, "noise PSD is null");
+  PBB_CHECK_ARG(n > 0, 3, "n must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= 64, 4, "need 0 < D <= 64");
+  PBB_CHECK_ARG(filter != nullptr, 7, "filter is null");
+  PBB_CHECK_ARG(scratch != nullptr, 8, "scratch (n * D * D complex128) is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int r = solve_launch(noise_psd, target_psd, n, D, D, 0, scratch, status, 0, st);  // phi, stable_solve (:735)
+  if (r) return r;
+  LaunchScope ls("wmwf_filter_kernel", st);
+  wmwf_filter_kernel<<<blocks_for((size_t)n * D * D, 256), 256, 0, st>>>(
+      reinterpret_cast<const double2*>(scratch), reinterpret_cast<const double2*>(target_psd), n, D,
+      frequency_dependent, distortion_weight, reinterpret_cast<double2*>(filter));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_weighted_channel_sum(const void* filter, const void* weight, int n, int D, void* out, void* stream) {
+  PBB_CHECK_ARG(filter != nullptr, 1, "filter is null");
+  PBB_CHECK_ARG(weight != nullptr, 2, "weight is null");
+  PBB_CHECK_ARG(n > 0 && D > 0, 3, "bad shape");
+  PBB_CHECK_ARG(out != nullptr, 5, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("weighted_channel_sum_kernel", st);
+  weighted_channel_sum_kernel<<<blocks_for((size_t)n * D, 256), 256, 0, st>>>(
+      reinterpret_cast<const double2*>(filter), reinterpret_cast<const double2*>(weight), n, D,
+      reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_reference_channel_snr(const void* w_mat, const void* target_psd, const void* noise_psd, int n, int D,
+                              void* num, void* den, void* num_sum, void* den_sum, void* stream) {
+  PBB_CHECK_ARG(w_mat && target_psd && noise_psd, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
+  PBB_CHECK_ARG(num && den && num_sum && den_sum, 6, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  {
+    LaunchScope ls("reference_snr_kernel", st);
+    reference_snr_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(w_mat),
+                                           reinterpret_cast<const double2*>(target_psd),
+                                           reinterpret_cast<const double2*>(noise_psd), n, D,
+                                           reinterpret_cast<double2*>(num), reinterpret_cast<double2*>(den));
+    PBB_CUDA(cudaGetLastError());
+  }
+  LaunchScope ls("colsum_kernel", st);
+  colsum_kernel<<<1, 128, 0, st>>>(reinterpret_cast<const double*>(num), reinterpret_cast<double*>(num_sum), n, 2 * D);
+  colsum_kernel<<<1, 128, 0, st>>>(reinterpret_cast<const double*>(den), reinterpret_cast<double*>(den_sum), n, 2 * D);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_mvdr_merl(const void* target_psd, const void* noise_psd, int n, int D, void* w, void* scratch, int* status,
+                  void* stream) {
+  PBB_CHECK_ARG(target_psd != nullptr, 1, "target PSD is null");
+  PBB_CHECK_ARG(noise_psd != nullptr, 2, "noise PSD is null");
+  PBB_CHECK_ARG(n > 0, 3, "n must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= 64, 4, "need 0 < D <= 64");
+  PBB_CHECK_ARG(w != nullptr, 5, "w is null");
+  PBB_CHECK_ARG(scratch != nullptr, 6, "scratch (n * D * D complex128) is null");
+  PBB_CHECK_ARG(status != nullptr, 7, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  int r = solve_launch(noise_psd, target_psd, n, D, D, 0, scratch, status, 1, st);  // np.linalg.solve (:277)
+  if (r) return r;
+  LaunchScope ls("merl_kernel", st);
+  merl_kernel<<<blocks_for(n, 128), 128, 0, st>>>(reinterpret_cast<const double2*>(scratch), n, D,
+                                                  reinterpret_cast<double2*>(w));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_condition_covariance(const void* x, int n, int D, double gamma, void* out, void* stream) {
+  PBB_CHECK_ARG(x != nullptr, 1, "x is null");
+  PBB_CHECK_ARG(n > 0 && D > 0, 2, "bad shape");
+  PBB_CHECK_ARG(out != nullptr, 5, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("condition_covariance_kernel", st);
+  condition_covariance_kernel<<<blocks_for((size_t)n * D * D, 256), 256, 0, st>>>(
+      reinterpret_cast<const double2*>(x), n, D, gamma, reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_distortionless_normalization(const void* vector, const void* atf, const void* noise_psd, int n, int D,
+                                     void* out, void* stream) {
+  PBB_CHECK_ARG(vector && atf && noise_psd, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
+  PBB_CHECK_ARG(out != nullptr, 6, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("distortionless_kernel", st);
+  distortionless_kernel<<<blocks_for(n, 128), 128, 0, st>>>(
+      reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(atf),
+      reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_mvdr_snr_postfilter(const void* vector, const void* target_psd, const void* noise_psd, int n, int D,
+                            void* out, void* stream) {
+  PBB_CHECK_ARG(vector && target_psd && noise_psd, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
+  PBB_CHECK_ARG(out != nullptr, 6, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("snr_postfilter_kernel", st);
+  snr_postfilter_kernel<<<blocks_for(n, 128), 128, 0, st>>>(
+      reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(target_psd),
+      reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_zero_degree_normalization(const void* vector, int n, int D, int reference_channel, void* out, void* stream) {
+  PBB_CHECK_ARG(vector != nullptr, 1, "vector is null");
+  PBB_CHECK_ARG(n > 0 && D > 0, 2, "bad shape");
+  PBB_CHECK_ARG(reference_channel >= 0 && reference_channel < D, 4, "need 0 <= reference_channel < D");
+  PBB_CHECK_ARG(out != nullptr, 5, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("zero_degree_kernel", st);
+  zero_degree_kernel<<<blocks_for((size_t)n * D, 256), 256, 0, st>>>(reinterpret_cast<const double2*>(vector), n, D,
+                                                                      reference_channel,
+                                                                      reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_phase_correction(const void* vector, int A, int M, int F, int D, int scan_bins, void* out, void* stream) {
+  PBB_CHECK_ARG(vector != nullptr, 1, "vector is null");
+  PBB_CHECK_ARG(A > 0 && M > 0 && F > 0 && D > 0, 2, "bad shape");
+  PBB_CHECK_ARG(!scan_bins || (A == 1 && M == 1), 6, "scan_bins needs A = M = 1");
+  PBB_CHECK_ARG(out != nullptr, 7, "out is null");
+  PBB_CHECK_ARG(out != vector, 7, "out must not alias vector");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("phase_correction_kernel", st);
+  const size_t threads = scan_bins ? 1 : (size_t)M * F;
+  phase_correction_kernel<<<blocks_for(threads, 128), 128, 0, st>>>(reinterpret_cast<const double2*>(vector), A, M, F,
+                                                                    D, scan_bins, reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_apply_online_beamforming_vector(const void* vector, const void* mix, int dtype, int B, int F, int D, int T,
+                                        long long vector_frame_stride, long long vector_bin_stride,
+                                        long long mix_batch_stride, long long mix_bin_stride, void* out,
+                                        void* stream) {
+  PBB_CHECK_ARG(vector && mix, 1, "input is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 3, "bad dtype");
+  PBB_CHECK_ARG(B > 0 && F > 0 && F <= 65535 && D > 0 && T > 0, 4, "bad shape");
+  PBB_CHECK_ARG(vector_frame_stride >= 0 && vector_bin_stride >= 0 && mix_batch_stride >= 0 && mix_bin_stride >= 0,
+                8, "strides must be non-negative");
+  PBB_CHECK_ARG(out != nullptr, 12, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  dim3 grid((T + 127) / 128, F);
+  LaunchScope ls("apply_online_kernel", st);
+  if (dtype == PBB_C128)
+    apply_online_kernel<double2><<<grid, 128, 0, st>>>(
+        reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(mix), B, F, D, T,
+        vector_frame_stride, vector_bin_stride, mix_batch_stride, mix_bin_stride, reinterpret_cast<double2*>(out));
+  else
+    apply_online_kernel<float2><<<grid, 128, 0, st>>>(
+        reinterpret_cast<const double2*>(vector), reinterpret_cast<const float2*>(mix), B, F, D, T,
+        vector_frame_stride, vector_bin_stride, mix_batch_stride, mix_bin_stride, reinterpret_cast<double2*>(out));
   PBB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -165,8 +165,12 @@ __host__ __device__ inline size_t solve_smem_per_warp(int D, int R) {
 // ~1e-7 of the largest count as zero there).  An
 // all-zero A gives X = 0 (test_beamformer.py:211-376).  Non-finite input propagates as NaN, as it does in LAPACK.
 // status (may be null) is only set when the fallback is unavailable (D > kLstsqMaxD).
+// strict != 0 is plain np.linalg.solve (get_mvdr_vector_merl, beamformer.py:277): a zero pivot takes no fallback and
+// sets status instead; x of that system is then undefined.  fallback (may be null) is set to 1 when any system of the
+// batch met a zero pivot, i.e. when the reference's stable_solve left np.linalg.solve for its per-matrix loop.
 __global__ void solve_kernel(const double2* __restrict__ a, const double2* __restrict__ b, int n, int D, int R,
-                             int hermitize, double2* __restrict__ x, int* status, int warps) {
+                             int hermitize, double2* __restrict__ x, int* status, int warps, int strict = 0,
+                             int* fallback = nullptr) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m = blockIdx.x * warps + warp;
@@ -222,6 +226,7 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
     }
     __syncwarp();
   }
+  if (singular && fallback && lane == 0) atomicOr(fallback, 1);
   if (nonfinite) {
     for (int i = lane; i < D * R; i += 32) X[i] = make_double2(NAN, NAN);
     __syncwarp();
@@ -237,7 +242,7 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
       }
     }
     __syncwarp();
-  } else if (D > kLstsqMaxD) {
+  } else if (strict || D > kLstsqMaxD) {
     if (lane == 0 && status) atomicMax(status, m + 1);
   } else {
     // ---- minimum-norm least squares (np.linalg.lstsq) ----
@@ -339,6 +344,29 @@ __global__ void mvdr_scale_kernel(const double2* __restrict__ atf, const double2
   for (int d = 0; d < D; ++d) w[(size_t)m * D + d] = cdiv(x[(size_t)m * D + d], den);
 }
 
+// ---- quadratic forms w^H T w and w^H N w of one D-vector, w_d = wat(d) --------------
+// The per-channel SNR terms of get_optimal_reference_channel (beamformer.py:616-620, w = w_mat[:, R]) and of
+// mvdr_snr_postfilter (:502-509).  T and N point at one D x D matrix each.
+template <class W>
+__device__ __forceinline__ void quad_forms(W wat, const double2* __restrict__ T, const double2* __restrict__ N, int D,
+                                           double2& qt, double2& qn) {
+  qt = make_double2(0.0, 0.0);
+  qn = make_double2(0.0, 0.0);
+  for (int d = 0; d < D; ++d) {
+    const double2 w = wat(d);
+    const double2 wd = make_double2(w.x, -w.y);  // conj(w_d)
+    double2 tt = make_double2(0.0, 0.0), nn = make_double2(0.0, 0.0);
+    for (int e = 0; e < D; ++e) {
+      const double2 we = wat(e);
+      const double2 a = cmul(T[d * D + e], we);
+      const double2 b = cmul(N[d * D + e], we);
+      tt.x += a.x; tt.y += a.y; nn.x += b.x; nn.y += b.y;
+    }
+    const double2 a = cmul(wd, tt), b = cmul(wd, nn);
+    qt.x += a.x; qt.y += a.y; qn.x += b.x; qn.y += b.y;
+  }
+}
+
 // ---- Souden MVDR pieces (beamformer.py:601-698) --------------------------------
 // mat = phi / max(trace(phi).real, eps); per-bin SNR numerators / denominators for
 // every candidate reference channel R: w_R = mat[:, R]
@@ -356,20 +384,9 @@ __global__ void souden_kernel(const double2* __restrict__ phi, const double2* __
     const double2 v = ph[d * D + R];
     mat[(size_t)m * D * D + d * D + R] = make_double2(v.x * s, v.y * s);
   }
-  // quadratic forms w^H T w and w^H N w with w = mat[:, R]
-  double2 qt = make_double2(0.0, 0.0), qn = make_double2(0.0, 0.0);
-  for (int d = 0; d < D; ++d) {
-    const double2 wd = make_double2(ph[d * D + R].x * s, -ph[d * D + R].y * s);  // conj(w_d)
-    double2 tt = make_double2(0.0, 0.0), nn = make_double2(0.0, 0.0);
-    for (int e = 0; e < D; ++e) {
-      const double2 we = make_double2(ph[e * D + R].x * s, ph[e * D + R].y * s);
-      const double2 a = cmul(target[(size_t)m * D * D + d * D + e], we);
-      const double2 b = cmul(noise[(size_t)m * D * D + d * D + e], we);
-      tt.x += a.x; tt.y += a.y; nn.x += b.x; nn.y += b.y;
-    }
-    const double2 a = cmul(wd, tt), b = cmul(wd, nn);
-    qt.x += a.x; qt.y += a.y; qn.x += b.x; qn.y += b.y;
-  }
+  double2 qt, qn;
+  quad_forms([&](int d) { return make_double2(ph[d * D + R].x * s, ph[d * D + R].y * s); },
+             target + (size_t)m * D * D, noise + (size_t)m * D * D, D, qt, qn);
   num[(size_t)m * D + R] = qt;
   den[(size_t)m * D + R] = qn;
 }

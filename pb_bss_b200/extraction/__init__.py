@@ -2,11 +2,23 @@
 from . import linalg  # noqa: F401
 from .beamformer import (  # noqa: F401
     apply_beamforming_vector,
+    apply_online_beamforming_vector,
     blind_analytic_normalization,
+    condition_covariance,
+    distortionless_normalization,
     get_gev_vector,
+    get_lcmv_vector,
+    get_lcmv_vector_souden,
     get_mvdr_vector,
+    get_mvdr_vector_merl,
     get_mvdr_vector_souden,
+    get_optimal_reference_channel,
+    get_pca,
     get_pca_vector,
     get_power_spectral_density_matrix,
+    get_wmwf_vector,
+    mvdr_snr_postfilter,
+    phase_correction,
+    zero_degree_normalization,
 )
 from .beamformer_wrapper import get_bf_vector  # noqa: F401

@@ -18,6 +18,18 @@ __all__ = [
     'get_gev_vector',
     'blind_analytic_normalization',
     'apply_beamforming_vector',
+    'get_pca',
+    'get_mvdr_vector_merl',
+    'get_lcmv_vector',
+    'get_lcmv_vector_souden',
+    'get_wmwf_vector',
+    'get_optimal_reference_channel',
+    'condition_covariance',
+    'distortionless_normalization',
+    'mvdr_snr_postfilter',
+    'zero_degree_normalization',
+    'phase_correction',
+    'apply_online_beamforming_vector',
 ]
 
 
@@ -266,4 +278,308 @@ def apply_beamforming_vector(vector, mix):
     _lib.check(lib.pbb_apply_beamforming_vector(_device.ptr(vf), _device.ptr(yf), code, F, D, T,
                                                 _device.ptr(out), _device.stream_ptr()),
                'pbb_apply_beamforming_vector')
+    return _device.to_host(out.reshape(*lead, T), like_numpy)
+
+
+def _status():
+    s = _device.empty((1,), torch.int32)
+    s.zero_()
+    return s
+
+
+def _tiny(*arrays):
+    """np.finfo(dtype).tiny of the dtype the reference computes in (float32's tiny for complex64 inputs)."""
+    def np_dtype(a):
+        if _device.is_tensor(a):
+            return np.dtype(str(a.dtype).replace('torch.', ''))
+        return np.asarray(a).dtype
+    return np.finfo(np.result_type(*[np_dtype(a) for a in arrays])).tiny
+
+
+def get_pca(target_psd_matrix, return_all_vecs=False):
+    """All principal components and eigenvalues, beamformer.py:163-194: (eigenvectors, eigenvalues) with
+    return_all_vecs, else the eigenvector of the largest eigenvalue (..., D) and that eigenvalue (...)."""
+    w, v = eigh(target_psd_matrix)
+    if return_all_vecs:
+        return v, w
+    vec, val = v[..., -1], w[..., -1]
+    if _device.is_tensor(vec):
+        vec, val = vec.contiguous(), val.contiguous()
+    return vec, val
+
+
+def get_optimal_reference_channel(w_mat, target_psd_matrix, noise_psd_matrix, eps=None):
+    """Reference channel of the largest summed SNR, beamformer.py:601-624.  w_mat, target, noise (F, D, D).
+    The per-bin quadratic forms and their sums over the bins run on the device; the D sums come to the host for the
+    division by max(den, eps) (NumPy's complex maximum), the finiteness assertion and the argmax."""
+    if np.ndim(w_mat) != 3:
+        raise ValueError(
+            'Estimating the ref_channel expects currently that the input '
+            'has 3 ndims (frequency x sensors x sensors). '
+            'Considering an independent dim in the SNR estimate is not '
+            'unique.')
+    if eps is None:
+        eps = _tiny(w_mat)
+    w = _device.to_device(w_mat, torch.complex128)
+    n, D, _ = w.shape
+    t = _device.to_device(target_psd_matrix, torch.complex128).expand(n, D, D).contiguous()
+    nz = _device.to_device(noise_psd_matrix, torch.complex128).expand(n, D, D).contiguous()
+    num = _device.empty((n, D), torch.complex128)
+    den = _device.empty((n, D), torch.complex128)
+    nsum = _device.empty((D,), torch.complex128)
+    dsum = _device.empty((D,), torch.complex128)
+    lib = _lib.load()
+    _lib.check(lib.pbb_reference_channel_snr(_device.ptr(w), _device.ptr(t), _device.ptr(nz), n, D, _device.ptr(num),
+                                             _device.ptr(den), _device.ptr(nsum), _device.ptr(dsum),
+                                             _device.stream_ptr()), 'pbb_reference_channel_snr')
+    ns, ds = nsum.cpu().numpy(), dsum.cpu().numpy()
+    snr = ns / np.maximum(ds, eps)
+    assert np.all(np.isfinite(snr)), snr
+    return int(np.argmax(snr.real))
+
+
+def get_mvdr_vector_merl(target_psd_matrix, noise_psd_matrix):
+    """MVDR variant of MERL TR2016-072, beamformer.py:263-289.  target, noise (F, D, D) -> (F, D).
+
+    G = solve(noise, target) with np.linalg.solve (an exactly singular noise matrix raises
+    np.linalg.LinAlgError, there is no lstsq fallback), h = G / trace(G).  The reference then picks the channel of
+    the largest post-SNR, but its np.sum over the per-channel einsum output sums the channels as well, so the SNR is
+    a scalar and the argmax is always 0: the result is h[..., 0], the WMWF filter with distortion_weight = 0 at
+    channel 0.  This is reproduced, and no SNR is computed."""
+    like_numpy = not _device.is_tensor(target_psd_matrix)
+    t = _device.to_device(target_psd_matrix, torch.complex128)
+    nz = _device.to_device(noise_psd_matrix, torch.complex128)
+    if t.dim() != 3 or nz.dim() != 3:
+        raise ValueError('einstein sum subscripts string contains too many subscripts for operand 1: '
+                         f'target {tuple(t.shape)} and noise {tuple(nz.shape)} must be (bins, sensors, sensors)')
+    if t.shape != nz.shape or t.shape[-1] != t.shape[-2]:
+        raise ValueError(f'shape mismatch: target {tuple(t.shape)}, noise {tuple(nz.shape)}')
+    n, D, _ = t.shape
+    w = _device.empty((n, D), torch.complex128)
+    scratch = _device.empty((n, D, D), torch.complex128)
+    status = _status()
+    lib = _lib.load()
+    _lib.check(lib.pbb_mvdr_merl(_device.ptr(t), _device.ptr(nz), n, D, _device.ptr(w), _device.ptr(scratch),
+                                 _device.ptr(status), _device.stream_ptr()), 'pbb_mvdr_merl')
+
+    def on_error(s):
+        raise np.linalg.LinAlgError(f'Singular matrix (get_mvdr_vector_merl: noise PSD matrix of bin {s - 1})')
+    _device.check_status(status, on_error)
+    return _device.to_host(w, like_numpy)
+
+
+def get_lcmv_vector(atf_vectors, response_vector, noise_psd_matrix):
+    """LCMV beamformer, beamformer.py:414-456.  atf_vectors (K, F, D), response_vector (K,), noise_psd_matrix
+    (F, D, D) -> (F, D).  Like the reference the response is rounded to complex64, so H^H w meets
+    float32(response), and both solves have stable_solve semantics (an exactly singular system takes its
+    minimum-norm solution)."""
+    like_numpy = not _device.is_tensor(atf_vectors)
+    a = _device.to_device(atf_vectors, torch.complex128)
+    if a.dim() != 3:
+        raise ValueError(f'not enough values to unpack (expected 3, got {a.dim()})' if a.dim() < 3
+                         else f'too many values to unpack (expected 3, got {a.dim()})')
+    K, F, D = a.shape
+    nz = _device.to_device(noise_psd_matrix, torch.complex128)
+    assert tuple(nz.shape) == (F, D, D), nz.shape
+    r = _device.to_device(response_vector if _device.is_tensor(response_vector) else np.asarray(response_vector),
+                          torch.complex128).reshape(-1)
+    if r.numel() != K:
+        raise ValueError(f'response_vector has {r.numel()} entries for {K} ATF vectors')
+    w = _device.empty((F, D), torch.complex128)
+    scratch = _device.empty((F * (2 * D * K + K * K + 2 * K) + 1,), torch.complex128)
+    status = _status()
+    lib = _lib.load()
+    _lib.check(lib.pbb_lcmv(_device.ptr(a), _device.ptr(r), _device.ptr(nz), K, F, D, _device.ptr(w),
+                            _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_lcmv')
+
+    def on_error(s):
+        raise np.linalg.LinAlgError(f'get_lcmv_vector: singular system in bin {s - 1} (D or K > 40: no lstsq fallback)')
+    _device.check_status(status, on_error)
+    return _device.to_host(w, like_numpy)
+
+
+def get_lcmv_vector_souden(target_psd_matrix, interference_psd_matrix, noise_psd_matrix, ref_channel=None,
+                           eps=None, return_ref_channel=False):
+    """beamformer.py:756-787: not implemented in the reference either, which raises before computing anything."""
+    raise NotImplementedError(
+        'This is not yet thoroughly tested. It also misses the response vector,'
+        'thus it is unclear, how to select, which speaker to attend to.'
+    )
+
+
+def get_wmwf_vector(target_psd_matrix, noise_psd_matrix, reference_channel=None, channel_selection_vector=None,
+                    distortion_weight=1.):
+    """Speech distortion weighted multichannel Wiener filter, beamformer.py:701-753.
+
+    phi = stable_solve(noise, target), lambda = trace(phi); the filter is phi / (distortion_weight + lambda) or, with
+    distortion_weight='frequency_dependent', phi / sqrt(target[..., 0, 0] * lambda).  Then the channel_selection_vector
+    weighted sum over the columns, or column reference_channel (chosen by get_optimal_reference_channel when None)."""
+    assert noise_psd_matrix is not None
+    like_numpy = not _device.is_tensor(target_psd_matrix)
+    t = _device.to_device(target_psd_matrix, torch.complex128)
+    nz = _device.to_device(noise_psd_matrix, torch.complex128)
+    D = t.shape[-1]
+    lead = tuple(torch.broadcast_shapes(t.shape[:-2], nz.shape[:-2]))
+    tf = t.expand(*lead, D, D).reshape(-1, D, D).contiguous()
+    nf = nz.expand(*lead, D, D).reshape(-1, D, D).contiguous()
+    n = tf.shape[0]
+    frequency_dependent = isinstance(distortion_weight, str)
+    if frequency_dependent and distortion_weight != 'frequency_dependent':
+        raise TypeError(f'distortion_weight must be a number or "frequency_dependent", got {distortion_weight!r}')
+    mu = 0.0 if frequency_dependent else float(distortion_weight)
+    filt = _device.empty((n, D, D), torch.complex128)
+    scratch = _device.empty((n, D, D), torch.complex128)
+    status = _status()
+    lib = _lib.load()
+    _lib.check(lib.pbb_wmwf(_device.ptr(tf), _device.ptr(nf), n, D, int(frequency_dependent), mu, _device.ptr(filt),
+                            _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_wmwf')
+
+    def on_error(s):
+        raise np.linalg.LinAlgError(f'get_wmwf_vector: singular noise PSD matrix {s - 1} (D > 40: no lstsq fallback)')
+    _device.check_status(status, on_error)
+    filt = filt.reshape(*lead, D, D)
+    if channel_selection_vector is not None:
+        sel = _device.to_device(channel_selection_vector, torch.complex128)[..., None, :]
+        shape = tuple(torch.broadcast_shapes(filt.shape, sel.shape))
+        ff = filt.expand(shape).reshape(-1, D, D).contiguous()
+        sf = sel.expand(shape).reshape(-1, D, D).contiguous()
+        out = _device.empty((ff.shape[0], D), torch.complex128)
+        _lib.check(lib.pbb_weighted_channel_sum(_device.ptr(ff), _device.ptr(sf), ff.shape[0], D, _device.ptr(out),
+                                                _device.stream_ptr()), 'pbb_weighted_channel_sum')
+        return _device.to_host(out.reshape(shape[:-1]), like_numpy)
+    if reference_channel is None:
+        reference_channel = get_optimal_reference_channel(filt, tf.reshape(*lead, D, D), nf.reshape(*lead, D, D),
+                                                          eps=_tiny(target_psd_matrix, noise_psd_matrix))
+    assert np.isscalar(reference_channel), reference_channel
+    return _device.to_host(filt[..., reference_channel].contiguous(), like_numpy)
+
+
+def condition_covariance(x, gamma):
+    """(x + gamma * trace(x) / D * I) / (1 + gamma) with the complex trace, beamformer.py:563-569; x (..., D, D)."""
+    like_numpy = not _device.is_tensor(x)
+    xd = _device.to_device(x, torch.complex128)
+    D = xd.shape[-1]
+    xf, lead = _flat(xd, 2)
+    out = _device.empty(xf.shape, torch.complex128)
+    lib = _lib.load()
+    _lib.check(lib.pbb_condition_covariance(_device.ptr(xf), xf.shape[0], D, float(gamma), _device.ptr(out),
+                                            _device.stream_ptr()), 'pbb_condition_covariance')
+    return _device.to_host(out.reshape(*lead, D, D), like_numpy)
+
+
+def _bins(name, t, ndim):
+    if t.dim() != ndim:
+        raise ValueError(f'{name} must have {ndim} dims (the reference einsum subscripts are fixed), '
+                         f'got shape {tuple(t.shape)}')
+    return t
+
+
+def distortionless_normalization(vector, atf_vector, noise_psd_matrix):
+    """N w w^H a / (w^H N w), beamformer.py:491-499.  vector, atf_vector (F, D), noise_psd_matrix (F, D, D)."""
+    like_numpy = not _device.is_tensor(vector)
+    v = _bins('vector', _device.to_device(vector, torch.complex128), 2)
+    a = _bins('atf_vector', _device.to_device(atf_vector, torch.complex128), 2)
+    nz = _bins('noise_psd_matrix', _device.to_device(noise_psd_matrix, torch.complex128), 3)
+    F, D = v.shape
+    if a.shape != v.shape or tuple(nz.shape) != (F, D, D):
+        raise ValueError(f'shape mismatch: {tuple(v.shape)}, {tuple(a.shape)}, {tuple(nz.shape)}')
+    out = _device.empty((F, D), torch.complex128)
+    lib = _lib.load()
+    _lib.check(lib.pbb_distortionless_normalization(_device.ptr(v), _device.ptr(a), _device.ptr(nz), F, D,
+                                                    _device.ptr(out), _device.stream_ptr()),
+               'pbb_distortionless_normalization')
+    return _device.to_host(out, like_numpy)
+
+
+def mvdr_snr_postfilter(vector, target_psd_matrix, noise_psd_matrix):
+    """(w^H T w) / (w^H N w) per bin, beamformer.py:502-509.  vector (F, D), PSDs (F, D, D) -> (F, 1)."""
+    like_numpy = not _device.is_tensor(vector)
+    v = _bins('vector', _device.to_device(vector, torch.complex128), 2)
+    t = _bins('target_psd_matrix', _device.to_device(target_psd_matrix, torch.complex128), 3)
+    nz = _bins('noise_psd_matrix', _device.to_device(noise_psd_matrix, torch.complex128), 3)
+    F, D = v.shape
+    if tuple(t.shape) != (F, D, D) or tuple(nz.shape) != (F, D, D):
+        raise ValueError(f'shape mismatch: {tuple(v.shape)}, {tuple(t.shape)}, {tuple(nz.shape)}')
+    out = _device.empty((F, 1), torch.complex128)
+    lib = _lib.load()
+    _lib.check(lib.pbb_mvdr_snr_postfilter(_device.ptr(v), _device.ptr(t), _device.ptr(nz), F, D, _device.ptr(out),
+                                           _device.stream_ptr()), 'pbb_mvdr_snr_postfilter')
+    return _device.to_host(out, like_numpy)
+
+
+def zero_degree_normalization(vector, reference_channel):
+    """vector * exp(-1j * angle(vector[..., reference_channel])), beamformer.py:512-514; vector (..., D)."""
+    like_numpy = not _device.is_tensor(vector)
+    v = _device.to_device(vector, torch.complex128)
+    D = v.shape[-1]
+    ref = int(reference_channel)
+    if not -D <= ref < D:
+        raise IndexError(f'index {ref} is out of bounds for axis {v.dim() - 1} with size {D}')
+    vf, lead = _flat(v, 1)
+    out = _device.empty(vf.shape, torch.complex128)
+    lib = _lib.load()
+    _lib.check(lib.pbb_zero_degree_normalization(_device.ptr(vf), vf.shape[0], D, ref % D, _device.ptr(out),
+                                                 _device.stream_ptr()), 'pbb_zero_degree_normalization')
+    return _device.to_host(out.reshape(*lead, D), like_numpy)
+
+
+def phase_correction(vector):
+    """Phase correction of consecutive bins, beamformer.py:517-560; vector (..., bins, sensors), not modified.
+
+    Bin f >= 1 is multiplied by the cumulative product of exp(1j * angle(sum_d conj(w_f) w_{f-1})).  The reference
+    takes that product along axis 0 of the whole array, and so does this: for an (F, D) input it runs over the bins,
+    for a (K, F, D) input over K, for every bin on its own.  Real input raises a TypeError, as NumPy's in-place
+    complex multiplication does in the reference."""
+    like_numpy = not _device.is_tensor(vector)
+    if like_numpy:
+        vector = np.asarray(vector)
+        complex_in = np.iscomplexobj(vector)
+    else:
+        complex_in = vector.is_complex()
+    if not complex_in:
+        raise TypeError(f"Cannot cast ufunc 'multiply' output from dtype('complex128') to the real input's dtype "
+                        f"({vector.dtype}) with casting rule 'same_kind'")
+    v = _device.to_device(vector, torch.complex128)
+    if v.dim() < 2:
+        raise IndexError('too many indices for array: phase_correction needs (..., bins, sensors)')
+    F, D = v.shape[-2:]
+    if v.dim() == 2:
+        A, M, scan = 1, 1, 1
+    else:
+        A, M, scan = v.shape[0], int(np.prod(v.shape[1:-2])), 0
+    out = _device.empty(tuple(v.shape), torch.complex128)
+    if out.numel() == 0:
+        return _device.to_host(out, like_numpy)
+    lib = _lib.load()
+    _lib.check(lib.pbb_phase_correction(_device.ptr(v), A, M, F, D, scan, _device.ptr(out), _device.stream_ptr()),
+               'pbb_phase_correction')
+    return _device.to_host(out, like_numpy)
+
+
+def apply_online_beamforming_vector(vector, mix):
+    """Time-varying beamforming, beamformer.py:586-598: out[..., f, t] = sum_d conj(vector[t, f, d]) mix[..., f, d, t].
+
+    vector (T, F, D); mix (..., F, D, T) complex64 or complex128 -> (..., F, T) complex128.  The leading dims of the
+    mix are read in place by one launch that reads the vector once; a mix that is only broadcast over a leading dim
+    (stride 0) is not copied either."""
+    like_numpy = not _device.is_tensor(mix)
+    v = _device.to_device(vector, torch.complex128)
+    if v.dim() != 3:
+        raise ValueError("axes don't match array: vector must be (frames, bins, sensors)")
+    y = _device.to_device(mix)
+    code = _device.complex_dtype_code(y)
+    T, Fv, D = v.shape
+    if y.dim() < 2 or y.shape[-2] != D or y.shape[-1] != T:
+        raise ValueError(f'operands could not be broadcast together: vector {tuple(v.shape)}, mix {tuple(y.shape)}')
+    lead = tuple(torch.broadcast_shapes((Fv,), y.shape[:-2]))
+    F = lead[-1]
+    B = int(np.prod(lead[:-1])) if len(lead) > 1 else 1
+    ye = y.expand(*lead, D, T).reshape(B, F, D, T)
+    if ye.stride(2) != T or ye.stride(3) != 1:
+        ye = ye.contiguous()
+    out = _device.empty((B, F, T), torch.complex128)
+    lib = _lib.load()
+    _lib.check(lib.pbb_apply_online_beamforming_vector(
+        _device.ptr(v), _device.ptr(ye), code, B, F, D, T, Fv * D, D if Fv == F else 0, ye.stride(0), ye.stride(1),
+        _device.ptr(out), _device.stream_ptr()), 'pbb_apply_online_beamforming_vector')
     return _device.to_host(out.reshape(*lead, T), like_numpy)
