@@ -13,14 +13,9 @@
 #include "em_kernels.cuh"
 #include "em_persistent.cuh"
 #include "em_ws.cuh"
-#include "em_ls.cuh"
 #include "em_sticky.cuh"
 #include "bingham.cuh"
 #include "prof.cuh"
-
-#ifndef PBB_CTA_FPL
-#define PBB_CTA_FPL 2
-#endif
 
 namespace pbb {
 
@@ -118,7 +113,7 @@ static CacgmmWorkspace carve(void* base, int F, int T, int D, int K) {
   const size_t o_flags = take((size_t)(F + 1) * sizeof(int) + 16 * sizeof(unsigned long long) + 8);
   const size_t o_dead = take((size_t)F * sizeof(int));
   const size_t o_part = take((size_t)F * max_chunks(T) * K * (NS + 1) * sizeof(double));
-  const size_t o_coef = take((size_t)F * (K * NS + 8) * sizeof(double));  // em_ls.cuh model blocks: + 64 B per bin
+  const size_t o_coef = take((size_t)F * K * NS * sizeof(double));
   const size_t o_ld = take((size_t)F * (K > 4 ? K : 4) * sizeof(double) + 64);  // lean kernel: stride 4
   const size_t o_w = take((size_t)F * K * sizeof(double));
   const size_t o_ew = take((size_t)F * (K > 4 ? K : 4) * sizeof(double) + 64);  // lean kernel: stride 4
@@ -168,10 +163,9 @@ static int choose_frame_split(int F, int T, int D, int K, int ctas_per_sm, int s
 // Cluster size of the sticky-bins kernel (em_sticky.cuh), 0 = not applicable: the largest of 4, 2, 1 whose parts fit
 // the ring (ceil(nchunks / S) <= kWsStages), that leaves every part a stage and whose F clusters run at once:
 // F <= clusters[i] for S = 1 << i.  Clusters of 4 are placed within a GPC, so on an H100 (132 SMs in GPCs of uneven
-// size) fewer of them fit than 2 x SMs / 4; a second wave would double the fit time.  force: -1 automatic, 0 off,
-// S > 0 only that size (PBB_STICKY).
+// size) fewer of them fit than 2 x SMs / 4; a second wave would double the fit time.  force: -1 automatic, S > 0
+// only that size (PBB_STICKY).
 static int choose_sticky(int F, int T, const int clusters[3], int force) {
-  if (force == 0) return 0;
   const int zs = (T + 31) / 32 * 32;
   const int nchunks = (zs + kStageFrames - 1) / kStageFrames;
   for (int c = 4, i = 2; c >= 1; c /= 2, --i) {
@@ -183,14 +177,58 @@ static int choose_sticky(int F, int T, const int clusters[3], int force) {
   return 0;
 }
 
-static int setup_frame_split(PersistArgs* p, const CacgmmWorkspace& ws, int F, int T, int D, int K, int ctas_per_sm,
-                             cudaStream_t st) {
-  int dev = 0, sms = 0;
+// Persistent kernels of a fit, numbered as pbb_em_dispatch reports them (pbb.h).
+enum { kKernelWs = 0, kKernelSticky = 1, kKernelSingle = 2 };
+
+// Tuning overrides of the kernel choice (environment of pbb_cacgmm_fit).
+struct PlanOverrides {
+  int tsplit = 0;       // > 0: frame split into that many parts (PBB_TSPLIT)
+  int sticky = -1;      // sticky-bins cluster size: -1 automatic, 0 off, S > 0 only S (PBB_STICKY)
+  bool single = false;  // single-role kernel only (PBB_EM_KERNEL=single; the complex Watson fit has no other)
+};
+
+struct FitPlan {
+  int kernel;  // kKernel*
+  int split;   // sticky: CTAs per cluster; otherwise parts per bin-iteration (1 = no frame split)
+};
+
+static PlanOverrides env_overrides() {
+  static const bool single = [] {
+    const char* e = getenv("PBB_EM_KERNEL");
+    return e != nullptr && !strcmp(e, "single");
+  }();
+  PlanOverrides o;
+  o.single = single;
+  if (const char* e = getenv("PBB_TSPLIT")) o.tsplit = atoi(e);
+  if (const char* e = getenv("PBB_STICKY")) o.sticky = atoi(e);
+  return o;
+}
+
+// The sticky-bins kernel exists for the lean D = 8 fit of device-resident input.
+static bool sticky_eligible(int D, bool lean, bool streamed, const PlanOverrides& o) {
+  return D == 8 && lean && !streamed && !o.single && o.sticky != 0;
+}
+
+// Which persistent kernel a fit runs and how it splits a bin-iteration (pure host logic).  sms: SMs of the device;
+// clusters: sticky-kernel clusters of 1, 2, 4 CTAs the device runs at once, read only when sticky_eligible.
+static FitPlan plan_persistent_fit(int F, int T, int D, int K, bool lean, bool streamed, int sms,
+                                   const int* clusters, const PlanOverrides& o) {
+  if (sticky_eligible(D, lean, streamed, o)) {
+    const int S = choose_sticky(F, T, clusters, o.sticky);
+    if (S > 0) return {kKernelSticky, S};
+  }
+  const int kernel = D == 8 && lean && !o.single ? kKernelWs : kKernelSingle;
+  return {kernel, choose_frame_split(F, T, D, K, persist_ctas_per_sm(D, !lean), sms, o.tsplit)};
+}
+
+static int device_sms(int* sms) {
+  int dev = 0;
   PBB_CUDA(cudaGetDevice(&dev));
-  PBB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  int force = 0;
-  if (const char* e = getenv("PBB_TSPLIT")) force = atoi(e);  // tuning override
-  const int S = choose_frame_split(F, T, D, K, ctas_per_sm, sms, force);
+  PBB_CUDA(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+  return 0;
+}
+
+static int setup_frame_split(PersistArgs* p, const CacgmmWorkspace& ws, int F, int D, int K, int S, cudaStream_t st) {
   if (S > 1) {
     p->tsplit = S;
     p->tpart = ws.part + (size_t)F * K * ((size_t)D * D + 1);
@@ -213,22 +251,8 @@ static int launch_normalize(const void* y, void* z, int F, int T, int D, int swa
   return 0;
 }
 
-// D = 8 lean fits run on em_ws_kernel.  PBB_EM_KERNEL=ls selects the round-2 lane = slot kernel (em_ls.cuh, staged
-// layout 1; 3.88 ms vs 3.18 ms on the C2 fit on an H100, scripts/ab_kernels.py), PBB_EM_KERNEL=single (or PBB_NO_WS) the
-// single-role persistent kernel.
-static int em_kernel_choice() {
-  static const int c = [] {
-    const char* e = getenv("PBB_EM_KERNEL");
-    if (e == nullptr) return getenv("PBB_NO_WS") != nullptr ? 2 : 1;
-    if (!strcmp(e, "ls")) return 0;
-    if (!strcmp(e, "single")) return 2;
-    return 1;
-  }();
-  return c;  // 0 = em_ls_kernel, 1 = em_ws_kernel, 2 = em_persistent_kernel
-}
-static bool use_ls_kernel(int D, bool full) { return D == 8 && !full && em_kernel_choice() == 0; }
 template <typename CT>
-static int launch_normalize_staged(const void* y, void* z, int F, int T, int D, int* dead, int layout, cudaStream_t st) {
+static int launch_normalize_staged(const void* y, void* z, int F, int T, int D, int* dead, cudaStream_t st) {
   if (dead != nullptr) PBB_CUDA(cudaMemsetAsync(dead, 0, (size_t)F * sizeof(int), st));
   const int block = 64;  // divides kStageFrames
   const int nchunks = (((T + 31) / 32 * 32) + kStageFrames - 1) / kStageFrames;
@@ -236,8 +260,7 @@ static int launch_normalize_staged(const void* y, void* z, int F, int T, int D, 
   const size_t smem = (size_t)block * (D + 1) * sizeof(double2);
   LaunchScope ls("normalize_staged_kernel", st);
   normalize_staged_kernel<CT><<<grid, block, smem, st>>>(reinterpret_cast<const CT*>(y), reinterpret_cast<CT*>(z), F, T, D,
-                                                          layout == 0 ? stage_rows(D) : D, kStageFrames, nchunks, dead,
-                                                          layout);
+                                                          stage_rows(D), kStageFrames, nchunks, dead);
   PBB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -448,8 +471,7 @@ static int get_load_stream(LoadStream** out) {
 
 template <typename CT>
 static int launch_stream_load(const void* y, void* z, const double* aff_src, double* aff_dst, int F, int T, int D, int K,
-                              int* dead, int* flags, int* next_bin, int* started, int* ctas_out, int layout,
-                              cudaStream_t st) {
+                              int* dead, int* flags, int* next_bin, int* started, int* ctas_out, cudaStream_t st) {
   const int nchunks = (((T + 31) / 32 * 32) + kStageFrames - 1) / kStageFrames;
   const size_t smem = (size_t)kStageFrames * (D + 1) * sizeof(double2);
   LaunchScope ls("stream_load_kernel", st);
@@ -459,7 +481,7 @@ static int launch_stream_load(const void* y, void* z, const double* aff_src, dou
   *ctas_out = ctas;
   stream_load_kernel<CT><<<ctas, kLoadThreads, smem, st>>>(
       reinterpret_cast<const CT*>(y), reinterpret_cast<CT*>(z), aff_src, aff_dst, F, T, D, K,
-      layout == 0 ? stage_rows(D) : D, kStageFrames, nchunks, dead, flags, next_bin, started, layout);
+      stage_rows(D), kStageFrames, nchunks, dead, flags, next_bin, started);
   PBB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -489,25 +511,21 @@ static int launch_persistent_generic(Kern kern, int threads, size_t smem, int* c
   return 0;
 }
 
-// full = saliency / activity mask / log-domain softmax; lean = product-form softmax, 2 frames per lane
+// full = saliency / activity mask / log-domain softmax; lean = product-form softmax, 2 frames per lane;
+// ws = the warp-specialised em_ws_kernel (D = 8, lean) instead of the single-role kernel
 template <int D, int K, typename CT>
-static int launch_persist_t(const PersistArgs& a, bool full, cudaStream_t st) {
+static int launch_persist_t(const PersistArgs& a, bool full, bool ws, cudaStream_t st) {
   static int cache_full = 0, cache_lean = 0;
   if (full)
     return launch_persistent_generic(em_persistent_kernel<D, K, CT, true, 1>, persist_threads(D, K),
                                      sizeof(PersistSmem<D, K, CT>), &cache_full, a, "em_persistent_kernel", st);
   if constexpr (D == 8) {
-    // lane = slot variant (em_ls.cuh): one task per SM, 16 compute warps, no barrier in the hot loop
-    static int cache_ls = 0, cache_ws = 0;
-    if (em_kernel_choice() == 0)
-      return launch_persistent_generic(em_ls_kernel<K, CT>, kLsThreads, sizeof(LsSmem<K, CT>), &cache_ls, a,
-                                       "em_ls_kernel", st);
-    // warp-specialised variant of round 1 (em_ws.cuh): PBB_EM_KERNEL=ws
-    if (em_kernel_choice() == 1)
+    static int cache_ws = 0;
+    if (ws)
       return launch_persistent_generic(em_ws_kernel<K, CT>, 256, sizeof(WsSmem<D, K, CT>), &cache_ws, a,
                                        "em_ws_kernel", st);
   }
-  return launch_persistent_generic(em_persistent_kernel<D, K, CT, false, PBB_CTA_FPL>, persist_threads(D, K),
+  return launch_persistent_generic(em_persistent_kernel<D, K, CT, false, 2>, persist_threads(D, K),
                                    sizeof(PersistSmem<D, K, CT>), &cache_lean, a, "em_persistent_kernel", st);
 }
 
@@ -515,7 +533,7 @@ static int launch_persist_t(const PersistArgs& a, bool full, cudaStream_t st) {
 template <int D, int K, typename CT>
 static int launch_persist_cw_t(const PersistArgs& a, cudaStream_t st) {
   static int cache = 0;
-  return launch_persistent_generic(em_persistent_kernel<D, K, CT, false, PBB_CTA_FPL, 1>, persist_threads(D, K),
+  return launch_persistent_generic(em_persistent_kernel<D, K, CT, false, 2, 1>, persist_threads(D, K),
                                    sizeof(PersistSmem<D, K, CT>), &cache, a, "em_persistent_kernel_cw", st);
 }
 template <int D>
@@ -536,17 +554,17 @@ static int launch_persist_cw(const PersistArgs& a, int D, int K, int dtype, cuda
 }
 
 template <int D, int K>
-static int launch_persist_dk(const PersistArgs& a, int dtype, bool full, cudaStream_t st) {
-  if (dtype == PBB_C128) return launch_persist_t<D, K, double2>(a, full, st);
-  return launch_persist_t<D, K, float2>(a, full, st);
+static int launch_persist_dk(const PersistArgs& a, int dtype, bool full, bool ws, cudaStream_t st) {
+  if (dtype == PBB_C128) return launch_persist_t<D, K, double2>(a, full, ws, st);
+  return launch_persist_t<D, K, float2>(a, full, ws, st);
 }
 
 template <int D>
-static int launch_persist_d(const PersistArgs& a, int K, int dtype, bool full, cudaStream_t st) {
+static int launch_persist_d(const PersistArgs& a, int K, int dtype, bool full, bool ws, cudaStream_t st) {
   switch (K) {
-    case 2: return launch_persist_dk<D, 2>(a, dtype, full, st);
-    case 3: return launch_persist_dk<D, 3>(a, dtype, full, st);
-    default: return launch_persist_dk<D, 4>(a, dtype, full, st);
+    case 2: return launch_persist_dk<D, 2>(a, dtype, full, ws, st);
+    case 3: return launch_persist_dk<D, 3>(a, dtype, full, ws, st);
+    default: return launch_persist_dk<D, 4>(a, dtype, full, ws, st);
   }
 }
 
@@ -566,47 +584,58 @@ static void sticky_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, un
   cfg->attrs = attr;
   cfg->numAttrs = 1;
 }
+// clusters of 1, 2, 4 CTAs of em_sticky_kernel the device runs at once (queried once per instantiation)
 template <int K, typename CT>
-static int launch_sticky_t(const PersistArgs& a, int force, bool* used, cudaStream_t st) {
-  static int clusters[3] = {-1, -1, -1};  // clusters of 1, 2, 4 CTAs the device runs at once (queried once)
-  const size_t smem = sizeof(WsSmem<8, K, CT>);
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  if (clusters[0] < 0) {
+static int sticky_clusters_t(int clusters[3], cudaStream_t st) {
+  static int cache[3] = {-1, -1, -1};
+  if (cache[0] < 0) {
+    const size_t smem = sizeof(WsSmem<8, K, CT>);
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr[1];
     PBB_CUDA(cudaFuncSetAttribute(em_sticky_kernel<K, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     for (int i = 0; i < 3; ++i) {
       sticky_config(&cfg, attr, 1u << i, 1 << i, smem, st);
       int n = 0;
       PBB_CUDA(cudaOccupancyMaxActiveClusters(&n, em_sticky_kernel<K, CT>, &cfg));
-      clusters[i] = n;
+      cache[i] = n;
     }
   }
-  const int S = choose_sticky(a.F, a.T, clusters, force);
-  if (S == 0) return 0;
-  *used = true;
-  sticky_config(&cfg, attr, (unsigned)(a.F * S), S, smem, st);
+  for (int i = 0; i < 3; ++i) clusters[i] = cache[i];
+  return 0;
+}
+static int sticky_clusters(int K, int dtype, int clusters[3], cudaStream_t st) {
+  const bool c128 = dtype == PBB_C128;
+  switch (K) {
+    case 2: return c128 ? sticky_clusters_t<2, double2>(clusters, st) : sticky_clusters_t<2, float2>(clusters, st);
+    case 3: return c128 ? sticky_clusters_t<3, double2>(clusters, st) : sticky_clusters_t<3, float2>(clusters, st);
+    default: return c128 ? sticky_clusters_t<4, double2>(clusters, st) : sticky_clusters_t<4, float2>(clusters, st);
+  }
+}
+
+// one cluster of S CTAs per bin; sticky_clusters has set the kernel's shared-memory limit
+template <int K, typename CT>
+static int launch_sticky_t(const PersistArgs& a, int S, cudaStream_t st) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute attr[1];
+  sticky_config(&cfg, attr, (unsigned)(a.F * S), S, sizeof(WsSmem<8, K, CT>), st);
   LaunchScope ls("em_sticky_kernel", st);
   PBB_CUDA(cudaLaunchKernelEx(&cfg, em_sticky_kernel<K, CT>, a));
   return 0;
 }
-static int launch_sticky(const PersistArgs& a, int K, int dtype, bool* used, cudaStream_t st) {
-  *used = false;
-  int force = -1;
-  if (const char* e = getenv("PBB_STICKY")) force = atoi(e);
-  if (force == 0) return 0;
+static int launch_sticky(const PersistArgs& a, int K, int dtype, int S, cudaStream_t st) {
   const bool c128 = dtype == PBB_C128;
   switch (K) {
-    case 2: return c128 ? launch_sticky_t<2, double2>(a, force, used, st) : launch_sticky_t<2, float2>(a, force, used, st);
-    case 3: return c128 ? launch_sticky_t<3, double2>(a, force, used, st) : launch_sticky_t<3, float2>(a, force, used, st);
-    default: return c128 ? launch_sticky_t<4, double2>(a, force, used, st) : launch_sticky_t<4, float2>(a, force, used, st);
+    case 2: return c128 ? launch_sticky_t<2, double2>(a, S, st) : launch_sticky_t<2, float2>(a, S, st);
+    case 3: return c128 ? launch_sticky_t<3, double2>(a, S, st) : launch_sticky_t<3, float2>(a, S, st);
+    default: return c128 ? launch_sticky_t<4, double2>(a, S, st) : launch_sticky_t<4, float2>(a, S, st);
   }
 }
 
-static int launch_persist(const PersistArgs& a, int D, int K, int dtype, bool full, cudaStream_t st) {
+static int launch_persist(const PersistArgs& a, int D, int K, int dtype, bool full, bool ws, cudaStream_t st) {
   switch (D) {
-    case 4: return launch_persist_d<4>(a, K, dtype, full, st);
-    case 6: return launch_persist_d<6>(a, K, dtype, full, st);
-    default: return launch_persist_d<8>(a, K, dtype, full, st);
+    case 4: return launch_persist_d<4>(a, K, dtype, full, ws, st);
+    case 6: return launch_persist_d<6>(a, K, dtype, full, ws, st);
+    default: return launch_persist_d<8>(a, K, dtype, full, ws, st);
   }
 }
 
@@ -716,14 +745,10 @@ int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms,
   PBB_CHECK_ARG(K >= 2 && K <= 4, 4, "persistent kernels: K in {2, 3, 4}");
   PBB_CHECK_ARG(sms > 0, 7, "sms must be positive");
   PBB_CHECK_ARG(kernel != nullptr && split != nullptr, 8, "output is null");
-  if (D == 8 && lean && !streamed) {
-    // machine model: two CTAs per SM, clusters placed anywhere
-    const int clusters[3] = {2 * sms, sms, sms / 2};
-    const int S = choose_sticky(F, T, clusters, -1);
-    if (S > 0) { *kernel = 1; *split = S; return 0; }
-  }
-  *kernel = (D == 8 && lean) ? 0 : 2;
-  *split = choose_frame_split(F, T, D, K, lean ? (D == 4 ? 4 : 2) : (D == 8 ? 3 : D == 6 ? 4 : 6), sms, 0);
+  const int clusters[3] = {2 * sms, sms, sms / 2};  // machine model: two CTAs per SM, clusters placed anywhere
+  const FitPlan plan = plan_persistent_fit(F, T, D, K, lean != 0, streamed != 0, sms, clusters, PlanOverrides{});
+  *kernel = plan.kernel;
+  *split = plan.split;
   return 0;
 }
 
@@ -787,11 +812,11 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
   const bool streamed = persistent && y_host && init_aff != nullptr && !(opt->reserved & 2) &&
                         ws.aff_stage != nullptr;
   const bool fast_sm = softmax_fast_ok(D, opt);
-  // lean variant: product-form softmax, needs (K-1) D log10(1/floor) < 290 (em_persistent.cuh)
-  // (one decade of margin per factor: em_ls.cuh scales the class matrices to trace [1, 2) instead of D)
+  // lean variant: product-form softmax, needs (K-1) D log10(1/floor) < 290 (em_persistent.cuh).  The extra decade
+  // per factor below is a margin kept as is: without it some fits (e.g. K = 4, D = 8 with floors between about 1e-12
+  // and 1e-11) would move from the full variant to the lean one.
   const bool lean_ok = fast_sm && (K - 1) * D * (log10(1.0 / opt->eigenvalue_floor) + 1.0) < 290.0;
   const bool full = saliency != nullptr || activity != nullptr || !lean_ok || init_aff == nullptr;
-  const int layout = persistent && use_ls_kernel(D, full) ? 1 : 0;
   // Thread safety: the side stream and the fork / join events of the streamed upload exist once per device, so two
   // host threads enqueueing streamed fits on the same device are serialised from here to the end of the call
   // (the enqueue only; the GPU work of the two fits still overlaps as far as their streams allow).
@@ -815,8 +840,8 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
     int* started = reinterpret_cast<int*>(ws.phase + 14);
     int ctas = 0;
     r = dtype == PBB_C128
-            ? launch_stream_load<double2>(y, ws.z, init_aff, aff_dst, F, T, D, K, ws.dead, ws.flags, next_bin, started, &ctas, layout, l->stream)
-            : launch_stream_load<float2>(y, ws.z, init_aff, aff_dst, F, T, D, K, ws.dead, ws.flags, next_bin, started, &ctas, layout, l->stream);
+            ? launch_stream_load<double2>(y, ws.z, init_aff, aff_dst, F, T, D, K, ws.dead, ws.flags, next_bin, started, &ctas, l->stream)
+            : launch_stream_load<float2>(y, ws.z, init_aff, aff_dst, F, T, D, K, ws.dead, ws.flags, next_bin, started, &ctas, l->stream);
     if (r) return r;
     PBB_CUDA(cudaEventRecord(l->join, l->stream));
     // Hold the EM kernel back until every loader CTA runs: launched at the same moment, the EM grid
@@ -829,8 +854,8 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
     }
     if (aff_host) init_aff = ws.aff_stage;
   } else if (persistent)  // chunk-major staged layout: one TMA bulk copy per ring stage
-    r = dtype == PBB_C128 ? launch_normalize_staged<double2>(y, ws.z, F, T, D, ws.dead, layout, st)
-                          : launch_normalize_staged<float2>(y, ws.z, F, T, D, ws.dead, layout, st);
+    r = dtype == PBB_C128 ? launch_normalize_staged<double2>(y, ws.z, F, T, D, ws.dead, st)
+                          : launch_normalize_staged<float2>(y, ws.z, F, T, D, ws.dead, st);
   else
     r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
                           : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
@@ -902,15 +927,16 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
         if ((r = streamed_order(F, opt->iterations, c, cap < 1 ? 1 : cap, &p.order))) return r;
       }
     }
-    bool sticky = false;
-    if (D == 8 && !full && !streamed && em_kernel_choice() == 1) {
-      if ((r = launch_sticky(p, K, dtype, &sticky, st))) return r;  // few bins: one cluster per bin (em_sticky.cuh)
-    }
-    if (!sticky) {
-      if (!(D == 8 && !full && em_kernel_choice() == 0))  // (not in the opt-in em_ls kernel)
-        if ((r = setup_frame_split(&p, ws, F, T, D, K, full ? (D == 8 ? 3 : D == 6 ? 4 : 6) : (D == 4 ? 4 : 2), st)))
-          return r;
-      if ((r = launch_persist(p, D, K, dtype, full, st))) return r;
+    const PlanOverrides ov = env_overrides();
+    int clusters[3] = {0, 0, 0}, sms = 0;
+    if (sticky_eligible(D, !full, streamed, ov) && (r = sticky_clusters(K, dtype, clusters, st))) return r;
+    if ((r = device_sms(&sms))) return r;
+    const FitPlan plan = plan_persistent_fit(F, T, D, K, !full, streamed, sms, clusters, ov);
+    if (plan.kernel == kKernelSticky) {
+      if ((r = launch_sticky(p, K, dtype, plan.split, st))) return r;  // few bins: one cluster per bin (em_sticky.cuh)
+    } else {
+      if ((r = setup_frame_split(&p, ws, F, D, K, plan.split, st))) return r;
+      if ((r = launch_persist(p, D, K, dtype, full, plan.kernel == kKernelWs, st))) return r;
     }
     if (streamed) {
       LoadStream* l = nullptr;
@@ -1080,8 +1106,8 @@ int pbb_cwmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
   const bool persistent = fast_shape(D, K) && saliency == nullptr;
   int r;
   if (persistent)
-    r = dtype == PBB_C128 ? launch_normalize_staged<double2>(y, ws.z, F, T, D, ws.dead, 0, st)
-                          : launch_normalize_staged<float2>(y, ws.z, F, T, D, ws.dead, 0, st);
+    r = dtype == PBB_C128 ? launch_normalize_staged<double2>(y, ws.z, F, T, D, ws.dead, st)
+                          : launch_normalize_staged<float2>(y, ws.z, F, T, D, ws.dead, st);
   else
     r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
                           : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
@@ -1113,7 +1139,12 @@ int pbb_cwmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
     p.coef = ws.coef; p.ld = ws.ld; p.w = ws.w; p.ew = ws.ew;
     p.part = ws.part; p.flags = ws.flags; p.ticket = ws.ticket; p.status = status; p.phase = ws.phase;
     p.spline = u.spline;
-    if ((r = setup_frame_split(&p, ws, F, T, D, K, D == 4 ? 4 : 2, st))) return r;
+    PlanOverrides ov = env_overrides();
+    ov.single = true;
+    int sms = 0;
+    if ((r = device_sms(&sms))) return r;
+    const FitPlan plan = plan_persistent_fit(F, T, D, K, true, false, sms, nullptr, ov);
+    if ((r = setup_frame_split(&p, ws, F, D, K, plan.split, st))) return r;
     if ((r = launch_persist_cw(p, D, K, dtype, st))) return r;
 #ifdef PBB_PHASE_TIMING
     {

@@ -909,23 +909,13 @@ __global__ void normalize_kernel(const CT* __restrict__ y, CT* __restrict__ z, i
   }
 }
 
-// Staged layouts of the persistent kernels (one ring stage = one contiguous block):
-//   layout 0 (em_persistent.cuh / em_ws.cuh): out[f][c][r][i] = z[f][row_channel(D, r)][c * SF + i], rows = stage_rows(D)
-//   layout 1 (em_ls.cuh, D = 8): frame-major, out[f][c][i][d ^ swz(i)] = z[f][d][c * SF + i], rows = D;
-//            swz(i) = i & 7 for complex128, (i >> 1) & 7 for complex64 (one 128-byte line = 1 or 2 frames)
-// Frames >= T are zero.
-template <typename CT>
-__device__ __forceinline__ int staged_index(int layout, int D, int SF, int r, int i) {
-  if (layout == 0) return r * SF + i;
-  const int sw = sizeof(CT) == 8 ? ((i >> 1) & 7) : (i & 7);
-  return i * D + (r ^ sw);
-}
-__device__ __forceinline__ int staged_channel(int layout, int D, int r) { return layout == 0 ? row_channel(D, r) : r; }
+// Staged layout of the persistent kernels (one ring stage = one contiguous block):
+//   out[f][c][r][i] = z[f][row_channel(D, r)][c * SF + i], rows = stage_rows(D); frames >= T are zero.
 
-// Normalisation into a staged layout.  One CTA per (frame tile, bin).
+// Normalisation into the staged layout.  One CTA per (frame tile, bin).
 template <typename CT>
 __global__ void normalize_staged_kernel(const CT* __restrict__ y, CT* __restrict__ z, int F, int T, int D, int rows,
-                                        int SF, int nchunks, int* __restrict__ dead, int layout) {
+                                        int SF, int nchunks, int* __restrict__ dead) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* tile = reinterpret_cast<double2*>(smem_raw);  // [blockDim.x][D + 1]
   const int f = blockIdx.y;
@@ -960,12 +950,12 @@ __global__ void normalize_staged_kernel(const CT* __restrict__ y, CT* __restrict
   const int c = t0 / SF, i0 = t0 - c * SF;
   CT* __restrict__ zc = z + ((size_t)f * nchunks + c) * rows * SF;
   for (int i = threadIdx.x; i < rows * (int)blockDim.x; i += blockDim.x) {
-    // consecutive threads write consecutive addresses in either layout
-    const int r = layout == 0 ? i / (int)blockDim.x : i % rows;
-    const int tt = layout == 0 ? i - r * (int)blockDim.x : i / rows;
+    // consecutive threads write consecutive addresses
+    const int r = i / (int)blockDim.x;
+    const int tt = i - r * (int)blockDim.x;
     double2 v = make_double2(0.0, 0.0);
-    if (tt < nt) v = tile[tt * ldt + staged_channel(layout, D, r)];
-    st_cplx(zc + staged_index<CT>(layout, D, SF, r, i0 + tt), v.x, v.y);
+    if (tt < nt) v = tile[tt * ldt + row_channel(D, r)];
+    st_cplx(zc + r * SF + i0 + tt, v.x, v.y);
   }
 }
 
@@ -986,7 +976,7 @@ __global__ void __launch_bounds__(kLoadThreads, 3)
 stream_load_kernel(const CT* __restrict__ y, CT* __restrict__ z, const double* __restrict__ aff_src,
                    double* __restrict__ aff_dst, int F, int T, int D, int K, int rows, int SF, int nchunks,
                    int* __restrict__ dead, int* __restrict__ flags, int* __restrict__ next_bin,
-                   int* __restrict__ started, int layout) {
+                   int* __restrict__ started) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* tile = reinterpret_cast<double2*>(smem_raw);  // [SF][D + 1]
   __shared__ int s_bin[2];
@@ -1063,12 +1053,16 @@ stream_load_kernel(const CT* __restrict__ y, CT* __restrict__ z, const double* _
       }
       __syncthreads();
       CT* __restrict__ zc = z + ((size_t)f * nchunks + c) * rows * SF;
-      for (int i = tid; i < rows * SF; i += kLoadThreads) {
-        const int r = layout == 0 ? i / SF : i % rows;
-        const int tt = layout == 0 ? i - r * SF : i / rows;
-        double2 x = make_double2(0.0, 0.0);
-        if (tt < nt) x = tile[tt * ldt + staged_channel(layout, D, r)];
-        st_cplx(zc + staged_index<CT>(layout, D, SF, r, tt), x.x, x.y);
+      // (rolled loops: with the next chunk's loads in flight, an unrolled store loop spills at 168 registers)
+#pragma unroll 1
+      for (int r = 0; r < rows; ++r) {
+        const int ch = row_channel(D, r);
+#pragma unroll 1
+        for (int tt = tid; tt < SF; tt += kLoadThreads) {
+          double2 x = make_double2(0.0, 0.0);
+          if (tt < nt) x = tile[tt * ldt + ch];
+          st_cplx(zc + r * SF + tt, x.x, x.y);
+        }
       }
       __syncthreads();
     }

@@ -706,22 +706,11 @@ __device__ __forceinline__ double warp_hpd_inverse(double2* __restrict__ A, int 
 // Model update of one (bin, class) by one warp (cACGMM): scatter sums Sk[0..NS) + sum of gamma
 // Sk[NS] -> E-step coefficients in a.coef (+ the published scalars), see the file header.
 // A, V: D x D shared-memory scratch of the warp; lamk: D doubles.
-// Model block of a bin in the E-phase order of em_ls.cuh (tabE[s] = half << 5 | entry << 1 | part, bit 8 = sign):
-// 2 x (16 K + 1) double2 coefficients followed by ew[4]; one contiguous block = one TMA bulk copy.
-__host__ __device__ constexpr int ls_model_doubles(int K) { return 2 * (2 * (16 * K + 1)) + 4; }
-__device__ __forceinline__ void ls_store_coef(double* __restrict__ blk, const int* __restrict__ tabE, int K, int k,
-                                              int s, double v) {
-  const int te = tabE[s];
-  const int h = (te >> 5) & 1, e = (te >> 1) & 15, part = te & 1;
-  blk[((h * (16 * K + 1) + e * K + k) << 1) + part] = (te & 256) ? -v : v;
-}
-
-template <int D, bool FULL, bool LS = false>
+template <int D, bool FULL>
 __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin, int k, int K, int lane,
                                                   double2* __restrict__ A, double2* __restrict__ V,
                                                   double* __restrict__ lamk, const double* __restrict__ Sk,
                                                   const int* __restrict__ tab, double* __restrict__ ld_out,
-                                                  const int* __restrict__ tabE = nullptr,
                                                   double* __restrict__ coef_out = nullptr) {
   // coef_out: destination of the class's NS slot coefficients instead of a.coef (em_sticky.cuh: shared memory)
   constexpr int NS = D * D;
@@ -782,8 +771,7 @@ __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin,
     // on det B in the reference's lambda_max = 1 scale -- take the eigendecomposition path there.
     const bool no_floor = ok && isfinite(tinv) && (tr * tn * tinv * a.eigenvalue_floor < 0.5) &&
                           dead_bin == 0;
-    double* __restrict__ co = coef_out != nullptr ? coef_out
-                              : LS ? a.coef + (size_t)bin * ls_model_doubles(K) : a.coef + ((size_t)bin * K + k) * NS;
+    double* __restrict__ co = coef_out != nullptr ? coef_out : a.coef + ((size_t)bin * K + k) * NS;
     PBB_PHU(10);  // log det, trace of the inverse, floor test
     if (__any_sync(0xffffffffu, bad)) {
       if (lane == 0) atomicMax(a.status, bin + 1);
@@ -793,9 +781,7 @@ __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin,
         const int pk = tab[s];
         const int d = pk & 255, e = (pk >> 8) & 255, kind = pk >> 16;
         const double2 u = A[d * D + e], v = A[e * D + d];
-        const double cv = kind == 0 ? u.x : (kind == 1 ? (u.x + v.x) : -(u.y - v.y));
-        if constexpr (LS) ls_store_coef(co, tabE, K, k, s, cv);
-        else co[s] = cv;
+        co[s] = kind == 0 ? u.x : (kind == 1 ? (u.x + v.x) : -(u.y - v.y));
       }
     } else {
       // reference semantics: eigendecomposition, normalise, floor (cacg.py:95-126)
@@ -817,15 +803,7 @@ __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin,
         lamk[d] = l;
       }
       __syncwarp();
-      if constexpr (LS) {
-        // the eigenvalues are in lamk, A is free: slot-ordered coefficients there, then the permuted store
-        __syncwarp();
-        ldk = model_from_eig_warp(V, lamk, tab, D, lane, Ad);
-        __syncwarp();
-        for (int s = lane; s < NS; s += 32) ls_store_coef(co, tabE, K, k, s, Ad[s]);
-      } else {
-        ldk = model_from_eig_warp(V, lamk, tab, D, lane, co);
-      }
+      ldk = model_from_eig_warp(V, lamk, tab, D, lane, co);
     }
     if (lane == 0) {
       *ld_out = ldk;
@@ -843,9 +821,14 @@ __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin,
 // arithmetic (the slot-group warps then exchange on named barrier 1) and update class g in the update phase.
 __host__ __device__ constexpr int persist_extra_warps(int D, int K) { return K > D / 2 ? K - D / 2 : 0; }
 __host__ __device__ constexpr int persist_threads(int D, int K) { return 32 * (D / 2 + persist_extra_warps(D, K)); }
+// CTAs per SM of em_persistent_kernel (full variant: one frame per lane; lean: two), which the host's frame split
+// plans with; em_ws_kernel runs the lean D = 8 figure as well
+__host__ __device__ constexpr int persist_ctas_per_sm(int D, bool full) {
+  return full ? (D == 8 ? 3 : (D == 6 ? 4 : 6)) : (D == 4 ? 4 : 2);
+}
 
 template <int D, int K, typename CT, bool FULL, int FPL, int MODEL = 0>
-__global__ void __launch_bounds__(persist_threads(D, K), (FPL == 2 ? (D == 8 ? 2 : (D == 6 ? 2 : 4)) : (D == 8 ? 3 : (D == 6 ? 4 : 6))))
+__global__ void __launch_bounds__(persist_threads(D, K), persist_ctas_per_sm(D, FULL))
 em_persistent_kernel(const PersistArgs a) {
   using SM = PersistSmem<D, K, CT>;
   using G = GroupDims<D>;

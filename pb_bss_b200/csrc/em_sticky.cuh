@@ -22,12 +22,10 @@
 
 namespace pbb {
 
-#ifndef PBB_STICKY_EM_REGS
 // Register budget of the EM warps (the helpers get 256 - this), multiple of 8.  200 / 56 instead of em_ws_kernel's
 // 208 / 48: the update warps spill less, and a spill reload behind a cluster barrier (which invalidates the L1) is
-// an L2 round trip.  scripts/sticky_regs_ab.py times the two splits against each other.
-#define PBB_STICKY_EM_REGS 200
-#endif
+// an L2 round trip.
+constexpr int kStickyEmRegs = 200;
 
 __device__ __forceinline__ void sticky_cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -70,7 +68,7 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
 
   if (warp < M) {
     // =============================== EM warps ===============================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(PBB_STICKY_EM_REGS));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kStickyEmRegs));
     const int g = warp;
     int buf = 0;
 #pragma unroll 1
@@ -154,7 +152,7 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
       }
     }
   } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(256 - PBB_STICKY_EM_REGS));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(256 - kStickyEmRegs));
     const int u = warp - M - 1;  // updater index (warp M only keeps the barriers company)
 #pragma unroll 1
     for (int it = 0; it < a.iterations; ++it) {
@@ -188,7 +186,7 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
             // the class model goes to a staging row in this CTA's shared memory, then into every CTA's model buffer
             // through DSMEM: no L2 round trip between the update and the next sweep
             cacg_update_class<D, false>(a, bin, k, K, lane, sm.A[k], sm.V[k], sm.lam[k], sm.S[1][k], sm.tab, &sm.ld[k],
-                                        nullptr, &sm.coef[1][k][0]);
+                                        &sm.coef[1][k][0]);
             __syncwarp();
             const double c0v = sm.coef[1][k][lane], c1v = sm.coef[1][k][lane + 32];
             const double ldk = sm.ld[k], sgam = sm.S[1][k][NS];

@@ -31,19 +31,10 @@
 
 namespace pbb {
 
-// Posterior once per frame instead of once per slot group (lean_chunk2_split): -3 % on C2.
-#ifndef PBB_NO_SOFTMAX_SPLIT
-#define PBB_SOFTMAX_SPLIT 1
-#endif
-#ifndef PBB_WS_LEAD
-#define PBB_WS_LEAD 2  // chunks the EM warps have left when the producer takes the next ticket
-#endif
+constexpr int kWsLead = 2;  // chunks the EM warps have left when the producer takes the next ticket
 constexpr int kWsStages = 3;
-#ifndef PBB_WS_EM_REGS
-#define PBB_WS_EM_REGS 208
-#endif
-constexpr int kWsEmRegs = PBB_WS_EM_REGS;  // 128 threads x 208 + 128 threads x 48 = 32768 = 256 x 128
-constexpr int kWsHelperRegs = 256 - PBB_WS_EM_REGS;
+constexpr int kWsEmRegs = 208;  // 128 threads x 208 + 128 threads x 48 = 32768 = 256 x 128
+constexpr int kWsHelperRegs = 256 - kWsEmRegs;
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -78,8 +69,8 @@ struct WsSmem {
   double2 V[K][NS];       // updaters: eigenvectors (Jacobi fallback)
   double coef[2][K][NS];  // model of the current / next task (producer writes, EM reads)
   double xq[2][M][2 * K][32];
-  double cwx[K][64];       // PBB_SOFTMAX_SPLIT: gamma / q per (class, frame of the step)
-  double sgp[2][M][K];     // PBB_SOFTMAX_SPLIT: sum of gamma per slot-group warp
+  double cwx[K][64];       // gamma / q per (class, frame of the step)
+  double sgp[2][M][K];     // sum of gamma per slot-group warp
   double S[2][K][NS + 1];  // scatter sums of the last / second last task (EM writes, updaters read)
   double lam[K][D];
   double ld[K];
@@ -163,7 +154,7 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
         const int t_chunk = c * kStageFrames;
         const int nsteps = (min(kStageFrames, zs - t_chunk)) >> 5;
         if (!mstep_only) {
-#ifdef PBB_SOFTMAX_SPLIT
+          // posterior once per frame instead of once per slot group (lean_chunk2_split): -3 % on C2
           lean_chunk2_split<D, K, CT>(sm, mb, g, st, nsteps >> 1, lane, a.aff_eps, acc, sg);
           if (nsteps & 1) {
             // odd tail step: every group evaluates all 32 frames; only group 0 counts them
@@ -175,10 +166,6 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
 #pragma unroll
             for (int k = 0; k < K; ++k) sg[k] += g == 0 ? sgt[k] : 0.0;
           }
-#else
-          lean_chunk2<D, K, CT, MODEL, true>(sm, mb, g, st, nsteps >> 1, lane, buf, a.aff_eps, acc, sg);
-          if (nsteps & 1) lean_chunk<D, K, CT, MODEL, true>(sm, mb, g, st, 1, lane, buf, a.aff_eps, acc, sg, nsteps - 1);
-#endif
         } else {
           general_chunk<D, K, CT, false>(a, sm, g, bin, st, t_chunk, nsteps, lane, buf, true, true, acc, sg);
         }
@@ -193,21 +180,15 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
 #pragma unroll
         for (int k = 0; k < K; ++k) q1[k] = 0.0;
         softmax_product<D, K>(q1, sm.ew[mb], a.aff_eps, gp, cp);
-#ifdef PBB_SOFTMAX_SPLIT
         // every padded frame was counted once, by whichever warp evaluated it: take them out in one place
         const int npad_lane = (g == 0 && lane >= 32 - (zs - T)) ? 1 : 0;
-#else
-        const int npad_lane = (lane >= 32 - (zs - T)) ? 1 : 0;
-#endif
 #pragma unroll
         for (int k = 0; k < K; ++k) sg[k] -= npad_lane ? gp[k] : 0.0;
       }
-#ifdef PBB_SOFTMAX_SPLIT
       if (mstep_only && g != 0) {  // the M-step-only pass counts gamma in every group: keep group 0's
 #pragma unroll
         for (int k = 0; k < K; ++k) sg[k] = 0.0;
       }
-#endif
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.model_empty[mb]);  // done with this task's model
 
@@ -232,11 +213,7 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
 #pragma unroll
       for (int k = 0; k < K; ++k) {
         const double v = warp_sum(sg[k]);
-#ifdef PBB_SOFTMAX_SPLIT
         if (lane == 0) sm.sgp[sb][g][k] = v;
-#else
-        if (g == 0 && lane == 0) sm.S[sb][k][NS] = v;
-#endif
       }
       if (g == 0 && lane == 0) { sm.sdesc[sb][0] = bin; sm.sdesc[sb][1] = it; sm.sdesc[sb][2] = part; }
       __syncwarp();
@@ -338,7 +315,7 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
           // Do not take the next ticket too early: with two tickets per CTA in flight the grid holds
           // more tasks than there are bins and most dependencies are still executing.  Wait until the
           // EM warps have ~2 chunks left (enough to hide ticket, flag and model latency).
-          const unsigned x = chunk_cnt - (unsigned)(ncp >= PBB_WS_LEAD + 1 ? PBB_WS_LEAD + 1 : ncp);
+          const unsigned x = chunk_cnt - (unsigned)(ncp >= kWsLead + 1 ? kWsLead + 1 : ncp);
           mbar_wait_relaxed(&sm.empty[x % kWsStages], (x / kWsStages) & 1u, 100);
         }
         __syncwarp();
@@ -359,14 +336,12 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
         const int bin = sm.sdesc[sb][0], it = sm.sdesc[sb][1];
         if (bin < 0) break;
         const bool last_it = it == a.iterations - 1;
-#ifdef PBB_SOFTMAX_SPLIT
         // sum of gamma = the four groups' shares, added in a fixed order
         for (int k = u; k < K; k += NU)
           if (lane == 0)
             sm.S[sb][k][NS] = (sm.sgp[sb][0][k] + sm.sgp[sb][1][k]) + (sm.sgp[sb][2][k] + sm.sgp[sb][3][k]);
         __syncwarp();
         if (last_it && S == 1) asm volatile("bar.sync 2, %0;" ::"n"(NU * 32) : "memory");
-#endif
         if (S > 1) {
           // frame split: leave this part's sums in L2; whoever delivers the last part adds them up in a fixed order
           const int part = sm.sdesc[sb][2];
