@@ -557,6 +557,122 @@ int pbb_apply_online_beamforming_vector(const void* vector, const void* mix,
                                         void* stream);
 
 /* ------------------------------------------------------------------------
+ * Oracle masks (pb_bss/extraction/mask_module.py) and array geometry
+ * (pb_bss/extraction/beamform_utils.py), csrc/api_mask.cu.
+ *
+ * The masks read the signal in its own layout: a pbb_mask_layout describes an
+ * index space (row-major over `shape`) and, for every dim, the stride of the
+ * input (in elements of the input dtype, complex elements counted once) and of
+ * the output.  Inputs may be complex or real (dtype PBB_C64 / PBB_C128 /
+ * PBB_F32 / PBB_F64); the arithmetic is fp64, and |s|^2 is re*re + im*im
+ * rounded like NumPy (no FMA).  Real-valued masks are stored as float for the
+ * 32-bit dtypes and double otherwise.
+ */
+#define PBB_F32 2
+#define PBB_F64 3
+#define PBB_MASK_MAX_DIMS 8
+
+typedef struct pbb_mask_layout {
+  int nd; /* 0 <= nd <= PBB_MASK_MAX_DIMS; nd = 0 is a single index */
+  int reserved;
+  long long shape[PBB_MASK_MAX_DIMS];
+  long long in_stride[PBB_MASK_MAX_DIMS];
+  long long out_stride[PBB_MASK_MAX_DIMS];
+} pbb_mask_layout;
+
+/* Source-reduction masks; kind: */
+enum {
+  PBB_MASK_IDEAL_BINARY = 0,    /* ideal_binary_mask (mask_module.py:90-136): 1 at the first argmax */
+  PBB_MASK_WIENER_LIKE = 1,     /* wiener_like_mask (:139-179): p / (sum_k p + eps) */
+  PBB_MASK_IDEAL_RATIO = 2,     /* ideal_ratio_mask (:182-232): |s| / (sum_k |s| + eps) */
+  PBB_MASK_IDEAL_AMPLITUDE = 3, /* ideal_amplitude_mask (:235-287): |s| / (|sum_k s| + eps) */
+  PBB_MASK_PHASE_SENSITIVE = 4, /* phase_sensitive_mask (:290-322): |s| / (|o| + eps) cos(angle s - angle o) */
+  PBB_MASK_IDEAL_COMPLEX = 5    /* ideal_complex_mask (:325-347): s / o, NumPy's complex division, no eps */
+};
+/* For every index r of `rest` (the dims other than the source and sensor axes)
+ * and source k: p = sum over the D sensors (channel order; D = 1 without
+ * sensor pooling, which only kinds 0 and 1 allow) of |s|^2 at
+ * signal + rest.in(r) + k source_stride + d sensor_stride, o = sum_k s.  The
+ * mask goes to out + rest.out(r) + k out_source_stride; kind 5 stores the
+ * input's element type, the others a real of its precision. */
+int pbb_source_mask(const void* signal, int dtype, int kind, int K, int D,
+                    long long source_stride, long long sensor_stride,
+                    long long out_source_stride, const pbb_mask_layout* rest,
+                    double eps, void* out, void* stream);
+
+/* Rows of at most this many elements are selected by one warp in shared
+ * memory, several rows per CTA (read in tiles of consecutive rows, so that a
+ * row stride of 1 -- the frequency axis of an (F, T) STFT -- coalesces);
+ * longer rows are spread over several CTAs per row with histograms in global
+ * memory and a pass kernel per digit (scratch: pbb_row_select_scratch_bytes). */
+#define PBB_ROW_SELECT_SHORT_MAX 4096
+size_t pbb_row_select_scratch_bytes(long long rows, long long n);
+
+/* lorenz_mask (mask_module.py:350-417): each row (index space `rows`, elements
+ * `elems`, n = product of elems.shape) holds p = sum over the D sensors of
+ * |s|^2 (sensor_stride between them).  The threshold is the smallest of the
+ * descending-sorted values whose Lorenz value cumsum / sum is < lorenz_fraction,
+ * found by a radix select over the bit patterns of the non-negative doubles
+ * (8 digits of 8 bits) that carries per-bucket counts, sums and maxima; the
+ * mask stores mask_high where p > threshold, else mask_low.  A row where no
+ * value qualifies (np.min of an empty array) sets *status = 1 + its index
+ * (the first such row).  Bucket sums are accumulated with atomics, so a
+ * Lorenz value within a few ulp of lorenz_fraction may round either way. */
+int pbb_lorenz_mask(const void* signal, int dtype, int D, long long sensor_stride,
+                    const pbb_mask_layout* rows, const pbb_mask_layout* elems,
+                    double lorenz_fraction, double mask_low, double mask_high,
+                    void* out, void* scratch, size_t scratch_bytes, int* status,
+                    void* stream);
+
+/* quantile_mask (mask_module.py:420-493) for one quantile: x = |s| of every row
+ * (rounded to float for the 32-bit dtypes, as np.abs does), the order
+ * statistics k_lower and k_upper (0-based, ascending) selected exactly, and
+ * np.percentile's linear interpolation (numpy _lerp) evaluated in the input
+ * precision: x_lo + (x_hi - x_lo) gamma, or x_hi - (x_hi - x_lo) one_minus_gamma
+ * when gamma >= 0.5.  The caller computes k_lower, k_upper, gamma and
+ * one_minus_gamma as NumPy does.  mask_high where x > threshold (below = 0) or
+ * x < threshold (below = 1), else mask_low. */
+int pbb_quantile_mask(const void* signal, int dtype, const pbb_mask_layout* rows,
+                      const pbb_mask_layout* elems, long long k_lower,
+                      long long k_upper, double gamma, double one_minus_gamma,
+                      int below, double mask_low, double mask_high, void* out,
+                      void* scratch, size_t scratch_bytes, void* stream);
+
+/* biased_binary_mask (mask_module.py:496-550) with components = 2: for every
+ * index r of `rest` (signal without the component axis), p0 / p1 = |s|^2 of
+ * component 0 / 1 (component_stride apart) and j = r mod L (the last axis):
+ * speech = p0 / speech_div[j] > p1 and > 0.005, noise = p0 / noise_div[j] < p1
+ * or < 0.005; force[j] != 0 sets speech = 0, noise = 1.  out (uint8 / bool) gets
+ * speech at rest.out(r) and noise at rest.out(r) + out_component_stride.
+ * speech_div, noise_div (L doubles) and force (L bytes) are device arrays. */
+int pbb_biased_binary_mask(const void* signal, int dtype, long long component_stride,
+                           long long out_component_stride, const pbb_mask_layout* rest,
+                           int L, const double* speech_div, const double* noise_div,
+                           const unsigned char* force, void* out, void* stream);
+
+/* get_steering_vector (beamform_utils.py:36-63): out[a][m][f] (A, M, F)
+ * complex128 = exp(-2j pi freq[f] tdoa[a][m]) with NumPy's operation order;
+ * normalize != 0 divides by the 2-norm over m (the reference's axis -2). */
+int pbb_steering_vector(const double* tdoa, int A, int M, const double* freq, int F,
+                        int normalize, void* out, void* stream);
+
+/* get_diffuse_noise_psd (beamform_utils.py:66-97): out (F, D, D) float64 =
+ * np.sinc(2 freq[f] distances[d][e] / sound_velocity), sinc(0) = 1. */
+int pbb_diffuse_noise_coherence(const double* distances, int D, const double* freq,
+                                int F, double sound_velocity, double* out,
+                                void* stream);
+
+/* get_nearfield_time_of_flight (beamform_utils.py:100-116): out[s][m] (S, M) =
+ * |source[:, s] - sensor[:, m]| / sound_velocity; source (3, S), sensor (3, M).
+ * get_farfield_time_difference_of_arrival (:119-159): out[m][k] (M, K) =
+ * (sensor[:, m] - sensor[:, reference_channel]) . u_k / sound_velocity with u_k
+ * = -(rotate_y(elevation) rotate_z(azimuth))[:, 0]; angles (2, K).  One kernel
+ * serves both (mode 0 = near field, 1 = far field; `points` is source or angles). */
+int pbb_array_geometry(int mode, const double* points, int S, const double* sensor,
+                       int M, int reference_channel, double sound_velocity,
+                       double* out, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

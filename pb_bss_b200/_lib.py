@@ -29,7 +29,26 @@ class CacgmmOptions(ctypes.Structure):
     ]
 
 
+PBB_F32, PBB_F64 = 2, 3
+MASK_MAX_DIMS = 8
+MASK_IDEAL_BINARY, MASK_WIENER_LIKE, MASK_IDEAL_RATIO, MASK_IDEAL_AMPLITUDE, MASK_PHASE_SENSITIVE, \
+    MASK_IDEAL_COMPLEX = range(6)
+ROW_SELECT_SHORT_MAX = 4096  # PBB_ROW_SELECT_SHORT_MAX
+
+
+class MaskLayout(ctypes.Structure):
+    """struct pbb_mask_layout (include/pbb.h)."""
+    _fields_ = [
+        ('nd', ctypes.c_int),
+        ('reserved', ctypes.c_int),
+        ('shape', ctypes.c_longlong * MASK_MAX_DIMS),
+        ('in_stride', ctypes.c_longlong * MASK_MAX_DIMS),
+        ('out_stride', ctypes.c_longlong * MASK_MAX_DIMS),
+    ]
+
+
 _vp, _i, _d, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_size_t
+_ll, _lay = ctypes.c_longlong, ctypes.POINTER(MaskLayout)
 
 # name -> (restype, argtypes); mirrors include/pbb.h one to one
 SIGNATURES = {
@@ -109,6 +128,14 @@ SIGNATURES = {
     'pbb_phase_correction': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     'pbb_apply_online_beamforming_vector': (_i, [_vp, _vp, _i, _i, _i, _i, _i, ctypes.c_longlong, ctypes.c_longlong,
                                                  ctypes.c_longlong, ctypes.c_longlong, _vp, _vp]),
+    'pbb_source_mask': (_i, [_vp, _i, _i, _i, _i, _ll, _ll, _ll, _lay, _d, _vp, _vp]),
+    'pbb_row_select_scratch_bytes': (_sz, [_ll, _ll]),
+    'pbb_lorenz_mask': (_i, [_vp, _i, _i, _ll, _lay, _lay, _d, _d, _d, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_quantile_mask': (_i, [_vp, _i, _lay, _lay, _ll, _ll, _d, _d, _i, _d, _d, _vp, _vp, _sz, _vp]),
+    'pbb_biased_binary_mask': (_i, [_vp, _i, _ll, _ll, _lay, _i, _vp, _vp, _vp, _vp, _vp]),
+    'pbb_steering_vector': (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
+    'pbb_diffuse_noise_coherence': (_i, [_vp, _i, _vp, _i, _d, _vp, _vp]),
+    'pbb_array_geometry': (_i, [_i, _vp, _i, _vp, _i, _i, _d, _vp, _vp]),
 }
 
 _lib = None

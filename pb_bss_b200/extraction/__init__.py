@@ -22,3 +22,17 @@ from .beamformer import (  # noqa: F401
     zero_degree_normalization,
 )
 from .beamformer_wrapper import get_bf_vector  # noqa: F401
+from .beamformer_wrapper import get_bf_vector as get_single_source_bf_vector  # noqa: F401
+from . import mask_module  # noqa: F401
+from .mask_module import (  # noqa: F401
+    biased_binary_mask,
+    ideal_amplitude_mask,
+    ideal_binary_mask,
+    ideal_complex_mask,
+    ideal_ratio_mask,
+    lorenz_mask,
+    phase_sensitive_mask,
+    quantile_mask,
+    voiced_unvoiced_split_characteristic,
+    wiener_like_mask,
+)
