@@ -692,7 +692,10 @@ int pbb_dhtv_mapping(const double* mask, int K, int F, int T, const int* plan,
  * distance); algorithm 0 = 'greedy', 1 = 'optimal' (brute force over the K! permutations).  The whole plan runs in
  * one launch: a single thread-block cluster that keeps a segment's feature rows in distributed shared memory when the
  * widest segment fits (<= 16 bins per CTA of a 16- or 8-CTA cluster and <= 200 KB; the reference's plans do), else one
- * cooperative launch with grid-wide barriers.  The integer mapping is the same on both. */
+ * cooperative launch with grid-wide barriers.  The two add the centroid in different orders, so the integer mapping
+ * is the same on both wherever no decision lies within rounding of a tie, and on exact ties (first maximum in
+ * row-major order); tests/test_permutation_gpu.py::test_dhtv_every_kernel_matches_the_oracle checks both against the
+ * reference.  K * T * 8 bytes must not exceed 200 KB (the centroid lives in shared memory). */
 int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan,
                         int nplan, double* features, double* centroid,
                         long long* mapping, int metric, int algorithm, void* stream);

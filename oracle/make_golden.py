@@ -261,6 +261,108 @@ def make_permutation_greedy_oracle(ref):
     np.savez_compressed(os.path.join(OUT, 'permutation_greedy_oracle.npz'), **out)
 
 
+METRICS = ('cos', 'multiply', 'euclidean')
+
+
+def permutation_classes_cases():
+    """The DHTV cases of tests/golden/permutation_classes.npz: name -> (mask, plan).
+
+    k{K}: well-separated permuted masks, K = 2..9, F = 33 with a small plan of the reference's shape (widest segment
+    13 bins).  k{K}s: the same for the brute-force 'optimal' at K = 8, 9, a few bins.  tie_*: exact ties that do not
+    depend on rounding (T a multiple of 8, so every row of a numpy operand has the same alignment): two classes equal
+    in every bin (a 2x2 block of equal scores), bins that are zero in every class, a constant mask (every score ties:
+    the first iteration changes nothing).  plan_edge: a plan with a 0-iteration segment and 1-bin segments."""
+    def plan_of(stft_size, start, width, shift, main, sub):
+        from .pb_bss_oracle import dhtv_alignment_plan
+        return dhtv_alignment_plan(stft_size, start, width, shift, main, sub)
+
+    cases = {}
+    k_plan = plan_of(64, 8, 12, 4, 6, 2)
+    for K, T in ((2, 80), (3, 72), (4, 64), (5, 56), (6, 50), (7, 46), (8, 42), (9, 40)):
+        cases[f'k{K}'] = (synth.permuted_mask(K, 33, T, seed=40 + K)[0], k_plan)
+    cases['k8s'] = (synth.permuted_mask(8, 5, 24, seed=58)[0], [[3, 0, 5]])
+    cases['k9s'] = (synth.permuted_mask(9, 3, 24, seed=59)[0], [[2, 0, 3]])
+    tie_plan = plan_of(32, 4, 8, 4, 4, 2)
+    for K in (3, 9):
+        rng = np.random.RandomState(70 + K)
+        # a pair of equal classes p, p + 1; the other classes are shuffled among the other positions in every bin, so
+        # the centroid's rows p and p + 1 stay equal as well
+        clean = synth.permuted_mask(K, 17, 32, seed=60 + K)[1]
+        p = K // 2
+        clean[p + 1] = clean[p]
+        others = [k for k in range(K) if k not in (p, p + 1)]
+        mask = clean.copy()
+        for f in range(17):
+            mask[others, f] = clean[rng.permutation(others), f]
+        cases[f'tie_pair_k{K}'] = (mask, tie_plan)
+        mask = synth.permuted_mask(K, 17, 32, seed=80 + K)[0]
+        mask[:, [2, 7, 8, 15]] = 0.0
+        cases[f'tie_zero_k{K}'] = (mask, tie_plan)
+        cases[f'tie_const_k{K}'] = (np.full((K, 17, 64), 0.5), tie_plan)
+    cases['plan_edge'] = (synth.permuted_mask(4, 33, 40, seed=90)[0],
+                          [[3, 0, 20], [0, 5, 25], [2, 20, 21], [2, 10, 33], [1, 32, 33]])
+    return cases
+
+
+def permutation_classes_combos(name, K):
+    """(metric, algorithm) pairs the fixture holds for a DHTV case: 'optimal' only where the brute force of the
+    reference stays affordable (K <= 7, or the few-bin k8s / k9s cases).  plan_edge is scored by 'multiply' only: in
+    a 1-bin segment the centroid is the bin itself, so the cos diagonal ties within rounding and the euclidean one
+    exactly."""
+    algorithms = ('greedy', 'optimal') if K <= 7 or name in ('k8s', 'k9s') else ('greedy',)
+    metrics = ('multiply',) if name == 'plan_edge' else METRICS
+    return [(m, a) for m in metrics for a in algorithms]
+
+
+def make_permutation_classes(ref):
+    """DHTV, Greedy and Oracle permutation alignment for K = 2..9, exact ties and degenerate plans
+    (permutation_alignment.py:133-786) -> tests/golden/permutation_classes.npz."""
+    pa = ref.permutation_alignment
+
+    class PlanAligner(pa.DHTVPermutationAlignment):
+        """The reference's DHTV alignment with a given plan in place of the one derived from the segment settings."""
+        def __init__(self, plan, **kw):
+            super().__init__(stft_size=0, segment_start=0, segment_width=0, segment_shift=1, main_iterations=0,
+                             sub_iterations=0, **kw)
+            self.plan = plan
+
+        @property
+        def alignment_plan(self):
+            return [list(p) for p in self.plan]
+
+    out = {}
+    cases = permutation_classes_cases()
+    out['dhtv_cases'] = np.array(sorted(cases))
+    for name, (mask, plan) in cases.items():
+        out[f'{name}_mask'] = mask
+        out[f'{name}_plan'] = np.asarray(plan, dtype=np.int64)
+        for metric, algorithm in permutation_classes_combos(name, mask.shape[0]):
+            al = PlanAligner(plan, similarity_metric=metric, algorithm=algorithm)
+            out[f'{name}_{metric}_{algorithm}'] = al.calculate_mapping(mask.copy())
+    # Greedy / Oracle alignment: the k{K} masks (Oracle against the unshuffled masks; 'optimal' for K <= 7) and
+    # K-class noise against an independent reference (few bins, odd T)
+    for K in range(2, 10):
+        mask, clean, perm = synth.permuted_mask(K, 33, cases[f'k{K}'][0].shape[2], seed=40 + K)
+        # the reference mask of the Oracle alignment is the unshuffled one: mask[argsort(perm, 0), range(F)]
+        out[f'k{K}_perm'] = perm.astype(np.int8)
+        rng = np.random.RandomState(100 + K)
+        F = 9 if K <= 7 else 3
+        noise = rng.uniform(size=(K, F, 21))
+        out[f'noise_k{K}_mask'] = noise / noise.sum(0, keepdims=True)
+        out[f'noise_k{K}_reference'] = rng.uniform(size=(K, F, 21))
+        for metric in METRICS:
+            out[f'k{K}_greedy_{metric}'] = pa.GreedyPermutationAlignment(metric).calculate_mapping(mask)
+            out[f'noise_k{K}_greedy_{metric}'] = pa.GreedyPermutationAlignment(metric).calculate_mapping(
+                out[f'noise_k{K}_mask'])
+            for alg in ('greedy', 'optimal'):
+                al = pa.OraclePermutationAlignment(metric, alg)
+                if alg == 'greedy' or K <= 7:
+                    out[f'k{K}_oracle_{metric}_{alg}'] = al.calculate_mapping(mask, clean)
+                out[f'noise_k{K}_oracle_{metric}_{alg}'] = al.calculate_mapping(out[f'noise_k{K}_mask'],
+                                                                               out[f'noise_k{K}_reference'])
+    np.savez_compressed(os.path.join(OUT, 'permutation_classes.npz'), **out)
+
+
 def make_beamformer(ref):
     bf = ref.beamformer
     F, D, T, K = 9, 6, 80, 3
@@ -412,6 +514,9 @@ def main():
     if len(sys.argv) > 1 and sys.argv[1] == 'permutation':
         make_permutation(ref)
         return
+    if len(sys.argv) > 1 and sys.argv[1] == 'permutation_classes':
+        make_permutation_classes(ref)
+        return
     if len(sys.argv) > 1 and sys.argv[1] == 'gcacgmm':
         make_gcacgmm(ref)
         return
@@ -426,6 +531,7 @@ def main():
     make_cwmm_coupled(ref)
     make_permutation(ref)
     make_permutation_greedy_oracle(ref)
+    make_permutation_classes(ref)
     make_beamformer(ref)
     make_bf_wrapper(ref)
     make_initializer(ref)

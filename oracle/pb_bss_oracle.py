@@ -393,21 +393,36 @@ def dhtv_plan_from_stft_size(stft_size):
     return dhtv_alignment_plan(stft_size, start, 100, 20, 20, 2)
 
 
-def greedy_mapping_from_score_matrix(score):
+def greedy_mapping_from_score_matrix(score, return_margin=False):
     """score (K, K) [reference, mask] -> reverse permutation (K,).
 
     pb_bss/permutation_alignment.py:525-553: K times take the first argmax of
     the row-major flattened matrix, then blank its row and column.
+
+    return_margin: also return the smallest gap, over the K rounds, between the
+    chosen entry and the largest entry still in play in its row or column (inf
+    if there was none).  0 means an exact tie decided by the scan order.  Only
+    these runner-ups matter: if a near-equal entry in another row and column
+    were taken first, the chosen one would still be taken next (greedy matching
+    is fixed by the order of entries that share a row or column).
     """
     score = np.array(score, dtype=np.float64)
     K = score.shape[-1]
     out = np.zeros(K, dtype=np.int64)
+    margin = np.inf
     for _ in range(K):
-        i, j = np.unravel_index(np.argmax(score.reshape(-1)), score.shape)
+        flat = score.reshape(-1)
+        n = np.argmax(flat)
+        i, j = np.unravel_index(n, score.shape)
+        if return_margin:
+            rest = np.concatenate([np.delete(score[i], j), np.delete(score[:, j], i)])
+            rest = rest[rest > -np.inf]
+            if rest.size:
+                margin = min(margin, score[i, j] - rest.max())
         score[i, :] = -np.inf
         score[:, j] = -np.inf
         out[i] = j
-    return out
+    return (out, margin) if return_margin else out
 
 
 def _vector_norm(a):
@@ -416,29 +431,50 @@ def _vector_norm(a):
     return a / np.maximum(n, np.finfo(n.dtype).tiny)
 
 
-def dhtv_calculate_mapping(mask, plan):
+def _relative_margin(gap, score):
+    """A decision margin in units of the largest |score| of its matrix."""
+    scale = np.max(np.abs(score))
+    if scale > 0:
+        return gap / scale
+    return np.inf if gap > 0 else 0.0
+
+
+def dhtv_calculate_mapping(mask, plan, similarity_metric='cos', algorithm='greedy', return_margin=False):
     """mask (K, F, T) -> mapping (K, F) int.
 
-    pb_bss/permutation_alignment.py:295-355 with similarity 'cos'
-    (score = einsum('K...T,k...T->...kK'), :404-410) and the greedy assignment.
+    pb_bss/permutation_alignment.py:295-355.  For 'cos' the features and the
+    centroid are L2-normalised over time and scored by the inner product
+    (_ScoreMatrix.multiply, :158-162); 'multiply' and 'euclidean' score the raw
+    masks.  The assignment is _mapping_from_score_matrix(algorithm).
+
+    return_margin: also return the smallest decision margin of every
+    assignment made (see greedy_ / optimal_mapping_from_score_matrix), relative
+    to the largest |score| of its bin's score matrix.
     """
     K, F, _ = mask.shape
-    features = _vector_norm(mask)
+    cos = similarity_metric == 'cos'
+    metric = 'multiply' if cos else similarity_metric
+    assign = {'greedy': greedy_mapping_from_score_matrix, 'optimal': optimal_mapping_from_score_matrix}[algorithm]
+    features = _vector_norm(mask) if cos else np.array(mask, dtype=np.float64)
     mapping = np.repeat(np.arange(K)[:, None], F, axis=1)
+    margin = np.inf
     for iterations, start, end in plan:
         for _ in range(iterations):
-            centroid = _vector_norm(np.mean(features[:, start:end, :], axis=1))
+            centroid = np.mean(features[:, start:end, :], axis=1)
+            if cos:
+                centroid = _vector_norm(centroid)
             nothing_changed = True
             for f in range(start, end):
-                score = np.einsum('KT,kT->kK', features[:, f, :], centroid)
-                perm = greedy_mapping_from_score_matrix(score)
+                score = score_matrix(features[:, f:f + 1, :], centroid[:, None, :], metric)[0]
+                perm, gap = assign(score, return_margin=True)
+                margin = min(margin, _relative_margin(gap, score))
                 if not (perm == np.arange(K)).all():
                     nothing_changed = False
                     features[:, f, :] = features[perm, f, :]
                     mapping[:, f] = mapping[perm, f]
             if nothing_changed:
                 break
-    return mapping
+    return (mapping, margin) if return_margin else mapping
 
 
 def score_matrix(mask, reference_mask, similarity_metric):
@@ -453,40 +489,71 @@ def score_matrix(mask, reference_mask, similarity_metric):
     raise ValueError(similarity_metric)
 
 
-def optimal_mapping_from_score_matrix(score):
-    """score (K, K) -> first best of itertools.permutations (pb_bss/permutation_alignment.py:556-585)."""
-    import itertools
+_PERMUTATIONS = {}
+
+
+def _permutations(K):
+    """itertools.permutations(range(K)) as a (K!, K) index array, in that order."""
+    if K not in _PERMUTATIONS:
+        import itertools
+        _PERMUTATIONS[K] = np.array(list(itertools.permutations(range(K))), dtype=np.intp).reshape(-1, K)
+    return _PERMUTATIONS[K]
+
+
+def optimal_mapping_from_score_matrix(score, return_margin=False):
+    """score (K, K) -> first best of itertools.permutations (pb_bss/permutation_alignment.py:556-585).
+
+    Every permutation's score is summed left to right, one class at a time, as
+    the reference's sum() does; np.argmax returns the first maximum, which is
+    the reference's strict '>'.  return_margin: also return the gap between the
+    best and the second-best permutation sum (inf for K = 1).
+    """
+    score = np.asarray(score)
     K = score.shape[-1]
-    best, best_perm = float('-inf'), None
-    for perm in itertools.permutations(range(K)):
-        s = sum(score[range(K), perm])
-        if s > best:
-            best, best_perm = s, perm
-    return np.asarray(best_perm, dtype=np.int64)
+    perms = _permutations(K)
+    sums = score[0, perms[:, 0]]
+    for k in range(1, K):
+        sums = sums + score[k, perms[:, k]]
+    best = int(np.argmax(sums))
+    out = perms[best].astype(np.int64)
+    if not return_margin:
+        return out
+    margin = np.inf if len(sums) == 1 else float(sums[best] - np.delete(sums, best).max())
+    return out, margin
 
 
-def mapping_from_score_matrix(scores, algorithm):
-    """scores (F, K, K) -> mapping (K, F), pb_bss/permutation_alignment.py:458-590."""
+def mapping_from_score_matrix(scores, algorithm, return_margin=False):
+    """scores (F, K, K) -> mapping (K, F), pb_bss/permutation_alignment.py:458-590.
+
+    return_margin: also return the smallest decision margin over the bins,
+    each relative to the largest |score| of its bin."""
     if not np.all(np.isfinite(scores)):
         raise ValueError('score matrix is infeasible')
     fn = {'greedy': greedy_mapping_from_score_matrix, 'optimal': optimal_mapping_from_score_matrix}[algorithm]
-    return np.stack([fn(sc) for sc in scores], axis=1)
+    res = [fn(sc, return_margin=True) for sc in scores]
+    mapping = np.stack([r[0] for r in res], axis=1) if res else np.zeros((scores.shape[-1], 0), np.int64)
+    if not return_margin:
+        return mapping
+    return mapping, min((_relative_margin(r[1], sc) for r, sc in zip(res, scores)), default=np.inf)
 
 
-def greedy_permutation_alignment(mask, similarity_metric='euclidean'):
+def greedy_permutation_alignment(mask, similarity_metric='euclidean', return_margin=False):
     """GreedyPermutationAlignment.calculate_mapping, pb_bss/permutation_alignment.py:612-714
     (the pairwise assignment is always 'greedy', :703)."""
     K, F, _ = mask.shape
-    pair = mapping_from_score_matrix(score_matrix(mask[:, 1:], mask[:, :-1], similarity_metric), 'greedy')
+    pair, margin = mapping_from_score_matrix(score_matrix(mask[:, 1:], mask[:, :-1], similarity_metric), 'greedy',
+                                             return_margin=True)
     mapping = np.concatenate([np.arange(K)[:, None], pair], axis=1)
     for f in range(1, F):
         mapping[:, f] = mapping[mapping[:, f - 1], f]
-    return mapping
+    return (mapping, margin) if return_margin else mapping
 
 
-def oracle_permutation_alignment(mask, reference_mask, similarity_metric='euclidean', algorithm='optimal'):
+def oracle_permutation_alignment(mask, reference_mask, similarity_metric='euclidean', algorithm='optimal',
+                                 return_margin=False):
     """OraclePermutationAlignment.calculate_mapping, pb_bss/permutation_alignment.py:723-786."""
-    return mapping_from_score_matrix(score_matrix(mask, reference_mask, similarity_metric), algorithm)
+    return mapping_from_score_matrix(score_matrix(mask, reference_mask, similarity_metric), algorithm,
+                                     return_margin=return_margin)
 
 
 def apply_mapping(mask, mapping):

@@ -45,6 +45,18 @@ def structured_stft(F, T, D, K, seed=0, dtype=np.complex128):
     return y.astype(dtype), labels
 
 
+def permuted_mask(K, F, T, seed=0, noise=0.35):
+    """Permutation-alignment input: well-separated class masks proto**4 + noise
+    (normalised over K), each bin's classes shuffled.  Returns (mask, clean,
+    perm) with mask = clean[perm, range(F)], all (K, F, ...)."""
+    rng = np.random.RandomState(seed)
+    proto = rng.uniform(size=(K, 1, T)) ** 4
+    clean = proto + noise * rng.uniform(size=(K, F, T))
+    clean /= clean.sum(0, keepdims=True)
+    perm = np.stack([rng.permutation(K) for _ in range(F)], axis=1)
+    return clean[perm, np.arange(F)], clean, perm
+
+
 def pos_def_hermitian(*shape, seed=0):
     """Random Hermitian positive definite matrices (..., D, D)."""
     rng = np.random.RandomState(seed)

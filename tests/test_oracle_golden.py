@@ -220,6 +220,97 @@ def test_greedy_and_oracle_permutation_alignment(metric):
                                           g[f'oracle_{tag}{metric}_{alg}'])
 
 
+@pytest.mark.parametrize('metric', ['cos', 'multiply', 'euclidean'])
+@pytest.mark.parametrize('algorithm', ['greedy', 'optimal'])
+def test_dhtv_options(metric, algorithm):
+    # DHTVPermutationAlignment's similarity_metric / algorithm (permutation_alignment.py:133-163,295-355), K = 3
+    g = load_golden('permutation')
+    mapping, margin = O.dhtv_calculate_mapping(g['a_mask'], O.dhtv_plan_from_stft_size(512), metric, algorithm,
+                                               return_margin=True)
+    np.testing.assert_array_equal(mapping, g[f'opt_{metric}_{algorithm}'])
+    assert margin > MARGIN
+
+
+# smallest decision margin (relative to the largest |score| of the bin) for which the device kernels must reproduce
+# the reference's integer mapping: the kernels sum in other orders, so closer decisions may legitimately differ
+MARGIN = 1e-9
+CLASS_CASES = ('k2', 'k3', 'k4', 'k5', 'k6', 'k7', 'k8', 'k9', 'k8s', 'k9s', 'plan_edge',
+               'tie_const_k3', 'tie_const_k9', 'tie_pair_k3', 'tie_pair_k9', 'tie_zero_k3', 'tie_zero_k9')
+
+
+def test_permutation_classes_inputs_are_the_generators():
+    from oracle.make_golden import permutation_classes_cases
+    g = load_golden('permutation_classes')
+    assert sorted(g['dhtv_cases'].tolist()) == sorted(CLASS_CASES)
+    for name, (mask, plan) in permutation_classes_cases().items():
+        np.testing.assert_array_equal(g[f'{name}_mask'], mask)
+        assert g[f'{name}_plan'].tolist() == plan
+
+
+@pytest.mark.parametrize('name', CLASS_CASES)
+def test_dhtv_classes_and_ties(name):
+    """DHTV alignment, K = 2..9, every metric and assignment the fixture holds.  Exact ties (tie_*) follow the first
+    maximum in row-major order; every other decision is far from a tie, so any correct kernel reproduces it."""
+    g = load_golden('permutation_classes')
+    mask, plan = g[f'{name}_mask'], g[f'{name}_plan'].tolist()
+    combos = [(m, a) for m in METRICS for a in ('greedy', 'optimal') if f'{name}_{m}_{a}' in g]
+    keys = [f'{name}_{m}_{a}' for m, a in combos]
+    assert len(keys) >= 2
+    for key, (metric, algorithm) in zip(keys, combos):
+        mapping, margin = O.dhtv_calculate_mapping(mask, plan, metric, algorithm, return_margin=True)
+        np.testing.assert_array_equal(mapping, g[key], err_msg=key)
+        if name.startswith('tie_'):
+            assert margin == 0, key
+        else:
+            assert margin > MARGIN, (key, margin)
+    if name.startswith('tie_const'):
+        # every score ties: the first iteration keeps the identity and the reference stops there
+        assert all((g[k] == np.arange(mask.shape[0])[:, None]).all() for k in keys)
+
+
+@pytest.mark.parametrize('K', range(2, 10))
+def test_greedy_and_oracle_alignment_classes(K):
+    g = load_golden('permutation_classes')
+    mask, perm = g[f'k{K}_mask'], g[f'k{K}_perm']
+    reference = mask[np.argsort(perm, axis=0), np.arange(mask.shape[1])]
+    for tag, m, ref in (('k', mask, reference), ('noise_k', g[f'noise_k{K}_mask'], g[f'noise_k{K}_reference'])):
+        for metric in METRICS:
+            got, margin = O.greedy_permutation_alignment(m, metric, return_margin=True)
+            np.testing.assert_array_equal(got, g[f'{tag}{K}_greedy_{metric}'])
+            assert margin > MARGIN
+            for alg in ('greedy', 'optimal'):
+                key = f'{tag}{K}_oracle_{metric}_{alg}'
+                if key in g:
+                    got, margin = O.oracle_permutation_alignment(m, ref, metric, alg, return_margin=True)
+                    np.testing.assert_array_equal(got, g[key], err_msg=key)
+                    assert margin > MARGIN, key
+    # the Oracle alignment undoes the shuffle
+    np.testing.assert_array_equal(O.apply_mapping(mask, g[f'k{K}_oracle_euclidean_greedy']), reference)
+
+
+def test_assignment_margins_and_the_vectorised_brute_force():
+    import itertools
+    sm = np.array([[11, 10, 0], [4, 5, 10], [6, 0, 5]])  # permutation_alignment.py:475-508
+    assert O.greedy_mapping_from_score_matrix(sm, return_margin=True)[1] == 1  # 11 over 10; then 10 over 5
+    p, m = O.optimal_mapping_from_score_matrix(sm, return_margin=True)
+    np.testing.assert_array_equal(p, [1, 2, 0])
+    assert m == 5  # 26 over 21
+    rng = np.random.RandomState(3)
+    for K in (1, 2, 3, 4, 5, 6):
+        for _ in range(20):
+            score = rng.randint(0, 3, size=(K, K)).astype(np.float64)  # many exact ties
+            if rng.rand() < 0.5:
+                score = rng.uniform(-1, 1, size=(K, K))
+            best, best_perm = float('-inf'), None
+            for perm in itertools.permutations(range(K)):  # the reference's loop
+                s = sum(score[range(K), perm])
+                if s > best:
+                    best, best_perm = s, perm
+            np.testing.assert_array_equal(O.optimal_mapping_from_score_matrix(score), best_perm)
+    assert O.greedy_mapping_from_score_matrix(np.zeros((4, 4)), return_margin=True)[1] == 0
+    np.testing.assert_array_equal(O.greedy_mapping_from_score_matrix(np.zeros((4, 4))), np.arange(4))
+
+
 def test_mapping_from_score_matrix_doctest():
     # permutation_alignment.py:475-508: 'optimal' and 'greedy' differ on this matrix
     g = load_golden('permutation_greedy_oracle')
