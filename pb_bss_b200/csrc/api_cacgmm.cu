@@ -6,6 +6,8 @@
 #include <cstring>
 #include <map>
 #include <mutex>
+#include <optional>
+#include <type_traits>
 #include <vector>
 
 #include <cuda.h>
@@ -79,12 +81,20 @@ __global__ void unit_norm_over_classes_kernel(double* __restrict__ w, int K, int
 }
 
 // ---- workspace carving -------------------------------------------------------
+// Control block of the persistent fits, cleared by one memset (control_bytes) before the launch: flags (F) and the
+// ticket, then, 8-byte aligned, the PBB_PHASE_TIMING cycle sums (kPhaseWords; the kernels write 0..11) and the
+// two counters of the streamed upload's stream_load_kernel.
+constexpr int kPhaseWords = 16;
+
 struct CacgmmWorkspace {
   void* z;
   int zs;       // padded row stride of z (frames)
   int* flags;   // (F) per-bin model version, persistent kernel
   int* ticket;  // (1)
-  unsigned long long* phase;  // (16) debug phase counters
+  unsigned long long* phase;  // (kPhaseWords) debug phase counters
+  int* load_started;          // (1) stream_load_kernel CTAs running
+  int* load_next_bin;         // (1) next bin a stream_load_kernel CTA takes
+  size_t control_bytes;       // flags .. load_next_bin
   int* dead;    // (F) bins with an all-zero observation frame
   double* part;
   double* coef;
@@ -109,8 +119,10 @@ static CacgmmWorkspace carve(void* base, int F, int T, int D, int K) {
   const size_t nchunks = ((size_t)zs + kStageFrames - 1) / kStageFrames;
   const size_t z_plain = (size_t)F * D * zs * sizeof(double2);
   const size_t z_staged = (size_t)F * nchunks * stage_rows(D % 2 == 0 ? D : D + 1) * kStageFrames * sizeof(double2);
+  const size_t o_phase = align_up((size_t)(F + 1) * sizeof(int), 8);
+  ws.control_bytes = o_phase + kPhaseWords * sizeof(unsigned long long) + 2 * sizeof(int);
   const size_t o_z = take(z_plain > z_staged ? z_plain : z_staged);
-  const size_t o_flags = take((size_t)(F + 1) * sizeof(int) + 16 * sizeof(unsigned long long) + 8);
+  const size_t o_flags = take(ws.control_bytes);
   const size_t o_dead = take((size_t)F * sizeof(int));
   const size_t o_part = take((size_t)F * max_chunks(T) * K * (NS + 1) * sizeof(double));
   const size_t o_coef = take((size_t)F * K * NS * sizeof(double));
@@ -125,8 +137,10 @@ static CacgmmWorkspace carve(void* base, int F, int T, int D, int K) {
   ws.zs = zs;
   ws.flags = reinterpret_cast<int*>(b + o_flags);
   ws.ticket = ws.flags + F;
+  ws.phase = reinterpret_cast<unsigned long long*>(b + o_flags + o_phase);
+  ws.load_started = reinterpret_cast<int*>(ws.phase + kPhaseWords);
+  ws.load_next_bin = ws.load_started + 1;
   ws.dead = reinterpret_cast<int*>(b + o_dead);
-  ws.phase = reinterpret_cast<unsigned long long*>(b + o_flags + (((size_t)(F + 1) * sizeof(int) + 7) / 8) * 8);
   ws.part = reinterpret_cast<double*>(b + o_part);
   ws.coef = reinterpret_cast<double*>(b + o_coef);
   ws.ld = reinterpret_cast<double*>(b + o_ld);
@@ -137,6 +151,35 @@ static CacgmmWorkspace carve(void* base, int F, int T, int D, int K) {
   ws.tcount = reinterpret_cast<int*>(b + o_tcount);
   ws.bytes = off;
   return ws;
+}
+
+// ---- tuning overrides ------------------------------------------------------------
+// Environment variables for A/B runs.  PBB_EM_KERNEL is read once per process, the others on every persistent fit;
+// pbb_em_dispatch uses none of them (Tuning{}).
+struct Tuning {
+  int tsplit = 0;       // > 0: frame split into that many parts (PBB_TSPLIT)
+  int sticky = -1;      // sticky-bins cluster size: -1 automatic, 0 off, S > 0 only S (PBB_STICKY)
+  bool single = false;  // single-role kernel only (PBB_EM_KERNEL=single; the complex Watson fit has no other)
+  int load_ctas = 0;    // > 0: stream_load_kernel CTAs (PBB_LOAD_CTAS)
+  std::optional<int> wave_c;     // bins joining per slot of the streamed task order (PBB_WAVE_C)
+  std::optional<int> order_cap;  // tasks per slot of the streamed task order (PBB_ORDER_CAP)
+  bool order = true;    // explicit streamed task order; PBB_NO_ORDER: the wave_c rounds of decode_ticket
+};
+
+static Tuning read_tuning() {
+  static const bool single = [] {
+    const char* e = getenv("PBB_EM_KERNEL");
+    return e != nullptr && !strcmp(e, "single");
+  }();
+  Tuning t;
+  t.single = single;
+  if (const char* e = getenv("PBB_TSPLIT")) t.tsplit = atoi(e);
+  if (const char* e = getenv("PBB_STICKY")) t.sticky = atoi(e);
+  if (const char* e = getenv("PBB_LOAD_CTAS")) t.load_ctas = atoi(e);
+  if (const char* e = getenv("PBB_WAVE_C")) t.wave_c = atoi(e);
+  if (const char* e = getenv("PBB_ORDER_CAP")) t.order_cap = atoi(e);
+  t.order = getenv("PBB_NO_ORDER") == nullptr;
+  return t;
 }
 
 // Frame split of the persistent kernels (em_ws.cuh, em_persistent.cuh): with fewer bins than CTA slots the fit is
@@ -180,39 +223,20 @@ static int choose_sticky(int F, int T, const int clusters[3], int force) {
 // Persistent kernels of a fit, numbered as pbb_em_dispatch reports them (pbb.h).
 enum { kKernelWs = 0, kKernelSticky = 1, kKernelSingle = 2 };
 
-// Tuning overrides of the kernel choice (environment of pbb_cacgmm_fit).
-struct PlanOverrides {
-  int tsplit = 0;       // > 0: frame split into that many parts (PBB_TSPLIT)
-  int sticky = -1;      // sticky-bins cluster size: -1 automatic, 0 off, S > 0 only S (PBB_STICKY)
-  bool single = false;  // single-role kernel only (PBB_EM_KERNEL=single; the complex Watson fit has no other)
-};
-
 struct FitPlan {
   int kernel;  // kKernel*
   int split;   // sticky: CTAs per cluster; otherwise parts per bin-iteration (1 = no frame split)
 };
 
-static PlanOverrides env_overrides() {
-  static const bool single = [] {
-    const char* e = getenv("PBB_EM_KERNEL");
-    return e != nullptr && !strcmp(e, "single");
-  }();
-  PlanOverrides o;
-  o.single = single;
-  if (const char* e = getenv("PBB_TSPLIT")) o.tsplit = atoi(e);
-  if (const char* e = getenv("PBB_STICKY")) o.sticky = atoi(e);
-  return o;
-}
-
 // The sticky-bins kernel exists for the lean D = 8 fit of device-resident input.
-static bool sticky_eligible(int D, bool lean, bool streamed, const PlanOverrides& o) {
+static bool sticky_eligible(int D, bool lean, bool streamed, const Tuning& o) {
   return D == 8 && lean && !streamed && !o.single && o.sticky != 0;
 }
 
 // Which persistent kernel a fit runs and how it splits a bin-iteration (pure host logic).  sms: SMs of the device;
 // clusters: sticky-kernel clusters of 1, 2, 4 CTAs the device runs at once, read only when sticky_eligible.
 static FitPlan plan_persistent_fit(int F, int T, int D, int K, bool lean, bool streamed, int sms,
-                                   const int* clusters, const PlanOverrides& o) {
+                                   const int* clusters, const Tuning& o) {
   if (sticky_eligible(D, lean, streamed, o)) {
     const int S = choose_sticky(F, T, clusters, o.sticky);
     if (S > 0) return {kKernelSticky, S};
@@ -238,52 +262,81 @@ static int setup_frame_split(PersistArgs* p, const CacgmmWorkspace& ws, int F, i
   return 0;
 }
 
+// ---- shape / dtype dispatch ------------------------------------------------------
+// fn(ct) with a value of the storage type (double2 for PBB_C128, float2 for PBB_C64) standing for the type
+template <class Fn>
+static int with_ct(int dtype, Fn&& fn) {
+  return dtype == PBB_C128 ? fn(double2{}) : fn(float2{});
+}
+// fn(k, ct) with k = std::integral_constant<int, K> for the instantiated K in {2, 3, 4}
+template <class Fn>
+static int with_k_ct(int K, int dtype, Fn&& fn) {
+  auto on_k = [&](auto k) { return with_ct(dtype, [&](auto ct) { return fn(k, ct); }); };
+  switch (K) {
+    case 2: return on_k(std::integral_constant<int, 2>{});
+    case 3: return on_k(std::integral_constant<int, 3>{});
+    default: return on_k(std::integral_constant<int, 4>{});
+  }
+}
+// fn(d, k, ct) with d for the instantiated D in {4, 6, 8}
+template <class Fn>
+static int with_d_k_ct(int D, int K, int dtype, Fn&& fn) {
+  auto on_d = [&](auto d) { return with_k_ct(K, dtype, [&](auto k, auto ct) { return fn(d, k, ct); }); };
+  switch (D) {
+    case 4: return on_d(std::integral_constant<int, 4>{});
+    case 6: return on_d(std::integral_constant<int, 6>{});
+    default: return on_d(std::integral_constant<int, 8>{});
+  }
+}
+// complex Bingham kernels are instantiated for D = 2..6, the reference's domain (complex_bingham_utils.py:342-348)
+template <class Fn>
+static int with_bingham_d(int D, Fn&& fn) {
+  switch (D) {
+    case 2: return fn(std::integral_constant<int, 2>{});
+    case 3: return fn(std::integral_constant<int, 3>{});
+    case 4: return fn(std::integral_constant<int, 4>{});
+    case 5: return fn(std::integral_constant<int, 5>{});
+    case 6: return fn(std::integral_constant<int, 6>{});
+    default: set_error("complex Bingham: D = %d, need 2 <= D <= 6", D); return -5;
+  }
+}
+
 // ---- launches ------------------------------------------------------------------
-template <typename CT>
-static int launch_normalize(const void* y, void* z, int F, int T, int D, int swap, int zs, cudaStream_t st) {
-  const int block = D <= 16 ? 128 : 32;
-  dim3 grid((T + block - 1) / block, F);
-  const size_t smem = (size_t)block * (D + 1) * sizeof(double2);
-  LaunchScope ls("normalize_kernel", st);
-  normalize_kernel<CT><<<grid, block, smem, st>>>(reinterpret_cast<const CT*>(y), reinterpret_cast<CT*>(z), F, T,
-                                                    D, swap, zs);
+template <typename Kern, typename... Args>
+static int launch_kernel(const char* name, Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                         Args... args) {
+  LaunchScope ls(name, st);
+  kern<<<grid, block, smem, st>>>(args...);
   PBB_CUDA(cudaGetLastError());
   return 0;
 }
 
 template <typename CT>
-static int launch_normalize_staged(const void* y, void* z, int F, int T, int D, int* dead, cudaStream_t st) {
-  if (dead != nullptr) PBB_CUDA(cudaMemsetAsync(dead, 0, (size_t)F * sizeof(int), st));
-  const int block = 64;  // divides kStageFrames
-  const int nchunks = (((T + 31) / 32 * 32) + kStageFrames - 1) / kStageFrames;
-  dim3 grid(nchunks * (kStageFrames / block), F);
-  const size_t smem = (size_t)block * (D + 1) * sizeof(double2);
-  LaunchScope ls("normalize_staged_kernel", st);
-  normalize_staged_kernel<CT><<<grid, block, smem, st>>>(reinterpret_cast<const CT*>(y), reinterpret_cast<CT*>(z), F, T, D,
-                                                          stage_rows(D), kStageFrames, nchunks, dead);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+static int launch_normalize(const CT* y, CT* z, int F, int T, int D, int swap, int zs, cudaStream_t st) {
+  const int block = D <= 16 ? 128 : 32;
+  return launch_kernel("normalize_kernel", normalize_kernel<CT>, dim3((T + block - 1) / block, F), block,
+                       (size_t)block * (D + 1) * sizeof(double2), st, y, z, F, T, D, swap, zs);
+}
+
+// y -> ws.z, rows padded to ws.zs frames, or (staged) in the chunk-major layout of the persistent kernels: one TMA
+// bulk copy per ring stage, ws.dead cleared and set for bins with an all-zero frame
+static int normalize(const void* y, int dtype, const CacgmmWorkspace& ws, int F, int T, int D, bool staged,
+                     cudaStream_t st) {
+  if (staged) PBB_CUDA(cudaMemsetAsync(ws.dead, 0, (size_t)F * sizeof(int), st));
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    const CT* src = static_cast<const CT*>(y);
+    CT* dst = static_cast<CT*>(ws.z);
+    if (!staged) return launch_normalize(src, dst, F, T, D, 1, ws.zs, st);
+    const int block = 64;  // divides kStageFrames
+    const int nchunks = (ws.zs + kStageFrames - 1) / kStageFrames;
+    return launch_kernel("normalize_staged_kernel", normalize_staged_kernel<CT>,
+                         dim3(nchunks * (kStageFrames / block), F), block, (size_t)block * (D + 1) * sizeof(double2),
+                         st, src, dst, F, T, D, stage_rows(D), kStageFrames, nchunks, ws.dead);
+  });
 }
 
 static bool fast_shape(int D, int K) { return (D == 4 || D == 6 || D == 8) && K >= 2 && K <= 4; }
-
-template <int D, int K>
-static cudaError_t launch_fast_dk(const EmArgs& a, int dtype, cudaStream_t st) {
-  dim3 grid(a.nch, a.F);
-  LaunchScope ls("em_fast_kernel", st);
-  if (dtype == PBB_C128) em_fast_kernel<D, K, double2><<<grid, 32 * kEmGroups, 0, st>>>(a);
-  else em_fast_kernel<D, K, float2><<<grid, 32 * kEmGroups, 0, st>>>(a);
-  return cudaGetLastError();
-}
-
-template <int D>
-static cudaError_t launch_fast_d(const EmArgs& a, int dtype, cudaStream_t st) {
-  switch (a.K) {
-    case 2: return launch_fast_dk<D, 2>(a, dtype, st);
-    case 3: return launch_fast_dk<D, 3>(a, dtype, st);
-    default: return launch_fast_dk<D, 4>(a, dtype, st);
-  }
-}
 
 // Fills nch / frames_per_block and launches the EM kernel for the shape.
 int launch_em(EmArgs a, int dtype, int frames_per_block, cudaStream_t st) {
@@ -293,66 +346,93 @@ int launch_em(EmArgs a, int dtype, int frames_per_block, cudaStream_t st) {
     if (fpb > (a.T + 31) / 32 * 32) fpb = (a.T + 31) / 32 * 32;
     a.frames_per_block = fpb;
     a.nch = (a.T + fpb - 1) / fpb;
-    cudaError_t e;
-    switch (a.D) {
-      case 4: e = launch_fast_d<4>(a, dtype, st); break;
-      case 6: e = launch_fast_d<6>(a, dtype, st); break;
-      default: e = launch_fast_d<8>(a, dtype, st); break;
-    }
-    PBB_CUDA(e);
-    return a.nch;
+    const int r = with_d_k_ct(a.D, a.K, dtype, [&](auto d, auto k, auto ct) {
+      return launch_kernel("em_fast_kernel", em_fast_kernel<decltype(d)::value, decltype(k)::value, decltype(ct)>,
+                           dim3(a.nch, a.F), 32 * kEmGroups, 0, st, a);
+    });
+    return r ? r : a.nch;
   }
   a.frames_per_block = kGenFrames;
   a.nch = (a.T + kGenFrames - 1) / kGenFrames;
   a.softmax_fast = 0;
-  dim3 grid(a.nch, a.F);
   const size_t smem = (size_t)2 * a.K * kGenFrames * sizeof(double) + (size_t)a.D * a.D * sizeof(int);
-  LaunchScope ls("em_generic_kernel", st);
-  if (dtype == PBB_C128) {
-    PBB_CUDA(cudaFuncSetAttribute(em_generic_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    em_generic_kernel<double2><<<grid, kGenFrames, smem, st>>>(a);
-  } else {
-    PBB_CUDA(cudaFuncSetAttribute(em_generic_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    em_generic_kernel<float2><<<grid, kGenFrames, smem, st>>>(a);
-  }
-  PBB_CUDA(cudaGetLastError());
-  return a.nch;
+  const int r = with_ct(dtype, [&](auto ct) {
+    const auto kern = em_generic_kernel<decltype(ct)>;
+    PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    return launch_kernel("em_generic_kernel", kern, dim3(a.nch, a.F), kGenFrames, smem, st, a);
+  });
+  return r ? r : a.nch;
 }
 
-static int update_warps(int D, int K) {
-  const size_t per = update_smem_per_warp(D);
-  int w = (int)((size_t)(200 * 1024) / per);
-  if (w > K) w = K;
-  if (w > 16) w = 16;
-  if (w < 1) w = 1;
-  return w;
-}
-
-static int launch_update(UpdArgs u, cudaStream_t st) {
-  u.warps = update_warps(u.D, u.K);
-  const size_t smem = update_smem_per_warp(u.D) * u.warps + (size_t)2 * u.K * sizeof(double) +
-                      (size_t)u.D * u.D * sizeof(int);
-  PBB_CUDA(cudaFuncSetAttribute(cacg_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  const int threads = 32 * u.warps < u.K ? ((u.K + 31) / 32 * 32) : 32 * u.warps;
-  LaunchScope ls("cacg_update_kernel", st);
-  cacg_update_kernel<<<u.F, threads, smem, st>>>(u);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
-}
-
-static int launch_from_eig(FromEigArgs u, cudaStream_t st) {
-  const size_t per = from_eig_smem_per_warp(u.D);
+// cacg_update_kernel (UpdArgs) or cw_update_kernel (CwUpdArgs): one CTA per bin, up to 16 warps
+template <typename U>
+static int launch_update(void (*kern)(U), const char* name, U u, cudaStream_t st) {
+  const size_t per = update_smem_per_warp(u.D);
   int w = (int)((size_t)(200 * 1024) / per);
   if (w > u.K) w = u.K;
   if (w > 16) w = 16;
+  if (w < 1) w = 1;
   u.warps = w;
-  const size_t smem = per * w + (size_t)u.K * sizeof(double) + (size_t)u.D * u.D * sizeof(int);
-  PBB_CUDA(cudaFuncSetAttribute(cacg_from_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  const size_t smem = per * w + (size_t)2 * u.K * sizeof(double) + (size_t)u.D * u.D * sizeof(int);
+  PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
   const int threads = 32 * w < u.K ? ((u.K + 31) / 32 * 32) : 32 * w;
-  LaunchScope ls("cacg_from_eig_kernel", st);
-  cacg_from_eig_kernel<<<u.F, threads, smem, st>>>(u);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel(name, kern, u.F, threads, smem, st, u);
+}
+
+// E-step form of a model given by eigenvectors, eigenvalues and weights (null: 1/K) into the workspace
+static int launch_from_eig(const CacgmmWorkspace& ws, int F, int D, int K, const void* evec, const double* eval,
+                           const double* weight, cudaStream_t st) {
+  FromEigArgs u;
+  u.F = F; u.D = D; u.K = K;
+  u.evec = reinterpret_cast<const double2*>(evec);
+  u.eval = eval; u.weight = weight;
+  u.coef = ws.coef; u.ld = ws.ld; u.w = ws.w; u.ew = ws.ew;
+  const size_t per = from_eig_smem_per_warp(D);
+  int w = (int)((size_t)(200 * 1024) / per);
+  if (w > K) w = K;
+  if (w > 16) w = 16;
+  u.warps = w;
+  const size_t smem = per * w + (size_t)K * sizeof(double) + (size_t)D * D * sizeof(int);
+  PBB_CUDA(cudaFuncSetAttribute(cacg_from_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  const int threads = 32 * w < K ? ((K + 31) / 32 * 32) : 32 * w;
+  return launch_kernel("cacg_from_eig_kernel", cacg_from_eig_kernel, F, threads, smem, st, u);
+}
+
+// ---- kernel arguments --------------------------------------------------------------
+// the workspace and shape part of the arguments; each entry point adds what is specific to it
+static EmArgs em_args(const CacgmmWorkspace& ws, int F, int T, int D, int K) {
+  EmArgs a;
+  memset(&a, 0, sizeof(a));
+  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  a.coef = ws.coef; a.ld = ws.ld; a.w = ws.w; a.ew = ws.ew; a.part = ws.part;
+  return a;
+}
+
+static UpdArgs upd_args(const CacgmmWorkspace& ws, int F, int T, int D, int K, const pbb_cacgmm_options* opt,
+                        bool has_saliency, void* evec, double* eval, double* weight, int* status) {
+  UpdArgs u;
+  memset(&u, 0, sizeof(u));
+  u.F = F; u.T = T; u.D = D; u.K = K;
+  u.part = ws.part;
+  u.covariance_norm = opt->covariance_norm;
+  u.weight_mode = opt->weight_mode;
+  u.has_saliency = has_saliency;
+  u.eigenvalue_floor = opt->eigenvalue_floor;
+  u.evec = reinterpret_cast<double2*>(evec);
+  u.eval = eval; u.weight = weight;
+  u.coef = ws.coef; u.ld = ws.ld; u.ew = ws.ew;
+  u.status = status;
+  return u;
+}
+
+static PersistArgs persist_args(const CacgmmWorkspace& ws, int F, int T, int iterations, int* status) {
+  PersistArgs p;
+  memset(&p, 0, sizeof(p));
+  p.z = ws.z; p.zs = ws.zs; p.F = F; p.T = T;
+  p.iterations = iterations;
+  p.coef = ws.coef; p.ld = ws.ld; p.w = ws.w; p.ew = ws.ew;
+  p.part = ws.part; p.flags = ws.flags; p.ticket = ws.ticket; p.status = status; p.phase = ws.phase;
+  return p;
 }
 
 // ---- persistent kernel launch ---------------------------------------------------
@@ -418,18 +498,19 @@ static int streamed_order(int F, int I, int arrive, int cap, const int** out) {
   return 0;
 }
 
-// device-usable address of a pinned host allocation, nullptr for device memory, error otherwise
-static int classify_pointer(const void* p, const void** dev_alias, bool* is_host, const char* what) {
+// Replaces *p by the address the kernels use: itself for device memory, the mapped device alias of pinned host
+// memory (*is_host = true); any other memory is an error.
+template <typename P>
+static int device_alias(P** p, bool* is_host, const char* what) {
   cudaPointerAttributes at;
-  PBB_CUDA(cudaPointerGetAttributes(&at, p));
+  PBB_CUDA(cudaPointerGetAttributes(&at, *p));
   if (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) {
     *is_host = false;
-    *dev_alias = p;
     return 0;
   }
   if (at.type == cudaMemoryTypeHost && at.devicePointer != nullptr) {
     *is_host = true;
-    *dev_alias = at.devicePointer;
+    *p = static_cast<P*>(at.devicePointer);
     return 0;
   }
   set_error("%s must be device memory or pinned (page-locked, mapped) host memory", what);
@@ -469,22 +550,19 @@ static int get_load_stream(LoadStream** out) {
   return 0;
 }
 
-template <typename CT>
-static int launch_stream_load(const void* y, void* z, const double* aff_src, double* aff_dst, int F, int T, int D, int K,
-                              int* dead, int* flags, int* next_bin, int* started, int* ctas_out, cudaStream_t st) {
-  const int nchunks = (((T + 31) / 32 * 32) + kStageFrames - 1) / kStageFrames;
+static int launch_stream_load(const void* y, int dtype, const CacgmmWorkspace& ws, const double* aff_src,
+                              double* aff_dst, int F, int T, int D, int K, int ctas, cudaStream_t st) {
+  const int nchunks = (ws.zs + kStageFrames - 1) / kStageFrames;
   const size_t smem = (size_t)kStageFrames * (D + 1) * sizeof(double2);
-  LaunchScope ls("stream_load_kernel", st);
-  int ctas = kLoadCtas;
-  if (const char* e = getenv("PBB_LOAD_CTAS")) ctas = atoi(e) > 0 ? atoi(e) : ctas;  // tuning override
-  ctas = ctas < F ? ctas : F;
-  *ctas_out = ctas;
-  stream_load_kernel<CT><<<ctas, kLoadThreads, smem, st>>>(
-      reinterpret_cast<const CT*>(y), reinterpret_cast<CT*>(z), aff_src, aff_dst, F, T, D, K,
-      stage_rows(D), kStageFrames, nchunks, dead, flags, next_bin, started);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_kernel("stream_load_kernel", stream_load_kernel<CT>, ctas, kLoadThreads, smem, st,
+                         static_cast<const CT*>(y), static_cast<CT*>(ws.z), aff_src, aff_dst, F, T, D, K,
+                         stage_rows(D), kStageFrames, nchunks, ws.dead, ws.flags, ws.load_next_bin,
+                         ws.load_started);
+  });
 }
+
 template <typename Kern>
 static int launch_persistent_generic(Kern kern, int threads, size_t smem, int* cache, const PersistArgs& a,
                                      const char* name, cudaStream_t st) {
@@ -498,9 +576,8 @@ static int launch_persistent_generic(Kern kern, int threads, size_t smem, int* c
     if (n < 1) { set_error("%s does not fit on this device", name); return 1; }
     *cache = n;
   }
-  int dev = 0, sms = 0;
-  PBB_CUDA(cudaGetDevice(&dev));
-  PBB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int sms = 0;
+  if (int r = device_sms(&sms)) return r;
   long long grid = (long long)(*cache) * sms - reserve;
   if (grid < 1) grid = 1;
   const long long tasks = (long long)a.iterations * a.F * (a.tsplit > 1 ? a.tsplit : 1);
@@ -512,133 +589,103 @@ static int launch_persistent_generic(Kern kern, int threads, size_t smem, int* c
 }
 
 // full = saliency / activity mask / log-domain softmax; lean = product-form softmax, 2 frames per lane;
-// ws = the warp-specialised em_ws_kernel (D = 8, lean) instead of the single-role kernel
-template <int D, int K, typename CT>
-static int launch_persist_t(const PersistArgs& a, bool full, bool ws, cudaStream_t st) {
-  static int cache_full = 0, cache_lean = 0;
-  if (full)
-    return launch_persistent_generic(em_persistent_kernel<D, K, CT, true, 1>, persist_threads(D, K),
-                                     sizeof(PersistSmem<D, K, CT>), &cache_full, a, "em_persistent_kernel", st);
-  if constexpr (D == 8) {
-    static int cache_ws = 0;
-    if (ws)
-      return launch_persistent_generic(em_ws_kernel<K, CT>, 256, sizeof(WsSmem<D, K, CT>), &cache_ws, a,
-                                       "em_ws_kernel", st);
-  }
-  return launch_persistent_generic(em_persistent_kernel<D, K, CT, false, 2>, persist_threads(D, K),
-                                   sizeof(PersistSmem<D, K, CT>), &cache_lean, a, "em_persistent_kernel", st);
-}
+// ws = the warp-specialised em_ws_kernel (D = 8, lean) instead of the single-role kernel;
+// cw = complex Watson EM (lean structure, MODEL = 1)
+enum class Persist { kFull, kLean, kWs, kCw };
 
-// complex Watson EM on the persistent kernel (lean structure, MODEL = 1)
-template <int D, int K, typename CT>
-static int launch_persist_cw_t(const PersistArgs& a, cudaStream_t st) {
-  static int cache = 0;
-  return launch_persistent_generic(em_persistent_kernel<D, K, CT, false, 2, 1>, persist_threads(D, K),
-                                   sizeof(PersistSmem<D, K, CT>), &cache, a, "em_persistent_kernel_cw", st);
-}
-template <int D>
-static int launch_persist_cw_d(const PersistArgs& a, int K, int dtype, cudaStream_t st) {
-  const bool c128 = dtype == PBB_C128;
-  switch (K) {
-    case 2: return c128 ? launch_persist_cw_t<D, 2, double2>(a, st) : launch_persist_cw_t<D, 2, float2>(a, st);
-    case 3: return c128 ? launch_persist_cw_t<D, 3, double2>(a, st) : launch_persist_cw_t<D, 3, float2>(a, st);
-    default: return c128 ? launch_persist_cw_t<D, 4, double2>(a, st) : launch_persist_cw_t<D, 4, float2>(a, st);
-  }
-}
-static int launch_persist_cw(const PersistArgs& a, int D, int K, int dtype, cudaStream_t st) {
-  switch (D) {
-    case 4: return launch_persist_cw_d<4>(a, K, dtype, st);
-    case 6: return launch_persist_cw_d<6>(a, K, dtype, st);
-    default: return launch_persist_cw_d<8>(a, K, dtype, st);
-  }
-}
-
-template <int D, int K>
-static int launch_persist_dk(const PersistArgs& a, int dtype, bool full, bool ws, cudaStream_t st) {
-  if (dtype == PBB_C128) return launch_persist_t<D, K, double2>(a, full, ws, st);
-  return launch_persist_t<D, K, float2>(a, full, ws, st);
-}
-
-template <int D>
-static int launch_persist_d(const PersistArgs& a, int K, int dtype, bool full, bool ws, cudaStream_t st) {
-  switch (K) {
-    case 2: return launch_persist_dk<D, 2>(a, dtype, full, ws, st);
-    case 3: return launch_persist_dk<D, 3>(a, dtype, full, ws, st);
-    default: return launch_persist_dk<D, 4>(a, dtype, full, ws, st);
-  }
+static int launch_persist(const PersistArgs& a, int D, int K, int dtype, Persist v, cudaStream_t st) {
+  return with_d_k_ct(D, K, dtype, [&](auto d, auto k, auto ct) {
+    constexpr int Dc = decltype(d)::value, Kc = decltype(k)::value;
+    using CT = decltype(ct);
+    static int cache[4] = {0, 0, 0, 0};  // occupancy per Persist, queried on the first launch
+    const int threads = persist_threads(Dc, Kc);
+    const size_t smem = sizeof(PersistSmem<Dc, Kc, CT>);
+    int* c = &cache[(int)v];
+    if (v == Persist::kFull)
+      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, true, 1>, threads, smem, c, a,
+                                       "em_persistent_kernel", st);
+    if (v == Persist::kCw)
+      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 2, 1>, threads, smem, c, a,
+                                       "em_persistent_kernel_cw", st);
+    if constexpr (Dc == 8) {
+      if (v == Persist::kWs)
+        return launch_persistent_generic(em_ws_kernel<Kc, CT>, 256, sizeof(WsSmem<Dc, Kc, CT>), c, a, "em_ws_kernel",
+                                         st);
+    }
+    return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 2>, threads, smem,
+                                     &cache[(int)Persist::kLean], a, "em_persistent_kernel", st);
+  });
 }
 
 // "Sticky bins" (em_sticky.cuh): when the device runs F clusters of S CTAs at once, a cluster keeps one bin for the
 // whole fit (choose_sticky).  PBB_STICKY=0 disables it, PBB_STICKY=S forces a cluster size (A/B).
-static void sticky_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* attr, unsigned ctas, int S, size_t smem,
-                          cudaStream_t st) {
-  memset(cfg, 0, sizeof(*cfg));
-  cfg->gridDim = dim3(ctas);
-  cfg->blockDim = dim3(256);
-  cfg->dynamicSmemBytes = smem;
-  cfg->stream = st;
-  attr->id = cudaLaunchAttributeClusterDimension;
-  attr->val.clusterDim.x = (unsigned)S;
-  attr->val.clusterDim.y = 1;
-  attr->val.clusterDim.z = 1;
-  cfg->attrs = attr;
-  cfg->numAttrs = 1;
-}
-// clusters of 1, 2, 4 CTAs of em_sticky_kernel the device runs at once (queried once per instantiation)
-template <int K, typename CT>
-static int sticky_clusters_t(int clusters[3], cudaStream_t st) {
-  static int cache[3] = {-1, -1, -1};
-  if (cache[0] < 0) {
-    const size_t smem = sizeof(WsSmem<8, K, CT>);
-    cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute attr[1];
-    PBB_CUDA(cudaFuncSetAttribute(em_sticky_kernel<K, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    for (int i = 0; i < 3; ++i) {
-      sticky_config(&cfg, attr, 1u << i, 1 << i, smem, st);
-      int n = 0;
-      PBB_CUDA(cudaOccupancyMaxActiveClusters(&n, em_sticky_kernel<K, CT>, &cfg));
-      cache[i] = n;
-    }
-  }
-  for (int i = 0; i < 3; ++i) clusters[i] = cache[i];
-  return 0;
-}
+// Clusters of 1, 2, 4 CTAs of em_sticky_kernel the device runs at once (queried once per instantiation).
 static int sticky_clusters(int K, int dtype, int clusters[3], cudaStream_t st) {
-  const bool c128 = dtype == PBB_C128;
-  switch (K) {
-    case 2: return c128 ? sticky_clusters_t<2, double2>(clusters, st) : sticky_clusters_t<2, float2>(clusters, st);
-    case 3: return c128 ? sticky_clusters_t<3, double2>(clusters, st) : sticky_clusters_t<3, float2>(clusters, st);
-    default: return c128 ? sticky_clusters_t<4, double2>(clusters, st) : sticky_clusters_t<4, float2>(clusters, st);
-  }
+  return with_k_ct(K, dtype, [&](auto k, auto ct) {
+    static int cache[3] = {-1, -1, -1};
+    if (cache[0] < 0) {
+      const auto kern = em_sticky_kernel<decltype(k)::value, decltype(ct)>;
+      const size_t smem = sizeof(WsSmem<8, decltype(k)::value, decltype(ct)>);
+      PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      for (int i = 0; i < 3; ++i) {
+        const ClusterLaunch cl(1u << i, 256, smem, 1u << i, st);
+        int n = 0;
+        PBB_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cl.cfg));
+        cache[i] = n;
+      }
+    }
+    for (int i = 0; i < 3; ++i) clusters[i] = cache[i];
+    return 0;
+  });
 }
 
 // one cluster of S CTAs per bin; sticky_clusters has set the kernel's shared-memory limit
-template <int K, typename CT>
-static int launch_sticky_t(const PersistArgs& a, int S, cudaStream_t st) {
-  cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[1];
-  sticky_config(&cfg, attr, (unsigned)(a.F * S), S, sizeof(WsSmem<8, K, CT>), st);
-  LaunchScope ls("em_sticky_kernel", st);
-  PBB_CUDA(cudaLaunchKernelEx(&cfg, em_sticky_kernel<K, CT>, a));
-  return 0;
-}
 static int launch_sticky(const PersistArgs& a, int K, int dtype, int S, cudaStream_t st) {
-  const bool c128 = dtype == PBB_C128;
-  switch (K) {
-    case 2: return c128 ? launch_sticky_t<2, double2>(a, S, st) : launch_sticky_t<2, float2>(a, S, st);
-    case 3: return c128 ? launch_sticky_t<3, double2>(a, S, st) : launch_sticky_t<3, float2>(a, S, st);
-    default: return c128 ? launch_sticky_t<4, double2>(a, S, st) : launch_sticky_t<4, float2>(a, S, st);
-  }
+  return with_k_ct(K, dtype, [&](auto k, auto ct) {
+    const ClusterLaunch cl((unsigned)(a.F * S), 256, sizeof(WsSmem<8, decltype(k)::value, decltype(ct)>),
+                           (unsigned)S, st);
+    LaunchScope ls("em_sticky_kernel", st);
+    PBB_CUDA(cudaLaunchKernelEx(&cl.cfg, em_sticky_kernel<decltype(k)::value, decltype(ct)>, a));
+    return 0;
+  });
 }
 
-static int launch_persist(const PersistArgs& a, int D, int K, int dtype, bool full, bool ws, cudaStream_t st) {
-  switch (D) {
-    case 4: return launch_persist_d<4>(a, K, dtype, full, ws, st);
-    case 6: return launch_persist_d<6>(a, K, dtype, full, ws, st);
-    default: return launch_persist_d<8>(a, K, dtype, full, ws, st);
-  }
+// Plan and launch of a persistent fit whose control block is clear: the sticky-bins kernel when the plan picks it,
+// otherwise the frame split and the task kernel.  model: kFull, kLean or kCw (always the single-role kernel).
+static int launch_planned(PersistArgs p, const CacgmmWorkspace& ws, int D, int K, int dtype, Persist model,
+                          bool streamed, Tuning tu, cudaStream_t st) {
+  if (model == Persist::kCw) tu.single = true;
+  const bool lean = model != Persist::kFull;
+  int clusters[3] = {0, 0, 0}, sms = 0, r;
+  if (sticky_eligible(D, lean, streamed, tu) && (r = sticky_clusters(K, dtype, clusters, st))) return r;
+  if ((r = device_sms(&sms))) return r;
+  const FitPlan plan = plan_persistent_fit(p.F, p.T, D, K, lean, streamed, sms, clusters, tu);
+  if (plan.kernel == kKernelSticky) return launch_sticky(p, K, dtype, plan.split, st);  // few bins: one cluster per bin
+  if ((r = setup_frame_split(&p, ws, p.F, D, K, plan.split, st))) return r;
+  if (plan.kernel == kKernelWs) model = Persist::kWs;
+  return launch_persist(p, D, K, dtype, model, st);
 }
 
+#ifdef PBB_PHASE_TIMING
+// cycles per task of the persistent kernel's phases (PBB_PH / PBB_PHU in em_persistent.cuh and em_ws.cuh)
+static void print_phases(const CacgmmWorkspace& ws, long long tasks, bool cw, cudaStream_t st) {
+  unsigned long long ph[12];
+  cudaStreamSynchronize(st);
+  cudaMemcpy(ph, ws.phase, sizeof(ph), cudaMemcpyDeviceToHost);
+  if (!cw)
+    fprintf(stderr, "[phase] update of class 0, cycles per task: build %.0f  gauss-jordan %.0f  logdet/tinv %.0f  stores %.0f\n",
+            ph[8] / (double)tasks, ph[9] / (double)tasks, ph[10] / (double)tasks, ph[11] / (double)tasks);
+  unsigned long long tot = 0;
+  for (int i = 0; i < 8; ++i) tot += ph[i];
+  static const char* nm[8] = {"ticket+flag / model wait", "chunk-top / updater busy", "tma-wait", "em-steps", "reduce", "update / S wait", "publish / hand-over", "task-start / updater idle"};
+  static const char* nm_cw[8] = {"flag wait", "chunk top / staging", "tma-wait", "em-steps", "reduce", "update (jacobi)", "publish", "task-start"};
+  for (int i = 0; i < 8; ++i)
+    fprintf(stderr, "[phase%s] %-20s %6.2f%%  %8.0f cycles per task\n", cw ? " cw" : "", cw ? nm_cw[i] : nm[i],
+            100.0 * ph[i] / (double)tot, ph[i] / (double)tasks);
+}
+#endif
+
+// ---- entry-point steps ------------------------------------------------------------
 static bool softmax_fast_ok(int D, const pbb_cacgmm_options* o) {
   if (o->covariance_norm != PBB_NORM_EIGENVALUE) return false;
   if (!(o->eigenvalue_floor > 0.0) || o->eigenvalue_floor > 1.0) return false;
@@ -654,67 +701,159 @@ static int check_shape(int F, int T, int D, int K, int dtype) {
   return 0;
 }
 
-static int launch_cw_update(CwUpdArgs u, cudaStream_t st) {
-  u.warps = update_warps(u.D, u.K);
-  const size_t smem = update_smem_per_warp(u.D) * u.warps + (size_t)2 * u.K * sizeof(double) +
-                      (size_t)u.D * u.D * sizeof(int);
-  PBB_CUDA(cudaFuncSetAttribute(cw_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  const int threads = 32 * u.warps < u.K ? ((u.K + 31) / 32 * 32) : 32 * u.warps;
-  LaunchScope ls("cw_update_kernel", st);
-  cw_update_kernel<<<u.F, threads, smem, st>>>(u);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// complex Bingham kernels are instantiated for D = 2..6, the reference's domain (complex_bingham_utils.py:342-348)
-template <template <int> class Launch, typename... Args>
-static int bingham_dispatch(int D, Args... args) {
-  switch (D) {
-    case 2: return Launch<2>::run(args...);
-    case 3: return Launch<3>::run(args...);
-    case 4: return Launch<4>::run(args...);
-    case 5: return Launch<5>::run(args...);
-    case 6: return Launch<6>::run(args...);
-    default: set_error("complex Bingham: D = %d, need 2 <= D <= 6", D); return -5;
-  }
-}
-template <int D> struct CbUpdateLaunch {
-  static int run(CbUpdArgs u, cudaStream_t st) {
-    LaunchScope ls("cb_update_kernel", st);
-    cb_update_kernel<D><<<u.F, 32 * kCbWarps, 0, st>>>(u);
-    PBB_CUDA(cudaGetLastError());
-    return 0;
-  }
-};
-template <int D> struct CbFromModelLaunch {
-  static int run(CbFromModelArgs u, cudaStream_t st) {
-    LaunchScope ls("cb_from_model_kernel", st);
-    cb_from_model_kernel<D><<<u.F, 32 * kCbWarps, 0, st>>>(u);
-    PBB_CUDA(cudaGetLastError());
-    return 0;
-  }
-};
-template <int D> struct BinghamParametersLaunch {
-  static int run(const double* s, int n, double eps, double mc, double* lam, int* status, cudaStream_t st) {
-    LaunchScope ls("bingham_parameters_kernel", st);
-    bingham_parameters_kernel<D><<<(n + 3) / 4, 128, 0, st>>>(s, n, eps, mc, lam, status);
-    PBB_CUDA(cudaGetLastError());
-    return 0;
-  }
-};
-template <int D> struct BinghamLogNormLaunch {
-  static int run(const double* lam, int n, double eps, double* out, cudaStream_t st) {
-    LaunchScope ls("bingham_log_norm_kernel", st);
-    bingham_log_norm_kernel<D><<<(n + 127) / 128, 128, 0, st>>>(lam, n, eps, out);
-    PBB_CUDA(cudaGetLastError());
-    return 0;
-  }
-};
-
 static int check_cbmm_shape(int F, int T, int D, int K, int dtype) {
   if (int r = check_shape(F, T, D, K, dtype)) return r;
   PBB_CHECK_ARG(D >= 2 && D <= 6, 5, "complex Bingham: need 2 <= D <= 6 (complex_bingham_utils.py:342-348)");
   PBB_CHECK_ARG((long long)F * K <= kCbMaxIndex, 6, "F * K too large for the status word");
+  return 0;
+}
+
+enum class Layout { kNone, kPlain, kStaged };
+
+// Opening of the EM entry points, after their other argument checks: the workspace (argument ws_arg) and status
+// (ws_arg + 2) checks, the workspace carve, the status reset and, unless layout is kNone, normalize.
+static int begin_call(const void* y, int dtype, int F, int T, int D, int K, void* workspace, size_t workspace_bytes,
+                      int ws_arg, const char* ws_msg, int* status, Layout layout, cudaStream_t st,
+                      CacgmmWorkspace* ws) {
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= carve(nullptr, F, T, D, K).bytes, ws_arg, ws_msg);
+  PBB_CHECK_ARG(status != nullptr, ws_arg + 2, "status is null");
+  *ws = carve(workspace, F, T, D, K);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  return layout == Layout::kNone ? 0 : normalize(y, dtype, *ws, F, T, D, layout == Layout::kStaged, st);
+}
+
+// One pbb_cacgmm_fit call after its argument checks.
+struct FitCall {
+  const void* y;
+  int dtype, F, T, D, K;
+  const double *init_aff, *saliency;
+  const uint8_t* activity;
+  const pbb_cacgmm_options* opt;
+  void* evec;
+  double *eval, *weight;
+  int* status;
+  cudaStream_t st;
+  CacgmmWorkspace ws;
+  bool y_host, aff_host;  // y / the initial affiliations are pinned host memory
+};
+
+// y (and the initial affiliations) may be pinned host memory: the kernels then read them in place over PCIe.  The
+// model may be written straight into pinned host memory as well (write-only on this path).
+static int resolve_host_aliases(FitCall& c) {
+  int r;
+  bool h = false;
+  if ((r = device_alias(&c.y, &c.y_host, "y"))) return r;
+  if (c.init_aff != nullptr && (r = device_alias(&c.init_aff, &c.aff_host, "initial affiliations"))) return r;
+  if ((r = device_alias(&c.evec, &h, "eigenvectors"))) return r;
+  if ((r = device_alias(&c.eval, &h, "eigenvalues"))) return r;
+  return device_alias(&c.weight, &h, "weight");
+}
+
+// Streamed upload: on the persistent path with a host-resident y and an affiliation initialisation, a separate
+// small kernel on a side stream reads them over PCIe into the staged layout while the EM kernel runs.  Clears the
+// control block (flags[bin] = -1 until the bin has arrived) and fills the upload fields of p.
+static int start_streamed_upload(FitCall& c, LoadStream& l, const Tuning& tu, PersistArgs* p) {
+  const CacgmmWorkspace& ws = c.ws;
+  const int F = c.F, T = c.T, D = c.D, K = c.K, iterations = c.opt->iterations;
+  PBB_CUDA(cudaMemsetAsync(ws.flags, 0, ws.control_bytes, c.st));
+  PBB_CUDA(cudaMemsetAsync(ws.flags, 0xFF, (size_t)F * sizeof(int), c.st));
+  PBB_CUDA(cudaMemsetAsync(ws.dead, 0, (size_t)F * sizeof(int), c.st));
+  PBB_CUDA(cudaEventRecord(l.fork, c.st));
+  PBB_CUDA(cudaStreamWaitEvent(l.stream, l.fork, 0));
+  const int ctas = std::min(tu.load_ctas > 0 ? tu.load_ctas : kLoadCtas, F);
+  if (int r = launch_stream_load(c.y, c.dtype, ws, c.init_aff, c.aff_host ? ws.aff_stage : nullptr, F, T, D, K, ctas,
+                                 l.stream))
+    return r;
+  PBB_CUDA(cudaEventRecord(l.join, l.stream));
+  // Hold the EM kernel back until every loader CTA runs: launched at the same moment, the EM grid
+  // could take the whole machine first and leave the loader only the reserved slots (it would still
+  // finish -- bins are handed out by a counter -- but at a fraction of the link rate).
+  if (l.wait_value != nullptr) {
+    if (l.wait_value(reinterpret_cast<CUstream>(c.st), reinterpret_cast<CUdeviceptr>(ws.load_started),
+                     (cuuint32_t)ctas, CU_STREAM_WAIT_VALUE_GEQ) != CUDA_SUCCESS)
+      l.wait_value = nullptr;  // not supported here: rely on the reserved slots
+  }
+  if (c.aff_host) c.init_aff = ws.aff_stage;
+  // bins joining per slot ~ slot duration / arrival time of one bin at ~50 GB/s of PCIe reads
+  const double bin_bytes = (double)T * D * (c.dtype == PBB_C128 ? 16.0 : 8.0) + (c.aff_host ? 8.0 * K * T : 0.0);
+  // one slot of the order table = one link of a bin's dependency chain (task + update + staging
+  // of the next model, ~23 us at D = 8, K = 3, T = 500), during which the machine runs ~1.6 tasks per CTA
+  const double round_us = 23.0 * (T / 500.0) * (D * D / 64.0) * (K / 3.0);
+  int wave = tu.wave_c ? *tu.wave_c : (int)(round_us / (bin_bytes / 50e3) + 0.5);
+  wave = wave < 1 ? 1 : (wave > F ? F : wave);
+  p->wave_c = wave;
+  p->wait_load = 1;
+  if ((long long)F * iterations <= kMaxOrder && F <= 4096 && iterations < 32768 && tu.order) {
+    int sms = 0;
+    if (int r = device_sms(&sms)) return r;
+    const int cap = tu.order_cap ? *tu.order_cap : (int)(1.6 * (2 * sms - kLoadReserve));
+    if (int r = streamed_order(F, iterations, wave, cap < 1 ? 1 : cap, &p->order)) return r;
+  }
+  return 0;
+}
+
+// Persistent fit: every EM iteration in one launch (em_persistent.cuh), then the last iteration's raw scatter sums
+// through cacg_update_kernel for the reference-exact model.  p carries the streamed-upload fields; load is the side
+// stream of a streamed upload (which has cleared the control block), else null.
+static int run_persistent_fit(const FitCall& c, PersistArgs p, bool full, bool fast_sm, const LoadStream* load,
+                              const Tuning& tu) {
+  const CacgmmWorkspace& ws = c.ws;
+  const pbb_cacgmm_options* opt = c.opt;
+  int r;
+  if (load == nullptr) PBB_CUDA(cudaMemsetAsync(ws.flags, 0, ws.control_bytes, c.st));
+  if (c.init_aff == nullptr && (r = launch_from_eig(ws, c.F, c.D, c.K, c.evec, c.eval, c.weight, c.st))) return r;
+  p.first_is_m = c.init_aff != nullptr;
+  p.user_model = c.init_aff == nullptr;
+  p.softmax_fast = fast_sm;
+  p.aff_in = c.init_aff; p.saliency = c.saliency; p.activity = c.activity;
+  p.aff_eps = opt->affiliation_eps; p.eigenvalue_floor = opt->eigenvalue_floor;
+  p.covariance_norm = opt->covariance_norm; p.weight_mode = opt->weight_mode;
+  p.dead = ws.dead;
+  if ((r = launch_planned(p, ws, c.D, c.K, c.dtype, full ? Persist::kFull : Persist::kLean, load != nullptr, tu,
+                          c.st)))
+    return r;
+  if (load != nullptr) PBB_CUDA(cudaStreamWaitEvent(c.st, load->join, 0));
+#ifdef PBB_PHASE_TIMING
+  print_phases(ws, (long long)c.F * opt->iterations, false, c.st);
+#endif
+  UpdArgs u = upd_args(ws, c.F, c.T, c.D, c.K, opt, c.saliency != nullptr, c.evec, c.eval, c.weight, c.status);
+  u.nch = 1;         // the last iteration's raw scatter sums -> reference-exact model
+  u.coef = nullptr;  // nobody reads the E-step form of the final model
+  return launch_update(cacg_update_kernel, "cacg_update_kernel", u, c.st);
+}
+
+// Per-iteration fit: one EM launch and one update launch per iteration.
+static int run_iterative_fit(const FitCall& c, bool fast_sm) {
+  const CacgmmWorkspace& ws = c.ws;
+  EmArgs a = em_args(ws, c.F, c.T, c.D, c.K);
+  a.activity = c.activity; a.aff_eps = c.opt->affiliation_eps; a.saliency = c.saliency;
+  UpdArgs u = upd_args(ws, c.F, c.T, c.D, c.K, c.opt, c.saliency != nullptr, c.evec, c.eval, c.weight, c.status);
+  int it = 0, r;
+  if (c.init_aff != nullptr) {
+    // iteration 0: M-step from the initial affiliations, q = 1 (cacgmm.py:206-228,269)
+    a.mode = kModeM; a.aff_in = c.init_aff; a.q_in = nullptr;
+    int nch = launch_em(a, c.dtype, c.opt->frames_per_block, c.st);
+    if (nch <= 0) return nch ? nch : 1;
+    u.nch = nch;
+    if ((r = launch_update(cacg_update_kernel, "cacg_update_kernel", u, c.st))) return r;
+    it = 1;
+  } else {
+    // warm start: the model in the output arrays drives the first E-step (cacgmm.py:229-234)
+    if ((r = launch_from_eig(ws, c.F, c.D, c.K, c.evec, c.eval, c.weight, c.st))) return r;
+  }
+  // the update kernel writes the E-step weights into `weight`; the E-step reads them from there
+  a.w = c.weight;
+  for (; it < c.opt->iterations; ++it) {
+    a.mode = kModeEM;
+    // a user-supplied model gives no bound on q / log det: keep the log-domain softmax for its E-step
+    a.softmax_fast = (fast_sm && !(c.init_aff == nullptr && it == 0)) ? 1 : 0;
+    if (c.init_aff == nullptr && it == 0) a.w = ws.w;
+    int nch = launch_em(a, c.dtype, c.opt->frames_per_block, c.st);
+    if (nch <= 0) return nch ? nch : 1;
+    a.w = c.weight;
+    u.nch = nch;
+    if ((r = launch_update(cacg_update_kernel, "cacg_update_kernel", u, c.st))) return r;
+  }
   return 0;
 }
 
@@ -734,8 +873,10 @@ int pbb_normalize_observation(const void* y, void* z, int F, int T, int D, int d
   PBB_CHECK_ARG(D > 0 && D < 256, 5, "bad D");
   PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 6, "bad dtype");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return dtype == PBB_C128 ? launch_normalize<double2>(y, z, F, T, D, swap, T, st)
-                           : launch_normalize<float2>(y, z, F, T, D, swap, T, st);
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_normalize(static_cast<const CT*>(y), static_cast<CT*>(z), F, T, D, swap, T, st);
+  });
 }
 
 int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms, int* kernel, int* split) {
@@ -746,7 +887,7 @@ int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms,
   PBB_CHECK_ARG(sms > 0, 7, "sms must be positive");
   PBB_CHECK_ARG(kernel != nullptr && split != nullptr, 8, "output is null");
   const int clusters[3] = {2 * sms, sms, sms / 2};  // machine model: two CTAs per SM, clusters placed anywhere
-  const FitPlan plan = plan_persistent_fit(F, T, D, K, lean != 0, streamed != 0, sms, clusters, PlanOverrides{});
+  const FitPlan plan = plan_persistent_fit(F, T, D, K, lean != 0, streamed != 0, sms, clusters, Tuning{});
   *kernel = plan.kernel;
   *split = plan.split;
   return 0;
@@ -780,222 +921,39 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
   PBB_CHECK_ARG(opt->covariance_norm >= 0 && opt->covariance_norm <= 2, 10, "bad covariance_norm");
   PBB_CHECK_ARG(opt->weight_mode == PBB_WEIGHT_TIME || opt->weight_mode == PBB_WEIGHT_CONST, 10, "bad weight_mode");
   PBB_CHECK_ARG(eigenvectors && eigenvalues && weight, 11, "model output is null");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 14,
-                "workspace too small (pbb_cacgmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 16, "status is null");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  const bool persistent = fast_shape(D, K) && !(opt->reserved & 1);
+  FitCall c{y, dtype, F, T, D, K, init_aff, saliency, activity, opt, eigenvectors, eigenvalues, weight, status,
+            reinterpret_cast<cudaStream_t>(stream)};
   int r;
-  // y (and the initial affiliations) may be pinned host memory: the kernels then read them in
-  // place over PCIe.  On the persistent path with an affiliation initialisation that read is a
-  // separate small kernel on a side stream that overlaps the EM kernel ("streamed upload").
-  bool y_host = false, aff_host = false;
-  if ((r = classify_pointer(y, &y, &y_host, "y"))) return r;
-  if (init_aff != nullptr) {
-    const void* alias = nullptr;
-    if ((r = classify_pointer(init_aff, &alias, &aff_host, "initial affiliations"))) return r;
-    init_aff = static_cast<const double*>(alias);
-  }
-  // the model may be written straight into pinned host memory as well (write-only on this path)
-  {
-    bool h = false;
-    const void* alias = nullptr;
-    if ((r = classify_pointer(eigenvectors, &alias, &h, "eigenvectors"))) return r;
-    eigenvectors = const_cast<void*>(alias);
-    if ((r = classify_pointer(eigenvalues, &alias, &h, "eigenvalues"))) return r;
-    eigenvalues = static_cast<double*>(const_cast<void*>(alias));
-    if ((r = classify_pointer(weight, &alias, &h, "weight"))) return r;
-    weight = static_cast<double*>(const_cast<void*>(alias));
-  }
-  const bool streamed = persistent && y_host && init_aff != nullptr && !(opt->reserved & 2) &&
-                        ws.aff_stage != nullptr;
+  if ((r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 14,
+                      "workspace too small (pbb_cacgmm_workspace_bytes)", status, Layout::kNone, c.st, &c.ws)))
+    return r;
+  if ((r = resolve_host_aliases(c))) return r;
+  const bool persistent = fast_shape(D, K) && !(opt->reserved & 1);
   const bool fast_sm = softmax_fast_ok(D, opt);
+  if (!persistent) {
+    if ((r = normalize(c.y, dtype, c.ws, F, T, D, false, c.st))) return r;
+    return run_iterative_fit(c, fast_sm);
+  }
+  const bool streamed = c.y_host && c.init_aff != nullptr && !(opt->reserved & 2);
   // lean variant: product-form softmax, needs (K-1) D log10(1/floor) < 290 (em_persistent.cuh).  The extra decade
   // per factor below is a margin kept as is: without it some fits (e.g. K = 4, D = 8 with floors between about 1e-12
   // and 1e-11) would move from the full variant to the lean one.
   const bool lean_ok = fast_sm && (K - 1) * D * (log10(1.0 / opt->eigenvalue_floor) + 1.0) < 290.0;
-  const bool full = saliency != nullptr || activity != nullptr || !lean_ok || init_aff == nullptr;
+  const bool full = saliency != nullptr || activity != nullptr || !lean_ok || c.init_aff == nullptr;
+  const Tuning tu = read_tuning();
+  PersistArgs p = persist_args(c.ws, F, T, opt->iterations, status);
+  if (!streamed) {
+    if ((r = normalize(c.y, dtype, c.ws, F, T, D, true, c.st))) return r;
+    return run_persistent_fit(c, p, full, fast_sm, nullptr, tu);
+  }
   // Thread safety: the side stream and the fork / join events of the streamed upload exist once per device, so two
   // host threads enqueueing streamed fits on the same device are serialised from here to the end of the call
   // (the enqueue only; the GPU work of the two fits still overlaps as far as their streams allow).
-  std::unique_lock<std::mutex> stream_lock;
-  if (streamed) {
-    LoadStream* lsm = nullptr;
-    if ((r = get_load_stream(&lsm))) return r;
-    stream_lock = std::unique_lock<std::mutex>(lsm->mu);
-  }
-  if (streamed) {
-    // flags[bin] = -1 until the bin has arrived
-    PBB_CUDA(cudaMemsetAsync(ws.flags, 0, (size_t)(F + 1) * sizeof(int) + 16 * sizeof(unsigned long long) + 8, st));
-    PBB_CUDA(cudaMemsetAsync(ws.flags, 0xFF, (size_t)F * sizeof(int), st));
-    PBB_CUDA(cudaMemsetAsync(ws.dead, 0, (size_t)F * sizeof(int), st));
-    LoadStream* l = nullptr;
-    if ((r = get_load_stream(&l))) return r;
-    PBB_CUDA(cudaEventRecord(l->fork, st));
-    PBB_CUDA(cudaStreamWaitEvent(l->stream, l->fork, 0));
-    double* aff_dst = aff_host ? ws.aff_stage : nullptr;
-    int* next_bin = reinterpret_cast<int*>(ws.phase + 15);
-    int* started = reinterpret_cast<int*>(ws.phase + 14);
-    int ctas = 0;
-    r = dtype == PBB_C128
-            ? launch_stream_load<double2>(y, ws.z, init_aff, aff_dst, F, T, D, K, ws.dead, ws.flags, next_bin, started, &ctas, l->stream)
-            : launch_stream_load<float2>(y, ws.z, init_aff, aff_dst, F, T, D, K, ws.dead, ws.flags, next_bin, started, &ctas, l->stream);
-    if (r) return r;
-    PBB_CUDA(cudaEventRecord(l->join, l->stream));
-    // Hold the EM kernel back until every loader CTA runs: launched at the same moment, the EM grid
-    // could take the whole machine first and leave the loader only the reserved slots (it would still
-    // finish -- bins are handed out by a counter -- but at a fraction of the link rate).
-    if (l->wait_value != nullptr) {
-      if (l->wait_value(reinterpret_cast<CUstream>(st), reinterpret_cast<CUdeviceptr>(started), (cuuint32_t)ctas,
-                        CU_STREAM_WAIT_VALUE_GEQ) != CUDA_SUCCESS)
-        l->wait_value = nullptr;  // not supported here: rely on the reserved slots
-    }
-    if (aff_host) init_aff = ws.aff_stage;
-  } else if (persistent)  // chunk-major staged layout: one TMA bulk copy per ring stage
-    r = dtype == PBB_C128 ? launch_normalize_staged<double2>(y, ws.z, F, T, D, ws.dead, st)
-                          : launch_normalize_staged<float2>(y, ws.z, F, T, D, ws.dead, st);
-  else
-    r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                          : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
-
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
-  a.coef = ws.coef; a.ld = ws.ld; a.w = ws.w; a.ew = ws.ew;
-  a.activity = activity; a.aff_eps = opt->affiliation_eps;
-  a.saliency = saliency; a.part = ws.part;
-
-  UpdArgs u;
-  memset(&u, 0, sizeof(u));
-  u.F = F; u.T = T; u.D = D; u.K = K;
-  u.part = ws.part;
-  u.covariance_norm = opt->covariance_norm;
-  u.weight_mode = opt->weight_mode;
-  u.has_saliency = saliency != nullptr;
-  u.eigenvalue_floor = opt->eigenvalue_floor;
-  u.evec = reinterpret_cast<double2*>(eigenvectors);
-  u.eval = eigenvalues; u.weight = weight;
-  u.coef = ws.coef; u.ld = ws.ld; u.ew = ws.ew;
-  u.status = status;
-
-  if (persistent) {
-    // ---- persistent path: every EM iteration in one launch (em_persistent.cuh) ----
-    if (!streamed)
-      PBB_CUDA(cudaMemsetAsync(ws.flags, 0, (size_t)(F + 1) * sizeof(int) + 16 * sizeof(unsigned long long) + 8, st));
-    if (init_aff == nullptr) {
-      FromEigArgs fe;
-      fe.F = F; fe.D = D; fe.K = K;
-      fe.evec = reinterpret_cast<const double2*>(eigenvectors);
-      fe.eval = eigenvalues; fe.weight = weight;
-      fe.coef = ws.coef; fe.ld = ws.ld; fe.w = ws.w; fe.ew = ws.ew;
-      if ((r = launch_from_eig(fe, st))) return r;
-    }
-    PersistArgs p;
-    memset(&p, 0, sizeof(p));
-    p.z = ws.z; p.zs = ws.zs; p.F = F; p.T = T;
-    p.iterations = opt->iterations;
-    p.first_is_m = init_aff != nullptr;
-    p.user_model = init_aff == nullptr;
-    p.softmax_fast = fast_sm;
-    p.aff_in = init_aff; p.saliency = saliency; p.activity = activity;
-    p.aff_eps = opt->affiliation_eps; p.eigenvalue_floor = opt->eigenvalue_floor;
-    p.covariance_norm = opt->covariance_norm; p.weight_mode = opt->weight_mode;
-    p.coef = ws.coef; p.ld = ws.ld; p.w = ws.w; p.ew = ws.ew;
-    p.part = ws.part; p.flags = ws.flags; p.ticket = ws.ticket; p.status = status;
-    p.phase = ws.phase; p.dead = ws.dead;
-    if (streamed) {
-      // bins joining per slot ~ slot duration / arrival time of one bin at ~50 GB/s of PCIe reads
-      const double bin_bytes = (double)T * D * (dtype == PBB_C128 ? 16.0 : 8.0) + (aff_host ? 8.0 * K * T : 0.0);
-      // one slot of the order table = one link of a bin's dependency chain (task + update + staging
-      // of the next model, ~23 us at D = 8, K = 3, T = 500), during which the machine runs ~1.6 tasks per CTA
-      const double round_us = 23.0 * (T / 500.0) * (D * D / 64.0) * (K / 3.0);
-      int c = (int)(round_us / (bin_bytes / 50e3) + 0.5);
-      if (const char* e = getenv("PBB_WAVE_C")) c = atoi(e);  // tuning override
-      c = c < 1 ? 1 : (c > F ? F : c);
-      p.wave_c = c;
-      p.wait_load = 1;
-      const long long tasks = (long long)F * opt->iterations;
-      if (tasks <= kMaxOrder && F <= 4096 && opt->iterations < 32768 && !getenv("PBB_NO_ORDER")) {
-        int dev = 0, sms = 0;
-        PBB_CUDA(cudaGetDevice(&dev));
-        PBB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        int cap = (int)(1.6 * (2 * sms - kLoadReserve));
-        if (const char* e = getenv("PBB_ORDER_CAP")) cap = atoi(e);  // tuning override
-        if ((r = streamed_order(F, opt->iterations, c, cap < 1 ? 1 : cap, &p.order))) return r;
-      }
-    }
-    const PlanOverrides ov = env_overrides();
-    int clusters[3] = {0, 0, 0}, sms = 0;
-    if (sticky_eligible(D, !full, streamed, ov) && (r = sticky_clusters(K, dtype, clusters, st))) return r;
-    if ((r = device_sms(&sms))) return r;
-    const FitPlan plan = plan_persistent_fit(F, T, D, K, !full, streamed, sms, clusters, ov);
-    if (plan.kernel == kKernelSticky) {
-      if ((r = launch_sticky(p, K, dtype, plan.split, st))) return r;  // few bins: one cluster per bin (em_sticky.cuh)
-    } else {
-      if ((r = setup_frame_split(&p, ws, F, D, K, plan.split, st))) return r;
-      if ((r = launch_persist(p, D, K, dtype, full, plan.kernel == kKernelWs, st))) return r;
-    }
-    if (streamed) {
-      LoadStream* l = nullptr;
-      if ((r = get_load_stream(&l))) return r;
-      PBB_CUDA(cudaStreamWaitEvent(st, l->join, 0));
-    }
-#ifdef PBB_PHASE_TIMING
-    {
-      unsigned long long ph[16];
-      cudaStreamSynchronize(st);
-      cudaMemcpy(ph, ws.phase, sizeof(ph), cudaMemcpyDeviceToHost);
-      fprintf(stderr, "[phase] update of class 0, cycles per task: build %.0f  gauss-jordan %.0f  logdet/tinv %.0f  stores %.0f\n",
-              ph[8] / (double)((size_t)F * opt->iterations), ph[9] / (double)((size_t)F * opt->iterations),
-              ph[10] / (double)((size_t)F * opt->iterations), ph[11] / (double)((size_t)F * opt->iterations));
-      fprintf(stderr, "[phase] producer, cycles per task: ticket->dependency %.0f  model buffer wait %.0f  model issue %.0f  ring refill %.0f\n",
-              ph[12] / (double)((size_t)F * opt->iterations), ph[13] / (double)((size_t)F * opt->iterations),
-              ph[14] / (double)((size_t)F * opt->iterations), ph[15] / (double)((size_t)F * opt->iterations));
-      unsigned long long tot = 0;
-      for (int i = 0; i < 8; ++i) tot += ph[i];
-      static const char* nm[8] = {"ticket+flag / model wait", "chunk-top / updater busy", "tma-wait", "em-steps", "reduce", "update / S wait", "publish / hand-over", "task-start / updater idle"};
-      for (int i = 0; i < 8; ++i) fprintf(stderr, "[phase] %-20s %6.2f%%  %8.0f cycles per task\n", nm[i], 100.0 * ph[i] / (double)tot, ph[i] / (double)((size_t)F * opt->iterations));
-    }
-#endif
-    u.nch = 1;  // the last iteration's raw scatter sums -> reference-exact model
-    u.coef = nullptr;  // nobody reads the E-step form of the final model
-    return launch_update(u, st);
-  }
-  int it = 0;
-  if (init_aff != nullptr) {
-    // iteration 0: M-step from the initial affiliations, q = 1 (cacgmm.py:206-228,269)
-    a.mode = kModeM; a.aff_in = init_aff; a.q_in = nullptr;
-    int nch = launch_em(a, dtype, opt->frames_per_block, st);
-    if (nch <= 0) return nch ? nch : 1;
-    u.nch = nch;
-    if ((r = launch_update(u, st))) return r;
-    it = 1;
-  } else {
-    // warm start: the model in the output arrays drives the first E-step (cacgmm.py:229-234)
-    FromEigArgs fe;
-    fe.F = F; fe.D = D; fe.K = K;
-    fe.evec = reinterpret_cast<const double2*>(eigenvectors);
-    fe.eval = eigenvalues; fe.weight = weight;
-    fe.coef = ws.coef; fe.ld = ws.ld; fe.w = ws.w; fe.ew = ws.ew;
-    if ((r = launch_from_eig(fe, st))) return r;
-  }
-  // the update kernel writes the E-step weights into `weight`; the E-step reads them from there
-  a.w = weight;
-  for (; it < opt->iterations; ++it) {
-    a.mode = kModeEM;
-    // a user-supplied model gives no bound on q / log det: keep the log-domain softmax for its E-step
-    a.softmax_fast = (fast_sm && !(init_aff == nullptr && it == 0)) ? 1 : 0;
-    if (init_aff == nullptr && it == 0) a.w = ws.w;
-    int nch = launch_em(a, dtype, opt->frames_per_block, st);
-    if (nch <= 0) return nch ? nch : 1;
-    a.w = weight;
-    u.nch = nch;
-    if ((r = launch_update(u, st))) return r;
-  }
-  return 0;
+  LoadStream* load = nullptr;
+  if ((r = get_load_stream(&load))) return r;
+  std::lock_guard<std::mutex> stream_lock(load->mu);
+  if ((r = start_streamed_upload(c, *load, tu, &p))) return r;
+  return run_persistent_fit(c, p, full, fast_sm, load, tu);
 }
 
 int pbb_cacgmm_predict(const void* y, int dtype, int F, int T, int D, int K, const void* eigenvectors,
@@ -1007,29 +965,18 @@ int pbb_cacgmm_predict(const void* y, int dtype, int F, int T, int D, int K, con
   PBB_CHECK_ARG(eigenvectors && eigenvalues, 7, "model is null");
   PBB_CHECK_ARG(weight != nullptr || weight_mode == PBB_WEIGHT_CONST, 9, "weight is null");
   PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_TIED, 10, "bad weight_mode");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 16,
-                "workspace too small (pbb_cacgmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 18, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
-  FromEigArgs fe;
-  fe.F = F; fe.D = D; fe.K = K;
-  fe.evec = reinterpret_cast<const double2*>(eigenvectors);
-  fe.eval = eigenvalues;
+  CacgmmWorkspace ws;
+  int r;
+  if ((r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 16,
+                      "workspace too small (pbb_cacgmm_workspace_bytes)", status, Layout::kPlain, st, &ws)))
+    return r;
   const bool tied = weight_mode == PBB_WEIGHT_TIED_TIME || weight_mode == PBB_WEIGHT_TIED;
-  fe.weight = (weight_mode == PBB_WEIGHT_CONST || tied) ? nullptr : weight;
-  fe.coef = ws.coef; fe.ld = ws.ld; fe.w = ws.w; fe.ew = ws.ew;
-  if ((r = launch_from_eig(fe, st))) return r;
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
-  a.mode = kModeE; a.softmax_fast = 0;
+  const double* w = (weight_mode == PBB_WEIGHT_CONST || tied) ? nullptr : weight;
+  if ((r = launch_from_eig(ws, F, D, K, eigenvectors, eigenvalues, w, st))) return r;
+  EmArgs a = em_args(ws, F, T, D, K);
+  a.mode = kModeE;
   if (tied) { a.w_time = weight; a.w_time_st = weight_mode == PBB_WEIGHT_TIED_TIME ? 1 : 0; }
-  a.coef = ws.coef; a.ld = ws.ld; a.w = ws.w; a.ew = ws.ew;
   a.activity = activity; a.aff_eps = affiliation_eps;
   a.aff_out = affiliation; a.q_out = quadratic;
   a.loglik_part = loglik ? ws.loglik_part : nullptr;
@@ -1052,35 +999,19 @@ int pbb_cacgmm_mstep(const void* y, int dtype, int F, int T, int D, int K, const
   PBB_CHECK_ARG(affiliation != nullptr, 7, "affiliation is null");
   PBB_CHECK_ARG(opt != nullptr, 10, "options are null");
   PBB_CHECK_ARG(eigenvectors && eigenvalues && weight, 11, "model output is null");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 14,
-                "workspace too small (pbb_cacgmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 16, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  CacgmmWorkspace ws;
+  if (int r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 14,
+                         "workspace too small (pbb_cacgmm_workspace_bytes)", status, Layout::kPlain, st, &ws))
+    return r;
+  EmArgs a = em_args(ws, F, T, D, K);
   a.mode = kModeM; a.aff_in = affiliation; a.q_in = quadratic;
-  a.saliency = saliency; a.part = ws.part;
+  a.saliency = saliency;
   int nch = launch_em(a, dtype, opt->frames_per_block, st);
   if (nch <= 0) return nch ? nch : 1;
-  UpdArgs u;
-  memset(&u, 0, sizeof(u));
-  u.F = F; u.T = T; u.D = D; u.K = K; u.nch = nch;
-  u.part = ws.part;
-  u.covariance_norm = opt->covariance_norm;
-  u.weight_mode = opt->weight_mode;
-  u.has_saliency = saliency != nullptr;
-  u.eigenvalue_floor = opt->eigenvalue_floor;
-  u.evec = reinterpret_cast<double2*>(eigenvectors);
-  u.eval = eigenvalues; u.weight = weight;
-  u.coef = ws.coef; u.ld = ws.ld; u.ew = ws.ew;
-  u.status = status;
-  return launch_update(u, st);
+  UpdArgs u = upd_args(ws, F, T, D, K, opt, saliency != nullptr, eigenvectors, eigenvalues, weight, status);
+  u.nch = nch;
+  return launch_update(cacg_update_kernel, "cacg_update_kernel", u, st);
 }
 
 size_t pbb_cwmm_workspace_bytes(int F, int T, int D, int K) { return pbb_cacgmm_workspace_bytes(F, T, D, K); }
@@ -1097,27 +1028,18 @@ int pbb_cwmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
   PBB_CHECK_ARG(weight_mode == PBB_WEIGHT_TIME || weight_mode == PBB_WEIGHT_CONST, 10, "bad weight_mode");
   PBB_CHECK_ARG(spline_t && spline_c && spline_n >= 3, 11, "spline table is missing");
   PBB_CHECK_ARG(mode && concentration && weight, 15, "model output is null");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 18,
-                "workspace too small (pbb_cwmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 20, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
   const bool persistent = fast_shape(D, K) && saliency == nullptr;
+  CacgmmWorkspace ws;
   int r;
-  if (persistent)
-    r = dtype == PBB_C128 ? launch_normalize_staged<double2>(y, ws.z, F, T, D, ws.dead, st)
-                          : launch_normalize_staged<float2>(y, ws.z, F, T, D, ws.dead, st);
-  else
-    r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                          : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  if ((r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 18,
+                      "workspace too small (pbb_cwmm_workspace_bytes)", status,
+                      persistent ? Layout::kStaged : Layout::kPlain, st, &ws)))
+    return r;
+  EmArgs a = em_args(ws, F, T, D, K);
   a.model_kind = 1;
-  a.coef = ws.coef; a.ld = ws.ld; a.w = weight; a.ew = ws.ew;
-  a.saliency = saliency; a.part = ws.part;
+  a.w = weight;
+  a.saliency = saliency;
   CwUpdArgs u;
   memset(&u, 0, sizeof(u));
   u.F = F; u.T = T; u.D = D; u.K = K;
@@ -1130,35 +1052,17 @@ int pbb_cwmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
   if (persistent) {
     // every EM iteration in one launch (em_persistent.cuh, MODEL = 1); the last iteration's raw
     // scatter sums go through cw_update_kernel for the reference-exact mode / concentration / weight
-    PBB_CUDA(cudaMemsetAsync(ws.flags, 0, (size_t)(F + 1) * sizeof(int) + 16 * sizeof(unsigned long long) + 8, st));
-    PersistArgs p;
-    memset(&p, 0, sizeof(p));
-    p.z = ws.z; p.zs = ws.zs; p.F = F; p.T = T;
-    p.iterations = iterations; p.first_is_m = 1; p.user_model = 0; p.softmax_fast = 0;
-    p.aff_in = init_aff; p.aff_eps = 0.0; p.weight_mode = weight_mode;
-    p.coef = ws.coef; p.ld = ws.ld; p.w = ws.w; p.ew = ws.ew;
-    p.part = ws.part; p.flags = ws.flags; p.ticket = ws.ticket; p.status = status; p.phase = ws.phase;
+    PBB_CUDA(cudaMemsetAsync(ws.flags, 0, ws.control_bytes, st));
+    PersistArgs p = persist_args(ws, F, T, iterations, status);
+    p.first_is_m = 1;
+    p.aff_in = init_aff; p.weight_mode = weight_mode;
     p.spline = u.spline;
-    PlanOverrides ov = env_overrides();
-    ov.single = true;
-    int sms = 0;
-    if ((r = device_sms(&sms))) return r;
-    const FitPlan plan = plan_persistent_fit(F, T, D, K, true, false, sms, nullptr, ov);
-    if ((r = setup_frame_split(&p, ws, F, D, K, plan.split, st))) return r;
-    if ((r = launch_persist_cw(p, D, K, dtype, st))) return r;
+    if ((r = launch_planned(p, ws, D, K, dtype, Persist::kCw, false, read_tuning(), st))) return r;
 #ifdef PBB_PHASE_TIMING
-    {
-      unsigned long long ph[16];
-      cudaStreamSynchronize(st);
-      cudaMemcpy(ph, ws.phase, sizeof(ph), cudaMemcpyDeviceToHost);
-      unsigned long long tot = 0;
-      for (int i = 0; i < 8; ++i) tot += ph[i];
-      static const char* nm[8] = {"flag wait", "chunk top / staging", "tma-wait", "em-steps", "reduce", "update (jacobi)", "publish", "task-start"};
-      for (int i = 0; i < 8; ++i) fprintf(stderr, "[phase cw] %-20s %6.2f%%  %8.0f cycles per task\n", nm[i], 100.0 * ph[i] / (double)tot, ph[i] / (double)((size_t)F * iterations));
-    }
+    print_phases(ws, (long long)F * iterations, true, st);
 #endif
     u.nch = 1;
-    return launch_cw_update(u, st);
+    return launch_update(cw_update_kernel, "cw_update_kernel", u, st);
   }
   for (int it = 0; it < iterations; ++it) {
     if (it == 0) { a.mode = kModeM; a.aff_in = init_aff; a.q_in = nullptr; }
@@ -1166,7 +1070,7 @@ int pbb_cwmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
     int nch = launch_em(a, dtype, 0, st);
     if (nch <= 0) return nch ? nch : 1;
     u.nch = nch;
-    if ((r = launch_cw_update(u, st))) return r;
+    if ((r = launch_update(cw_update_kernel, "cw_update_kernel", u, st))) return r;
   }
   return 0;
 }
@@ -1180,31 +1084,22 @@ int pbb_cwmm_predict(const void* y, int dtype, int F, int T, int D, int K, const
   PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_TIED, 10, "bad weight_mode");
   PBB_CHECK_ARG(weight != nullptr || weight_mode == PBB_WEIGHT_CONST, 9, "weight is null");
   PBB_CHECK_ARG(affiliation != nullptr, 11, "affiliation output is null");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 12,
-                "workspace too small (pbb_cwmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 14, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
+  CacgmmWorkspace ws;
+  int r;
+  if ((r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 12,
+                      "workspace too small (pbb_cwmm_workspace_bytes)", status, Layout::kPlain, st, &ws)))
+    return r;
   CwFromModelArgs fm;
   fm.F = F; fm.D = D; fm.K = K;
   const bool tied = weight_mode == PBB_WEIGHT_TIED_TIME || weight_mode == PBB_WEIGHT_TIED;
   fm.mode = reinterpret_cast<const double2*>(mode); fm.concentration = concentration;
   fm.weight = (tied || weight_mode == PBB_WEIGHT_CONST) ? nullptr : weight;
   fm.coef = ws.coef; fm.ld = ws.ld; fm.ew = ws.ew; fm.w = ws.w;
-  {
-    LaunchScope ls("cw_from_model_kernel", st);
-    cw_from_model_kernel<<<F, 128, (size_t)D * D * sizeof(int), st>>>(fm);
-    PBB_CUDA(cudaGetLastError());
-  }
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  if ((r = launch_kernel("cw_from_model_kernel", cw_from_model_kernel, F, 128, (size_t)D * D * sizeof(int), st, fm)))
+    return r;
+  EmArgs a = em_args(ws, F, T, D, K);
   a.mode = kModeE; a.model_kind = 1;
-  a.coef = ws.coef; a.ld = ws.ld; a.w = ws.w; a.ew = ws.ew;
   if (tied) { a.w_time = weight; a.w_time_st = weight_mode == PBB_WEIGHT_TIED_TIME ? 1 : 0; }
   a.aff_out = affiliation;
   int nch = launch_em(a, dtype, 0, st);
@@ -1225,21 +1120,16 @@ int pbb_cbmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
   PBB_CHECK_ARG(affiliation_eps >= 0.0 && affiliation_eps < 0.5, 11, "need 0 <= affiliation_eps < 0.5");
   PBB_CHECK_ARG(max_concentration > 0.0, 13, "max_concentration must be positive (complex_bingham.py:221)");
   PBB_CHECK_ARG(eigenvectors && eigenvalues && weight, 14, "model output is null");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 17,
-                "workspace too small (pbb_cbmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 19, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  CacgmmWorkspace ws;
+  int r;
+  if ((r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 17,
+                      "workspace too small (pbb_cbmm_workspace_bytes)", status, Layout::kPlain, st, &ws)))
+    return r;
+  EmArgs a = em_args(ws, F, T, D, K);
   a.model_kind = 1;  // lp = ew q - ld with ew = -1, q = y^H (-B) y
-  a.coef = ws.coef; a.ld = ws.ld; a.w = weight; a.ew = ws.ew;
-  a.saliency = saliency; a.part = ws.part; a.aff_eps = affiliation_eps;
+  a.w = weight;
+  a.saliency = saliency; a.aff_eps = affiliation_eps;
   CbUpdArgs u;
   memset(&u, 0, sizeof(u));
   u.F = F; u.T = T; u.K = K;
@@ -1255,7 +1145,11 @@ int pbb_cbmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
     if (nch <= 0) return nch ? nch : 1;
     u.nch = nch;
     u.coef = it + 1 < iterations ? ws.coef : nullptr;  // nobody reads the E-step form of the final model
-    if ((r = bingham_dispatch<CbUpdateLaunch>(D, u, st))) return r;
+    if ((r = with_bingham_d(D, [&](auto d) {
+           return launch_kernel("cb_update_kernel", cb_update_kernel<decltype(d)::value>, u.F, 32 * kCbWarps, 0, st,
+                                u);
+         })))
+      return r;
   }
   return 0;
 }
@@ -1270,27 +1164,25 @@ int pbb_cbmm_predict(const void* y, int dtype, int F, int T, int D, int K, const
   PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_TIED, 10, "bad weight_mode");
   PBB_CHECK_ARG(affiliation_eps >= 0.0 && affiliation_eps < 0.5, 11, "need 0 <= affiliation_eps < 0.5");
   PBB_CHECK_ARG(affiliation != nullptr, 12, "affiliation output is null");
-  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_cacgmm_workspace_bytes(F, T, D, K), 13,
-                "workspace too small (pbb_cbmm_workspace_bytes)");
-  PBB_CHECK_ARG(status != nullptr, 15, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  CacgmmWorkspace ws = carve(workspace, F, T, D, K);
-  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  int r = dtype == PBB_C128 ? launch_normalize<double2>(y, ws.z, F, T, D, 1, ws.zs, st)
-                            : launch_normalize<float2>(y, ws.z, F, T, D, 1, ws.zs, st);
-  if (r) return r;
+  CacgmmWorkspace ws;
+  int r;
+  if ((r = begin_call(y, dtype, F, T, D, K, workspace, workspace_bytes, 13,
+                      "workspace too small (pbb_cbmm_workspace_bytes)", status, Layout::kPlain, st, &ws)))
+    return r;
   const bool tied = weight_mode == PBB_WEIGHT_TIED_TIME || weight_mode == PBB_WEIGHT_TIED;
   CbFromModelArgs fm;
   fm.F = F; fm.K = K;
   fm.evec = reinterpret_cast<const double2*>(eigenvectors); fm.eval = eigenvalues;
   fm.weight = (tied || weight_mode == PBB_WEIGHT_CONST) ? nullptr : weight;
   fm.coef = ws.coef; fm.ld = ws.ld; fm.ew = ws.ew; fm.w = ws.w;
-  if ((r = bingham_dispatch<CbFromModelLaunch>(D, fm, st))) return r;
-  EmArgs a;
-  memset(&a, 0, sizeof(a));
-  a.z = ws.z; a.zs = ws.zs; a.F = F; a.T = T; a.D = D; a.K = K;
+  if ((r = with_bingham_d(D, [&](auto d) {
+         return launch_kernel("cb_from_model_kernel", cb_from_model_kernel<decltype(d)::value>, F, 32 * kCbWarps, 0,
+                              st, fm);
+       })))
+    return r;
+  EmArgs a = em_args(ws, F, T, D, K);
   a.mode = kModeE; a.model_kind = 1;
-  a.coef = ws.coef; a.ld = ws.ld; a.w = ws.w; a.ew = ws.ew;
   if (tied) { a.w_time = weight; a.w_time_st = weight_mode == PBB_WEIGHT_TIED_TIME ? 1 : 0; }
   a.aff_eps = affiliation_eps;
   a.aff_out = affiliation;
@@ -1308,8 +1200,10 @@ int pbb_bingham_parameters(const double* scatter_eigenvalues, int n, int D, doub
   PBB_CHECK_ARG(status != nullptr, 7, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  return bingham_dispatch<BinghamParametersLaunch>(D, scatter_eigenvalues, n, eps, max_concentration, eigenvalues,
-                                                   status, st);
+  return with_bingham_d(D, [&](auto d) {
+    return launch_kernel("bingham_parameters_kernel", bingham_parameters_kernel<decltype(d)::value>, (n + 3) / 4, 128,
+                         0, st, scatter_eigenvalues, n, eps, max_concentration, eigenvalues, status);
+  });
 }
 
 int pbb_bingham_log_norm(const double* eigenvalues, int n, int D, double eps, double* log_norm, void* stream) {
@@ -1318,7 +1212,10 @@ int pbb_bingham_log_norm(const double* eigenvalues, int n, int D, double eps, do
   PBB_CHECK_ARG(D >= 2 && D <= 6, 3, "complex Bingham: need 2 <= D <= 6 (complex_bingham_utils.py:342-348)");
   PBB_CHECK_ARG(log_norm != nullptr, 5, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return bingham_dispatch<BinghamLogNormLaunch>(D, eigenvalues, n, eps, log_norm, st);
+  return with_bingham_d(D, [&](auto d) {
+    return launch_kernel("bingham_log_norm_kernel", bingham_log_norm_kernel<decltype(d)::value>, (n + 127) / 128, 128,
+                         0, st, eigenvalues, n, eps, log_norm);
+  });
 }
 
 int pbb_bingham_log_pdf(const void* y, int dtype, int M, int T, int D, const void* eigenvectors,
@@ -1333,15 +1230,11 @@ int pbb_bingham_log_pdf(const void* y, int dtype, int M, int T, int D, const voi
   const long long n = (long long)M * T;
   const unsigned blocks = (unsigned)((n + 127) / 128);
   const double2* V = static_cast<const double2*>(eigenvectors);
-  LaunchScope ls("bingham_log_pdf_kernel", st);
-  if (dtype == PBB_C128)
-    bingham_log_pdf_kernel<double2><<<blocks, 128, 0, st>>>(static_cast<const double2*>(y), V, eigenvalues, log_norm,
-                                                            M, T, D, log_pdf);
-  else
-    bingham_log_pdf_kernel<float2><<<blocks, 128, 0, st>>>(static_cast<const float2*>(y), V, eigenvalues, log_norm,
-                                                           M, T, D, log_pdf);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_kernel("bingham_log_pdf_kernel", bingham_log_pdf_kernel<CT>, blocks, 128, 0, st,
+                         static_cast<const CT*>(y), V, eigenvalues, log_norm, M, T, D, log_pdf);
+  });
 }
 
 int pbb_mixture_weight_over_bins(const double* affiliation, int F, int K, int T, int flags, double* weight_kt,

@@ -876,22 +876,10 @@ int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan
                                  : K == 4 ? dhtv_cluster_kernel<4> : dhtv_cluster_kernel<0>;
         PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         if (C > 8) PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        cudaLaunchConfig_t cfg;
-        memset(&cfg, 0, sizeof(cfg));
-        cfg.gridDim = dim3(C);
-        cfg.blockDim = dim3(kDhtvClThreads);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = C;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1;
+        const ClusterLaunch cl(C, kDhtvClThreads, smem, C, st);
         if (cluster_ctas < 0) {
           int nclusters = 0;
-          if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cfg) != cudaSuccess || nclusters < 1) {
+          if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cl.cfg) != cudaSuccess || nclusters < 1) {
             (void)cudaGetLastError();
             if (C == 8) cluster_ctas = 0;
             continue;  // try the portable size
@@ -900,7 +888,7 @@ int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan
         }
         LaunchScope ls("dhtv_cluster_kernel", st);
         const int* plan_c = plan_dev;
-        PBB_CUDA(cudaLaunchKernelEx(&cfg, kern, features, plan_c, nplan, K, F, T, mapping, metric, algorithm));
+        PBB_CUDA(cudaLaunchKernelEx(&cl.cfg, kern, features, plan_c, nplan, K, F, T, mapping, metric, algorithm));
 #ifdef PBB_PHASE_TIMING
         {
           unsigned long long ph[8], zero[8] = {0};

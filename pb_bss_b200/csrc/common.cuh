@@ -31,6 +31,28 @@ int cuda_fail(cudaError_t e, const char* what);
     if (_e != cudaSuccess) return ::pbb::cuda_fail(_e, #call);\
   } while (0)
 
+// ---- thread-block cluster launch (host) ----------------------------------------
+// Configuration of a 1-D grid launched in clusters of `cluster` CTAs, for cudaLaunchKernelEx and
+// cudaOccupancyMaxActiveClusters.  cfg points at attr, so the object is not copied.
+struct ClusterLaunch {
+  cudaLaunchConfig_t cfg{};
+  cudaLaunchAttribute attr{};
+  ClusterLaunch(unsigned ctas, unsigned threads, size_t smem, unsigned cluster, cudaStream_t st) {
+    cfg.gridDim = dim3(ctas);
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cluster;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+  }
+  ClusterLaunch(const ClusterLaunch&) = delete;
+  ClusterLaunch& operator=(const ClusterLaunch&) = delete;
+};
+
 // ---- compile-time loop -----------------------------------------------------
 template <class F, int... I>
 __device__ __forceinline__ void static_for_impl(F&& f, std::integer_sequence<int, I...>) {
