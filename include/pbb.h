@@ -676,11 +676,11 @@ int pbb_array_geometry(int mode, const double* points, int S, const double* sens
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 
-/* DHTVPermutationAlignment.calculate_mapping (:295-355), similarity 'cos',
- * greedy assignment (:525-553).  mask (K, F, T) float64 is only read;
+/* DHTVPermutationAlignment.calculate_mapping (:295-355) with its defaults: pbb_dhtv_mapping_ex with similarity 'cos'
+ * and the greedy assignment (:525-553).  mask (K, F, T) float64 is only read;
  * plan: nplan triples (iterations, start, end) as produced by
- * alignment_plan (:204-293) -- a small HOST array (it drives the launch
- * sequence); features (K, F, T) and centroid
+ * alignment_plan (:204-293) -- a small HOST array (checked and sized on the host,
+ * then copied into the scratch); features (K, F, T) and centroid
  * (pbb_dhtv_scratch_doubles doubles) are device scratch; mapping (K, F) int64 out.
  * The reference's early exit is reproduced with device-side flags. */
 size_t pbb_dhtv_scratch_doubles(int K, int T, const int* plan, int nplan);
@@ -695,7 +695,8 @@ int pbb_dhtv_mapping(const double* mask, int K, int F, int T, const int* plan,
  * cooperative launch with grid-wide barriers.  The two add the centroid in different orders, so the integer mapping
  * is the same on both wherever no decision lies within rounding of a tie, and on exact ties (first maximum in
  * row-major order); tests/test_permutation_gpu.py::test_dhtv_every_kernel_matches_the_oracle checks both against the
- * reference.  K * T * 8 bytes must not exceed 200 KB (the centroid lives in shared memory). */
+ * reference.  K * T * 8 bytes must not exceed 200 KB (the centroid lives in shared memory).  Needs a device with
+ * cooperative launch (every H100 has it); elsewhere the call fails with a runtime error before any device work. */
 int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan,
                         int nplan, double* features, double* centroid,
                         long long* mapping, int metric, int algorithm, void* stream);

@@ -1,9 +1,10 @@
 // Frequency permutation alignment on the device (pb_bss/permutation_alignment.py):
-// DHTVPermutationAlignment.calculate_mapping (:295-355) with the 'cos' similarity
-// (_ScoreMatrix.multiply, :404-410) and the greedy assignment (:525-553), and
-// apply_mapping (:54-104).  See include/pbb.h.
+// DHTVPermutationAlignment.calculate_mapping (:295-355) with every similarity metric (:380-420) and
+// assignment (:458-590), the score matrices and assignments of Greedy / OraclePermutationAlignment
+// (:592-786), and apply_mapping (:54-104).  A DHTV plan runs in one launch: dhtv_cluster_kernel when
+// its widest segment fits one thread-block cluster, else dhtv_coop_kernel.  See include/pbb.h.
 #include <cooperative_groups.h>
-#include <cstring>
+#include <cstdlib>
 
 #include "common.cuh"
 #include "prof.cuh"
@@ -11,7 +12,6 @@
 namespace pbb {
 
 constexpr int kDhtvMaxK = 9;       // the reference asserts K < 10 (permutation_alignment.py:200)
-constexpr int kDhtvThreads = 1024;
 
 __device__ inline double block_sum(double v, double* red) {
   v = warp_sum(v);
@@ -37,112 +37,15 @@ __global__ void dhtv_normalize_kernel(const double* __restrict__ mask, double* _
   for (int t = threadIdx.x; t < T; t += blockDim.x) feat[(size_t)row * T + t] = m[t] / d;
 }
 
-// One alignment iteration = two launches (centroid partial sums over bin slices, then one
-// warp per bin: scores, greedy assignment, permutation).  Every launch of the fixed plan is
-// issued up front; the reference's early exit ("nothing changed", :352-353) is a device-side
-// flag: iteration i of a segment returns immediately unless iteration i-1 changed something.
-constexpr int kDhtvSlices = 8;   // bin slices of the centroid sum (summed in fixed order)
+constexpr int kDhtvSlices = 8;   // bin slices of dhtv_coop_kernel's centroid sum (summed in fixed order)
 
 __global__ void dhtv_init_mapping_kernel(long long* __restrict__ mapping, int K, int F) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < K * F) mapping[i] = i / F;
 }
 
-// partial[slice][k][t] = sum over the slice's bins of features[k][f][t]
-__global__ void dhtv_centroid_kernel(const double* __restrict__ feat, double* __restrict__ partial,
-                                     const int* __restrict__ prev_changed, int K, int F, int T, int start, int end) {
-  if (prev_changed != nullptr && *prev_changed == 0) return;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= K * T) return;
-  const int k = i / T, t = i - k * T;
-  const int n = end - start, per = (n + kDhtvSlices - 1) / kDhtvSlices;
-  const int f0 = start + blockIdx.y * per, f1 = min(end, f0 + per);
-  double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-  int f = f0;
-  for (; f + 3 < f1; f += 4) {
-    s0 += feat[((size_t)k * F + f) * T + t];
-    s1 += feat[((size_t)k * F + f + 1) * T + t];
-    s2 += feat[((size_t)k * F + f + 2) * T + t];
-    s3 += feat[((size_t)k * F + f + 3) * T + t];
-  }
-  for (; f < f1; ++f) s0 += feat[((size_t)k * F + f) * T + t];
-  partial[(size_t)blockIdx.y * K * T + i] = (s0 + s1) + (s2 + s3);
-}
-
-// one CTA = 4 warps = 4 bins of the segment
-__global__ void __launch_bounds__(128) dhtv_assign_kernel(double* __restrict__ feat, const double* __restrict__ partial,
-                                                          const int* __restrict__ prev_changed,
-                                                          int* __restrict__ changed, int K, int F, int T, int start,
-                                                          int end, long long* __restrict__ mapping) {
-  if (prev_changed != nullptr && *prev_changed == 0) return;
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  double* cent = reinterpret_cast<double*>(smem_raw);  // [K][T]
-  __shared__ double red[4];
-  __shared__ double cnorm[kDhtvMaxK];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  // centroid = mean over the segment's bins, then L2-normalised over time (:334-340)
-  const double inv_n = 1.0 / (double)(end - start);
-  for (int i = tid; i < K * T; i += blockDim.x) {
-    double s = 0.0;
-    for (int sl = 0; sl < kDhtvSlices; ++sl) s += partial[(size_t)sl * K * T + i];
-    cent[i] = s * inv_n;
-  }
-  __syncthreads();
-  for (int k = 0; k < K; ++k) {
-    double s = 0.0;
-    for (int t = tid; t < T; t += blockDim.x) { const double c = cent[k * T + t]; s += c * c; }
-    const double n = sqrt(block_sum(s, red));
-    if (tid == 0) cnorm[k] = fmax(n, kTiny);
-  }
-  __syncthreads();
-  for (int i = tid; i < K * T; i += blockDim.x) cent[i] = cent[i] / cnorm[i / T];
-  __syncthreads();
-  const int f = start + blockIdx.x * 4 + warp;
-  if (f >= end) return;
-  double score[kDhtvMaxK * kDhtvMaxK];
-  for (int kr = 0; kr < K; ++kr)
-    for (int km = 0; km < K; ++km) {
-      double s = 0.0;
-      for (int t = lane; t < T; t += 32) s += feat[((size_t)km * F + f) * T + t] * cent[kr * T + t];
-      score[kr * K + km] = warp_sum(s);  // identical in every lane
-    }
-  int perm[kDhtvMaxK];
-  for (int r = 0; r < K; ++r) {
-    // first maximum of the row-major flattened matrix (np.argmax), then blank its row and column (:525-553)
-    int bi = 0, bj = 0;
-    double best = -INFINITY;
-    bool found = false;
-    for (int i = 0; i < K; ++i)
-      for (int j = 0; j < K; ++j) {
-        const double v = score[i * K + j];
-        if (!found || v > best) { best = v; bi = i; bj = j; found = true; }
-      }
-    for (int j = 0; j < K; ++j) score[bi * K + j] = -INFINITY;
-    for (int i = 0; i < K; ++i) score[i * K + bj] = -INFINITY;
-    perm[bi] = bj;
-  }
-  bool ident = true;
-  for (int k = 0; k < K; ++k) ident = ident && perm[k] == k;
-  if (ident) return;
-  for (int t = lane; t < T; t += 32) {
-    double v[kDhtvMaxK];
-    for (int k = 0; k < K; ++k) v[k] = feat[((size_t)k * F + f) * T + t];
-    for (int k = 0; k < K; ++k) feat[((size_t)k * F + f) * T + t] = v[perm[k]];
-  }
-  if (lane == 0) {
-    long long mv[kDhtvMaxK];
-    for (int k = 0; k < K; ++k) mv[k] = mapping[(size_t)k * F + f];
-    for (int k = 0; k < K; ++k) mapping[(size_t)k * F + f] = mv[perm[k]];
-    *changed = 1;
-  }
-}
-
-// The whole alignment plan in ONE cooperative launch: every iteration is the same two phases as the launch pair above
-// (same arithmetic, same summation order: the mapping is bit-identical), separated by grid-wide barriers, and the
-// reference's early exit (:352-353) really skips the remaining iterations of a segment instead of launching kernels
-// that return at once.  plan: DEVICE copy of (iterations, start, end) triples.
-// Reverse permutation of one bin from its score matrix (_mapping_from_score_matrix, :458-590; every lane of the warp
-// computes the same).  greedy: K times the first maximum of the row-major flattened matrix, then blank its row and
+// Reverse permutation of one bin from its score matrix (_mapping_from_score_matrix, :458-590), by one thread; score
+// is overwritten.  greedy: K times the first maximum of the row-major flattened matrix, then blank its row and
 // column; optimal: the first best of itertools.permutations(range(K)) (lexicographic order, strict >), scores summed
 // left to right like Python's sum().
 __device__ __forceinline__ void dhtv_assign(double* __restrict__ score, int K, int optimal, int* __restrict__ perm) {
@@ -207,8 +110,8 @@ __device__ __forceinline__ void dhtv_grid_barrier(unsigned* counter, unsigned& g
   __syncthreads();
 }
 
-// block_sum over the FIRST 128 threads only, in the order of the 128-thread launch pair (dhtv_assign_kernel): the
-// centroid norms -- and with them every score and the integer mapping -- stay bit-identical whatever the block size
+// block_sum over the FIRST 128 threads only, in a fixed order: dhtv_coop_kernel's block size varies with K, its
+// centroid norms -- and with them every score and the integer mapping -- do not
 __device__ inline double block_sum_first128(double v, double* red) {
   v = warp_sum(threadIdx.x < 128 ? v : 0.0);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -220,6 +123,10 @@ __device__ inline double block_sum_first128(double v, double* red) {
 
 constexpr int kDhtvCoopMaxWarps = 16;
 
+// The whole alignment plan in ONE cooperative launch, for segments too wide for dhtv_cluster_kernel.  Each iteration
+// has two phases separated by grid-wide barriers: (A) centroid partial sums over kDhtvSlices bin slices, (B) per bin
+// the scores, the assignment and the permutation.  The reference's early exit (:352-353) skips the remaining
+// iterations of a segment.  plan: DEVICE copy of (iterations, start, end) triples.
 // One CTA per bin of the segment, one WARP per (reference class, mask class) score: a single warp per bin spends
 // ~25k cycles per iteration on its K^2 dot products and the assignment (latency of one dependent instruction stream);
 // spread over K^2 warps the bin takes ~2k.
@@ -247,7 +154,7 @@ __global__ void __launch_bounds__(32 * kDhtvCoopMaxWarps) dhtv_coop_kernel(
     const int iters = plan[3 * p], start = plan[3 * p + 1], end = plan[3 * p + 2];
     const int n = end - start, per = (n + kDhtvSlices - 1) / kDhtvSlices;
     for (int it = 0; it < iters; ++it, ++idx) {
-      // ---- phase A: partial[slice][k][t] = sum over the slice's bins (dhtv_centroid_kernel) ----
+      // ---- phase A: partial[slice][k][t] = sum over the slice's bins ----
       for (int e = gtid; e < kDhtvSlices * K * T; e += gthreads) {
         const int sl = e / (K * T), i = e - sl * (K * T);
         const int k = i / T, t = i - k * T;
@@ -266,7 +173,7 @@ __global__ void __launch_bounds__(32 * kDhtvCoopMaxWarps) dhtv_coop_kernel(
       DH_PH(0);  // phase A
       dhtv_grid_barrier(bar, generation);
       DH_PH(1);  // barrier 1
-      // ---- phase B: one CTA per bin (dhtv_assign_kernel); CTAs without a bin skip the centroid ----
+      // ---- phase B: one CTA per bin; CTAs without a bin skip the centroid ----
       if ((int)blockIdx.x < n) {
         const double inv_n = 1.0 / (double)n;
 #pragma unroll 2
@@ -296,8 +203,7 @@ __global__ void __launch_bounds__(32 * kDhtvCoopMaxWarps) dhtv_coop_kernel(
         DH_PH(3);  // centroid norms
         for (int f = start + blockIdx.x; f < end; f += gridDim.x) {
           // score[kr][km] = <centroid kr, feature km of this bin> by warp (kr, km): 16 values per lane at a time with
-          // every load in flight; the sum runs over t in ascending order per lane, then the usual warp reduction --
-          // bit-identical to dhtv_assign_kernel
+          // every load in flight; the sum runs over t in ascending order per lane, then the usual warp reduction
           for (int pair = warp; pair < K * K; pair += nwarps) {
             const int kr = pair / K, km = pair - kr * K;
             const double* __restrict__ row = feat + ((size_t)km * F + f) * T;
@@ -733,10 +639,7 @@ __global__ void __launch_bounds__(128) score_matrix_kernel(const double* __restr
     }
 }
 
-// _mapping_from_score_matrix (:458-590), one thread per bin.  greedy: K times the first
-// maximum of the row-major flattened matrix, then blank its row and column; optimal: the
-// first best of itertools.permutations(range(K)) (lexicographic order, strict >), the score
-// of a permutation summed left to right like Python's sum().
+// _mapping_from_score_matrix (:458-590), one thread per bin: dhtv_assign on finite scores.
 __global__ void mapping_from_score_kernel(const double* __restrict__ scores, int F, int K, int optimal,
                                           long long* __restrict__ mapping, int* __restrict__ status) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -753,40 +656,7 @@ __global__ void mapping_from_score_kernel(const double* __restrict__ scores, int
     return;
   }
   int out[kDhtvMaxK];
-  if (!optimal) {
-    for (int r = 0; r < K; ++r) {
-      int bi = 0, bj = 0;
-      double best = -INFINITY;
-      bool found = false;
-      for (int i = 0; i < K; ++i)
-        for (int j = 0; j < K; ++j) {
-          const double v = sc[i * K + j];
-          if (!found || v > best) { best = v; bi = i; bj = j; found = true; }
-        }
-      for (int j = 0; j < K; ++j) sc[bi * K + j] = -INFINITY;
-      for (int i = 0; i < K; ++i) sc[i * K + bj] = -INFINITY;
-      out[bi] = bj;
-    }
-  } else {
-    int perm[kDhtvMaxK];
-    for (int k = 0; k < K; ++k) { perm[k] = k; out[k] = k; }
-    double best = -INFINITY;
-    while (true) {
-      double s = 0.0;
-      for (int k = 0; k < K; ++k) s += sc[k * K + perm[k]];
-      if (s > best) {
-        best = s;
-        for (int k = 0; k < K; ++k) out[k] = perm[k];
-      }
-      int i = K - 2;  // next lexicographic permutation
-      while (i >= 0 && perm[i] > perm[i + 1]) --i;
-      if (i < 0) break;
-      int j = K - 1;
-      while (perm[j] < perm[i]) --j;
-      int tmp = perm[i]; perm[i] = perm[j]; perm[j] = tmp;
-      for (int a = i + 1, b = K - 1; a < b; ++a, --b) { tmp = perm[a]; perm[a] = perm[b]; perm[b] = tmp; }
-    }
-  }
+  dhtv_assign(sc, K, optimal, out);
   for (int k = 0; k < K; ++k) mapping[(size_t)k * F + f] = out[k];
 }
 
@@ -807,6 +677,122 @@ __global__ void chain_mapping_kernel(const long long* __restrict__ pair, int K, 
   }
 }
 
+// ---- host side of pbb_dhtv_mapping_ex ----------------------------------------------------------------------------
+
+// One checked alignment and its `centroid` scratch: kDhtvSlices * K * T doubles of partial sums, then the int
+// "changed" flags (one per iteration and a spare), the grid-barrier counter and the device copy of the plan.
+struct DhtvCall {
+  double* features;
+  long long* mapping;
+  int nplan, K, F, T, metric, algorithm;
+  int total_iters, widest;
+  double* partial;
+  int* changed;
+  unsigned* bar;
+  int* plan_dev;
+};
+
+// Checks the arguments and the HOST plan, and fills c but its scratch pointers: total_iters = planned iterations of
+// all segments, widest = bins of the widest segment (at least 1).
+static int check_dhtv_args(const double* mask, int K, int F, int T, const int* plan, int nplan, double* features,
+                           const double* centroid, long long* mapping, int metric, int algorithm, DhtvCall* c) {
+  PBB_CHECK_ARG(mask != nullptr, 1, "mask is null");
+  PBB_CHECK_ARG(metric >= 0 && metric <= 2, 10, "metric: 0 multiply, 1 cos, 2 euclidean");
+  PBB_CHECK_ARG(algorithm == 0 || algorithm == 1, 11, "algorithm: 0 greedy, 1 optimal");
+  PBB_CHECK_ARG(K > 0 && K <= kDhtvMaxK, 2, "need 0 < K < 10 (permutation_alignment.py:200)");
+  PBB_CHECK_ARG(F > 0, 3, "F must be positive");
+  PBB_CHECK_ARG(T > 0, 4, "T must be positive");
+  PBB_CHECK_ARG(plan != nullptr && nplan > 0 && nplan <= 4096, 5, "alignment plan: HOST array of (iterations, start, end)");
+  PBB_CHECK_ARG(features && centroid, 7, "scratch is null (pbb_dhtv_scratch_doubles)");
+  PBB_CHECK_ARG(mapping != nullptr, 9, "mapping is null");
+  PBB_CHECK_ARG((size_t)K * T * sizeof(double) <= 200 * 1024, 4, "K * T too large for the shared-memory centroid");
+  int total_iters = 0, widest = 1;
+  for (int p = 0; p < nplan; ++p) {
+    PBB_CHECK_ARG(plan[3 * p] >= 0 && plan[3 * p + 1] >= 0 && plan[3 * p + 2] <= F && plan[3 * p + 1] < plan[3 * p + 2],
+                  5, "alignment plan entry out of range");
+    total_iters += plan[3 * p];
+    if (plan[3 * p + 2] - plan[3 * p + 1] > widest) widest = plan[3 * p + 2] - plan[3 * p + 1];
+  }
+  *c = DhtvCall{features, mapping, nplan, K, F, T, metric, algorithm, total_iters, widest};
+  return 0;
+}
+
+#ifdef PBB_PHASE_TIMING
+// Prints and clears the cycles the kernel that just ran on st spent in each of its 8 phases (DH_PH).
+static void print_dhtv_phases(cudaStream_t st, const char* tag, const char* const (&names)[8]) {
+  unsigned long long ph[8], zero[8] = {0};
+  cudaStreamSynchronize(st);
+  cudaMemcpyFromSymbol(ph, g_dhtv_phase, sizeof(ph));
+  cudaMemcpyToSymbol(g_dhtv_phase, zero, sizeof(zero));
+  for (int i = 0; i < 8; ++i) fprintf(stderr, "[%s] %-26s %10llu cycles\n", tag, names[i], ph[i]);
+}
+#endif
+
+// dhtv_cluster_kernel, when the widest segment fits one thread-block cluster and a cluster of 16 (non-portable size)
+// or 8 CTAs can be scheduled.  *launched stays false when it does not apply.
+static int launch_dhtv_cluster(const DhtvCall& c, cudaStream_t st, bool* launched) {
+  static int cluster_ctas = -1;  // 16 (non-portable size), 8, or 0 = not available
+  for (int C = cluster_ctas < 0 ? 16 : cluster_ctas; C >= 8; C /= 2) {
+    const int per = (c.widest + C - 1) / C;
+    const size_t smem = (size_t)(2 + per) * c.K * c.T * sizeof(double);
+    if (per > kDhtvClMaxLocal || smem > 200 * 1024) break;
+    using ClusterKern = void (*)(double*, const int*, int, int, int, int, long long*, int, int);
+    const ClusterKern kern = c.K == 2 ? dhtv_cluster_kernel<2> : c.K == 3 ? dhtv_cluster_kernel<3>
+                             : c.K == 4 ? dhtv_cluster_kernel<4> : dhtv_cluster_kernel<0>;
+    PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    if (C > 8) PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+    const ClusterLaunch cl(C, kDhtvClThreads, smem, C, st);
+    if (cluster_ctas < 0) {
+      int nclusters = 0;
+      if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cl.cfg) != cudaSuccess || nclusters < 1) {
+        (void)cudaGetLastError();
+        if (C == 8) cluster_ctas = 0;
+        continue;  // try the portable size
+      }
+      cluster_ctas = C;
+    }
+    LaunchScope ls("dhtv_cluster_kernel", st);
+    PBB_CUDA(cudaLaunchKernelEx(&cl.cfg, kern, c.features, c.plan_dev, c.nplan, c.K, c.F, c.T, c.mapping, c.metric,
+                                c.algorithm));
+    *launched = true;
+#ifdef PBB_PHASE_TIMING
+    print_dhtv_phases(st, "dhtv cluster", {"segment load (+store)", "partial sums", "barrier 1 + reduce-scatter",
+                                           "cluster barrier 2", "norms + scores", "assignment", "permutation",
+                                           "cluster barrier 3"});
+    unsigned long long its = 0, z = 0;
+    cudaMemcpyFromSymbol(&its, g_dhtv_iters, sizeof(its));
+    cudaMemcpyToSymbol(g_dhtv_iters, &z, sizeof(z));
+    fprintf(stderr, "[dhtv cluster] iterations executed %llu of %d planned\n", its, c.total_iters);
+#endif
+    return 0;
+  }
+  return 0;
+}
+
+// dhtv_coop_kernel: one CTA per bin of the widest segment, as many as can be resident.
+static int launch_dhtv_coop(DhtvCall c, int dev, cudaStream_t st) {
+  const size_t smem = (size_t)c.K * c.T * sizeof(double);
+  PBB_CUDA(cudaFuncSetAttribute(dhtv_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  int per_sm = 0, sms = 0;
+  int warps = c.K * c.K < kDhtvCoopMaxWarps ? c.K * c.K : kDhtvCoopMaxWarps;
+  if (warps < 4) warps = 4;  // the centroid norms are summed by the first 128 threads
+  const int threads = 32 * warps;
+  PBB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dhtv_coop_kernel, threads, smem));
+  PBB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  int grid = c.widest;
+  if (grid > per_sm * sms) grid = per_sm * sms;
+  if (grid < 1) grid = 1;
+  void* args[] = {&c.features, &c.partial, &c.changed, &c.plan_dev, &c.nplan, &c.K,
+                  &c.F,        &c.T,       &c.mapping, &c.bar,      &c.metric, &c.algorithm};
+  LaunchScope ls("dhtv_coop_kernel", st);
+  PBB_CUDA(cudaLaunchCooperativeKernel((const void*)dhtv_coop_kernel, dim3(grid), dim3(threads), args, smem, st));
+#ifdef PBB_PHASE_TIMING
+  print_dhtv_phases(st, "dhtv", {"phase A", "barrier 1", "centroid combine", "centroid norms", "scores", "assignment",
+                                 "permute/rest", "barrier 2"});
+#endif
+  return 0;
+}
+
 }  // namespace pbb
 
 using namespace pbb;
@@ -820,28 +806,19 @@ int pbb_dhtv_mapping(const double* mask, int K, int F, int T, const int* plan, i
 
 int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan, int nplan, double* features,
                         double* centroid, long long* mapping, int metric, int algorithm, void* stream) {
-  PBB_CHECK_ARG(mask != nullptr, 1, "mask is null");
-  PBB_CHECK_ARG(metric >= 0 && metric <= 2, 10, "metric: 0 multiply, 1 cos, 2 euclidean");
-  PBB_CHECK_ARG(algorithm == 0 || algorithm == 1, 11, "algorithm: 0 greedy, 1 optimal");
-  PBB_CHECK_ARG(K > 0 && K <= kDhtvMaxK, 2, "need 0 < K < 10 (permutation_alignment.py:200)");
-  PBB_CHECK_ARG(F > 0, 3, "F must be positive");
-  PBB_CHECK_ARG(T > 0, 4, "T must be positive");
-  PBB_CHECK_ARG(plan != nullptr && nplan > 0 && nplan <= 4096, 5, "alignment plan: HOST array of (iterations, start, end)");
-  PBB_CHECK_ARG(features && centroid, 7, "scratch is null (pbb_dhtv_scratch_doubles)");
-  PBB_CHECK_ARG(mapping != nullptr, 9, "mapping is null");
-  PBB_CHECK_ARG((size_t)K * T * sizeof(double) <= 200 * 1024, 4, "K * T too large for the shared-memory centroid");
+  DhtvCall c;
+  if (int rc = check_dhtv_args(mask, K, F, T, plan, nplan, features, centroid, mapping, metric, algorithm, &c)) return rc;
+  // segments too wide for a cluster run on dhtv_coop_kernel, which needs a cooperative launch (every H100 has it)
+  int dev = 0, coop = 0;
+  PBB_CUDA(cudaGetDevice(&dev));
+  PBB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  if (!coop) { set_error("DHTV alignment: device %d does not support cooperative launch", dev); return 1; }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int total_iters = 0;
-  for (int p = 0; p < nplan; ++p) {
-    PBB_CHECK_ARG(plan[3 * p] >= 0 && plan[3 * p + 1] >= 0 && plan[3 * p + 2] <= F && plan[3 * p + 1] < plan[3 * p + 2],
-                  5, "alignment plan entry out of range");
-    total_iters += plan[3 * p];
-  }
-  // centroid scratch: kDhtvSlices * K * T doubles of partial sums, then the int "changed" flags
-  double* partial = centroid;
-  int* changed = reinterpret_cast<int*>(centroid + (size_t)kDhtvSlices * K * T);
-  PBB_CUDA(cudaMemsetAsync(changed, 0, (size_t)(total_iters + 2) * sizeof(int), st));
-  PBB_CUDA(cudaFuncSetAttribute(dhtv_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  c.partial = centroid;
+  c.changed = reinterpret_cast<int*>(centroid + (size_t)kDhtvSlices * K * T);
+  c.bar = reinterpret_cast<unsigned*>(c.changed + c.total_iters + 1);  // zeroed with the flags
+  c.plan_dev = c.changed + c.total_iters + 2;
+  PBB_CUDA(cudaMemsetAsync(c.changed, 0, (size_t)(c.total_iters + 2) * sizeof(int), st));
   {
     LaunchScope ls("dhtv_normalize_kernel", st);
     if (metric == 1) dhtv_normalize_kernel<<<K * F, 128, 0, st>>>(mask, features, K * F, T);
@@ -849,109 +826,12 @@ int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan
     dhtv_init_mapping_kernel<<<(K * F + 255) / 256, 256, 0, st>>>(mapping, K, F);
     PBB_CUDA(cudaGetLastError());
   }
-  // One cooperative launch runs the whole plan (PBB_DHTV_MULTI=1: the launch pair per iteration, for A/B).
-  static const bool multi = getenv("PBB_DHTV_MULTI") != nullptr;
-  int dev = 0, coop = 0;
-  PBB_CUDA(cudaGetDevice(&dev));
-  PBB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!multi && coop) {
-    // the plan travels in the scratch, behind the flags
-    int* plan_dev = changed + total_iters + 2;
-    unsigned* bar = reinterpret_cast<unsigned*>(changed + total_iters + 1);  // zeroed with the flags
-    PBB_CUDA(cudaMemcpyAsync(plan_dev, plan, (size_t)3 * nplan * sizeof(int), cudaMemcpyHostToDevice, st));
-    int widest_seg = 1;
-    for (int p = 0; p < nplan; ++p)
-      widest_seg = plan[3 * p + 2] - plan[3 * p + 1] > widest_seg ? plan[3 * p + 2] - plan[3 * p + 1] : widest_seg;
-    // Segments that fit into the shared memory of one thread-block cluster (the reference's plans do: ~100 bins):
-    // dhtv_cluster_kernel.  PBB_DHTV_COOP=1 keeps the grid-barrier kernel (A/B).
-    static const bool no_cluster = getenv("PBB_DHTV_COOP") != nullptr;
-    if (!no_cluster) {
-      static int cluster_ctas = -1;  // 16 (non-portable size), 8, or 0 = not available
-      for (int C = cluster_ctas < 0 ? 16 : cluster_ctas; C >= 8; C /= 2) {
-        const int per = (widest_seg + C - 1) / C;
-        const size_t smem = (size_t)(2 + per) * K * T * sizeof(double);
-        if (per > kDhtvClMaxLocal || smem > 200 * 1024) break;
-        using ClusterKern = void (*)(double*, const int*, int, int, int, int, long long*, int, int);
-        const ClusterKern kern = K == 2 ? dhtv_cluster_kernel<2> : K == 3 ? dhtv_cluster_kernel<3>
-                                 : K == 4 ? dhtv_cluster_kernel<4> : dhtv_cluster_kernel<0>;
-        PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        if (C > 8) PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-        const ClusterLaunch cl(C, kDhtvClThreads, smem, C, st);
-        if (cluster_ctas < 0) {
-          int nclusters = 0;
-          if (cudaOccupancyMaxActiveClusters(&nclusters, kern, &cl.cfg) != cudaSuccess || nclusters < 1) {
-            (void)cudaGetLastError();
-            if (C == 8) cluster_ctas = 0;
-            continue;  // try the portable size
-          }
-          cluster_ctas = C;
-        }
-        LaunchScope ls("dhtv_cluster_kernel", st);
-        const int* plan_c = plan_dev;
-        PBB_CUDA(cudaLaunchKernelEx(&cl.cfg, kern, features, plan_c, nplan, K, F, T, mapping, metric, algorithm));
-#ifdef PBB_PHASE_TIMING
-        {
-          unsigned long long ph[8], zero[8] = {0};
-          cudaStreamSynchronize(st);
-          cudaMemcpyFromSymbol(ph, g_dhtv_phase, sizeof(ph));
-          cudaMemcpyToSymbol(g_dhtv_phase, zero, sizeof(zero));
-          static const char* nm[8] = {"segment load (+store)", "partial sums", "barrier 1 + reduce-scatter", "cluster barrier 2",
-                                      "norms + scores", "assignment", "permutation", "cluster barrier 3"};
-          for (int i = 0; i < 8; ++i) fprintf(stderr, "[dhtv cluster] %-22s %10llu cycles\n", nm[i], ph[i]);
-          unsigned long long its = 0, z = 0;
-          cudaMemcpyFromSymbol(&its, g_dhtv_iters, sizeof(its));
-          cudaMemcpyToSymbol(g_dhtv_iters, &z, sizeof(z));
-          fprintf(stderr, "[dhtv cluster] iterations executed %llu of %d planned\n", its, total_iters);
-        }
-#endif
-        return 0;
-      }
-    }
-    const size_t smem = (size_t)K * T * sizeof(double);
-    PBB_CUDA(cudaFuncSetAttribute(dhtv_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    int per_sm = 0, sms = 0;
-    int warps = K * K < kDhtvCoopMaxWarps ? K * K : kDhtvCoopMaxWarps;
-    if (warps < 4) warps = 4;  // the centroid norms are summed by the first 128 threads
-    const int threads = 32 * warps;
-    PBB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dhtv_coop_kernel, threads, smem));
-    PBB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    int widest = 1;  // one CTA per bin of the widest segment
-    for (int p = 0; p < nplan; ++p) widest = plan[3 * p + 2] - plan[3 * p + 1] > widest ? plan[3 * p + 2] - plan[3 * p + 1] : widest;
-    int grid = widest;
-    if (grid > per_sm * sms) grid = per_sm * sms;
-    if (grid < 1) grid = 1;
-    void* args[] = {(void*)&features, (void*)&partial, (void*)&changed, (void*)&plan_dev, (void*)&nplan,
-                    (void*)&K, (void*)&F, (void*)&T, (void*)&mapping, (void*)&bar, (void*)&metric, (void*)&algorithm};
-    LaunchScope ls("dhtv_coop_kernel", st);
-    PBB_CUDA(cudaLaunchCooperativeKernel((const void*)dhtv_coop_kernel, dim3(grid), dim3(threads), args, smem, st));
-#ifdef PBB_PHASE_TIMING
-    {
-      unsigned long long ph[8], zero[8] = {0};
-      cudaStreamSynchronize(st);
-      cudaMemcpyFromSymbol(ph, g_dhtv_phase, sizeof(ph));
-      cudaMemcpyToSymbol(g_dhtv_phase, zero, sizeof(zero));
-      static const char* nm[8] = {"phase A", "barrier 1", "centroid combine", "centroid norms", "scores", "assignment", "permute/rest", "barrier 2"};
-      for (int i = 0; i < 8; ++i) fprintf(stderr, "[dhtv] %-18s %10llu cycles\n", nm[i], ph[i]);
-    }
-#endif
-    return 0;
-  }
-  PBB_CHECK_ARG(metric == 1 && algorithm == 0, 10,
-                "only similarity_metric='cos' with algorithm='greedy' has the multi-launch path (no cooperative launch here)");
-  LaunchScope ls("dhtv_iterations", st);
-  int idx = 0;
-  for (int p = 0; p < nplan; ++p) {
-    const int iters = plan[3 * p], start = plan[3 * p + 1], end = plan[3 * p + 2];
-    for (int it = 0; it < iters; ++it, ++idx) {
-      const int* prev = it == 0 ? nullptr : changed + idx - 1;
-      dhtv_centroid_kernel<<<dim3((K * T + 127) / 128, kDhtvSlices), 128, 0, st>>>(features, partial, prev, K, F, T,
-                                                                                   start, end);
-      dhtv_assign_kernel<<<(end - start + 3) / 4, 128, (size_t)K * T * sizeof(double), st>>>(
-          features, partial, prev, changed + idx, K, F, T, start, end, mapping);
-    }
-  }
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_CUDA(cudaMemcpyAsync(c.plan_dev, plan, (size_t)3 * nplan * sizeof(int), cudaMemcpyHostToDevice, st));
+  // The reference's plans (~100-bin segments) fit a cluster.  PBB_DHTV_COOP=1 keeps the grid-barrier kernel (A/B).
+  static const bool no_cluster = getenv("PBB_DHTV_COOP") != nullptr;
+  bool launched = false;
+  if (int rc = no_cluster ? 0 : launch_dhtv_cluster(c, st, &launched)) return rc;
+  return launched ? 0 : launch_dhtv_coop(c, dev, st);
 }
 
 // doubles of `centroid` scratch pbb_dhtv_mapping needs

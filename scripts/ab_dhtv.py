@@ -1,6 +1,5 @@
-"""A/B of the DHTV alignment kernels: cluster / DSMEM kernel (default) vs grid-barrier kernel (PBB_DHTV_COOP=1) vs the
-launch pair per iteration (PBB_DHTV_MULTI=1, cos / greedy only) on cACGMM masks, for every similarity metric and both
-assignments; time per calculate_mapping at C3 size.  The kernels add the centroid in different orders, so a mapping
+"""A/B of the DHTV alignment kernels: cluster / DSMEM kernel (default) vs grid-barrier kernel (PBB_DHTV_COOP=1) on
+cACGMM masks, for every similarity metric and both assignments; time per calculate_mapping at C3 size.  The kernels add the centroid in different orders, so a mapping
 may differ where a decision lies within rounding of a tie; tests/test_permutation_gpu.py checks them against the
 oracle with that precondition."""
 import os, subprocess, sys, tempfile
@@ -10,7 +9,6 @@ if len(sys.argv) > 1 and sys.argv[1] == 'child':
     from oracle import synth
     from pb_bss_b200.distribution import CACGMMTrainer
     from pb_bss_b200.permutation_alignment import DHTVPermutationAlignment
-    multi = 'PBB_DHTV_MULTI' in os.environ
     out = {}
     for (F, T, K, seed) in ((513, 500, 3, 5), (257, 300, 2, 6), (513, 200, 4, 7)):
         y, _ = synth.structured_stft(F, T, 8, K, seed=seed)
@@ -19,8 +17,6 @@ if len(sys.argv) > 1 and sys.argv[1] == 'child':
         mask = m.predict(torch.from_numpy(y).cuda()).permute(1, 0, 2).contiguous()
         for metric in ('cos', 'multiply', 'euclidean'):
             for algorithm in ('greedy', 'optimal'):
-                if multi and (metric, algorithm) != ('cos', 'greedy'):
-                    continue
                 # the metric is fixed when the aligner is constructed: one aligner per metric
                 al = DHTVPermutationAlignment(stft_size=2 * (F - 1), segment_start=100 if F == 513 else 70,
                                               segment_width=100, segment_shift=20, main_iterations=20,
@@ -41,16 +37,15 @@ else:
     import numpy as np
     res = {}
     tmp = tempfile.mkdtemp()
-    for tag, env in (('cluster', {}), ('coop', {'PBB_DHTV_COOP': '1'}), ('multi', {'PBB_DHTV_MULTI': '1'})):
+    for tag, env in (('cluster', {}), ('coop', {'PBB_DHTV_COOP': '1'})):
         e = dict(os.environ); e.update(env)
         path = os.path.join(tmp, f'ab_dhtv_{tag}.npz')
         subprocess.run(['timeout', '300', sys.executable, __file__, 'child', tag, path], env=e, check=True)
         res[tag] = np.load(path)
     for k in res['cluster'].files:
         same_coop = np.array_equal(res['cluster'][k], res['coop'][k])
-        same_multi = np.array_equal(res['cluster'][k], res['multi'][k]) if k in res['multi'].files else None
         nonid = int((res['cluster'][k] != np.arange(res['cluster'][k].shape[0])[:, None]).any(0).sum())
-        print(f'{k}: cluster == coop {same_coop}, cluster == multi {same_multi}, bins with a non-identity mapping {nonid}')
+        print(f'{k}: cluster == coop {same_coop}, bins with a non-identity mapping {nonid}')
     # the metrics really differ: not every metric gives the same mapping
     for F, K in ((513, 3), (257, 2), (513, 4)):
         maps = [res['cluster'][f'{F}_{K}_{m}_greedy'] for m in ('cos', 'multiply', 'euclidean')]

@@ -147,9 +147,9 @@ def test_full_size_greedy_alignment_against_the_oracle():
 
 # ---- every DHTV kernel on the same inputs ---------------------------------------------------------------------------
 # pbb_dhtv_mapping_ex runs dhtv_cluster_kernel when the widest segment fits one thread-block cluster (templated for
-# K = 2, 3, 4, generic for K = 5..9), dhtv_coop_kernel (grid barriers) when it does not or with PBB_DHTV_COOP=1, and
-# the launch pair per iteration with PBB_DHTV_MULTI=1 (cos / greedy only).  The switches are read once per process, so
-# each path runs in a child process of its own (this file run as a script) over the same cases.
+# K = 2, 3, 4, generic for K = 5..9), and dhtv_coop_kernel (grid barriers) when it does not or with PBB_DHTV_COOP=1.
+# The switch is read once per process, so each path runs in a child process of its own (this file run as a script)
+# over the same cases.
 #
 # The kernels add the centroid in different orders and apply the cos normalisation differently, so a decision within
 # rounding of a tie may legitimately differ between them.  Generated cases therefore assert the oracle's decision
@@ -162,7 +162,7 @@ ALL = tuple((m, a) for m in METRICS for a in ALGORITHMS)
 GREEDY = tuple((m, 'greedy') for m in METRICS)
 SOME = (('cos', 'greedy'), ('multiply', 'greedy'), ('euclidean', 'optimal'))
 MULTIPLY = (('multiply', 'greedy'), ('multiply', 'optimal'))
-KERNELS = {'cluster': 'dhtv_cluster_kernel', 'coop': 'dhtv_coop_kernel', 'multi': 'dhtv_iterations'}
+KERNELS = {'cluster': 'dhtv_cluster_kernel', 'coop': 'dhtv_coop_kernel'}
 
 
 def _generated_dhtv_cases():
@@ -256,15 +256,12 @@ def _run_dhtv_cases(out_path):
     """Child process: every case on the path this process's environment selects -> mappings and launched kernels."""
     import torch
     from pb_bss_b200 import _lib
-    multi = 'PBB_DHTV_MULTI' in os.environ
     lib = _lib.load()
     lib.pbb_profile_enable(1)
     out = {}
     for name, mask, plan, combos, _ in _dhtv_cases(load_golden('permutation_classes')):
         m = torch.from_numpy(mask).cuda()
         for metric, algorithm in combos:
-            if multi and (metric, algorithm) != ('cos', 'greedy'):
-                continue
             lib.pbb_profile_reset()
             key = f'{name}_{metric}_{algorithm}'
             out[key] = _aligner(plan, metric, algorithm).calculate_mapping(m).cpu().numpy()
@@ -273,19 +270,19 @@ def _run_dhtv_cases(out_path):
     np.savez(out_path, **out)
 
 
-PATHS = {'default': {}, 'coop': {'PBB_DHTV_COOP': '1'}, 'multi': {'PBB_DHTV_MULTI': '1'}}
+PATHS = {'default': {}, 'coop': {'PBB_DHTV_COOP': '1'}}
 
 
 @pytest.fixture(scope='module')
 def dhtv_paths(tmp_path_factory):
-    """Runs the three child processes (concurrently, while the oracle runs here) -> (expected, results, kernels):
+    """Runs the two child processes (concurrently, while the oracle runs here) -> (expected, results, kernels):
     the fixture's mapping for its cases, the oracle's for the generated ones."""
     import subprocess
     tmp = tmp_path_factory.mktemp('dhtv')
     procs = {}
     try:
         for path, env in PATHS.items():
-            e = {k: v for k, v in os.environ.items() if k not in ('PBB_DHTV_COOP', 'PBB_DHTV_MULTI')}
+            e = {k: v for k, v in os.environ.items() if k != 'PBB_DHTV_COOP'}
             e.update(env)
             procs[path] = subprocess.Popen([sys.executable, os.path.abspath(__file__), str(tmp / f'{path}.npz')], env=e)
         g = load_golden('permutation_classes')
@@ -317,10 +314,9 @@ def test_dhtv_every_kernel_matches_the_oracle(dhtv_paths, path):
     and assignment.  Asserts which kernel ran, so the coverage cannot silently move to another kernel."""
     expected, results, kernels = dhtv_paths
     got = results[path]
-    keys = [k for k in expected if path != 'multi' or k.endswith('_cos_greedy')]
-    assert sorted(k for k in got if not k.startswith('kernels_')) == sorted(keys)
+    assert sorted(k for k in got if not k.startswith('kernels_')) == sorted(expected)
     ran = {}
-    for key in keys:
+    for key in expected:
         launched = got[f'kernels_{key}'].item().split(',')
         want = KERNELS[kernels[key] if path == 'default' else path]
         assert want in launched and not (set(KERNELS.values()) - {want}) & set(launched), (path, key, launched)
