@@ -673,6 +673,41 @@ int pbb_array_geometry(int mode, const double* points, int S, const double* sens
                        double* out, void* stream);
 
 /* ------------------------------------------------------------------------
+ * STFT / iSTFT (nara_wpe.utils.stft / istft, as restated in oracle/transform_oracle.py) and the Griffin-Lim / MISI
+ * step of pb_bss/transform/griffin_lim_module.py.  size is a power of two in [64, 4096], 1 <= shift <=
+ * window_length <= size.  All arithmetic is fp64; twiddle is the host-built table (cos, sin)(2 pi k / size), k < size,
+ * as size double pairs.  Spectra are (rows, frames, size/2 + 1) complex128, frame-major.
+ */
+
+/* nara_wpe stft: frame t of row r holds x[r][t shift - offset + j] * window[j] for j < window_length (zero outside
+ * [0, n): offset = window_length - shift with fading, else 0; the end padding of pad=True is the same zero read), then
+ * rfft(frame, n=size) -> out[r][t].  x (rows, n) float32 (dtype PBB_F32) or float64 (PBB_F64); window (wl) float64.
+ * Replaces the np.pad / segment_axis / einsum / rfft sequence of nara_wpe.utils.stft. */
+int pbb_stft(const void* x, int dtype, long long rows, long long n, int size, int shift,
+             int window_length, int offset, int frames, const double* window,
+             const double* twiddle, void* out, void* stream);
+
+/* GriffinLim.step / MISI.step (griffin_lim_module.py:63-66, 112-130), the STFT half: X_dash_dash = stft(x) and, in
+ * the same pass, X_dash = |X| exp(i angle(X_dash_dash)) (exp(i angle(0)) = 1).  y == NULL: Griffin-Lim, x = x_hat
+ * (K, n).  y != NULL (n float64): MISI, x = x_hat + (y - sum_k x_hat) / K with the sum in row order.  X, X_dash_dash
+ * and X_dash are (K, frames, size/2 + 1) complex128.  The iSTFT half is pbb_istft. */
+int pbb_griffin_lim_stft(const double* x_hat, int K, long long n, const double* y,
+                         const void* X, int size, int shift, int window_length, int offset,
+                         int frames, const double* window, const double* twiddle,
+                         void* X_dash_dash, void* X_dash, void* stream);
+
+/* nara_wpe istft: frame_t = irfft(X[r][t], n=size)[:window_length] * synthesis_window (the imaginary parts of the DC
+ * and Nyquist bins are ignored), overlap-added into frames * shift + window_length - shift samples in increasing t
+ * from 0.0 (the order of np.add.at; no atomics), of which out[r] (n_out float64) receives those from crop on
+ * (crop = window_length - shift with fading).  synthesis_window (wl) is nara_wpe's biorthogonal window.  The windowed
+ * frames go to workspace (pbb_istft_workspace_bytes).  Replaces the irfft / np.add.at sequence of
+ * nara_wpe.utils.istft. */
+size_t pbb_istft_workspace_bytes(long long rows, int frames, int window_length);
+int pbb_istft(const void* X, long long rows, int frames, int size, int shift, int window_length,
+              int crop, long long n_out, const double* synthesis_window, const double* twiddle,
+              void* workspace, size_t workspace_bytes, double* out, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

@@ -3,7 +3,8 @@
 Host side: Python mirroring the reference's public API for this path
 (``distribution.CACGMMTrainer/CACGMM/CWMMTrainer/CWMM``,
 ``extraction.get_power_spectral_density_matrix/get_mvdr_vector/get_gev_vector``,
-``permutation_alignment.DHTVPermutationAlignment``).  All arithmetic runs in
+``permutation_alignment.DHTVPermutationAlignment``), plus the STFT / iSTFT ends and
+Griffin-Lim / MISI (``transform``).  All arithmetic runs in
 hand-written sm_90a CUDA kernels behind the C ABI of ``include/pbb.h``
 (``libpbb.so``, bound with ctypes in ``_lib.py``); torch tensors are only the
 device-memory containers.  There is no CPU fallback.
@@ -13,6 +14,7 @@ from . import distribution  # noqa: F401
 from . import extraction  # noqa: F401
 from . import permutation_alignment  # noqa: F401
 from . import initializer  # noqa: F401
+from . import transform  # noqa: F401
 from ._device import deferred_status  # noqa: F401
 
-__all__ = ['distribution', 'extraction', 'permutation_alignment', 'initializer']
+__all__ = ['distribution', 'extraction', 'permutation_alignment', 'initializer', 'transform']

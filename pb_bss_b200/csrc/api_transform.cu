@@ -1,0 +1,176 @@
+// C-ABI entry points for the STFT / iSTFT of nara_wpe.utils and the Griffin-Lim / MISI phase reconstruction of
+// pb_bss/transform/griffin_lim_module.py -- see include/pbb.h and csrc/fft.cuh.
+#include "common.cuh"
+#include "fft.cuh"
+#include "prof.cuh"
+
+namespace pbb {
+
+static int log2_size(int size) {
+  if (size < kFftMinSize || size > kFftMaxSize || (size & (size - 1)) != 0) return -1;
+  int l = 0;
+  while ((1 << l) < size) ++l;
+  return l;
+}
+
+static int sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+      n = 132;
+  }
+  return n;
+}
+
+// Frames per CTA: as many as the 64 KB shared-memory budget allows, halved while the grid would not give every SM
+// two CTAs.
+static int frames_per_cta(int size, long long rows, int frames) {
+  int fpc = kFftFrameBudget / size;
+  while (fpc > 1 && rows * ((frames + fpc - 1) / fpc) < 2ll * sm_count()) fpc /= 2;
+  return fpc;
+}
+
+template <class K>
+static int fft_launch(K kernel, const char* name, long long rows, int frames, int fpc, int size, void* params_ptr,
+                      cudaStream_t st) {
+  const size_t smem = (size_t)fpc * size * sizeof(double2);  // two buffers of fpc * size / 2 points
+  PBB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const long long ctas = rows * ((frames + fpc - 1) / fpc);
+  if (ctas > 0x7fffffffll) {
+    set_error("argument: %lld CTAs exceed the grid", ctas);
+    return -1;
+  }
+  LaunchScope ls(name, st);
+  void* args[] = {params_ptr};
+  PBB_CUDA(cudaLaunchKernel((const void*)kernel, dim3((unsigned)ctas), dim3(kFftThreads), args, smem, st));
+  return 0;
+}
+
+}  // namespace pbb
+
+using namespace pbb;
+
+extern "C" {
+
+int pbb_stft(const void* x, int dtype, long long rows, long long n, int size, int shift, int window_length,
+             int offset, int frames, const double* window, const double* twiddle, void* out, void* stream) {
+  const int logN = log2_size(size);
+  PBB_CHECK_ARG(x != nullptr, 1, "x is null");
+  PBB_CHECK_ARG(dtype == PBB_F32 || dtype == PBB_F64, 2, "dtype must be PBB_F32 or PBB_F64");
+  PBB_CHECK_ARG(rows > 0, 3, "rows must be positive");
+  PBB_CHECK_ARG(n >= 0, 4, "n must be non-negative");
+  PBB_CHECK_ARG(logN > 0, 5, "size must be a power of two in [64, 4096]");
+  PBB_CHECK_ARG(window_length >= 1 && window_length <= size, 7, "window_length must be in [1, size]");
+  PBB_CHECK_ARG(shift >= 1 && shift <= window_length, 6, "shift must be in [1, window_length]");
+  PBB_CHECK_ARG(offset >= 0 && offset < window_length, 8, "offset must be in [0, window_length)");
+  PBB_CHECK_ARG(frames > 0, 9, "frames must be positive");
+  PBB_CHECK_ARG(window != nullptr, 10, "window is null");
+  PBB_CHECK_ARG(twiddle != nullptr, 11, "twiddle is null");
+  PBB_CHECK_ARG(out != nullptr, 12, "out is null");
+  StftParams p{};
+  p.x = x;
+  p.rows = rows;
+  p.n = n;
+  p.logM = logN - 1;
+  p.shift = shift;
+  p.wl = window_length;
+  p.offset = offset;
+  p.frames = frames;
+  p.fpc = frames_per_cta(size, rows, frames);
+  p.tiles = (frames + p.fpc - 1) / p.fpc;
+  p.window = window;
+  p.tw = reinterpret_cast<const double2*>(twiddle);
+  p.out = reinterpret_cast<double2*>(out);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (dtype == PBB_F32) return fft_launch(stft_kernel<float, STFT_PLAIN>, "stft_kernel", rows, frames, p.fpc, size, &p, st);
+  return fft_launch(stft_kernel<double, STFT_PLAIN>, "stft_kernel", rows, frames, p.fpc, size, &p, st);
+}
+
+int pbb_griffin_lim_stft(const double* x_hat, int K, long long n, const double* y, const void* X, int size, int shift,
+                         int window_length, int offset, int frames, const double* window, const double* twiddle,
+                         void* X_dash_dash, void* X_dash, void* stream) {
+  const int logN = log2_size(size);
+  PBB_CHECK_ARG(x_hat != nullptr, 1, "x_hat is null");
+  PBB_CHECK_ARG(K > 0, 2, "K must be positive");
+  PBB_CHECK_ARG(n >= 0, 3, "n must be non-negative");
+  PBB_CHECK_ARG(X != nullptr, 5, "X is null");
+  PBB_CHECK_ARG(logN > 0, 6, "size must be a power of two in [64, 4096]");
+  PBB_CHECK_ARG(window_length >= 1 && window_length <= size, 8, "window_length must be in [1, size]");
+  PBB_CHECK_ARG(shift >= 1 && shift <= window_length, 7, "shift must be in [1, window_length]");
+  PBB_CHECK_ARG(offset >= 0 && offset < window_length, 9, "offset must be in [0, window_length)");
+  PBB_CHECK_ARG(frames > 0, 10, "frames must be positive");
+  PBB_CHECK_ARG(window != nullptr, 11, "window is null");
+  PBB_CHECK_ARG(twiddle != nullptr, 12, "twiddle is null");
+  PBB_CHECK_ARG(X_dash_dash != nullptr, 13, "X_dash_dash is null");
+  PBB_CHECK_ARG(X_dash != nullptr, 14, "X_dash is null");
+  StftParams p{};
+  p.x = x_hat;
+  p.rows = K;
+  p.n = n;
+  p.logM = logN - 1;
+  p.shift = shift;
+  p.wl = window_length;
+  p.offset = offset;
+  p.frames = frames;
+  p.fpc = frames_per_cta(size, K, frames);
+  p.tiles = (frames + p.fpc - 1) / p.fpc;
+  p.window = window;
+  p.tw = reinterpret_cast<const double2*>(twiddle);
+  p.X = reinterpret_cast<const double2*>(X);
+  p.y = y;
+  p.out = reinterpret_cast<double2*>(X_dash_dash);
+  p.out_dash = reinterpret_cast<double2*>(X_dash);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (y != nullptr)
+    return fft_launch(stft_kernel<double, STFT_MISI>, "stft_misi_kernel", K, frames, p.fpc, size, &p, st);
+  return fft_launch(stft_kernel<double, STFT_GRIFFIN_LIM>, "stft_griffin_lim_kernel", K, frames, p.fpc, size, &p, st);
+}
+
+size_t pbb_istft_workspace_bytes(long long rows, int frames, int window_length) {
+  if (rows <= 0 || frames <= 0 || window_length <= 0) return 0;
+  return (size_t)rows * frames * window_length * sizeof(double);
+}
+
+int pbb_istft(const void* X, long long rows, int frames, int size, int shift, int window_length, int crop,
+              long long n_out, const double* synthesis_window, const double* twiddle, void* workspace,
+              size_t workspace_bytes, double* out, void* stream) {
+  const int logN = log2_size(size);
+  PBB_CHECK_ARG(X != nullptr, 1, "X is null");
+  PBB_CHECK_ARG(rows > 0, 2, "rows must be positive");
+  PBB_CHECK_ARG(frames > 0, 3, "frames must be positive");
+  PBB_CHECK_ARG(logN > 0, 4, "size must be a power of two in [64, 4096]");
+  PBB_CHECK_ARG(window_length >= 1 && window_length <= size, 6, "window_length must be in [1, size]");
+  PBB_CHECK_ARG(shift >= 1 && shift <= window_length, 5, "shift must be in [1, window_length]");
+  const long long full = (long long)frames * shift + window_length - shift;
+  PBB_CHECK_ARG(crop >= 0, 7, "crop must be non-negative");
+  PBB_CHECK_ARG(n_out >= 0 && crop + n_out <= full, 8, "crop + n_out exceeds frames * shift + window_length - shift");
+  PBB_CHECK_ARG(synthesis_window != nullptr, 9, "synthesis_window is null");
+  PBB_CHECK_ARG(twiddle != nullptr, 10, "twiddle is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_istft_workspace_bytes(rows, frames, window_length), 11,
+                "workspace too small (pbb_istft_workspace_bytes)");
+  PBB_CHECK_ARG(out != nullptr || n_out == 0, 13, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  IstftParams p{};
+  p.X = reinterpret_cast<const double2*>(X);
+  p.rows = rows;
+  p.logM = logN - 1;
+  p.wl = window_length;
+  p.frames = frames;
+  p.fpc = frames_per_cta(size, rows, frames);
+  p.tiles = (frames + p.fpc - 1) / p.fpc;
+  p.synthesis = synthesis_window;
+  p.tw = reinterpret_cast<const double2*>(twiddle);
+  p.framebuf = reinterpret_cast<double*>(workspace);
+  const int rc = fft_launch(istft_frames_kernel, "istft_frames_kernel", rows, frames, p.fpc, size, &p, st);
+  if (rc != 0 || n_out == 0) return rc;
+  long long blocks = (rows * n_out + 255) / 256;
+  if (blocks > 4ll * 32 * sm_count()) blocks = 4ll * 32 * sm_count();
+  LaunchScope ls("overlap_add_kernel", st);
+  overlap_add_kernel<<<(unsigned)blocks, 256, 0, st>>>(p.framebuf, rows, frames, window_length, shift, crop, n_out,
+                                                       out);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"
