@@ -114,7 +114,8 @@ __global__ void gaussian_fit_partial_kernel(const double* __restrict__ x, const 
     if (threadIdx.x == 0) partial[((size_t)f * K + k) * (E + 1) + e] = s;
   }
 }
-// mean[k][e] = sum_f partial / max(denominator, tiny); denominator kept in denom[k]
+// mean[k][e] = sum_f partial / max(denominator, tiny); the unclamped denominator sum_t w is kept in denom[k]: the
+// von Mises-Fisher fit divides by it as it is (von_mises_fisher.py:137)
 __global__ void gaussian_fit_mean_kernel(const double* __restrict__ partial, int F, int E, int K,
                                          double* __restrict__ mean, double* __restrict__ denom) {
   const int k = blockIdx.x, e = threadIdx.x;
@@ -122,7 +123,7 @@ __global__ void gaussian_fit_mean_kernel(const double* __restrict__ partial, int
   double s = 0.0;
   for (int f = 0; f < F; ++f) s += partial[((size_t)f * K + k) * (E + 1) + e];
   __shared__ double den;
-  if (e == E) { den = fmax(s, kTiny); denom[k] = den; }
+  if (e == E) { den = fmax(s, kTiny); denom[k] = s; }
   __syncthreads();
   if (e < E) mean[k * E + e] = s / den;
 }
@@ -135,13 +136,13 @@ __global__ void gaussian_fit_cov_kernel(const double* __restrict__ partial, cons
     double s = 0.0;
     for (int f = 0; f < F; ++f) s += partial[((size_t)f * K + k) * (E + 1) + e];
     v[e] = s;
-    if (!spherical) cov[k * E + e] = s / denom[k];
+    if (!spherical) cov[k * E + e] = s / fmax(denom[k], kTiny);
   }
   __syncthreads();
   if (spherical && e == 0) {
     double s = 0.0;
     for (int i = 0; i < E; ++i) s += v[i];
-    cov[k] = s / (denom[k] * (double)E);
+    cov[k] = s / (fmax(denom[k], kTiny) * (double)E);
   }
 }
 

@@ -72,6 +72,12 @@ def integrated_posterior(model, spectral, od, affiliation_eps, inline_permutatio
     K = spatial.shape[1]
     assert spectral.shape == spatial.shape, (spectral.shape, spatial.shape)
     mode = _weight_layout(model.weight_constant_axis)
+    if mode == _lib.WEIGHT_CONST:
+        # the reference unsqueezes its scalar weight 1 / K to len(axes) dims (gcacgmm.py:109, utils.py:324-329): an
+        # axis below -len(axes), as in (-2,) or (-3, -2), raises IndexError there
+        axes = _axes(model.weight_constant_axis)
+        if axes[0] < -len(axes):
+            raise IndexError((), [], model.weight_constant_axis)
     w = None if mode == _lib.WEIGHT_CONST else _device.to_device(model.weight, torch.float64).contiguous()
     aff = _device.empty((F, K, T), torch.float64)
     lib = _lib.load()
