@@ -7,7 +7,6 @@ tensors out (everything stays resident in HBM).
 """
 import ctypes
 from dataclasses import dataclass, field
-from operator import xor
 
 import numpy as np
 import torch
@@ -17,54 +16,15 @@ from .complex_angular_central_gaussian import (
     ComplexAngularCentralGaussian,
     normalize_observation,
 )
+from .mixture_model_utils import (check_initialization, coupled_fit, fit_tied_leading, flatten_obs, initial_affiliation,
+                                  model_to_host, saliency_bn, status_check, weight_mode, weight_to_device,
+                                  weight_to_host)
 from .utils import _ProbabilisticModel
 
 __all__ = ['CACGMM', 'CACGMMTrainer', 'normalize_observation']
 
 _NORMS = {'eigenvalue': _lib.NORM_EIGENVALUE, 'trace': _lib.NORM_TRACE,
           False: _lib.NORM_NONE}
-
-
-def _weight_mode(weight_constant_axis, ndim):
-    """Maps ``weight_constant_axis`` (mixture_model_utils.py:133-203) onto the
-    modes the kernels implement; ``ndim`` is the affiliation rank.
-    WEIGHT_TIME: (-1,); WEIGHT_CONST: -2; WEIGHT_TIED_TIME: (-3,) and
-    WEIGHT_TIED: (-3, -1) (frequency-tied, only for a single independent dim)."""
-    if isinstance(weight_constant_axis, list):
-        weight_constant_axis = tuple(weight_constant_axis)
-    if isinstance(weight_constant_axis, int):
-        ax = weight_constant_axis % ndim - ndim
-        if ax == -2:
-            return _lib.WEIGHT_CONST  # constant 1/K, shape (K, 1)
-        axes = (ax,)
-    else:
-        axes = tuple(sorted(a % ndim - ndim for a in weight_constant_axis))
-    if axes == (-1,):
-        return _lib.WEIGHT_TIME
-    if ndim >= 3 and axes == (-3,):
-        return _lib.WEIGHT_TIED_TIME
-    if ndim >= 3 and axes == (-3, -1):
-        return _lib.WEIGHT_TIED
-    raise NotImplementedError(
-        f'weight_constant_axis={weight_constant_axis!r}: supported on the '
-        'device are (-1,), -2, (-3,) and (-3, -1) (the last independent dim, the bins, tied).')
-
-
-def _flatten_obs(y):
-    *independent, N, D = y.shape
-    F = int(np.prod(independent)) if independent else 1
-    return tuple(independent), F, N, D
-
-
-def _status_check(status, what, defer=None):
-    def on_error(s):
-        # the reference asserts finiteness at cacg.py:127,326,333
-        raise AssertionError(f'{what}: non-finite covariance / eigenvalues in bin {s - 1}')
-    if defer is not None:
-        # coupled EM loop: keep the stream full, look at every status word once after the last iteration
-        defer.append((status, what))
-        return
-    _device.check_status(status, on_error)  # synchronises the stream unless inside _device.deferred_status()
 
 
 @dataclass
@@ -74,30 +34,21 @@ class CACGMM(_ProbabilisticModel):
         default_factory=ComplexAngularCentralGaussian)
 
     # -- device views of the model ------------------------------------------------
-    def _device_model(self, independent, F, N=None):
+    def _device_model(self, independent, F, N):
         V = _device.to_device(self.cacg.covariance_eigenvectors, torch.complex128)
         lam = _device.to_device(self.cacg.covariance_eigenvalues, torch.float64)
         K, D = V.shape[-3], V.shape[-1]
         V = V.expand(*independent, K, D, D).reshape(F, K, D, D).contiguous()
         lam = lam.expand(*independent, K, D).reshape(F, K, D).contiguous()
-        w = _device.to_device(self.weight, torch.float64)
-        if w.shape[-1] != 1:
-            # frequency-tied, time-varying weights (1, K, T) of weight_constant_axis=(-3,)
-            assert w.dim() == 3 and w.shape[0] == 1 and len(independent) == 1, tuple(w.shape)
-            # the reference broadcasts weight (1, K, T) against the (F, K, N) log-pdf and fails for T != N
-            if N is not None and w.shape[-1] != N:
-                raise ValueError(f'time-varying weight has {w.shape[-1]} frames, the observation {N}')
-            return V, lam, w[0].contiguous(), K, _lib.WEIGHT_TIED_TIME
-        w = w[..., 0].expand(*independent, K).reshape(F, K).contiguous()
-        return V, lam, w, K, _lib.WEIGHT_TIME
+        return V, lam, *weight_to_device(self.weight, independent, F, K, N), K
 
     def _run_predict(self, y, source_activity_mask, affiliation_eps,
-                     want_aff=True, want_q=False, want_ll=False, defer=None):
+                     want_aff=True, want_q=False, want_ll=False):
         like_numpy = not _device.is_tensor(y)
         yd = _device.to_device(y)
         code = _device.complex_dtype_code(yd)
-        independent, F, N, D = _flatten_obs(yd)
-        V, lam, w, K, wmode = self._device_model(independent, F, N)
+        independent, F, N, D = flatten_obs(yd)
+        V, lam, w, wmode, K = self._device_model(independent, F, N)
         assert V.shape[-1] == D, (V.shape, D)
         act = None
         if source_activity_mask is not None:
@@ -117,7 +68,7 @@ class CACGMM(_ProbabilisticModel):
             float(affiliation_eps), _device.ptr(aff), _device.ptr(q),
             _device.ptr(ll), _device.ptr(ws), nbytes, _device.ptr(status),
             _device.stream_ptr()), 'pbb_cacgmm_predict')
-        _status_check(status, 'CACGMM.predict', defer)
+        status_check(status, 'CACGMM.predict')
         shape = (*independent, K, N)
         if aff is not None:
             aff = _device.to_host(aff.reshape(shape), like_numpy)
@@ -186,32 +137,26 @@ class CACGMMTrainer:
                 communicate, once per iteration.
         Returns: CACGMM
         """
-        assert xor(initialization is None, num_classes is None), (
-            'Incompatible input combination. '
-            'Exactly one of the two inputs has to be None: '
-            f'{initialization is None} xor {num_classes is None}')
+        check_initialization(initialization, num_classes)
         assert covariance_norm in _NORMS, covariance_norm
         like_numpy = not _device.is_tensor(y)
-        weight_mode_probe = _weight_mode(weight_constant_axis, y.ndim)
-        coupled = inline_permutation_aligner is not None or weight_mode_probe in (
-            _lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED)
+        mode = weight_mode(weight_constant_axis, y.ndim)
+        tied = mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED)
+        coupled = inline_permutation_aligner is not None or tied
         # pinned host tensors stay where they are: pbb_cacgmm_fit streams them in while it computes
         yd = _device.to_device(y, keep_pinned=not coupled)
         assert yd.is_complex(), yd.dtype
         assert yd.shape[-1] > 1, yd.shape
         assert iterations > 0, iterations
         code = _device.complex_dtype_code(yd)
-        independent, F, N, D = _flatten_obs(yd)
+        independent, F, N, D = flatten_obs(yd)
         assert D < 35, f'Channels: {D}, sure?'
 
         init_dev = None
         model_in = None
         if initialization is None:
             K = num_classes
-            shape = (*independent, K, N)
-            aff = np.random.uniform(size=shape)
-            aff /= np.einsum('...kn->...n', aff)[..., None, :]
-            init_dev = _device.to_device(aff, torch.float64).reshape(F, K, N)
+            init_dev = initial_affiliation(None, K, independent, N)
         elif isinstance(initialization, CACGMM):
             model_in = initialization
             K = initialization.cacg.covariance_eigenvectors.shape[-3]
@@ -231,22 +176,29 @@ class CACGMMTrainer:
         else:
             raise TypeError('No sufficient initialization.')
         assert K < 20, f'num_classes: {K}, sure?'
-        weight_mode = _weight_mode(weight_constant_axis, len(independent) + 2)
-        if weight_mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED) and len(independent) > 1:
-            # the weights are tied over the LAST independent dim (the bins); the dims in front of it stay
-            # independent problems: fit them one after the other and stack the models
-            return self._fit_tied_leading(
-                y, initialization, independent, iterations, like_numpy, saliency=saliency,
-                source_activity_mask=source_activity_mask, weight_constant_axis=weight_constant_axis,
-                hermitize=hermitize, covariance_norm=covariance_norm, affiliation_eps=affiliation_eps,
-                eigenvalue_floor=eigenvalue_floor, inline_permutation_aligner=inline_permutation_aligner)
-        if inline_permutation_aligner is not None or weight_mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED):
+        sal = saliency_bn(saliency, independent, N)
+        if tied and len(independent) > 1:
+            assert model_in is None, 'warm start with tied weights: one leading dim only'
+            model = fit_tied_leading(
+                self.fit, independent[:-1], y=yd, initialization=init_dev.reshape(*independent, K, N),
+                iterations=iterations, saliency=saliency, source_activity_mask=source_activity_mask,
+                weight_constant_axis=weight_constant_axis, hermitize=hermitize, covariance_norm=covariance_norm,
+                affiliation_eps=affiliation_eps, eigenvalue_floor=eigenvalue_floor,
+                inline_permutation_aligner=inline_permutation_aligner)
+            return model_to_host(model) if like_numpy else model
+        if coupled:
             # frequency-tied weights and the inline permutation alignment couple the bins inside the
             # EM loop (cacgmm.py:252-278): one E-step / alignment / M-step round trip per iteration
-            return self._fit_coupled(
-                yd, like_numpy, init_dev, model_in, K, iterations, saliency, source_activity_mask,
-                weight_mode, hermitize, covariance_norm, affiliation_eps, eigenvalue_floor,
-                inline_permutation_aligner, weight_constant_axis, total_bins, bin_group)
+            mask = source_activity_mask
+            if mask is not None and not _device.is_tensor(mask):
+                mask = _device.to_device(mask)   # uploaded once, not per iteration
+            model = coupled_fit(
+                yd, init_dev, model_in, iterations, weight_constant_axis, sal, inline_permutation_aligner,
+                predict=lambda m: m._run_predict(yd, mask, affiliation_eps, want_q=True)[:2],
+                m_step=lambda aff, q: cacgmm_m_step(yd, q, aff, saliency=sal, hermitize=hermitize,
+                                                    covariance_norm=covariance_norm, eigenvalue_floor=eigenvalue_floor),
+                saliency_form=sal is not None, total_bins=total_bins, bin_group=bin_group)
+            return model_to_host(model) if like_numpy else model
 
         act = None
         if source_activity_mask is not None:
@@ -257,13 +209,9 @@ class CACGMMTrainer:
                     source_activity_mask.shape, initialization.shape)
             act = _device.to_device(source_activity_mask).to(torch.uint8)
             act = act.expand(*independent, K, N).reshape(F, K, N).contiguous()
-        sal = None
-        if saliency is not None:
-            sal = _device.to_device(saliency, torch.float64)
-            sal = sal.expand(*independent, N).reshape(F, N).contiguous()
 
         if model_in is not None:
-            V, lam, w, _, wm_in = model_in._device_model(independent, F)
+            V, lam, w, wm_in, _ = model_in._device_model(independent, F, N)
             assert wm_in == _lib.WEIGHT_TIME, 'warm start with frequency-tied weights goes through the coupled loop'
             V, lam, w = V.clone(), lam.clone(), w.clone()
         elif yd.device.type == 'cpu':
@@ -278,7 +226,7 @@ class CACGMMTrainer:
         status = _device.empty((1,), torch.int32)
         opts = _lib.CacgmmOptions(
             iterations=int(iterations), covariance_norm=_NORMS[covariance_norm],
-            weight_mode=weight_mode, hermitize=int(bool(hermitize)),
+            weight_mode=mode, hermitize=int(bool(hermitize)),
             affiliation_eps=float(affiliation_eps),
             eigenvalue_floor=float(eigenvalue_floor),
             frames_per_block=int(frames_per_block),
@@ -291,130 +239,14 @@ class CACGMMTrainer:
             _device.ptr(sal), _device.ptr(act), ctypes.byref(opts),
             _device.ptr(V), _device.ptr(lam), _device.ptr(w), _device.ptr(ws),
             nbytes, _device.ptr(status), _device.stream_ptr()), 'pbb_cacgmm_fit')
-        _status_check(status, 'CACGMMTrainer.fit')
-
-        if weight_mode == _lib.WEIGHT_CONST:
-            weight = np.full([K, 1], 1 / K)  # mixture_model_utils.py:180-183
-            if not like_numpy:
-                weight = _device.to_device(weight)
-        else:
-            weight = _device.to_host(w.reshape(*independent, K, 1), like_numpy)
+        status_check(status, 'CACGMMTrainer.fit')
         return CACGMM(
-            weight=weight,
+            weight=weight_to_host(mode, w, independent, K, like_numpy),
             cacg=ComplexAngularCentralGaussian(
                 covariance_eigenvectors=_device.to_host(
                     V.reshape(*independent, K, D, D), like_numpy),
                 covariance_eigenvalues=_device.to_host(
                     lam.reshape(*independent, K, D), like_numpy)))
-
-    def _fit_tied_leading(self, y, initialization, independent, iterations, like_numpy, *, saliency,
-                          source_activity_mask, **kw):
-        """Frequency-tied weights with more than one independent dim, e.g. (B, F, T, D): every index of the leading
-        dims is its own coupled fit (the reference's mean over axis -3 keeps them apart, mixture_model_utils.py:187)."""
-        lead = tuple(independent[:-1])
-
-        def pick(x, idx):
-            if x is None or isinstance(x, CACGMM):
-                return x
-            nlead = x.ndim - (y.ndim - len(lead))     # how many of the leading dims x carries
-            if nlead <= 0:
-                return x
-            sub = tuple(i if x.shape[d] != 1 else 0 for d, i in enumerate(idx[len(lead) - nlead:]))
-            return x[sub]
-
-        assert not isinstance(initialization, CACGMM), 'warm start with tied weights: one leading dim only'
-        models = [self.fit(pick(y, idx), initialization=pick(initialization, idx), iterations=iterations,
-                           saliency=pick(saliency, idx), source_activity_mask=pick(source_activity_mask, idx), **kw)
-                  for idx in np.ndindex(*lead)]
-        stack = (lambda xs: np.stack(xs).reshape(*lead, *xs[0].shape)) if like_numpy else \
-            (lambda xs: torch.stack(xs).reshape(*lead, *xs[0].shape))
-        return CACGMM(
-            weight=stack([m.weight for m in models]),
-            cacg=ComplexAngularCentralGaussian(
-                covariance_eigenvectors=stack([m.cacg.covariance_eigenvectors for m in models]),
-                covariance_eigenvalues=stack([m.cacg.covariance_eigenvalues for m in models])))
-
-    def _fit_coupled(self, yd, like_numpy, init_dev, model_in, K, iterations, saliency, source_activity_mask,
-                     weight_mode, hermitize, covariance_norm, affiliation_eps, eigenvalue_floor, aligner,
-                     weight_constant_axis, total_bins=None, bin_group=None):
-        """EM with per-iteration coupling across bins: frequency-tied mixture weights
-        (``weight_constant_axis`` (-3,) / (-3, -1), mixture_model_utils.py:187-190) and / or the
-        inline permutation alignment (mixture_model_utils.py:264-306).  Every step runs on the
-        device; the loop itself is the reference's (cacgmm.py:252-278)."""
-        from .. import parallel
-        from ..permutation_alignment import apply_mapping
-        independent, F, N, D = _flatten_obs(yd)
-        F_all = F if total_bins is None else int(total_bins)
-        lo, hi = parallel.local_bins(F_all, bin_group) if F_all != F else (0, F)
-        assert hi - lo == F, ('this rank holds bins', (lo, hi), 'but y has', F)
-        tied = weight_mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED)
-        if aligner is not None:
-            message = ('Inline permutation alignment reduces mismatch between frequency independent '
-                       'mixtures weights and a frequency independent observation model. Therefore, we '
-                       f'require `affiliation.ndim == 3` and a corresponding `weight_constant_axis` '
-                       f'({weight_constant_axis}).')
-            assert len(independent) == 1 and tied, message
-        sal_w = None
-        if tied and saliency is not None:
-            # estimate_mixture_weight with a saliency (mixture_model_utils.py:192-203): the tied weight is the
-            # L1-normalised sum of affiliation * saliency over the bins (and frames)
-            if F_all != F:
-                raise NotImplementedError('saliency with frequency-tied weights is single-rank only')
-            sal_w = _device.to_device(saliency, torch.float64).expand(*independent, N).reshape(F, 1, N)
-        lib = _lib.load()
-        model = model_in
-        affiliation = init_dev.reshape(*independent, K, N) if init_dev is not None else None
-        quadratic_form = None
-        m_axis = (-1,) if tied else weight_constant_axis
-        # no host synchronisation inside the loop: the per-call status words are collected and read once at the end
-        pending = []
-        if source_activity_mask is not None and not _device.is_tensor(source_activity_mask):
-            source_activity_mask = _device.to_device(source_activity_mask)   # uploaded once, not per iteration
-        for _ in range(iterations):
-            if model is not None:
-                affiliation, quadratic_form, _, _ = model._run_predict(
-                    yd, source_activity_mask, affiliation_eps, want_q=True, defer=pending)
-                if aligner is not None:
-                    mask_kft = affiliation.permute(1, 0, 2).contiguous()
-                    if F_all != F:  # the alignment needs every bin: gather, align replicated, keep the slice
-                        every = parallel.all_gather_bins(affiliation.contiguous(), F_all, bin_group)
-                        mapping = aligner.calculate_mapping(every.permute(1, 0, 2).contiguous())[:, lo:hi].contiguous()
-                    else:
-                        mapping = aligner.calculate_mapping(mask_kft)
-                    affiliation = apply_mapping(mask_kft, mapping).permute(1, 0, 2).contiguous()
-                    quadratic_form = apply_mapping(quadratic_form.permute(1, 0, 2).contiguous(),
-                                                   mapping).permute(1, 0, 2).contiguous()
-            model = cacgmm_m_step(
-                yd, quadratic_form, affiliation, saliency=saliency, hermitize=hermitize,
-                covariance_norm=covariance_norm, eigenvalue_floor=eigenvalue_floor,
-                weight_constant_axis=m_axis, defer=pending)
-            if tied:
-                aff = affiliation.reshape(F, K, N)
-                if sal_w is not None:
-                    aff = aff * sal_w
-                aff = aff.contiguous()
-                w_kt = _device.empty((K, N), torch.float64)
-                w_k = _device.empty((K,), torch.float64)
-                flags = int(weight_mode == _lib.WEIGHT_TIED) | (2 if sal_w is not None else 0)
-                _lib.check(lib.pbb_mixture_weight_over_bins(
-                    _device.ptr(aff), F, K, N, flags, _device.ptr(w_kt),
-                    _device.ptr(w_k), _device.stream_ptr()), 'pbb_mixture_weight_over_bins')
-                if F_all != F:  # sum over the other ranks' bins
-                    w_kt = parallel.mean_over_all_bins(w_kt, F, F_all, bin_group)
-                    w_k = parallel.mean_over_all_bins(w_k, F, F_all, bin_group)
-                model.weight = w_kt[None] if weight_mode == _lib.WEIGHT_TIED_TIME else w_k[None, :, None]
-        if pending:
-            words = torch.stack([st.reshape(()) for st, _ in pending]).cpu().tolist()   # the one synchronisation
-            for s_, (_, what) in zip(words, pending):
-                if s_ != 0:
-                    raise AssertionError(f'{what}: non-finite covariance / eigenvalues in bin {s_ - 1}')
-        if like_numpy:
-            model = CACGMM(
-                weight=_device.to_host(model.weight, True) if _device.is_tensor(model.weight) else model.weight,
-                cacg=ComplexAngularCentralGaussian(
-                    covariance_eigenvectors=_device.to_host(model.cacg.covariance_eigenvectors, True),
-                    covariance_eigenvalues=_device.to_host(model.cacg.covariance_eigenvalues, True)))
-        return model
 
     def fit_predict(self, y, initialization=None, num_classes=None,
                     iterations=100, **kwargs):
@@ -441,7 +273,7 @@ class CACGMMTrainer:
 
 def cacgmm_m_step(y, quadratic_form, affiliation, *, saliency=None,
                   hermitize=True, covariance_norm='eigenvalue',
-                  eigenvalue_floor=1e-10, weight_constant_axis=(-1,), defer=None):
+                  eigenvalue_floor=1e-10, weight_constant_axis=(-1,)):
     """One M-step from given affiliations / quadratic forms (``pbb_cacgmm_mstep``).
 
     estimate_mixture_weight (mixture_model_utils.py:133-203) +
@@ -452,7 +284,7 @@ def cacgmm_m_step(y, quadratic_form, affiliation, *, saliency=None,
     like_numpy = not _device.is_tensor(y)
     yd = _device.to_device(y)
     code = _device.complex_dtype_code(yd)
-    independent, F, N, D = _flatten_obs(yd)
+    independent, F, N, D = flatten_obs(yd)
     aff = _device.to_device(affiliation, torch.float64)
     K = aff.shape[-2]
     aff = aff.expand(*independent, K, N).reshape(F, K, N).contiguous()
@@ -464,14 +296,14 @@ def cacgmm_m_step(y, quadratic_form, affiliation, *, saliency=None,
     if saliency is not None:
         sal = _device.to_device(saliency, torch.float64)
         sal = sal.expand(*independent, N).reshape(F, N).contiguous()
-    weight_mode = _weight_mode(weight_constant_axis, len(independent) + 2)
+    mode = weight_mode(weight_constant_axis, len(independent) + 2)
     V = _device.empty((F, K, D, D), torch.complex128)
     lam = _device.empty((F, K, D), torch.float64)
     w = _device.empty((F, K), torch.float64)
     status = _device.empty((1,), torch.int32)
     opts = _lib.CacgmmOptions(
         iterations=1, covariance_norm=_NORMS[covariance_norm],
-        weight_mode=weight_mode, hermitize=int(bool(hermitize)),
+        weight_mode=mode, hermitize=int(bool(hermitize)),
         affiliation_eps=0., eigenvalue_floor=float(eigenvalue_floor),
         frames_per_block=0, reserved=0)
     lib = _lib.load()
@@ -482,15 +314,9 @@ def cacgmm_m_step(y, quadratic_form, affiliation, *, saliency=None,
         _device.ptr(sal), ctypes.byref(opts), _device.ptr(V), _device.ptr(lam),
         _device.ptr(w), _device.ptr(ws), nbytes, _device.ptr(status),
         _device.stream_ptr()), 'pbb_cacgmm_mstep')
-    _status_check(status, 'cacgmm_m_step', defer)
-    if weight_mode == _lib.WEIGHT_CONST:
-        weight = np.full([K, 1], 1 / K)
-        if not like_numpy:
-            weight = _device.to_device(weight)
-    else:
-        weight = _device.to_host(w.reshape(*independent, K, 1), like_numpy)
+    status_check(status, 'cacgmm_m_step')
     return CACGMM(
-        weight=weight,
+        weight=weight_to_host(mode, w, independent, K, like_numpy),
         cacg=ComplexAngularCentralGaussian(
             covariance_eigenvectors=_device.to_host(
                 V.reshape(*independent, K, D, D), like_numpy),

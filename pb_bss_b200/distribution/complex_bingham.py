@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from .. import _device, _lib
-from .cacgmm import _flatten_obs
+from .mixture_model_utils import flatten_obs
 from .utils import _ProbabilisticModel
 
 __all__ = ['ComplexBingham', 'ComplexBinghamTrainer']
@@ -180,7 +180,7 @@ class ComplexBinghamTrainer:
         observations of fit() and of the mixture model unchanged."""
         like_numpy = not _device.is_tensor(y)
         yd = _device.to_device(y)
-        independent, F, N, D = _flatten_obs(yd)
+        independent, F, N, D = flatten_obs(yd)
         _check_dimension(D)
         if saliency is None:
             aff = torch.ones((F, 1, N), dtype=torch.float64, device=yd.device)
@@ -196,7 +196,7 @@ class ComplexBinghamTrainer:
 def _cbmm_fit_device(yd, init, sal, K, iterations, weight_mode, affiliation_eps, eigenvalue_eps,
                      max_concentration, what):
     """One ``pbb_cbmm_fit`` call: (eigenvectors (F, K, D, D), eigenvalues (F, K, D), weight (F, K)) tensors."""
-    independent, F, N, D = _flatten_obs(yd)
+    independent, F, N, D = flatten_obs(yd)
     _check_dimension(D)
     code = _device.complex_dtype_code(yd)
     V = _device.empty((F, K, D, D), torch.complex128)

@@ -3,14 +3,15 @@
 the kernels behind ``pbb_cwmm_fit`` / ``pbb_cwmm_predict``."""
 from dataclasses import dataclass
 from functools import cached_property
-from operator import xor
 
 import numpy as np
 import torch
 
 from .. import _device, _lib
-from .cacgmm import _flatten_obs, _status_check, _weight_mode
 from .complex_watson import ComplexWatson, ComplexWatsonTrainer
+from .mixture_model_utils import (check_initialization, coupled_fit, fit_tied_leading, flatten_obs, initial_affiliation,
+                                  model_to_host, saliency_bn, status_check, weight_mode, weight_to_device,
+                                  weight_to_host)
 from .utils import _ProbabilisticModel
 
 __all__ = ['CWMM', 'CWMMTrainer']
@@ -26,22 +27,14 @@ class CWMM(_ProbabilisticModel):
         like_numpy = not _device.is_tensor(y)
         yd = _device.to_device(y)
         code = _device.complex_dtype_code(yd)
-        independent, F, N, D = _flatten_obs(yd)
+        independent, F, N, D = flatten_obs(yd)
         mode = _device.to_device(self.complex_watson.mode, torch.complex128)
         K = mode.shape[-2]
         assert mode.shape[-1] == D, (mode.shape, D)
         mode = mode.expand(*independent, K, D).reshape(F, K, D).contiguous()
         kappa = _device.to_device(self.complex_watson.concentration, torch.float64)
         kappa = kappa.expand(*independent, K).reshape(F, K).contiguous()
-        w = _device.to_device(self.weight, torch.float64)
-        wmode = _lib.WEIGHT_TIME
-        if w.shape[-1] != 1:
-            # frequency-tied weights (weight_constant_axis=(-3,), mixture_model_utils.py:187-190): (1, K, N)
-            assert w.shape[-1] == N and all(int(n) == 1 for n in w.shape[:-2]), (w.shape, N)
-            w = w.reshape(K, N).contiguous()
-            wmode = _lib.WEIGHT_TIED_TIME
-        else:
-            w = w[..., 0].expand(*independent, K).reshape(F, K).contiguous()
+        w, wmode = weight_to_device(self.weight, independent, F, K, N)
         aff = _device.empty((F, K, N), torch.float64)
         status = _device.empty((1,), torch.int32)
         lib = _lib.load()
@@ -52,7 +45,7 @@ class CWMM(_ProbabilisticModel):
             _device.ptr(kappa), _device.ptr(w), wmode, _device.ptr(aff),
             _device.ptr(ws), nbytes, _device.ptr(status),
             _device.stream_ptr()), 'pbb_cwmm_predict')
-        _status_check(status, 'CWMM.predict')
+        status_check(status, 'CWMM.predict')
         return _device.to_host(aff.reshape(*independent, K, N), like_numpy)
 
 
@@ -77,29 +70,17 @@ class CWMMTrainer:
         y: (..., T, D); initialization: affiliations (..., K, T) or None with
         ``num_classes`` (then drawn from NumPy's global RNG, cwmm.py:121-127).
         """
-        assert xor(initialization is None, num_classes is None), (
-            'Incompatible input combination. '
-            'Exactly one of the two inputs has to be None: '
-            f'{initialization is None} xor {num_classes is None}')
+        check_initialization(initialization, num_classes)
         assert affiliation_eps == 0, affiliation_eps  # cwmm.py:161
         like_numpy = not _device.is_tensor(y)
         yd = _device.to_device(y)
         assert yd.is_complex(), yd.dtype
         assert yd.shape[-1] > 1
         assert iterations > 0, iterations
-        code = _device.complex_dtype_code(yd)
-        independent, F, N, D = _flatten_obs(yd)
-        if initialization is None:
-            shape = (*independent, num_classes, N)
-            initialization = np.random.uniform(size=shape)
-            initialization /= np.einsum('...kn->...n', initialization)[..., None, :]
-        K = initialization.shape[-2]
-        init = _device.to_device(initialization, torch.float64)
-        init = init.expand(*independent, K, N).reshape(F, K, N).contiguous()
-        sal = None
-        if saliency is not None:
-            sal = _device.to_device(saliency, torch.float64)
-            sal = sal.expand(*independent, N).reshape(F, N).contiguous()
+        independent, F, N, D = flatten_obs(yd)
+        init = initial_affiliation(initialization, num_classes, independent, N)
+        K = init.shape[-2]
+        sal = saliency_bn(saliency, independent, N)
         if self.dimension is None:
             self.dimension = D
         else:
@@ -107,18 +88,29 @@ class CWMMTrainer:
                 'You initialized the trainer with a different dimension than '
                 'you are using to fit a model. Use a new trainer, when you '
                 'change the dimension.')
-        weight_mode = _weight_mode(weight_constant_axis, len(independent) + 2)
-        tied = weight_mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED)
-        if inline_permutation_aligner is not None or tied:
-            return self._fit_coupled(yd, like_numpy, init, sal, K, iterations, weight_mode,
-                                     inline_permutation_aligner, weight_constant_axis)
-        return self._fit_device(yd, like_numpy, init, sal, K, iterations, weight_mode)
+        mode = weight_mode(weight_constant_axis, len(independent) + 2)
+        tied = mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED)
+        if tied and len(independent) > 1:
+            model = fit_tied_leading(
+                self.fit, independent[:-1], y=yd, initialization=init.reshape(*independent, K, N),
+                iterations=iterations, saliency=saliency, weight_constant_axis=weight_constant_axis,
+                inline_permutation_aligner=inline_permutation_aligner)
+        elif inline_permutation_aligner is not None or tied:
+            # mode / concentration of every (bin, class) from the affiliations: pbb_cwmm_fit with one iteration
+            model = coupled_fit(
+                yd, init, None, iterations, weight_constant_axis, sal, inline_permutation_aligner,
+                predict=lambda m: (m.predict(yd), None),
+                m_step=lambda aff, q: self._fit_device(yd, False, aff, sal, K, 1, _lib.WEIGHT_TIME),
+                saliency_form=True)
+        else:
+            return self._fit_device(yd, like_numpy, init, sal, K, iterations, mode)
+        return model_to_host(model) if like_numpy else model
 
     def _fit_device(self, yd, like_numpy, init, sal, K, iterations, weight_mode):
         """All iterations in one C-ABI call (bins independent).  With ``iterations=1`` this is exactly the
         reference's ``_m_step`` from the given affiliations (cwmm.py:220-240)."""
         code = _device.complex_dtype_code(yd)
-        independent, F, N, D = _flatten_obs(yd)
+        independent, F, N, D = flatten_obs(yd)
         t_dev, c_dev = self.complex_watson_trainer.device_spline_table()
         mode = _device.empty((F, K, D), torch.complex128)
         kappa = _device.empty((F, K), torch.float64)
@@ -134,61 +126,12 @@ class CWMMTrainer:
             float(self.max_concentration), _device.ptr(mode),
             _device.ptr(kappa), _device.ptr(w), _device.ptr(ws), nbytes,
             _device.ptr(status), _device.stream_ptr()), 'pbb_cwmm_fit')
-        _status_check(status, 'CWMMTrainer.fit')
-        if weight_mode == _lib.WEIGHT_CONST:
-            weight = np.full([K, 1], 1 / K)
-            if not like_numpy:
-                weight = _device.to_device(weight)
-        else:
-            weight = _device.to_host(w.reshape(*independent, K, 1), like_numpy)
+        status_check(status, 'CWMMTrainer.fit')
         return CWMM(
-            weight=weight,
+            weight=weight_to_host(weight_mode, w, independent, K, like_numpy),
             complex_watson=ComplexWatson(
                 mode=_device.to_host(mode.reshape(*independent, K, D), like_numpy),
                 concentration=_device.to_host(kappa.reshape(*independent, K), like_numpy)))
-
-    def _fit_coupled(self, yd, like_numpy, init, sal, K, iterations, weight_mode, aligner, weight_constant_axis):
-        """EM with per-iteration coupling across bins (cwmm.py:152-184): frequency-tied weights
-        (``weight_constant_axis`` (-3,) / (-3, -1)) and / or the inline permutation alignment
-        (mixture_model_utils.py:264-306).  Every step runs on the device."""
-        from ..permutation_alignment import apply_mapping
-        independent, F, N, D = _flatten_obs(yd)
-        tied = weight_mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED)
-        if aligner is not None:
-            message = ('Inline permutation alignment reduces mismatch between frequency independent '
-                       'mixtures weights and a frequency independent observation model. Therefore, we '
-                       f'require `affiliation.ndim == 3` and a corresponding `weight_constant_axis` '
-                       f'({weight_constant_axis}).')
-            assert len(independent) == 1 and tied, message
-        lib = _lib.load()
-        affiliation = init
-        model = None
-        for _ in range(iterations):
-            if model is not None:
-                affiliation = model.predict(yd).reshape(F, K, N)
-                if aligner is not None:
-                    mask_kft = affiliation.permute(1, 0, 2).contiguous()
-                    mapping = aligner.calculate_mapping(mask_kft)
-                    affiliation = apply_mapping(mask_kft, mapping).permute(1, 0, 2).contiguous()
-            # mode / concentration of every (bin, class) from the affiliations; per-bin weights unless tied
-            model = self._fit_device(yd, False, affiliation.contiguous(), sal, K, 1,
-                                     _lib.WEIGHT_TIME if tied else weight_mode)
-            if tied:
-                w_kt = _device.empty((K, N), torch.float64)
-                w_k = _device.empty((K,), torch.float64)
-                flags = (1 if weight_mode == _lib.WEIGHT_TIED else 0) | 2
-                # with a saliency the tied weight sums affiliation * saliency (mixture_model_utils.py:192-203)
-                aff_w = (affiliation * sal[:, None, :] if sal is not None else affiliation).contiguous()
-                _lib.check(lib.pbb_mixture_weight_over_bins(
-                    _device.ptr(aff_w), F, K, N, flags, _device.ptr(w_kt), _device.ptr(w_k),
-                    _device.stream_ptr()), 'pbb_mixture_weight_over_bins')
-                model.weight = w_kt[None] if weight_mode == _lib.WEIGHT_TIED_TIME else w_k[None, :, None]
-        if like_numpy:
-            model = CWMM(
-                weight=_device.to_host(model.weight, True) if _device.is_tensor(model.weight) else model.weight,
-                complex_watson=ComplexWatson(mode=_device.to_host(model.complex_watson.mode, True),
-                                             concentration=_device.to_host(model.complex_watson.concentration, True)))
-        return model
 
     def fit_predict(self, y, initialization=None, num_classes=None,
                     iterations=100, **kwargs):

@@ -5,19 +5,20 @@ Same class / argument names and defaults as the reference.  Every array of size 
 quadratic form and the cACG M-step are the cACGMM kernels (``pbb_cacgmm_predict`` / ``pbb_cacgmm_mstep``), the
 spectral log pdf, the Gaussian fit, the posterior (with the optional per-bin pairing of spatial and spectral classes)
 and the class weights are the kernels of ``csrc/api_integration.cu``.  The Gaussians are tied over all bins, so the
-EM loop is a per-iteration sequence of launches like the frequency-tied cACGMM (``CACGMMTrainer._fit_coupled``)."""
+EM loop is a per-iteration sequence of launches like the frequency-tied cACGMM (``mixture_model_utils.coupled_fit``)."""
 import ctypes
 from dataclasses import dataclass
-from operator import xor
 from typing import Any
 
 import numpy as np
 import torch
 
 from .. import _device, _lib
-from .cacgmm import CACGMM, _NORMS, _status_check
+from .cacgmm import CACGMM, _NORMS
 from .complex_angular_central_gaussian import ComplexAngularCentralGaussian
 from .gaussian import gaussian_fit_fkt
+from .mixture_model_utils import (check_initialization, initial_affiliation, masked_affiliation, model_to_host,
+                                  saliency_bn, status_check)
 from .utils import _ProbabilisticModel
 
 
@@ -128,16 +129,8 @@ def cacg_m_step(od, affiliation, quadratic_form, sal, hermitize, covariance_norm
         _device.ptr(quadratic_form), _device.ptr(sal), ctypes.byref(opts), _device.ptr(V), _device.ptr(lam),
         _device.ptr(w_unused), _device.ptr(ws), nbytes, _device.ptr(status), _device.stream_ptr()),
         'pbb_cacgmm_mstep')
-    _status_check(status, what)
+    status_check(status, what)
     return ComplexAngularCentralGaussian(covariance_eigenvectors=V, covariance_eigenvalues=lam)
-
-
-def model_to_host(model):
-    model.weight = _device.to_host(model.weight, True) if _device.is_tensor(model.weight) else model.weight
-    model.cacg = ComplexAngularCentralGaussian(
-        covariance_eigenvectors=_device.to_host(model.cacg.covariance_eigenvectors, True),
-        covariance_eigenvalues=_device.to_host(model.cacg.covariance_eigenvalues, True))
-    return model
 
 
 @dataclass
@@ -170,10 +163,7 @@ class GCACGMMTrainer:
             fixed_covariance=None, affiliation_eps=1e-10, weight_constant_axis=(-1,), spatial_weight=1.,
             spectral_weight=1., inline_permutation_alignment=False) -> GCACGMM:
         """EM of the integrated model, signature and semantics of gcacgmm.py:131-227."""
-        assert xor(initialization is None, num_classes is None), (
-            'Incompatible input combination. '
-            'Exactly one of the two inputs has to be None: '
-            f'{initialization is None} xor {num_classes is None}')
+        check_initialization(initialization, num_classes)
         like_numpy = not _device.is_tensor(observation)
         od = _unit_norm_obs(observation)
         assert not (embedding.is_complex() if _device.is_tensor(embedding) else np.iscomplexobj(embedding)), (
@@ -182,12 +172,8 @@ class GCACGMMTrainer:
         assert od.shape[-1] > 1
         F, T, D = od.shape
         assert ed.shape[:2] == (F, T), (ed.shape, od.shape)
-        if initialization is None:
-            initialization = np.random.uniform(size=(F, num_classes, T))   # gcacgmm.py:187-192, host stream
-            initialization /= np.einsum('...kt->...t', initialization)[..., None, :]
-        affiliation = _device.to_device(initialization, torch.float64).contiguous()
-        K = affiliation.shape[-2]
-        sal = None if saliency is None else _device.to_device(saliency, torch.float64).contiguous()
+        affiliation = initial_affiliation(initialization, num_classes, (F,), T)   # gcacgmm.py:187-192, host stream
+        sal = saliency_bn(saliency, (F,), T)
         quadratic_form = None
         model = None
         for _ in range(iterations):
@@ -208,7 +194,7 @@ class GCACGMMTrainer:
     def _m_step(self, od, ed, quadratic_form, affiliation, sal, hermitize, covariance_norm, eigenvalue_floor,
                 covariance_type, fixed_covariance, weight_constant_axis, spatial_weight, spectral_weight):
         """gcacgmm.py:269-333 on device tensors."""
-        masked = affiliation if sal is None else (affiliation * sal[:, None, :]).contiguous()
+        masked = masked_affiliation(affiliation, sal)
         weight = class_weights(masked, weight_constant_axis)
         gaussian = gaussian_fit_fkt(ed, masked, covariance_type)
         if fixed_covariance is not None:

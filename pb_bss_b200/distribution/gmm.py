@@ -10,7 +10,6 @@ with the leading dims as its bin axis).  All arithmetic is float64.  NumPy in gi
 CUDA tensors out (the diagonal / spherical parameters are host arrays, as in the integrated model)."""
 import math
 from dataclasses import dataclass
-from operator import xor
 from typing import Any
 
 import numpy as np
@@ -19,6 +18,7 @@ import torch
 from .. import _device, _lib
 from .gaussian import (_ILL_DEFINED, MAX_K, DiagonalGaussian, Gaussian, SphericalGaussian, _dev, _is_real,
                        check_embedding_dim, full_fit_bkn, full_log_pdf_bkn, precision_cholesky, small_log_pdf_kn)
+from .mixture_model_utils import check_initialization, initial_affiliation, masked_affiliation, saliency_bn
 from .utils import _ProbabilisticModel
 
 
@@ -91,25 +91,6 @@ def posterior(log_pdf, mode, w):
     return aff
 
 
-def initial_affiliation(initialization, num_classes, lead, N):
-    """The reference's random initialisation from NumPy's global stream (gmm.py:71-76, vmfmm.py:80-85), or the given
-    one broadcast to the leading dims -> (B, K, N) device."""
-    if initialization is None:
-        initialization = np.random.uniform(size=(*lead, num_classes, N))
-        initialization /= np.einsum('...kn->...n', initialization)[..., None, :]
-    aff = _dev(initialization)
-    K = aff.shape[-2]
-    return aff.expand(lead + (K, N)).reshape(math.prod(lead), K, N).contiguous()
-
-
-def saliency_bn(saliency, lead, N):
-    return None if saliency is None else _dev(saliency).expand(lead + (N,)).reshape(math.prod(lead), N).contiguous()
-
-
-def masked_affiliation(aff, sal):
-    return aff if sal is None else (aff * sal[:, None, :]).contiguous()
-
-
 def _gaussian_log_pdf_bkn(gaussian, x, lead):
     """x (B, N, E) device with leading dims lead -> (B, K, N) for the GMM's Gaussian (model dims (..., K))."""
     B, N, E = x.shape
@@ -155,10 +136,7 @@ class GMMTrainer:
     def fit(self, y, initialization=None, num_classes=None, iterations=100, *, saliency=None,
             weight_constant_axis=(-1,), covariance_type='full', fixed_covariance=None):
         """EM of gmm.py:33-89: y (..., N, E), initialization (..., K, N), saliency (..., N)."""
-        assert xor(initialization is None, num_classes is None), (
-            'Incompatible input combination. '
-            'Exactly one of the two inputs has to be None: '
-            f'{initialization is None} xor {num_classes is None}')
+        check_initialization(initialization, num_classes)
         assert _is_real(y), y.dtype
         return self._fit(y, initialization=initialization, num_classes=num_classes, iterations=iterations,
                          saliency=saliency, weight_constant_axis=weight_constant_axis,

@@ -1,0 +1,200 @@
+"""The EM plumbing the mixture-model trainers share (pb_bss/distribution/mixture_model_utils.py): the fit preamble,
+the weight layouts between the public models and the kernels, models to NumPy, and the EM loop whose bins couple in
+every iteration (frequency-tied mixture weights, inline permutation alignment) for cACGMM, CWMM and CBMM."""
+import copy
+import dataclasses
+import math
+from operator import xor
+
+import numpy as np
+import torch
+
+from .. import _device, _lib
+from .gaussian import _dev
+from .utils import _ProbabilisticModel
+
+
+def check_initialization(initialization, num_classes):
+    assert xor(initialization is None, num_classes is None), (
+        'Incompatible input combination. '
+        'Exactly one of the two inputs has to be None: '
+        f'{initialization is None} xor {num_classes is None}')
+
+
+def flatten_obs(y):
+    *independent, N, D = y.shape
+    F = int(np.prod(independent)) if independent else 1
+    return tuple(independent), F, N, D
+
+
+def weight_mode(weight_constant_axis, ndim):
+    """Maps ``weight_constant_axis`` (mixture_model_utils.py:133-203) onto the
+    modes the kernels implement; ``ndim`` is the affiliation rank.
+    WEIGHT_TIME: (-1,); WEIGHT_CONST: -2; WEIGHT_TIED_TIME: (-3,) and
+    WEIGHT_TIED: (-3, -1) (frequency-tied, only for a single independent dim)."""
+    if isinstance(weight_constant_axis, list):
+        weight_constant_axis = tuple(weight_constant_axis)
+    if isinstance(weight_constant_axis, int):
+        ax = weight_constant_axis % ndim - ndim
+        if ax == -2:
+            return _lib.WEIGHT_CONST  # constant 1/K, shape (K, 1)
+        axes = (ax,)
+    else:
+        axes = tuple(sorted(a % ndim - ndim for a in weight_constant_axis))
+    if axes == (-1,):
+        return _lib.WEIGHT_TIME
+    if ndim >= 3 and axes == (-3,):
+        return _lib.WEIGHT_TIED_TIME
+    if ndim >= 3 and axes == (-3, -1):
+        return _lib.WEIGHT_TIED
+    raise NotImplementedError(
+        f'weight_constant_axis={weight_constant_axis!r}: supported on the '
+        'device are (-1,), -2, (-3,) and (-3, -1) (the last independent dim, the bins, tied).')
+
+
+def status_check(status, what):
+    """Reads a cACGMM / CWMM status word now (synchronises the stream) or at the end of the enclosing
+    ``_device.deferred_status()`` block."""
+    def on_error(s):
+        # the reference asserts finiteness at cacg.py:127,326,333
+        raise AssertionError(f'{what}: non-finite covariance / eigenvalues in bin {s - 1}')
+    _device.check_status(status, on_error)
+
+
+def initial_affiliation(initialization, num_classes, lead, N):
+    """The reference's random initialisation from NumPy's global stream (gmm.py:71-76, vmfmm.py:80-85), or the given
+    one broadcast to the leading dims -> (B, K, N) device."""
+    if initialization is None:
+        initialization = np.random.uniform(size=(*lead, num_classes, N))
+        initialization /= np.einsum('...kn->...n', initialization)[..., None, :]
+    aff = _dev(initialization)
+    K = aff.shape[-2]
+    return aff.expand(lead + (K, N)).reshape(math.prod(lead), K, N).contiguous()
+
+
+def saliency_bn(saliency, lead, N):
+    return None if saliency is None else _dev(saliency).expand(lead + (N,)).reshape(math.prod(lead), N).contiguous()
+
+
+def masked_affiliation(aff, sal):
+    return aff if sal is None else (aff * sal[:, None, :]).contiguous()
+
+
+def weight_to_device(weight, independent, F, K, N):
+    """A model's weight -> (device weight, mode) for the predict kernels: (..., K, 1) -> (F, K) WEIGHT_TIME; the
+    time-varying weight (..., K, T) of weight_constant_axis=(-3,), shared by every bin -> (K, T) WEIGHT_TIED_TIME."""
+    w = _device.to_device(weight, torch.float64)
+    if w.shape[-1] == 1:
+        return w[..., 0].expand(*independent, K).reshape(F, K).contiguous(), _lib.WEIGHT_TIME
+    assert all(int(n) == 1 for n in w.shape[:-2]), (tuple(w.shape), independent)
+    # the reference broadcasts the weight against the (..., K, N) log pdf, which fails for T != N
+    if w.shape[-1] != N:
+        raise ValueError(f'time-varying weight has {w.shape[-1]} frames, the observation {N}')
+    return w.reshape(K, N).contiguous(), _lib.WEIGHT_TIED_TIME
+
+
+def weight_to_host(mode, w, independent, K, like_numpy):
+    """The per-bin weight (F, K) of a fit -> the reference's (..., K, 1), or (K, 1) of 1/K for WEIGHT_CONST."""
+    if mode == _lib.WEIGHT_CONST:
+        weight = np.full([K, 1], 1 / K)  # mixture_model_utils.py:180-183
+        return weight if like_numpy else _device.to_device(weight)
+    return _device.to_host(w.reshape(*independent, K, 1), like_numpy)
+
+
+def _walk(models, leaf):
+    """A copy of ``models[0]`` whose every field is ``leaf`` of that field of all ``models``; fields that are models
+    themselves are walked the same way.  No constructor runs, so nothing is recomputed."""
+    out = copy.copy(models[0])
+    for f in dataclasses.fields(out):
+        values = [getattr(m, f.name) for m in models]
+        setattr(out, f.name, _walk(values, leaf) if isinstance(values[0], _ProbabilisticModel) else leaf(values))
+    return out
+
+
+def model_to_host(model):
+    """The model with every tensor, also those of its sub-models, as a NumPy array; other fields stay as they are."""
+    return _walk([model], lambda v: _device.to_host(v[0], True) if _device.is_tensor(v[0]) else v[0])
+
+
+# trailing dims of the trainers' array arguments; the dims in front of them are the leading independent dims
+_TRAILING_DIMS = {'y': 3, 'initialization': 3, 'saliency': 2, 'source_activity_mask': 3}
+
+
+def fit_tied_leading(fit, lead, **kwargs):
+    """Frequency-tied weights with more than one independent dim, e.g. y (B, F, T, D): the weights are tied over the
+    last independent dim (the bins) only, the reference's mean over axis -3 keeps the leading indices apart
+    (mixture_model_utils.py:187).  So every index of ``lead`` is its own ``fit(**kwargs)``, with the array arguments
+    picked at that index (singleton dims broadcast), and the models are stacked to (*lead, ...)."""
+    def pick(name, x, idx):
+        nlead = x.ndim - _TRAILING_DIMS[name] if name in _TRAILING_DIMS and x is not None else 0
+        if nlead <= 0:
+            return x
+        return x[tuple(i if x.shape[d] != 1 else 0 for d, i in enumerate(idx[len(lead) - nlead:]))]
+
+    def stack(values):
+        x = torch.stack(values) if _device.is_tensor(values[0]) else np.stack(values)
+        return x.reshape(*lead, *values[0].shape)
+    models = [fit(**{k: pick(k, v, idx) for k, v in kwargs.items()}) for idx in np.ndindex(*lead)]
+    return _walk(models, stack)
+
+
+def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, aligner, predict, m_step,
+                saliency_form, total_bins=None, bin_group=None):
+    """EM whose bins couple in every iteration: frequency-tied mixture weights (``weight_constant_axis`` (-3,) /
+    (-3, -1), mixture_model_utils.py:187-190) and / or the inline permutation alignment
+    (mixture_model_utils.py:264-306).  The loop is the reference's (cacgmm.py:252-278, cwmm.py:152-184,
+    cbmm.py:186-203); every step runs on the device and the status words are read once, after the last iteration.
+
+    yd: (F, N, D) device observation; affiliation: initial (F, K, N) device affiliations, or ``model`` to start from;
+    sal: (F, N) device saliency or None.  ``predict(model)`` -> (affiliation (F, K, N), quadratic form or None);
+    ``m_step(affiliation, quadratic_form)`` -> model with per-bin weights, which then get the tied weight.
+    saliency_form: L1-normalise the tied weight over the classes (flag bit 1 of ``pbb_mixture_weight_over_bins``).
+    total_bins, bin_group: ``yd`` holds this rank's slice of ``total_bins`` bins (pb_bss_b200.parallel).
+    Returns the model of device tensors."""
+    from .. import parallel
+    from ..permutation_alignment import apply_mapping
+    independent, F, N, _ = flatten_obs(yd)
+    mode = weight_mode(weight_constant_axis, len(independent) + 2)
+    if aligner is not None:
+        message = ('Inline permutation alignment reduces mismatch between frequency independent '
+                   'mixtures weights and a frequency independent observation model. Therefore, we '
+                   f'require `affiliation.ndim == 3` and a corresponding `weight_constant_axis` '
+                   f'({weight_constant_axis}).')
+        assert len(independent) == 1 and mode in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED), message
+    F_all = F if total_bins is None else int(total_bins)
+    lo, hi = parallel.local_bins(F_all, bin_group) if F_all != F else (0, F)
+    assert hi - lo == F, ('this rank holds bins', (lo, hi), 'but y has', F)
+    if sal is not None and F_all != F:
+        raise NotImplementedError('saliency with frequency-tied weights is single-rank only')
+    lib = _lib.load()
+    quadratic_form = None
+    with _device.deferred_status():
+        for _ in range(iterations):
+            if model is not None:
+                affiliation, quadratic_form = predict(model)
+                if aligner is not None:
+                    mask_kft = affiliation.permute(1, 0, 2).contiguous()
+                    if F_all != F:  # the alignment needs every bin: gather, align replicated, keep the slice
+                        every = parallel.all_gather_bins(affiliation.contiguous(), F_all, bin_group)
+                        mapping = aligner.calculate_mapping(every.permute(1, 0, 2).contiguous())[:, lo:hi].contiguous()
+                    else:
+                        mapping = aligner.calculate_mapping(mask_kft)
+                    affiliation = apply_mapping(mask_kft, mapping).permute(1, 0, 2).contiguous()
+                    if quadratic_form is not None:
+                        quadratic_form = apply_mapping(quadratic_form.permute(1, 0, 2).contiguous(),
+                                                       mapping).permute(1, 0, 2).contiguous()
+            model = m_step(affiliation, quadratic_form)
+            # the tied weight: with a saliency, the sum of affiliation * saliency (mixture_model_utils.py:192-203)
+            K = affiliation.shape[1]
+            masked = masked_affiliation(affiliation, sal).contiguous()
+            w_kt = _device.empty((K, N), torch.float64)
+            w_k = _device.empty((K,), torch.float64)
+            flags = int(mode == _lib.WEIGHT_TIED) | (2 if saliency_form else 0)
+            _lib.check(lib.pbb_mixture_weight_over_bins(
+                _device.ptr(masked), F, K, N, flags, _device.ptr(w_kt), _device.ptr(w_k),
+                _device.stream_ptr()), 'pbb_mixture_weight_over_bins')
+            if F_all != F:  # sum over the other ranks' bins
+                w_kt = parallel.mean_over_all_bins(w_kt, F, F_all, bin_group)
+                w_k = parallel.mean_over_all_bins(w_k, F, F_all, bin_group)
+            model.weight = w_kt[None] if mode == _lib.WEIGHT_TIED_TIME else w_k[None, :, None]
+    return model

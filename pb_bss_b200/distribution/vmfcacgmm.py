@@ -3,15 +3,15 @@
 model.  Same names, arguments and defaults as the reference; the F*T-sized work runs in the device kernels shared
 with gcacgmm.py."""
 from dataclasses import dataclass
-from operator import xor
 
 import numpy as np
 import torch
 
 from .. import _device
 from .complex_angular_central_gaussian import ComplexAngularCentralGaussian
-from .gcacgmm import (_unit_norm_obs, cacg_m_step, class_weights,
-                      integrated_posterior, model_to_host)
+from .gcacgmm import _unit_norm_obs, cacg_m_step, class_weights, integrated_posterior
+from .mixture_model_utils import (check_initialization, initial_affiliation, masked_affiliation, model_to_host,
+                                  saliency_bn)
 from .utils import _ProbabilisticModel
 from .von_mises_fisher import VonMisesFisher, vmf_fit_fkt
 
@@ -49,21 +49,15 @@ class VMFCACGMMTrainer:
             eigenvalue_floor=1e-10, affiliation_eps=1e-10, weight_constant_axis=(-1,), spatial_weight=1.,
             spectral_weight=1., inline_permutation_alignment=False) -> VMFCACGMM:
         """EM of the integrated model, signature and semantics of vmfcacgmm.py:101-199."""
-        assert xor(initialization is None, num_classes is None), (
-            'Incompatible input combination. '
-            'Exactly one of the two inputs has to be None: '
-            f'{initialization is None} xor {num_classes is None}')
+        check_initialization(initialization, num_classes)
         like_numpy = not _device.is_tensor(observation)
         od = _unit_norm_obs(observation)
         ed = _real(embedding)
         assert od.shape[-1] > 1
         F, T, D = od.shape
         assert ed.shape[:2] == (F, T), (ed.shape, od.shape)
-        if initialization is None:
-            initialization = np.random.uniform(size=(F, num_classes, T))   # vmfcacgmm.py:165-169, host stream
-            initialization /= np.einsum('...kt->...t', initialization)[..., None, :]
-        affiliation = _device.to_device(initialization, torch.float64).contiguous()
-        sal = None if saliency is None else _device.to_device(saliency, torch.float64).contiguous()
+        affiliation = initial_affiliation(initialization, num_classes, (F,), T)   # vmfcacgmm.py:165-169, host stream
+        sal = saliency_bn(saliency, (F,), T)
         quadratic_form = None
         model = None
         for _ in range(iterations):
@@ -71,7 +65,7 @@ class VMFCACGMMTrainer:
                 affiliation, quadratic_form = model._predict(
                     od, ed, inline_permutation_alignment=inline_permutation_alignment,
                     affiliation_eps=affiliation_eps)
-            masked = affiliation if sal is None else (affiliation * sal[:, None, :]).contiguous()
+            masked = masked_affiliation(affiliation, sal)
             model = VMFCACGMM(
                 weight=class_weights(masked, weight_constant_axis), weight_constant_axis=weight_constant_axis,
                 # the M-step fits the vMF on the embedding as given (vmfcacgmm.py:280-285 calls _fit, which does not

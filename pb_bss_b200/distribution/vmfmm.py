@@ -7,15 +7,14 @@ Same class / argument names, defaults and error types as the reference (``salien
 ``ive``) run on the host, as in ``VonMisesFisher``, which costs one small copy per iteration."""
 import math
 from dataclasses import dataclass
-from operator import xor
 from typing import Any
 
 import numpy as np
 
 from .. import _device
 from .gaussian import _dev, _is_real, check_embedding_dim
-from .gmm import (check_classes, initial_affiliation, masked_affiliation, mixture_weight, posterior, saliency_bn,
-                  weight_from_public, weight_kind, weight_to_public)
+from .gmm import check_classes, mixture_weight, posterior, weight_from_public, weight_kind, weight_to_public
+from .mixture_model_utils import check_initialization, initial_affiliation, masked_affiliation, saliency_bn
 from .utils import _ProbabilisticModel
 from .von_mises_fisher import VonMisesFisher, _np, vmf_fit_bkn, vmf_log_pdf_bkn
 
@@ -56,10 +55,7 @@ class VMFMMTrainer:
     def fit(self, y, initialization=None, num_classes=None, iterations=100, saliency=None,
             weight_constant_axis=(-1,), min_concentration=1e-10, max_concentration=500) -> VMFMM:
         """EM of vmfmm.py:43-98: y (..., N, E), initialization (..., K, N), saliency (..., N)."""
-        assert xor(initialization is None, num_classes is None), (
-            'Incompatible input combination. '
-            'Exactly one of the two inputs has to be None: '
-            f'{initialization is None} xor {num_classes is None}')
+        check_initialization(initialization, num_classes)
         assert _is_real(y), y.dtype
         like_numpy = not _device.is_tensor(y)
         yd = _dev(y)

@@ -67,24 +67,6 @@ def test_no_cpu_fallback_without_gpu():
         CACGMMTrainer().fit(y, num_classes=2, iterations=1)
 
 
-def test_weight_axis_mapping():
-    from pb_bss_b200 import _lib
-    from pb_bss_b200.distribution.cacgmm import _weight_mode
-    assert _weight_mode((-1,), 3) == _lib.WEIGHT_TIME
-    assert _weight_mode([-1], 3) == _lib.WEIGHT_TIME
-    assert _weight_mode(2, 3) == _lib.WEIGHT_TIME
-    assert _weight_mode(-2, 3) == _lib.WEIGHT_CONST
-    assert _weight_mode(1, 3) == _lib.WEIGHT_CONST
-    assert _weight_mode((-3,), 3) == _lib.WEIGHT_TIED_TIME
-    assert _weight_mode((-3, -1), 3) == _lib.WEIGHT_TIED
-    assert _weight_mode((-1, -3), 3) == _lib.WEIGHT_TIED
-    # more than one independent dim: the bins (axis -3) are tied, the dims in front stay independent fits
-    assert _weight_mode((-3,), 4) == _lib.WEIGHT_TIED_TIME
-    assert _weight_mode((-3, -1), 5) == _lib.WEIGHT_TIED
-    with pytest.raises(NotImplementedError):
-        _weight_mode((-4, -1), 4)
-
-
 @pytest.mark.parametrize('F,I,arrive,cap', [(513, 100, 15, 467), (129, 20, 30, 292), (7, 5, 1, 292), (40, 12, 3, 10),
                                             (513, 1, 8, 292), (1, 9, 4, 4), (2000, 3, 64, 50)])
 def test_streamed_task_order_is_a_valid_schedule(F, I, arrive, cap):
