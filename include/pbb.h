@@ -387,7 +387,9 @@ int pbb_bingham_log_pdf(const void* y, int dtype, int M, int T, int D, const voi
  * Batched Hermitian eigendecomposition, ascending eigenvalues
  * (np.linalg.eigh as used in complex_angular_central_gaussian.py:95 and
  * pb_bss/utils.py:154).  a: (n, D, D) complex128 (only read), w: (n, D),
- * v: (n, D, D) complex128, columns are eigenvectors. */
+ * v: (n, D, D) complex128, columns are eigenvectors.  0 < D <= 64.  Exact
+ * under power-of-two scaling: w(2^k a) = 2^k w(a), v(2^k a) = v(a) for even k.
+ * status = 1 + index of the first matrix with non-finite input. */
 int pbb_heig_batched(const void* a, int n, int D, double* w, void* v,
                      int* status, void* stream);
 
@@ -399,7 +401,7 @@ int pbb_heig_batched(const void* a, int n, int D, double* w, void* v,
 /* get_power_spectral_density_matrix (beamformer.py:59-160) for observation
  * (F, D, T) and mask (F, K, T) float64 (or NULL: plain average over time,
  * K must be 1).  normalize: divide by max(sum_t mask, 1e-10) (:127-131).
- * psd: (F, K, D, D). */
+ * psd: (F, K, D, D).  D < 35, K < 20, any F. */
 size_t pbb_psd_workspace_bytes(int F, int T, int D, int K);
 int pbb_power_spectral_density(const void* observation, int dtype, int F,
                                int D, int T, const double* mask, int K,
@@ -411,13 +413,17 @@ int pbb_power_spectral_density(const void* observation, int dtype, int F,
  * ITYPE=1 (w^H noise w = 1).  Replaces _c_get_gev_vector
  * (cythonized/get_gev_vector.pyx:42-150); unlike it, matrices are row-major
  * (n, D, D).  status = 1 + index of the first pair whose noise matrix is not
- * positive definite (the Cython code raises ValueError there, :130-147). */
+ * positive definite (the Cython code raises ValueError there, :130-147).
+ * 0 < D <= 64.  Target times 2^k and noise times 2^j (j even) give exactly
+ * 2^(-j/2) w. */
 int pbb_gev_batched(const void* target_psd, const void* noise_psd, int n,
                     int D, void* w, int* status, void* stream);
 
 /* np.linalg.solve for a batch: a (n, D, D), b (n, D, R) -> x (n, D, R), partial
- * pivoting.  hermitize != 0 solves with (a + a^H) / 2.  status flags singular
- * matrices (the reference falls back to lstsq, math/solve.py:95-114). */
+ * pivoting.  hermitize != 0 solves with (a + a^H) / 2.  An exactly singular
+ * matrix gets the minimum-norm (lstsq) solution for D <= 40 (the reference's
+ * fallback, math/solve.py:95-114); status flags one for D > 40.  0 < D, R <= 64.
+ * x(2^k a, b) = 2^-k x(a, b) exactly for even k.  Non-finite a gives NaN. */
 int pbb_solve_batched(const void* a, const void* b, int n, int D, int R,
                       int hermitize, void* x, int* status, void* stream);
 
@@ -454,7 +460,7 @@ int pbb_apply_beamforming_vector(const void* vector, const void* mix, int dtype,
                                  int F, int D, int T, void* out, void* stream);
 
 /* The same for B beamformers per bin that share ONE mix (the K sources of a separation on one STFT; the reference
- * broadcasts the mix in its einsum): vector (B, F, D), mix (F, D, T), out (B, F, T).  B, F <= 65535. */
+ * broadcasts the mix in its einsum): vector (B, F, D), mix (F, D, T), out (B, F, T).  B <= 65535, any F. */
 int pbb_apply_beamforming_vector_shared(const void* vector, const void* mix, int dtype,
                                         int B, int F, int D, int T, void* out, void* stream);
 

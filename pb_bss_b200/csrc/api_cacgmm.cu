@@ -338,30 +338,41 @@ static int normalize(const void* y, int dtype, const CacgmmWorkspace& ws, int F,
 
 static bool fast_shape(int D, int K) { return (D == 4 || D == 6 || D == 8) && K >= 2 && K <= 4; }
 
-// Fills nch / frames_per_block and launches the EM kernel for the shape.
+// Fills nch / frames_per_block and launches the EM kernel for the shape.  The bins lie on gridDim.y (at most 65535):
+// more bins take one launch per 65535, each bin's work unchanged.  A failed launch returns the (positive) CUDA error
+// negated: the callers take any positive value for nch.
 int launch_em(EmArgs a, int dtype, int frames_per_block, cudaStream_t st) {
+  constexpr int kMaxGridY = 65535;
+  const int F = a.F;
   if (fast_shape(a.D, a.K)) {
     int fpb = frames_per_block > 0 ? frames_per_block : 128;
     fpb = (fpb + 31) / 32 * 32;
     if (fpb > (a.T + 31) / 32 * 32) fpb = (a.T + 31) / 32 * 32;
     a.frames_per_block = fpb;
     a.nch = (a.T + fpb - 1) / fpb;
-    const int r = with_d_k_ct(a.D, a.K, dtype, [&](auto d, auto k, auto ct) {
-      return launch_kernel("em_fast_kernel", em_fast_kernel<decltype(d)::value, decltype(k)::value, decltype(ct)>,
-                           dim3(a.nch, a.F), 32 * kEmGroups, 0, st, a);
-    });
-    return r ? r : a.nch;
+    for (a.f0 = 0; a.f0 < F; a.f0 += kMaxGridY) {
+      const int r = with_d_k_ct(a.D, a.K, dtype, [&](auto d, auto k, auto ct) {
+        return launch_kernel("em_fast_kernel", em_fast_kernel<decltype(d)::value, decltype(k)::value, decltype(ct)>,
+                             dim3(a.nch, std::min(F - a.f0, kMaxGridY)), 32 * kEmGroups, 0, st, a);
+      });
+      if (r) return r > 0 ? -r : r;
+    }
+    return a.nch;
   }
   a.frames_per_block = kGenFrames;
   a.nch = (a.T + kGenFrames - 1) / kGenFrames;
   a.softmax_fast = 0;
   const size_t smem = (size_t)2 * a.K * kGenFrames * sizeof(double) + (size_t)a.D * a.D * sizeof(int);
-  const int r = with_ct(dtype, [&](auto ct) {
-    const auto kern = em_generic_kernel<decltype(ct)>;
-    PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    return launch_kernel("em_generic_kernel", kern, dim3(a.nch, a.F), kGenFrames, smem, st, a);
-  });
-  return r ? r : a.nch;
+  for (a.f0 = 0; a.f0 < F; a.f0 += kMaxGridY) {
+    const int r = with_ct(dtype, [&](auto ct) {
+      const auto kern = em_generic_kernel<decltype(ct)>;
+      PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+      return launch_kernel("em_generic_kernel", kern, dim3(a.nch, std::min(F - a.f0, kMaxGridY)), kGenFrames, smem,
+                           st, a);
+    });
+    if (r) return r > 0 ? -r : r;
+  }
+  return a.nch;
 }
 
 // cacg_update_kernel (UpdArgs) or cw_update_kernel (CwUpdArgs): one CTA per bin, up to 16 warps

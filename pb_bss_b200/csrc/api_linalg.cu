@@ -23,6 +23,7 @@ __global__ void heig_batched_kernel(const double2* __restrict__ a, int n, int D,
   double* rot = reinterpret_cast<double*>(V + D * D);
   const double2* __restrict__ am = a + (size_t)m * D * D;
   bool bad = false;
+  double amax = 0.0;
   // Hermitian part of the input, (A + A^H) / 2: LAPACK reads one triangle only
   for (int i = lane; i < D * D; i += 32) {
     const int r = i / D, c = i - r * D;
@@ -30,13 +31,17 @@ __global__ void heig_batched_kernel(const double2* __restrict__ a, int n, int D,
     const double2 h = make_double2(0.5 * (x.x + y.x), r == c ? 0.0 : 0.5 * (x.y - y.y));
     bad |= !isfinite(h.x) || !isfinite(h.y);
     A[i] = h;
+    amax = cabs_max(amax, h);
   }
+  // diagonalise 2^-escale A (linalg_kernels.cuh: even_exponent): same V, eigenvalues times 2^escale
+  const int escale = even_exponent(amax);
+  for (int i = lane; i < D * D; i += 32) A[i] = cscalbn(A[i], -escale);
   __syncwarp();
   const int sweeps = warp_jacobi_any(A, V, rot, D, lane);
-  if ((__any_sync(0xffffffffu, bad) || sweeps > kJacobiMaxSweeps) && lane == 0 && status) atomicMax(status, m + 1);
+  if ((__any_sync(0xffffffffu, bad) || sweeps > kJacobiMaxSweeps) && lane == 0 && status) record_first(status, m + 1);
   for (int x = lane; x < D; x += 32) {
     const int r = eig_rank(A, D, x);
-    w[(size_t)m * D + r] = A[x * D + x].x;
+    w[(size_t)m * D + r] = scalbn(A[x * D + x].x, escale);
     for (int d = 0; d < D; ++d) v[(size_t)m * D * D + d * D + r] = V[d * D + x];
   }
 }
@@ -193,10 +198,10 @@ static int apply_bf_launch(const void* vector, const void* mix, int dtype, int B
                            void* stream) {
   PBB_CHECK_ARG(vector && mix, 1, "input is null");
   PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 3, "bad dtype");
-  PBB_CHECK_ARG(B > 0 && B <= 65535 && F > 0 && F <= 65535 && D > 0 && T > 0, 4, "bad shape");
+  PBB_CHECK_ARG(B > 0 && B <= 65535 && F > 0 && D > 0 && T > 0, 4, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 7, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  dim3 grid((T + 255) / 256, F, B);
+  dim3 grid((T + 255) / 256, F < 65535 ? F : 65535, B);
   LaunchScope ls("apply_bf_kernel", st);
   if (dtype == PBB_C128)
     apply_bf_kernel<double2><<<grid, 256, 0, st>>>(reinterpret_cast<const double2*>(vector),

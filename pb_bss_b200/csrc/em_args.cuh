@@ -32,6 +32,7 @@ struct EmArgs {
   double* loglik_part;     // (F, NCH) or null
   int nch;
   int frames_per_block;    // multiple of 32
+  int f0;                  // first bin of the launch: launch_em covers F > 65535 bins (gridDim.y) in several launches
 };
 
 // host launcher (defined in api_cacgmm.cu): fills nch / frames_per_block, launches the EM

@@ -298,7 +298,7 @@ template <int D, int K, typename CT>
 __global__ void __launch_bounds__(32 * kEmGroups, 3) em_fast_kernel(const EmArgs a) {
   using S = EmFastSmem<D, K>;
   __shared__ __align__(16) S sm;
-  const int f = blockIdx.y, chunk = blockIdx.x;
+  const int f = a.f0 + blockIdx.y, chunk = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (a.mode != kModeM) {
     const double* __restrict__ cf = a.coef + (size_t)f * K * S::NS;
@@ -340,7 +340,7 @@ __global__ void __launch_bounds__(kGenFrames) em_generic_kernel(const EmArgs a) 
   double* g_s = c_s + (size_t)K * kGenFrames;                 // [K][kGenFrames] gamma*saliency
   int* tab = reinterpret_cast<int*>(g_s + (size_t)K * kGenFrames);  // [NS]
   __shared__ double red[kGenFrames / 32];
-  const int f = blockIdx.y, chunk = blockIdx.x;
+  const int f = a.f0 + blockIdx.y, chunk = blockIdx.x;
   const int tid = threadIdx.x;
   const int t_begin = chunk * kGenFrames;
   const int t_end = min(T, t_begin + kGenFrames);

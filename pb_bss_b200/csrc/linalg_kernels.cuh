@@ -19,6 +19,33 @@ __device__ __forceinline__ double2 cdiv(double2 a, double2 b) {
   return make_double2((a.x * b.x + a.y * b.y) / d, (a.y * b.x - a.x * b.y) / d);
 }
 
+// ---- input scaling -------------------------------------------------------------
+// The Jacobi rotation test (|a_pq|^2 > eps^2 |a_pp a_qq| and > 1e-300), the Cholesky and cdiv square the entries:
+// above ~1e154 those squares overflow, below ~1e-150 they fall under 1e-300 or underflow, and the result is silently
+// wrong (the diagonal comes back as the eigenvalues).  The kernels below therefore work on the matrix times 2^-e,
+// e = even_exponent(max |entry|), so that its largest entry lies in [1, 4), and undo the scaling afterwards.  Scaling
+// by a power of two is exact: results at ordinary scales do not change, and w(2^k A) = 2^k w(A) bit for bit for even k.
+// e is even so that a Cholesky factor scales by the exact power 2^(e/2).  0 for a zero or non-finite maximum.
+__device__ __forceinline__ int even_exponent(double amax) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmax(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if (!(amax > 0.0) || !isfinite(amax)) return 0;
+  return ilogb(amax) & ~1;  // floor to even, also for negative exponents
+}
+__device__ __forceinline__ double cabs_max(double m, double2 v) { return fmax(m, fmax(fabs(v.x), fabs(v.y))); }
+__device__ __forceinline__ double2 cscalbn(double2 v, int e) { return make_double2(scalbn(v.x, e), scalbn(v.y, e)); }
+
+// status = 1 + the FIRST failing matrix (status starts at 0), like the reference's loop over the bins that raises at
+// the first bad one (beamformer.py:395-409)
+__device__ inline void record_first(int* status, int v) {
+  int old = atomicCAS(status, 0, v);
+  while (old != 0 && v < old) {
+    const int prev = atomicCAS(status, old, v);
+    if (prev == old) break;
+    old = prev;
+  }
+}
+
 // ---- Cholesky B = L L^H, lower triangle in place (warp) ------------------------
 // returns false if B is not positive definite (LAPACK zpotrf INFO > 0, which is
 // what zhegvd reports as INFO = N + i, get_gev_vector.pyx:130-147)
@@ -103,6 +130,7 @@ __global__ void gev_kernel(const double2* __restrict__ a, const double2* __restr
   const double2* __restrict__ am = a + (size_t)m * D * D;
   const double2* __restrict__ bm = b + (size_t)m * D * D;
   bool bad = false;
+  double amax = 0.0, bmax = 0.0;
   // zhegvd reads the lower triangles (UPLO = 'L'); use the Hermitian parts
   for (int i = lane; i < D * D; i += 32) {
     const int r = i / D, c = i - r * D;
@@ -111,6 +139,14 @@ __global__ void gev_kernel(const double2* __restrict__ a, const double2* __restr
     C[i] = make_double2(0.5 * (x.x + y.x), r == c ? 0.0 : 0.5 * (x.y - y.y));
     L[i] = make_double2(0.5 * (p.x + q.x), r == c ? 0.0 : 0.5 * (p.y - q.y));
     bad |= !isfinite(C[i].x) || !isfinite(C[i].y) || !isfinite(L[i].x) || !isfinite(L[i].y);
+    amax = cabs_max(amax, C[i]);
+    bmax = cabs_max(bmax, L[i]);
+  }
+  // solve with 2^-ea A and 2^-eb B: y does not change, and w = 2^(-eb/2) times the w of the scaled pair
+  const int ea = even_exponent(amax), eb = even_exponent(bmax);
+  for (int i = lane; i < D * D; i += 32) {
+    C[i] = cscalbn(C[i], -ea);
+    L[i] = cscalbn(L[i], -eb);
   }
   __syncwarp();
   const bool pd = warp_cholesky(L, D, lane);
@@ -142,9 +178,9 @@ __global__ void gev_kernel(const double2* __restrict__ a, const double2* __restr
   for (int d = lane; d < D; d += 32) yv[d] = V[d * D + best];
   __syncwarp();
   warp_trsm_lower_h(L, yv, D, 1, lane);
-  for (int d = lane; d < D; d += 32) out[(size_t)m * D + d] = yv[d];
+  for (int d = lane; d < D; d += 32) out[(size_t)m * D + d] = cscalbn(yv[d], -eb / 2);
   if ((!pd || __any_sync(0xffffffffu, bad) || sweeps > kJacobiMaxSweeps) && lane == 0 && status)
-    atomicMax(status, m + 1);
+    record_first(status, m + 1);
 }
 
 // shared memory of one warp of solve_kernel: A, X and -- when the minimum-norm fallback is available (D <= kLstsqMaxD)
@@ -179,6 +215,8 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
   double2* A = reinterpret_cast<double2*>(smem_raw + per * warp);
   double2* X = A + D * D;
   const double2* __restrict__ am = a + (size_t)m * D * D;
+  double amax0 = 0.0;
+  bool bad = false;
   for (int i = lane; i < D * D; i += 32) {
     const int r = i / D, c = i - r * D;
     const double2 u = am[i];
@@ -188,11 +226,18 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
     } else {
       A[i] = u;
     }
+    amax0 = cabs_max(amax0, A[i]);
+    bad |= !isfinite(A[i].x) || !isfinite(A[i].y);
   }
+  // both branches solve with 2^-escale A: X = 2^-escale times that solution (minimum-norm one included)
+  const int escale = even_exponent(amax0);
+  for (int i = lane; i < D * D; i += 32) A[i] = cscalbn(A[i], -escale);
   for (int i = lane; i < D * R; i += 32) X[i] = b[(size_t)m * D * R + i];
   __syncwarp();
-  bool singular = false, nonfinite = false;
-  for (int j = 0; j < D; ++j) {
+  // a NaN in A can hide from the pivot search (NaN > best is false) and end as a zero pivot: decide non-finite input
+  // up front, so that it gives NaN and never the minimum-norm fallback
+  bool singular = false, nonfinite = __any_sync(0xffffffffu, bad);
+  for (int j = 0; j < D && !nonfinite; ++j) {
     // pivot search (every lane redundantly: D is tiny)
     int piv = j;
     double best = -1.0;
@@ -253,8 +298,8 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
     double asym = 0.0, amax = 0.0;
     for (int i = lane; i < D * D; i += 32) {
       const int r = i / D, c = i - r * D;
-      double2 u = am[i];
-      const double2 v = am[c * D + r];
+      double2 u = cscalbn(am[i], -escale);
+      const double2 v = cscalbn(am[c * D + r], -escale);
       if (hermitize) u = make_double2(0.5 * (u.x + v.x), 0.5 * (u.y - v.y));
       A[i] = u;
       asym = fmax(asym, hermitize ? 0.0 : fabs(u.x - v.x) + fabs(u.y + v.y));
@@ -327,7 +372,7 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
     for (int i = lane; i < D * R; i += 32) X[i] = Y[i];
     __syncwarp();
   }
-  for (int i = lane; i < D * R; i += 32) x[(size_t)m * D * R + i] = X[i];
+  for (int i = lane; i < D * R; i += 32) x[(size_t)m * D * R + i] = cscalbn(X[i], -escale);
 }
 
 // ---- MVDR: w = N^{-1} a / (a^H N^{-1} a) given x = N^{-1} a (beamformer.py:257-258) ----
@@ -423,21 +468,23 @@ __global__ void ban_kernel(const double2* __restrict__ vec, const double2* __res
 
 // ---- apply a beamforming vector: out[b][f][t] = sum_d conj(w[b][f][d]) Y[f][d][t] (beamformer.py:572-583);
 // blockIdx.z = b runs over beamformers that share one mix (K sources on one STFT), 1 otherwise
+// bins beyond gridDim.y (at most 65535) are taken in strides of gridDim.y
 template <typename CT>
 __global__ void apply_bf_kernel(const double2* __restrict__ w, const CT* __restrict__ Y, int F, int D, int T,
                                 double2* __restrict__ out) {
-  const int f = blockIdx.y;
-  const size_t bf = (size_t)blockIdx.z * F + f;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
-  double2 s = make_double2(0.0, 0.0);
-  for (int d = 0; d < D; ++d) {
-    const double2 wd = w[bf * D + d];
-    const double2 y = ld_cplx(Y + ((size_t)f * D + d) * T + t);
-    s.x += wd.x * y.x + wd.y * y.y;
-    s.y += wd.x * y.y - wd.y * y.x;
+  for (int f = blockIdx.y; f < F; f += gridDim.y) {
+    const size_t bf = (size_t)blockIdx.z * F + f;
+    double2 s = make_double2(0.0, 0.0);
+    for (int d = 0; d < D; ++d) {
+      const double2 wd = w[bf * D + d];
+      const double2 y = ld_cplx(Y + ((size_t)f * D + d) * T + t);
+      s.x += wd.x * y.x + wd.y * y.y;
+      s.y += wd.x * y.y - wd.y * y.x;
+    }
+    out[bf * T + t] = s;
   }
-  out[bf * T + t] = s;
 }
 
 // ---- rank-1 PSD approximations (beamformer_wrapper.py:11-69) ---------------------
