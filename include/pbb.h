@@ -123,6 +123,12 @@ int pbb_streamed_task_order(int F, int iterations, int arrive, int cap, int* ord
  * clusters it runs at once, which on a GPU with uneven GPCs can pick a smaller cluster. */
 int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms, int* kernel, int* split);
 
+/* Host only: the plan of the last persistent fit (pbb_cacgmm_fit / pbb_cwmm_fit) the calling host thread launched,
+ * with the environment overrides applied.  *kernel and *split as in pbb_em_dispatch (*kernel = -1: none yet);
+ * *variant: 0 = lean (product-form softmax), 1 = full with the integer-power softmax, 2 = full with the log-domain
+ * softmax, 3 = complex Watson. */
+int pbb_em_last_plan(int* kernel, int* split, int* variant);
+
 /* Bytes of scratch pbb_cacgmm_fit / _predict need for this problem size. */
 size_t pbb_cacgmm_workspace_bytes(int F, int T, int D, int K);
 

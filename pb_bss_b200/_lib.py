@@ -62,6 +62,7 @@ SIGNATURES = {
     'pbb_normalize_observation': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
     'pbb_streamed_task_order': (_i, [_i, _i, _i, _i, ctypes.POINTER(_i)]),
     'pbb_em_dispatch': (_i, [_i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
+    'pbb_em_last_plan': (_i, [ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i)]),
     'pbb_cacgmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'pbb_cacgmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp,
                             ctypes.POINTER(CacgmmOptions), _vp, _vp, _vp,

@@ -311,11 +311,22 @@ static int launch_kernel(const char* name, Kern kern, dim3 grid, dim3 block, siz
   return 0;
 }
 
+// The normalisation kernels put the bins on gridDim.y (at most 65535): more bins take one launch per 65535, with
+// y, z (and dead) offset to the launch's first bin.
+constexpr int kNormMaxGridY = 65535;
+
 template <typename CT>
 static int launch_normalize(const CT* y, CT* z, int F, int T, int D, int swap, int zs, cudaStream_t st) {
   const int block = D <= 16 ? 128 : 32;
-  return launch_kernel("normalize_kernel", normalize_kernel<CT>, dim3((T + block - 1) / block, F), block,
-                       (size_t)block * (D + 1) * sizeof(double2), st, y, z, F, T, D, swap, zs);
+  for (int f0 = 0; f0 < F; f0 += kNormMaxGridY) {
+    const int nf = std::min(F - f0, kNormMaxGridY);
+    // per-bin stride of z: D rows of zs frames (swap), or zs = T frames of D channels
+    if (int r = launch_kernel("normalize_kernel", normalize_kernel<CT>, dim3((T + block - 1) / block, nf), block,
+                              (size_t)block * (D + 1) * sizeof(double2), st, y + (size_t)f0 * T * D,
+                              z + (size_t)f0 * D * zs, nf, T, D, swap, zs))
+      return r;
+  }
+  return 0;
 }
 
 // y -> ws.z, rows padded to ws.zs frames, or (staged) in the chunk-major layout of the persistent kernels: one TMA
@@ -330,9 +341,17 @@ static int normalize(const void* y, int dtype, const CacgmmWorkspace& ws, int F,
     if (!staged) return launch_normalize(src, dst, F, T, D, 1, ws.zs, st);
     const int block = 64;  // divides kStageFrames
     const int nchunks = (ws.zs + kStageFrames - 1) / kStageFrames;
-    return launch_kernel("normalize_staged_kernel", normalize_staged_kernel<CT>,
-                         dim3(nchunks * (kStageFrames / block), F), block, (size_t)block * (D + 1) * sizeof(double2),
-                         st, src, dst, F, T, D, stage_rows(D), kStageFrames, nchunks, ws.dead);
+    const size_t bin_elems = (size_t)nchunks * stage_rows(D) * kStageFrames;  // out[f][c][r][i]
+    for (int f0 = 0; f0 < F; f0 += kNormMaxGridY) {
+      const int nf = std::min(F - f0, kNormMaxGridY);
+      if (int r = launch_kernel("normalize_staged_kernel", normalize_staged_kernel<CT>,
+                                dim3(nchunks * (kStageFrames / block), nf), block,
+                                (size_t)block * (D + 1) * sizeof(double2), st, src + (size_t)f0 * T * D,
+                                dst + (size_t)f0 * bin_elems, nf, T, D, stage_rows(D), kStageFrames, nchunks,
+                                ws.dead + f0))
+        return r;
+    }
+    return 0;
   });
 }
 
@@ -376,12 +395,27 @@ int launch_em(EmArgs a, int dtype, int frames_per_block, cudaStream_t st) {
 }
 
 // cacg_update_kernel (UpdArgs) or cw_update_kernel (CwUpdArgs): one CTA per bin, up to 16 warps
+// Warps per CTA are also capped by the kernel's own limit (its registers): at small D the shared memory would allow
+// 16 warps, more than cacg_update_kernel / cw_update_kernel can launch with, and the class loop covers K > warps.
+// cap: the kernel's limit in warps, queried on the first launch (0 until then).
+static int max_warps(const void* kern, int* cap, int* w) {
+  if (*cap == 0) {
+    cudaFuncAttributes at;
+    PBB_CUDA(cudaFuncGetAttributes(&at, kern));
+    *cap = at.maxThreadsPerBlock / 32;
+  }
+  if (*w > *cap) *w = *cap;
+  return 0;
+}
+
 template <typename U>
 static int launch_update(void (*kern)(U), const char* name, U u, cudaStream_t st) {
   const size_t per = update_smem_per_warp(u.D);
   int w = (int)((size_t)(200 * 1024) / per);
   if (w > u.K) w = u.K;
   if (w > 16) w = 16;
+  static int cap = 0;  // one kernel per instantiation (UpdArgs / CwUpdArgs)
+  if (int r = max_warps(reinterpret_cast<const void*>(kern), &cap, &w)) return r;
   if (w < 1) w = 1;
   u.warps = w;
   const size_t smem = per * w + (size_t)2 * u.K * sizeof(double) + (size_t)u.D * u.D * sizeof(int);
@@ -402,6 +436,8 @@ static int launch_from_eig(const CacgmmWorkspace& ws, int F, int D, int K, const
   int w = (int)((size_t)(200 * 1024) / per);
   if (w > K) w = K;
   if (w > 16) w = 16;
+  static int cap = 0;
+  if (int r = max_warps(reinterpret_cast<const void*>(cacg_from_eig_kernel), &cap, &w)) return r;
   u.warps = w;
   const size_t smem = per * w + (size_t)K * sizeof(double) + (size_t)D * D * sizeof(int);
   PBB_CUDA(cudaFuncSetAttribute(cacg_from_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
@@ -612,9 +648,10 @@ static int launch_persist(const PersistArgs& a, int D, int K, int dtype, Persist
     const int threads = persist_threads(Dc, Kc);
     const size_t smem = sizeof(PersistSmem<Dc, Kc, CT>);
     int* c = &cache[(int)v];
+    // the full variant's launches carry their own name, so that profiles and tests can tell it from the lean one
     if (v == Persist::kFull)
       return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, true, 1>, threads, smem, c, a,
-                                       "em_persistent_kernel", st);
+                                       "em_persistent_kernel_full", st);
     if (v == Persist::kCw)
       return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 2, 1>, threads, smem, c, a,
                                        "em_persistent_kernel_cw", st);
@@ -661,6 +698,10 @@ static int launch_sticky(const PersistArgs& a, int K, int dtype, int S, cudaStre
   });
 }
 
+// The plan of the last persistent fit this host thread launched (pbb_em_last_plan): kernel, split, variant.
+struct LastPlan { int kernel, split, variant; };
+static thread_local LastPlan g_last_plan = {-1, 0, -1};
+
 // Plan and launch of a persistent fit whose control block is clear: the sticky-bins kernel when the plan picks it,
 // otherwise the frame split and the task kernel.  model: kFull, kLean or kCw (always the single-role kernel).
 static int launch_planned(PersistArgs p, const CacgmmWorkspace& ws, int D, int K, int dtype, Persist model,
@@ -671,6 +712,7 @@ static int launch_planned(PersistArgs p, const CacgmmWorkspace& ws, int D, int K
   if (sticky_eligible(D, lean, streamed, tu) && (r = sticky_clusters(K, dtype, clusters, st))) return r;
   if ((r = device_sms(&sms))) return r;
   const FitPlan plan = plan_persistent_fit(p.F, p.T, D, K, lean, streamed, sms, clusters, tu);
+  g_last_plan = {plan.kernel, plan.split, model == Persist::kCw ? 3 : (lean ? 0 : (p.softmax_fast ? 1 : 2))};
   if (plan.kernel == kKernelSticky) return launch_sticky(p, K, dtype, plan.split, st);  // few bins: one cluster per bin
   if ((r = setup_frame_split(&p, ws, p.F, D, K, plan.split, st))) return r;
   if (plan.kernel == kKernelWs) model = Persist::kWs;
@@ -901,6 +943,14 @@ int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms,
   const FitPlan plan = plan_persistent_fit(F, T, D, K, lean != 0, streamed != 0, sms, clusters, Tuning{});
   *kernel = plan.kernel;
   *split = plan.split;
+  return 0;
+}
+
+int pbb_em_last_plan(int* kernel, int* split, int* variant) {
+  PBB_CHECK_ARG(kernel != nullptr && split != nullptr && variant != nullptr, 1, "output is null");
+  *kernel = g_last_plan.kernel;
+  *split = g_last_plan.split;
+  *variant = g_last_plan.variant;
   return 0;
 }
 

@@ -763,13 +763,20 @@ __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin,
     PBB_PHU(9);   // Gauss-Jordan
     double ldk = log(det);
     double tinv = 0.0;
+    bool diag_pos = true;
 #pragma unroll
-    for (int d = 0; d < D; ++d) tinv += A[d * D + d].x;  // every lane reads the diagonal (broadcast loads)
-    // lambda_min / lambda_max >= 1 / (tr(A) tr(A^-1))
+    for (int d = 0; d < D; ++d) {  // every lane reads the diagonal (broadcast loads)
+      tinv += A[d * D + d].x;
+      diag_pos = diag_pos && A[d * D + d].x > 0.0;
+    }
+    // lambda_min / lambda_max >= 1 / (tr(A) tr(A^-1)) holds for a positive definite A only.  Positive pivots do not
+    // prove that in floating point: a singular scatter matrix (rank-deficient observations) can pass Gauss-Jordan
+    // with noise-level positive pivots and come out with a negative diagonal in its "inverse", which made the bound
+    // negative and skipped the floor.  Every diagonal entry of the inverse of a positive definite matrix is positive.
     // A bin with an all-zero frame must keep the reference's own normalisation: such a frame has
     // q = `tiny` for every class whatever the scale of B (cacg.py:198), so its posterior depends
     // on det B in the reference's lambda_max = 1 scale -- take the eigendecomposition path there.
-    const bool no_floor = ok && isfinite(tinv) && (tr * tn * tinv * a.eigenvalue_floor < 0.5) &&
+    const bool no_floor = ok && diag_pos && isfinite(tinv) && (tr * tn * tinv * a.eigenvalue_floor < 0.5) &&
                           dead_bin == 0;
     double* __restrict__ co = coef_out != nullptr ? coef_out : a.coef + ((size_t)bin * K + k) * NS;
     PBB_PHU(10);  // log det, trace of the inverse, floor test
