@@ -720,6 +720,35 @@ int pbb_istft(const void* X, long long rows, int frames, int size, int shift, in
               void* workspace, size_t workspace_bytes, double* out, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Gammatone filterbank (pb_bss/transform/gammatone.py:6-102, Slaney's Apple TR #35), csrc/gammatone.cuh.
+ *
+ * Filter i is a cascade of four second-order sections with numerators [b0_k, b1_k, 0] and the shared denominator
+ * [1, a1, a2], each run from zero state in direct form II transposed (scipy.signal.lfilter).  The cascade is one
+ * linear recurrence with 8 states, made parallel over time by a scan over chunks of L samples: the zero-start end
+ * state of every (row, filter, chunk), a carry s_{c+1} = M s_c + z_c over the chunks (M = the cascade's zero-input
+ * transition over L samples), and a rerun of every chunk from its carried start state that writes the output.  All
+ * fp64, no atomics (bitwise reproducible).
+ *
+ * L is the largest power of two in [PBB_GAMMATONE_CHUNK_MIN, PBB_GAMMATONE_CHUNK_MAX] that still gives at least
+ * PBB_GAMMATONE_MIN_CHUNKS (row, filter, chunk) sequences, else PBB_GAMMATONE_CHUNK_MIN; a host-only function of
+ * the shape.  Signals of at most L samples are one chunk and skip the scan. */
+#define PBB_GAMMATONE_CHUNK_MIN 128
+#define PBB_GAMMATONE_CHUNK_MAX 1024
+#define PBB_GAMMATONE_MIN_CHUNKS 65536
+#define PBB_GAMMATONE_CARRY_GROUP 32 /* chunks per group of the two-level carry: M^32 is the group transition */
+int pbb_gammatone_chunk_length(long long rows, int n, long long N);
+/* Bytes of the scan's state workspace (0 when N fits one chunk). */
+size_t pbb_gammatone_workspace_bytes(long long rows, int n, long long N);
+/* x (rows, N) float32 (dtype PBB_F32) or float64 (PBB_F64), contiguous; out (n, rows, N) float64.
+ * coef (n, 10) float64: b0_0, b1_0, ..., b0_3, b1_3, a1, a2 per filter.  transition (n, 2, 8, 8) float64, row-major:
+ * M and M^PBB_GAMMATONE_CARRY_GROUP on the state vector (u_0, v_0, ..., u_3, v_3) of the four sections, where a
+ * section with input w and output y = b0 w + u updates u <- b1 w + v - a1 y, v <- -a2 y.  chunk_length must be
+ * pbb_gammatone_chunk_length(rows, n, N): M depends on it. */
+int pbb_gammatone(const void* x, int dtype, long long rows, long long N, int n, const double* coef,
+                  const double* transition, int chunk_length, void* workspace, size_t workspace_bytes,
+                  double* out, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

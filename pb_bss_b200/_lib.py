@@ -141,6 +141,9 @@ SIGNATURES = {
     'pbb_griffin_lim_stft': (_i, [_vp, _i, _ll, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'pbb_istft_workspace_bytes': (_sz, [_ll, _i, _i]),
     'pbb_istft': (_i, [_vp, _ll, _i, _i, _i, _i, _i, _ll, _vp, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_gammatone_chunk_length': (_i, [_ll, _i, _ll]),
+    'pbb_gammatone_workspace_bytes': (_sz, [_ll, _i, _ll]),
+    'pbb_gammatone': (_i, [_vp, _i, _ll, _ll, _i, _vp, _vp, _i, _vp, _sz, _vp, _vp]),
 }
 
 _lib = None

@@ -1,7 +1,9 @@
 // C-ABI entry points for the STFT / iSTFT of nara_wpe.utils and the Griffin-Lim / MISI phase reconstruction of
-// pb_bss/transform/griffin_lim_module.py -- see include/pbb.h and csrc/fft.cuh.
+// pb_bss/transform/griffin_lim_module.py, and the gammatone filterbank of pb_bss/transform/gammatone.py -- see
+// include/pbb.h, csrc/fft.cuh and csrc/gammatone.cuh.
 #include "common.cuh"
 #include "fft.cuh"
+#include "gammatone.cuh"
 #include "prof.cuh"
 
 namespace pbb {
@@ -44,6 +46,40 @@ static int fft_launch(K kernel, const char* name, long long rows, int frames, in
   LaunchScope ls(name, st);
   void* args[] = {params_ptr};
   PBB_CUDA(cudaLaunchKernel((const void*)kernel, dim3((unsigned)ctas), dim3(kFftThreads), args, smem, st));
+  return 0;
+}
+
+struct GtShape {
+  long long chunks, groups;
+};
+
+static GtShape gammatone_shape(long long N, int L) {
+  const long long C = (N + L - 1) / L;
+  return {C, (C + kGtGroup - 1) / kGtGroup};
+}
+
+template <class T>
+static int gammatone_launch(const GtParams& p, cudaStream_t st) {
+  const long long ctas = (p.total + 31) / 32 * ((p.n + kGtFilters - 1) / kGtFilters);
+  if (ctas > 0x7fffffffll || p.rows * p.n > 0x7fffffffll) {
+    set_error("argument: %lld CTAs exceed the grid", ctas);
+    return -1;
+  }
+  GtParams q = p;
+  if (p.chunks > 1) {
+    {
+      LaunchScope ls("gammatone_chunk_state_kernel", st);
+      gammatone_chunk_kernel<T, false><<<(unsigned)ctas, kGtThreads, 0, st>>>(q);
+      PBB_CUDA(cudaGetLastError());
+    }
+    const long long units = p.groups < kGtGroup ? p.groups : kGtGroup;
+    LaunchScope ls("gammatone_carry_kernel", st);
+    gammatone_carry_kernel<<<(unsigned)(p.rows * p.n), (unsigned)((units * 8 + 31) / 32 * 32), 0, st>>>(q);
+    PBB_CUDA(cudaGetLastError());
+  }
+  LaunchScope ls("gammatone_output_kernel", st);
+  gammatone_chunk_kernel<T, true><<<(unsigned)ctas, kGtThreads, 0, st>>>(q);
+  PBB_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -171,6 +207,56 @@ int pbb_istft(const void* X, long long rows, int frames, int size, int shift, in
                                                        out);
   PBB_CUDA(cudaGetLastError());
   return 0;
+}
+
+int pbb_gammatone_chunk_length(long long rows, int n, long long N) {
+  int L = PBB_GAMMATONE_CHUNK_MAX;
+  if (rows <= 0 || n <= 0 || N <= 0) return L;
+  while (L > PBB_GAMMATONE_CHUNK_MIN && rows * n * ((N + L - 1) / L) < PBB_GAMMATONE_MIN_CHUNKS) L /= 2;
+  return L;
+}
+
+size_t pbb_gammatone_workspace_bytes(long long rows, int n, long long N) {
+  if (rows <= 0 || n <= 0 || N <= 0) return 0;
+  const GtShape s = gammatone_shape(N, pbb_gammatone_chunk_length(rows, n, N));
+  if (s.chunks == 1) return 0;
+  return (size_t)(rows * n) * (size_t)(s.chunks + s.groups) * 8 * sizeof(double);
+}
+
+int pbb_gammatone(const void* x, int dtype, long long rows, long long N, int n, const double* coef,
+                  const double* transition, int chunk_length, void* workspace, size_t workspace_bytes, double* out,
+                  void* stream) {
+  PBB_CHECK_ARG(x != nullptr, 1, "x is null");
+  PBB_CHECK_ARG(dtype == PBB_F32 || dtype == PBB_F64, 2, "dtype must be PBB_F32 or PBB_F64");
+  PBB_CHECK_ARG(rows > 0, 3, "rows must be positive");
+  PBB_CHECK_ARG(N > 0, 4, "N must be positive");
+  PBB_CHECK_ARG(n > 0, 5, "n must be positive");
+  PBB_CHECK_ARG(coef != nullptr, 6, "coef is null");
+  PBB_CHECK_ARG(transition != nullptr, 7, "transition is null");
+  PBB_CHECK_ARG(chunk_length == pbb_gammatone_chunk_length(rows, n, N), 8,
+                "chunk_length must be pbb_gammatone_chunk_length(rows, n, N)");
+  const size_t need = pbb_gammatone_workspace_bytes(rows, n, N);
+  PBB_CHECK_ARG(need == 0 || (workspace != nullptr && workspace_bytes >= need), 9,
+                "workspace too small (pbb_gammatone_workspace_bytes)");
+  PBB_CHECK_ARG(out != nullptr, 11, "out is null");
+  const GtShape s = gammatone_shape(N, chunk_length);
+  GtParams p{};
+  p.x = x;
+  p.rows = rows;
+  p.N = N;
+  p.chunks = s.chunks;
+  p.total = rows * s.chunks;
+  p.groups = s.groups;
+  p.n = n;
+  p.L = chunk_length;
+  p.coef = coef;
+  p.trans = transition;
+  p.state = static_cast<double*>(workspace);
+  p.group = p.state + rows * n * s.chunks * 8;
+  p.out = out;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (dtype == PBB_F32) return gammatone_launch<float>(p, st);
+  return gammatone_launch<double>(p, st);
 }
 
 }  // extern "C"
