@@ -749,6 +749,43 @@ int pbb_gammatone(const void* x, int dtype, long long rows, long long N, int n, 
                   double* out, void* stream);
 
 /* ------------------------------------------------------------------------
+ * SRMR, the speech-to-reverberation modulation energy ratio (pb_bss/evaluation/module_srmr.py:42-186), csrc/srmr.cuh
+ * and csrc/fft_large.cuh.  One pass per step of the reference, every row of a batch at once; all sizes derive from
+ * N, and the per-row lengths N_r after the VAD stay on the device.  fp64 (the VAD's threshold compare in the input
+ * precision), no float atomics: bitwise reproducible, and a row's results do not depend on the rest of the batch. */
+#define PBB_SRMR_MAX_SAMPLES 4194304 /* 2^22 */
+#define PBB_SRMR_VAD_TILE 4096       /* samples per CTA of the VAD passes */
+/* _preprocessing_vad (:158-186) and the normalisation (:58-60).  x (rows, N) float32 (PBB_F32) or float64 (PBB_F64).
+ * threshold = max|x|^2 / 1e5 in x's precision; the samples strictly between two above-threshold samples more than
+ * `gap` (0.05 sample_rate) apart are removed.  out (rows, N) float64: the kept samples of each row at its start, zero
+ * after; nr (rows) long long: N_r.  normalise != 0: out becomes (out - mean) / std (population std) over the first N_r
+ * samples; stats (rows, 2) float64 gets mean and std (either way, unused entries when normalise = 0). */
+size_t pbb_srmr_vad_workspace_bytes(long long rows, long long N);
+int pbb_srmr_vad(const void* x, int dtype, long long rows, long long N, double gap, int normalise, void* workspace,
+                 size_t workspace_bytes, double* out, long long* nr, double* stats, void* stream);
+/* |scipy.signal.hilbert(y[s, :N_r])| (:65-67) of every sequence s = f rows + r of y (n rows, N) float64, in place
+ * (entries past N_r are left as they are).  The imaginary part of the analytic signal is y convolved with the
+ * discrete Hilbert kernel of length N_r, one real FFT of M = 2P = nextpow2(2N - 1) points per sequence (at least 2),
+ * computed as a four-step complex FFT of P points in global memory.  `group` sequences are transformed at a time,
+ * which sets the workspace (pbb_srmr_hilbert_workspace_bytes); the result does not depend on it. */
+int pbb_srmr_fft_log2(long long N); /* log2 M */
+size_t pbb_srmr_hilbert_workspace_bytes(long long rows, long long N, long long group);
+int pbb_srmr_hilbert(double* y, long long rows, long long N, int n, const long long* nr, long long group,
+                     void* workspace, size_t workspace_bytes, void* stream);
+/* The modulation filterbank and energies (:70-118): means (rows, n, 8) float64 of the Hamming-windowed frame energies
+ * of the eight modulation filters over the first N_r samples of every envelope env (n rows, N).  hop = int(sr / 1000)
+ * * 64, frames of 4 hop.  coef (8, 3): b0, a1, a2 of b = [b0, 0, -b0], a = [1, a1, a2].  transition (8, 4): the
+ * filter's zero-input state transition over hop samples, row-major 2 x 2 on (z0, z1) of lfilter's direct form II
+ * transposed.  window (4 hop): scipy.signal.windows.hamming(4 hop, sym=True). */
+size_t pbb_srmr_means_workspace_bytes(long long rows, long long N, int n, int hop);
+int pbb_srmr_means(const double* env, long long rows, long long N, int n, const long long* nr, int hop,
+                   const double* coef, const double* transition, const double* window, void* workspace,
+                   size_t workspace_bytes, double* means, void* stream);
+/* The ratio (:104-154): out (rows) float64 from means (rows, n, 8), erb (n) = cfs / 9.26449 + 24.7 and cutoff (8). */
+int pbb_srmr_ratio(const double* means, long long rows, int n, const double* erb, const double* cutoff, double* out,
+                   void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

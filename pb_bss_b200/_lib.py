@@ -144,6 +144,14 @@ SIGNATURES = {
     'pbb_gammatone_chunk_length': (_i, [_ll, _i, _ll]),
     'pbb_gammatone_workspace_bytes': (_sz, [_ll, _i, _ll]),
     'pbb_gammatone': (_i, [_vp, _i, _ll, _ll, _i, _vp, _vp, _i, _vp, _sz, _vp, _vp]),
+    'pbb_srmr_vad_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_srmr_vad': (_i, [_vp, _i, _ll, _ll, _d, _i, _vp, _sz, _vp, _vp, _vp, _vp]),
+    'pbb_srmr_fft_log2': (_i, [_ll]),
+    'pbb_srmr_hilbert_workspace_bytes': (_sz, [_ll, _ll, _ll]),
+    'pbb_srmr_hilbert': (_i, [_vp, _ll, _ll, _i, _vp, _ll, _vp, _sz, _vp]),
+    'pbb_srmr_means_workspace_bytes': (_sz, [_ll, _ll, _i, _i]),
+    'pbb_srmr_means': (_i, [_vp, _ll, _ll, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_srmr_ratio': (_i, [_vp, _ll, _i, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

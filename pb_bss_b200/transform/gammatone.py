@@ -89,16 +89,22 @@ def _cascade_step(coef, state):
     return out
 
 
+def chunk_transition(step, coef, dim, length):
+    """(n, dim, dim): the zero-input state transition of n linear recurrences over `length` samples, the recurrence
+    ``step(coef, state)`` (states (n, dim, m)) run from the dim unit states."""
+    M = np.broadcast_to(np.eye(dim), (coef.shape[0], dim, dim)).copy()
+    for _ in range(length):
+        M = step(coef, M)
+    return M
+
+
 def transition_matrices(coef, chunk_length):
     """(n, 2, 8, 8): the cascade's zero-input state transition over chunk_length samples, M, and over CARRY_GROUP
     chunks, M^CARRY_GROUP.  M is the recurrence run from the 8 unit states and M^CARRY_GROUP a chain of products, as
     the device applies them.  Repeated squaring would be faster but cancels in the blocks that map the first section's
     states (about 1e10 times the signal, through 1 / gain) into the later sections': at 48 kHz it costs the output a
     factor of 40 in accuracy."""
-    n = coef.shape[0]
-    M = np.broadcast_to(np.eye(8), (n, 8, 8)).copy()
-    for _ in range(chunk_length):
-        M = _cascade_step(coef, M)
+    M = chunk_transition(_cascade_step, coef, 8, chunk_length)
     MG = M
     for _ in range(CARRY_GROUP - 1):
         MG = M @ MG
@@ -137,9 +143,16 @@ def gammatone_filterbank(signal, sample_rate=16000, n=23, low_freq=125, high_fre
     else:
         x = x if x.dtype in (torch.float32, torch.float64) else x.to(torch.float64)
     xd = _device.to_device(x)
-    shape = tuple(xd.shape)
-    if not shape:
+    if not xd.shape:
         raise ValueError('gammatone_filterbank needs a signal with at least one axis')
+    out = filterbank_tensor(xd, sample_rate, n, low_freq, high_freq)
+    return list(out.cpu().numpy()) if like_numpy else list(out.unbind(0))
+
+
+def filterbank_tensor(xd, sample_rate, n, low_freq, high_freq):
+    """The (n, *xd.shape) float64 CUDA tensor of the filter outputs of a contiguous float32 / float64 CUDA tensor xd
+    with at least one axis, enqueued on the current stream."""
+    shape = tuple(xd.shape)
     N = shape[-1]
     rows = int(np.prod(shape[:-1], dtype=np.int64))
     out = _device.empty((n,) + shape, torch.float64)
@@ -152,4 +165,4 @@ def gammatone_filterbank(signal, sample_rate=16000, n=23, low_freq=125, high_fre
         _lib.check(lib.pbb_gammatone(_device.ptr(xd), _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64,
                                      rows, N, n, _device.ptr(coef), _device.ptr(trans), L, _device.ptr(ws), nbytes,
                                      _device.ptr(out), _device.stream_ptr()), 'pbb_gammatone')
-    return list(out.cpu().numpy()) if like_numpy else list(out.unbind(0))
+    return out
