@@ -786,6 +786,38 @@ int pbb_srmr_ratio(const double* means, long long rows, int n, const double* erb
                    void* stream);
 
 /* ------------------------------------------------------------------------
+ * BSS Eval v3 (Vincent, Gribonval and Fevotte 2006), mir_eval_sources of pb_bss/evaluation/module_mir_eval.py:5-141:
+ * mir_eval.separation.bss_eval_sources and its _bss_decomp_mtifilt / _project / _bss_source_crit with 512-tap
+ * time-invariant distortion filters, and pb_bss's _bss_eval_sources_and_noise (:94-141) for K + 1 estimates.
+ * csrc/bss_eval.cuh.  fp64 throughout, no float atomics: bitwise reproducible, and an item's results do not depend
+ * on the rest of the batch or on `group`.
+ *
+ * x (items, K + E, T) float64: per item the K references, then the E estimates (E = K or K + 1).  For every item
+ * the lag correlations r_ab[d] = sum_u a[u] b[u + d] (d < 512) on the fp64 tensor cores, the system G c = D of
+ * order N = 512 K (G[(i,t1),(j,t2)] = r_ij[t1 - t2], D[(i,t), e] = r_(i, estimate e)[t]) and the K diagonal blocks
+ * are factored ONCE each by LU with partial pivoting (mir_eval solves per (estimate, reference) pair), and the sums
+ * of squares of the explicit residual signals P_j x, x - P_j x, P_all x - P_j x, P_all x and x - P_all x over T + 511
+ * samples give SDR / SIR / SAR of every (estimate e, reference j) pair with mir_eval's _safe_db (a zero denominator
+ * gives +inf, a zero numerator over a positive one -inf).
+ * compute_permutation != 0: sdr / sir / sar / selection (items, K) of the first maximiser, in
+ * itertools.permutations(range(E), K) order, of the mean SIR (np.mean's summation order; np.argmax: the first NaN
+ * wins).  compute_permutation = 0 (needs E = K): the pairs (k, k); selection is not written (may be null).
+ * pairs (items, 3, E, K) float64, may be null: SDR, SIR, SAR of every pair.
+ * *status (long long; set to 0 by the call) = ((item + 1) << 3) | flags of the first failing item, flags: 1 = an
+ * all-zero reference or estimate (mir_eval's validate raises ValueError; the reference's K + 1 path would fall
+ * through to lstsq), 2 = a non-finite sample, 4 = an exactly zero LU pivot (mir_eval switches to lstsq there).  A
+ * failing item's outputs are NaN.  Items run `group` at a time, which sets the workspace
+ * (pbb_bss_eval_workspace_bytes: G alone is group * N * (N + 16) * 8 bytes, 135 MB per item at K = 8). */
+#define PBB_BSS_EVAL_FILTER 512
+#define PBB_BSS_EVAL_MAX_SOURCES 8        /* K <= 8, N <= 4096 (OutputMetrics asserts K <= 8) */
+#define PBB_BSS_EVAL_MAX_SAMPLES 4194304  /* 2^22 */
+#define PBB_BSS_EVAL_MAX_GROUP 65535
+size_t pbb_bss_eval_workspace_bytes(long long group, int K, int E, long long T);
+int pbb_bss_eval(const double* x, long long items, int K, int E, long long T, int compute_permutation,
+                 long long group, void* workspace, size_t workspace_bytes, double* sdr, double* sir, double* sar,
+                 long long* selection, double* pairs, long long* status, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

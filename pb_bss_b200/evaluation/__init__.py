@@ -1,3 +1,4 @@
+from .module_mir_eval import mir_eval_sources  # noqa: F401
 from .module_srmr import srmr  # noqa: F401
 
-__all__ = ['srmr']
+__all__ = ['mir_eval_sources', 'srmr']
