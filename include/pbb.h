@@ -691,10 +691,16 @@ int pbb_array_geometry(int mode, const double* points, int S, const double* sens
  * as size double pairs.  Spectra are (rows, frames, size/2 + 1) complex128, frame-major.
  */
 
+/* Host only: the frames per CTA (fpc) of the forward and inverse kernels for rows x frames frames of `size` points on
+ * a GPU with `sms` SMs.  fpc starts at 4096 / size (two 32 KB ping-pong buffers) and is halved while
+ * rows * ceil(frames / fpc) < 2 sms.  pbb_stft, pbb_istft and pbb_griffin_lim_stft launch with this value for the
+ * current device.  A frame's arithmetic does not depend on fpc. */
+int pbb_stft_frames_per_cta(int size, long long rows, int frames, int sms);
+
 /* nara_wpe stft: frame t of row r holds x[r][t shift - offset + j] * window[j] for j < window_length (zero outside
  * [0, n): offset = window_length - shift with fading, else 0; the end padding of pad=True is the same zero read), then
  * rfft(frame, n=size) -> out[r][t].  x (rows, n) float32 (dtype PBB_F32) or float64 (PBB_F64); window (wl) float64.
- * Replaces the np.pad / segment_axis / einsum / rfft sequence of nara_wpe.utils.stft. */
+ * Replaces the np.pad / segment_axis / einsum / rfft sequence of nara_wpe.utils.stft.  x may be null when n = 0. */
 int pbb_stft(const void* x, int dtype, long long rows, long long n, int size, int shift,
              int window_length, int offset, int frames, const double* window,
              const double* twiddle, void* out, void* stream);
@@ -702,7 +708,8 @@ int pbb_stft(const void* x, int dtype, long long rows, long long n, int size, in
 /* GriffinLim.step / MISI.step (griffin_lim_module.py:63-66, 112-130), the STFT half: X_dash_dash = stft(x) and, in
  * the same pass, X_dash = |X| exp(i angle(X_dash_dash)) (exp(i angle(0)) = 1).  y == NULL: Griffin-Lim, x = x_hat
  * (K, n).  y != NULL (n float64): MISI, x = x_hat + (y - sum_k x_hat) / K with the sum in row order.  X, X_dash_dash
- * and X_dash are (K, frames, size/2 + 1) complex128.  The iSTFT half is pbb_istft. */
+ * and X_dash are (K, frames, size/2 + 1) complex128.  The iSTFT half is pbb_istft.  With n = 0, x_hat and y may be
+ * null (every frame of x is zero, so both forms give X_dash_dash = 0 and X_dash = |X|). */
 int pbb_griffin_lim_stft(const double* x_hat, int K, long long n, const double* y,
                          const void* X, int size, int shift, int window_length, int offset,
                          int frames, const double* window, const double* twiddle,

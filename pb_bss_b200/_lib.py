@@ -137,6 +137,7 @@ SIGNATURES = {
     'pbb_steering_vector': (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
     'pbb_diffuse_noise_coherence': (_i, [_vp, _i, _vp, _i, _d, _vp, _vp]),
     'pbb_array_geometry': (_i, [_i, _vp, _i, _vp, _i, _i, _d, _vp, _vp]),
+    'pbb_stft_frames_per_cta': (_i, [_i, _ll, _i, _i]),
     'pbb_stft': (_i, [_vp, _i, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_griffin_lim_stft': (_i, [_vp, _i, _ll, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'pbb_istft_workspace_bytes': (_sz, [_ll, _i, _i]),

@@ -25,12 +25,8 @@ static int sm_count() {
   return n;
 }
 
-// Frames per CTA: as many as the 64 KB shared-memory budget allows, halved while the grid would not give every SM
-// two CTAs.
 static int frames_per_cta(int size, long long rows, int frames) {
-  int fpc = kFftFrameBudget / size;
-  while (fpc > 1 && rows * ((frames + fpc - 1) / fpc) < 2ll * sm_count()) fpc /= 2;
-  return fpc;
+  return pbb_stft_frames_per_cta(size, rows, frames, sm_count());
 }
 
 template <class K>
@@ -89,10 +85,23 @@ using namespace pbb;
 
 extern "C" {
 
+// Frames per CTA: as many as the 64 KB shared-memory budget allows, halved while the grid would not give every SM
+// two CTAs.
+int pbb_stft_frames_per_cta(int size, long long rows, int frames, int sms) {
+  PBB_CHECK_ARG(log2_size(size) > 0, 1, "size must be a power of two in [64, 4096]");
+  PBB_CHECK_ARG(rows > 0, 2, "rows must be positive");
+  PBB_CHECK_ARG(frames > 0, 3, "frames must be positive");
+  PBB_CHECK_ARG(sms > 0, 4, "sms must be positive");
+  int fpc = kFftFrameBudget / size;
+  while (fpc > 1 && rows * ((frames + fpc - 1) / fpc) < 2ll * sms) fpc /= 2;
+  return fpc;
+}
+
 int pbb_stft(const void* x, int dtype, long long rows, long long n, int size, int shift, int window_length,
              int offset, int frames, const double* window, const double* twiddle, void* out, void* stream) {
   const int logN = log2_size(size);
-  PBB_CHECK_ARG(x != nullptr, 1, "x is null");
+  // an empty CUDA tensor has a null data pointer; with n = 0 no sample is read
+  PBB_CHECK_ARG(x != nullptr || n == 0, 1, "x is null");
   PBB_CHECK_ARG(dtype == PBB_F32 || dtype == PBB_F64, 2, "dtype must be PBB_F32 or PBB_F64");
   PBB_CHECK_ARG(rows > 0, 3, "rows must be positive");
   PBB_CHECK_ARG(n >= 0, 4, "n must be non-negative");
@@ -127,7 +136,7 @@ int pbb_griffin_lim_stft(const double* x_hat, int K, long long n, const double* 
                          int window_length, int offset, int frames, const double* window, const double* twiddle,
                          void* X_dash_dash, void* X_dash, void* stream) {
   const int logN = log2_size(size);
-  PBB_CHECK_ARG(x_hat != nullptr, 1, "x_hat is null");
+  PBB_CHECK_ARG(x_hat != nullptr || n == 0, 1, "x_hat is null");
   PBB_CHECK_ARG(K > 0, 2, "K must be positive");
   PBB_CHECK_ARG(n >= 0, 3, "n must be non-negative");
   PBB_CHECK_ARG(X != nullptr, 5, "X is null");
