@@ -825,6 +825,49 @@ int pbb_bss_eval(const double* x, long long items, int K, int E, long long T, in
                  long long* selection, double* pairs, long long* status, void* stream);
 
 /* ------------------------------------------------------------------------
+ * STOI, the short-time objective intelligibility (Taal et al. 2011) of pb_bss/evaluation/module_stoi.py:4-25, i.e.
+ * pystoi.stoi(x, y, fs_sig) with extended=False, for every row of a batch at once.  csrc/stoi.cuh.  fp64 throughout,
+ * no float atomics: bitwise reproducible, and a row's results do not depend on the rest of the batch or on `group`.
+ *
+ * x (reference) and y (estimate) are (rows, n), both float32 (PBB_F32) or both float64 (PBB_F64), read in place.
+ * Per row:
+ *  1. up / down != 1 (10000 / fs in lowest terms): scipy.signal.resample_poly(s, 10000, fs, window=h / h.sum()) of x
+ *     and y, L = ceil(n up / down) samples.  taps (up, taps_per_phase) float64: taps[ph][m] = hp[ph + m up] (0 past
+ *     the end), where hp is resample_poly's filter: the window times up, preceded by its n_pre_pad zeros; pre_remove
+ *     is its n_pre_remove.  Output j is sum_m taps[ph][m] x[i0 - m] with t = (j + pre_remove) down, ph = t mod up,
+ *     i0 = t / up (x = 0 outside [0, n)).  up = down = 1: L = n, the input is framed as it is; taps may be null.
+ *  2. the silent-frame removal (pystoi.utils.remove_silent_frames): F frames f with 128 f < L - 256 (strict),
+ *     E_f = 20 log10(||window * x_f|| + eps); frame f is kept where (max E - 40) - E_f < 0 (a NaN max keeps none);
+ *     K_r kept frames, M_r = max(K_r - 1, 0) STFT frames of the overlap-added signal.
+ *  3. the STFT (pystoi.utils.stft): STFT frame i is kept frames i - 1, i, i + 1 overlap-added, windowed again,
+ *     rfft(n=512) with the twiddle table (512 (cos, sin)(2 pi k / 512) pairs, the STFT's convention); band energies
+ *     sqrt(sum_{bands[b][0] <= k < bands[b][1]} |X_k|^2) for the 15 one-third octave bands (bands (15, 2) int).
+ *     window (256) float64 = np.hanning(258)[1:-1].
+ *  4. M_r < 30: out[r] = 1e-5 (pystoi warns and returns 1e-5).  Else the J_r = M_r - 29 segments of 30 frames:
+ *     y' = min(y_seg ||x_seg|| / (||y_seg|| + eps), x_seg (1 + 10^(15/20))) (NaN if either is), both mean-removed and
+ *     divided by (norm + eps), and out[r] = sum of the inner products over (segment, band) / (J_r 15).
+ * out (rows) float64.  frames (rows, 2) long long, may be null: K_r, M_r.  resampled (rows, 2, L) float64, may be
+ * null: x and y at 10 kHz (not written at 10 kHz).  energies (rows, 2, 15, M_max = F - 1) float64, may be null: the
+ * band energies of x and y (entries from M_r on are not written).  status (2 long long, set by the call): the number
+ * of rows with M_r < 30 and the first such row (-1: none).  Rows run `group` at a time, which sets the workspace
+ * (pbb_stoi_workspace_bytes; 0 for an invalid shape).  n must be in [1, PBB_STOI_MAX_SAMPLES] and L in
+ * (PBB_STOI_FRAME, PBB_STOI_MAX_RESAMPLED]: at most 256 samples at 10 kHz give no frame, where pystoi raises. */
+#define PBB_STOI_FS 10000
+#define PBB_STOI_FRAME 256
+#define PBB_STOI_NFFT 512
+#define PBB_STOI_BANDS 15
+#define PBB_STOI_SEGMENT 30
+#define PBB_STOI_DYN_RANGE 40
+#define PBB_STOI_MAX_SAMPLES 4194304    /* 2^22 */
+#define PBB_STOI_MAX_RESAMPLED 8388608  /* 2^23 samples at 10 kHz */
+#define PBB_STOI_MAX_GROUP 65535
+size_t pbb_stoi_workspace_bytes(long long group, long long n, int up, int down);
+int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+             const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
+             const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
+             long long* frames, double* resampled, double* energies, long long* status, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

@@ -155,6 +155,9 @@ SIGNATURES = {
     'pbb_srmr_ratio': (_i, [_vp, _ll, _i, _vp, _vp, _vp, _vp]),
     'pbb_bss_eval_workspace_bytes': (_sz, [_ll, _i, _i, _ll]),
     'pbb_bss_eval': (_i, [_vp, _ll, _i, _i, _ll, _i, _ll, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'pbb_stoi_workspace_bytes': (_sz, [_ll, _ll, _i, _i]),
+    'pbb_stoi': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _vp, _vp, _vp, _vp,
+                      _vp, _vp]),
 }
 
 _lib = None

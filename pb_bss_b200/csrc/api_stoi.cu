@@ -1,0 +1,171 @@
+// C-ABI entry points for STOI, pb_bss/evaluation/module_stoi.py -- see include/pbb.h and csrc/stoi.cuh.
+#include "common.cuh"
+#include "prof.cuh"
+#include "stoi.cuh"
+
+namespace pbb {
+
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+static long long gcd_ll(long long a, long long b) {
+  while (b) {
+    const long long t = a % b;
+    a = b;
+    b = t;
+  }
+  return a;
+}
+
+struct StoiShape {
+  long long L;         // length at 10 kHz: ceil(n up / down)
+  int F, Mmax, blocks;
+  bool resample;
+};
+
+static bool stoi_shape(long long n, int up, int down, StoiShape* s) {
+  if (n < 1 || n > PBB_STOI_MAX_SAMPLES || up < 1 || down < 1 || gcd_ll(up, down) != 1) return false;
+  const long long L = (n * up + down - 1) / down;
+  if (L <= kStoiFrame || L > PBB_STOI_MAX_RESAMPLED) return false;
+  s->L = L;
+  s->F = (int)((L - kStoiFrame + kStoiHop - 1) / kStoiHop);  // 128 f < L - 256
+  s->Mmax = s->F - 1;
+  s->blocks = s->Mmax >= kStoiSeg ? (s->Mmax - kStoiSeg + 1 + kStoiSegBlock - 1) / kStoiSegBlock : 1;
+  s->resample = !(up == 1 && down == 1);
+  return true;
+}
+
+struct StoiLayout {
+  size_t sig, energy, kept, km, tob, partial, total;  // byte offsets
+};
+
+static StoiLayout stoi_layout(long long group, const StoiShape& s) {
+  StoiLayout l;
+  l.sig = 0;
+  l.energy = align256(l.sig + (s.resample ? (size_t)group * 2 * s.L * sizeof(double) : 0));
+  l.kept = align256(l.energy + (size_t)group * s.F * sizeof(double));
+  l.km = align256(l.kept + (size_t)group * s.F * sizeof(int));
+  l.tob = align256(l.km + (size_t)group * 2 * sizeof(long long));
+  l.partial = align256(l.tob + (size_t)group * 2 * kStoiBands * s.Mmax * sizeof(double));
+  l.total = l.partial + (size_t)group * s.blocks * sizeof(double);
+  return l;
+}
+
+template <class T>
+static int stoi_group(StoiParams p, const StoiShape& s, cudaStream_t st) {
+  if (s.resample) {
+    const long long total = p.rows * 2 * p.L;
+    const long long ctas = std::min<long long>((total + kStoiThreads - 1) / kStoiThreads, 1ll << 20);
+    LaunchScope ls("stoi_resample_kernel", st);
+    stoi_resample_kernel<T><<<(unsigned)ctas, kStoiThreads, 0, st>>>(p);
+    PBB_CUDA(cudaGetLastError());
+  }
+  // past the resampler every sample is read from p.sig as double, or from the input as T at 10 kHz
+  auto run = [&](auto tag) -> int {
+    using U = decltype(tag);
+    {
+      const long long warps = p.rows * p.F;
+      LaunchScope ls("stoi_energy_kernel", st);
+      stoi_energy_kernel<U><<<(unsigned)((warps * 32 + kStoiThreads - 1) / kStoiThreads), kStoiThreads, 0, st>>>(p);
+      PBB_CUDA(cudaGetLastError());
+    }
+    {
+      LaunchScope ls("stoi_compact_kernel", st);
+      stoi_compact_kernel<<<(unsigned)p.rows, kStoiCompactThreads, 0, st>>>(p);
+      PBB_CUDA(cudaGetLastError());
+    }
+    if (p.Mmax > 0) {
+      const long long ctas = p.rows * 2 * ((p.Mmax + kStoiFpc - 1) / kStoiFpc);
+      LaunchScope ls("stoi_bands_kernel", st);
+      stoi_bands_kernel<U><<<(unsigned)ctas, kStoiThreads, 0, st>>>(p);
+      PBB_CUDA(cudaGetLastError());
+    }
+    {
+      LaunchScope ls("stoi_segment_kernel", st);
+      stoi_segment_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, 0, st>>>(p);
+      PBB_CUDA(cudaGetLastError());
+    }
+    LaunchScope ls("stoi_value_kernel", st);
+    stoi_value_kernel<<<1, kStoiThreads, 0, st>>>(p);
+    PBB_CUDA(cudaGetLastError());
+    return 0;
+  };
+  if (s.resample) return run(double{});
+  return run(T{});
+}
+
+}  // namespace pbb
+
+using namespace pbb;
+
+extern "C" {
+
+size_t pbb_stoi_workspace_bytes(long long group, long long n, int up, int down) {
+  StoiShape s;
+  if (group <= 0 || group > PBB_STOI_MAX_GROUP || !stoi_shape(n, up, down, &s)) return 0;
+  return stoi_layout(group, s).total;
+}
+
+int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+             const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
+             const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
+             long long* frames, double* resampled, double* energies, long long* status, void* stream) {
+  StoiShape s;
+  PBB_CHECK_ARG(x != nullptr, 1, "x is null");
+  PBB_CHECK_ARG(y != nullptr, 2, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_F32 || dtype == PBB_F64, 3, "dtype must be PBB_F32 or PBB_F64");
+  PBB_CHECK_ARG(rows > 0 && rows <= 0x7fffffffll / 64, 4, "rows out of range");
+  PBB_CHECK_ARG(stoi_shape(n, up, down, &s), 5,
+                "n must be in [1, PBB_STOI_MAX_SAMPLES], up / down in lowest terms, and ceil(n up / down) in "
+                "(PBB_STOI_FRAME, PBB_STOI_MAX_RESAMPLED]");
+  PBB_CHECK_ARG(!s.resample || taps != nullptr, 8, "taps is null");
+  PBB_CHECK_ARG(!s.resample || taps_per_phase > 0, 9, "taps_per_phase must be positive");
+  PBB_CHECK_ARG(pre_remove >= 0, 10, "pre_remove must not be negative");
+  PBB_CHECK_ARG(window != nullptr && bands != nullptr && twiddle != nullptr, 11, "a table is null");
+  PBB_CHECK_ARG(group > 0 && group <= PBB_STOI_MAX_GROUP, 14, "group must be in [1, PBB_STOI_MAX_GROUP]");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_stoi_workspace_bytes(group, n, up, down), 15,
+                "workspace too small (pbb_stoi_workspace_bytes)");
+  PBB_CHECK_ARG(out != nullptr, 17, "out is null");
+  PBB_CHECK_ARG(status != nullptr, 21, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const StoiLayout l = stoi_layout(group, s);
+  char* w = static_cast<char*>(workspace);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(long long), st));
+  PBB_CUDA(cudaMemsetAsync(status + 1, 0xff, sizeof(long long), st));
+  const size_t esz = dtype == PBB_F32 ? sizeof(float) : sizeof(double);
+  for (long long g0 = 0; g0 < rows; g0 += group) {
+    const long long g = rows - g0 < group ? rows - g0 : group;
+    StoiParams p{};
+    p.x = static_cast<const char*>(x) + (size_t)g0 * n * esz;
+    p.y = static_cast<const char*>(y) + (size_t)g0 * n * esz;
+    p.rows = g;
+    p.n = n;
+    p.L = s.L;
+    p.F = s.F;
+    p.Mmax = s.Mmax;
+    p.blocks = s.blocks;
+    p.up = up;
+    p.down = down;
+    p.tpp = taps_per_phase;
+    p.pre_remove = pre_remove;
+    p.taps = taps;
+    p.window = window;
+    p.bands = bands;
+    p.tw = reinterpret_cast<const double2*>(twiddle);
+    p.sig = !s.resample ? nullptr
+            : resampled ? resampled + (size_t)g0 * 2 * s.L
+                        : reinterpret_cast<double*>(w + l.sig);
+    p.energy = reinterpret_cast<double*>(w + l.energy);
+    p.kept = reinterpret_cast<int*>(w + l.kept);
+    p.km = frames ? frames + 2 * g0 : reinterpret_cast<long long*>(w + l.km);
+    p.tob = energies ? energies + (size_t)g0 * 2 * kStoiBands * s.Mmax : reinterpret_cast<double*>(w + l.tob);
+    p.partial = reinterpret_cast<double*>(w + l.partial);
+    p.out = out + g0;
+    p.status = status;
+    p.row0 = g0;
+    const int rc = dtype == PBB_F32 ? stoi_group<float>(p, s, st) : stoi_group<double>(p, s, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+}  // extern "C"

@@ -1,4 +1,5 @@
 from .module_mir_eval import mir_eval_sources  # noqa: F401
 from .module_srmr import srmr  # noqa: F401
+from .module_stoi import stoi  # noqa: F401
 
-__all__ = ['mir_eval_sources', 'srmr']
+__all__ = ['mir_eval_sources', 'srmr', 'stoi']
