@@ -868,6 +868,51 @@ int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long 
              long long* frames, double* resampled, double* energies, long long* status, void* stream);
 
 /* ------------------------------------------------------------------------
+ * SI-SDR (pb_bss/evaluation/module_si_sdr.py:4-56) and the invasive SxR (pb_bss/evaluation/sxr_module.py:17-274).
+ * csrc/sxr.cuh.  fp64 throughout, no float atomics.  A row of n samples is summed in ceil(n / PBB_SXR_CHUNK) chunks,
+ * each in a fixed order inside one CTA, then the chunk partials in a fixed order: the tree depends on n only, so a
+ * row's value is bitwise the same in any batch.  Products and differences round as NumPy's do (no FMA); only the order
+ * of the length-n sums differs from NumPy's pairwise sum.  Every call only enqueues work on `stream`. */
+#define PBB_SXR_CHUNK 8192
+#define PBB_SXR_MAX_K 9    /* sxr_module asserts K < 10 */
+#define PBB_SXR_MAX_D 29   /* input_sxr asserts D < 30 */
+#define PBB_I16 4
+#define PBB_I32 5
+#define PBB_I64 6
+/* get_variance_for_zero_mean_signal (:17-23) over the last axis: out[r] = mean |x[r, :]|^2, float64 (rows).  x (rows, n)
+ * contiguous, dtype PBB_F32 / PBB_F64 / PBB_I16 / PBB_I32 / PBB_I64 (x^2 in fp64) or PBB_C64 / PBB_C128 (re re + im im).
+ * n = 0 gives NaN (np.mean of nothing) and x may then be null.  Workspace: rows * chunks doubles
+ * (pbb_mean_square_workspace_bytes; may be null when that is 0). */
+size_t pbb_mean_square_workspace_bytes(long long rows, long long n);
+int pbb_mean_square(const void* x, int dtype, long long rows, long long n, void* workspace, size_t workspace_bytes,
+                    double* out, void* stream);
+/* si_sdr (:38-56) per row: alpha = <r, e> / <r, r> (pass 1), then 10 log10(sum (alpha r)^2 / sum (e - alpha r)^2) from
+ * the rounded projection alpha r and residual e - alpha r (pass 2), with the same summation tree for every sum: e = 2^j r
+ * gives alpha = 2^j, a zero residual and +inf; a zero reference or estimate gives NaN.  reference / estimation float64,
+ * row r at reference + reference_offsets[r] and estimation + estimation_offsets[r] (device int64 element offsets, so a
+ * broadcast operand is not materialised), n contiguous samples each.  Workspace: pbb_si_sdr_workspace_bytes. */
+size_t pbb_si_sdr_workspace_bytes(long long rows, long long n);
+int pbb_si_sdr(const double* reference, const double* estimation, const long long* reference_offsets,
+               const long long* estimation_offsets, long long rows, long long n, void* workspace,
+               size_t workspace_bytes, double* out, void* stream);
+/* input_sxr (:94-165) from the powers S (K, D) and N (D), float64 on the device, in the reference's order of
+ * operations: I[k, d] = np.sum of S[n != k, d], the channel means (average_channels), S / (I + N), S / I, S / N in dB
+ * (IEEE inf / nan for zero powers), then the source mean (average_sources).  sdr / sir / snr have the shape of the
+ * result: (K, D), (K), (D) or one value.  np.sum of fewer than 8 values is a left-to-right loop, from 8 on NumPy's
+ * 8-accumulator pairwise pattern; np.mean(axis=0) of (K, D > 1) adds the rows in order.  1 <= K <= PBB_SXR_MAX_K,
+ * 1 <= D <= PBB_SXR_MAX_D. */
+int pbb_input_sxr(const double* S, const double* N, int K, int D, int average_sources, int average_channels,
+                  double* sdr, double* sir, double* snr, void* stream);
+/* output_sxr (:168-274) from S (K_source, K_target) and N (K_target): the mutual power np.sum(S[k, p[k]]) of every
+ * p of itertools.permutations(range(K_target), K_source) (up to 9! = 362880, unranked in parallel), the first maximiser
+ * as np.argmax picks it (a NaN wins), then SDR / SIR / SNR (K_source, or their means with average_sources) and
+ * selection (K_source) int64.  1 <= K_source <= K_target <= PBB_SXR_MAX_K.  Workspace:
+ * pbb_output_sxr_workspace_bytes. */
+size_t pbb_output_sxr_workspace_bytes(int K_source, int K_target);
+int pbb_output_sxr(const double* S, const double* N, int K_source, int K_target, int average_sources, void* workspace,
+                   size_t workspace_bytes, double* sdr, double* sir, double* snr, long long* selection, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

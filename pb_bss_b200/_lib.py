@@ -30,6 +30,7 @@ class CacgmmOptions(ctypes.Structure):
 
 
 PBB_F32, PBB_F64 = 2, 3
+PBB_I16, PBB_I32, PBB_I64 = 4, 5, 6
 MASK_MAX_DIMS = 8
 MASK_IDEAL_BINARY, MASK_WIENER_LIKE, MASK_IDEAL_RATIO, MASK_IDEAL_AMPLITUDE, MASK_PHASE_SENSITIVE, \
     MASK_IDEAL_COMPLEX = range(6)
@@ -158,6 +159,13 @@ SIGNATURES = {
     'pbb_stoi_workspace_bytes': (_sz, [_ll, _ll, _i, _i]),
     'pbb_stoi': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _vp, _vp, _vp, _vp,
                       _vp, _vp]),
+    'pbb_mean_square_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_mean_square': (_i, [_vp, _i, _ll, _ll, _vp, _sz, _vp, _vp]),
+    'pbb_si_sdr_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_si_sdr': (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp, _sz, _vp, _vp]),
+    'pbb_input_sxr': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_output_sxr_workspace_bytes': (_sz, [_i, _i]),
+    'pbb_output_sxr': (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

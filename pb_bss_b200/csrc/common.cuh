@@ -168,6 +168,9 @@ __device__ __forceinline__ double2 ld_cplx(const float2* p) {
 __device__ __forceinline__ void st_cplx(double2* p, double re, double im) { *p = make_double2(re, im); }
 __device__ __forceinline__ void st_cplx(float2* p, double re, double im) { *p = make_float2((float)re, (float)im); }
 
+// |s|^2 as NumPy rounds it: two products, one sum, no FMA contraction
+__device__ __forceinline__ double abs2_rn(double2 v) { return __dadd_rn(__dmul_rn(v.x, v.x), __dmul_rn(v.y, v.y)); }
+
 // ---- warp reductions ---------------------------------------------------------
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll

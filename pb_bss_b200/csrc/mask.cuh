@@ -42,9 +42,6 @@ __device__ __forceinline__ void st_elem(float* p, double2 v) { *p = (float)v.x; 
 __device__ __forceinline__ void st_elem(double2* p, double2 v) { *p = v; }
 __device__ __forceinline__ void st_elem(float2* p, double2 v) { *p = make_float2((float)v.x, (float)v.y); }
 
-// |s|^2 as NumPy rounds it: two products, one sum, no FMA contraction
-__device__ __forceinline__ double abs2_rn(double2 v) { return __dadd_rn(__dmul_rn(v.x, v.x), __dmul_rn(v.y, v.y)); }
-
 // |s| rounded to nearest (np.abs = hypot): the square root of the exact sum of squares, corrected by one Newton step
 // on the residual; scaled by a power of two so that neither square over- or underflows
 __device__ __forceinline__ double abs_rn(double2 v) {

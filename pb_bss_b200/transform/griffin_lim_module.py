@@ -2,14 +2,13 @@
 
 The state (x_hat, X_dash, X_dash_dash) lives on the device; ``step()`` only enqueues kernels (one STFT pass that also
 forms X_dash, one iSTFT) and never synchronises the host.  The attributes are numpy arrays, copied on access, when the
-instance was built from numpy, and CUDA tensors otherwise.  ``evaluate()`` is not provided: it needs
-pb_bss.evaluation (mir_eval), which this package does not build.
+instance was built from numpy, and CUDA tensors otherwise.
 """
 import numpy as np
 import torch
 
 from .. import _device
-from .fourier import griffin_lim_stft, istft
+from .fourier import griffin_lim_stft, istft, stft
 
 
 class GriffinLim:
@@ -40,6 +39,22 @@ class GriffinLim:
             self._x_hat = (self._y[None, :] / K_dev).repeat(K, 1)
         else:
             raise ValueError(first_guess)
+
+    def evaluate(self, speech_source):
+        """dict of mir_eval_sdr and mir_eval_sir, the means over the sources of OutputMetrics(x_hat, speech_source,
+        enable_si_sdr=True).mir_eval, and inconsistency, the mean of |X_dash - stft(istft(X_dash))|^2 with this
+        instance's transforms.  np.float64 values for an instance built from numpy, 0-d CUDA tensors otherwise."""
+        from ..evaluation import OutputMetrics
+        from ..evaluation.sxr_module import get_variance_for_zero_mean_signal
+        metrics = OutputMetrics(speech_prediction=self._x_hat, speech_source=_device.to_device(speech_source),
+                                enable_si_sdr=True)
+        inconsistency = get_variance_for_zero_mean_signal(
+            self._X_dash - stft(self._istft(self._X_dash), size=self.size, shift=self.shift, fading=self.fading))
+        sdr, sir = metrics.mir_eval['sdr'], metrics.mir_eval['sir']
+        if self._numpy:
+            return dict(mir_eval_sdr=np.mean(sdr.cpu().numpy()), mir_eval_sir=np.mean(sir.cpu().numpy()),
+                        inconsistency=np.float64(inconsistency.cpu().numpy()))
+        return dict(mir_eval_sdr=sdr.mean(), mir_eval_sir=sir.mean(), inconsistency=inconsistency)
 
     def _istft(self, X):
         return istft(X, size=self.size, shift=self.shift, fading=self.fading)
