@@ -913,6 +913,37 @@ int pbb_output_sxr(const double* S, const double* N, int K_source, int K_target,
                    size_t workspace_bytes, double* sdr, double* sir, double* snr, long long* selection, void* stream);
 
 /* ------------------------------------------------------------------------
+ * k-means of BinaryGMMTrainer (pb_bss/distribution/gmm.py:176-230): sklearn.cluster.KMeans(n_clusters=K) with its
+ * defaults (k-means++, n_init='auto' = 1, Lloyd, max_iter 300, tol 1e-4), in fp64.
+ */
+#define PBB_KMEANS_MAX_K 16
+#define PBB_KMEANS_MAX_E 64
+
+/* Workspace of pbb_kmeans_fit: (N (E + 7) + O(256 (K E + K + 2 E))) doubles; 0 for a shape outside the limits. */
+size_t pbb_kmeans_workspace_bytes(long long N, int E, int K);
+/* KMeans.fit on x (N, E) float64 row-major: X_mean and the centred copy, tol = 1e-4 * mean(var(x, axis=0)), the
+ * initial centres, then _kmeans_single_lloyd (the labels as the first argmin of |c|^2 - 2 x.c; strict convergence
+ * when no label changed, else stop when the summed squared centre shift is <= tol; the final E-step when not strict;
+ * empty clusters relocated as _relocate_empty_clusters_dense, with the farthest points taken largest first, ties to
+ * the lower index).  Initial centres: init (K, E) device, raw coordinates, when not null; else _kmeans_plusplus with
+ * n_local_trials L = 2 + int(log K) from the host's draws: first = the index of the first centre
+ * (random_state.choice), uniforms (K - 1, L) device = the unscaled random_state.uniform draws of the K - 1 rounds.
+ * Out: centres (K, E) with X_mean added back, labels (N) int32, inertia, n_iter.  *status (device) is zeroed, then
+ * bit 0 = x holds a non-finite value (nothing is fitted), bit 1 = fewer distinct labels than K, with their count in
+ * bits 8 and up.  Every sum runs in an order that depends on N only, so the results are bitwise repeatable and
+ * do not depend on the grid: max_ctas > 0 caps the CTAs of the two cooperative launches (0 = as many as the device
+ * holds at once, up to one per chunk of at most 256).  Relocation follows sklearn: no point moves when the largest
+ * distance to an old centre is 0.  Needs a device with cooperative launch (every H100 has it).
+ * 1 <= K <= min(N, PBB_KMEANS_MAX_K), 1 <= E <= PBB_KMEANS_MAX_E, N < 2^31. */
+int pbb_kmeans_fit(const double* x, long long N, int E, int K, long long first, const double* uniforms,
+                   const double* init, int max_iter, void* workspace, size_t workspace_bytes, double* centres,
+                   int* labels, double* inertia, int* n_iter, int* status, int max_ctas, void* stream);
+/* KMeans.predict: labels (N) int32 = the first argmin of |c|^2 - 2 x.c over centres (K, E); one_hot (K, N) float64
+ * (labels_to_one_hot(labels, K, axis=-2)).  Either output may be null. */
+int pbb_kmeans_predict(const double* x, long long N, int E, int K, const double* centres, int* labels,
+                       double* one_hot, void* stream);
+
+/* ------------------------------------------------------------------------
  * Frequency permutation alignment (pb_bss/permutation_alignment.py).
  */
 

@@ -166,6 +166,9 @@ SIGNATURES = {
     'pbb_input_sxr': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_output_sxr_workspace_bytes': (_sz, [_i, _i]),
     'pbb_output_sxr': (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
+    'pbb_kmeans_workspace_bytes': (_sz, [_ll, _i, _i]),
+    'pbb_kmeans_fit': (_i, [_vp, _ll, _i, _i, _ll, _vp, _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
+    'pbb_kmeans_predict': (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

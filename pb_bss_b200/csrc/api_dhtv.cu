@@ -93,23 +93,6 @@ __device__ unsigned long long g_dhtv_iters;
 #define DH_PH(i) do { } while (0)
 #endif
 
-// Grid-wide barrier of a cooperative launch (all CTAs are resident): a monotonic arrival counter, one atomic and a
-// short acquire spin per CTA -- about a third of the latency of cooperative_groups' grid.sync() here.
-__device__ __forceinline__ void dhtv_grid_barrier(unsigned* counter, unsigned& generation) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    ++generation;
-    __threadfence();
-    atomicAdd(counter, 1u);
-    const unsigned target = generation * gridDim.x;
-    unsigned seen;
-    do {
-      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
-    } while (seen < target);
-  }
-  __syncthreads();
-}
-
 // block_sum over the FIRST 128 threads only, in a fixed order: dhtv_coop_kernel's block size varies with K, its
 // centroid norms -- and with them every score and the integer mapping -- do not
 __device__ inline double block_sum_first128(double v, double* red) {
@@ -171,7 +154,7 @@ __global__ void __launch_bounds__(32 * kDhtvCoopMaxWarps) dhtv_coop_kernel(
         partial[(size_t)sl * K * T + i] = (s0 + s1) + (s2 + s3);
       }
       DH_PH(0);  // phase A
-      dhtv_grid_barrier(bar, generation);
+      grid_barrier(bar, generation);
       DH_PH(1);  // barrier 1
       // ---- phase B: one CTA per bin; CTAs without a bin skip the centroid ----
       if ((int)blockIdx.x < n) {
@@ -258,7 +241,7 @@ __global__ void __launch_bounds__(32 * kDhtvCoopMaxWarps) dhtv_coop_kernel(
         }
       }
       DH_PH(6);  // permutation / rest of phase B
-      dhtv_grid_barrier(bar, generation);
+      grid_barrier(bar, generation);
       DH_PH(7);  // barrier 2
       if (__ldcg(changed + idx) == 0) {  // nothing moved: the segment has converged (:352-353)
         idx += iters - it;

@@ -171,6 +171,25 @@ __device__ __forceinline__ void st_cplx(float2* p, double re, double im) { *p = 
 // |s|^2 as NumPy rounds it: two products, one sum, no FMA contraction
 __device__ __forceinline__ double abs2_rn(double2 v) { return __dadd_rn(__dmul_rn(v.x, v.x), __dmul_rn(v.y, v.y)); }
 
+// ---- grid barrier -------------------------------------------------------------
+// Grid-wide barrier of a cooperative launch (all CTAs are resident): a monotonic arrival counter, one atomic and a
+// short acquire spin per CTA -- about a third of the latency of cooperative_groups' grid.sync() here.  The counter
+// is zeroed before the launch; generation starts at 0 in every CTA.
+__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& generation) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    ++generation;
+    __threadfence();
+    atomicAdd(counter, 1u);
+    const unsigned target = generation * gridDim.x;
+    unsigned seen;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(counter) : "memory");
+    } while (seen < target);
+  }
+  __syncthreads();
+}
+
 // ---- warp reductions ---------------------------------------------------------
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll

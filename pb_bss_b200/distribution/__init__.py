@@ -10,7 +10,7 @@ from .complex_watson import ComplexWatson, ComplexWatsonTrainer  # noqa: F401
 from .cwmm import CWMM, CWMMTrainer  # noqa: F401
 from .gaussian import DiagonalGaussian, Gaussian, GaussianTrainer, SphericalGaussian  # noqa: F401
 from .gcacgmm import GCACGMM, GCACGMMTrainer  # noqa: F401
-from .gmm import GMM, GMMTrainer  # noqa: F401
+from .gmm import GMM, BinaryGMM, BinaryGMMTrainer, GMMTrainer  # noqa: F401
 from .von_mises_fisher import VonMisesFisher, VonMisesFisherTrainer  # noqa: F401
 from .vmfcacgmm import VMFCACGMM, VMFCACGMMTrainer  # noqa: F401
 from .vmfmm import VMFMM, VMFMMTrainer  # noqa: F401

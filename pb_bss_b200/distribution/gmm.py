@@ -7,8 +7,12 @@ launches on the caller's stream without a host synchronisation: class weights (`
 spherical model, which the reference only accepts without a leading dim > 1), the precision Cholesky factors
 (``pbb_precision_cholesky``, status words read when the loop ends) and the posterior (``pbb_log_pdf_to_affiliation``
 with the leading dims as its bin axis).  All arithmetic is float64.  NumPy in gives NumPy out, a CUDA tensor in gives
-CUDA tensors out (the diagonal / spherical parameters are host arrays, as in the integrated model)."""
+CUDA tensors out (the diagonal / spherical parameters are host arrays, as in the integrated model).
+
+BinaryGMM / BinaryGMMTrainer (gmm.py:176-230) are the k-means baseline of deep clustering, sklearn's
+``KMeans(n_clusters=K)`` on the device (``pbb_kmeans_fit`` / ``pbb_kmeans_predict``)."""
 import math
+import warnings
 from dataclasses import dataclass
 from typing import Any
 
@@ -244,3 +248,152 @@ class GMMTrainer:
             gaussian = cls(mean=state['mean'].reshape(lead + (K, E)).cpu().numpy(),
                            covariance=state['cov'].reshape(lead + state['cov'].shape).cpu().numpy())
         return GMM(weight=weight, gaussian=gaussian)
+
+
+KMEANS_MAX_K = 16    # PBB_KMEANS_MAX_K
+_KMEANS_MAX_ITER = 300
+
+
+class ConvergenceWarning(UserWarning):
+    """sklearn.exceptions.ConvergenceWarning, which the k-means fit issues for fewer distinct clusters than K."""
+
+
+def _kmeans_draws(N, K, sklearn_dtype):
+    """The draws of sklearn's _kmeans_plusplus from NumPy's global RandomState (random_state=None), in its order:
+    the first centre's index, then (K - 1, n_local_trials) unscaled uniforms.  They do not depend on the data."""
+    w = np.ones(N, dtype=sklearn_dtype)
+    first = int(np.random.choice(N, p=w / w.sum()))
+    L = 2 + int(np.log(K))
+    u = np.array([np.random.uniform(size=L) for _ in range(K - 1)], dtype=np.float64).reshape(K - 1, L)
+    return first, u
+
+
+def _check_kmeans_input(x, K):
+    """sklearn's validation of X and n_clusters, and the device limits; x is a CUDA tensor or an ndarray."""
+    if x.ndim != 2:
+        raise ValueError(f'Expected 2D array, got {x.ndim}D array instead.')
+    if not _is_real(x):
+        raise ValueError('Complex data not supported')
+    N, E = x.shape
+    if not 1 <= K <= KMEANS_MAX_K:
+        raise ValueError(f'n_clusters={K}: the device k-means supports 1 <= K <= {KMEANS_MAX_K}')
+    check_embedding_dim(E)
+    if N < K:
+        raise ValueError(f'n_samples={N} should be >= n_clusters={K}.')
+
+
+def _kmeans_fit(x, K, init=None, max_ctas=0):
+    """KMeans(n_clusters=K).fit(x) on the device, or KMeans(n_clusters=K, init=init, n_init=1).fit(x) with init (K, E)
+    -- the latter only for tests, as is max_ctas > 0, a cap on the grid (the results do not depend on it).  x: a 2-D
+    ndarray or CUDA tensor, already checked."""
+    like_numpy = not _device.is_tensor(x)
+    N, E = x.shape
+    xd = _dev(x)
+    dev_init, uniforms, first = None, None, 0
+    if init is not None:
+        dev_init = _dev(init)
+    else:
+        f32 = x.dtype == (np.float32 if like_numpy else torch.float32)
+        first, u = _kmeans_draws(N, K, np.float32 if f32 else np.float64)
+        if K > 1:
+            uniforms = _device.to_device(u, torch.float64)
+    lib = _lib.load()
+    ws = _device.workspace(int(lib.pbb_kmeans_workspace_bytes(N, E, K)))
+    centres = _device.empty((K, E), torch.float64)
+    labels = _device.empty((N,), torch.int32)
+    inertia = _device.empty((), torch.float64)
+    n_iter = _device.empty((), torch.int32)
+    status = _device.empty((1,), torch.int32)
+    _lib.check(lib.pbb_kmeans_fit(_device.ptr(xd), N, E, K, first, _device.ptr(uniforms), _device.ptr(dev_init),
+                                  _KMEANS_MAX_ITER, _device.ptr(ws), ws.numel(), _device.ptr(centres),
+                                  _device.ptr(labels), _device.ptr(inertia), _device.ptr(n_iter), _device.ptr(status),
+                                  max_ctas, _device.stream_ptr()), 'pbb_kmeans_fit')
+
+    def on_status(s):
+        if s & 1:
+            raise ValueError('Input X contains NaN or infinity.')
+        warnings.warn(f'Number of distinct clusters ({s >> 8}) found smaller than n_clusters ({K}). Possibly due to '
+                      'duplicate points in X.', ConvergenceWarning, stacklevel=3)
+    _device.check_status(status, on_status)
+    if like_numpy:
+        return KMeans(K, centres.cpu().numpy(), labels.cpu().numpy(), float(inertia.item()), int(n_iter.item()))
+    return KMeans(K, centres, labels, inertia, n_iter)
+
+
+@dataclass
+class KMeans:
+    """The fitted attributes of sklearn.cluster.KMeans that BinaryGMM users read.  From NumPy input: ndarrays, a float
+    inertia_ and an int n_iter_; from a CUDA tensor: CUDA tensors, inertia_ and n_iter_ 0-d (read without a host
+    synchronisation only when asked for)."""
+    n_clusters: int
+    cluster_centers_: Any   # (K, E) float64
+    labels_: Any            # (N_fit,) int32
+    inertia_: Any
+    n_iter_: Any
+
+    def _labels_one_hot(self, x, one_hot):
+        N, E = x.shape
+        K = self.n_clusters
+        if E != self.cluster_centers_.shape[1]:
+            raise ValueError(f'X has {E} features, but KMeans is expecting {self.cluster_centers_.shape[1]} features '
+                             'as input.')
+        xd = _dev(x)
+        lib = _lib.load()
+        labels = None if one_hot else _device.empty((N,), torch.int32)
+        oh = _device.empty((K, N), torch.float64) if one_hot else None
+        _lib.check(lib.pbb_kmeans_predict(_device.ptr(xd), N, E, K, _device.ptr(_dev(self.cluster_centers_)),
+                                          _device.ptr(labels), _device.ptr(oh), _device.stream_ptr()),
+                   'pbb_kmeans_predict')
+        return oh if one_hot else labels
+
+    def predict(self, x):
+        """KMeans.predict: x (N, E) real -> the index of the closest centre (N,) int32."""
+        like_numpy = not _device.is_tensor(x)
+        if x.ndim != 2:
+            raise ValueError(f'Expected 2D array, got {x.ndim}D array instead.')
+        if not _is_real(x):
+            raise ValueError('Complex data not supported')
+        return _device.to_host(self._labels_one_hot(x, one_hot=False), like_numpy)
+
+
+@dataclass
+class BinaryGMM(_ProbabilisticModel):
+    kmeans: KMeans
+
+    def predict(self, x):
+        """x (N, E) -> affiliation (K, N), the one-hot of the closest centre in x.dtype (gmm.py:180-198)."""
+        like_numpy = not _device.is_tensor(x)
+        N, D = x.shape
+        assert _is_real(x), x.dtype
+        check_embedding_dim(D)
+        oh = self.kmeans._labels_one_hot(x, one_hot=True)
+        if like_numpy:
+            return oh.cpu().numpy().astype(x.dtype, copy=False)
+        return oh if oh.dtype == x.dtype else oh.to(x.dtype)
+
+
+class BinaryGMMTrainer:
+    """k-means trainer (gmm.py:201-230): sklearn's ``KMeans(n_clusters=num_classes).fit`` on the device, with its
+    k-means++ draws taken from NumPy's global RandomState in sklearn's order, so ``np.random.seed(s)`` reproduces the
+    reference's fit.  Integer and float32 input are computed in float64 (sklearn computes float32 in float32).  With
+    CUDA input the fit only enqueues work, except that a CUDA ``saliency`` selects its rows with a host
+    synchronisation (``x[saliency]``); the non-finite check and the distinct-cluster warning come from a device
+    status word, read at the end of a ``deferred_status()`` block."""
+
+    def fit(self, x, num_classes, saliency=None):
+        """x (N, E) real, num_classes K, saliency None or a boolean (N,) selecting the rows to fit."""
+        if x.ndim != 2:
+            raise ValueError(f'Expected 2D array, got {x.ndim}D array instead.')
+        N, D = x.shape
+        if saliency is not None:
+            assert saliency.dtype in (bool, np.bool_, torch.bool), (
+                'Only boolean saliency supported. '
+                f'Current dtype: {saliency.dtype}.'
+            )
+            assert tuple(saliency.shape) == (N,)
+            if _device.is_tensor(x):
+                x = x[_device.to_device(saliency)]
+            else:
+                x = x[np.asarray(saliency.cpu() if _device.is_tensor(saliency) else saliency), :]
+        _check_kmeans_input(x, num_classes)
+        return BinaryGMM(kmeans=_kmeans_fit(x, num_classes))
