@@ -1002,6 +1002,84 @@ int pbb_mapping_from_score_matrix(const double* scores, int F, int K,
 int pbb_chain_mapping(const long long* pair_mapping, int K, int F,
                       long long* mapping, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Single distributions (pb_bss/distribution/complex_angular_central_gaussian.py, complex_watson.py,
+ * complex_circular_symmetric_gaussian.py).  Every model and output is fp64 / complex128; the observation may be
+ * complex64 or complex128 (`dtype`).  Model broadcasting over leading dims is resolved by the caller: y_stride is
+ * the number of elements between the observations of consecutive models, 0 when all models share one y.
+ * ------------------------------------------------------------------------ */
+
+/* ComplexAngularCentralGaussian.from_covariance (complex_angular_central_gaussian.py:81-132) for covariance
+ * (n, D, D): covariance_norm PBB_NORM_TRACE divides by max(real trace, tiny) first (into a copy: the input is not
+ * changed); the Hermitian part is diagonalised (pbb_heig_batched's Jacobi solver); PBB_NORM_EIGENVALUE scales the
+ * eigenvalues by 1 / max(lambda_max, tiny) and floors them at eigenvalue_floor, the other norms floor them at
+ * lambda_max * eigenvalue_floor.  eigenvectors (n, D, D) columns, eigenvalues (n, D) ascending.  0 < D <= 64.
+ * *status (reset by the call) = 1 + the first matrix with non-finite input or eigenvalues (the reference asserts
+ * np.isfinite, :127). */
+int pbb_cacg_from_covariance(const void* covariance, int n, int D, int covariance_norm, double eigenvalue_floor,
+                             void* eigenvectors, double* eigenvalues, int* status, void* stream);
+
+/* ComplexAngularCentralGaussian._log_pdf (:167-203) from the quadratic forms of pbb_cacgmm_predict: quadratic_out
+ * (F, K, T), a buffer of its own, receives max(|q|, q_floor) of quadratic (F, K, T) -- q_floor =
+ * np.finfo(y.dtype).tiny -- and log_pdf (F, K, T) = -D log q - sum_d log eigenvalues (F, K, D).  F * K <= 65535.
+ * pbb_cacg_log_pdf is this with q_floor = DBL_MIN and no quadratic_out. */
+int pbb_cacg_log_pdf_floor(const double* quadratic, const double* eigenvalues, int F, int K, int T, int D,
+                           double q_floor, double* quadratic_out, double* log_pdf, void* stream);
+
+/* The log normalisers of ComplexWatson (complex_watson.py:89-214) for kappa (n), any values, dimension D
+ * (0 < D <= 64), each formula in the reference's order of operations:
+ *   PBB_CW_NORM_1F1     log_norm_1f1 (:157-168) = the mixture model's cw_log_norm: the series of 1F1(1; D; kappa)
+ *                       below kappa = 20, Mardia's closed form above; finite where scipy's hyp1f1 overflows
+ *                       (kappa > ~710), where the reference returns inf;
+ *   PBB_CW_NORM_LOW     log_norm_low_concentration (:90-107), 20 Taylor terms;
+ *   PBB_CW_NORM_MEDIUM  log_norm_medium_concentration (:110-138), kappa < 1e-2 clamped to 1e-2;
+ *   PBB_CW_NORM_HIGH    log_norm_high_concentration (:141-154);
+ *   PBB_CW_NORM_TRAN_VU log_norm_tran_vu (:171-214): low below kappa = 1 / D, the unclamped medium formula from
+ *                       there on. */
+enum { PBB_CW_NORM_1F1 = 0, PBB_CW_NORM_LOW = 1, PBB_CW_NORM_MEDIUM = 2, PBB_CW_NORM_HIGH = 3,
+       PBB_CW_NORM_TRAN_VU = 4 };
+int pbb_cw_log_norm(const double* kappa, long long n, int D, int variant, double* log_norm, void* stream);
+
+/* ComplexWatson.log_pdf (complex_watson.py:73-87): log_pdf (M, N) = kappa |sum_d y_d conj(mode_d)|^2 -
+ * log_norm_1f1(kappa, D) for y (M, N, D) as given (not normalised), mode (M, D) complex128, concentration (M).
+ * 0 < D <= 64. */
+int pbb_cw_log_pdf(const void* y, int dtype, long long y_stride, int M, int N, int D, const void* mode,
+                   const double* concentration, double* log_pdf, void* stream);
+
+/* Scratch of pbb_ccsg_log_pdf / pbb_ccsg_sample for M models (classes) of dimension D. */
+size_t pbb_ccsg_workspace_bytes(int M, int D);
+
+/* ComplexCircularSymmetricGaussian.log_pdf (complex_circular_symmetric_gaussian.py:26-48): log_pdf (M, N) =
+ * -D log pi - log|det S| - Re(y^H S^-1 y) for y (M, N, D) and any invertible covariance S (M, D, D) complex128 --
+ * np.linalg.slogdet and np.linalg.solve, not a Cholesky factor: one LU factorisation with partial pivoting per model
+ * (a warp each), then one thread per (model, frame), so one model with many frames fills the GPU.  0 < D <= 64.
+ * *status (reset by the call) = 1 + the first model with an exactly zero pivot (np.linalg.solve raises
+ * LinAlgError); non-finite covariances give NaN, as in LAPACK. */
+int pbb_ccsg_log_pdf(const void* y, int dtype, long long y_stride, int M, int N, int D, const void* covariance,
+                     double* log_pdf, void* workspace, size_t workspace_bytes, int* status, void* stream);
+
+/* ComplexCircularSymmetricGaussian.sample (:50-72) and sample_complex_angular_central_gaussian
+ * (complex_angular_central_gaussian.py:58-65) for C classes at once; the standard normals are drawn on the host
+ * (NumPy's global stream, in the reference's call order).  eigenvalues == NULL: a (C, D, D) are the covariances
+ * (lower triangles read, like np.linalg.cholesky); else a are eigenvectors (columns) and the covariance is
+ * V diag(eigenvalues) V^H (ComplexAngularCentralGaussian.covariance, :140-148).  normals (2, S, D): the real parts
+ * of all S samples, then the imaginary parts; sample i belongs to the class c with offsets[c] <= i < offsets[c + 1]
+ * (offsets (C + 1), offsets[0] = 0, offsets[C] = S) and is written to out row dest[i] (dest may be NULL: row i).
+ * out (S, D) = L (re + i im) / sqrt(2), L = cholesky(covariance); unit_norm != 0 then divides every row by its
+ * norm.  0 < D <= 64.  *status (reset by the call) = 1 + the first class whose covariance is not positive definite
+ * (np.linalg.cholesky raises LinAlgError). */
+int pbb_ccsg_sample(const void* a, const double* eigenvalues, int C, int D, const double* normals,
+                    const long long* offsets, const long long* dest, long long S, int unit_norm, void* out,
+                    void* workspace, size_t workspace_bytes, int* status, void* stream);
+
+/* ComplexCircularSymmetricGaussianTrainer._fit, covariance_type 'full' (:94-116): covariance (F, D, D) =
+ * sum_n s_n y_n y_n^H / max(sum_n s_n, denominator_floor) for observation (F, D, N) and saliency (F, N), or the
+ * plain average over N without a saliency.  denominator_floor = np.finfo(y.dtype).tiny, the reference's floor (the
+ * float32 tiny for complex64 y).  The sums are pbb_power_spectral_density's; N > 0, D < 35; workspace:
+ * pbb_psd_workspace_bytes(F, N, D, 1). */
+int pbb_ccsg_fit(const void* observation, int dtype, int F, int D, int N, const double* saliency,
+                 double denominator_floor, void* covariance, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

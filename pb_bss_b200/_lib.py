@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get('PBB_LIB') or os.path.join(_HERE, 'libpbb.so')
 
 PBB_C64, PBB_C128 = 0, 1
 NORM_NONE, NORM_EIGENVALUE, NORM_TRACE = 0, 1, 2
+CW_NORM_1F1, CW_NORM_LOW, CW_NORM_MEDIUM, CW_NORM_HIGH, CW_NORM_TRAN_VU = range(5)
 WEIGHT_TIME, WEIGHT_CONST, WEIGHT_TIED_TIME, WEIGHT_TIED, WEIGHT_FRAME = 0, 1, 2, 3, 4
 
 
@@ -169,6 +170,14 @@ SIGNATURES = {
     'pbb_kmeans_workspace_bytes': (_sz, [_ll, _i, _i]),
     'pbb_kmeans_fit': (_i, [_vp, _ll, _i, _i, _ll, _vp, _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
     'pbb_kmeans_predict': (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_cacg_from_covariance': (_i, [_vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp]),
+    'pbb_cacg_log_pdf_floor': (_i, [_vp, _vp, _i, _i, _i, _i, _d, _vp, _vp, _vp]),
+    'pbb_cw_log_norm': (_i, [_vp, _ll, _i, _i, _vp, _vp]),
+    'pbb_cw_log_pdf': (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_ccsg_workspace_bytes': (_sz, [_i, _i]),
+    'pbb_ccsg_log_pdf': (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_ccsg_sample': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _ll, _i, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_ccsg_fit': (_i, [_vp, _i, _i, _i, _i, _vp, _d, _vp, _vp, _sz, _vp]),
 }
 
 _lib = None

@@ -37,14 +37,17 @@ __device__ inline double block_sum_256(double v, double* red) {
   return s;
 }
 
+// q_out (may be null, never q) receives the floored quadratic form
 __global__ void cacg_log_pdf_kernel(const double* __restrict__ q, const double* __restrict__ eigenvalues, int F, int K,
-                                    int T, int D, double* __restrict__ out) {
+                                    int T, int D, double* __restrict__ out, double q_floor = kTiny,
+                                    double* __restrict__ q_out = nullptr) {
   const int fk = blockIdx.y;
   double ld = 0.0;
   for (int d = 0; d < D; ++d) ld += log(eigenvalues[(size_t)fk * D + d]);
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
-  const double qq = fmax(fabs(q[(size_t)fk * T + t]), kTiny);
+  const double qq = fmax(fabs(q[(size_t)fk * T + t]), q_floor);
+  if (q_out) q_out[(size_t)fk * T + t] = qq;
   out[(size_t)fk * T + t] = -(double)D * log(qq) - ld;
 }
 
@@ -515,6 +518,20 @@ int pbb_cacg_log_pdf(const double* quadratic, const double* eigenvalues, int F, 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   LaunchScope ls("cacg_log_pdf_kernel", st);
   cacg_log_pdf_kernel<<<dim3((T + 127) / 128, F * K), 128, 0, st>>>(quadratic, eigenvalues, F, K, T, D, log_pdf);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_cacg_log_pdf_floor(const double* quadratic, const double* eigenvalues, int F, int K, int T, int D,
+                           double q_floor, double* quadratic_out, double* log_pdf, void* stream) {
+  PBB_CHECK_ARG(quadratic && eigenvalues, 1, "input is null");
+  PBB_CHECK_ARG(F > 0 && K > 0 && T > 0 && D > 0 && F * K <= 65535, 3, "bad shape");
+  PBB_CHECK_ARG(quadratic_out != nullptr && quadratic_out != quadratic, 8, "quadratic_out is null or the input");
+  PBB_CHECK_ARG(log_pdf != nullptr, 9, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("cacg_log_pdf_kernel", st);
+  cacg_log_pdf_kernel<<<dim3((T + 127) / 128, F * K), 128, 0, st>>>(quadratic, eigenvalues, F, K, T, D, log_pdf,
+                                                                      q_floor, quadratic_out);
   PBB_CUDA(cudaGetLastError());
   return 0;
 }

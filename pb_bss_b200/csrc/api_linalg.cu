@@ -1,11 +1,13 @@
 // C-ABI entry points for the beamforming side: batched small-matrix linear algebra,
 // PSD estimation and beamformer application (see include/pbb.h).
 #include "common.cuh"
+#include <algorithm>
 #include <cstring>
 #include "em_args.cuh"
 #include "heig.cuh"
 #include "linalg_kernels.cuh"
 #include "extraction.cuh"
+#include "distribution.cuh"
 #include "prof.cuh"
 
 namespace pbb {
@@ -486,6 +488,157 @@ int pbb_apply_online_beamforming_vector(const void* vector, const void* mix, int
     apply_online_kernel<float2><<<grid, 128, 0, st>>>(
         reinterpret_cast<const double2*>(vector), reinterpret_cast<const float2*>(mix), B, F, D, T,
         vector_frame_stride, vector_bin_stride, mix_batch_stride, mix_bin_stride, reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- single distributions of pb_bss/distribution (csrc/distribution.cuh) -----------------------------------------
+
+int pbb_cacg_from_covariance(const void* covariance, int n, int D, int covariance_norm, double eigenvalue_floor,
+                             void* eigenvectors, double* eigenvalues, int* status, void* stream) {
+  PBB_CHECK_ARG(covariance != nullptr, 1, "covariance is null");
+  PBB_CHECK_ARG(n > 0, 2, "n must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= kDistMaxD, 3, "need 0 < D <= 64");
+  PBB_CHECK_ARG(covariance_norm >= PBB_NORM_NONE && covariance_norm <= PBB_NORM_TRACE, 4, "bad covariance_norm");
+  PBB_CHECK_ARG(eigenvectors != nullptr && eigenvalues != nullptr, 6, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t per = from_covariance_smem_per_warp(D);
+  const int warps = warps_for(per);
+  if (status) PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  PBB_CUDA(cudaFuncSetAttribute(cacg_from_covariance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  LaunchScope ls("cacg_from_covariance_kernel", st);
+  cacg_from_covariance_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
+      reinterpret_cast<const double2*>(covariance), n, D, covariance_norm, eigenvalue_floor,
+      reinterpret_cast<double2*>(eigenvectors), eigenvalues, status, warps);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_cw_log_norm(const double* kappa, long long n, int D, int variant, double* log_norm, void* stream) {
+  PBB_CHECK_ARG(kappa != nullptr, 1, "kappa is null");
+  PBB_CHECK_ARG(n > 0, 2, "n must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= kDistMaxD, 3, "need 0 < D <= 64");
+  PBB_CHECK_ARG(variant >= PBB_CW_NORM_1F1 && variant <= PBB_CW_NORM_TRAN_VU, 4, "bad variant");
+  PBB_CHECK_ARG(log_norm != nullptr, 5, "log_norm is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("cw_log_norm_kernel", st);
+  cw_log_norm_kernel<<<blocks_for((size_t)n, 256), 256, 0, st>>>(kappa, n, D, variant, log_norm);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_cw_log_pdf(const void* y, int dtype, long long y_stride, int M, int N, int D, const void* mode,
+                   const double* concentration, double* log_pdf, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "bad dtype");
+  PBB_CHECK_ARG(y_stride >= 0, 3, "y_stride must be non-negative");
+  PBB_CHECK_ARG(M > 0 && N > 0 && D > 0 && D <= kDistMaxD, 4, "bad shape");
+  PBB_CHECK_ARG(mode != nullptr && concentration != nullptr, 7, "model is null");
+  PBB_CHECK_ARG(log_pdf != nullptr, 9, "log_pdf is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const dim3 grid(blocks_for((size_t)N, 256), std::min(M, kDistMaxGridY));
+  LaunchScope ls("cw_log_pdf_kernel", st);
+  if (dtype == PBB_C128)
+    cw_log_pdf_kernel<double2><<<grid, 256, 0, st>>>(reinterpret_cast<const double2*>(y), y_stride, M, N, D,
+                                                     reinterpret_cast<const double2*>(mode), concentration, log_pdf);
+  else
+    cw_log_pdf_kernel<float2><<<grid, 256, 0, st>>>(reinterpret_cast<const float2*>(y), y_stride, M, N, D,
+                                                    reinterpret_cast<const double2*>(mode), concentration, log_pdf);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// workspace of pbb_ccsg_log_pdf (LU (M, D, D) | perm (M, D) | logdet (M)) and of pbb_ccsg_sample (L (M, D, D))
+size_t pbb_ccsg_workspace_bytes(int M, int D) {
+  if (M <= 0 || D <= 0 || D > kDistMaxD) return 0;
+  const size_t lu = (size_t)M * D * D * sizeof(double2);
+  const size_t perm = ((size_t)M * D * sizeof(int) + 15) & ~(size_t)15;
+  return lu + perm + (size_t)M * sizeof(double);
+}
+
+int pbb_ccsg_log_pdf(const void* y, int dtype, long long y_stride, int M, int N, int D, const void* covariance,
+                     double* log_pdf, void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "bad dtype");
+  PBB_CHECK_ARG(y_stride >= 0, 3, "y_stride must be non-negative");
+  PBB_CHECK_ARG(M > 0 && N > 0 && D > 0 && D <= kDistMaxD, 4, "bad shape");
+  PBB_CHECK_ARG(covariance != nullptr, 7, "covariance is null");
+  PBB_CHECK_ARG(log_pdf != nullptr, 8, "log_pdf is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_ccsg_workspace_bytes(M, D), 9,
+                "workspace too small (pbb_ccsg_workspace_bytes)");
+  PBB_CHECK_ARG(status != nullptr, 11, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  double2* lu = reinterpret_cast<double2*>(workspace);
+  int* perm = reinterpret_cast<int*>(lu + (size_t)M * D * D);
+  double* logdet = reinterpret_cast<double*>(reinterpret_cast<char*>(perm) +
+                                             (((size_t)M * D * sizeof(int) + 15) & ~(size_t)15));
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  // one factorisation per warp: as many warps per CTA as their shared memory allows (one at D = 64)
+  const size_t lu_per_warp = (size_t)D * D * sizeof(double2) + kDistMaxD * sizeof(int);
+  const int warps = warps_for(lu_per_warp);
+  const size_t lu_smem = (size_t)warps * lu_per_warp;
+  PBB_CUDA(cudaFuncSetAttribute(ccsg_lu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  {
+    LaunchScope ls("ccsg_lu_kernel", st);
+    ccsg_lu_kernel<<<(M + warps - 1) / warps, 32 * warps, lu_smem, st>>>(
+        reinterpret_cast<const double2*>(covariance), M, D, lu, perm, logdet, status, warps);
+    PBB_CUDA(cudaGetLastError());
+  }
+  const size_t smem = ccsg_log_pdf_smem(D);
+  const dim3 grid(blocks_for((size_t)N, kCcsgThreads), std::min(M, kDistMaxGridY));
+  LaunchScope ls("ccsg_log_pdf_kernel", st);
+  if (dtype == PBB_C128) {
+    PBB_CUDA(cudaFuncSetAttribute(ccsg_log_pdf_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    ccsg_log_pdf_kernel<double2><<<grid, kCcsgThreads, smem, st>>>(reinterpret_cast<const double2*>(y), y_stride, M,
+                                                                   N, D, lu, perm, logdet, log_pdf);
+  } else {
+    PBB_CUDA(cudaFuncSetAttribute(ccsg_log_pdf_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    ccsg_log_pdf_kernel<float2><<<grid, kCcsgThreads, smem, st>>>(reinterpret_cast<const float2*>(y), y_stride, M,
+                                                                  N, D, lu, perm, logdet, log_pdf);
+  }
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_ccsg_sample(const void* a, const double* eigenvalues, int C, int D, const double* normals,
+                    const long long* offsets, const long long* dest, long long S, int unit_norm, void* out,
+                    void* workspace, size_t workspace_bytes, int* status, void* stream) {
+  PBB_CHECK_ARG(a != nullptr, 1, "covariance / eigenvectors are null");
+  PBB_CHECK_ARG(C > 0 && D > 0 && D <= kDistMaxD, 3, "bad shape");
+  PBB_CHECK_ARG(S >= 0, 8, "S must be non-negative");
+  PBB_CHECK_ARG(S == 0 || (normals != nullptr && offsets != nullptr && out != nullptr), 5, "samples are null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_ccsg_workspace_bytes(C, D), 11,
+                "workspace too small (pbb_ccsg_workspace_bytes)");
+  PBB_CHECK_ARG(status != nullptr, 13, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  double2* L = reinterpret_cast<double2*>(workspace);
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  const size_t chol_per_warp = (size_t)D * D * sizeof(double2);
+  const int warps = warps_for(chol_per_warp);
+  {
+    LaunchScope ls("ccsg_cholesky_kernel", st);
+    PBB_CUDA(cudaFuncSetAttribute(ccsg_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    ccsg_cholesky_kernel<<<(C + warps - 1) / warps, 32 * warps, (size_t)warps * chol_per_warp, st>>>(
+        reinterpret_cast<const double2*>(a), eigenvalues, C, D, L, status, warps);
+    PBB_CUDA(cudaGetLastError());
+  }
+  if (S == 0) return 0;
+  LaunchScope ls("ccsg_sample_kernel", st);
+  ccsg_sample_kernel<<<blocks_for((size_t)S, 128), 128, 0, st>>>(L, C, D, normals, offsets, dest, S, unit_norm,
+                                                                reinterpret_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_ccsg_fit(const void* observation, int dtype, int F, int D, int N, const double* saliency,
+                 double denominator_floor, void* covariance, void* workspace, size_t workspace_bytes, void* stream) {
+  int r = pbb_power_spectral_density(observation, dtype, F, D, N, saliency, 1, 0, covariance, workspace,
+                                     workspace_bytes, stream);
+  if (r || saliency == nullptr) return r;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("ccsg_fit_scale_kernel", st);
+  ccsg_fit_scale_kernel<<<F, 256, 0, st>>>(saliency, N, D, denominator_floor,
+                                           reinterpret_cast<double2*>(covariance));
   PBB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -693,30 +693,6 @@ __device__ inline double cw_spline_eval(const CwSpline& sp, double x) {
   return (1.0 - a2) * d1 + a2 * d2;
 }
 
-// log( 1F1(1; D; kappa) * 2 pi^D / (D-1)! )  (complex_watson.py:157-168).  Series
-// for small kappa, Mardia's closed form (complex_watson.py:109-138) otherwise.
-__device__ inline double cw_log_norm(double kappa, int D) {
-  double lfact = 0.0;
-  for (int r = 2; r < D; ++r) lfact += log((double)r);
-  const double base = log(2.0) + (double)D * log(3.14159265358979323846) - lfact;
-  if (kappa < 20.0) {
-    double s = 1.0, term = 1.0;
-    for (int n = 1; n < 400; ++n) {
-      term *= kappa / (double)(D + n - 1);
-      s += term;
-      if (term < 1e-17 * s) break;
-    }
-    return base + log(s);
-  }
-  double part = 0.0, pw = 1.0, fr = 1.0;  // sum_{r=0}^{D-2} kappa^r / r!
-  for (int r = 0; r <= D - 2; ++r) {
-    if (r > 0) { pw *= kappa; fr *= (double)r; }
-    part += pw / fr;
-  }
-  return log(2.0) + (double)D * log(3.14159265358979323846) + (1.0 - (double)D) * log(kappa) + kappa +
-         log1p(-exp(-kappa) * part);
-}
-
 struct CwUpdArgs {
   int F, T, D, K;
   int nch;

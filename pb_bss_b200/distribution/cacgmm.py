@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from .. import _device, _lib
+from . import complex_circular_symmetric_gaussian as _ccsg
 from .complex_angular_central_gaussian import (
     ComplexAngularCentralGaussian,
     normalize_observation,
@@ -21,10 +22,37 @@ from .mixture_model_utils import (check_initialization, coupled_fit, fit_tied_le
                                   weight_to_host)
 from .utils import _ProbabilisticModel
 
-__all__ = ['CACGMM', 'CACGMMTrainer', 'normalize_observation']
+__all__ = ['CACGMM', 'CACGMMTrainer', 'sample_cacgmm', 'normalize_observation']
 
 _NORMS = {'eigenvalue': _lib.NORM_EIGENVALUE, 'trace': _lib.NORM_TRACE,
           False: _lib.NORM_NONE}
+
+
+def sample_cacgmm(size, weight, covariance, return_label=False):
+    """``size`` samples (size, D) of a cACGMM (cacgmm.py:27-55): labels from ``np.random.choice(range(K), size,
+    p=weight)``, then, class by class, ``from_covariance(covariance[l]).sample((count_l,))`` -- the same draws from
+    NumPy's global stream in the same order, so the result equals that loop exactly.  The K models come from one
+    ``pbb_cacg_from_covariance`` and all samples from one ``pbb_ccsg_sample`` launch.  The argument checks are
+    assertions, as in the reference."""
+    assert weight.ndim == 1, weight
+    assert isinstance(size, int), size
+    assert covariance.ndim == 3, covariance.shape
+    num_classes, = weight.shape
+    D = covariance.shape[-1]
+    assert tuple(covariance.shape) == (num_classes, D, D), (covariance.shape, num_classes, D)
+    p = weight.cpu().numpy() if _device.is_tensor(weight) else weight
+    labels = np.random.choice(range(num_classes), size=size, p=p)
+    model = ComplexAngularCentralGaussian.from_covariance(_device.to_device(covariance, torch.complex128))
+    draws, dest = [], []
+    for k in range(num_classes):
+        rows = np.flatnonzero(labels == k)
+        draws.append((np.random.normal(size=(rows.size, D)), np.random.normal(size=(rows.size, D))))
+        dest.append(rows)
+    x = _ccsg.sample_classes(model.covariance_eigenvectors, model.covariance_eigenvalues, draws, True,
+                             not _device.is_tensor(covariance), dest=np.concatenate(dest))
+    if return_label:
+        return x, labels
+    return x
 
 
 @dataclass
