@@ -118,7 +118,7 @@ static CacgmmWorkspace carve(void* base, int F, int T, int D, int K) {
   const int zs = (T + 31) / 32 * 32;
   const size_t nchunks = ((size_t)zs + kStageFrames - 1) / kStageFrames;
   const size_t z_plain = (size_t)F * D * zs * sizeof(double2);
-  const size_t z_staged = (size_t)F * nchunks * stage_rows(D % 2 == 0 ? D : D + 1) * kStageFrames * sizeof(double2);
+  const size_t z_staged = (size_t)F * nchunks * D * kStageFrames * sizeof(double2);
   const size_t o_phase = align_up((size_t)(F + 1) * sizeof(int), 8);
   ws.control_bytes = o_phase + kPhaseWords * sizeof(unsigned long long) + 2 * sizeof(int);
   const size_t o_z = take(z_plain > z_staged ? z_plain : z_staged);
@@ -341,14 +341,13 @@ static int normalize(const void* y, int dtype, const CacgmmWorkspace& ws, int F,
     if (!staged) return launch_normalize(src, dst, F, T, D, 1, ws.zs, st);
     const int block = 64;  // divides kStageFrames
     const int nchunks = (ws.zs + kStageFrames - 1) / kStageFrames;
-    const size_t bin_elems = (size_t)nchunks * stage_rows(D) * kStageFrames;  // out[f][c][r][i]
+    const size_t bin_elems = (size_t)nchunks * D * kStageFrames;  // out[f][c][d][i]
     for (int f0 = 0; f0 < F; f0 += kNormMaxGridY) {
       const int nf = std::min(F - f0, kNormMaxGridY);
       if (int r = launch_kernel("normalize_staged_kernel", normalize_staged_kernel<CT>,
                                 dim3(nchunks * (kStageFrames / block), nf), block,
                                 (size_t)block * (D + 1) * sizeof(double2), st, src + (size_t)f0 * T * D,
-                                dst + (size_t)f0 * bin_elems, nf, T, D, stage_rows(D), kStageFrames, nchunks,
-                                ws.dead + f0))
+                                dst + (size_t)f0 * bin_elems, nf, T, D, kStageFrames, nchunks, ws.dead + f0))
         return r;
     }
     return 0;
@@ -605,8 +604,7 @@ static int launch_stream_load(const void* y, int dtype, const CacgmmWorkspace& w
     using CT = decltype(ct);
     return launch_kernel("stream_load_kernel", stream_load_kernel<CT>, ctas, kLoadThreads, smem, st,
                          static_cast<const CT*>(y), static_cast<CT*>(ws.z), aff_src, aff_dst, F, T, D, K,
-                         stage_rows(D), kStageFrames, nchunks, ws.dead, ws.flags, ws.load_next_bin,
-                         ws.load_started);
+                         kStageFrames, nchunks, ws.dead, ws.flags, ws.load_next_bin, ws.load_started);
   });
 }
 

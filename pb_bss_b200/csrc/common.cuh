@@ -91,10 +91,13 @@ __host__ __device__ constexpr GroupShape group_shape(int D) {
   const int half = (M % 2 == 0) ? 1 : 0;
   return {M, nfull, half, 2 + 2 * nfull + 2 * half, 4 + 8 * nfull + 4 * half};
 }
-// Row layout of the staged observation: rows 0..D-1 are the channels; the rows
-// after that repeat the first channels (pair-swapped when M is even) so that
-// group g finds its NLOC local channels in the CONSECUTIVE rows 2g .. 2g+NLOC-1
-// -- one base address plus compile-time offsets for every group.
+// Row layout of a ring stage of the observation in shared memory: rows 0..D-1
+// are the channels; the rows after that repeat the first channels (pair-swapped
+// when M is even) so that group g finds its NLOC local channels in the
+// CONSECUTIVE rows 2g .. 2g+NLOC-1 -- one base address plus compile-time
+// offsets for every group.  The repeated rows exist on chip only: global memory
+// holds the D channel rows, and stage_g2s (em_persistent.cuh) copies the
+// repeated ones from there.
 //   D=8: rows = 0 1 2 3 4 5 6 7 | 1 0 3 2      D=6: 0..5 | 0 1      D=4: 0..3 | 1 0
 __host__ __device__ constexpr int stage_rows(int D) {
   const GroupShape gs = group_shape(D);

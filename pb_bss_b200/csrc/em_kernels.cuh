@@ -885,13 +885,14 @@ __global__ void normalize_kernel(const CT* __restrict__ y, CT* __restrict__ z, i
   }
 }
 
-// Staged layout of the persistent kernels (one ring stage = one contiguous block):
-//   out[f][c][r][i] = z[f][row_channel(D, r)][c * SF + i], rows = stage_rows(D); frames >= T are zero.
+// Staged layout of the persistent kernels (the channel rows of one ring stage = one contiguous block):
+//   out[f][c][d][i] = z[f][d][c * SF + i]; frames >= T are zero.  The repeated rows of a stage (common.cuh) are
+//   added in shared memory only (stage_g2s, em_persistent.cuh).
 
 // Normalisation into the staged layout.  One CTA per (frame tile, bin).
 template <typename CT>
-__global__ void normalize_staged_kernel(const CT* __restrict__ y, CT* __restrict__ z, int F, int T, int D, int rows,
-                                        int SF, int nchunks, int* __restrict__ dead) {
+__global__ void normalize_staged_kernel(const CT* __restrict__ y, CT* __restrict__ z, int F, int T, int D, int SF,
+                                        int nchunks, int* __restrict__ dead) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* tile = reinterpret_cast<double2*>(smem_raw);  // [blockDim.x][D + 1]
   const int f = blockIdx.y;
@@ -924,14 +925,14 @@ __global__ void normalize_staged_kernel(const CT* __restrict__ y, CT* __restrict
   }
   __syncthreads();
   const int c = t0 / SF, i0 = t0 - c * SF;
-  CT* __restrict__ zc = z + ((size_t)f * nchunks + c) * rows * SF;
-  for (int i = threadIdx.x; i < rows * (int)blockDim.x; i += blockDim.x) {
+  CT* __restrict__ zc = z + ((size_t)f * nchunks + c) * D * SF;
+  for (int i = threadIdx.x; i < D * (int)blockDim.x; i += blockDim.x) {
     // consecutive threads write consecutive addresses
-    const int r = i / (int)blockDim.x;
-    const int tt = i - r * (int)blockDim.x;
+    const int d = i / (int)blockDim.x;
+    const int tt = i - d * (int)blockDim.x;
     double2 v = make_double2(0.0, 0.0);
-    if (tt < nt) v = tile[tt * ldt + row_channel(D, r)];
-    st_cplx(zc + r * SF + i0 + tt, v.x, v.y);
+    if (tt < nt) v = tile[tt * ldt + d];
+    st_cplx(zc + d * SF + i0 + tt, v.x, v.y);
   }
 }
 
@@ -950,7 +951,7 @@ constexpr int kLoadBatch = 8;  // 16-byte loads per thread and batch: 16 KB per 
 template <typename CT>
 __global__ void __launch_bounds__(kLoadThreads, 3)
 stream_load_kernel(const CT* __restrict__ y, CT* __restrict__ z, const double* __restrict__ aff_src,
-                   double* __restrict__ aff_dst, int F, int T, int D, int K, int rows, int SF, int nchunks,
+                   double* __restrict__ aff_dst, int F, int T, int D, int K, int SF, int nchunks,
                    int* __restrict__ dead, int* __restrict__ flags, int* __restrict__ next_bin,
                    int* __restrict__ started) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1028,16 +1029,15 @@ stream_load_kernel(const CT* __restrict__ y, CT* __restrict__ z, const double* _
         }
       }
       __syncthreads();
-      CT* __restrict__ zc = z + ((size_t)f * nchunks + c) * rows * SF;
+      CT* __restrict__ zc = z + ((size_t)f * nchunks + c) * D * SF;
       // (rolled loops: with the next chunk's loads in flight, an unrolled store loop spills at 168 registers)
 #pragma unroll 1
-      for (int r = 0; r < rows; ++r) {
-        const int ch = row_channel(D, r);
+      for (int d = 0; d < D; ++d) {
 #pragma unroll 1
         for (int tt = tid; tt < SF; tt += kLoadThreads) {
           double2 x = make_double2(0.0, 0.0);
-          if (tt < nt) x = tile[tt * ldt + ch];
-          st_cplx(zc + r * SF + tt, x.x, x.y);
+          if (tt < nt) x = tile[tt * ldt + d];
+          st_cplx(zc + d * SF + tt, x.x, x.y);
         }
       }
       __syncthreads();

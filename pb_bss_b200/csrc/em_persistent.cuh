@@ -42,8 +42,8 @@ namespace pbb {
 #endif
 
 struct PersistArgs {
-  const void* z;   // staged layout (F, nchunks, ROWS, kStageFrames): every ring stage is one
-                   // contiguous block (channels + repeated rows, zero padded), see normalize_staged_kernel
+  const void* z;   // staged layout (F, nchunks, D, kStageFrames): the channel rows of a ring stage are one
+                   // contiguous block (zero padded), see normalize_staged_kernel and stage_g2s
   int zs;          // padded frame count, multiple of 32
   int F, T;
   int iterations;  // EM iterations in this launch
@@ -107,6 +107,26 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+
+constexpr int kStageFrames = 128;  // frames per ring stage (4 steps of 32)
+
+// One ring stage of the staged observation into shared memory, all copies completing on `bar` (armed here for the
+// whole stage).  Global memory holds the D channel rows of each (bin, chunk) only, so that the observation the fit
+// re-reads every iteration stays small enough for L2; the stage in shared memory has stage_rows(D) rows.  One bulk
+// copy brings the channel rows, then one per repeated row (common.cuh) copies its channel row again -- from the L2
+// lines the first copy has just brought in.
+template <int D, typename CT>
+__device__ __forceinline__ void stage_g2s(CT (*dst)[kStageFrames], const CT* z, int bin, int nchunks, int chunk,
+                                          uint64_t* bar) {
+  constexpr int ROWS = stage_rows(D);
+  constexpr uint32_t kRowBytes = kStageFrames * sizeof(CT);
+  const CT* src = z + ((size_t)bin * nchunks + chunk) * (D * kStageFrames);
+  mbar_expect_tx(bar, ROWS * kRowBytes);
+  bulk_g2s(dst[0], src, D * kRowBytes, bar);
+#pragma unroll
+  for (int r = D; r < ROWS; ++r) bulk_g2s(dst[r], src + row_channel(D, r) * kStageFrames, kRowBytes, bar);
+}
+
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
   asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -166,7 +186,6 @@ __device__ __forceinline__ double2 lds_cplx(const float2* p) {
   return make_double2((double)v.x, (double)v.y);
 }
 
-constexpr int kStageFrames = 128;  // frames per ring stage (4 steps of 32)
 constexpr int kStages = 2;
 
 template <int D, int K, typename CT>
@@ -879,15 +898,11 @@ em_persistent_kernel(const PersistArgs a) {
   }
   unsigned chunk_cnt = 0;  // chunks consumed so far by this CTA (ring position)
 
-  // One 1-D TMA bulk copy per ring stage: the staged layout keeps the ROWS x kStageFrames block
-  // of a (bin, chunk) contiguous, so a single elected lane issues a single UBLKCP.
-  constexpr uint32_t kStageBytes = (uint32_t)(SM::ROWS * kStageFrames * sizeof(CT));
+  // 1-D TMA bulk copies per ring stage (stage_g2s), issued by a single elected lane.
   auto issue_chunk = [&](int bin, int c, unsigned n) {  // warp 0
     if (lane == 0) {
       const int st = n & 1u;
-      mbar_expect_tx(&sm.full[st], kStageBytes);
-      bulk_g2s(&sm.zbuf[st][0][0], zbase + ((size_t)bin * nchunks + c) * (SM::ROWS * kStageFrames), kStageBytes,
-               &sm.full[st]);
+      stage_g2s<D>(sm.zbuf[st], zbase, bin, nchunks, c, &sm.full[st]);
     }
   };
   // streamed upload: a bin's observation may not have arrived yet; its first task issues its own

@@ -6,7 +6,7 @@
 // H100 -- is all there is, and most SMs idle.  Here a cluster of S = 1, 2 or 4 CTAs keeps ONE bin from the first to
 // the last iteration:
 //   * CTA p of the cluster holds the ring stages [p n / S, (p + 1) n / S) of the bin's staged observation in shared
-//     memory for the whole fit (at most kWsStages of them: one TMA bulk copy each, at the start);
+//     memory for the whole fit (at most kWsStages of them, copied in once at the start by stage_g2s);
 //   * per iteration its four EM warps sweep those frames (the hot loop of em_ws_kernel, unchanged) and leave the
 //     scatter sums in shared memory -> cluster barrier -> the update warps of CTA 0 add the S partial sums in rank
 //     order through DSMEM (bit-reproducible), update the model (cacg_update_class, unchanged) and store it into
@@ -48,7 +48,6 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
   const int T = a.T, zs = a.zs;
   const int nchunks = (zs + kStageFrames - 1) / kStageFrames;
   const int c0 = part * nchunks / S, c1 = (part + 1) * nchunks / S;  // this CTA's ring stages (c1 - c0 <= kWsStages)
-  constexpr uint32_t kStageBytes = (uint32_t)(SM::ROWS * kStageFrames * sizeof(CT));
 
   for (int s = tid; s < NS; s += blockDim.x) sm.tab[s] = slot_pack(D, s);
   if (tid == 0) {
@@ -59,11 +58,7 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
   if (tid == 0) {
     // the part's observation: resident for the whole fit
     const CT* __restrict__ zbase = reinterpret_cast<const CT*>(a.z);
-    for (int c = c0; c < c1; ++c) {
-      mbar_expect_tx(&sm.full[c - c0], kStageBytes);
-      bulk_g2s(&sm.zbuf[c - c0][0][0], zbase + ((size_t)bin * nchunks + c) * (SM::ROWS * kStageFrames), kStageBytes,
-               &sm.full[c - c0]);
-    }
+    for (int c = c0; c < c1; ++c) stage_g2s<D>(sm.zbuf[c - c0], zbase, bin, nchunks, c, &sm.full[c - c0]);
   }
 
   if (warp < M) {

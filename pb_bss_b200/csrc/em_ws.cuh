@@ -98,7 +98,6 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
   const int nchunks = (zs + kStageFrames - 1) / kStageFrames;
   const int S = a.tsplit > 1 ? a.tsplit : 1;  // parts per (bin, iteration); the host keeps S <= nchunks
   const int total = a.iterations * F * S;
-  constexpr uint32_t kStageBytes = (uint32_t)(SM::ROWS * kStageFrames * sizeof(CT));
 
   for (int s = tid; s < NS; s += blockDim.x) sm.tab[s] = slot_pack(D, s);
   if (tid == 0) {
@@ -268,9 +267,7 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
                   : "memory");
               if (!done) break;
             }
-            mbar_expect_tx(&sm.full[st], kStageBytes);
-            bulk_g2s(&sm.zbuf[st][0][0], zbase + ((size_t)bin * nchunks + c0 + issued) * (SM::ROWS * kStageFrames),
-                     kStageBytes, &sm.full[st]);
+            stage_g2s<D>(sm.zbuf[st], zbase, bin, nchunks, c0 + issued, &sm.full[st]);
             ++chunk_cnt;
             ++issued;
           }
