@@ -648,17 +648,17 @@ static int launch_persist(const PersistArgs& a, int D, int K, int dtype, Persist
     int* c = &cache[(int)v];
     // the full variant's launches carry their own name, so that profiles and tests can tell it from the lean one
     if (v == Persist::kFull)
-      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, true, 1>, threads, smem, c, a,
+      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, true>, threads, smem, c, a,
                                        "em_persistent_kernel_full", st);
     if (v == Persist::kCw)
-      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 2, 1>, threads, smem, c, a,
+      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 1>, threads, smem, c, a,
                                        "em_persistent_kernel_cw", st);
     if constexpr (Dc == 8) {
       if (v == Persist::kWs)
         return launch_persistent_generic(em_ws_kernel<Kc, CT>, 256, sizeof(WsSmem<Dc, Kc, CT>), c, a, "em_ws_kernel",
                                          st);
     }
-    return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 2>, threads, smem,
+    return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false>, threads, smem,
                                      &cache[(int)Persist::kLean], a, "em_persistent_kernel", st);
   });
 }

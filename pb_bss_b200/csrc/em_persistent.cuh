@@ -179,6 +179,21 @@ __device__ __forceinline__ void decode_ticket(int t, int F, int I, int c, int& b
   bin = (int)(first < F ? first : F) + (int)(t - wave_prefix(lo, F, I, c));
   it = lo - bin / c;
 }
+// Task of ticket t: S consecutive tickets per (bin, iteration) (frame split), part = t mod S.  With the explicit order
+// table, ord = order_entry(a, t, S) = bin | iteration << 16 (loaded by the caller, which may issue it early).
+__device__ __forceinline__ int order_entry(const PersistArgs& a, int t, int S) {
+  return a.order != nullptr ? __ldcg(a.order + t / S) : 0;
+}
+__device__ __forceinline__ void decode_task(const PersistArgs& a, int t, int S, int ord, int& bin, int& it, int& part) {
+  const int tt = t / S;
+  part = t - tt * S;
+  if (a.order != nullptr) {
+    bin = ord & 0xffff;
+    it = ord >> 16;
+  } else {
+    decode_ticket(tt, a.F, a.iterations, a.wave_c, bin, it);
+  }
+}
 
 __device__ __forceinline__ double2 lds_cplx(const double2* p) { return *p; }
 __device__ __forceinline__ double2 lds_cplx(const float2* p) {
@@ -333,61 +348,78 @@ __device__ __forceinline__ void em_exchange_barrier() {
   else __syncthreads();
 }
 
-template <int D, int K, typename CT, int MODEL, bool NAMED = false, typename SMT>
-__device__ __forceinline__ void lean_chunk(SMT& sm, int cb, int g, int st, int nsteps, int lane,
-                                           int& buf, double eps, double (&acc)[K * GroupDims<D>::NSG],
-                                           double (&sg)[K], int j0 = 0) {
+// Front half of a lean step for FR = 1 or 2 frames per lane (frames zrow, zrow + 32): z loads -> psi slots ->
+// this group's share of the K quadratic forms, 2K independent FMA chains per frame (coefficients cg, broadcast from
+// shared memory) -> partial forms of frame f, class k stored at xw[(f K + k) 32].  The psi slots stay with the caller
+// for the M-step.
+template <int D, int K, int FR, typename CT>
+__device__ __forceinline__ void lean_partial_forms(const CT* __restrict__ zrow, const double* __restrict__ cg,
+                                                   double* __restrict__ xw, double (&psi)[FR][GroupDims<D>::NSG]) {
   using G = GroupDims<D>;
-  constexpr int NSG = G::NSG, NLOC = G::NLOC, M = G::M, NS = G::NS;
-  const CT* __restrict__ zrow = &sm.zbuf[st][2 * g][0] + lane + 32 * j0;
-  const double* __restrict__ cg = &sm.coef[cb][0][g * NSG];
-#pragma unroll 1
-  for (int j = 0; j < nsteps; ++j, zrow += 32) {
+  constexpr int NSG = G::NSG, NLOC = G::NLOC, NS = G::NS;
+  {
     double2 x[NLOC];
 #pragma unroll
-    for (int l = 0; l < NLOC; ++l) x[l] = lds_cplx(zrow + l * kStageFrames);
-    double psi[NSG];
-    group_psi<D>(x, psi);
-    // this group's share of the K quadratic forms: 2K independent FMA chains
-    double p0[K], p1[K];
+    for (int f = 0; f < FR; ++f) {
 #pragma unroll
-    for (int k = 0; k < K; ++k) { p0[k] = 0.0; p1[k] = 0.0; }
-#pragma unroll
-    for (int i = 0; i < NSG; i += 2) {
-#pragma unroll
-      for (int k = 0; k < K; ++k) {
-        const double2 cc = *reinterpret_cast<const double2*>(cg + k * NS + i);
-        p0[k] = fma(cc.x, psi[i], p0[k]);
-        p1[k] = fma(cc.y, psi[i + 1], p1[k]);
-      }
+      for (int l = 0; l < NLOC; ++l) x[l] = lds_cplx(zrow + l * kStageFrames + 32 * f);
+      group_psi<D>(x, psi[f]);
     }
-    double* __restrict__ xw = &sm.xq[buf][g][0][lane];
+  }
+  double p0[FR][K], p1[FR][K];
 #pragma unroll
-    for (int k = 0; k < K; ++k) xw[k * 32] = p0[k] + p1[k];
-    em_exchange_barrier<D, NAMED>();
-    const double* __restrict__ xr = &sm.xq[buf][0][0][lane];
-    double q[K];
+  for (int k = 0; k < K; ++k)
+#pragma unroll
+    for (int f = 0; f < FR; ++f) { p0[f][k] = 0.0; p1[f][k] = 0.0; }
+#pragma unroll
+  for (int i = 0; i < NSG; i += 2) {
 #pragma unroll
     for (int k = 0; k < K; ++k) {
-      double v = xr[k * 32];
+      const double2 cc = *reinterpret_cast<const double2*>(cg + k * NS + i);
 #pragma unroll
-      for (int gg = 1; gg < M; ++gg) v += xr[(gg * 2 * K + k) * 32];
-      q[k] = fabs(v);
+      for (int f = 0; f < FR; ++f) p0[f][k] = fma(cc.x, psi[f][i], p0[f][k]);
+#pragma unroll
+      for (int f = 0; f < FR; ++f) p1[f][k] = fma(cc.y, psi[f][i + 1], p1[f][k]);
     }
-    buf ^= 1;
-    double gam[K], cw[K];
-    if constexpr (MODEL == 1) softmax_watson<K>(q, sm.ew[cb], sm.ld, sm.w, gam, cw);
-    else softmax_product<D, K>(q, sm.ew[cb], eps, gam, cw);
+  }
 #pragma unroll
-    for (int k = 0; k < K; ++k) {
-      sg[k] += gam[k];
+  for (int k = 0; k < K; ++k)
 #pragma unroll
-      for (int i = 0; i < NSG; ++i) acc[k * NSG + i] = fma(cw[k], psi[i], acc[k * NSG + i]);
-    }
+    for (int f = 0; f < FR; ++f) xw[(f * K + k) * 32] = p0[f][k] + p1[f][k];
+}
+
+// One lean step with one frame per lane (frame 32 j + lane of the stage): the odd tail step of a short last chunk.
+template <int D, int K, typename CT, int MODEL, bool NAMED = false, typename SMT>
+__device__ __forceinline__ void lean_step(SMT& sm, int cb, int g, int st, int j, int lane, int& buf, double eps,
+                                          double (&acc)[K * GroupDims<D>::NSG], double (&sg)[K]) {
+  using G = GroupDims<D>;
+  constexpr int NSG = G::NSG, M = G::M;
+  double psi[1][NSG];
+  lean_partial_forms<D, K, 1, CT>(&sm.zbuf[st][2 * g][0] + lane + 32 * j, &sm.coef[cb][0][g * NSG],
+                                  &sm.xq[buf][g][0][lane], psi);
+  em_exchange_barrier<D, NAMED>();
+  const double* __restrict__ xr = &sm.xq[buf][0][0][lane];
+  double q[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double v = xr[k * 32];
+#pragma unroll
+    for (int gg = 1; gg < M; ++gg) v += xr[(gg * 2 * K + k) * 32];
+    q[k] = fabs(v);
+  }
+  buf ^= 1;
+  double gam[K], cw[K];
+  if constexpr (MODEL == 1) softmax_watson<K>(q, sm.ew[cb], sm.ld, sm.w, gam, cw);
+  else softmax_product<D, K>(q, sm.ew[cb], eps, gam, cw);
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    sg[k] += gam[k];
+#pragma unroll
+    for (int i = 0; i < NSG; ++i) acc[k * NSG + i] = fma(cw[k], psi[0][i], acc[k * NSG + i]);
   }
 }
 
-// Same as lean_chunk with TWO frames per lane and step (frames t and t + 32):
+// The lean step loop with TWO frames per lane and step (frames t and t + 32):
 // the coefficient loads, the barrier and the loop overhead are shared by the two
 // frames, and their E-step / softmax dependency chains interleave, which is what
 // keeps the fp64 pipe busy with only two warps per scheduler.
@@ -396,41 +428,13 @@ __device__ __forceinline__ void lean_chunk2(SMT& sm, int cb, int g, int st, int 
                                             int& buf, double eps, double (&acc)[K * GroupDims<D>::NSG],
                                             double (&sg)[K]) {
   using G = GroupDims<D>;
-  constexpr int NSG = G::NSG, NLOC = G::NLOC, M = G::M, NS = G::NS;
+  constexpr int NSG = G::NSG, M = G::M;
   const CT* __restrict__ zrow = &sm.zbuf[st][2 * g][0] + lane;
   const double* __restrict__ cg = &sm.coef[cb][0][g * NSG];
 #pragma unroll 1
   for (int j = 0; j < nsteps2; ++j, zrow += 64) {
-    double psiA[NSG], psiB[NSG];
-    {
-      double2 x[NLOC];
-#pragma unroll
-      for (int l = 0; l < NLOC; ++l) x[l] = lds_cplx(zrow + l * kStageFrames);
-      group_psi<D>(x, psiA);
-#pragma unroll
-      for (int l = 0; l < NLOC; ++l) x[l] = lds_cplx(zrow + l * kStageFrames + 32);
-      group_psi<D>(x, psiB);
-    }
-    double pA0[K], pA1[K], pB0[K], pB1[K];
-#pragma unroll
-    for (int k = 0; k < K; ++k) { pA0[k] = 0.0; pA1[k] = 0.0; pB0[k] = 0.0; pB1[k] = 0.0; }
-#pragma unroll
-    for (int i = 0; i < NSG; i += 2) {
-#pragma unroll
-      for (int k = 0; k < K; ++k) {
-        const double2 cc = *reinterpret_cast<const double2*>(cg + k * NS + i);
-        pA0[k] = fma(cc.x, psiA[i], pA0[k]);
-        pB0[k] = fma(cc.x, psiB[i], pB0[k]);
-        pA1[k] = fma(cc.y, psiA[i + 1], pA1[k]);
-        pB1[k] = fma(cc.y, psiB[i + 1], pB1[k]);
-      }
-    }
-    double* __restrict__ xw = &sm.xq[buf][g][0][lane];
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-      xw[k * 32] = pA0[k] + pA1[k];
-      xw[(K + k) * 32] = pB0[k] + pB1[k];
-    }
+    double psi[2][NSG];
+    lean_partial_forms<D, K, 2, CT>(zrow, cg, &sm.xq[buf][g][0][lane], psi);
     em_exchange_barrier<D, NAMED>();
     const double* __restrict__ xr = &sm.xq[buf][0][0][lane];
     double qA[K], qB[K];
@@ -459,8 +463,8 @@ __device__ __forceinline__ void lean_chunk2(SMT& sm, int cb, int g, int st, int 
       sg[k] += gA[k] + gB[k];
 #pragma unroll
       for (int i = 0; i < NSG; ++i) {
-        acc[k * NSG + i] = fma(cA[k], psiA[i], acc[k * NSG + i]);
-        acc[k * NSG + i] = fma(cB[k], psiB[i], acc[k * NSG + i]);
+        acc[k * NSG + i] = fma(cA[k], psi[0][i], acc[k * NSG + i]);
+        acc[k * NSG + i] = fma(cB[k], psi[1][i], acc[k * NSG + i]);
       }
     }
   }
@@ -477,7 +481,7 @@ template <int D, int K, typename CT, typename SMT>
 __device__ __forceinline__ void lean_chunk2_split(SMT& sm, int cb, int g, int st, int nsteps2, int lane, double eps,
                                                   double (&acc)[K * GroupDims<D>::NSG], double (&sg)[K]) {
   using G = GroupDims<D>;
-  constexpr int NSG = G::NSG, NLOC = G::NLOC, M = G::M, NS = G::NS;
+  constexpr int NSG = G::NSG, M = G::M;
   static_assert(M == 4, "frame split assumes four slot-group warps");
   const CT* __restrict__ zrow = &sm.zbuf[st][2 * g][0] + lane;
   const double* __restrict__ cg = &sm.coef[cb][0][g * NSG];
@@ -485,36 +489,8 @@ __device__ __forceinline__ void lean_chunk2_split(SMT& sm, int cb, int g, int st
   const int fhalf = fsel >> 5, fl = fsel & 31;   // its half (A / B) and lane
 #pragma unroll 1
   for (int j = 0; j < nsteps2; ++j, zrow += 64) {
-    double psiA[NSG], psiB[NSG];
-    {
-      double2 x[NLOC];
-#pragma unroll
-      for (int l = 0; l < NLOC; ++l) x[l] = lds_cplx(zrow + l * kStageFrames);
-      group_psi<D>(x, psiA);
-#pragma unroll
-      for (int l = 0; l < NLOC; ++l) x[l] = lds_cplx(zrow + l * kStageFrames + 32);
-      group_psi<D>(x, psiB);
-    }
-    double pA0[K], pA1[K], pB0[K], pB1[K];
-#pragma unroll
-    for (int k = 0; k < K; ++k) { pA0[k] = 0.0; pA1[k] = 0.0; pB0[k] = 0.0; pB1[k] = 0.0; }
-#pragma unroll
-    for (int i = 0; i < NSG; i += 2) {
-#pragma unroll
-      for (int k = 0; k < K; ++k) {
-        const double2 cc = *reinterpret_cast<const double2*>(cg + k * NS + i);
-        pA0[k] = fma(cc.x, psiA[i], pA0[k]);
-        pB0[k] = fma(cc.x, psiB[i], pB0[k]);
-        pA1[k] = fma(cc.y, psiA[i + 1], pA1[k]);
-        pB1[k] = fma(cc.y, psiB[i + 1], pB1[k]);
-      }
-    }
-    double* __restrict__ xw = &sm.xq[0][g][0][lane];
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-      xw[k * 32] = pA0[k] + pA1[k];
-      xw[(K + k) * 32] = pB0[k] + pB1[k];
-    }
+    double psi[2][NSG];
+    lean_partial_forms<D, K, 2, CT>(zrow, cg, &sm.xq[0][g][0][lane], psi);
     em_exchange_barrier<D, true>();
     {
       const double* __restrict__ xr = &sm.xq[0][0][fhalf * K][fl];
@@ -546,9 +522,9 @@ __device__ __forceinline__ void lean_chunk2_split(SMT& sm, int cb, int g, int st
 #pragma unroll
     for (int k = 0; k < K; ++k) {
 #pragma unroll
-      for (int i = 0; i < NSG; ++i) acc[k * NSG + i] = fma(cA[k], psiA[i], acc[k * NSG + i]);
+      for (int i = 0; i < NSG; ++i) acc[k * NSG + i] = fma(cA[k], psi[0][i], acc[k * NSG + i]);
 #pragma unroll
-      for (int i = 0; i < NSG; ++i) acc[k * NSG + i] = fma(cB[k], psiB[i], acc[k * NSG + i]);
+      for (int i = 0; i < NSG; ++i) acc[k * NSG + i] = fma(cB[k], psi[1][i], acc[k * NSG + i]);
     }
   }
 }
@@ -841,6 +817,66 @@ __device__ __forceinline__ void cacg_update_class(const PersistArgs& a, int bin,
     PBB_PHU(11);  // coefficient stores
 }
 
+// E-step weight of class k of the lean model from its published form (cacg_update_class: a.ew holds sum gamma_k and
+// a.ld log det_k, stride 4): ew_k = w_k exp(ld_min - ld_k), w_k = 1 / K or sum gamma_k / T.  ld[0 .. K) are the
+// classes' log dets (ldk = ld[k]); fmin is exact, so the minimum does not depend on the class it starts from.
+template <int K>
+__device__ __forceinline__ double lean_ew(double sgam, double ldk, const double* ld, int weight_mode, int T) {
+  double ldmin = ld[0];
+#pragma unroll
+  for (int j = 1; j < K; ++j) ldmin = fmin(ldmin, ld[j]);
+  const double wk = weight_mode == PBB_WEIGHT_CONST ? 1.0 / K : sgam / (double)T;
+  return wk * exp(ldmin - ldk);
+}
+
+// Posterior of a padded frame (z = 0) under the staged model: the lean sweeps count the zs - T padded frames of the
+// last ring stage like observations, and the caller subtracts this from the lanes that counted them.
+template <int D, int K, int MODEL, typename SMT>
+__device__ __forceinline__ void padded_gamma(const SMT& sm, int cb, double eps, double (&gp)[K]) {
+  double q[K], cw[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) q[k] = 0.0;
+  if constexpr (MODEL == 1) softmax_watson<K>(q, sm.ew[cb], sm.ld, sm.w, gp, cw);
+  else softmax_product<D, K>(q, sm.ew[cb], eps, gp, cw);
+}
+
+// End of a sweep, after warp_reduce_halving of acc (the 32 frames of warp g reduced): the lanes store the group's
+// slots [g NSG, (g + 1) NSG) into the scatter-sum rows S[k].  The callers then add up the warp's sum of gamma, each
+// into its own destination.
+template <int D, int K>
+__device__ __forceinline__ void store_group_sums(const double (&acc)[K * GroupDims<D>::NSG], int g, int lane,
+                                                 double (*S)[D * D + 1]) {
+  constexpr int NSG = GroupDims<D>::NSG;
+  int lo, hi;
+  reduce_range<K * NSG>(lane, lo, hi);
+#pragma unroll
+  for (int j = 0; j < HalvingSizes<K * NSG>::n5; ++j) {
+    const int idx = lo + j;
+    if (idx < hi) {
+      const int k = idx / NSG, i = idx - k * NSG;
+      S[k][g * NSG + i] = acc[j];
+    }
+  }
+}
+
+// Frame split (PersistArgs::tsplit = S > 1): every part of (bin, it) leaves its scatter sums in a.tpart[bin][part] and
+// counts itself here (one thread); true for the part that arrives last, which then adds the S parts.
+__device__ __forceinline__ bool split_last_part(const PersistArgs& a, int bin, int it, int S) {
+  const int old = atomicAdd(a.tcount + bin, 1);
+  __threadfence();
+  return old + 1 == (it + 1) * S;
+}
+// Element i of the bin's scatter sums (row of K (NS + 1)): the parts added in the order p = 0 .. S-1, so that the
+// result does not depend on which CTA delivers the last part.
+template <int D, int K>
+__device__ __forceinline__ double split_sum(const PersistArgs& a, int bin, int S, int i) {
+  constexpr int kRow = K * (D * D + 1);
+  const double* __restrict__ tb = a.tpart + (size_t)bin * S * kRow;
+  double v = __ldcg(tb + i);
+  for (int q = 1; q < S; ++q) v += __ldcg(tb + (size_t)q * kRow + i);
+  return v;
+}
+
 // Threads of a CTA: the D / 2 slot-group warps and, when there are more classes than those, one "update only" warp
 // per class beyond them (D = 6, K = 4: the fourth class had to wait for a whole class update of warp 0, a quarter of
 // the complex Watson chain).  The extra warps follow the control flow, take every CTA-wide barrier, skip the E / M
@@ -853,7 +889,7 @@ __host__ __device__ constexpr int persist_ctas_per_sm(int D, bool full) {
   return full ? (D == 8 ? 3 : (D == 6 ? 4 : 6)) : (D == 4 ? 4 : 2);
 }
 
-template <int D, int K, typename CT, bool FULL, int FPL, int MODEL = 0>
+template <int D, int K, typename CT, bool FULL, int MODEL = 0>
 __global__ void __launch_bounds__(persist_threads(D, K), persist_ctas_per_sm(D, FULL))
 em_persistent_kernel(const PersistArgs a) {
   using SM = PersistSmem<D, K, CT>;
@@ -871,11 +907,6 @@ em_persistent_kernel(const PersistArgs a) {
   const int S = a.tsplit > 1 ? a.tsplit : 1;
   const int total = a.iterations * F * S;
   const CT* __restrict__ zbase = reinterpret_cast<const CT*>(a.z);
-  auto decode = [&](int t, int& b, int& i, int& p) {
-    const int tt = t / S;
-    p = t - tt * S;
-    decode_ticket(tt, F, a.iterations, a.wave_c, b, i);
-  };
 
   for (int s = tid; s < NS; s += blockDim.x) sm.tab[s] = slot_pack(D, s);
   if (tid == 0) {
@@ -886,16 +917,7 @@ em_persistent_kernel(const PersistArgs a) {
   __syncthreads();
   int cur = sm.tick[0];
   int bin = 0, it = 0, part = 0;
-  if (cur < total) {
-    if (a.order != nullptr) {
-      const int v = __ldcg(a.order + cur / S);
-      bin = v & 0xffff;
-      it = v >> 16;
-      part = cur % S;
-    } else {
-      decode(cur, bin, it, part);
-    }
-  }
+  if (cur < total) decode_task(a, cur, S, order_entry(a, cur, S), bin, it, part);
   unsigned chunk_cnt = 0;  // chunks consumed so far by this CTA (ring position)
 
   // 1-D TMA bulk copies per ring stage (stage_g2s), issued by a single elected lane.
@@ -964,13 +986,7 @@ em_persistent_kernel(const PersistArgs a) {
     if (!FULL && MODEL == 0 && !mstep_only && tid < 32) {
       // weights and ew from the published raw scalars (sum of gamma, log det): all of it lives in warp 0
       __syncwarp();
-      if (tid < K) {
-        double ldmin = sm.raw[cb][4];
-#pragma unroll
-        for (int j = 1; j < K; ++j) ldmin = fmin(ldmin, sm.raw[cb][4 + j]);
-        const double wk = a.weight_mode == PBB_WEIGHT_CONST ? 1.0 / K : sm.raw[cb][tid] / (double)T;
-        sm.ew[cb][tid] = wk * exp(ldmin - sm.raw[cb][4 + tid]);
-      }
+      if (tid < K) sm.ew[cb][tid] = lean_ew<K>(sm.raw[cb][tid], sm.raw[cb][4 + tid], &sm.raw[cb][4], a.weight_mode, T);
     }
     const bool fast = FULL ? (a.softmax_fast && !(a.user_model && it == 0)) : true;
     const bool lean = !FULL && !mstep_only;
@@ -1000,13 +1016,16 @@ em_persistent_kernel(const PersistArgs a) {
       if (tid == 0) {
         const int c_probe = ncp >= 3 ? c1 - 3 : -1;
         const int c_pub = ncp >= 2 ? c1 - 2 : c0;
+        const int c_first = c_probe >= 0 ? c_probe : c_pub;
+        // explicit order: ticket (atomic, task start) -> table entry (issued at c_first) -> decoded at c_pub; no flag
+        // probe / model prefetch in this mode
         if (a.order != nullptr) {
-          // explicit order: ticket (atomic, task start) -> table entry (issued here) -> decoded one chunk
-          // top later; no flag probe / model prefetch in this mode
-          if (c == (c_probe >= 0 ? c_probe : c_pub) && tnext < total) oraw = __ldcg(a.order + tnext / S);
+          if (c == c_first && tnext < total) oraw = __ldcg(a.order + tnext / S);
           if (c == c_pub) { nbin = oraw & 0xffff; nit = oraw >> 16; npart = tnext % S; }
-        } else if (c == (c_probe >= 0 ? c_probe : c_pub) && tnext < total) {
-          decode(tnext, nbin, nit, npart);
+        } else if (c == c_first && tnext < total) {
+          const int tt = tnext / S;
+          npart = tnext - tt * S;
+          decode_ticket(tt, F, a.iterations, a.wave_c, nbin, nit);
         }
         if (c == c_probe && !FULL && tnext < total && a.order == nullptr) {
           probe = (a.first_is_m && nit == 0) ? -1 : ld_acquire_gpu(a.flags + nbin) - nit;  // >= 0: published
@@ -1058,52 +1077,25 @@ em_persistent_kernel(const PersistArgs a) {
       const int t_chunk = c * kStageFrames;
       const int nsteps = (min(kStageFrames, zs - t_chunk)) >> 5;
       if (lean) {
-        if constexpr (FPL == 2) {
-          lean_chunk2<D, K, CT, MODEL, NAMED>(sm, cb, g, st, nsteps >> 1, lane, buf, a.aff_eps, acc, sg);
-          if (nsteps & 1) {  // odd tail step of a short last chunk
-            lean_chunk<D, K, CT, MODEL, NAMED>(sm, cb, g, st, 1, lane, buf, a.aff_eps, acc, sg, nsteps - 1);
-          }
-        } else {
-          lean_chunk<D, K, CT, MODEL, NAMED>(sm, cb, g, st, nsteps, lane, buf, a.aff_eps, acc, sg);
+        lean_chunk2<D, K, CT, MODEL, NAMED>(sm, cb, g, st, nsteps >> 1, lane, buf, a.aff_eps, acc, sg);
+        if (nsteps & 1) {  // odd tail step of a short last chunk
+          lean_step<D, K, CT, MODEL, NAMED>(sm, cb, g, st, nsteps - 1, lane, buf, a.aff_eps, acc, sg);
         }
       }
       else general_chunk<D, K, CT, FULL, NAMED>(a, sm, g, bin, st, t_chunk, nsteps, lane, buf, mstep_only, fast, acc, sg);
       PBB_PH(3);  // EM steps
     }
-    if (lean && MODEL == 0 && zs > T && c1 == nchunks) {
+    if (lean && zs > T && c1 == nchunks) {
       // the zs - T padded frames of every row behaved like zero observations
-      double q1[K], gp[K], cp[K];
-#pragma unroll
-      for (int k = 0; k < K; ++k) q1[k] = 0.0;
-      softmax_product<D, K>(q1, sm.ew[cb], a.aff_eps, gp, cp);
+      double gp[K];
+      padded_gamma<D, K, MODEL>(sm, cb, a.aff_eps, gp);
       const int npad_lane = (lane >= 32 - (zs - T)) ? 1 : 0;  // zs - T < 32: last step's tail lanes
 #pragma unroll
       for (int k = 0; k < K; ++k) sg[k] -= npad_lane ? gp[k] : 0.0;
     }
-    if (lean && MODEL == 1 && zs > T && c1 == nchunks) {
-      double q1[K], gp[K], cp[K];
-#pragma unroll
-      for (int k = 0; k < K; ++k) q1[k] = 0.0;
-      softmax_watson<K>(q1, sm.ew[cb], sm.ld, sm.w, gp, cp);
-      const int npad_lane = (lane >= 32 - (zs - T)) ? 1 : 0;
-#pragma unroll
-      for (int k = 0; k < K; ++k) sg[k] -= npad_lane ? gp[k] : 0.0;
-    }
 
-    // ---- reduce the 32 frames of each warp; group g owns slots [g*NSG, (g+1)*NSG) ----
     warp_reduce_halving<K * NSG>(acc, lane);
-    if (XW == 0 || g < M) {
-      int lo, hi;
-      reduce_range<K * NSG>(lane, lo, hi);
-#pragma unroll
-      for (int j = 0; j < HalvingSizes<K * NSG>::n5; ++j) {
-        const int idx = lo + j;
-        if (idx < hi) {
-          const int k = idx / NSG, i = idx - k * NSG;
-          sm.S[k][g * NSG + i] = acc[j];
-        }
-      }
-    }
+    if (XW == 0 || g < M) store_group_sums<D, K>(acc, g, lane, sm.S);
 #pragma unroll
     for (int k = 0; k < K; ++k) {
       const double v = warp_sum(sg[k]);
@@ -1119,20 +1111,11 @@ em_persistent_kernel(const PersistArgs a) {
       for (int i = tid; i < kRow; i += blockDim.x) __stcg(tp + i, (&sm.S[0][0])[i]);
       __threadfence();
       __syncthreads();
-      if (tid == 0) {
-        const int old = atomicAdd(a.tcount + bin, 1);
-        __threadfence();
-        sm.tick[5] = (old + 1 == (it + 1) * S);
-      }
+      if (tid == 0) sm.tick[5] = split_last_part(a, bin, it, S);
       __syncthreads();
       deliver = sm.tick[5] != 0;
       if (deliver) {
-        const double* __restrict__ tb = a.tpart + (size_t)bin * S * kRow;
-        for (int i = tid; i < kRow; i += blockDim.x) {
-          double v = __ldcg(tb + i);
-          for (int q = 1; q < S; ++q) v += __ldcg(tb + (size_t)q * kRow + i);  // fixed order: independent of who is last
-          (&sm.S[0][0])[i] = v;
-        }
+        for (int i = tid; i < kRow; i += blockDim.x) (&sm.S[0][0])[i] = split_sum<D, K>(a, bin, S, i);
         __syncthreads();
       }
     }

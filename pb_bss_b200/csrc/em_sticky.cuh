@@ -33,7 +33,7 @@ __device__ __forceinline__ void sticky_cluster_sync() {
 
 template <int K, typename CT>
 __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) {
-  constexpr int D = 8, MODEL = 0;
+  constexpr int D = 8;
   using SM = WsSmem<D, K, CT>;
   using G = GroupDims<D>;
   constexpr int NS = D * D, M = D / 2, NSG = G::NSG;
@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
   const int S = (int)cluster.num_blocks(), part = (int)cluster.block_rank();
   const int bin = blockIdx.x / S;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int T = a.T, zs = a.zs;
+  const int zs = a.zs;
   const int nchunks = (zs + kStageFrames - 1) / kStageFrames;
   const int c0 = part * nchunks / S, c1 = (part + 1) * nchunks / S;  // this CTA's ring stages (c1 - c0 <= kWsStages)
 
@@ -65,7 +65,6 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
     // =============================== EM warps ===============================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kStickyEmRegs));
     const int g = warp;
-    int buf = 0;
 #pragma unroll 1
     for (int it = 0; it < a.iterations; ++it) {
       const bool mstep_only = a.first_is_m && it == 0;
@@ -79,52 +78,11 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
       for (int c = c0; c < c1; ++c) {
         const int st = c - c0;
         mbar_wait(&sm.full[st], 0u);  // completes once; later iterations pass straight through
-        const int t_chunk = c * kStageFrames;
-        const int nsteps = (min(kStageFrames, zs - t_chunk)) >> 5;
-        if (!mstep_only) {
-          lean_chunk2_split<D, K, CT>(sm, 0, g, st, nsteps >> 1, lane, a.aff_eps, acc, sg);
-          if (nsteps & 1) {
-            // odd tail step: every group evaluates all 32 frames; only group 0 counts them
-            double sgt[K];
-#pragma unroll
-            for (int k = 0; k < K; ++k) sgt[k] = 0.0;
-            buf = 0;
-            lean_chunk<D, K, CT, MODEL, true>(sm, 0, g, st, 1, lane, buf, a.aff_eps, acc, sgt, nsteps - 1);
-#pragma unroll
-            for (int k = 0; k < K; ++k) sg[k] += g == 0 ? sgt[k] : 0.0;
-          }
-        } else {
-          general_chunk<D, K, CT, false>(a, sm, g, bin, st, t_chunk, nsteps, lane, buf, true, true, acc, sg);
-        }
+        ws_stage<K, CT>(a, sm, 0, g, bin, st, c, lane, mstep_only, acc, sg);
       }
-      if (!mstep_only && zs > T && c1 == nchunks) {
-        // the zs - T padded frames of every row behaved like zero observations: take them out in one place
-        double q1[K], gp[K], cp[K];
-#pragma unroll
-        for (int k = 0; k < K; ++k) q1[k] = 0.0;
-        softmax_product<D, K>(q1, sm.ew[0], a.aff_eps, gp, cp);
-        const int npad_lane = (g == 0 && lane >= 32 - (zs - T)) ? 1 : 0;
-#pragma unroll
-        for (int k = 0; k < K; ++k) sg[k] -= npad_lane ? gp[k] : 0.0;
-      }
-      if (mstep_only && g != 0) {  // the M-step-only pass counts gamma in every group: keep group 0's
-#pragma unroll
-        for (int k = 0; k < K; ++k) sg[k] = 0.0;
-      }
-      // ---- reduce the 32 frames of each warp; group g owns slots [g*NSG, (g+1)*NSG) ----
+      ws_task_end<K, CT>(a, sm, 0, g, c1, nchunks, lane, mstep_only, sg);
       warp_reduce_halving<K * NSG>(acc, lane);
-      {
-        int lo, hi;
-        reduce_range<K * NSG>(lane, lo, hi);
-#pragma unroll
-        for (int j = 0; j < HalvingSizes<K * NSG>::n5; ++j) {
-          const int idx = lo + j;
-          if (idx < hi) {
-            const int k = idx / NSG, i = idx - k * NSG;
-            sm.S[0][k][g * NSG + i] = acc[j];
-          }
-        }
-      }
+      store_group_sums<D, K>(acc, g, lane, sm.S[0]);
 #pragma unroll
       for (int k = 0; k < K; ++k) {
         const double v = warp_sum(sg[k]);
@@ -134,15 +92,7 @@ __global__ void __launch_bounds__(256, 2) em_sticky_kernel(const PersistArgs a) 
       sticky_cluster_sync();  // (2) CTA 0 has stored the new model into every CTA's shared memory
       if (it + 1 < a.iterations) {
         // weights and ew from the raw scalars (sum of gamma, log det), as the producer warp of em_ws_kernel does
-        if (tid < K) {
-          const double ldk = sm.ld[tid];
-          double ldmin = ldk;
-#pragma unroll
-          for (int j = 0; j < K; ++j) ldmin = fmin(ldmin, sm.ld[j]);
-          const double sgam = sm.S[1][tid][NS];
-          const double wk = a.weight_mode == PBB_WEIGHT_CONST ? 1.0 / K : sgam / (double)T;
-          sm.ew[0][tid] = wk * exp(ldmin - ldk);
-        }
+        if (tid < K) sm.ew[0][tid] = lean_ew<K>(sm.S[1][tid][NS], sm.ld[tid], sm.ld, a.weight_mode, a.T);
         asm volatile("bar.sync 1, %0;" ::"n"(32 * M) : "memory");
       }
     }

@@ -84,9 +84,54 @@ struct WsSmem {
   uint64_t s_full[2], s_empty[2];
 };
 
+// EM warp g's share of one ring stage st (chunk c of the bin) in em_ws_kernel and em_sticky_kernel, model buffer mb.
+// The E + M sweep computes the posterior once per frame (lean_chunk2_split: -3 % on C2), so sg counts the frames
+// this warp evaluated; in the odd tail step of a short last chunk every group evaluates all 32 frames and only group
+// 0 counts them.  The M-step-only pass counts gamma in every group (ws_task_end keeps group 0's).
+template <int K, typename CT>
+__device__ __forceinline__ void ws_stage(const PersistArgs& a, WsSmem<8, K, CT>& sm, int mb, int g, int bin, int st,
+                                         int c, int lane, bool mstep_only,
+                                         double (&acc)[K * GroupDims<8>::NSG], double (&sg)[K]) {
+  constexpr int D = 8;
+  const int t_chunk = c * kStageFrames;
+  const int nsteps = (min(kStageFrames, a.zs - t_chunk)) >> 5;
+  int buf = 0;
+  if (!mstep_only) {
+    lean_chunk2_split<D, K, CT>(sm, mb, g, st, nsteps >> 1, lane, a.aff_eps, acc, sg);
+    if (nsteps & 1) {
+      double sgt[K];
+#pragma unroll
+      for (int k = 0; k < K; ++k) sgt[k] = 0.0;
+      lean_step<D, K, CT, 0, true>(sm, mb, g, st, nsteps - 1, lane, buf, a.aff_eps, acc, sgt);
+#pragma unroll
+      for (int k = 0; k < K; ++k) sg[k] += g == 0 ? sgt[k] : 0.0;
+    }
+  } else {
+    general_chunk<D, K, CT, false>(a, sm, g, bin, st, t_chunk, nsteps, lane, buf, true, true, acc, sg);
+  }
+}
+
+// End of EM warp g's sweep of stages [.., c1): every padded frame was counted once, by whichever warp evaluated it,
+// so group 0 takes them out; the M-step-only pass keeps group 0's sum of gamma only.
+template <int K, typename CT>
+__device__ __forceinline__ void ws_task_end(const PersistArgs& a, const WsSmem<8, K, CT>& sm, int mb, int g, int c1,
+                                            int nchunks, int lane, bool mstep_only, double (&sg)[K]) {
+  if (!mstep_only && a.zs > a.T && c1 == nchunks) {
+    double gp[K];
+    padded_gamma<8, K, 0>(sm, mb, a.aff_eps, gp);
+    const int npad_lane = (g == 0 && lane >= 32 - (a.zs - a.T)) ? 1 : 0;
+#pragma unroll
+    for (int k = 0; k < K; ++k) sg[k] -= npad_lane ? gp[k] : 0.0;
+  }
+  if (mstep_only && g != 0) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) sg[k] = 0.0;
+  }
+}
+
 template <int K, typename CT>
 __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
-  constexpr int D = 8, MODEL = 0;
+  constexpr int D = 8;
   using SM = WsSmem<D, K, CT>;
   using G = GroupDims<D>;
   constexpr int NS = D * D, M = D / 2, NSG = G::NSG;
@@ -117,7 +162,6 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWsEmRegs));
     const int g = warp;
     unsigned chunk_cnt = 0;
-    int buf = 0;
 #ifdef PBB_PHASE_TIMING
     long long _tp = clock64();
 #endif
@@ -150,65 +194,22 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
         const int st = chunk_cnt % kWsStages;
         mbar_wait(&sm.full[st], (chunk_cnt / kWsStages) & 1u);
         PBB_PH(2);  // TMA wait
-        const int t_chunk = c * kStageFrames;
-        const int nsteps = (min(kStageFrames, zs - t_chunk)) >> 5;
-        if (!mstep_only) {
-          // posterior once per frame instead of once per slot group (lean_chunk2_split): -3 % on C2
-          lean_chunk2_split<D, K, CT>(sm, mb, g, st, nsteps >> 1, lane, a.aff_eps, acc, sg);
-          if (nsteps & 1) {
-            // odd tail step: every group evaluates all 32 frames; only group 0 counts them
-            double sgt[K];
-#pragma unroll
-            for (int k = 0; k < K; ++k) sgt[k] = 0.0;
-            buf = 0;
-            lean_chunk<D, K, CT, MODEL, true>(sm, mb, g, st, 1, lane, buf, a.aff_eps, acc, sgt, nsteps - 1);
-#pragma unroll
-            for (int k = 0; k < K; ++k) sg[k] += g == 0 ? sgt[k] : 0.0;
-          }
-        } else {
-          general_chunk<D, K, CT, false>(a, sm, g, bin, st, t_chunk, nsteps, lane, buf, true, true, acc, sg);
-        }
+        ws_stage<K, CT>(a, sm, mb, g, bin, st, c, lane, mstep_only, acc, sg);
         __syncwarp();
         if (lane == 0) mbar_arrive(&sm.empty[st]);
         ++chunk_cnt;
         PBB_PH(3);  // EM steps
       }
-      if (!mstep_only && zs > T && c1 == nchunks) {
-        // the zs - T padded frames of every row behaved like zero observations
-        double q1[K], gp[K], cp[K];
-#pragma unroll
-        for (int k = 0; k < K; ++k) q1[k] = 0.0;
-        softmax_product<D, K>(q1, sm.ew[mb], a.aff_eps, gp, cp);
-        // every padded frame was counted once, by whichever warp evaluated it: take them out in one place
-        const int npad_lane = (g == 0 && lane >= 32 - (zs - T)) ? 1 : 0;
-#pragma unroll
-        for (int k = 0; k < K; ++k) sg[k] -= npad_lane ? gp[k] : 0.0;
-      }
-      if (mstep_only && g != 0) {  // the M-step-only pass counts gamma in every group: keep group 0's
-#pragma unroll
-        for (int k = 0; k < K; ++k) sg[k] = 0.0;
-      }
+      ws_task_end<K, CT>(a, sm, mb, g, c1, nchunks, lane, mstep_only, sg);
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.model_empty[mb]);  // done with this task's model
 
-      // ---- reduce the 32 frames of each warp; group g owns slots [g*NSG, (g+1)*NSG) ----
       warp_reduce_halving<K * NSG>(acc, lane);
       const int sb = n & 1;
       PBB_PH(4);  // reduce
       mbar_wait(&sm.s_empty[sb], ((n >> 1) & 1u) ^ 1u);  // updaters are done with task n - 2
       PBB_PH(5);  // wait for the S buffer
-      {
-        int lo, hi;
-        reduce_range<K * NSG>(lane, lo, hi);
-#pragma unroll
-        for (int j = 0; j < HalvingSizes<K * NSG>::n5; ++j) {
-          const int idx = lo + j;
-          if (idx < hi) {
-            const int k = idx / NSG, i = idx - k * NSG;
-            sm.S[sb][k][g * NSG + i] = acc[j];
-          }
-        }
-      }
+      store_group_sums<D, K>(acc, g, lane, sm.S[sb]);
 #pragma unroll
       for (int k = 0; k < K; ++k) {
         const double v = warp_sum(sg[k]);
@@ -232,17 +233,7 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
         if (lane == 0) t = atomicAdd(a.ticket, 1);
         t = __shfl_sync(0xffffffffu, t, 0);
         int bin = -1, it = 0, part = 0;
-        if (t < total) {
-          const int tt = t / S;
-          part = t - tt * S;
-          if (a.order != nullptr) {
-            const int v = __ldcg(a.order + tt);
-            bin = v & 0xffff;
-            it = v >> 16;
-          } else {
-            decode_ticket(tt, F, a.iterations, a.wave_c, bin, it);
-          }
-        }
+        if (t < total) decode_task(a, t, S, order_entry(a, t, S), bin, it, part);
         const int c0 = part * nchunks / S, ncp = (part + 1) * nchunks / S - c0;  // this task's ring stages
         const bool mstep_only = a.first_is_m && it == 0;
         const bool late_z = mstep_only && a.wait_load;  // streamed upload: the bin may not have arrived yet
@@ -294,13 +285,11 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
           for (int i = lane; i < K * NS; i += 32) (&sm.coef[mb][0][0])[i] = __ldcg(cf + i);
           if (lane < K) {
             // weights and ew from the published raw scalars (sum of gamma, log det)
-            const double ldk = __ldcg(a.ld + (size_t)bin * 4 + lane);
-            double ldmin = ldk;
+            double ld[K];
 #pragma unroll
-            for (int j = 0; j < K; ++j) ldmin = fmin(ldmin, __ldcg(a.ld + (size_t)bin * 4 + j));
-            const double sgam = __ldcg(a.ew + (size_t)bin * 4 + lane);
-            const double wk = a.weight_mode == PBB_WEIGHT_CONST ? 1.0 / K : sgam / (double)T;
-            sm.ew[mb][lane] = wk * exp(ldmin - ldk);
+            for (int j = 0; j < K; ++j) ld[j] = __ldcg(a.ld + (size_t)bin * 4 + j);
+            sm.ew[mb][lane] = lean_ew<K>(__ldcg(a.ew + (size_t)bin * 4 + lane), __ldcg(a.ld + (size_t)bin * 4 + lane),
+                                         ld, a.weight_mode, T);
           }
         }
         if (lane == 0) { sm.desc[mb][0] = bin; sm.desc[mb][1] = it; sm.desc[mb][2] = part; }
@@ -348,24 +337,15 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
             for (int i = lane; i < NS + 1; i += 32) __stcg(tp + k * (NS + 1) + i, sm.S[sb][k][i]);
           __threadfence();
           asm volatile("bar.sync 2, %0;" ::"n"(NU * 32) : "memory");
-          if (u == 0 && lane == 0) {
-            const int old = atomicAdd(a.tcount + bin, 1);
-            __threadfence();
-            sm.tlast = (old + 1 == (it + 1) * S);
-          }
+          if (u == 0 && lane == 0) sm.tlast = split_last_part(a, bin, it, S);
           asm volatile("bar.sync 2, %0;" ::"n"(NU * 32) : "memory");
           if (!sm.tlast) {
             __syncwarp();
             if (lane == 0) mbar_arrive(&sm.s_empty[sb]);
             continue;  // (tlast is rewritten behind the next task's first updater barrier: everyone has read it by then)
           }
-          const double* __restrict__ tb = a.tpart + (size_t)bin * S * kRow;
           for (int k = u; k < K; k += NU)
-            for (int i = lane; i < NS + 1; i += 32) {
-              double v = __ldcg(tb + k * (NS + 1) + i);
-              for (int q = 1; q < S; ++q) v += __ldcg(tb + (size_t)q * kRow + k * (NS + 1) + i);
-              sm.S[sb][k][i] = v;
-            }
+            for (int i = lane; i < NS + 1; i += 32) sm.S[sb][k][i] = split_sum<D, K>(a, bin, S, k * (NS + 1) + i);
           __syncwarp();
           if (last_it) asm volatile("bar.sync 2, %0;" ::"n"(NU * 32) : "memory");
         }

@@ -1,25 +1,53 @@
-"""A/B timing of the C2 fit for several builds of the library: python scripts/ab_libs.py lib1.so lib2.so ..."""
-import os, sys, subprocess
+"""A/B timing and bit check of the C2 fit for several builds of the library: python scripts/ab_libs.py lib1.so lib2.so ...
+
+For every build (PBB_LIB; 'default' = the package's own library) it times the C2 fit (F = 513, em_ws_kernel) and the
+F = 65 fit of scripts/one_fit_small.py (em_sticky_kernel), saves the fitted eigenvectors, eigenvalues and weights of
+both, and reports whether they are byte-identical to those of the first build.  Environment variables such as
+PBB_STICKY or PBB_TSPLIT pass through to every build."""
+import os, sys, subprocess, tempfile
+SHAPES = {'C2': 513, 'F65': 65}  # bins; T = 500, D = 8, K = 3, 100 iterations
 if sys.argv[1] == 'child':
-    import time, torch
+    import numpy as np, torch
     sys.path.insert(0, '.')
     from oracle import synth
     from pb_bss_b200.distribution import CACGMMTrainer
-    F, T, D, K, I = 513, 500, 8, 3, 100
-    y = torch.from_numpy(synth.noise_stft(F, T, D)).cuda()
-    init = torch.from_numpy(synth.init_affiliation(F, K, T)).cuda()
-    tr = CACGMMTrainer()
-    for _ in range(3): tr.fit(y, initialization=init, iterations=I)
-    ts = []
-    for _ in range(10):
-        torch.cuda.synchronize(); e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-        e0.record(); tr.fit(y, initialization=init, iterations=I); e1.record(); torch.cuda.synchronize()
-        ts.append(e0.elapsed_time(e1))
-    ts.sort()
-    m = tr.fit(y, initialization=init, iterations=I)
-    print('%-50s min %.3f  median %.3f ms  checksum %.15e' % (os.environ.get('PBB_LIB', 'default'), ts[0], ts[len(ts) // 2], float(m.cacg.covariance_eigenvalues.sum())), flush=True)
+    T, D, K, I = 500, 8, 3, 100
+    out, line = {}, os.environ.get('PBB_LIB', 'default')
+    for name, F in SHAPES.items():
+        y = torch.from_numpy(synth.noise_stft(F, T, D)).cuda()
+        init = torch.from_numpy(synth.init_affiliation(F, K, T)).cuda()
+        tr = CACGMMTrainer()
+        for _ in range(3): tr.fit(y, initialization=init, iterations=I)
+        ts = []
+        for _ in range(10):
+            torch.cuda.synchronize(); e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
+            e0.record(); tr.fit(y, initialization=init, iterations=I); e1.record(); torch.cuda.synchronize()
+            ts.append(e0.elapsed_time(e1))
+        ts.sort()
+        m = tr.fit(y, initialization=init, iterations=I)
+        for key, v in (('vec', m.cacg.covariance_eigenvectors), ('val', m.cacg.covariance_eigenvalues), ('w', m.weight)):
+            out['%s_%s' % (name, key)] = v.cpu().numpy() if torch.is_tensor(v) else np.asarray(v)
+        line += '  %s min %.3f median %.3f ms' % (name, ts[0], ts[len(ts) // 2])
+    np.savez(sys.argv[2], **out)
+    print(line, flush=True)
 else:
-    for lib in sys.argv[1:]:
+    import numpy as np
+    tmp = tempfile.mkdtemp(prefix='ab_libs_')
+    first = None
+    for i, lib in enumerate(sys.argv[1:]):
         e = dict(os.environ)
         if lib != 'default': e['PBB_LIB'] = lib
-        subprocess.run(['timeout', '120', sys.executable, __file__, 'child'], env=e)
+        path = os.path.join(tmp, '%d.npz' % i)
+        r = subprocess.run(['timeout', '300', sys.executable, __file__, 'child', path], env=e)
+        if r.returncode != 0 or not os.path.exists(path):
+            print('%s: failed (exit %d)' % (lib, r.returncode), flush=True)
+            continue
+        res = dict(np.load(path))
+        if first is None:
+            first = (lib, res)
+            continue
+        ref = first[1]
+        diff = sorted(k for k in res if res[k].dtype != ref[k].dtype or res[k].shape != ref[k].shape
+                      or res[k].tobytes() != ref[k].tobytes())
+        print('%s vs %s: %s' % (lib, first[0], 'byte-identical' if not diff else 'DIFFERENT: ' + ', '.join(diff)),
+              flush=True)
