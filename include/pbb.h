@@ -61,6 +61,9 @@ extern "C" {
 #define PBB_WEIGHT_TIED 3     /* (-3, -1): frequency-tied, one per class: array (K) */
 #define PBB_WEIGHT_FRAME 4    /* one weight per (bin, frame), the same for every class: array (F, T); only
                                  pbb_log_pdf_to_affiliation (GMM / VMFMM weight_constant_axis (-2,)) */
+#define PBB_WEIGHT_BCAST 8    /* PBB_WEIGHT_BCAST | 1 (spans F) | 2 (spans K) | 4 (spans T): a contiguous (F', K', T')
+                                 array with F' = F or 1 etc., read with stride 0 along the dims whose bit is clear,
+                                 i.e. any weight that broadcasts to (F, K, T); only pbb_log_pdf_to_affiliation */
 
 const char* pbb_last_error(void);
 int pbb_version(void);
@@ -228,7 +231,9 @@ int pbb_gaussian_fit(const double* embedding, const double* weight, int F, int T
  * null) with the weight layouts of pbb_cacgmm_predict; inline_pa != 0:
  * log_pdf_to_affiliation_for_integration_models_with_inline_pa (:58-130) -- per bin the classes of log_pdf_a are
  * re-paired with those of log_pdf_b by the first permutation (itertools order) that maximises the auxiliary function;
- * permutation (F, K) int32 (may be null) receives the choice.  K <= 6. */
+ * permutation (F, K) int32 (may be null) receives the choice.  K <= 6.  weight_mode: PBB_WEIGHT_TIME, _CONST, _TIED_TIME,
+ * _TIED, _FRAME, or PBB_WEIGHT_BCAST with its bits (the weight of the public
+ * log_pdf_to_affiliation_for_integration_models_with_inline_pa, any shape that broadcasts to (F, K, T)). */
 int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
                                double scale_a, double scale_b, const double* weight,
                                int weight_mode, const uint8_t* activity,
@@ -1079,6 +1084,86 @@ int pbb_ccsg_sample(const void* a, const double* eigenvalues, int C, int D, cons
  * pbb_psd_workspace_bytes(F, N, D, 1). */
 int pbb_ccsg_fit(const void* observation, int dtype, int F, int D, int N, const double* saliency,
                  double denominator_floor, void* covariance, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Building blocks of pb_bss.distribution.mixture_model_utils, pb_bss.distribution.utils, pb_bss.utils and
+ * pb_bss.evaluation.sxr_module, csrc/api_mm_utils.cu.
+ *
+ * The operands are read and written in their own layouts: a pbb_nd_layout describes an index space (row-major over
+ * `shape`) and, for every operand, the stride of every dim in elements (complex elements counted once); a stride of
+ * 0 broadcasts the operand along that dim.  The arithmetic is fp64 and every result is rounded once to its storage
+ * type; all sums run in a fixed order, so results are bit-reproducible from call to call.  Element types are PBB_F32,
+ * PBB_F64, PBB_C64, PBB_C128 and, where stated, PBB_I32 / PBB_I64. */
+#define PBB_ND_MAX_DIMS 8
+#define PBB_ND_OPERANDS 4
+
+typedef struct pbb_nd_layout {
+  int nd; /* 0 <= nd <= PBB_ND_MAX_DIMS; nd = 0 is a single index */
+  int reserved;
+  long long shape[PBB_ND_MAX_DIMS];
+  long long stride[PBB_ND_OPERANDS][PBB_ND_MAX_DIMS];
+} pbb_nd_layout;
+
+/* log_pdf_to_affiliation (mixture_model_utils.py:7-55) for any K: for every index c of `columns` (the dims of
+ * log_pdf other than the class axis; operands 0 log_pdf, 1 weight, 2 mask, 3 out) and with class_stride[4] the
+ * strides of the class axis of the same operands: a_k = exp(l_k - max_k l_k) * weight_k * mask_k, out_k =
+ * a_k / max(sum_k a_k, tiny of dtype), clipped to [eps, 1 - eps] if eps != 0.  log_pdf and out are PBB_F32 / PBB_F64
+ * (`dtype`), weight float64 (null: 1), mask bool bytes (null: all set). */
+int pbb_affiliation_nd(const void* log_pdf, int dtype, const double* weight, const uint8_t* mask,
+                       const pbb_nd_layout* columns, int K, const long long* class_stride, double affiliation_eps,
+                       void* out, void* stream);
+
+/* The reductions below cut the reduced index space of every output into chunks whose length depends on the number of
+ * outputs and of reduced elements only -- about 16384 warps in all, at least 256 elements per chunk, one chunk when
+ * the outputs alone are that many; a warp reduces one (output, chunk) -- lane l takes the elements l, l + 32, ... of the chunk in order, and
+ * the lanes are combined by a fixed butterfly; fewer than 32 elements are one thread's loop -- and a second kernel
+ * combines the chunk partials of every output in chunk order the same way.  The partition depends on the shapes only,
+ * so results are bit-reproducible, and a long reduction with few outputs (np.sum over every axis, the frequency-tied
+ * mixture weights) spreads over the whole GPU.  workspace: pbb_reduce_workspace_bytes(outputs, n) bytes, n = the
+ * number of reduced elements per output. */
+size_t pbb_reduce_workspace_bytes(long long outs, long long n);
+
+/* The sum over a set of axes (np.sum / np.mean, estimate_mixture_weight mixture_model_utils.py:185-201, get_energy
+ * sxr_module.py:13-14): for every index o of `outer` (operands 0 x, 1 multiplier, 2 out) the sum over the index space
+ * `reduced` (operands 0 x, 1 multiplier) of v = x * multiplier (square = 0, real x) or v = re*re + im*im (square = 1,
+ * no FMA), divided by `divisor`.  multiplier float64, may be null.  out is PBB_F32 or PBB_F64 (`out_dtype`). */
+int pbb_axis_sum(const void* x, int dtype, const double* multiplier, const pbb_nd_layout* outer,
+                 const pbb_nd_layout* reduced, int square, double divisor, void* out, int out_dtype, void* workspace,
+                 size_t workspace_bytes, void* stream);
+
+/* _unit_norm (pb_bss/distribution/utils.py:223-256): for every index r of `rows` (operands 0 x, 1 out; rows.nd < 8)
+ * the vector norm of the n elements x_stride apart with np.linalg.norm's `ord` (2: sqrt of sum re*re + im*im; 1: sum
+ * |x|; +inf / -inf: max / min |x|; 0: count of non-zeros; other p: (sum |x|^p)^(1/p)), then eps_style 0 'plus' (norm
+ * + eps), 1 'max' (max(norm, eps)), 2 'where' (eps where norm == 0); then out = x / norm (out_stride apart; complex:
+ * both parts divided) in a second pass over every element.  x and out have the same dtype; the norms are kept in the
+ * workspace, pbb_reduce_workspace_bytes(rows, n). */
+int pbb_unit_norm(const void* x, int dtype, const pbb_nd_layout* rows, long long n, long long x_stride,
+                  long long out_stride, double ord, double eps, int eps_style, void* out, void* workspace,
+                  size_t workspace_bytes, void* stream);
+
+/* force_hermitian (pb_bss/distribution/utils.py:318-330): out = (A + A^H) / 2 of each of the `batch` contiguous
+ * D x D matrices; real input stays real (A + A^T) / 2. */
+int pbb_force_hermitian(const void* a, int dtype, long long batch, int D, void* out, void* stream);
+
+/* abs_square (pb_bss/utils.py:314-336): out = re*re + im*im (complex, in the precision of the input, no FMA) or
+ * x*x (real; PBB_I32 / PBB_I64 wrap like NumPy) of n contiguous elements; out has the real type of x. */
+int pbb_abs_square(const void* x, int dtype, long long n, void* out, void* stream);
+
+/* labels_to_one_hot (pb_bss/utils.py:234-311) written in its final layout: out (outer, C, inner) of elements of
+ * elem_size bytes (1, 2, 4, 8 or 16) gets the bit pattern `one` (elem_size bytes, host pointer) where
+ * labels[o][i] (int64, (outer, inner)) wraps to c (a negative label l counts as C + l), else zero bytes.  A label
+ * outside [-C, C) sets *status (reset by the call) = 1 + its index (the smallest such index). */
+int pbb_labels_to_one_hot(const long long* labels, long long outer, long long inner, int C, int elem_size,
+                          const void* one, void* out, int* status, void* stream);
+
+/* N *= factor of set_snr (sxr_module.py:51-78): out = x * factor over the index space `layout` (operands 0 x,
+ * 1 factor (float64), 2 out); x and out of `dtype` (complex: both parts scaled), out may be x. */
+int pbb_scale_nd(const void* x, int dtype, const double* factor, const pbb_nd_layout* layout, void* out,
+                 void* stream);
+
+/* VonMisesFisher.pdf (von_mises_fisher.py:82-83): exp of pbb_vmf_log_pdf, same arguments, in one pass. */
+int pbb_vmf_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
+                int B, int N, int E, int K, double* pdf, void* stream);
 
 #ifdef __cplusplus
 }

@@ -49,8 +49,23 @@ class MaskLayout(ctypes.Structure):
     ]
 
 
+ND_MAX_DIMS, ND_OPERANDS = 8, 4
+WEIGHT_BCAST = 8
+
+
+class NdLayout(ctypes.Structure):
+    """struct pbb_nd_layout (include/pbb.h)."""
+    _fields_ = [
+        ('nd', ctypes.c_int),
+        ('reserved', ctypes.c_int),
+        ('shape', ctypes.c_longlong * ND_MAX_DIMS),
+        ('stride', (ctypes.c_longlong * ND_MAX_DIMS) * ND_OPERANDS),
+    ]
+
+
 _vp, _i, _d, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_size_t
 _ll, _lay = ctypes.c_longlong, ctypes.POINTER(MaskLayout)
+_nd = ctypes.POINTER(NdLayout)
 
 # name -> (restype, argtypes); mirrors include/pbb.h one to one
 SIGNATURES = {
@@ -178,6 +193,15 @@ SIGNATURES = {
     'pbb_ccsg_log_pdf': (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp]),
     'pbb_ccsg_sample': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _ll, _i, _vp, _vp, _sz, _vp, _vp]),
     'pbb_ccsg_fit': (_i, [_vp, _i, _i, _i, _i, _vp, _d, _vp, _vp, _sz, _vp]),
+    'pbb_affiliation_nd': (_i, [_vp, _i, _vp, _vp, _nd, _i, ctypes.POINTER(_ll), _d, _vp, _vp]),
+    'pbb_reduce_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_axis_sum': (_i, [_vp, _i, _vp, _nd, _nd, _i, _d, _vp, _i, _vp, _sz, _vp]),
+    'pbb_unit_norm': (_i, [_vp, _i, _nd, _ll, _ll, _ll, _d, _d, _i, _vp, _vp, _sz, _vp]),
+    'pbb_force_hermitian': (_i, [_vp, _i, _ll, _i, _vp, _vp]),
+    'pbb_abs_square': (_i, [_vp, _i, _ll, _vp, _vp]),
+    'pbb_labels_to_one_hot': (_i, [_vp, _ll, _ll, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_scale_nd': (_i, [_vp, _i, _vp, _nd, _vp, _vp]),
+    'pbb_vmf_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
 }
 
 _lib = None

@@ -150,6 +150,10 @@ __global__ void gaussian_fit_cov_kernel(const double* __restrict__ partial, cons
 }
 
 __device__ __forceinline__ double weight_of(const double* __restrict__ w, int mode, int f, int k, int t, int K, int T) {
+  if (mode >= PBB_WEIGHT_BCAST) {  // (F', K', T') with stride 0 along the dims whose bit is clear
+    const int kn = mode & 2 ? K : 1, tn = mode & 4 ? T : 1;
+    return w[((size_t)(mode & 1 ? f : 0) * kn + (mode & 2 ? k : 0)) * tn + (mode & 4 ? t : 0)];
+  }
   switch (mode) {
     case PBB_WEIGHT_CONST: return 1.0 / K;
     case PBB_WEIGHT_TIED_TIME: return w[(size_t)k * T + t];
@@ -450,6 +454,7 @@ __global__ void __launch_bounds__(32) precision_cholesky_kernel(const double* __
 
 // VonMisesFisher.log_pdf (von_mises_fisher.py:65-79) for B models: out[b][k][n] = concentration[b][k]
 // <mean[b][k], x / max(||x||, tiny)> - log_norm[b][k].
+template <bool EXP>
 __global__ void __launch_bounds__(128) vmf_log_pdf_kernel(const double* __restrict__ x, const double* __restrict__ mean,
                                                           const double* __restrict__ concentration,
                                                           const double* __restrict__ log_norm, int N, int E, int K,
@@ -475,7 +480,8 @@ __global__ void __launch_bounds__(128) vmf_log_pdf_kernel(const double* __restri
   for (int k = 0; k < kIntMaxK; ++k)
     if (k < K) {
       const size_t bk = (size_t)b * K + k;
-      out[bk * N + n] = concentration[bk] * (dot[k] / nrm) - log_norm[bk];
+      const double lp = concentration[bk] * (dot[k] / nrm) - log_norm[bk];
+      out[bk * N + n] = EXP ? exp(lp) : lp;  // EXP: VonMisesFisher.pdf
     }
 }
 
@@ -502,6 +508,22 @@ inline FullFitChunks full_fit_chunks(int B, int N, int K) {
   c.chunk_len = per * kFitTileN;
   c.nchunks = (N + c.chunk_len - 1) / c.chunk_len;
   return c;
+}
+
+template <bool EXP>
+static int vmf_log_pdf_launch(const double* embedding, const double* mean, const double* concentration,
+                              const double* log_norm, int B, int N, int E, int K, double* out, void* stream) {
+  PBB_CHECK_ARG(embedding && mean && concentration && log_norm, 1, "input is null");
+  PBB_CHECK_ARG(B > 0 && B <= 65535 && N > 0, 5, "bad shape");
+  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 7, "need 0 < E <= 64");
+  PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 8, "need 0 < K <= 6");
+  PBB_CHECK_ARG(out != nullptr, 9, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls(EXP ? "vmf_pdf_kernel" : "vmf_log_pdf_kernel", st);
+  vmf_log_pdf_kernel<EXP><<<dim3((N + 127) / 128, B), 128, 0, st>>>(embedding, mean, concentration, log_norm, N, E, K,
+                                                                     out);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
 }
 
 }  // namespace pbb
@@ -579,7 +601,9 @@ int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
                                void* stream) {
   PBB_CHECK_ARG(log_pdf_a != nullptr, 1, "log pdf is null");
   PBB_CHECK_ARG(weight != nullptr || weight_mode == PBB_WEIGHT_CONST, 5, "weight is null");
-  PBB_CHECK_ARG(weight_mode >= 0 && weight_mode <= PBB_WEIGHT_FRAME, 6, "bad weight_mode");
+  PBB_CHECK_ARG((weight_mode >= 0 && weight_mode <= PBB_WEIGHT_FRAME) ||
+                    (weight_mode >= PBB_WEIGHT_BCAST && weight_mode < 2 * PBB_WEIGHT_BCAST),
+                6, "bad weight_mode");
   PBB_CHECK_ARG(F > 0 && T > 0, 10, "bad shape");
   PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 11, "need 0 < K <= 6 (K! pairings per bin)");
   PBB_CHECK_ARG(!inline_pa || log_pdf_b != nullptr, 9, "the inline alignment pairs TWO log pdfs");
@@ -674,17 +698,12 @@ int pbb_precision_cholesky(const double* covariance, int M, int E, double* preci
 
 int pbb_vmf_log_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
                     int B, int N, int E, int K, double* log_pdf, void* stream) {
-  PBB_CHECK_ARG(embedding && mean && concentration && log_norm, 1, "input is null");
-  PBB_CHECK_ARG(B > 0 && B <= 65535 && N > 0, 5, "bad shape");
-  PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 7, "need 0 < E <= 64");
-  PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 8, "need 0 < K <= 6");
-  PBB_CHECK_ARG(log_pdf != nullptr, 9, "output is null");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("vmf_log_pdf_kernel", st);
-  vmf_log_pdf_kernel<<<dim3((N + 127) / 128, B), 128, 0, st>>>(embedding, mean, concentration, log_norm, N, E, K,
-                                                                log_pdf);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return vmf_log_pdf_launch<false>(embedding, mean, concentration, log_norm, B, N, E, K, log_pdf, stream);
+}
+
+int pbb_vmf_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
+                int B, int N, int E, int K, double* pdf, void* stream) {
+  return vmf_log_pdf_launch<true>(embedding, mean, concentration, log_norm, B, N, E, K, pdf, stream);
 }
 
 int pbb_vmf_resultant(const double* embedding, const double* weight, int B, int N, int E, int K, double* resultant,

@@ -17,7 +17,8 @@ import torch
 
 from .. import _device, _lib
 from .mixture_model_utils import flatten_obs
-from .utils import _ProbabilisticModel
+from .complex_watson import normalize_observation  # noqa: F401  (complex_bingham.py:12-25, the same function)
+from .utils import _ProbabilisticModel, force_hermitian  # noqa: F401  (complex_bingham.py:597)
 
 __all__ = ['ComplexBingham', 'ComplexBinghamTrainer']
 

@@ -15,6 +15,7 @@ Differences from the reference:
     computed; under NumPy 2 the reference's versions raise AttributeError (``np.asfarray`` was removed).
   - D is limited to 64.
 """
+import math
 from dataclasses import dataclass
 from functools import cached_property
 
@@ -27,6 +28,22 @@ from .mixture_model_utils import status_check
 from .utils import _ProbabilisticModel
 
 __all__ = ['ComplexWatson', 'ComplexWatsonTrainer']
+
+
+def normalize_observation(observation):
+    """(..., N, D) -> unit-norm (..., N, D) on the device: observation / max(norm over D, tiny)
+    (complex_watson.py:16-29, complex_bingham.py:12-25; pbb_normalize_observation with swap = 0, the layout kept).
+    Zero vectors stay zero.  Complex input; numpy in -> numpy out, CUDA tensor in -> CUDA tensor out."""
+    like_numpy = not _device.is_tensor(observation)
+    y = _device.to_device(observation)
+    code = _device.complex_dtype_code(y)
+    *independent, N, D = y.shape
+    z = torch.empty(tuple(y.shape), dtype=y.dtype, device=y.device)
+    if z.numel():
+        lib = _lib.load()
+        _lib.check(lib.pbb_normalize_observation(_device.ptr(y), _device.ptr(z), math.prod(independent), N, D, code,
+                                                 0, _device.stream_ptr()), 'pbb_normalize_observation')
+    return _device.to_host(z, like_numpy)
 
 
 @dataclass

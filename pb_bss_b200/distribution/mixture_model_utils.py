@@ -1,17 +1,23 @@
-"""The EM plumbing the mixture-model trainers share (pb_bss/distribution/mixture_model_utils.py): the fit preamble,
-the weight layouts between the public models and the kernels, models to NumPy, and the EM loop whose bins couple in
-every iteration (frequency-tied mixture weights, inline permutation alignment) for cACGMM, CWMM and CBMM."""
+"""pb_bss/distribution/mixture_model_utils.py on the device: the public building blocks (log_pdf_to_affiliation,
+its inline-permutation-alignment variant, estimate_mixture_weight, apply_inline_permutation_alignment), and the EM
+plumbing the mixture-model trainers share: the fit preamble, the weight layouts between the public models and the
+kernels, models to NumPy, and the EM loop whose bins couple in every iteration (frequency-tied mixture weights, inline
+permutation alignment) for cACGMM, CWMM and CBMM."""
 import copy
+import ctypes
 import dataclasses
 import math
 from operator import xor
 
 import numpy as np
 import torch
+from numpy.lib.array_utils import normalize_axis_tuple
 
-from .. import _device, _lib
+from .. import _device, _lib, _nd
 from .gaussian import _dev
-from .utils import _ProbabilisticModel
+from .utils import _ProbabilisticModel, _unit_norm
+
+MAX_INLINE_PA_K = 6  # pbb_log_pdf_to_affiliation enumerates the K! pairings of every bin
 
 
 def check_initialization(initialization, num_classes):
@@ -198,3 +204,154 @@ def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, a
                 w_k = parallel.mean_over_all_bins(w_k, F, F_all, bin_group)
             model.weight = w_kt[None] if mode == _lib.WEIGHT_TIED_TIME else w_k[None, :, None]
     return model
+
+
+# ---- the public building blocks (mixture_model_utils.py:7-306) -------------------------------------------------------
+
+def log_pdf_to_affiliation(weight, log_pdf, source_activity_mask=None, affiliation_eps=0.):
+    """The posterior of a mixture model from its log-pdfs (mixture_model_utils.py:7-55), on the device.
+
+    log_pdf (..., K, N) float32 / float64 (other dtypes are taken as float64), any K and leading dims; weight any
+    shape that broadcasts to log_pdf; source_activity_mask a bool array of such a shape.  Per column: subtract the
+    max over K, exp, times weight, times mask, divide by max(sum over K, tiny of the dtype), clip to
+    [eps, 1 - eps] if eps != 0.  Every operand is read in its own strides (pbb_affiliation_nd), the arithmetic is fp64
+    and the result, of log_pdf's shape and dtype, is rounded once.  A weight or mask that would broadcast log_pdf to a
+    larger shape raises ValueError, as the reference's in-place product does."""
+    like = _nd.like_numpy(weight, log_pdf, source_activity_mask)
+    lp = _nd.device_view(log_pdf)
+    if lp.is_complex():
+        raise TypeError(f'log_pdf must be real, got {lp.dtype}')
+    nd = lp.dim()
+    if nd < 2:
+        raise np.exceptions.AxisError(-2, nd)
+    w = _nd.device_view(weight).to(torch.float64)
+    shapes = [tuple(w.shape), tuple(lp.shape)]
+    m = None
+    if source_activity_mask is not None:
+        m = _nd.device_view(source_activity_mask, floating=False)
+        shapes.append(tuple(m.shape))
+    np.broadcast_shapes(*shapes)  # ValueError for incompatible shapes, as np.broadcast_arrays
+
+    def check_fits(operand_shape):  # the reference's in-place products raise ValueError here
+        bshape = np.broadcast_shapes(operand_shape, tuple(lp.shape))
+        if bshape != tuple(lp.shape):
+            raise ValueError(f'non-broadcastable output operand with shape {tuple(lp.shape)} doesn\'t match the '
+                             f'broadcast shape {bshape}')
+    check_fits(tuple(w.shape))  # affiliation *= weight
+    if source_activity_mask is not None:
+        assert m.dtype == torch.bool, (source_activity_mask.dtype if hasattr(source_activity_mask, 'dtype')
+                                       else m.dtype)
+        check_fits(tuple(m.shape))  # affiliation *= source_activity_mask
+    shape = tuple(lp.shape)
+    out = _device.empty(shape, lp.dtype)
+    ws = _nd.broadcast_strides(w, shape)
+    ms = _nd.broadcast_strides(m, shape) if m is not None else (0,) * nd
+    ls, os_ = lp.stride(), out.stride()
+    cols = [a for a in range(nd) if a != nd - 2]
+    lay = _nd.layout([shape[a] for a in cols], *[[s[a] for a in cols] for s in (ls, ws, ms, os_)])
+    cs = (ctypes.c_longlong * 4)(ls[-2], ws[-2], ms[-2], os_[-2])
+    if out.numel():
+        lib = _lib.load()
+        _lib.check(lib.pbb_affiliation_nd(_device.ptr(lp), _nd.CODES[lp.dtype], _device.ptr(w),
+                                          _device.ptr(m.view(torch.uint8)) if m is not None else None, lay, shape[-2],
+                                          cs, float(affiliation_eps), _device.ptr(out), _device.stream_ptr()),
+                   'pbb_affiliation_nd')
+    return _device.to_host(out, like)
+
+
+def log_pdf_to_affiliation_for_integration_models_with_inline_pa(weight, spatial_log_pdf, spectral_log_pdf,
+                                                                 source_activity_mask=None, affiliation_eps=0.):
+    """Inline permutation alignment of the integrated models (mixture_model_utils.py:58-130): per bin the spatial
+    classes are re-paired with the spectral ones by the first permutation (itertools order) that maximises the
+    auxiliary function, then log_pdf_to_affiliation of the paired sum.  spatial / spectral log-pdfs (F, K, T), weight
+    any shape that broadcasts to (F, K, T) (read with zero strides, PBB_WEIGHT_BCAST), the mask (F, K, T).  This is
+    pbb_log_pdf_to_affiliation with inline_pa = 1; it enumerates the K! permutations per bin, so K <= 6.  The result
+    is float64, as in the reference."""
+    like = _nd.like_numpy(weight, spatial_log_pdf, spectral_log_pdf, source_activity_mask)
+    a = _device.to_device(spatial_log_pdf, torch.float64)
+    b = _device.to_device(spectral_log_pdf, torch.float64)
+    F, K, T = a.shape
+    if K > MAX_INLINE_PA_K:
+        raise NotImplementedError(
+            f'log_pdf_to_affiliation_for_integration_models_with_inline_pa: need K <= {MAX_INLINE_PA_K} '
+            f'(K! pairings per bin), got K = {K}')
+    w = _nd.device_view(weight).to(torch.float64)
+    if w.dim() > 3 or np.broadcast_shapes(tuple(w.shape), (F, K, T)) != (F, K, T):
+        raise ValueError(f'weight of shape {tuple(w.shape)} does not broadcast to {(F, K, T)}')  # np.broadcast_to
+    w3 = w.reshape((1,) * (3 - w.dim()) + tuple(w.shape))
+    mode = _lib.WEIGHT_BCAST | sum(bit for bit, n in zip((1, 2, 4), w3.shape) if n != 1)
+    w3 = w3.contiguous()
+    act = None
+    if source_activity_mask is not None:
+        act = _device.to_device(source_activity_mask, torch.bool).expand(F, K, T).contiguous().view(torch.uint8)
+    out = _device.empty((F, K, T), torch.float64)
+    lib = _lib.load()
+    _lib.check(lib.pbb_log_pdf_to_affiliation(
+        _device.ptr(a), _device.ptr(b), 1.0, 1.0, _device.ptr(w3), mode, _device.ptr(act), float(affiliation_eps), 1,
+        F, K, T, _device.ptr(out), None, _device.stream_ptr()), 'pbb_log_pdf_to_affiliation')
+    return _device.to_host(out, like)
+
+
+def _promoted_float(aff_dtype, sal_dtype):
+    """The dtype of affiliation * saliency in NumPy (float32 * bool stays float32), float32 or float64."""
+    def np_dtype(d):
+        return torch.empty(0, dtype=d).numpy().dtype if isinstance(d, torch.dtype) else np.dtype(d)
+    return torch.float32 if np.result_type(np_dtype(aff_dtype), np_dtype(sal_dtype)) == np.float32 else torch.float64
+
+
+def estimate_mixture_weight(affiliation, saliency=None, weight_constant_axis=-1):
+    """The mixture weight (mixture_model_utils.py:133-203): an int axis equivalent to -2 gives np.full([K, 1], 1/K)
+    (host); otherwise the mean over ``weight_constant_axis`` with keepdims, or, with a saliency (..., N), the sum
+    over those axes of affiliation * saliency[..., None, :], L1-normalised over the classes (_unit_norm with ord=1,
+    axis=-2, eps=1e-10, eps_style='where').  The sums run on the device in a fixed order (pbb_axis_sum): fp64,
+    rounded once to the dtype NumPy returns; they are not NumPy's pairwise sums, so a result may differ from the
+    reference by the rounding of a reordered sum (a few ulp times the number of summed elements)."""
+    like = _nd.like_numpy(affiliation, saliency)
+    if not _device.is_tensor(affiliation):
+        affiliation = np.asarray(affiliation)
+    ndim = affiliation.ndim
+    if isinstance(weight_constant_axis, int) and weight_constant_axis % ndim - ndim == -2:
+        K = affiliation.shape[-2]
+        weight = np.full([K, 1], 1 / K)
+        return weight if like else _device.to_device(weight)
+    elif isinstance(weight_constant_axis, list):
+        weight_constant_axis = tuple(weight_constant_axis)
+    axes = tuple(sorted(normalize_axis_tuple(weight_constant_axis, ndim)))
+    x = _nd.device_view(affiliation)
+    if saliency is None:
+        weight = _nd.axis_sum(x, axes, True, divide_by_count=True)
+    else:
+        sal_dtype = saliency.dtype if _device.is_tensor(saliency) else np.asarray(saliency).dtype
+        s = _nd.device_view(saliency)
+        out_dtype = _promoted_float(x.dtype, sal_dtype)
+        mul = s.to(torch.float64)[..., None, :]
+        nd_all = max(x.dim(), mul.dim())
+        ax = tuple(sorted(normalize_axis_tuple(weight_constant_axis, nd_all)))
+        total = _nd.axis_sum(x, ax, True, multiplier=mul, out_dtype=out_dtype)
+        weight = _unit_norm(total, ord=1, axis=-2, eps=1e-10, eps_style='where')
+    return _device.to_host(weight, like)
+
+
+def apply_inline_permutation_alignment(affiliation, *, quadratic_form=None, weight_constant_axis, aligner):
+    """The inline permutation alignment step of the EM loops (mixture_model_utils.py:264-306): the aligner's
+    calculate_mapping of the (K, F, T) affiliation, applied to the affiliation and, if given, to the quadratic form.
+    affiliation / quadratic_form (F, K, T).  Both aligner steps run on the device."""
+    message = (
+        f'Inline permutation alignment reduces mismatch between frequency '
+        f'independent mixtures weights and a frequency independent '
+        f'observation model. Therefore, we require `affiliation.ndim == 3` '
+        f'({tuple(affiliation.shape)}) and a corresponding '
+        f'`weight_constant_axis` ({weight_constant_axis}).'
+    )
+    assert affiliation.ndim == 3, message
+    assert weight_constant_axis in ((-3,), (-3, -1), -3), message
+
+    def swap(x):
+        return x.permute(1, 0, 2) if _device.is_tensor(x) else np.transpose(x, (1, 0, 2))
+    affiliation = swap(affiliation)
+    mapping = aligner.calculate_mapping(affiliation)
+    affiliation = swap(aligner.apply_mapping(affiliation, mapping))
+    if quadratic_form is None:
+        return affiliation
+    quadratic_form = swap(aligner.apply_mapping(swap(quadratic_form), mapping))
+    return affiliation, quadratic_form

@@ -27,7 +27,22 @@ class VonMisesFisher(_ProbabilisticModel):
         return ((D / 2) * np.log(2 * np.pi) + np.log(ive(D / 2 - 1, kappa))
                 + (np.abs(kappa) - (D / 2 - 1) * np.log(kappa)))
 
-    def log_pdf(self, y):
+    def norm(self):
+        """exp(log_norm) (von_mises_fisher.py:62-63; the reference applies np.exp to the bound method and raises
+        TypeError, this evaluates the normaliser it means)."""
+        return np.exp(self.log_norm())
+
+    def sample(self, size):
+        """von_mises_fisher.py:85-91."""
+        raise NotImplementedError(
+            'A sampling method is not yet implemented. '
+            'Feel free to make a pull request.')
+
+    def pdf(self, y):
+        """exp(log_pdf(y)) (von_mises_fisher.py:82-90), in the same device pass as the log-pdf (pbb_vmf_pdf)."""
+        return self.log_pdf(y, _exp=True)
+
+    def log_pdf(self, y, _exp=False):
         """y (..., N, E) (any norm: normalised inside) -> (..., N), broadcast against the model dims
         (von_mises_fisher.py:65-79)."""
         like_numpy = not _device.is_tensor(y)
@@ -41,7 +56,7 @@ class VonMisesFisher(_ProbabilisticModel):
         m = _dev(np.broadcast_to(mean, L + (E,)).reshape(B, K, E))
         kap = _dev(np.broadcast_to(kappa, L).reshape(B, K))
         ln = _dev(np.broadcast_to(log_norm, L).reshape(B, K))
-        out = vmf_log_pdf_bkn(x, m, kap, ln)
+        out = vmf_log_pdf_bkn(x, m, kap, ln, exp=_exp)
         return _device.to_host(out.reshape(L + (yd.shape[-2],)), like_numpy)
 
     def log_pdf_fkt(self, embedding):
@@ -81,15 +96,15 @@ def vmf_fit_fkt(embedding, weight_fkt, min_concentration, max_concentration):
     return VonMisesFisher(mean=direction, concentration=concentration)
 
 
-def vmf_log_pdf_bkn(x, mean, concentration, log_norm):
-    """x (B, N, E), mean (B, K, E), concentration / log_norm (B, K) device -> (B, K, N)."""
+def vmf_log_pdf_bkn(x, mean, concentration, log_norm, exp=False):
+    """x (B, N, E), mean (B, K, E), concentration / log_norm (B, K) device -> (B, K, N); exp: the pdf."""
     B, N, E = x.shape
     K = mean.shape[1]
     out = _device.empty((B, K, N), torch.float64)
     lib = _lib.load()
-    _lib.check(lib.pbb_vmf_log_pdf(_device.ptr(x), _device.ptr(mean), _device.ptr(concentration),
-                                   _device.ptr(log_norm), B, N, E, K, _device.ptr(out), _device.stream_ptr()),
-               'pbb_vmf_log_pdf')
+    name = 'pbb_vmf_pdf' if exp else 'pbb_vmf_log_pdf'
+    _lib.check(getattr(lib, name)(_device.ptr(x), _device.ptr(mean), _device.ptr(concentration),
+                                  _device.ptr(log_norm), B, N, E, K, _device.ptr(out), _device.stream_ptr()), name)
     return out
 
 

@@ -23,7 +23,9 @@ import math
 import numpy as np
 import torch
 
-from .. import _device, _lib
+from numpy.lib.array_utils import normalize_axis_tuple
+
+from .. import _device, _lib, _nd
 
 __all__ = ['get_snr', 'input_sxr', 'output_sxr']
 
@@ -86,6 +88,17 @@ def _variance(X, axis=None, keepdims=False):
     return out.reshape(lead)
 
 
+def get_energy(x, axis=None, keepdims=False):
+    """sum |x * conj(x)| over ``axis`` (sxr_module.py:13-14): re*re + im*im per element (no FMA), summed on the device
+    in a fixed order (pbb_axis_sum; a long sum is split over chunks).  fp64, rounded once to the real dtype of x;
+    integer input gives float64 (the reference's integer sum is int64)."""
+    like = _like_numpy(x)
+    t = _nd.device_view(x)
+    nd = t.dim()
+    axes = tuple(range(nd)) if axis is None else tuple(sorted(normalize_axis_tuple(axis, nd)))
+    return _out(_nd.axis_sum(t, axes, keepdims, square=True), like)
+
+
 def get_variance_for_zero_mean_signal(X, axis=None, keepdims=False):
     """np.mean(|X|^2, axis, keepdims) (sxr_module.py:17-23): re^2 + im^2 for complex X, X^2 otherwise, in fp64."""
     return _out(_variance(X, axis, keepdims), _like_numpy(X))
@@ -103,6 +116,54 @@ def get_snr(X, N, *, axis=None, keepdims=False):
         with np.errstate(divide='ignore', invalid='ignore'):
             return 10 * np.log10(pX / pN)
     return 10 * torch.log10(pX / pN)
+
+
+def set_snr(X, N, snr, current_snr=None, *, axis=None, inplace=True):
+    """Rescales the noise N to the SNR ``snr`` (dB) against X (sxr_module.py:51-78): factor =
+    10 ** (-(snr - current_snr) / 20), current_snr = get_snr(X, N, axis=axis, keepdims=True) by default.  The few
+    factors are host math; the scaling is one device pass (pbb_scale_nd).  inplace=True scales the caller's NumPy array
+    or CUDA tensor N and returns None (an integer N raises NumPy's casting error, as the reference's ``N *= factor``);
+    inplace=False returns (X, N * factor) in NumPy's result dtype."""
+    if current_snr is None:
+        current_snr = get_snr(X, N, axis=axis, keepdims=True)
+    if _device.is_tensor(current_snr):
+        current_snr = current_snr.cpu().numpy()
+    factor = 10 ** (-(snr - current_snr) / 20)
+    n_tensor = _device.is_tensor(N)
+    n_dtype = np.dtype(str(N.dtype).replace('torch.', '')) if n_tensor else np.asarray(N).dtype
+    if inplace:
+        # NumPy's own casting check of ``N *= factor`` (UFuncTypeError for integer N)
+        np.multiply(np.zeros(1, n_dtype), factor if np.ndim(factor) == 0 else np.zeros((1,) * np.ndim(factor)),
+                    out=np.zeros((1,) * max(1, np.ndim(factor)), n_dtype), casting='same_kind')
+        out_dtype = n_dtype
+    else:
+        out_dtype = np.result_type(n_dtype, factor)
+    torch_out = getattr(torch, out_dtype.name)
+    if inplace and n_tensor:
+        x = N if N.device == _device.device() else None
+        if x is None:
+            raise ValueError('set_snr(inplace=True) scales a CUDA tensor or a NumPy array in place')
+    else:
+        x = _nd.device_view(N)
+        if x.dtype != torch_out:
+            x = x.to(torch_out)
+    if x.dtype not in _nd.CODES:
+        raise TypeError(f'set_snr: N of dtype {x.dtype} is not supported')
+    f = _device.to_device(np.asarray(factor, dtype=np.float64))
+    shape = tuple(np.broadcast_shapes(tuple(x.shape), tuple(f.shape)))
+    if shape != tuple(x.shape):
+        raise ValueError(f'non-broadcastable output operand with shape {tuple(x.shape)} doesn\'t match the broadcast '
+                         f'shape {shape}')
+    out = x if inplace and n_tensor else _device.empty(shape, x.dtype)
+    lay = _nd.layout(shape, x.stride(), _nd.broadcast_strides(f, shape), out.stride())
+    lib = _lib.load()
+    _lib.check(lib.pbb_scale_nd(_device.ptr(x) if x.numel() else None, _nd.CODES[x.dtype], _device.ptr(f), lay,
+                                _device.ptr(out) if out.numel() else None, _device.stream_ptr()), 'pbb_scale_nd')
+    if inplace:
+        if not n_tensor:
+            N[...] = out.cpu().numpy()
+        return None
+    return X, _device.to_host(out, not n_tensor)
 
 
 def _result(values, return_dict, strict):
