@@ -1165,6 +1165,48 @@ int pbb_scale_nd(const void* x, int dtype, const double* factor, const pbb_nd_la
 int pbb_vmf_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
                 int B, int N, int E, int K, double* pdf, void* stream);
 
+/* ---- WPE dereverberation (nara_wpe.wpe; contract restated in oracle/wpe_oracle.py) -------------------------------
+ * y is `bins` independent (D, T) problems of complex `dtype` (PBB_C64 / PBB_C128), element (b, d, t) at
+ * b ysb + d ysd + t yst (element strides, any sign); out likewise with its own strides.  All arithmetic is fp64;
+ * complex64 input is read as it is and the output rounded once at the store. */
+#define PBB_WPE_MAX_N 96          /* taps * D */
+#define PBB_WPE_MAX_D 30          /* channels: the per-bin solve, lstsq and filter kernels keep n x D blocks in
+                                     shared memory, which fits the 227 KB of a CTA for every taps * D <= 96 up to here */
+#define PBB_WPE_MAX_GROUP 65535   /* bins per group of pbb_wpe */
+#define PBB_WPE_NONFINITE 1       /* status bit: a non-finite output value (e.g. an all-zero bin) */
+#define PBB_WPE_LSTSQ 2           /* status bit: a bin's R had an exactly zero pivot and took the lstsq solution */
+
+/* Workspace of pbb_wpe for `group` bins: the weights, the power scratch, the partial statistics, the filters and the
+ * per-bin lstsq flags.  0 for an invalid shape. */
+size_t pbb_wpe_workspace_bytes(long long group, int D, long long T, int taps, int delay, int valid);
+
+/* wpe / wpe_v8 of nara_wpe.wpe: `iterations` times w = get_power_inverse(X, psd_context) per bin,
+ * R = sum_S w_t Yt_t Yt_t^H, P = sum_S w_t Yt_t Y_t^H (Yt: build_y_tilde(Y, taps, delay); S every frame, or
+ * t >= delay + taps - 1 with valid != 0), G = stable_solve(R, P) (np.linalg.solve; np.linalg.lstsq's minimum-norm
+ * solution for a bin with an exactly zero pivot), X = Y - G^H Yt; iterations = 0 copies y.  psd_context < 0 means
+ * inf.  out may be y (in place).  The bins run in groups of `group` bins sharing the workspace.  *status (reset by
+ * the call) ORs PBB_WPE_NONFINITE and PBB_WPE_LSTSQ over all bins and iterations; read it after the stream. */
+int pbb_wpe(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd, long long yst,
+            void* out, long long osb, long long osd, long long ost, int taps, int delay, int iterations,
+            long long psd_context, int valid, long long group, void* workspace, size_t workspace_bytes, int* status,
+            void* stream);
+
+/* Workspace of pbb_wpe_power: bins * T doubles. */
+size_t pbb_wpe_power_workspace_bytes(long long bins, long long T);
+
+/* get_power (inverse = 0) / get_power_inverse (inverse = 1) of nara_wpe.wpe, D <= PBB_WPE_MAX_D, any number of bins
+ * below 2^31: out (bins, T) float64 contiguous,
+ * lambda_t = mean over D of |y_dt|^2 with the psd_context moving mean (frames that exist only; < 0: the mean over all
+ * frames); the inverse is 1 / max(lambda, 1e-10 max lambda), the max over all bins. */
+int pbb_wpe_power(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                  long long yst, long long psd_context, int inverse, double* out, void* workspace,
+                  size_t workspace_bytes, void* stream);
+
+/* build_y_tilde of nara_wpe.wpe: out (bins, taps D, T) contiguous of y's dtype, row k D + d at frame t is
+ * y_{d, t - delay - k}, zero where t - delay - k < 0. */
+int pbb_wpe_build_y_tilde(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                          long long yst, int taps, int delay, void* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -202,6 +202,12 @@ SIGNATURES = {
     'pbb_labels_to_one_hot': (_i, [_vp, _ll, _ll, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_scale_nd': (_i, [_vp, _i, _vp, _nd, _vp, _vp]),
     'pbb_vmf_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    'pbb_wpe_workspace_bytes': (_sz, [_ll, _i, _ll, _i, _i, _i]),
+    'pbb_wpe': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _i, _ll, _vp, _sz,
+                     _vp, _vp]),
+    'pbb_wpe_power_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_wpe_power': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _ll, _i, _vp, _vp, _sz, _vp]),
+    'pbb_wpe_build_y_tilde': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _i, _i, _vp, _vp]),
 }
 
 _lib = None

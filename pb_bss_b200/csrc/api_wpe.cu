@@ -1,0 +1,232 @@
+// C-ABI entry points for WPE dereverberation, nara_wpe.wpe -- see include/pbb.h and csrc/wpe.cuh.
+#include "common.cuh"
+#include "prof.cuh"
+#include "wpe.cuh"
+
+namespace pbb {
+
+static size_t wpe_align(size_t b) { return (b + 255) & ~(size_t)255; }
+
+static WpeShape wpe_shape(int D, long long T, int taps, int delay, int valid, long long psd_context) {
+  WpeShape s{};
+  s.T = T;
+  s.D = D;
+  s.taps = taps;
+  s.delay = delay;
+  s.n = taps * D;
+  s.N2 = s.n + D;
+  s.T8 = (2 * s.N2 + 7) / 8;
+  s.ntiles = s.T8 * (s.T8 + 1) / 2;
+  s.tb = valid ? (long long)delay + taps - 1 : 0;
+  const long long tv = T - s.tb;
+  if (tv <= 0) {
+    s.parts = 1;
+    s.span = kWpeChunk;
+  } else {
+    long long parts = (tv + kWpePartFrames - 1) / kWpePartFrames;
+    parts = parts > kWpeMaxParts ? kWpeMaxParts : parts;
+    long long span = (tv + parts - 1) / parts;
+    s.span = (span + kWpeChunk - 1) / kWpeChunk * kWpeChunk;
+    s.parts = (int)((tv + s.span - 1) / s.span);
+  }
+  s.psd_context = psd_context;
+  return s;
+}
+
+struct WpeLayout {
+  size_t w, lam, part, G, lstsq, total;  // byte offsets
+};
+
+static WpeLayout wpe_layout(long long group, const WpeShape& s) {
+  WpeLayout l;
+  l.w = 0;
+  l.lam = wpe_align(l.w + (size_t)group * s.T * sizeof(double));
+  l.part = wpe_align(l.lam + (size_t)group * s.T * sizeof(double));
+  l.G = wpe_align(l.part + (size_t)group * s.parts * s.ntiles * 64 * sizeof(double));
+  l.lstsq = wpe_align(l.G + (size_t)group * s.n * s.D * sizeof(double2));
+  l.total = l.lstsq + (size_t)group * sizeof(int);
+  return l;
+}
+
+template <class TIn>
+static int wpe_filter_launch(const TIn* y, WpeStrides ys, const WpeShape& s, long long bins, const double2* G,
+                             TIn* out, WpeStrides os, int power, double* lam, double* pw, int* status,
+                             cudaStream_t st) {
+  const size_t smem = wpe_filter_smem_bytes(s.D, s.taps);
+  PBB_CUDA(cudaFuncSetAttribute(wpe_filter_kernel<TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchScope ls("wpe_filter_kernel", st);
+  wpe_filter_kernel<TIn><<<(unsigned)bins, 256, smem, st>>>(y, ys, s, G, out, os, power, lam, pw, status);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+template <int TPW, class TIn>
+static int wpe_corr_launch(const TIn* y, WpeStrides ys, const WpeShape& s, long long bins, const double* w,
+                           double* part, cudaStream_t st) {
+  const size_t smem = wpe_corr_smem_doubles(s.D, s.taps) * sizeof(double);
+  const unsigned passes = (unsigned)((s.ntiles + kWpeCorrWarps * TPW - 1) / (kWpeCorrWarps * TPW));
+  PBB_CUDA(cudaFuncSetAttribute(wpe_corr_kernel<TPW, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchScope ls("wpe_corr_kernel", st);
+  wpe_corr_kernel<TPW, TIn><<<dim3((unsigned)s.parts, (unsigned)bins, passes), 32 * kWpeCorrWarps, smem, st>>>(
+      y, ys, s, w, part);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// tiles per warp: the smallest instantiated slot count that covers every lower-triangle tile in one pass; more than
+// 16 x 22 tiles (n + D > 104) run in several passes of 22 slots
+template <class TIn>
+static int wpe_corr(const TIn* y, WpeStrides ys, const WpeShape& s, long long bins, const double* w, double* part,
+                    cudaStream_t st) {
+  const int tpw = (s.ntiles + kWpeCorrWarps - 1) / kWpeCorrWarps;
+  if (tpw <= 2) return wpe_corr_launch<2>(y, ys, s, bins, w, part, st);
+  if (tpw <= 6) return wpe_corr_launch<6>(y, ys, s, bins, w, part, st);
+  if (tpw <= 12) return wpe_corr_launch<12>(y, ys, s, bins, w, part, st);
+  if (tpw <= 16) return wpe_corr_launch<16>(y, ys, s, bins, w, part, st);
+  return wpe_corr_launch<22>(y, ys, s, bins, w, part, st);
+}
+
+template <class TIn>
+static int wpe_run(const TIn* y, WpeStrides ys, long long bins, TIn* out, WpeStrides os, const WpeShape& s,
+                   int iterations, long long group, char* ws, int* status, cudaStream_t st) {
+  const WpeLayout l = wpe_layout(group, s);
+  double* w = reinterpret_cast<double*>(ws + l.w);
+  double* lam = reinterpret_cast<double*>(ws + l.lam);
+  double* part = reinterpret_cast<double*>(ws + l.part);
+  double2* G = reinterpret_cast<double2*>(ws + l.G);
+  int* lstsq = reinterpret_cast<int*>(ws + l.lstsq);
+  const size_t solve_smem = wpe_solve_smem_bytes(s.n, s.D), lstsq_smem = wpe_lstsq_smem_bytes(s.n, s.D);
+  PBB_CUDA(cudaFuncSetAttribute(wpe_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem));
+  PBB_CUDA(cudaFuncSetAttribute(wpe_lstsq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lstsq_smem));
+  for (long long b0 = 0; b0 < bins; b0 += group) {
+    const long long g = bins - b0 < group ? bins - b0 : group;
+    const TIn* yg = y + b0 * ys.b;
+    TIn* og = out + b0 * os.b;
+    int rc = wpe_filter_launch<TIn>(yg, ys, s, g, nullptr, iterations == 0 ? og : nullptr, os,
+                                    iterations == 0 ? kWpePowerNone : kWpePowerInverse, lam, w, status, st);
+    if (rc) return rc;
+    for (int it = 0; it < iterations; ++it) {
+      const bool last = it == iterations - 1;
+      rc = wpe_corr<TIn>(yg, ys, s, g, w, part, st);
+      if (rc) return rc;
+      {
+        LaunchScope ls("wpe_solve_kernel", st);
+        wpe_solve_kernel<<<(unsigned)g, 256, solve_smem, st>>>(part, s, G, lstsq, status);
+        PBB_CUDA(cudaGetLastError());
+      }
+      {
+        LaunchScope ls("wpe_lstsq_kernel", st);
+        wpe_lstsq_kernel<<<(unsigned)g, 32, lstsq_smem, st>>>(part, s, lstsq, G);
+        PBB_CUDA(cudaGetLastError());
+      }
+      rc = wpe_filter_launch<TIn>(yg, ys, s, g, G, last ? og : nullptr, os, last ? kWpePowerNone : kWpePowerInverse,
+                                  lam, w, status, st);
+      if (rc) return rc;
+    }
+  }
+  return 0;
+}
+
+static bool wpe_valid_shape(int D, long long T, int taps, int delay) {
+  return D >= 1 && D <= PBB_WPE_MAX_D && T >= 1 && taps >= 1 && delay >= 0 && (long long)taps * D <= kWpeMaxN;
+}
+
+}  // namespace pbb
+
+using namespace pbb;
+
+extern "C" {
+
+size_t pbb_wpe_workspace_bytes(long long group, int D, long long T, int taps, int delay, int valid) {
+  if (group <= 0 || group > PBB_WPE_MAX_GROUP || !wpe_valid_shape(D, T, taps, delay)) return 0;
+  return wpe_layout(group, wpe_shape(D, T, taps, delay, valid, 0)).total;
+}
+
+int pbb_wpe(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd, long long yst,
+            void* out, long long osb, long long osd, long long ost, int taps, int delay, int iterations,
+            long long psd_context, int valid, long long group, void* workspace, size_t workspace_bytes, int* status,
+            void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0, 3, "bins must be positive");
+  PBB_CHECK_ARG(D >= 1 && D <= PBB_WPE_MAX_D, 4, "D must be in [1, PBB_WPE_MAX_D] (30)");
+  PBB_CHECK_ARG(T >= 1, 5, "T must be positive");
+  PBB_CHECK_ARG(out != nullptr, 9, "out is null");
+  PBB_CHECK_ARG(taps >= 1, 13, "taps must be positive");
+  PBB_CHECK_ARG(delay >= 0, 14, "delay must be >= 0");
+  PBB_CHECK_ARG((long long)taps * D <= kWpeMaxN, 13, "taps * D must be <= PBB_WPE_MAX_N (96)");
+  PBB_CHECK_ARG(iterations >= 0, 15, "iterations must be >= 0");
+  PBB_CHECK_ARG(group > 0 && group <= PBB_WPE_MAX_GROUP, 18, "group must be in [1, PBB_WPE_MAX_GROUP]");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid),
+                19, "workspace too small (pbb_wpe_workspace_bytes)");
+  PBB_CHECK_ARG(status != nullptr, 21, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const WpeShape s = wpe_shape(D, T, taps, delay, valid, psd_context);
+  const WpeStrides ys{ysb, ysd, yst}, os{osb, osd, ost};
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  char* ws = static_cast<char*>(workspace);
+  if (dtype == PBB_C64)
+    return wpe_run<float2>(static_cast<const float2*>(y), ys, bins, static_cast<float2*>(out), os, s, iterations,
+                           group, ws, status, st);
+  return wpe_run<double2>(static_cast<const double2*>(y), ys, bins, static_cast<double2*>(out), os, s, iterations,
+                          group, ws, status, st);
+}
+
+size_t pbb_wpe_power_workspace_bytes(long long bins, long long T) {
+  if (bins <= 0 || T <= 0) return 0;
+  return (size_t)bins * T * sizeof(double);
+}
+
+int pbb_wpe_power(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                  long long yst, long long psd_context, int inverse, double* out, void* workspace,
+                  size_t workspace_bytes, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0 && bins <= 0x7fffffffLL, 3, "bins must be in [1, 2^31 - 1]");
+  PBB_CHECK_ARG(D >= 1 && D <= PBB_WPE_MAX_D, 4, "D must be in [1, PBB_WPE_MAX_D] (30)");
+  PBB_CHECK_ARG(T >= 1, 5, "T must be positive");
+  PBB_CHECK_ARG(out != nullptr, 11, "out is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_wpe_power_workspace_bytes(bins, T), 12,
+                "workspace too small (pbb_wpe_power_workspace_bytes)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const WpeShape s = wpe_shape(D, T, 1, 0, 0, psd_context);
+  const WpeStrides ys{ysb, ysd, yst};
+  double* lam = static_cast<double*>(workspace);
+  int rc = dtype == PBB_C64
+               ? wpe_filter_launch<float2>(static_cast<const float2*>(y), ys, s, bins, nullptr, nullptr, ys,
+                                           kWpePowerPlain, lam, out, nullptr, st)
+               : wpe_filter_launch<double2>(static_cast<const double2*>(y), ys, s, bins, nullptr, nullptr, ys,
+                                            kWpePowerPlain, lam, out, nullptr, st);
+  if (rc || !inverse) return rc;
+  LaunchScope ls("wpe_power_inverse_kernel", st);
+  wpe_power_inverse_kernel<<<1, 1024, 0, st>>>(out, bins * T);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_wpe_build_y_tilde(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                          long long yst, int taps, int delay, void* out, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0, 3, "bins must be positive");
+  PBB_CHECK_ARG(D >= 1, 4, "D must be positive");
+  PBB_CHECK_ARG(T >= 1, 5, "T must be positive");
+  PBB_CHECK_ARG(taps >= 1, 9, "taps must be positive");
+  PBB_CHECK_ARG(delay >= 0, 10, "delay must be >= 0");
+  PBB_CHECK_ARG(out != nullptr, 11, "out is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const WpeStrides ys{ysb, ysd, yst};
+  const long long total = bins * taps * D * T;
+  const unsigned blocks = (unsigned)(total / 256 + 1 < 65536 ? total / 256 + 1 : 65536);
+  LaunchScope ls("wpe_y_tilde_kernel", st);
+  if (dtype == PBB_C64)
+    wpe_y_tilde_kernel<float2><<<blocks, 256, 0, st>>>(static_cast<const float2*>(y), ys, bins, D, T, taps, delay,
+                                                       static_cast<float2*>(out));
+  else
+    wpe_y_tilde_kernel<double2><<<blocks, 256, 0, st>>>(static_cast<const double2*>(y), ys, bins, D, T, taps, delay,
+                                                        static_cast<double2*>(out));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"

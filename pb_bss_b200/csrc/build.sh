@@ -11,7 +11,7 @@ mkdir -p $BUILD
 # objects built with other flags (another architecture) are not reused
 if [ "$(cat $BUILD/flags 2>/dev/null)" != "$FLAGS" ]; then rm -f $BUILD/*.o; echo "$FLAGS" > $BUILD/flags; fi
 pids=()
-for src in api_cacgmm api_linalg api_dhtv api_integration api_mask api_transform api_srmr api_bss_eval api_stoi api_sxr api_kmeans api_mm_utils prof; do
+for src in api_cacgmm api_linalg api_dhtv api_integration api_mask api_transform api_srmr api_bss_eval api_stoi api_sxr api_kmeans api_mm_utils api_wpe prof; do
   if [ ! -f $BUILD/$src.o ] || [ $src.cu -nt $BUILD/$src.o ] || [ -n "$(find . -maxdepth 1 -name '*.cuh' -newer $BUILD/$src.o)" ] || [ ../../include/pbb.h -nt $BUILD/$src.o ]; then
     ( $NVCC $FLAGS -c $src.cu -o $BUILD/$src.o > $BUILD/$src.log 2>&1 || { cat $BUILD/$src.log; exit 1; } ) &
     pids+=($!)

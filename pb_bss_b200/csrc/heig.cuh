@@ -40,21 +40,22 @@ __device__ inline int warp_jacobi(double2* __restrict__ A, double2* __restrict__
   for (; sweep < kJacobiMaxSweeps; ++sweep) {
     unsigned rotated = 0;
     for (int r = 0; r < n - 1; ++r) {
-      // ---- (a) rotation parameters, one lane per pair -----------------------
+      // ---- (a) rotation parameters, one lane per pair (lanes take pairs l, l + 32, ... for D > 64) ----
       bool act = false;
-      if (lane < npair) {
+      for (int pl = lane; pl < npair; pl += 32) {
         const int m = n - 1;
         int p, q;
-        if (lane == 0) { p = r % m; q = n - 1; }
-        else { p = (r + lane) % m; q = (r - lane + m) % m; }
+        if (pl == 0) { p = r % m; q = n - 1; }
+        else { p = (r + pl) % m; q = (r - pl + m) % m; }
         if (p > q) { int t = p; p = q; q = t; }
         double c = 1.0, sr = 0.0, si = 0.0, an = 0.0, dn = 0.0;
+        bool pact = false;
         if (q < D) {
           const double a = A[p * D + p].x, d = A[q * D + q].x;
           const double2 b = A[p * D + q];
           const double m2 = b.x * b.x + b.y * b.y;
           if (m2 > eps2 * fabs(a * d) && m2 > 1e-300) {
-            act = true;
+            pact = true;
             const double dl = 0.5 * (d - a);
             const double sg = dl >= 0.0 ? 1.0 : -1.0;
             const double h = fabs(dl) + sqrt(dl * dl + m2);
@@ -67,9 +68,10 @@ __device__ inline int warp_jacobi(double2* __restrict__ A, double2* __restrict__
             dn = d + tb;
           }
         }
-        double* ro = rot + lane * 6;
+        double* ro = rot + pl * 6;
         ro[0] = c; ro[1] = sr; ro[2] = si; ro[3] = an; ro[4] = dn;
-        ro[5] = act ? (double)(p | (q << 8)) : -1.0;  // packed pair or "inactive"
+        ro[5] = pact ? (double)(p | (q << 8)) : -1.0;  // packed pair or "inactive"
+        act |= pact;
       }
       const unsigned any = __ballot_sync(0xffffffffu, act);
       rotated |= any;
@@ -108,8 +110,8 @@ __device__ inline int warp_jacobi(double2* __restrict__ A, double2* __restrict__
       }
       __syncwarp();
       // ---- exact values for the rotated 2x2 blocks ---------------------------
-      if (lane < npair) {
-        const double* ro = rot + lane * 6;
+      for (int pl = lane; pl < npair; pl += 32) {
+        const double* ro = rot + pl * 6;
         if (ro[5] >= 0.0) {
           const int pq = (int)ro[5];
           const int p = pq & 255, q = pq >> 8;
