@@ -1207,6 +1207,34 @@ int pbb_wpe_power(const void* y, int dtype, long long bins, int D, long long T, 
 int pbb_wpe_build_y_tilde(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
                           long long yst, int taps, int delay, void* out, void* stream);
 
+/* ---- Frame-online WPE (nara_wpe.wpe.online_wpe_step; contract restated in oracle/wpe_online_oracle.py) -------
+ * The recursive least-squares form of WPE (Yoshioka & Nakatani, IEEE TASLP 20(10), 2012; Caroselli et al.,
+ * Interspeech 2017), one recursion per bin, n = taps D.  For frame t the window w (n) holds the frames
+ * t - delay - 1 - k (k < taps) at index d taps + k, and one step is
+ *   pred = y_t - G^H w, u = Q w, den = alpha lambda + w^H u, k = u / den, Q <- (Q - k (w^H Q)) / alpha,
+ *   G <- G + k pred^H,
+ * the division by alpha taken as a multiplication by 1 / alpha (exact for alpha = 1). */
+#define PBB_WPE_ONLINE_MAX_SMEM 232448  /* bytes: pbb_wpe_online_smem_bytes must not exceed this (227 KB) */
+
+/* Shared memory of one pbb_wpe_online CTA; taps + delay + 1 frames of D channels stay in it.  0 for an invalid
+ * shape. */
+size_t pbb_wpe_online_smem_bytes(int D, int taps, int delay);
+
+/* online_wpe_step of nara_wpe.wpe over T >= 0 frames in one launch.  y: T frames of `bins` bins, element (b, d, t)
+ * at b ysb + d ysd + t yst, complex `dtype`; history: the taps + delay frames before them, same dtype, own strides
+ * (null: zeros).  power: null, or (bins) float64 lambda of the only frame (T = 1, the step API); when null, lambda
+ * of frame t is the mean of |.|^2 over the D channels and the taps + delay + 1 frames t - taps - delay .. t,
+ * history included, recomputed per frame in a fixed order.  inv_cov (bins, n, n) and filter_taps (bins, n, D)
+ * complex128 row-major (null: identity, zeros); inv_cov_out and filter_taps_out receive Q and G after the last
+ * frame (they may be the inputs).  z (b, d, t) gets pred of every frame, in y's dtype.  fp64 arithmetic, fixed-order
+ * sums: a stream split over several calls (history and Q, G passed on) is bitwise equal to one call.  An all-zero
+ * bin gives NaN in that bin. */
+int pbb_wpe_online(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                   long long yst, const void* history, long long hsb, long long hsd, long long hst,
+                   const double* power, const void* inv_cov, const void* filter_taps, void* z, long long zsb,
+                   long long zsd, long long zst, void* inv_cov_out, void* filter_taps_out, int taps, int delay,
+                   double alpha, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -208,6 +208,9 @@ SIGNATURES = {
     'pbb_wpe_power_workspace_bytes': (_sz, [_ll, _ll]),
     'pbb_wpe_power': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _ll, _i, _vp, _vp, _sz, _vp]),
     'pbb_wpe_build_y_tilde': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _i, _i, _vp, _vp]),
+    'pbb_wpe_online_smem_bytes': (_sz, [_i, _i, _i]),
+    'pbb_wpe_online': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _vp, _vp, _vp, _vp, _ll, _ll,
+                            _ll, _vp, _vp, _i, _i, _d, _vp]),
 }
 
 _lib = None

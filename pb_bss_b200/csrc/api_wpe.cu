@@ -1,7 +1,9 @@
-// C-ABI entry points for WPE dereverberation, nara_wpe.wpe -- see include/pbb.h and csrc/wpe.cuh.
+// C-ABI entry points for WPE dereverberation, nara_wpe.wpe -- see include/pbb.h, csrc/wpe.cuh and
+// csrc/wpe_online.cuh.
 #include "common.cuh"
 #include "prof.cuh"
 #include "wpe.cuh"
+#include "wpe_online.cuh"
 
 namespace pbb {
 
@@ -127,6 +129,34 @@ static int wpe_run(const TIn* y, WpeStrides ys, long long bins, TIn* out, WpeStr
   return 0;
 }
 
+template <int R, class TIn>
+static int wpe_online_launch(const TIn* y, WpeStrides ys, const TIn* hist, WpeStrides hs, const double* power,
+                             const double2* Qin, const double2* Gin, TIn* z, WpeStrides zs, double2* Qout,
+                             double2* Gout, long long bins, const WpeOnlineShape& s, cudaStream_t st) {
+  const size_t smem = wpe_online_smem_bytes(s.D, s.taps, s.delay);
+  PBB_CUDA(cudaFuncSetAttribute(wpe_online_kernel<R, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchScope ls("wpe_online_kernel", st);
+  wpe_online_kernel<R, TIn><<<(unsigned)bins, kWpeOnlineThreads, smem, st>>>(y, ys, hist, hs, power, Qin, Gin, z,
+                                                                              zs, Qout, Gout, s);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// R = ceil(n / 16): each of the 16 x 16 threads holds R x R entries of Q
+template <class TIn>
+static int wpe_online_run(const TIn* y, WpeStrides ys, const TIn* hist, WpeStrides hs, const double* power,
+                          const double2* Qin, const double2* Gin, TIn* z, WpeStrides zs, double2* Qout,
+                          double2* Gout, long long bins, const WpeOnlineShape& s, cudaStream_t st) {
+  switch ((s.n + 15) / 16) {
+    case 1: return wpe_online_launch<1>(y, ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, bins, s, st);
+    case 2: return wpe_online_launch<2>(y, ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, bins, s, st);
+    case 3: return wpe_online_launch<3>(y, ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, bins, s, st);
+    case 4: return wpe_online_launch<4>(y, ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, bins, s, st);
+    case 5: return wpe_online_launch<5>(y, ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, bins, s, st);
+    default: return wpe_online_launch<6>(y, ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, bins, s, st);
+  }
+}
+
 static bool wpe_valid_shape(int D, long long T, int taps, int delay) {
   return D >= 1 && D <= PBB_WPE_MAX_D && T >= 1 && taps >= 1 && delay >= 0 && (long long)taps * D <= kWpeMaxN;
 }
@@ -227,6 +257,54 @@ int pbb_wpe_build_y_tilde(const void* y, int dtype, long long bins, int D, long 
                                                         static_cast<double2*>(out));
   PBB_CUDA(cudaGetLastError());
   return 0;
+}
+
+size_t pbb_wpe_online_smem_bytes(int D, int taps, int delay) {
+  if (D < 1 || taps < 1 || delay < 0) return 0;
+  return wpe_online_smem_bytes(D, taps, delay);
+}
+
+int pbb_wpe_online(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                   long long yst, const void* history, long long hsb, long long hsd, long long hst,
+                   const double* power, const void* inv_cov, const void* filter_taps, void* z, long long zsb,
+                   long long zsd, long long zst, void* inv_cov_out, void* filter_taps_out, int taps, int delay,
+                   double alpha, void* stream) {
+  PBB_CHECK_ARG(y != nullptr || T == 0, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0 && bins <= 0x7fffffffLL, 3, "bins must be in [1, 2^31 - 1]");
+  PBB_CHECK_ARG(D >= 1 && D <= PBB_WPE_MAX_D, 4, "D must be in [1, PBB_WPE_MAX_D] (30)");
+  PBB_CHECK_ARG(T >= 0, 5, "T must be >= 0");
+  PBB_CHECK_ARG(power == nullptr || T == 1, 13, "power needs T = 1");
+  PBB_CHECK_ARG(z != nullptr || T == 0, 16, "z is null");
+  PBB_CHECK_ARG(inv_cov_out != nullptr, 20, "inv_cov_out is null");
+  PBB_CHECK_ARG(filter_taps_out != nullptr, 21, "filter_taps_out is null");
+  PBB_CHECK_ARG(taps >= 1, 22, "taps must be positive");
+  PBB_CHECK_ARG((long long)taps * D <= kWpeMaxN, 22, "taps * D must be <= PBB_WPE_MAX_N (96)");
+  PBB_CHECK_ARG(delay >= 0, 23, "delay must be >= 0");
+  PBB_CHECK_ARG(alpha > 0.0 && alpha <= 1.0, 24, "alpha must be in (0, 1]");
+  PBB_CHECK_ARG(wpe_online_smem_bytes(D, taps, delay) <= (size_t)PBB_WPE_ONLINE_MAX_SMEM, 23,
+                "taps + delay + 1 frames of D channels do not fit the shared memory of a CTA "
+                "(pbb_wpe_online_smem_bytes)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  WpeOnlineShape s{};
+  s.T = T;
+  s.D = D;
+  s.taps = taps;
+  s.delay = delay;
+  s.n = taps * D;
+  s.L = taps + delay + 1;
+  s.alpha = alpha;
+  s.inv_alpha = 1.0 / alpha;
+  const WpeStrides ys{ysb, ysd, yst}, hs{hsb, hsd, hst}, zs{zsb, zsd, zst};
+  const double2* Qin = static_cast<const double2*>(inv_cov);
+  const double2* Gin = static_cast<const double2*>(filter_taps);
+  double2* Qout = static_cast<double2*>(inv_cov_out);
+  double2* Gout = static_cast<double2*>(filter_taps_out);
+  if (dtype == PBB_C64)
+    return wpe_online_run<float2>(static_cast<const float2*>(y), ys, static_cast<const float2*>(history), hs, power,
+                                  Qin, Gin, static_cast<float2*>(z), zs, Qout, Gout, bins, s, st);
+  return wpe_online_run<double2>(static_cast<const double2*>(y), ys, static_cast<const double2*>(history), hs, power,
+                                 Qin, Gin, static_cast<double2*>(z), zs, Qout, Gout, bins, s, st);
 }
 
 }  // extern "C"

@@ -17,7 +17,17 @@ Documented differences from nara_wpe:
   - real input raises TypeError (nara_wpe would compute in the real domain);
   - taps * D > 96 or D > 30 raises NotImplementedError (wpe, get_power, get_power_inverse);
   - sums over frames run in a fixed order, not NumPy's pairwise order.
+
+Frame-online WPE: ``online_wpe_step`` and ``get_power_online`` keep nara_wpe's signatures; ``online_wpe`` (not in
+nara_wpe) runs the step over a whole stream (T, ..., D) in one launch and returns the state to continue it, so a
+one-frame chunk is a streaming step.  The contract is restated in ``oracle/wpe_online_oracle.py``.  One CTA per bin
+keeps the inverse correlation Q in registers over all frames.  nara_wpe's ``OnlineWPE`` class is not provided: its
+power smoothing and buffer handling are not part of the restated contract, and ``online_wpe`` with ``state`` covers
+streaming.  Differences from nara_wpe: alpha outside (0, 1] raises ValueError (nara_wpe does not check it); the
+division by alpha is a multiplication by 1 / alpha; the taps + delay + 1 frames of the buffer must fit the shared
+memory of a CTA (about 1500 frames at D = 8, 350 at D = 30), else NotImplementedError.
 """
+import collections
 import math
 
 import numpy as np
@@ -31,7 +41,8 @@ MAX_GROUP = 65535               # PBB_WPE_MAX_GROUP
 WORKSPACE_BYTES = 1 << 30       # bins run in groups whose workspace stays under this (one bin at least)
 NONFINITE, LSTSQ = 1, 2         # PBB_WPE_NONFINITE, PBB_WPE_LSTSQ
 
-__all__ = ['wpe', 'get_power', 'get_power_inverse', 'build_y_tilde']
+__all__ = ['wpe', 'get_power', 'get_power_inverse', 'build_y_tilde', 'online_wpe_step', 'get_power_online',
+           'online_wpe', 'OnlineWPEState']
 
 
 def _is_complex(x):
@@ -206,3 +217,130 @@ def build_y_tilde(Y, taps, delay):
                                                      taps, delay, _device.ptr(out), _device.stream_ptr()),
                    'pbb_wpe_build_y_tilde')
     return _device.to_host(out, like_numpy)
+
+
+OnlineWPEState = collections.namedtuple('OnlineWPEState', ['history', 'inv_cov', 'filter_taps'])
+OnlineWPEState.__doc__ = """State of ``online_wpe`` in nara_wpe's layouts: history (taps + delay, ..., D) in Y's dtype, the last
+frames of the stream; inv_cov (..., n, n) and filter_taps (..., n, D) complex128, n = taps D, window index d taps + k."""
+
+ONLINE_MAX_SMEM = 232448        # PBB_WPE_ONLINE_MAX_SMEM
+
+
+def get_power_online(signal):
+    """nara_wpe.wpe.get_power_online: (...,) float64, the mean over D and T of |signal (..., D, T)|^2, i.e.
+    get_power(signal, psd_context=inf)[..., 0]."""
+    if signal.shape[-1] == 0:
+        raise ValueError('get_power_online needs at least one frame')
+    return _power(signal, math.inf, False)[..., 0]
+
+
+def _check_online(taps, delay, alpha, D):
+    if taps < 1:
+        raise ValueError(f'taps must be >= 1, got {taps}')
+    if delay < 0:
+        raise ValueError(f'delay must be >= 0, got {delay}')
+    if not 0.0 < float(alpha) <= 1.0:
+        raise ValueError(f'alpha must be in (0, 1], got {alpha}')
+    if taps * D > MAX_N or D > MAX_D:
+        raise NotImplementedError(f'online WPE supports taps * D <= {MAX_N} and D <= {MAX_D}, got taps = {taps}, '
+                                  f'D = {D}')
+    if _lib.load().pbb_wpe_online_smem_bytes(D, taps, delay) > ONLINE_MAX_SMEM:
+        raise NotImplementedError(f'online WPE keeps taps + delay + 1 frames of D channels in shared memory; '
+                                  f'taps = {taps}, delay = {delay}, D = {D} do not fit')
+
+
+def _frames(t):
+    """(frames, ..., D) device tensor -> (..., D, frames) view, or one copy, and its (bin, d, t) element strides."""
+    return _layout(t.movedim(0, -1))
+
+
+def _state_tensor(x, shape, what):
+    x = x if _device.is_tensor(x) else torch.from_numpy(np.asarray(x))
+    if tuple(x.shape) != tuple(shape):
+        raise ValueError(f'{what} must have shape {tuple(shape)}, got {tuple(x.shape)}')
+    return x.to(device=_device.device(), dtype=torch.complex128).contiguous()
+
+
+def _online(y, hist, power, Q, G, taps, delay, alpha):
+    """Launch pbb_wpe_online.  y (T, ..., D) and hist (taps + delay, ..., D) device tensors of one complex dtype (hist
+    None: zeros), power (...) float64 or None, Q, G contiguous complex128 or None.  -> (Z like y, Q', G')."""
+    T, lead, D = y.shape[0], tuple(y.shape[1:-1]), y.shape[-1]
+    bins = int(np.prod(lead, dtype=np.int64))
+    n = taps * D
+    Z = torch.empty_like(y, memory_format=torch.contiguous_format)
+    Qo = _device.empty(lead + (n, n), torch.complex128)
+    Go = _device.empty(lead + (n, D), torch.complex128)
+    if bins == 0:
+        return Z, Qo, Go
+    yv, ys = _frames(y) if T else (y, (0, 0, 0))
+    zv, zs = _frames(Z) if T else (Z, (0, 0, 0))
+    hv, hs = _frames(hist) if hist is not None else (None, (0, 0, 0))
+    _lib.check(_lib.load().pbb_wpe_online(
+        _device.ptr(yv) if T else None, _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(hv), *hs,
+        _device.ptr(power), _device.ptr(Q), _device.ptr(G), _device.ptr(zv) if T else None, *zs, _device.ptr(Qo),
+        _device.ptr(Go), taps, delay, float(alpha), _device.stream_ptr()), 'pbb_wpe_online')
+    return Z, Qo, Go
+
+
+def _complex_dtype(x):
+    """torch complex dtype of a real or complex array: complex64 for single precision, else complex128."""
+    single = (x.dtype in (torch.float32, torch.complex64) if _device.is_tensor(x)
+              else np.asarray(x).dtype in (np.float32, np.complex64))
+    return torch.complex64 if single else torch.complex128
+
+
+def online_wpe_step(input_buffer, power_estimate, inv_cov, filter_taps, alpha, taps, delay):
+    """nara_wpe.wpe.online_wpe_step: one frame of recursive least-squares WPE per bin.
+
+    input_buffer (taps + delay + 1, ..., D) complex, the last frame the current one; power_estimate (...) lambda;
+    inv_cov (..., n, n) Q and filter_taps (..., n, D) G, n = taps D, window index d taps + k (real Q, G are promoted
+    to complex).  Returns (prediction (..., D) in input_buffer's dtype, inv_cov_k, filter_taps_k) with
+        pred = y_t - G^H w,  k = Q w / (alpha lambda + w^H Q w),  Q' = (Q - k w^H Q) / alpha,  G' = G + k pred^H;
+    Q' and G' are complex64 where Q, G are single precision, else complex128."""
+    if len(input_buffer.shape) < 3:
+        raise ValueError(f'input_buffer needs shape (taps + delay + 1, ..., D), got {tuple(input_buffer.shape)}')
+    L, lead, D = input_buffer.shape[0], tuple(input_buffer.shape[1:-1]), input_buffer.shape[-1]
+    _check_online(taps, delay, alpha, D)
+    if L != taps + delay + 1:
+        raise ValueError(f'input_buffer needs taps + delay + 1 = {taps + delay + 1} frames, got {L}')
+    n = taps * D
+    if tuple(power_estimate.shape) != lead:
+        raise ValueError(f'power_estimate must have shape {lead}, got {tuple(power_estimate.shape)}')
+    qdt, gdt = _complex_dtype(inv_cov), _complex_dtype(filter_taps)
+    buf, like_numpy = _prepare(input_buffer, 'online_wpe_step')
+    Q = _state_tensor(inv_cov, lead + (n, n), 'inv_cov')
+    G = _state_tensor(filter_taps, lead + (n, D), 'filter_taps')
+    p = power_estimate if _device.is_tensor(power_estimate) else torch.from_numpy(np.asarray(power_estimate))
+    p = p.to(device=buf.device, dtype=torch.float64).contiguous()
+    Z, Qo, Go = _online(buf[L - 1:], buf[:L - 1], p, Q, G, taps, delay, alpha)
+    return (_device.to_host(Z[0], like_numpy), _device.to_host(Qo.to(qdt), like_numpy),
+            _device.to_host(Go.to(gdt), like_numpy))
+
+
+def online_wpe(Y, taps=10, delay=2, alpha=0.9999, state=None):
+    """Frame-online WPE over a whole stream: ``online_wpe_step`` for every frame of Y (T, ..., D) (frames first;
+    an STFT X (D, T, F) passes as ``X.transpose(1, 2, 0)``), with lambda = the mean of |.|^2 over the D channels and
+    the taps + delay + 1 frames of the step's buffer.  Returns (Z (T, ..., D) in Y's dtype, OnlineWPEState).
+    state None starts from taps + delay zero frames, Q = I and G = 0; passing the returned state continues the
+    stream, and any split of a stream gives bitwise the same Z and state as one call."""
+    if len(Y.shape) < 2:
+        raise ValueError(f'online_wpe needs Y of shape (T, ..., D), got {tuple(Y.shape)}')
+    T, lead, D = Y.shape[0], tuple(Y.shape[1:-1]), Y.shape[-1]
+    _check_online(taps, delay, alpha, D)
+    n, H = taps * D, taps + delay
+    y, like_numpy = _prepare(Y, 'online_wpe')
+    if state is None:
+        hist, Q, G = None, None, None
+    else:
+        h = state.history if _device.is_tensor(state.history) else torch.from_numpy(np.asarray(state.history))
+        if tuple(h.shape) != (H,) + lead + (D,):
+            raise ValueError(f'state.history must have shape {(H,) + lead + (D,)}, got {tuple(h.shape)}')
+        hist = h.to(device=y.device, dtype=y.dtype)
+        Q = _state_tensor(state.inv_cov, lead + (n, n), 'state.inv_cov')
+        G = _state_tensor(state.filter_taps, lead + (n, D), 'state.filter_taps')
+    Z, Qo, Go = _online(y, hist, None, Q, G, taps, delay, alpha)
+    if hist is None:
+        hist = torch.zeros((H,) + lead + (D,), dtype=y.dtype, device=y.device)
+    history = torch.cat([hist, y])[T:].clone()
+    return (_device.to_host(Z, like_numpy),
+            OnlineWPEState(*(_device.to_host(t, like_numpy) for t in (history, Qo, Go))))
