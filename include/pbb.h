@@ -108,7 +108,7 @@ typedef struct pbb_cacgmm_options {
   double eigenvalue_floor; /* cacgmm.py:155 */
   int frames_per_block;    /* 0 = library default; tuning knob */
   int reserved;            /* bit 0: force the multi-kernel (non-persistent) path;
-                              bit 1: no streamed upload (see pbb_cacgmm_fit) */
+                              every other bit must be 0 */
 } pbb_cacgmm_options;
 
 /* Host-only helper (no GPU needed): the task order pbb_cacgmm_fit uses for a streamed upload.
@@ -116,18 +116,19 @@ typedef struct pbb_cacgmm_options {
  * per time slot, at most `cap` tasks run per slot; every (bin, it) comes after (bin, it - 1). */
 int pbb_streamed_task_order(int F, int iterations, int arrive, int cap, int* order);
 
-/* Host only: which persistent kernel pbb_cacgmm_fit runs for a device-resident problem on a GPU with `sms` SMs, and
- * how one EM iteration of a bin is split (DESIGN.md 6.1).  lean = no saliency / activity mask / user-supplied model
- * and eigenvalue_floor in the product-softmax range; streamed = pinned host input.
- * *kernel: 0 = em_ws_kernel (task kernel, D = 8), 1 = em_sticky_kernel (one cluster of *split CTAs per bin for the
- * whole fit), 2 = em_persistent_kernel (D = 4 / 6, full variant); *split = parts per bin-iteration (1 = none).  The
- * environment overrides of the library (PBB_TSPLIT, PBB_STICKY, PBB_EM_KERNEL) are not applied here.  The sticky
- * kernel's clusters are modelled as two CTAs per SM placed anywhere; pbb_cacgmm_fit instead asks the device how many
- * clusters it runs at once, which on a GPU with uneven GPCs can pick a smaller cluster. */
+/* Host only: which persistent kernel pbb_cacgmm_fit runs for a problem on a GPU with `sms` SMs, and how one EM
+ * iteration of a bin is split (DESIGN.md 6.1).  lean = no saliency / activity mask / user-supplied model and
+ * eigenvalue_floor in the product-softmax range; streamed = pinned host input (streamed upload).
+ * *kernel: 0 = em_ws_kernel (task kernel, lean D = 8), 1 = em_sticky_kernel (one cluster of *split CTAs per bin for
+ * the whole fit), 2 = em_persistent_kernel (lean D = 4 / 6, full variant); *split = parts per bin-iteration (1 =
+ * none).  This is the function the fit itself uses, except that the sticky kernel's clusters are modelled as two CTAs
+ * per SM placed anywhere; pbb_cacgmm_fit instead asks the device how many clusters it runs at once, which on a GPU
+ * with uneven GPCs can pick a smaller cluster.  The complex Watson fit (pbb_cwmm_fit) always runs
+ * em_persistent_kernel, split as reported for lean = 1, streamed = 1. */
 int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms, int* kernel, int* split);
 
-/* Host only: the plan of the last persistent fit (pbb_cacgmm_fit / pbb_cwmm_fit) the calling host thread launched,
- * with the environment overrides applied.  *kernel and *split as in pbb_em_dispatch (*kernel = -1: none yet);
+/* Host only: the plan of the last persistent fit (pbb_cacgmm_fit / pbb_cwmm_fit) the calling host thread launched.
+ * *kernel and *split as in pbb_em_dispatch (*kernel = -1: none yet);
  * *variant: 0 = lean (product-form softmax), 1 = full with the integer-power softmax, 2 = full with the log-domain
  * softmax, 3 = complex Watson. */
 int pbb_em_last_plan(int* kernel, int* split, int* variant);

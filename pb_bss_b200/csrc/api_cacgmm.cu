@@ -2,11 +2,9 @@
 #include <algorithm>
 #include <array>
 #include <cstdarg>
-#include <cstdlib>
 #include <cstring>
 #include <map>
 #include <mutex>
-#include <optional>
 #include <type_traits>
 #include <vector>
 
@@ -153,42 +151,13 @@ static CacgmmWorkspace carve(void* base, int F, int T, int D, int K) {
   return ws;
 }
 
-// ---- tuning overrides ------------------------------------------------------------
-// Environment variables for A/B runs.  PBB_EM_KERNEL is read once per process, the others on every persistent fit;
-// pbb_em_dispatch uses none of them (Tuning{}).
-struct Tuning {
-  int tsplit = 0;       // > 0: frame split into that many parts (PBB_TSPLIT)
-  int sticky = -1;      // sticky-bins cluster size: -1 automatic, 0 off, S > 0 only S (PBB_STICKY)
-  bool single = false;  // single-role kernel only (PBB_EM_KERNEL=single; the complex Watson fit has no other)
-  int load_ctas = 0;    // > 0: stream_load_kernel CTAs (PBB_LOAD_CTAS)
-  std::optional<int> wave_c;     // bins joining per slot of the streamed task order (PBB_WAVE_C)
-  std::optional<int> order_cap;  // tasks per slot of the streamed task order (PBB_ORDER_CAP)
-  bool order = true;    // explicit streamed task order; PBB_NO_ORDER: the wave_c rounds of decode_ticket
-};
-
-static Tuning read_tuning() {
-  static const bool single = [] {
-    const char* e = getenv("PBB_EM_KERNEL");
-    return e != nullptr && !strcmp(e, "single");
-  }();
-  Tuning t;
-  t.single = single;
-  if (const char* e = getenv("PBB_TSPLIT")) t.tsplit = atoi(e);
-  if (const char* e = getenv("PBB_STICKY")) t.sticky = atoi(e);
-  if (const char* e = getenv("PBB_LOAD_CTAS")) t.load_ctas = atoi(e);
-  if (const char* e = getenv("PBB_WAVE_C")) t.wave_c = atoi(e);
-  if (const char* e = getenv("PBB_ORDER_CAP")) t.order_cap = atoi(e);
-  t.order = getenv("PBB_NO_ORDER") == nullptr;
-  return t;
-}
-
 // Frame split of the persistent kernels (em_ws.cuh, em_persistent.cuh): with fewer bins than CTA slots the fit is
 // bound by the per-bin dependency chain (E / M sweep -> update -> publish -> next sweep), so the sweep of one bin is
 // spread over S CTAs.  The partial sums live behind the final iteration's block of ws.part (the multi-kernel path
 // uses max_chunks(T) blocks there).
-// Parts a bin-iteration is split into (pure host logic, unit-tested through pbb_em_dispatch).  force > 0 overrides
-// the choice (PBB_TSPLIT); the result always satisfies 1 <= S <= nchunks and S + 1 <= max_chunks(T).
-static int choose_frame_split(int F, int T, int D, int K, int ctas_per_sm, int sms, int force) {
+// Parts a bin-iteration is split into (pure host logic, unit-tested through pbb_em_dispatch); the result always
+// satisfies 1 <= S <= nchunks and S + 1 <= max_chunks(T).
+static int choose_frame_split(int F, int T, int D, int K, int ctas_per_sm, int sms) {
   const int zs = (T + 31) / 32 * 32;
   const int nchunks = (zs + kStageFrames - 1) / kStageFrames;
   const long long slots = (long long)ctas_per_sm * sms;
@@ -198,7 +167,6 @@ static int choose_frame_split(int F, int T, int D, int K, int ctas_per_sm, int s
   // D = 8, T = 500 gains 12 % with S = 4)
   const long long sweep = (long long)T * D * D * (K + 1);
   while (S < 4 && 2 * S <= nchunks && (long long)F * 2 * S <= slots && sweep >= 24000LL * 2 * S) S *= 2;
-  if (force > 0) S = force;
   if (S > nchunks) S = nchunks;
   if (S + 1 > max_chunks(T)) S = 1;
   return S < 1 ? 1 : S;
@@ -206,13 +174,11 @@ static int choose_frame_split(int F, int T, int D, int K, int ctas_per_sm, int s
 // Cluster size of the sticky-bins kernel (em_sticky.cuh), 0 = not applicable: the largest of 4, 2, 1 whose parts fit
 // the ring (ceil(nchunks / S) <= kWsStages), that leaves every part a stage and whose F clusters run at once:
 // F <= clusters[i] for S = 1 << i.  Clusters of 4 are placed within a GPC, so on an H100 (132 SMs in GPCs of uneven
-// size) fewer of them fit than 2 x SMs / 4; a second wave would double the fit time.  force: -1 automatic, S > 0
-// only that size (PBB_STICKY).
-static int choose_sticky(int F, int T, const int clusters[3], int force) {
+// size) fewer of them fit than 2 x SMs / 4; a second wave would double the fit time.
+static int choose_sticky(int F, int T, const int clusters[3]) {
   const int zs = (T + 31) / 32 * 32;
   const int nchunks = (zs + kStageFrames - 1) / kStageFrames;
   for (int c = 4, i = 2; c >= 1; c /= 2, --i) {
-    if (force > 0 && c != force) continue;
     if (c > nchunks || (nchunks + c - 1) / c > kWsStages) continue;
     if (F > clusters[i]) continue;
     return c;
@@ -228,21 +194,24 @@ struct FitPlan {
   int split;   // sticky: CTAs per cluster; otherwise parts per bin-iteration (1 = no frame split)
 };
 
-// The sticky-bins kernel exists for the lean D = 8 fit of device-resident input.
-static bool sticky_eligible(int D, bool lean, bool streamed, const Tuning& o) {
-  return D == 8 && lean && !streamed && !o.single && o.sticky != 0;
-}
+// Models of the persistent fit: full = saliency / activity mask / log-domain softmax; lean = product-form softmax,
+// 2 frames per lane; cw = complex Watson EM (lean structure, MODEL = 1, always the single-role kernel).
+enum class Persist { kFull, kLean, kCw };
+
+// The lean D = 8 fit runs em_ws_kernel, or the sticky-bins kernel for device-resident input.
+static bool runs_ws(int D, Persist model) { return D == 8 && model == Persist::kLean; }
+static bool sticky_eligible(int D, Persist model, bool streamed) { return runs_ws(D, model) && !streamed; }
 
 // Which persistent kernel a fit runs and how it splits a bin-iteration (pure host logic).  sms: SMs of the device;
 // clusters: sticky-kernel clusters of 1, 2, 4 CTAs the device runs at once, read only when sticky_eligible.
-static FitPlan plan_persistent_fit(int F, int T, int D, int K, bool lean, bool streamed, int sms,
-                                   const int* clusters, const Tuning& o) {
-  if (sticky_eligible(D, lean, streamed, o)) {
-    const int S = choose_sticky(F, T, clusters, o.sticky);
+static FitPlan plan_persistent_fit(int F, int T, int D, int K, Persist model, bool streamed, int sms,
+                                   const int* clusters) {
+  if (sticky_eligible(D, model, streamed)) {
+    const int S = choose_sticky(F, T, clusters);
     if (S > 0) return {kKernelSticky, S};
   }
-  const int kernel = D == 8 && lean && !o.single ? kKernelWs : kKernelSingle;
-  return {kernel, choose_frame_split(F, T, D, K, persist_ctas_per_sm(D, !lean), sms, o.tsplit)};
+  return {runs_ws(D, model) ? kKernelWs : kKernelSingle,
+          choose_frame_split(F, T, D, K, persist_ctas_per_sm(D, model == Persist::kFull), sms)};
 }
 
 static int device_sms(int* sms) {
@@ -633,16 +602,13 @@ static int launch_persistent_generic(Kern kern, int threads, size_t smem, int* c
   return 0;
 }
 
-// full = saliency / activity mask / log-domain softmax; lean = product-form softmax, 2 frames per lane;
-// ws = the warp-specialised em_ws_kernel (D = 8, lean) instead of the single-role kernel;
-// cw = complex Watson EM (lean structure, MODEL = 1)
-enum class Persist { kFull, kLean, kWs, kCw };
-
+// The task kernel of a model: em_ws_kernel for the lean D = 8 model (the warp-specialised kernel), otherwise
+// em_persistent_kernel.
 static int launch_persist(const PersistArgs& a, int D, int K, int dtype, Persist v, cudaStream_t st) {
   return with_d_k_ct(D, K, dtype, [&](auto d, auto k, auto ct) {
     constexpr int Dc = decltype(d)::value, Kc = decltype(k)::value;
     using CT = decltype(ct);
-    static int cache[4] = {0, 0, 0, 0};  // occupancy per Persist, queried on the first launch
+    static int cache[3] = {0, 0, 0};  // occupancy per Persist, queried on the first launch
     const int threads = persist_threads(Dc, Kc);
     const size_t smem = sizeof(PersistSmem<Dc, Kc, CT>);
     int* c = &cache[(int)v];
@@ -653,18 +619,16 @@ static int launch_persist(const PersistArgs& a, int D, int K, int dtype, Persist
     if (v == Persist::kCw)
       return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false, 1>, threads, smem, c, a,
                                        "em_persistent_kernel_cw", st);
-    if constexpr (Dc == 8) {
-      if (v == Persist::kWs)
-        return launch_persistent_generic(em_ws_kernel<Kc, CT>, 256, sizeof(WsSmem<Dc, Kc, CT>), c, a, "em_ws_kernel",
-                                         st);
-    }
-    return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false>, threads, smem,
-                                     &cache[(int)Persist::kLean], a, "em_persistent_kernel", st);
+    if constexpr (Dc == 8)
+      return launch_persistent_generic(em_ws_kernel<Kc, CT>, 256, sizeof(WsSmem<Dc, Kc, CT>), c, a, "em_ws_kernel", st);
+    else
+      return launch_persistent_generic(em_persistent_kernel<Dc, Kc, CT, false>, threads, smem, c, a,
+                                       "em_persistent_kernel", st);
   });
 }
 
 // "Sticky bins" (em_sticky.cuh): when the device runs F clusters of S CTAs at once, a cluster keeps one bin for the
-// whole fit (choose_sticky).  PBB_STICKY=0 disables it, PBB_STICKY=S forces a cluster size (A/B).
+// whole fit (choose_sticky).
 // Clusters of 1, 2, 4 CTAs of em_sticky_kernel the device runs at once (queried once per instantiation).
 static int sticky_clusters(int K, int dtype, int clusters[3], cudaStream_t st) {
   return with_k_ct(K, dtype, [&](auto k, auto ct) {
@@ -701,19 +665,17 @@ struct LastPlan { int kernel, split, variant; };
 static thread_local LastPlan g_last_plan = {-1, 0, -1};
 
 // Plan and launch of a persistent fit whose control block is clear: the sticky-bins kernel when the plan picks it,
-// otherwise the frame split and the task kernel.  model: kFull, kLean or kCw (always the single-role kernel).
+// otherwise the frame split and the task kernel.
 static int launch_planned(PersistArgs p, const CacgmmWorkspace& ws, int D, int K, int dtype, Persist model,
-                          bool streamed, Tuning tu, cudaStream_t st) {
-  if (model == Persist::kCw) tu.single = true;
-  const bool lean = model != Persist::kFull;
+                          bool streamed, cudaStream_t st) {
   int clusters[3] = {0, 0, 0}, sms = 0, r;
-  if (sticky_eligible(D, lean, streamed, tu) && (r = sticky_clusters(K, dtype, clusters, st))) return r;
+  if (sticky_eligible(D, model, streamed) && (r = sticky_clusters(K, dtype, clusters, st))) return r;
   if ((r = device_sms(&sms))) return r;
-  const FitPlan plan = plan_persistent_fit(p.F, p.T, D, K, lean, streamed, sms, clusters, tu);
-  g_last_plan = {plan.kernel, plan.split, model == Persist::kCw ? 3 : (lean ? 0 : (p.softmax_fast ? 1 : 2))};
+  const FitPlan plan = plan_persistent_fit(p.F, p.T, D, K, model, streamed, sms, clusters);
+  g_last_plan = {plan.kernel, plan.split,
+                 model == Persist::kCw ? 3 : (model == Persist::kLean ? 0 : (p.softmax_fast ? 1 : 2))};
   if (plan.kernel == kKernelSticky) return launch_sticky(p, K, dtype, plan.split, st);  // few bins: one cluster per bin
   if ((r = setup_frame_split(&p, ws, p.F, D, K, plan.split, st))) return r;
-  if (plan.kernel == kKernelWs) model = Persist::kWs;
   return launch_persist(p, D, K, dtype, model, st);
 }
 
@@ -803,7 +765,7 @@ static int resolve_host_aliases(FitCall& c) {
 // Streamed upload: on the persistent path with a host-resident y and an affiliation initialisation, a separate
 // small kernel on a side stream reads them over PCIe into the staged layout while the EM kernel runs.  Clears the
 // control block (flags[bin] = -1 until the bin has arrived) and fills the upload fields of p.
-static int start_streamed_upload(FitCall& c, LoadStream& l, const Tuning& tu, PersistArgs* p) {
+static int start_streamed_upload(FitCall& c, LoadStream& l, PersistArgs* p) {
   const CacgmmWorkspace& ws = c.ws;
   const int F = c.F, T = c.T, D = c.D, K = c.K, iterations = c.opt->iterations;
   PBB_CUDA(cudaMemsetAsync(ws.flags, 0, ws.control_bytes, c.st));
@@ -811,7 +773,7 @@ static int start_streamed_upload(FitCall& c, LoadStream& l, const Tuning& tu, Pe
   PBB_CUDA(cudaMemsetAsync(ws.dead, 0, (size_t)F * sizeof(int), c.st));
   PBB_CUDA(cudaEventRecord(l.fork, c.st));
   PBB_CUDA(cudaStreamWaitEvent(l.stream, l.fork, 0));
-  const int ctas = std::min(tu.load_ctas > 0 ? tu.load_ctas : kLoadCtas, F);
+  const int ctas = std::min(kLoadCtas, F);
   if (int r = launch_stream_load(c.y, c.dtype, ws, c.init_aff, c.aff_host ? ws.aff_stage : nullptr, F, T, D, K, ctas,
                                  l.stream))
     return r;
@@ -830,14 +792,15 @@ static int start_streamed_upload(FitCall& c, LoadStream& l, const Tuning& tu, Pe
   // one slot of the order table = one link of a bin's dependency chain (task + update + staging
   // of the next model, ~23 us at D = 8, K = 3, T = 500), during which the machine runs ~1.6 tasks per CTA
   const double round_us = 23.0 * (T / 500.0) * (D * D / 64.0) * (K / 3.0);
-  int wave = tu.wave_c ? *tu.wave_c : (int)(round_us / (bin_bytes / 50e3) + 0.5);
+  int wave = (int)(round_us / (bin_bytes / 50e3) + 0.5);
   wave = wave < 1 ? 1 : (wave > F ? F : wave);
   p->wave_c = wave;
   p->wait_load = 1;
-  if ((long long)F * iterations <= kMaxOrder && F <= 4096 && iterations < 32768 && tu.order) {
+  // the explicit task order where the table stays small; beyond that decode_ticket's rounds of wave_c bins
+  if ((long long)F * iterations <= kMaxOrder && F <= 4096 && iterations < 32768) {
     int sms = 0;
     if (int r = device_sms(&sms)) return r;
-    const int cap = tu.order_cap ? *tu.order_cap : (int)(1.6 * (2 * sms - kLoadReserve));
+    const int cap = (int)(1.6 * (2 * sms - kLoadReserve));
     if (int r = streamed_order(F, iterations, wave, cap < 1 ? 1 : cap, &p->order)) return r;
   }
   return 0;
@@ -846,8 +809,7 @@ static int start_streamed_upload(FitCall& c, LoadStream& l, const Tuning& tu, Pe
 // Persistent fit: every EM iteration in one launch (em_persistent.cuh), then the last iteration's raw scatter sums
 // through cacg_update_kernel for the reference-exact model.  p carries the streamed-upload fields; load is the side
 // stream of a streamed upload (which has cleared the control block), else null.
-static int run_persistent_fit(const FitCall& c, PersistArgs p, bool full, bool fast_sm, const LoadStream* load,
-                              const Tuning& tu) {
+static int run_persistent_fit(const FitCall& c, PersistArgs p, bool full, bool fast_sm, const LoadStream* load) {
   const CacgmmWorkspace& ws = c.ws;
   const pbb_cacgmm_options* opt = c.opt;
   int r;
@@ -860,8 +822,7 @@ static int run_persistent_fit(const FitCall& c, PersistArgs p, bool full, bool f
   p.aff_eps = opt->affiliation_eps; p.eigenvalue_floor = opt->eigenvalue_floor;
   p.covariance_norm = opt->covariance_norm; p.weight_mode = opt->weight_mode;
   p.dead = ws.dead;
-  if ((r = launch_planned(p, ws, c.D, c.K, c.dtype, full ? Persist::kFull : Persist::kLean, load != nullptr, tu,
-                          c.st)))
+  if ((r = launch_planned(p, ws, c.D, c.K, c.dtype, full ? Persist::kFull : Persist::kLean, load != nullptr, c.st)))
     return r;
   if (load != nullptr) PBB_CUDA(cudaStreamWaitEvent(c.st, load->join, 0));
 #ifdef PBB_PHASE_TIMING
@@ -938,7 +899,8 @@ int pbb_em_dispatch(int F, int T, int D, int K, int lean, int streamed, int sms,
   PBB_CHECK_ARG(sms > 0, 7, "sms must be positive");
   PBB_CHECK_ARG(kernel != nullptr && split != nullptr, 8, "output is null");
   const int clusters[3] = {2 * sms, sms, sms / 2};  // machine model: two CTAs per SM, clusters placed anywhere
-  const FitPlan plan = plan_persistent_fit(F, T, D, K, lean != 0, streamed != 0, sms, clusters, Tuning{});
+  const FitPlan plan =
+      plan_persistent_fit(F, T, D, K, lean ? Persist::kLean : Persist::kFull, streamed != 0, sms, clusters);
   *kernel = plan.kernel;
   *split = plan.split;
   return 0;
@@ -979,6 +941,7 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
   PBB_CHECK_ARG(opt->iterations > 0, 10, "iterations must be positive (cacgmm.py:200)");
   PBB_CHECK_ARG(opt->covariance_norm >= 0 && opt->covariance_norm <= 2, 10, "bad covariance_norm");
   PBB_CHECK_ARG(opt->weight_mode == PBB_WEIGHT_TIME || opt->weight_mode == PBB_WEIGHT_CONST, 10, "bad weight_mode");
+  PBB_CHECK_ARG((opt->reserved & ~1) == 0, 10, "reserved: only bit 0 (multi-kernel path) is defined");
   PBB_CHECK_ARG(eigenvectors && eigenvalues && weight, 11, "model output is null");
   FitCall c{y, dtype, F, T, D, K, init_aff, saliency, activity, opt, eigenvectors, eigenvalues, weight, status,
             reinterpret_cast<cudaStream_t>(stream)};
@@ -993,17 +956,16 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
     if ((r = normalize(c.y, dtype, c.ws, F, T, D, false, c.st))) return r;
     return run_iterative_fit(c, fast_sm);
   }
-  const bool streamed = c.y_host && c.init_aff != nullptr && !(opt->reserved & 2);
+  const bool streamed = c.y_host && c.init_aff != nullptr;
   // lean variant: product-form softmax, needs (K-1) D log10(1/floor) < 290 (em_persistent.cuh).  The extra decade
   // per factor below is a margin kept as is: without it some fits (e.g. K = 4, D = 8 with floors between about 1e-12
   // and 1e-11) would move from the full variant to the lean one.
   const bool lean_ok = fast_sm && (K - 1) * D * (log10(1.0 / opt->eigenvalue_floor) + 1.0) < 290.0;
   const bool full = saliency != nullptr || activity != nullptr || !lean_ok || c.init_aff == nullptr;
-  const Tuning tu = read_tuning();
   PersistArgs p = persist_args(c.ws, F, T, opt->iterations, status);
   if (!streamed) {
     if ((r = normalize(c.y, dtype, c.ws, F, T, D, true, c.st))) return r;
-    return run_persistent_fit(c, p, full, fast_sm, nullptr, tu);
+    return run_persistent_fit(c, p, full, fast_sm, nullptr);
   }
   // Thread safety: the side stream and the fork / join events of the streamed upload exist once per device, so two
   // host threads enqueueing streamed fits on the same device are serialised from here to the end of the call
@@ -1011,8 +973,8 @@ int pbb_cacgmm_fit(const void* y, int dtype, int F, int T, int D, int K, const d
   LoadStream* load = nullptr;
   if ((r = get_load_stream(&load))) return r;
   std::lock_guard<std::mutex> stream_lock(load->mu);
-  if ((r = start_streamed_upload(c, *load, tu, &p))) return r;
-  return run_persistent_fit(c, p, full, fast_sm, load, tu);
+  if ((r = start_streamed_upload(c, *load, &p))) return r;
+  return run_persistent_fit(c, p, full, fast_sm, load);
 }
 
 int pbb_cacgmm_predict(const void* y, int dtype, int F, int T, int D, int K, const void* eigenvectors,
@@ -1116,7 +1078,7 @@ int pbb_cwmm_fit(const void* y, int dtype, int F, int T, int D, int K, const dou
     p.first_is_m = 1;
     p.aff_in = init_aff; p.weight_mode = weight_mode;
     p.spline = u.spline;
-    if ((r = launch_planned(p, ws, D, K, dtype, Persist::kCw, false, read_tuning(), st))) return r;
+    if ((r = launch_planned(p, ws, D, K, dtype, Persist::kCw, false, st))) return r;
 #ifdef PBB_PHASE_TIMING
     print_phases(ws, (long long)F * iterations, true, st);
 #endif

@@ -236,7 +236,6 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
         if (t < total) decode_task(a, t, S, order_entry(a, t, S), bin, it, part);
         const int c0 = part * nchunks / S, ncp = (part + 1) * nchunks / S - c0;  // this task's ring stages
         const bool mstep_only = a.first_is_m && it == 0;
-        const bool late_z = mstep_only && a.wait_load;  // streamed upload: the bin may not have arrived yet
         int issued = 0;  // chunks of this task already requested (lane 0)
         auto issue_chunks = [&](int upto, bool blocking) {
           // lane 0: request chunks [issued, upto) of this task; non-blocking stops at a busy stage
@@ -264,19 +263,27 @@ __global__ void __launch_bounds__(256, 2) em_ws_kernel(const PersistArgs a) {
           }
         };
         if (bin >= 0 && lane == 0) {
+          // streamed upload: the bin's observation is in place once flags[bin] >= 0 (stream_load_kernel), which a
+          // task of any iteration may see before; the staged rows were written with ordinary stores by another
+          // CTA, so order them before this CTA's async-proxy (TMA) reads
+          bool z_ready = !a.wait_load;
+          if (!z_ready && ld_acquire_gpu(a.flags + bin) >= 0) {
+            asm volatile("fence.proxy.async;" ::: "memory");
+            z_ready = true;
+          }
           // the observation does not depend on the model: request what fits into the ring right away, so
           // that the copy overlaps the flag / model round trips below
-          if (!late_z) issue_chunks(ncp, false);
+          if (z_ready) issue_chunks(ncp, false);
           // dependency: the bin's previous iteration (or its arrival, streamed upload)
           if (mstep_only) {
             if (a.wait_load) while (ld_acquire_gpu(a.flags + bin) < 0) __nanosleep(200);
           } else {
             while (ld_acquire_gpu(a.flags + bin) < it) {
-              issue_chunks(ncp, false);  // keep the ring filled while the dependency is still executing
+              if (z_ready) issue_chunks(ncp, false);  // keep the ring filled while the dependency is still executing
               __nanosleep(40);
             }
           }
-          if (late_z) asm volatile("fence.proxy.async;" ::: "memory");
+          if (!z_ready) asm volatile("fence.proxy.async;" ::: "memory");
         }
         __syncwarp();
         mbar_wait_relaxed(&sm.model_empty[mb], ((n >> 1) & 1u) ^ 1u, 100);  // EM warps are done with task n - 2

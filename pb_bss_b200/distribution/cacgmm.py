@@ -138,7 +138,6 @@ class CACGMMTrainer:
             inline_permutation_aligner=None,
             frames_per_block=0,
             multi_kernel=False,
-            streamed_upload=True,
             total_bins=None,
             bin_group=None,
     ):
@@ -156,9 +155,6 @@ class CACGMMTrainer:
             frames_per_block: tuning knob of the multi-kernel EM path (0 = default).
             multi_kernel: force the one-kernel-pair-per-iteration path instead
                 of the persistent kernel (A/B testing; same results).
-            streamed_upload: with ``y`` / ``initialization`` in pinned host memory (CPU
-                tensors after ``.pin_memory()``) the upload overlaps the EM iterations;
-                False reads them in one pass before the EM kernel starts (A/B testing).
             total_bins, bin_group: bin-sharded multi-GPU use (pb_bss_b200.parallel):
                 ``y`` holds this rank's contiguous slice of ``total_bins`` bins.  Only
                 the couplings across bins (frequency-tied weights, inline alignment)
@@ -258,7 +254,7 @@ class CACGMMTrainer:
             affiliation_eps=float(affiliation_eps),
             eigenvalue_floor=float(eigenvalue_floor),
             frames_per_block=int(frames_per_block),
-            reserved=(1 if multi_kernel else 0) | (0 if streamed_upload else 2))
+            reserved=1 if multi_kernel else 0)
         lib = _lib.load()
         nbytes = lib.pbb_cacgmm_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)

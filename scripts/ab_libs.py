@@ -1,11 +1,12 @@
 """A/B timing and bit check of the C2 fit for several builds of the library: python scripts/ab_libs.py lib1.so lib2.so ...
 
-For every build (PBB_LIB; 'default' = the package's own library) it times the C2 fit (F = 513, em_ws_kernel) and the
-F = 65 fit of scripts/one_fit_small.py (em_sticky_kernel), saves the fitted eigenvectors, eigenvalues and weights of
-both, and reports whether they are byte-identical to those of the first build.  Environment variables such as
-PBB_STICKY or PBB_TSPLIT pass through to every build."""
+For every build (PBB_LIB; 'default' = the package's own library) it times the C2 fit (F = 513, em_ws_kernel), the
+F = 65 fit of scripts/one_fit_small.py (em_sticky_kernel) and the C2 fit from pinned host memory (streamed upload),
+saves the fitted eigenvectors, eigenvalues and weights of each, and reports whether they are byte-identical to those
+of the first build.  The library picks each fit's kernel from the problem alone, so other kernels are compared
+through other shapes, not through settings."""
 import os, sys, subprocess, tempfile
-SHAPES = {'C2': 513, 'F65': 65}  # bins; T = 500, D = 8, K = 3, 100 iterations
+SHAPES = {'C2': (513, False), 'F65': (65, False), 'C2pinned': (513, True)}  # bins, pinned; T = 500, D = 8, K = 3
 if sys.argv[1] == 'child':
     import numpy as np, torch
     sys.path.insert(0, '.')
@@ -13,9 +14,10 @@ if sys.argv[1] == 'child':
     from pb_bss_b200.distribution import CACGMMTrainer
     T, D, K, I = 500, 8, 3, 100
     out, line = {}, os.environ.get('PBB_LIB', 'default')
-    for name, F in SHAPES.items():
-        y = torch.from_numpy(synth.noise_stft(F, T, D)).cuda()
-        init = torch.from_numpy(synth.init_affiliation(F, K, T)).cuda()
+    for name, (F, pinned) in SHAPES.items():
+        y = torch.from_numpy(synth.noise_stft(F, T, D))
+        init = torch.from_numpy(synth.init_affiliation(F, K, T))
+        y, init = (y.pin_memory(), init.pin_memory()) if pinned else (y.cuda(), init.cuda())
         tr = CACGMMTrainer()
         for _ in range(3): tr.fit(y, initialization=init, iterations=I)
         ts = []

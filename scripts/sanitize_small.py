@@ -5,11 +5,9 @@ sys.path.insert(0, '.')
 from oracle import synth
 from pb_bss_b200.distribution import CACGMMTrainer, CWMMTrainer
 y, _ = synth.structured_stft(12, 300, 8, 3, seed=1); init = synth.init_affiliation(12, 3, 300)
-import os
 m = CACGMMTrainer().fit(y, initialization=init, iterations=4); m.predict(y)   # few bins: em_sticky_kernel (clusters)
-os.environ['PBB_STICKY'] = '0'                                                # the task kernel em_ws_kernel
-CACGMMTrainer().fit(y, initialization=init, iterations=4)
-os.environ.pop('PBB_STICKY')
+yw, _ = synth.structured_stft(12, 2000, 8, 3, seed=5); iw = synth.init_affiliation(12, 3, 2000)
+CACGMMTrainer().fit(yw, initialization=iw, iterations=3)   # 16 ring stages per bin: the task kernel em_ws_kernel
 sal = np.random.RandomState(0).uniform(0.2, 1, size=(12, 300))
 CACGMMTrainer().fit(y, initialization=init, iterations=3, saliency=sal)
 y6, _ = synth.structured_stft(7, 260, 6, 4, seed=2); i6 = synth.init_affiliation(7, 4, 260)

@@ -41,9 +41,6 @@ def resident():
 init_d = init_pin.cuda()
 print('fit resident               %.3f ms' % timed(resident))
 print('fit e2e streamed upload    %.3f ms' % timed(e2e))
-def e2e_ns():
-    tr.fit(y_pin, initialization=init_pin, iterations=I, streamed_upload=False)
-print('fit e2e zero-copy, serial  %.3f ms' % timed(e2e_ns))
 def e2e_copy():
     tr.fit(y_pin.cuda(non_blocking=True), initialization=init_pin.cuda(non_blocking=True), iterations=I)
 print('fit e2e memcpy then fit    %.3f ms' % timed(e2e_copy))

@@ -57,6 +57,22 @@ def test_bad_arguments_are_rejected_before_any_launch():
         _lib.check(rc, 'pbb_cacgmm_fit')
 
 
+def test_unknown_reserved_bits_are_rejected():
+    """pbb_cacgmm_options.reserved: bit 0 selects the multi-kernel path, any other bit is an error of the options
+    (argument 10), found before any device work; 0 and 1 pass on to the next check, the null model outputs
+    (argument 11)."""
+    from pb_bss_b200 import _lib
+    lib = _lib.load()
+    for reserved, want in ((0, -11), (1, -11), (2, -10), (3, -10), (1 << 30, -10), (-1, -10)):
+        opts = _lib.CacgmmOptions(iterations=1, covariance_norm=1, weight_mode=0, hermitize=1, affiliation_eps=1e-10,
+                                  eigenvalue_floor=1e-10, frames_per_block=0, reserved=reserved)
+        rc = lib.pbb_cacgmm_fit(1, 1, 1, 1, 4, 2, None, None, None, ctypes.byref(opts),
+                                None, None, None, None, 0, None, None)
+        assert rc == want, (reserved, rc, lib.pbb_last_error())
+        if want == -10:
+            assert b'reserved' in lib.pbb_last_error()
+
+
 def test_no_cpu_fallback_without_gpu():
     import torch
     if torch.cuda.is_available():

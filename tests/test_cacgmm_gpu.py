@@ -10,6 +10,7 @@ import pytest
 from conftest import load_golden
 from oracle import pb_bss_oracle as O
 from oracle import synth
+from test_em_kernels_gpu import device_fit, last_plan
 
 pytestmark = pytest.mark.gpu
 
@@ -353,7 +354,7 @@ def test_inline_permutation_alignment_matches_reference_golden():
 @pytest.mark.parametrize('shape', [(129, 200, 4, 2, 20), (40, 333, 8, 3, 12), (7, 130, 6, 4, 5), (3, 50, 8, 2, 3),
                                    (65, 257, 8, 4, 1)])
 @pytest.mark.parametrize('cdtype', ['complex128', 'complex64'])
-def test_pinned_host_inputs_stream_in_and_match_device_inputs(shape, cdtype):
+def test_pinned_host_inputs_match_device_inputs(shape, cdtype):
     """y / initialization in pinned host memory are read in place over PCIe by a loader kernel that
     overlaps the EM kernel (wave task order).  Every task computes exactly what it computes with
     device-resident inputs, so the models must be bit-identical."""
@@ -366,13 +367,12 @@ def test_pinned_host_inputs_stream_in_and_match_device_inputs(shape, cdtype):
     init = synth.init_affiliation(F, K, T, seed=7)
     y_pin, init_pin = torch.from_numpy(y).pin_memory(), torch.from_numpy(init).pin_memory()
     ref = CACGMMTrainer().fit(y_pin.cuda(), initialization=init_pin.cuda(), iterations=iters)
-    for kw in ({}, {'streamed_upload': False}):
-        got = CACGMMTrainer().fit(y_pin, initialization=init_pin, iterations=iters, **kw)
-        # pinned observation in -> the model is written to pinned host memory as well
-        assert not got.weight.is_cuda and got.weight.is_pinned()
-        assert torch.equal(got.weight, ref.weight.cpu()), kw
-        assert torch.equal(got.cacg.covariance_eigenvalues, ref.cacg.covariance_eigenvalues.cpu()), kw
-        assert torch.equal(got.cacg.covariance_eigenvectors, ref.cacg.covariance_eigenvectors.cpu()), kw
+    got = CACGMMTrainer().fit(y_pin, initialization=init_pin, iterations=iters)
+    # pinned observation in -> the model is written to pinned host memory as well
+    assert not got.weight.is_cuda and got.weight.is_pinned()
+    assert torch.equal(got.weight, ref.weight.cpu())
+    assert torch.equal(got.cacg.covariance_eigenvalues, ref.cacg.covariance_eigenvalues.cpu())
+    assert torch.equal(got.cacg.covariance_eigenvectors, ref.cacg.covariance_eigenvectors.cpu())
     # pinned observation, device initialisation; and a warm start from pinned memory
     got = CACGMMTrainer().fit(y_pin, initialization=init_pin.cuda(), iterations=iters)
     assert torch.equal(got.cacg.covariance_eigenvalues, ref.cacg.covariance_eigenvalues.cpu())
@@ -383,80 +383,65 @@ def test_pinned_host_inputs_stream_in_and_match_device_inputs(shape, cdtype):
     np.testing.assert_array_equal(got.predict(y_pin.cuda()).cpu().numpy(), ref.predict(y_pin.cuda()).cpu().numpy())
 
 
-def test_warp_specialised_and_single_role_kernels_agree(tmp_path):
-    """D = 8 fits run on em_ws_kernel (producer / EM / update warps); PBB_EM_KERNEL=single selects the single-role
-    persistent kernel."""
-    import os
-    import subprocess
-    import sys
-    code = (
-        "import sys, numpy as np\n"
-        "sys.path.insert(0, %r)\n"
-        "from oracle import synth\n"
-        "from pb_bss_b200.distribution import CACGMMTrainer\n"
-        "out = {}\n"
-        "for (F, T, K, I) in ((21, 333, 3, 9), (10, 128, 2, 5), (6, 500, 4, 4)):\n"
-        "    y, _ = synth.structured_stft(F, T, 8, K, seed=3)\n"
-        "    m = CACGMMTrainer().fit(y, initialization=synth.init_affiliation(F, K, T, seed=7), iterations=I)\n"
-        "    out['w%%d' %% K] = m.weight; out['c%%d' %% K] = m.cacg.covariance\n"
-        "np.savez(sys.argv[1], **out)\n" % os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    res = {}
-    for tag, env in (('ws', {}), ('single', {'PBB_EM_KERNEL': 'single'})):
-        path = str(tmp_path / f'{tag}.npz')
-        e = dict(os.environ)
-        e.update(env)
-        subprocess.run([sys.executable, '-c', code, path], check=True, env=e, timeout=300)
-        res[tag] = np.load(path)
-    for k in res['ws'].files:
-        np.testing.assert_allclose(res['ws'][k], res['single'][k], rtol=1e-10, atol=1e-13)
+def _check_fit(m, ref):
+    cov_ref = np.einsum('...de,...e,...fe->...df', ref['eigenvectors'], ref['eigenvalues'], ref['eigenvectors'].conj())
+    np.testing.assert_allclose(m.weight, ref['weight'], rtol=0, atol=1e-9)
+    np.testing.assert_allclose(m.cacg.covariance, cov_ref, rtol=0, atol=1e-8)
 
 
-@pytest.mark.parametrize('S', [2, 3, 4])
-def test_frame_split_of_a_bin_over_several_ctas(monkeypatch, S):
-    """em_ws_kernel with few bins: one EM iteration of a bin is split over S CTAs by ring stage (em_ws.cuh, "frame
-    split").  Whatever S, the result matches the oracle; and it is deterministic (partial sums added in part order)."""
-    import torch
-    from pb_bss_b200.distribution import CACGMMTrainer
-    monkeypatch.setenv('PBB_TSPLIT', str(S))
-    for (F, T, K, I) in ((5, 500, 3, 12), (9, 290, 2, 7), (3, 1100, 4, 5), (2, 129, 3, 4), (1, 512, 3, 6)):
+def _same_model(a, b):
+    return (np.array_equal(a.cacg.covariance_eigenvectors, b.cacg.covariance_eigenvectors)
+            and np.array_equal(a.cacg.covariance_eigenvalues, b.cacg.covariance_eigenvalues)
+            and np.array_equal(a.weight, b.weight))
+
+
+# D = 8, lean: (F, T, K, I, pinned host input) for which em_ws_kernel runs with the frame split S
+WS_SPLIT_CASES = {
+    1: [(300, 200, 3, 6, False), (300, 129, 2, 4, False), (2, 129, 3, 4, True)],
+    2: [(9, 290, 2, 7, True), (5, 350, 3, 12, True)],
+    4: [(5, 500, 3, 12, True), (3, 1100, 4, 5, True), (1, 512, 3, 6, True)],
+}
+
+
+@pytest.mark.parametrize('S', [1, 2, 4])
+def test_ws_kernel_frame_split_picked_by_the_library(S):
+    """em_ws_kernel: one EM iteration of a bin is split over the S CTAs the library picks, by ring stage (em_ws.cuh,
+    "frame split").  S = 1 runs device-resident input with more bins than sticky-bins clusters fit, and pinned host
+    input with a short sweep; S = 2 and 4 run pinned host input with few bins (the streamed upload never runs the
+    sticky-bins kernel).  Whatever S, the result matches the oracle; and it is deterministic (partial sums added in
+    part order)."""
+    for F, T, K, I, pinned in WS_SPLIT_CASES[S]:
         y, _ = synth.structured_stft(F, T, 8, K, seed=11)
         init = synth.init_affiliation(F, K, T, seed=5)
-        ref = O.cacgmm_fit(y, init, I)
-        m = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-        cov_ref = np.einsum('...de,...e,...fe->...df', ref['eigenvectors'], ref['eigenvalues'], ref['eigenvectors'].conj())
-        np.testing.assert_allclose(m.weight, ref['weight'], rtol=0, atol=1e-9)
-        np.testing.assert_allclose(m.cacg.covariance, cov_ref, rtol=0, atol=1e-8)
-        m2 = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-        assert np.array_equal(m.cacg.covariance, m2.cacg.covariance) and np.array_equal(m.weight, m2.weight)
-        # pinned host input: streamed upload with an explicit task order
-        mp = CACGMMTrainer().fit(torch.from_numpy(y).pin_memory(), initialization=torch.from_numpy(init).pin_memory(),
-                                 iterations=I)
-        np.testing.assert_allclose(mp.weight.numpy(), m.weight, rtol=0, atol=1e-12)
-    monkeypatch.setenv('PBB_TSPLIT', '1')
-    m1 = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-    np.testing.assert_allclose(m1.cacg.covariance, m.cacg.covariance, rtol=1e-9, atol=1e-12)
+        m = device_fit(y, init, I, pinned=pinned)
+        assert last_plan() == (0, S, 0), (F, T, last_plan())
+        _check_fit(m, O.cacgmm_fit(y, init, I))
+        assert _same_model(m, device_fit(y, init, I, pinned=pinned))
 
 
-@pytest.mark.parametrize('S', [2, 4])
-@pytest.mark.parametrize('D,K', [(6, 4), (4, 2), (4, 3), (8, 3)])
-@pytest.mark.parametrize('variant', ['lean', 'saliency'])
-def test_frame_split_on_the_single_role_kernel(monkeypatch, S, D, K, variant):
-    """Frame split in em_persistent_kernel (D = 4 / 6, and the full variant with saliency at any D)."""
-    from pb_bss_b200.distribution import CACGMMTrainer
-    monkeypatch.setenv('PBB_TSPLIT', str(S))
-    F, T, I = 4, 530, 6
+# the single-role kernel (em_persistent_kernel) at F = 4: the T at which the library splits a bin-iteration into
+# S = 1, 2, 4 parts (the sweep T D^2 (K + 1) must pay for each part, choose_frame_split)
+SINGLE_ROLE_T = {(6, 4): {1: 200, 2: 385, 4: 600}, (4, 2): {1: 530, 2: 1500, 4: 2100},
+                 (4, 3): {1: 530, 2: 1000, 4: 1600}, (8, 3): {1: 150, 2: 300, 4: 530}}
+
+
+@pytest.mark.parametrize('S', [1, 2, 4])
+@pytest.mark.parametrize('D,K,variant', [(6, 4, 'lean'), (4, 2, 'lean'), (4, 3, 'lean'), (6, 4, 'saliency'),
+                                         (4, 2, 'saliency'), (4, 3, 'saliency'), (8, 3, 'saliency')])
+def test_frame_split_on_the_single_role_kernel(S, D, K, variant):
+    """Frame split in em_persistent_kernel (lean D = 4 / 6, and the full variant with saliency at any D), at each split
+    the library picks."""
+    F, I = 4, 6
+    T = SINGLE_ROLE_T[D, K][S]
     y, _ = synth.structured_stft(F, T, D, K, seed=21)
     init = synth.init_affiliation(F, K, T, seed=3)
     sal = None
     if variant == 'saliency':
         sal = np.random.default_rng(4).uniform(0.2, 1.0, size=(F, T))
-    ref = O.cacgmm_fit(y, init, I, saliency=sal)
-    m = CACGMMTrainer().fit(y, initialization=init, iterations=I, saliency=sal)
-    cov_ref = np.einsum('...de,...e,...fe->...df', ref['eigenvectors'], ref['eigenvalues'], ref['eigenvectors'].conj())
-    np.testing.assert_allclose(m.weight, ref['weight'], rtol=0, atol=1e-9)
-    np.testing.assert_allclose(m.cacg.covariance, cov_ref, rtol=0, atol=1e-8)
-    m2 = CACGMMTrainer().fit(y, initialization=init, iterations=I, saliency=sal)
-    assert np.array_equal(m.cacg.covariance, m2.cacg.covariance)
+    m = device_fit(y, init, I, saliency=sal)
+    assert last_plan() == (2, S, 0 if sal is None else 1), (T, last_plan())
+    _check_fit(m, O.cacgmm_fit(y, init, I, saliency=sal))
+    assert _same_model(m, device_fit(y, init, I, saliency=sal))
 
 
 def test_time_varying_weight_needs_matching_frame_count():
@@ -472,29 +457,28 @@ def test_time_varying_weight_needs_matching_frame_count():
         m.predict(y2)
 
 
+# D = 8, lean, few bins: (F, T, K, I) for which device-resident input runs em_sticky_kernel with clusters of S CTAs
+STICKY_CASES = {
+    1: [(5, 100, 3, 12), (3, 128, 2, 6), (7, 97, 4, 5)],
+    2: [(5, 350, 3, 12), (3, 256, 2, 6), (7, 300, 4, 5), (2, 383, 3, 1)],
+    4: [(5, 500, 3, 12), (3, 512, 2, 6), (7, 1000, 4, 5), (2, 1100, 3, 1)],
+}
+
+
 @pytest.mark.parametrize('S', [1, 2, 4])
-def test_sticky_bins_kernel_matches_the_task_kernel_bit_for_bit(monkeypatch, S):
+def test_sticky_bins_kernel_matches_the_task_kernel_bit_for_bit(S):
     """em_sticky_kernel (one cluster of S CTAs per bin for the whole fit, few bins) sums the parts in the same order
-    as em_ws_kernel with the frame split S: identical models; and both match the oracle."""
-    from pb_bss_b200.distribution import CACGMMTrainer
-    for (F, T, K, I) in ((5, 350, 3, 12), (3, 128 * S, 2, 6), (7, 300, 4, 5), (2, 383, 3, 1)):
-        if (T + 127) // 128 < S:
-            continue
+    as em_ws_kernel with the frame split S, which the same fit from pinned host memory runs: identical models; and
+    both match the oracle."""
+    for F, T, K, I in STICKY_CASES[S]:
         y, _ = synth.structured_stft(F, T, 8, K, seed=31)
         init = synth.init_affiliation(F, K, T, seed=9)
-        monkeypatch.setenv('PBB_STICKY', str(S))
-        m = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-        monkeypatch.setenv('PBB_STICKY', '0')
-        monkeypatch.setenv('PBB_TSPLIT', str(S))
-        mt = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-        monkeypatch.delenv('PBB_TSPLIT')
-        assert np.array_equal(m.cacg.covariance_eigenvectors, mt.cacg.covariance_eigenvectors)
-        assert np.array_equal(m.cacg.covariance_eigenvalues, mt.cacg.covariance_eigenvalues)
-        assert np.array_equal(m.weight, mt.weight)
-        ref = O.cacgmm_fit(y, init, I)
-        cov_ref = np.einsum('...de,...e,...fe->...df', ref['eigenvectors'], ref['eigenvalues'], ref['eigenvectors'].conj())
-        np.testing.assert_allclose(m.weight, ref['weight'], rtol=0, atol=1e-9)
-        np.testing.assert_allclose(m.cacg.covariance, cov_ref, rtol=0, atol=1e-8)
+        m = device_fit(y, init, I)
+        assert last_plan() == (1, S, 0), (F, T, last_plan())
+        mt = device_fit(y, init, I, pinned=True)
+        assert last_plan() == (0, S, 0), (F, T, last_plan())
+        assert _same_model(m, mt)
+        _check_fit(m, O.cacgmm_fit(y, init, I))
 
 
 def test_argument_errors():

@@ -7,6 +7,7 @@ import pytest
 from conftest import load_golden, cos_similarity
 from oracle import pb_bss_oracle as O
 from oracle import synth
+from test_em_kernels_gpu import last_plan
 
 pytestmark = pytest.mark.gpu
 
@@ -62,16 +63,22 @@ def test_fit_matches_oracle(F, T, D, K, I):
     np.testing.assert_allclose(model.predict(y), O.cwmm_predict(y, ref), rtol=1e-5, atol=1e-8)
 
 
-@pytest.mark.parametrize('S', [2, 4])
-@pytest.mark.parametrize('F,T,D,K,I', [(5, 600, 6, 4, 6), (3, 515, 8, 3, 5), (4, 300, 4, 2, 5)])
-def test_frame_split_matches_oracle(monkeypatch, S, F, T, D, K, I):
-    """One EM iteration of a bin split over S CTAs (em_persistent.cuh, "frame split"): same model as the oracle."""
+# the T at which the library splits one bin-iteration of the complex Watson fit into S = 1, 2, 4 parts
+CW_SPLIT_T = {(6, 4): {1: 200, 2: 400, 4: 600}, (8, 3): {1: 150, 2: 300, 4: 515}, (4, 2): {1: 300, 2: 1200, 4: 2100}}
+
+
+@pytest.mark.parametrize('S', [1, 2, 4])
+@pytest.mark.parametrize('F,D,K,I', [(5, 6, 4, 6), (3, 8, 3, 5), (4, 4, 2, 5)])
+def test_frame_split_matches_oracle(F, D, K, I, S):
+    """One EM iteration of a bin split over the S CTAs the library picks (em_persistent.cuh, "frame split"): same
+    model as the oracle, and deterministic."""
     from pb_bss_b200.distribution import CWMMTrainer
-    monkeypatch.setenv('PBB_TSPLIT', str(S))
+    T = CW_SPLIT_T[D, K][S]
     y, _ = synth.structured_stft(F, T, D, K, seed=F * T)
     init = synth.init_affiliation(F, K, T, seed=K)
     ref = O.cwmm_fit(y, init, I)
     model = CWMMTrainer().fit(y, initialization=init, iterations=I)
+    assert last_plan() == (2, S, 3), (T, last_plan())
     np.testing.assert_allclose(model.weight, ref['weight'], rtol=1e-6, atol=1e-9)
     np.testing.assert_allclose(model.complex_watson.concentration, ref['concentration'], rtol=1e-6)
     np.testing.assert_allclose(cos_similarity(model.complex_watson.mode, ref['mode']), 1, atol=1e-9)

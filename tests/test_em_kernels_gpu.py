@@ -16,7 +16,6 @@ Tolerances are derived from error scales, not flat (DESIGN.md section 3):
   only accurate to cond eps relative.
 """
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -30,7 +29,6 @@ from oracle import synth
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EPS = np.finfo(np.float64).eps
 UNIT = {'complex128': 2.0 ** -53, 'complex64': 2.0 ** -24}
 FAST = [(D, K) for D in (4, 6, 8) for K in (2, 3, 4)]
@@ -70,8 +68,28 @@ def last_plan():
     return k.value, s.value, v.value
 
 
-def _nchunks(T):
-    return ((T + 31) // 32 * 32 + 127) // 128
+def dispatch(F, T, D, K, lean, streamed):
+    """(kernel, split) of pbb_em_dispatch on this GPU's SM count: the plan pbb_cacgmm_fit picks, as long as it picks
+    no sticky-bins clusters (which the fit counts on the device)."""
+    import ctypes
+    import torch
+    from pb_bss_b200 import _lib
+    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    k, s = ctypes.c_int(), ctypes.c_int()
+    _lib.check(_lib.load().pbb_em_dispatch(F, T, D, K, int(lean), int(streamed), sms, ctypes.byref(k),
+                                           ctypes.byref(s)), 'pbb_em_dispatch')
+    return k.value, s.value
+
+
+def device_fit(y, init, iterations, pinned=False, **kw):
+    """CACGMMTrainer().fit of NumPy y / init, or (pinned) of pinned host copies of them, which the library streams in
+    while it computes; the model with NumPy arrays."""
+    import torch
+    from pb_bss_b200.distribution import CACGMMTrainer
+    from pb_bss_b200.distribution.mixture_model_utils import model_to_host
+    if pinned:
+        y, init = torch.from_numpy(y).pin_memory(), torch.from_numpy(init).pin_memory()
+    return model_to_host(CACGMMTrainer().fit(y, initialization=init, iterations=iterations, **kw))
 
 
 class Launches:
@@ -94,19 +112,6 @@ class Launches:
 
     def __contains__(self, name):
         return name in self.names
-
-
-def _in_subprocess(tmp_path, env, child, *args):
-    """Runs _child_<child>(out, *args) of this module in a fresh interpreter with `env` added (for the settings
-    read once per process, PBB_EM_KERNEL) and returns its saved arrays."""
-    out = str(tmp_path / f'{child}.npz')
-    code = ('import sys; sys.path[:0] = [%r, %r]; import test_em_kernels_gpu as t; t._child_%s(*sys.argv[1:])'
-            % (ROOT, os.path.join(ROOT, 'tests'), child))
-    e = dict(os.environ)
-    e.update(env)
-    subprocess.run([sys.executable, '-c', code, out, *map(str, args)], check=True, env=e, timeout=600)
-    with np.load(out) as f:
-        return {k: f[k] for k in f.files}
 
 
 def _rand_model(F, K, D, seed, lam_min=0.05):
@@ -306,80 +311,56 @@ def test_persistent_kernels_match_oracle(D, K, variant, cdtype):
         check_model(m, ref, atol=tol, rtol=1e-5)
 
 
-def _d8_cases():
-    return [(5, 350, 3, 8), (3, 257, 2, 2), (2, 385, 4, 1), (4, 128, 3, 5), (2, 1000, 2, 8)]
+# D = 8, lean: (F, T, K, I, pinned host input, the plan the library picks: kernel, split)
+D8_CASES = [
+    (4, 128, 3, 5, False, (1, 1)),    # one ring stage: sticky bins, clusters of 1 CTA
+    (5, 350, 3, 8, False, (1, 2)),    # three stages: clusters of 2
+    (3, 257, 2, 2, False, (1, 2)),
+    (2, 385, 4, 1, False, (1, 4)),    # four stages: clusters of 4
+    (2, 1000, 2, 8, False, (1, 4)),
+    (300, 200, 3, 3, False, (0, 1)),  # more bins than clusters run at once: em_ws_kernel, no frame split
+    (2, 2100, 3, 2, False, (0, 4)),   # 17 stages: a part does not fit the ring of a sticky CTA
+    (5, 350, 3, 8, True, (0, 2)),     # pinned host input (streamed upload): em_ws_kernel with the frame split
+]
 
 
-def _child_single_role(out):
-    """PBB_EM_KERNEL=single: the D = 8 lean fits on em_persistent_kernel; saves models and launch names."""
-    from pb_bss_b200.distribution import CACGMMTrainer
-    res = {}
-    for F, T, K, I in _d8_cases():
-        y, _ = synth.structured_stft(F, T, 8, K, seed=T)
-        with Launches() as rec:
-            m = CACGMMTrainer().fit(y, initialization=synth.init_affiliation(F, K, T, seed=I), iterations=I)
-        res[f'w_{T}'], res[f'c_{T}'] = m.weight, m.cacg.covariance
-        res[f'names_{T}'] = np.array(','.join(rec.names))
-    np.savez(out, **res)
-
-
-def test_d8_kernels_match_oracle(tmp_path, monkeypatch):
-    """D = 8: em_ws_kernel (no sticky bins), the single-role kernel (a process with PBB_EM_KERNEL=single) and
-    em_sticky_kernel with clusters of 1, 2 and 4 CTAs, each against the oracle."""
-    from pb_bss_b200.distribution import CACGMMTrainer
-    single = _in_subprocess(tmp_path, {'PBB_EM_KERNEL': 'single', 'PBB_STICKY': '0'}, 'single_role')
-    ran_sticky = 0
-    for F, T, K, I in _d8_cases():
+def test_d8_plans_match_oracle():
+    """D = 8: every plan the library picks for the lean fit -- em_sticky_kernel with clusters of 1, 2 and 4 CTAs,
+    em_ws_kernel without and with the frame split -- each against the oracle."""
+    for F, T, K, I, pinned, plan in D8_CASES:
         y, _ = synth.structured_stft(F, T, 8, K, seed=T)
         init = synth.init_affiliation(F, K, T, seed=I)
-        ref = O.cacgmm_fit(y, init, I)
-        cov_ref = O.cacg_covariance_from_eig(ref['eigenvectors'], ref['eigenvalues'])
-        names = str(single[f'names_{T}']).split(',')
-        assert 'em_persistent_kernel' in names and 'em_ws_kernel' not in names, names
-        np.testing.assert_allclose(single[f'w_{T}'], ref['weight'], rtol=1e-6, atol=1e-9)
-        np.testing.assert_allclose(single[f'c_{T}'], cov_ref, rtol=1e-6, atol=1e-9)
-        monkeypatch.setenv('PBB_STICKY', '0')
         with Launches() as rec:
-            m = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-        assert 'em_ws_kernel' in rec and 'em_sticky_kernel' not in rec, rec.names
-        check_model(m, ref, atol=1e-9, rtol=1e-6)
-        for S in (1, 2, 4):
-            if _nchunks(T) < S:
-                continue
-            monkeypatch.setenv('PBB_STICKY', str(S))
-            with Launches() as rec:
-                m = CACGMMTrainer().fit(y, initialization=init, iterations=I)
-            # PBB_STICKY=S: clusters of S CTAs whenever every part fits the 3-stage ring (choose_sticky), else em_ws
-            sticky = S <= _nchunks(T) and -(-_nchunks(T) // S) <= 3
-            if sticky:
-                assert 'em_sticky_kernel' in rec and 'em_ws_kernel' not in rec, (T, S, rec.names)
-                assert last_plan()[:2] == (1, S)
-            else:
-                assert 'em_ws_kernel' in rec and 'em_sticky_kernel' not in rec, (T, S, rec.names)
-            ran_sticky += sticky
-            check_model(m, ref, atol=1e-9, rtol=1e-6)
-        monkeypatch.delenv('PBB_STICKY')
-    assert ran_sticky >= 8, ran_sticky
+            m = device_fit(y, init, I, pinned=pinned)
+        ran = 'em_sticky_kernel' if plan[0] == 1 else 'em_ws_kernel'
+        assert ran in rec and not set(rec.names) & (LEAN_NAMES - {ran}), (F, T, rec.names)
+        assert last_plan() == (*plan, 0), (F, T, last_plan())
+        check_model(m, O.cacgmm_fit(y, init, I), atol=1e-9, rtol=1e-6)
 
 
-@pytest.mark.parametrize('S', [2, 3, 4])
+# frame lengths among which every persistent shape finds each frame split the library picks at F = 2
+SPLIT_T = [129, 200, 257, 300, 385, 500, 1000, 1500, 2100]
+
+
+@pytest.mark.parametrize('S', [1, 2, 4])
 @pytest.mark.parametrize('D,K', FAST)
-def test_frame_split_all_shapes(monkeypatch, D, K, S):
-    """PBB_TSPLIT = 2, 3, 4 on every persistent shape, lean and full, where the 128-frame chunks allow it."""
-    from pb_bss_b200.distribution import CACGMMTrainer
-    monkeypatch.setenv('PBB_STICKY', '0')
-    monkeypatch.setenv('PBB_TSPLIT', str(S))
+def test_frame_split_picked_for_every_shape(D, K, S):
+    """Every persistent shape, lean and full, at each frame split S the library picks: the first two T of SPLIT_T for
+    which pbb_em_dispatch reports S, and the fit must run the plan it reports.  The lean D = 8 fit reads pinned host
+    input, so that it runs em_ws_kernel rather than the sticky-bins kernel."""
     F, I = 2, 4
-    for T in (128 * S, 128 * S + 1, 1000):
+    ts = [T for T in SPLIT_T if dispatch(F, T, D, K, lean=True, streamed=True)[1] == S][:2]
+    assert ts, (D, K, S)
+    for T in ts:
         y, _ = synth.structured_stft(F, T, D, K, seed=T + S)
         init = synth.init_affiliation(F, K, T, seed=S)
         for sal in (None, np.random.default_rng(T).uniform(0.2, 1.0, size=(F, T))):
-            ref = O.cacgmm_fit(y, init, I, saliency=sal)
-            m = CACGMMTrainer().fit(y, initialization=init, iterations=I, saliency=sal)
-            # the split really ran (choose_frame_split clamps S to the chunks and to S + 1 <= T / 32)
-            kernel, split, _ = last_plan()
-            assert split == min(S, _nchunks(T)) and kernel == (0 if D == 8 and sal is None else 2), (T, last_plan())
-            check_model(m, ref, atol=1e-9, rtol=1e-6)
+            lean = sal is None
+            pinned = lean and D == 8
+            m = device_fit(y, init, I, pinned=pinned, saliency=sal)
+            plan = dispatch(F, T, D, K, lean, pinned)
+            assert last_plan()[:2] == plan == (0 if pinned else 2, S), (T, last_plan(), plan)
+            check_model(m, O.cacgmm_fit(y, init, I, saliency=sal), atol=1e-9, rtol=1e-6)
 
 
 # ---- 4. the floor decision of the persistent update ------------------------------------------------------------------
