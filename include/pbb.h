@@ -857,7 +857,17 @@ int pbb_bss_eval(const double* x, long long items, int K, int E, long long T, in
  * band energies of x and y (entries from M_r on are not written).  status (2 long long, set by the call): the number
  * of rows with M_r < 30 and the first such row (-1: none).  Rows run `group` at a time, which sets the workspace
  * (pbb_stoi_workspace_bytes; 0 for an invalid shape).  n must be in [1, PBB_STOI_MAX_SAMPLES] and L in
- * (PBB_STOI_FRAME, PBB_STOI_MAX_RESAMPLED]: at most 256 samples at 10 kHz give no frame, where pystoi raises. */
+ * (PBB_STOI_FRAME, PBB_STOI_MAX_RESAMPLED]: at most 256 samples at 10 kHz give no frame, where pystoi raises.
+ *
+ * pbb_estoi: ESTOI, the extended STOI (Jensen and Taal, IEEE/ACM TASLP 24(11), 2016), i.e. pystoi.stoi(x, y, fs_sig,
+ * extended=True).  Exactly pbb_stoi's arguments, workspace (pbb_stoi_workspace_bytes), frames / resampled / energies
+ * outputs and status words; steps 1-3 and the 1e-5 rule of step 4 are the same bit for bit.  For M_r >= 30, each
+ * segment X, Y (15 bands x 30 frames) of the band energies, without clipping or scaling, is normalised per band (minus
+ * the mean over the frames, divided by the root of the sum of squares), then per frame (minus the mean over the bands,
+ * divided by the root of the sum of squares), and out[r] = the sum of X Y over (segment, band, frame) / (J_r 30).
+ * pystoi adds N(0, eps^2) noise before each normalisation; here a row or column whose centred sum of squares is zero
+ * up to rounding, at most 2^-92 times its sum of squares before centring, normalises to zeros (digital silence, and
+ * the constant columns of a segment of y with one non-zero frame); NaN and inf propagate. */
 #define PBB_STOI_FS 10000
 #define PBB_STOI_FRAME 256
 #define PBB_STOI_NFFT 512
@@ -872,6 +882,10 @@ int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long 
              const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
              const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
              long long* frames, double* resampled, double* energies, long long* status, void* stream);
+int pbb_estoi(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+              const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
+              const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
+              long long* frames, double* resampled, double* energies, long long* status, void* stream);
 
 /* ------------------------------------------------------------------------
  * SI-SDR (pb_bss/evaluation/module_si_sdr.py:4-56) and the invasive SxR (pb_bss/evaluation/sxr_module.py:17-274).

@@ -1,4 +1,4 @@
-// C-ABI entry points for STOI, pb_bss/evaluation/module_stoi.py -- see include/pbb.h and csrc/stoi.cuh.
+// C-ABI entry points for STOI and ESTOI, pb_bss/evaluation/module_stoi.py -- see include/pbb.h and csrc/stoi.cuh.
 #include "common.cuh"
 #include "prof.cuh"
 #include "stoi.cuh"
@@ -50,8 +50,9 @@ static StoiLayout stoi_layout(long long group, const StoiShape& s) {
   return l;
 }
 
+// One group of rows: the shared stages, then the segment kernel of STOI or (extended) ESTOI, then the values.
 template <class T>
-static int stoi_group(StoiParams p, const StoiShape& s, cudaStream_t st) {
+static int stoi_group(StoiParams p, const StoiShape& s, bool extended, cudaStream_t st) {
   if (s.resample) {
     const long long total = p.rows * 2 * p.L;
     const long long ctas = std::min<long long>((total + kStoiThreads - 1) / kStoiThreads, 1ll << 20);
@@ -79,7 +80,13 @@ static int stoi_group(StoiParams p, const StoiShape& s, cudaStream_t st) {
       stoi_bands_kernel<U><<<(unsigned)ctas, kStoiThreads, 0, st>>>(p);
       PBB_CUDA(cudaGetLastError());
     }
-    {
+    if (extended) {
+      PBB_CUDA(cudaFuncSetAttribute(estoi_segment_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int)kEstoiSmemBytes));
+      LaunchScope ls("estoi_segment_kernel", st);
+      estoi_segment_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, kEstoiSmemBytes, st>>>(p);
+      PBB_CUDA(cudaGetLastError());
+    } else {
       LaunchScope ls("stoi_segment_kernel", st);
       stoi_segment_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, 0, st>>>(p);
       PBB_CUDA(cudaGetLastError());
@@ -93,22 +100,12 @@ static int stoi_group(StoiParams p, const StoiShape& s, cudaStream_t st) {
   return run(T{});
 }
 
-}  // namespace pbb
-
-using namespace pbb;
-
-extern "C" {
-
-size_t pbb_stoi_workspace_bytes(long long group, long long n, int up, int down) {
-  StoiShape s;
-  if (group <= 0 || group > PBB_STOI_MAX_GROUP || !stoi_shape(n, up, down, &s)) return 0;
-  return stoi_layout(group, s).total;
-}
-
-int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
-             const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
-             const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
-             long long* frames, double* resampled, double* energies, long long* status, void* stream) {
+// pbb_stoi (extended = false) and pbb_estoi (extended = true): the same checks, workspace and stage outputs.
+static int stoi_call(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+                     const double* taps, int taps_per_phase, long long pre_remove, const double* window,
+                     const int* bands, const double* twiddle, long long group, void* workspace,
+                     size_t workspace_bytes, double* out, long long* frames, double* resampled, double* energies,
+                     long long* status, void* stream, bool extended) {
   StoiShape s;
   PBB_CHECK_ARG(x != nullptr, 1, "x is null");
   PBB_CHECK_ARG(y != nullptr, 2, "y is null");
@@ -162,10 +159,39 @@ int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long 
     p.out = out + g0;
     p.status = status;
     p.row0 = g0;
-    const int rc = dtype == PBB_F32 ? stoi_group<float>(p, s, st) : stoi_group<double>(p, s, st);
+    p.terms = extended ? kStoiSeg : kStoiBands;
+    const int rc = dtype == PBB_F32 ? stoi_group<float>(p, s, extended, st) : stoi_group<double>(p, s, extended, st);
     if (rc) return rc;
   }
   return 0;
+}
+
+}  // namespace pbb
+
+using namespace pbb;
+
+extern "C" {
+
+size_t pbb_stoi_workspace_bytes(long long group, long long n, int up, int down) {
+  StoiShape s;
+  if (group <= 0 || group > PBB_STOI_MAX_GROUP || !stoi_shape(n, up, down, &s)) return 0;
+  return stoi_layout(group, s).total;
+}
+
+int pbb_stoi(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+             const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
+             const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
+             long long* frames, double* resampled, double* energies, long long* status, void* stream) {
+  return stoi_call(x, y, dtype, rows, n, up, down, taps, taps_per_phase, pre_remove, window, bands, twiddle, group,
+                   workspace, workspace_bytes, out, frames, resampled, energies, status, stream, false);
+}
+
+int pbb_estoi(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+              const double* taps, int taps_per_phase, long long pre_remove, const double* window, const int* bands,
+              const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
+              long long* frames, double* resampled, double* energies, long long* status, void* stream) {
+  return stoi_call(x, y, dtype, rows, n, up, down, taps, taps_per_phase, pre_remove, window, bands, twiddle, group,
+                   workspace, workspace_bytes, out, frames, resampled, energies, status, stream, true);
 }
 
 }  // extern "C"

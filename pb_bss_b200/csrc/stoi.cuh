@@ -9,7 +9,10 @@
 //   stoi_bands_kernel      STFT frames of the overlap-added kept frames, windowed twice, 512-point real FFT,
 //                          one-third octave band energies
 //   stoi_segment_kernel    the correlation of every (segment, band), summed per block of segments
-//   stoi_value_kernel      per row: the sum of the block sums / (J 15), or 1e-5 below 30 frames; the status word
+//   estoi_segment_kernel   ESTOI (pbb_estoi; Jensen and Taal, IEEE/ACM TASLP 24(11), 2016) in place of the above:
+//                          the row- and column-normalised segments' inner products, summed per block of segments
+//   stoi_value_kernel      per row: the sum of the block sums / (J 15), or / (J 30) for ESTOI, or 1e-5 below 30
+//                          frames; the status word
 #pragma once
 #include "common.cuh"
 #include "fft_stages.cuh"
@@ -46,6 +49,7 @@ struct StoiParams {
   double* out;           // (rows)
   long long* status;     // (2) count of rows below 30 frames, first such row (-1: none)
   long long row0;        // index of the group's first row in the call
+  int terms;             // products summed per segment: 15 (STOI, one per band) or 30 (ESTOI, d_m times 30)
 };
 
 // numpy's maximum / minimum: NaN if either operand is NaN
@@ -205,10 +209,38 @@ __global__ void __launch_bounds__(kStoiThreads) stoi_bands_kernel(StoiParams p) 
   }
 }
 
+constexpr int kStoiSegFrames = kStoiSegBlock + kStoiSeg - 1;  // frames of a block of segments (the row stride W)
+
+// The band energies of frames seg0 .. seg0 + nfr - 1 of row r into sx, sy (15, kStoiSegFrames).
+__device__ __forceinline__ void stoi_stage_frames(const StoiParams& p, long long r, int seg0, int nfr, double* sx,
+                                                  double* sy) {
+  constexpr int W = kStoiSegFrames;
+  const double* tx = p.tob + 2 * r * kStoiBands * p.Mmax;
+  const double* ty = tx + kStoiBands * p.Mmax;
+  for (int q = threadIdx.x; q < kStoiBands * nfr; q += blockDim.x) {
+    const int b = q / nfr, f = q - b * nfr;
+    sx[b * W + f] = tx[b * p.Mmax + seg0 + f];
+    sy[b * W + f] = ty[b * p.Mmax + seg0 + f];
+  }
+}
+
+// The CTA's sum of every thread's `local`, a fixed tree (warp butterfly, then the warps in order), into
+// partial[blockIdx.x].  red holds kStoiThreads / 32 doubles.
+__device__ __forceinline__ void stoi_block_sum(const StoiParams& p, double local, double* red) {
+  local = warp_sum(local);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = local;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = red[0];
+    for (int w = 1; w < kStoiThreads / 32; ++w) t += red[w];
+    p.partial[blockIdx.x] = t;
+  }
+}
+
 // One CTA: kStoiSegBlock segments of one row.  The band energies of the block's frames are staged in shared memory;
 // thread q takes the (segment, band) items q, q + 256, ... in order, and the CTA's sum is a fixed tree.
 __global__ void __launch_bounds__(kStoiThreads) stoi_segment_kernel(StoiParams p) {
-  constexpr int W = kStoiSegBlock + kStoiSeg - 1;
+  constexpr int W = kStoiSegFrames;
   __shared__ double sx[kStoiBands * W], sy[kStoiBands * W];
   __shared__ double red[kStoiThreads / 32];
   const long long r = blockIdx.x / p.blocks;
@@ -219,13 +251,7 @@ __global__ void __launch_bounds__(kStoiThreads) stoi_segment_kernel(StoiParams p
     return;
   }
   const int ns = min(kStoiSegBlock, J - seg0), nfr = ns + kStoiSeg - 1;
-  const double* tx = p.tob + 2 * r * kStoiBands * p.Mmax;
-  const double* ty = tx + kStoiBands * p.Mmax;
-  for (int q = threadIdx.x; q < kStoiBands * nfr; q += blockDim.x) {
-    const int b = q / nfr, f = q - b * nfr;
-    sx[b * W + f] = tx[b * p.Mmax + seg0 + f];
-    sy[b * W + f] = ty[b * p.Mmax + seg0 + f];
-  }
+  stoi_stage_frames(p, r, seg0, nfr, sx, sy);
   __syncthreads();
   double local = 0.0;
   for (int q = threadIdx.x; q < ns * kStoiBands; q += blockDim.x) {
@@ -254,14 +280,105 @@ __global__ void __launch_bounds__(kStoiThreads) stoi_segment_kernel(StoiParams p
     }
     local += dot / ((sqrt(vy) + kStoiEps) * (sqrt(vx) + kStoiEps));
   }
-  local = warp_sum(local);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = local;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = red[0];
-    for (int w = 1; w < kStoiThreads / 32; ++w) t += red[w];
-    p.partial[blockIdx.x] = t;
+  stoi_block_sum(p, local, red);
+}
+
+// 1 / sqrt(s) of a centred sum of squares s, and 0 where s is zero up to rounding: at most 2^-92 = (64 eps)^2 times the
+// sum of squares before centring, raw.  ESTOI without pystoi's N(0, eps^2) noise, whose expected contribution to such
+// a row or column is zero: digital silence, and the columns of a segment with one non-zero frame, which are constant
+// in exact arithmetic.  A NaN s fails the comparison and stays NaN.
+constexpr double kEstoiTiny = 0x1p-92;
+__device__ __forceinline__ double estoi_inv_norm(double s, double raw) {
+  return s <= kEstoiTiny * raw ? 0.0 : 1.0 / sqrt(s);
+}
+
+// Dynamic shared memory of estoi_segment_kernel: the staged frames of x and y (15, kStoiSegFrames) and, per (segment,
+// band) of the block, the row mean and inverse norm of x and y.  53 040 bytes: above the 48 KB static limit.
+constexpr int kEstoiRows = kStoiSegBlock * kStoiBands;
+constexpr size_t kEstoiSmemBytes = (2 * kStoiBands * kStoiSegFrames + 4 * kEstoiRows) * sizeof(double);
+
+// One CTA: kStoiSegBlock segments of one row, the frames staged as in stoi_segment_kernel, so `partial` has the same
+// layout.  Phase A: thread q takes the (segment, band) rows q, q + 256, ...: the mean over the 30 frames and the inverse
+// root of the centred sum of squares, of x and of y.  Phase B: thread q takes the (segment, frame) columns q, q + 256,
+// ...: the row-normalised column of x and of y over the 15 bands (recomputed from the staged frames and the phase-A
+// scalars), its mean and inverse norm, and the inner product of the two normalised columns.  The CTA's sum is a fixed
+// tree; the value kernel divides the row's total by 30 J.
+__global__ void __launch_bounds__(kStoiThreads) estoi_segment_kernel(StoiParams p) {
+  constexpr int W = kStoiSegFrames;
+  extern __shared__ double smem[];
+  double* sx = smem;
+  double* sy = sx + kStoiBands * W;
+  double* mx = sy + kStoiBands * W;  // (kStoiSegBlock, 15): row means and inverse norms of x and y
+  double* ix = mx + kEstoiRows;
+  double* my = ix + kEstoiRows;
+  double* iy = my + kEstoiRows;
+  __shared__ double red[kStoiThreads / 32];
+  const long long r = blockIdx.x / p.blocks;
+  const int blk = (int)(blockIdx.x % p.blocks), seg0 = blk * kStoiSegBlock;
+  const int J = (int)p.km[2 * r + 1] - kStoiSeg + 1;
+  if (seg0 >= J) {
+    if (threadIdx.x == 0) p.partial[blockIdx.x] = 0.0;
+    return;
   }
+  const int ns = min(kStoiSegBlock, J - seg0), nfr = ns + kStoiSeg - 1;
+  stoi_stage_frames(p, r, seg0, nfr, sx, sy);
+  __syncthreads();
+  for (int q = threadIdx.x; q < ns * kStoiBands; q += blockDim.x) {
+    const int j = q / kStoiBands, b = q - j * kStoiBands;
+    const double* x = sx + b * W + j;
+    const double* y = sy + b * W + j;
+    double ax = 0.0, ay = 0.0, rx = 0.0, ry = 0.0;
+    // unrolled by 6, not fully: a full unroll holds the 60 staged values between the two passes in registers (155
+    // per thread, one CTA per SM)
+#pragma unroll 6
+    for (int k = 0; k < kStoiSeg; ++k) {
+      ax += x[k];
+      ay += y[k];
+      rx = fma(x[k], x[k], rx);
+      ry = fma(y[k], y[k], ry);
+    }
+    ax /= kStoiSeg;
+    ay /= kStoiSeg;
+    double vx = 0.0, vy = 0.0;
+#pragma unroll 6
+    for (int k = 0; k < kStoiSeg; ++k) {
+      const double e = x[k] - ax, a = y[k] - ay;
+      vx = fma(e, e, vx);
+      vy = fma(a, a, vy);
+    }
+    mx[q] = ax;
+    ix[q] = estoi_inv_norm(vx, rx);
+    my[q] = ay;
+    iy[q] = estoi_inv_norm(vy, ry);
+  }
+  __syncthreads();
+  double local = 0.0;
+  for (int q = threadIdx.x; q < ns * kStoiSeg; q += blockDim.x) {
+    const int j = q / kStoiSeg, n = q - j * kStoiSeg;
+    const double* x = sx + j + n;
+    const double* y = sy + j + n;
+    const int s0 = j * kStoiBands;
+    // the row-normalised values are recomputed from shared memory in the second pass rather than held in registers
+    double cu = 0.0, cv = 0.0, ru = 0.0, rv = 0.0;
+    for (int b = 0; b < kStoiBands; ++b) {
+      const double e = (x[b * W] - mx[s0 + b]) * ix[s0 + b], a = (y[b * W] - my[s0 + b]) * iy[s0 + b];
+      cu += e;
+      cv += a;
+      ru = fma(e, e, ru);
+      rv = fma(a, a, rv);
+    }
+    cu /= kStoiBands;
+    cv /= kStoiBands;
+    double su = 0.0, sv = 0.0, dot = 0.0;
+    for (int b = 0; b < kStoiBands; ++b) {
+      const double e = (x[b * W] - mx[s0 + b]) * ix[s0 + b] - cu, a = (y[b * W] - my[s0 + b]) * iy[s0 + b] - cv;
+      su = fma(e, e, su);
+      sv = fma(a, a, sv);
+      dot = fma(e, a, dot);
+    }
+    local += dot * estoi_inv_norm(su, ru) * estoi_inv_norm(sv, rv);
+  }
+  stoi_block_sum(p, local, red);
 }
 
 // One CTA for the group: the value of every row (block sums in order) and the status word.
@@ -279,7 +396,7 @@ __global__ void __launch_bounds__(kStoiThreads) stoi_value_kernel(StoiParams p) 
       const double* part = p.partial + r * p.blocks;
       double t = 0.0;
       for (int b = 0; b < p.blocks; ++b) t += part[b];
-      v = t / (double)((M - kStoiSeg + 1) * kStoiBands);
+      v = t / (double)((M - kStoiSeg + 1) * p.terms);
     }
     p.out[r] = v;
   }

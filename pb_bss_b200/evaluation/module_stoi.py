@@ -1,5 +1,6 @@
 """STOI, the short-time objective intelligibility of pb_bss/evaluation/module_stoi.py, on the device, with the
-reference's signature, broadcasting and return types: ``stoi(reference, estimation, sample_rate)``.
+reference's signature, broadcasting and return types, and ESTOI, its extended form:
+``stoi(reference, estimation, sample_rate, extended=False)``.
 
 The reference calls pystoi.stoi(x, y, fs_sig) (extended=False; Taal, Hendriks, Heusdens and Jensen, IEEE TASLP 19(7),
 2011) on every pair of the broadcast leading dims.  Here every pair runs in one pass per step (include/pbb.h,
@@ -8,10 +9,21 @@ of the reference, the 512-point STFT of the overlap-added kept frames, 15 one-th
 the clipped correlations of 30-frame segments.  fp64, bitwise reproducible, and a pair's value does not depend on
 the rest of the batch.
 
+``extended=True`` gives ESTOI (Jensen and Taal, IEEE/ACM TASLP 24(11), 2016), pystoi's stoi(x, y, fs,
+extended=True), the measure designed for modulated maskers such as competing talkers (pbb_estoi).  It shares every
+step up to the band envelopes bit for bit, and the 1e-5 rule below 30 frames; each 15 x 30 segment is then
+normalised per band over the frames and per frame over the bands, without clipping, and the value is the mean over
+the segments of the normalised inner product / 30.
+
 Documented differences from the reference:
   - integer and float32 input are computed in fp64 (at 10 kHz pystoi would frame float32 input in float32);
   - at most 2^22 samples per signal and 2^23 after resampling to 10 kHz; larger inputs raise ValueError, as does a
-    signal with no 256-sample frame at 10 kHz (where NumPy raises an AxisError inside pystoi).
+    signal with no 256-sample frame at 10 kHz (where NumPy raises an AxisError inside pystoi);
+  - ESTOI: pystoi adds N(0, eps^2) noise before each normalisation step, this does not; a band or frame whose centred
+    sum of squares is zero up to rounding (at most 2^-92 of its sum of squares) normalises to zeros, the expected
+    value of pystoi's random term there.  Digital silence in the estimate reaches this: its all-zero bands, and the
+    segments with one non-zero frame at either end of a silent stretch, whose frames are constant over the bands
+    after the first step in exact arithmetic.
 """
 import math
 import warnings
@@ -145,10 +157,10 @@ def _warn(status):
     return on_error
 
 
-def _stages(x, y, sample_rate, stages=True):
-    """Every step on the device for x, y (rows, n): dict of value (rows,), and with ``stages`` frames (rows, 2) int64
-    (K_r, M_r), resampled (rows, 2, L) (None at 10 kHz) and energies (rows, 2, 15, M_max), zero from M_r on.  The
-    status is checked (deferred inside ``deferred_status``)."""
+def _stages(x, y, sample_rate, stages=True, extended=False):
+    """Every step on the device for x, y (rows, n): dict of value (rows,), STOI or with ``extended`` ESTOI, and with
+    ``stages`` frames (rows, 2) int64 (K_r, M_r), resampled (rows, 2, L) (None at 10 kHz) and energies
+    (rows, 2, 15, M_max), zero from M_r on.  The status is checked (deferred inside ``deferred_status``)."""
     lib = _lib.load()
     rows, n = x.shape
     up, down = rates(sample_rate)
@@ -166,21 +178,28 @@ def _stages(x, y, sample_rate, stages=True):
         out['frames'] = _device.empty((rows, 2), torch.int64)
         out['resampled'] = _device.empty((rows, 2, L), torch.float64) if (up, down) != (1, 1) else None
         out['energies'] = torch.zeros((rows, 2, BANDS, m_max), dtype=torch.float64, device=x.device)
-    _lib.check(lib.pbb_stoi(_device.ptr(x), _device.ptr(y), _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64,
-                            rows, n, up, down, _device.ptr(taps), tpp, pre_remove, _device.ptr(win),
-                            _device.ptr(bands), _device.ptr(tw), group, _device.ptr(ws), nbytes, _device.ptr(value),
-                            _device.ptr(out.get('frames')), _device.ptr(out.get('resampled')),
-                            _device.ptr(out.get('energies')), _device.ptr(status), _device.stream_ptr()), 'pbb_stoi')
+    name = 'pbb_estoi' if extended else 'pbb_stoi'
+    _lib.check(getattr(lib, name)(_device.ptr(x), _device.ptr(y),
+                                  _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64, rows, n, up, down,
+                                  _device.ptr(taps), tpp, pre_remove, _device.ptr(win), _device.ptr(bands),
+                                  _device.ptr(tw), group, _device.ptr(ws), nbytes, _device.ptr(value),
+                                  _device.ptr(out.get('frames')), _device.ptr(out.get('resampled')),
+                                  _device.ptr(out.get('energies')), _device.ptr(status), _device.stream_ptr()), name)
     _device.check_status(status[:1], _warn(status))
     return out
 
 
-def stoi(reference, estimation, sample_rate):
+def stoi(reference, estimation, sample_rate, extended=False):
     """pb_bss.evaluation.stoi: the STOI of estimation against reference along the last axis, after broadcasting the
     two (NumPy's rules; ValueError if they do not broadcast).  1-D input gives an np.float64, n-D input an ndarray of
     the broadcast leading shape.  A CUDA tensor in (either argument) gives a float64 CUDA tensor of that shape (0-d
     for 1-D input), and the call only enqueues work on the current stream: the one host synchronisation is the read
     of the status word, which ``deferred_status()`` postpones to the end of its block.
+
+    With ``extended`` true the value is ESTOI (pystoi's stoi(x, y, fs, extended=True); Jensen and Taal, 2016), with
+    the same types, broadcasting, checks and warning.  Unlike pystoi, no random noise is added before its
+    normalisations: a band or frame of a segment whose centred sum of squares is zero up to rounding, such as digital
+    silence, normalises to zeros.
 
     A pair with fewer than 30 STFT frames after the silent-frame removal gives 1e-5 and a RuntimeWarning, as pystoi
     does.  float32 and integer input are computed in fp64; complex input raises TypeError; signals of more than 2^22
@@ -193,7 +212,7 @@ def stoi(reference, estimation, sample_rate):
         value = _device.empty(lead, torch.float64)
     else:
         x, y = _operands(reference, estimation, shape)
-        value = _stages(x, y, sample_rate, stages=False)['value'].reshape(lead)
+        value = _stages(x, y, sample_rate, stages=False, extended=bool(extended))['value'].reshape(lead)
     if not like_numpy:
         return value
     v = value.cpu().numpy()
