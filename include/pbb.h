@@ -476,12 +476,53 @@ int pbb_apply_beamforming_vector(const void* vector, const void* mix, int dtype,
 int pbb_apply_beamforming_vector_shared(const void* vector, const void* mix, int dtype,
                                         int B, int F, int D, int T, void* out, void* stream);
 
+/* Differentiates pbb_apply_beamforming_vector: grad_vector[f][a] = sum_t mix[f][a][t] conj(g[f][t]) (fixed order over
+ * t), grad_mix[f][a][t] = vector[f][a] g[f][t].  grad_out g (F, T); grad_vector (F, D) and grad_mix (F, D, T)
+ * complex128, either may be NULL. */
+int pbb_apply_beamforming_vector_backward(const void* vector, const void* mix, int dtype, int F, int D,
+                                          int T, const void* grad_out, void* grad_vector, void* grad_mix,
+                                          void* stream);
+
+/* Differentiates pbb_apply_beamforming_vector_shared: grad_vector (B, F, D) as above; grad_mix (F, D, T) =
+ * sum_b vector[b][f][a] g[b][f][t] summed in increasing b, without materialising the broadcast mix. */
+int pbb_apply_beamforming_vector_shared_backward(const void* vector, const void* mix, int dtype, int B,
+                                                 int F, int D, int T, const void* grad_out,
+                                                 void* grad_vector, void* grad_mix, void* stream);
+
 /* Plain np.linalg.solve without the lstsq fallback (get_mvdr_vector_merl,
  * beamformer.py:277): a (n, D, D), b (n, D, R) -> x (n, D, R).  status must not be
  * NULL; it is set to 1 + the index of an exactly singular matrix (a zero pivot,
  * where NumPy raises LinAlgError), whose x is then undefined. */
 int pbb_solve_batched_strict(const void* a, const void* b, int n, int D, int R,
                              void* x, int* status, void* stream);
+
+/* ---- Backward passes of the mask-based beamforming chain (torch.autograd in pb_bss_b200).  For a real loss L every
+ * gradient follows PyTorch's convention grad z = dL/dRe z + i dL/dIm z.  fp64, fixed-order sums and no atomics, so
+ * repeated calls are bitwise identical; each call only enqueues work on `stream` (no status word, no synchronisation).
+ * Gradients are written as complex128 / float64; shapes and limits are those of the forward. */
+
+/* Differentiates pbb_power_spectral_density.  With w_kt = mask_kt / max(S_k, 1e-10), S_k = sum_t mask_kt (normalize),
+ * mask_kt (normalize = 0) or 1 / T (mask NULL, K = 1), and G_k = grad_psd[f][k]:
+ *   grad_observation[f][:, t] = sum_k w_kt (G_k + G_k^H) y_t,
+ *   grad_mask[f][k][t] = (Re(y_t^H G_k y_t) - Re<G_k, psd_k>) / S_k while S_k > 1e-10, else Re(y_t^H G_k y_t) / 1e-10,
+ *                        and Re(y_t^H G_k y_t) without normalize (<A, B> = sum conj(A_ij) B_ij).
+ * psd is the forward's output (F, K, D, D); grad_psd the same shape; grad_observation (F, D, T) complex128 and
+ * grad_mask (F, K, T) float64, either may be NULL.  One pass reads the observation once for all K sources. */
+int pbb_power_spectral_density_backward(const void* observation, int dtype, int F, int D, int T,
+                                        const double* mask, int K, int normalize, const void* psd,
+                                        const void* grad_psd, void* grad_observation, double* grad_mask,
+                                        void* stream);
+
+/* Differentiates w = mat[:, ref_channel] of pbb_souden, mat = phi / max(lambda, eps), lambda = Re tr phi,
+ * phi = N^-1 X (phi: the forward's pbb_solve_batched output, noise_psd: N, grad_w (n, D)); ref_channel is a constant.
+ *   grad phi = g e_r^T / lambda - (Re(g^H phi[:, r]) / lambda^2) I (lambda > eps), g e_r^T / eps otherwise;
+ *   grad_target_psd = N^-H grad phi (the elimination of pbb_solve_batched on N^H, N is not assumed Hermitian);
+ *   grad_noise_psd = -grad_target_psd phi^H.
+ * A bin whose N^H meets an exactly zero pivot (a singular N: the forward's minimum-norm branch, which has no such
+ * derivative) or holds non-finite values gets NaN gradients; other bins are unaffected.  0 < D <= 64. */
+int pbb_souden_backward(const void* phi, const void* noise_psd, const void* grad_w, int n, int D,
+                        int ref_channel, double eps, void* grad_target_psd, void* grad_noise_psd,
+                        void* stream);
 
 /* get_lcmv_vector (beamformer.py:414-456): atf (K, F, D), response (K)
  * complex128 on the device, noise_psd (F, D, D) -> w (F, D).  X = solve(noise, H)
@@ -732,6 +773,25 @@ int pbb_istft(const void* X, long long rows, int frames, int size, int shift, in
               int crop, long long n_out, const double* synthesis_window, const double* twiddle,
               void* workspace, size_t workspace_bytes, double* out, void* stream);
 
+/* Differentiates pbb_stft wrt x (same arguments; grad_X (rows, frames, size/2 + 1) complex128 is the gradient of out).
+ * Per frame dL/dframe_j = size irfft(G^)_j, G^_k = G_k / 2 for 0 < k < size/2 and G_k at k = 0 and size/2, times
+ * window[j], then overlap-added in increasing t over the frames covering each sample of [0, n) (fading offset and the
+ * pad=False remainder as in the forward; a sample no frame covers gets 0).  grad_x (rows, n) float64.  The frames go
+ * to workspace (pbb_stft_backward_workspace_bytes). */
+size_t pbb_stft_backward_workspace_bytes(long long rows, int frames, int window_length);
+int pbb_stft_backward(const void* grad_X, long long rows, long long n, int size, int shift,
+                      int window_length, int offset, int frames, const double* window,
+                      const double* twiddle, void* workspace, size_t workspace_bytes, double* grad_x,
+                      void* stream);
+
+/* Differentiates pbb_istft wrt X (same arguments; grad_out (rows, n_out) float64 is the gradient of out).  The STFT
+ * of the gradient: frame t reads grad_out[t shift + j - crop] (zero outside [0, n_out)) times synthesis_window[j],
+ * h = that frame, and grad_X[r][t][k] = (2 / size) rfft(h)_k for 0 < k < size/2, (1 / size) Re rfft(h)_k with a zero
+ * imaginary part at k = 0 and size/2.  grad_X (rows, frames, size/2 + 1) complex128. */
+int pbb_istft_backward(const double* grad_out, long long rows, int frames, int size, int shift,
+                       int window_length, int crop, long long n_out, const double* synthesis_window,
+                       const double* twiddle, void* grad_X, void* stream);
+
 /* ------------------------------------------------------------------------
  * Gammatone filterbank (pb_bss/transform/gammatone.py:6-102, Slaney's Apple TR #35), csrc/gammatone.cuh.
  *
@@ -915,6 +975,20 @@ size_t pbb_si_sdr_workspace_bytes(long long rows, long long n);
 int pbb_si_sdr(const double* reference, const double* estimation, const long long* reference_offsets,
                const long long* estimation_offsets, long long rows, long long n, void* workspace,
                size_t workspace_bytes, double* out, void* stream);
+/* Differentiates pbb_si_sdr (same first six arguments, grad_out (rows) float64).  With p = alpha r and q = e - p as
+ * pass 2 forms them, P = sum p^2, Q = sum q^2: ds/de = (20 / ln 10)(p / P - q / Q), ds/dr = (20 alpha / ln 10)
+ * (1 / P + 1 / Q) q.  A broadcast operand's gradient sums the rows that read it: own row u of the reference
+ * (reference_rows of them, n samples each) is the sum over the rows reference_row_index[reference_row_start[u]] ..
+ * [reference_row_start[u + 1] - 1] in that order (device int64 tables); the same for the estimation.  grad_reference /
+ * grad_estimation (own rows, n) float64, either may be NULL.  inf / NaN rows (zero reference, e = 2^j r, ...) give
+ * non-finite gradients.  Workspace: pbb_si_sdr_backward_workspace_bytes. */
+size_t pbb_si_sdr_backward_workspace_bytes(long long rows, long long n);
+int pbb_si_sdr_backward(const double* reference, const double* estimation, const long long* reference_offsets,
+                        const long long* estimation_offsets, long long rows, long long n, const double* grad_out,
+                        long long reference_rows, const long long* reference_row_start,
+                        const long long* reference_row_index, long long estimation_rows,
+                        const long long* estimation_row_start, const long long* estimation_row_index, void* workspace,
+                        size_t workspace_bytes, double* grad_reference, double* grad_estimation, void* stream);
 /* input_sxr (:94-165) from the powers S (K, D) and N (D), float64 on the device, in the reference's order of
  * operations: I[k, d] = np.sum of S[n != k, d], the channel means (average_channels), S / (I + N), S / I, S / N in dB
  * (IEEE inf / nan for zero powers), then the source mean (average_sources).  sdr / sir / snr have the shape of the

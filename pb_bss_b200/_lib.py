@@ -133,6 +133,10 @@ SIGNATURES = {
     'pbb_matvec_batched': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
     'pbb_apply_beamforming_vector': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'pbb_apply_beamforming_vector_shared': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    'pbb_apply_beamforming_vector_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_apply_beamforming_vector_shared_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_power_spectral_density_backward': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
+    'pbb_souden_backward': (_i, [_vp, _vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp]),
     'pbb_solve_batched_strict': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     'pbb_lcmv': (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_wmwf': (_i, [_vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp]),
@@ -159,6 +163,9 @@ SIGNATURES = {
     'pbb_griffin_lim_stft': (_i, [_vp, _i, _ll, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'pbb_istft_workspace_bytes': (_sz, [_ll, _i, _i]),
     'pbb_istft': (_i, [_vp, _ll, _i, _i, _i, _i, _i, _ll, _vp, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_stft_backward_workspace_bytes': (_sz, [_ll, _i, _i]),
+    'pbb_stft_backward': (_i, [_vp, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp]),
+    'pbb_istft_backward': (_i, [_vp, _ll, _i, _i, _i, _i, _i, _ll, _vp, _vp, _vp, _vp]),
     'pbb_gammatone_chunk_length': (_i, [_ll, _i, _ll]),
     'pbb_gammatone_workspace_bytes': (_sz, [_ll, _i, _ll]),
     'pbb_gammatone': (_i, [_vp, _i, _ll, _ll, _i, _vp, _vp, _i, _vp, _sz, _vp, _vp]),
@@ -181,6 +188,9 @@ SIGNATURES = {
     'pbb_mean_square': (_i, [_vp, _i, _ll, _ll, _vp, _sz, _vp, _vp]),
     'pbb_si_sdr_workspace_bytes': (_sz, [_ll, _ll]),
     'pbb_si_sdr': (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp, _sz, _vp, _vp]),
+    'pbb_si_sdr_backward_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_si_sdr_backward': (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp, _ll, _vp, _vp, _ll, _vp, _vp, _vp, _sz, _vp, _vp,
+                                 _vp]),
     'pbb_input_sxr': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_output_sxr_workspace_bytes': (_sz, [_i, _i]),
     'pbb_output_sxr': (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),

@@ -282,6 +282,106 @@ int pbb_power_spectral_density(const void* observation, int dtype, int F, int D,
   return 0;
 }
 
+// ---- backward passes of the mask-based beamforming chain (linalg_kernels.cuh) --------------------------------------
+
+int pbb_power_spectral_density_backward(const void* observation, int dtype, int F, int D, int T, const double* mask,
+                                        int K, int normalize, const void* psd, const void* grad_psd,
+                                        void* grad_observation, double* grad_mask, void* stream) {
+  PBB_CHECK_ARG(observation != nullptr, 1, "observation is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "bad dtype");
+  PBB_CHECK_ARG(F > 0 && D > 0 && D < 35 && T > 0, 3, "bad shape");
+  PBB_CHECK_ARG(K > 0 && K < kMaxK, 7, "need 0 < K < 20");
+  PBB_CHECK_ARG(mask != nullptr || K == 1, 6, "mask is null and K != 1");
+  PBB_CHECK_ARG(psd != nullptr, 9, "psd is null");
+  PBB_CHECK_ARG(grad_psd != nullptr, 10, "grad_psd is null");
+  PBB_CHECK_ARG(grad_observation != nullptr || grad_mask != nullptr, 11, "both gradients are null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t smem = psd_backward_smem(D, K);
+  const long long ctas = (long long)F * ((T + kPsdBwdThreads - 1) / kPsdBwdThreads);
+  PBB_CHECK_ARG(ctas <= 0x7fffffffll, 3, "F * ceil(T / 64) exceeds the grid");
+  const unsigned grid = (unsigned)ctas;
+  const double2* P = reinterpret_cast<const double2*>(psd);
+  const double2* G = reinterpret_cast<const double2*>(grad_psd);
+  double2* gy = reinterpret_cast<double2*>(grad_observation);
+  LaunchScope ls("psd_backward_kernel", st);
+  if (dtype == PBB_C128) {
+    PBB_CUDA(cudaFuncSetAttribute(psd_backward_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    psd_backward_kernel<double2><<<grid, kPsdBwdThreads, smem, st>>>(
+        reinterpret_cast<const double2*>(observation), mask, P, G, F, D, T, K, normalize, gy, grad_mask);
+  } else {
+    PBB_CUDA(cudaFuncSetAttribute(psd_backward_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    psd_backward_kernel<float2><<<grid, kPsdBwdThreads, smem, st>>>(
+        reinterpret_cast<const float2*>(observation), mask, P, G, F, D, T, K, normalize, gy, grad_mask);
+  }
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_souden_backward(const void* phi, const void* noise_psd, const void* grad_w, int n, int D, int ref_channel,
+                        double eps, void* grad_target_psd, void* grad_noise_psd, void* stream) {
+  PBB_CHECK_ARG(phi && noise_psd && grad_w, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
+  PBB_CHECK_ARG(ref_channel >= 0 && ref_channel < D, 6, "ref_channel must be in [0, D)");
+  PBB_CHECK_ARG(grad_target_psd && grad_noise_psd, 8, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  {
+    // grad Phi goes to grad_noise_psd, which the last kernel overwrites
+    LaunchScope ls("souden_backward_kernel", st);
+    souden_backward_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(phi),
+                                             reinterpret_cast<const double2*>(grad_w), n, D, ref_channel, eps,
+                                             reinterpret_cast<double2*>(grad_noise_psd));
+    PBB_CUDA(cudaGetLastError());
+  }
+  // grad X = N^-H grad Phi; a zero pivot (no derivative: the forward's minimum-norm branch) or non-finite N gives NaN
+  const int rc = solve_launch(noise_psd, grad_noise_psd, n, D, D, 2, grad_target_psd, nullptr, 2, st);
+  if (rc) return rc;
+  LaunchScope ls("souden_noise_backward_kernel", st);
+  souden_noise_backward_kernel<<<blocks_for((size_t)n * D * D, 128), 128, 0, st>>>(
+      reinterpret_cast<const double2*>(grad_target_psd), reinterpret_cast<const double2*>(phi), n, D,
+      reinterpret_cast<double2*>(grad_noise_psd));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+static int apply_bf_backward_launch(const void* vector, const void* mix, int dtype, int B, int F, int D, int T,
+                                    const void* grad_out, void* grad_vector, void* grad_mix, void* stream) {
+  PBB_CHECK_ARG(vector && mix && grad_out, 1, "input is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 3, "bad dtype");
+  PBB_CHECK_ARG(B > 0 && B <= 65535 && F > 0 && D > 0 && T > 0, 4, "bad shape");
+  PBB_CHECK_ARG(grad_vector != nullptr || grad_mix != nullptr, 8, "both gradients are null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const double2* g = reinterpret_cast<const double2*>(grad_out);
+  if (grad_vector) {
+    LaunchScope ls("apply_bf_vector_backward_kernel", st);
+    const unsigned blocks = blocks_for((size_t)B * F * D * 32, 256);
+    if (dtype == PBB_C128)
+      apply_bf_vector_backward_kernel<double2><<<blocks, 256, 0, st>>>(
+          reinterpret_cast<const double2*>(mix), g, B, F, D, T, reinterpret_cast<double2*>(grad_vector));
+    else
+      apply_bf_vector_backward_kernel<float2><<<blocks, 256, 0, st>>>(
+          reinterpret_cast<const float2*>(mix), g, B, F, D, T, reinterpret_cast<double2*>(grad_vector));
+    PBB_CUDA(cudaGetLastError());
+  }
+  if (grad_mix) {
+    LaunchScope ls("apply_bf_mix_backward_kernel", st);
+    apply_bf_mix_backward_kernel<<<dim3((T + 255) / 256, F < 65535 ? F : 65535), 256, 0, st>>>(
+        reinterpret_cast<const double2*>(vector), g, B, F, D, T, reinterpret_cast<double2*>(grad_mix));
+    PBB_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+int pbb_apply_beamforming_vector_backward(const void* vector, const void* mix, int dtype, int F, int D, int T,
+                                          const void* grad_out, void* grad_vector, void* grad_mix, void* stream) {
+  return apply_bf_backward_launch(vector, mix, dtype, 1, F, D, T, grad_out, grad_vector, grad_mix, stream);
+}
+
+int pbb_apply_beamforming_vector_shared_backward(const void* vector, const void* mix, int dtype, int B, int F, int D,
+                                                 int T, const void* grad_out, void* grad_vector, void* grad_mix,
+                                                 void* stream) {
+  return apply_bf_backward_launch(vector, mix, dtype, B, F, D, T, grad_out, grad_vector, grad_mix, stream);
+}
+
 // ---- multi-source beamformers and vector post-processing (csrc/extraction.cuh) ----------------------------------
 
 int pbb_lcmv(const void* atf, const void* response, const void* noise_psd, int K, int F, int D, void* w,

@@ -109,6 +109,81 @@ int pbb_si_sdr(const double* reference, const double* estimation, const long lon
   return 0;
 }
 
+size_t pbb_si_sdr_backward_workspace_bytes(long long rows, long long n) {
+  if (!rows_ok(rows, n)) return 0;
+  return pbb_si_sdr_workspace_bytes(rows, n) + (size_t)(2 * rows) * sizeof(double);
+}
+
+int pbb_si_sdr_backward(const double* reference, const double* estimation, const long long* reference_offsets,
+                        const long long* estimation_offsets, long long rows, long long n, const double* grad_out,
+                        long long reference_rows, const long long* reference_row_start,
+                        const long long* reference_row_index, long long estimation_rows,
+                        const long long* estimation_row_start, const long long* estimation_row_index, void* workspace,
+                        size_t workspace_bytes, double* grad_reference, double* grad_estimation, void* stream) {
+  PBB_CHECK_ARG(reference != nullptr || n == 0 || rows == 0, 1, "reference is null");
+  PBB_CHECK_ARG(estimation != nullptr || n == 0 || rows == 0, 2, "estimation is null");
+  PBB_CHECK_ARG((reference_offsets != nullptr && estimation_offsets != nullptr) || rows == 0, 3, "an offset table is null");
+  PBB_CHECK_ARG(rows_ok(rows, n), 5, "rows and n must be non-negative and rows * chunks below 2^31");
+  PBB_CHECK_ARG(grad_out != nullptr || rows == 0, 7, "grad_out is null");
+  PBB_CHECK_ARG(grad_reference == nullptr || (reference_rows >= 0 && reference_rows <= rows &&
+                                              (rows == 0 || (reference_row_start && reference_row_index))),
+                8, "bad reference row table");
+  PBB_CHECK_ARG(grad_estimation == nullptr || (estimation_rows >= 0 && estimation_rows <= rows &&
+                                               (rows == 0 || (estimation_row_start && estimation_row_index))),
+                11, "bad estimation row table");
+  PBB_CHECK_ARG(workspace_bytes >= pbb_si_sdr_backward_workspace_bytes(rows, n) && (workspace != nullptr || rows == 0),
+                14, "workspace too small (pbb_si_sdr_backward_workspace_bytes)");
+  if (rows == 0 || n == 0) return 0;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const long long chunks = sxr_chunks(n);
+  double* p1 = static_cast<double*>(workspace);
+  double* p2 = p1 + rows * chunks * 2;
+  double* alpha = p2 + rows * chunks * 2;
+  double* coef = alpha + rows;
+  const unsigned grid = (unsigned)(rows * chunks);
+  // alpha, P and Q exactly as pbb_si_sdr forms them
+  {
+    LaunchScope ls("si_sdr_pass1_kernel", st);
+    si_sdr_pass1_kernel<<<grid, kSxrThreads, 0, st>>>(reference, estimation, reference_offsets, estimation_offsets, n,
+                                                      chunks, p1);
+    PBB_CUDA(cudaGetLastError());
+  }
+  {
+    LaunchScope ls("si_sdr_alpha_kernel", st);
+    si_sdr_alpha_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(p1, chunks, alpha);
+    PBB_CUDA(cudaGetLastError());
+  }
+  {
+    LaunchScope ls("si_sdr_pass2_kernel", st);
+    si_sdr_pass2_kernel<<<grid, kSxrThreads, 0, st>>>(reference, estimation, reference_offsets, estimation_offsets, n,
+                                                      chunks, alpha, p2);
+    PBB_CUDA(cudaGetLastError());
+  }
+  {
+    LaunchScope ls("si_sdr_backward_row_kernel", st);
+    si_sdr_backward_row_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(p2, chunks, grad_out, coef);
+    PBB_CUDA(cudaGetLastError());
+  }
+  const auto blocks = [](long long count) {
+    return (unsigned)std::min<long long>((count + kSxrThreads - 1) / kSxrThreads, 1ll << 20);
+  };
+  if (grad_estimation && estimation_rows > 0) {
+    LaunchScope ls("si_sdr_backward_kernel", st);
+    si_sdr_backward_kernel<true><<<blocks(estimation_rows * n), kSxrThreads, 0, st>>>(
+        reference, estimation, reference_offsets, estimation_offsets, n, alpha, coef, estimation_rows,
+        estimation_row_start, estimation_row_index, grad_estimation);
+    PBB_CUDA(cudaGetLastError());
+  }
+  if (grad_reference && reference_rows > 0) {
+    LaunchScope ls("si_sdr_backward_kernel", st);
+    si_sdr_backward_kernel<false><<<blocks(reference_rows * n), kSxrThreads, 0, st>>>(
+        reference, estimation, reference_offsets, estimation_offsets, n, alpha, coef, reference_rows,
+        reference_row_start, reference_row_index, grad_reference);
+    PBB_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
 int pbb_input_sxr(const double* S, const double* N, int K, int D, int average_sources, int average_channels,
                   double* sdr, double* sir, double* snr, void* stream) {
   PBB_CHECK_ARG(S != nullptr, 1, "S is null");

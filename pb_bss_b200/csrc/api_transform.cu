@@ -218,6 +218,86 @@ int pbb_istft(const void* X, long long rows, int frames, int size, int shift, in
   return 0;
 }
 
+int pbb_istft_backward(const double* grad_out, long long rows, int frames, int size, int shift, int window_length,
+                       int crop, long long n_out, const double* synthesis_window, const double* twiddle,
+                       void* grad_X, void* stream) {
+  const int logN = log2_size(size);
+  PBB_CHECK_ARG(grad_out != nullptr || n_out == 0, 1, "grad_out is null");
+  PBB_CHECK_ARG(rows > 0, 2, "rows must be positive");
+  PBB_CHECK_ARG(frames > 0, 3, "frames must be positive");
+  PBB_CHECK_ARG(logN > 0, 4, "size must be a power of two in [64, 4096]");
+  PBB_CHECK_ARG(window_length >= 1 && window_length <= size, 6, "window_length must be in [1, size]");
+  PBB_CHECK_ARG(shift >= 1 && shift <= window_length, 5, "shift must be in [1, window_length]");
+  const long long full = (long long)frames * shift + window_length - shift;
+  PBB_CHECK_ARG(crop >= 0, 7, "crop must be non-negative");
+  PBB_CHECK_ARG(n_out >= 0 && crop + n_out <= full, 8, "crop + n_out exceeds frames * shift + window_length - shift");
+  PBB_CHECK_ARG(synthesis_window != nullptr, 9, "synthesis_window is null");
+  PBB_CHECK_ARG(twiddle != nullptr, 10, "twiddle is null");
+  PBB_CHECK_ARG(grad_X != nullptr, 11, "grad_X is null");
+  StftParams p{};
+  p.x = grad_out;
+  p.rows = rows;
+  p.n = n_out;
+  p.logM = logN - 1;
+  p.shift = shift;
+  p.wl = window_length;
+  p.offset = crop;
+  p.frames = frames;
+  p.fpc = frames_per_cta(size, rows, frames);
+  p.tiles = (frames + p.fpc - 1) / p.fpc;
+  p.window = synthesis_window;
+  p.tw = reinterpret_cast<const double2*>(twiddle);
+  p.out = reinterpret_cast<double2*>(grad_X);
+  return fft_launch(istft_backward_kernel, "istft_backward_kernel", rows, frames, p.fpc, size, &p,
+                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+size_t pbb_stft_backward_workspace_bytes(long long rows, int frames, int window_length) {
+  return pbb_istft_workspace_bytes(rows, frames, window_length);
+}
+
+int pbb_stft_backward(const void* grad_X, long long rows, long long n, int size, int shift, int window_length,
+                      int offset, int frames, const double* window, const double* twiddle, void* workspace,
+                      size_t workspace_bytes, double* grad_x, void* stream) {
+  const int logN = log2_size(size);
+  PBB_CHECK_ARG(grad_X != nullptr, 1, "grad_X is null");
+  PBB_CHECK_ARG(rows > 0, 2, "rows must be positive");
+  PBB_CHECK_ARG(n >= 0, 3, "n must be non-negative");
+  PBB_CHECK_ARG(logN > 0, 4, "size must be a power of two in [64, 4096]");
+  PBB_CHECK_ARG(window_length >= 1 && window_length <= size, 6, "window_length must be in [1, size]");
+  PBB_CHECK_ARG(shift >= 1 && shift <= window_length, 5, "shift must be in [1, window_length]");
+  PBB_CHECK_ARG(offset >= 0 && offset < window_length, 7, "offset must be in [0, window_length)");
+  PBB_CHECK_ARG(frames > 0, 8, "frames must be positive");
+  PBB_CHECK_ARG(window != nullptr, 9, "window is null");
+  PBB_CHECK_ARG(twiddle != nullptr, 10, "twiddle is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_stft_backward_workspace_bytes(rows, frames, window_length),
+                11, "workspace too small (pbb_stft_backward_workspace_bytes)");
+  PBB_CHECK_ARG(grad_x != nullptr || n == 0, 13, "grad_x is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  IstftParams p{};
+  p.X = reinterpret_cast<const double2*>(grad_X);
+  p.rows = rows;
+  p.logM = logN - 1;
+  p.wl = window_length;
+  p.frames = frames;
+  p.fpc = frames_per_cta(size, rows, frames);
+  p.tiles = (frames + p.fpc - 1) / p.fpc;
+  p.synthesis = window;
+  p.tw = reinterpret_cast<const double2*>(twiddle);
+  p.framebuf = reinterpret_cast<double*>(workspace);
+  const int rc = fft_launch(stft_backward_kernel, "stft_backward_kernel", rows, frames, p.fpc,
+                            size, &p, st);
+  if (rc != 0 || n == 0) return rc;
+  // sample s of row r sums the frames t covering padded position s + offset; samples no frame covers get 0
+  long long blocks = (rows * n + 255) / 256;
+  if (blocks > 4ll * 32 * sm_count()) blocks = 4ll * 32 * sm_count();
+  LaunchScope ls("overlap_add_kernel", st);
+  overlap_add_kernel<<<(unsigned)blocks, 256, 0, st>>>(p.framebuf, rows, frames, window_length, shift, offset, n,
+                                                       grad_x);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 int pbb_gammatone_chunk_length(long long rows, int n, long long N) {
   int L = PBB_GAMMATONE_CHUNK_MAX;
   if (rows <= 0 || n <= 0 || N <= 0) return L;

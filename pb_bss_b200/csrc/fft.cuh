@@ -14,7 +14,10 @@ constexpr int kFftMinSize = 64, kFftMaxSize = 4096;
 constexpr int kFftFrameBudget = 4096;
 
 // ---- forward transform ----------------------------------------------------------------------------------------------
-enum { STFT_PLAIN = 0, STFT_GRIFFIN_LIM = 1, STFT_MISI = 2 };
+// STFT_ISTFT_BACKWARD: the gradient of the iSTFT wrt its spectrum, the STFT of the incoming gradient g (x = g,
+// window = synthesis window, offset = crop) scaled to (2 / size) X_k for 0 < k < size/2 and (1 / size) X_k at k = 0 and
+// size/2 (pbb_istft_backward)
+enum { STFT_PLAIN = 0, STFT_GRIFFIN_LIM = 1, STFT_MISI = 2, STFT_ISTFT_BACKWARD = 3 };
 
 struct StftParams {
   const void* x;        // (rows, n) real signal; MISI: x_hat (K, n) float64
@@ -32,7 +35,7 @@ struct StftParams {
 // (zero outside [0, n): fading and end padding are never materialised), windowed and packed into M complex points per
 // frame, transformed, split into M + 1 bins and written as contiguous rows.
 template <class TI, int MODE>
-__global__ void __launch_bounds__(kFftThreads) stft_kernel(StftParams p) {
+__device__ __forceinline__ void stft_body(const StftParams& p) {
   extern __shared__ double2 smem[];
   const int M = 1 << p.logM, F = M + 1;
   const long long row = blockIdx.x / p.tiles;
@@ -87,8 +90,13 @@ __global__ void __launch_bounds__(kFftThreads) stft_kernel(StftParams p) {
       const double2 t = cmul(w, fo);
       X = make_double2(fe.x + t.x, fe.y + t.y);
     }
+    if (MODE == STFT_ISTFT_BACKWARD) {
+      // powers of two: exact
+      const double sc = (k == 0 || k == M) ? 0.5 / M : 1.0 / M;
+      X = make_double2(X.x * sc, X.y * sc);
+    }
     p.out[obase + i] = X;
-    if (MODE != STFT_PLAIN) {
+    if (MODE == STFT_GRIFFIN_LIM || MODE == STFT_MISI) {
       const double2 T = __ldg(p.X + obase + i);
       // exp(i angle(X)) as X / |X| (within rounding of cos / sin of atan2, without their reduction stack frame);
       // exp(i angle(0)) = 1
@@ -97,6 +105,13 @@ __global__ void __launch_bounds__(kFftThreads) stft_kernel(StftParams p) {
       p.out_dash[obase + i] = make_double2(mag * c, mag * s);
     }
   }
+}
+
+template <class TI, int MODE>
+__global__ void __launch_bounds__(kFftThreads) stft_kernel(StftParams p) { stft_body<TI, MODE>(p); }
+
+__global__ void __launch_bounds__(kFftThreads) istft_backward_kernel(StftParams p) {
+  stft_body<double, STFT_ISTFT_BACKWARD>(p);
 }
 
 // ---- inverse transform ----------------------------------------------------------------------------------------------
@@ -109,9 +124,14 @@ struct IstftParams {
   double* framebuf;  // (rows, frames, wl): windowed frames
 };
 
-// irfft(X_t, n=size)[:wl] * synthesis window for fpc frames of one row.  The imaginary parts of the DC and Nyquist
-// bins are ignored, as np.fft.irfft does.
-__global__ void __launch_bounds__(kFftThreads) istft_frames_kernel(IstftParams p) {
+// ISTFT_PLAIN: irfft(X_t, n=size)[:wl] * synthesis window for fpc frames of one row.  The imaginary parts of the DC
+// and Nyquist bins are ignored, as np.fft.irfft does.
+// ISTFT_STFT_BACKWARD: the per-frame gradient of the STFT wrt its windowed frame, size irfft(G^)_j with G^_k = G_k / 2
+// for 0 < k < size/2 and G^_k = G_k at k = 0 and size/2, times the analysis window (`synthesis` holds it), X = G
+// (pbb_stft_backward)
+enum { ISTFT_PLAIN = 0, ISTFT_STFT_BACKWARD = 1 };
+template <int MODE>
+__device__ __forceinline__ void istft_frames_body(const IstftParams& p) {
   extern __shared__ double2 smem[];
   const int M = 1 << p.logM, F = M + 1;
   const long long row = blockIdx.x / p.tiles;
@@ -129,7 +149,11 @@ __global__ void __launch_bounds__(kFftThreads) istft_frames_kernel(IstftParams p
       Z = make_double2(0.5 * (x0 + xm), 0.5 * (x0 - xm));
     } else {
       // Fe = (X_k + conj X_{M-k}) / 2, Fo = (X_k - conj X_{M-k}) / 2 * conj W^k, Z_k = Fe + i Fo
-      const double2 a = __ldg(x + k), b = __ldg(x + M - k);
+      double2 a = __ldg(x + k), b = __ldg(x + M - k);
+      if (MODE == ISTFT_STFT_BACKWARD) {
+        a = make_double2(0.5 * a.x, 0.5 * a.y);
+        b = make_double2(0.5 * b.x, 0.5 * b.y);
+      }
       const double2 fe = make_double2(0.5 * (a.x + b.x), 0.5 * (a.y - b.y));
       const double2 fo = cmul(make_double2(0.5 * (a.x - b.x), 0.5 * (a.y + b.y)), __ldg(p.tw + k));
       Z = make_double2(fe.x - fo.y, fe.y + fo.x);
@@ -143,8 +167,15 @@ __global__ void __launch_bounds__(kFftThreads) istft_frames_kernel(IstftParams p
   for (int i = threadIdx.x; i < nf * p.wl; i += blockDim.x) {
     const int f = i / p.wl, j = i - f * p.wl;
     const double2 v = z[(f << p.logM) + (j >> 1)];
-    out[i] = __ldg(p.synthesis + j) * (((j & 1) ? v.y : v.x) / m);
+    if (MODE == ISTFT_PLAIN) out[i] = __ldg(p.synthesis + j) * (((j & 1) ? v.y : v.x) / m);
+    else out[i] = __ldg(p.synthesis + j) * (2.0 * ((j & 1) ? v.y : v.x));  // size irfft = 2 M (v / M)
   }
+}
+
+__global__ void __launch_bounds__(kFftThreads) istft_frames_kernel(IstftParams p) { istft_frames_body<ISTFT_PLAIN>(p); }
+
+__global__ void __launch_bounds__(kFftThreads) stft_backward_kernel(IstftParams p) {
+  istft_frames_body<ISTFT_STFT_BACKWARD>(p);
 }
 
 // out[r][m] = sum over the frames t covering sample m + crop of frame_t[m + crop - t shift], in increasing t from 0.0:

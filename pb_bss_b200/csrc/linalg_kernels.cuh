@@ -167,7 +167,8 @@ __host__ __device__ inline size_t solve_smem_per_warp(int D, int R) {
 }
 
 // ---- general complex solve A X = B with partial pivoting (np.linalg.solve / zgesv) ----
-// A (n, D, D), B (n, D, R) -> X (n, D, R).  hermitize: use (A + A^H) / 2 (beamformer.py:246-248).
+// A (n, D, D), B (n, D, R) -> X (n, D, R).  hermitize: use (A + A^H) / 2 (beamformer.py:246-248); hermitize = 2 solves
+// with A^H (the Souden backward, pbb_souden_backward).
 // An exactly singular system (zero pivot: LinAlgError in the reference) takes the reference's fallback,
 // np.linalg.lstsq (beamformer.py:251-256, math/solve.py:95-114): the minimum-norm solution X = A^+ B.  A Hermitian A
 // (the PSD matrices of this path) is pseudo-inverted through its eigendecomposition, eigenvalues below
@@ -176,7 +177,7 @@ __host__ __device__ inline size_t solve_smem_per_warp(int D, int R) {
 // all-zero A gives X = 0 (test_beamformer.py:211-376).  Non-finite input propagates as NaN, as it does in LAPACK.
 // status (may be null) is only set when the fallback is unavailable (D > kLstsqMaxD).
 // strict != 0 is plain np.linalg.solve (get_mvdr_vector_merl, beamformer.py:277): a zero pivot takes no fallback and
-// sets status instead; x of that system is then undefined.  fallback (may be null) is set to 1 when any system of the
+// sets status instead; x of that system is then undefined.  strict = 2 writes NaN there instead (no status).  fallback (may be null) is set to 1 when any system of the
 // batch met a zero pivot, i.e. when the reference's stable_solve left np.linalg.solve for its per-matrix loop.
 __global__ void solve_kernel(const double2* __restrict__ a, const double2* __restrict__ b, int n, int D, int R,
                              int hermitize, double2* __restrict__ x, int* status, int warps, int strict = 0,
@@ -194,7 +195,10 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
   for (int i = lane; i < D * D; i += 32) {
     const int r = i / D, c = i - r * D;
     const double2 u = am[i];
-    if (hermitize) {
+    if (hermitize == 2) {
+      const double2 v = am[c * D + r];
+      A[i] = make_double2(v.x, -v.y);
+    } else if (hermitize) {
       const double2 v = am[c * D + r];
       A[i] = make_double2(0.5 * (u.x + v.x), 0.5 * (u.y - v.y));
     } else {
@@ -246,7 +250,7 @@ __global__ void solve_kernel(const double2* __restrict__ a, const double2* __res
     __syncwarp();
   }
   if (singular && fallback && lane == 0) atomicOr(fallback, 1);
-  if (nonfinite) {
+  if (nonfinite || (singular && strict == 2)) {
     for (int i = lane; i < D * R; i += 32) X[i] = make_double2(NAN, NAN);
     __syncwarp();
   } else if (!singular) {
@@ -519,6 +523,184 @@ __global__ void psd_finalize_kernel(const double* __restrict__ part, int nch, in
     else if (si.kind == 1) { od[2 * (si.d * D + si.e)] = v; od[2 * (si.e * D + si.d)] = v; }
     else { od[2 * (si.d * D + si.e) + 1] = -v; od[2 * (si.e * D + si.d) + 1] = v; }
   }
+}
+
+// ================================ backward passes (pb_bss_b200 autograd) ================================
+// Gradients follow PyTorch's convention for a real loss L: grad z = dL/dRe z + i dL/dIm z.  fp64, fixed-order sums, no
+// atomics.
+
+// ---- Souden MVDR, w = Phi[:, r] / max(Re tr Phi, eps) per bin (pbb_souden_backward) ----
+// grad Phi = g e_r^T / lambda - (Re(g^H Phi[:, r]) / lambda^2) I for lambda = Re tr Phi > eps, g e_r^T / eps otherwise.
+// One CTA per bin, thread i writes row i.
+__global__ void souden_backward_kernel(const double2* __restrict__ phi, const double2* __restrict__ g, int n, int D,
+                                       int r, double eps, double2* __restrict__ gphi) {
+  const int m = blockIdx.x, i = threadIdx.x;
+  if (i >= D) return;
+  const double2* __restrict__ ph = phi + (size_t)m * D * D;
+  const double2* __restrict__ gm = g + (size_t)m * D;
+  double tr = 0.0, c = 0.0;
+  for (int d = 0; d < D; ++d) tr += ph[d * D + d].x;  // the forward's order
+  for (int d = 0; d < D; ++d) c += gm[d].x * ph[d * D + r].x + gm[d].y * ph[d * D + r].y;
+  const bool scaled = tr > eps;
+  const double inv = 1.0 / (scaled ? tr : eps), diag = scaled ? c * inv * inv : 0.0;
+  const double2 gi = gm[i];
+  double2* __restrict__ o = gphi + (size_t)m * D * D + (size_t)i * D;
+  for (int j = 0; j < D; ++j) {
+    double2 v = j == r ? make_double2(gi.x * inv, gi.y * inv) : make_double2(0.0, 0.0);
+    if (j == i) v.x -= diag;
+    o[j] = v;
+  }
+}
+
+// grad N = -grad X Phi^H per bin, one thread per entry
+__global__ void souden_noise_backward_kernel(const double2* __restrict__ gx, const double2* __restrict__ phi, int n,
+                                             int D, double2* __restrict__ gn) {
+  const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * D * D) return;
+  const long long m = idx / (D * D);
+  const int i = (int)(idx - m * D * D) / D, j = (int)(idx - m * D * D) % D;
+  const double2* __restrict__ x = gx + m * D * D + (size_t)i * D;
+  const double2* __restrict__ p = phi + m * D * D + (size_t)j * D;
+  double2 s = make_double2(0.0, 0.0);
+  for (int k = 0; k < D; ++k) {
+    const double2 q = cmulc(x[k], p[k]);
+    s.x += q.x; s.y += q.y;
+  }
+  gn[idx] = make_double2(-s.x, -s.y);
+}
+
+// ---- apply_beamforming_vector, out[b][f][t] = sum_a conj(w[b][f][a]) Y[f][a][t] ----
+// grad w[b][f][a] = sum_t Y[f][a][t] conj(g[b][f][t]): one warp per (b, f, a), lanes stride over t, then a fixed
+// butterfly.
+template <typename CT>
+__global__ void apply_bf_vector_backward_kernel(const CT* __restrict__ Y, const double2* __restrict__ g, int B, int F,
+                                                int D, int T, double2* __restrict__ gw) {
+  const long long w = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= (long long)B * F * D) return;
+  const long long bf = w / D;
+  const int a = (int)(w - bf * D), f = (int)(bf % F);
+  const CT* __restrict__ y = Y + ((size_t)f * D + a) * T;
+  const double2* __restrict__ gr = g + (size_t)bf * T;
+  double2 s = make_double2(0.0, 0.0);
+  for (int t = lane; t < T; t += 32) {
+    const double2 q = cmulc(ld_cplx(y + t), __ldg(gr + t));
+    s.x += q.x; s.y += q.y;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    s.x += __shfl_xor_sync(0xffffffffu, s.x, o);
+    s.y += __shfl_xor_sync(0xffffffffu, s.y, o);
+  }
+  if (lane == 0) gw[w] = s;
+}
+
+// grad Y[f][a][t] = sum_b w[b][f][a] g[b][f][t] in increasing b (B beamformers sharing one mix; B = 1 otherwise).  Bins
+// beyond gridDim.y are taken in strides of gridDim.y.
+__global__ void apply_bf_mix_backward_kernel(const double2* __restrict__ w, const double2* __restrict__ g, int B, int F,
+                                             int D, int T, double2* __restrict__ gY) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  for (int f = blockIdx.y; f < F; f += gridDim.y) {
+    for (int a = 0; a < D; ++a) {
+      double2 s = make_double2(0.0, 0.0);
+      for (int b = 0; b < B; ++b) {
+        const double2 q = cmul(__ldg(w + ((size_t)b * F + f) * D + a), __ldg(g + ((size_t)b * F + f) * T + t));
+        s.x += q.x; s.y += q.y;
+      }
+      gY[((size_t)f * D + a) * T + t] = s;
+    }
+  }
+}
+
+// ---- get_power_spectral_density_matrix, Phi_fk = sum_t w_fkt y_ft y_ft^H (pbb_power_spectral_density_backward) ----
+// w = m / max(S, 1e-10) with S = sum_t m (normalize), m (no normalize), 1 / T (no mask).  With G = grad Phi and
+// H = G + G^H:  grad y_t = sum_k w_kt H_k y_t;  dL/dm_kt = (Re(y^H G_k y) - Re<G_k, Phi_k>) / S_k while S_k > 1e-10,
+// Re(y^H G_k y) / max(S_k, 1e-10) otherwise or without normalize (times 1 / 1 there).  Re(y^H G y) = Re(y^H H y) / 2.
+// One CTA per (tile of kPsdBwdThreads frames, bin); thread = frame.  The frame's y and grad y live in shared memory
+// ([d][thread]), H_k is staged per source, so Y is read once for all K sources.
+constexpr int kPsdBwdThreads = 64;
+__host__ __device__ inline size_t psd_backward_smem(int D, int K) {
+  return (size_t)(D * D + 2 * D * kPsdBwdThreads) * sizeof(double2) + (size_t)3 * K * sizeof(double);
+}
+
+template <typename CT>
+__global__ void __launch_bounds__(kPsdBwdThreads) psd_backward_kernel(
+    const CT* __restrict__ Y, const double* __restrict__ mask, const double2* __restrict__ psd,
+    const double2* __restrict__ gpsd, int F, int D, int T, int K, int normalize, double2* __restrict__ gy_out,
+    double* __restrict__ gm_out) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  double2* H = reinterpret_cast<double2*>(smem_raw);
+  double2* ys = H + D * D;
+  double2* gys = ys + D * kPsdBwdThreads;
+  double* scale = reinterpret_cast<double*>(gys + D * kPsdBwdThreads);  // w = m * scale[k]
+  double* cterm = scale + K;                                             // Re<G_k, Phi_k> (0 where it drops out)
+  double* mscale = cterm + K;                                            // dL/dm = (q - cterm) * mscale
+  const int tiles = (T + kPsdBwdThreads - 1) / kPsdBwdThreads;
+  const int f = blockIdx.x / tiles, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int t = (blockIdx.x - f * tiles) * kPsdBwdThreads + tid;
+  // per-source scalars: one warp per source, lanes stride, fixed butterfly
+  for (int k = warp; k < K; k += kPsdBwdThreads / 32) {
+    const double* __restrict__ mk = mask ? mask + ((size_t)f * K + k) * T : nullptr;
+    const double2* __restrict__ G = gpsd + ((size_t)f * K + k) * D * D;
+    const double2* __restrict__ P = psd + ((size_t)f * K + k) * D * D;
+    double S = 0.0, c = 0.0;
+    if (mk && normalize)
+      for (int i = lane; i < T; i += 32) S += __ldg(mk + i);
+    for (int i = lane; i < D * D; i += 32) c += G[i].x * P[i].x + G[i].y * P[i].y;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      S += __shfl_xor_sync(0xffffffffu, S, o);
+      c += __shfl_xor_sync(0xffffffffu, c, o);
+    }
+    if (lane == 0) {
+      if (!mk) {
+        scale[k] = 1.0 / (double)T;
+      } else if (normalize) {
+        scale[k] = 1.0 / fmax(S, 1e-10);
+        cterm[k] = S > 1e-10 ? c : 0.0;
+        mscale[k] = scale[k];
+      } else {
+        scale[k] = 1.0;
+        cterm[k] = 0.0;
+        mscale[k] = 1.0;
+      }
+    }
+  }
+  const bool live = t < T;
+  if (live)
+    for (int d = 0; d < D; ++d) {
+      ys[d * kPsdBwdThreads + tid] = ld_cplx(Y + ((size_t)f * D + d) * T + t);
+      gys[d * kPsdBwdThreads + tid] = make_double2(0.0, 0.0);
+    }
+  for (int k = 0; k < K; ++k) {
+    __syncthreads();
+    const double2* __restrict__ G = gpsd + ((size_t)f * K + k) * D * D;
+    for (int i = tid; i < D * D; i += kPsdBwdThreads) {
+      const int r = i / D, c = i - r * D;
+      const double2 a = G[i], b = G[c * D + r];
+      H[i] = make_double2(a.x + b.x, a.y - b.y);
+    }
+    __syncthreads();
+    if (!live) continue;
+    const double wk = (mask ? __ldg(mask + ((size_t)f * K + k) * T + t) : 1.0) * scale[k];
+    double q = 0.0;
+    for (int i = 0; i < D; ++i) {
+      double2 u = make_double2(0.0, 0.0);
+      for (int j = 0; j < D; ++j) {
+        const double2 p = cmul(H[i * D + j], ys[j * kPsdBwdThreads + tid]);
+        u.x += p.x; u.y += p.y;
+      }
+      const double2 y = ys[i * kPsdBwdThreads + tid];
+      q += y.x * u.x + y.y * u.y;  // Re(conj(y_i) u_i)
+      double2& gy = gys[i * kPsdBwdThreads + tid];
+      gy.x += wk * u.x;
+      gy.y += wk * u.y;
+    }
+    if (mask && gm_out) gm_out[((size_t)f * K + k) * T + t] = (0.5 * q - cterm[k]) * mscale[k];
+  }
+  if (live && gy_out)
+    for (int d = 0; d < D; ++d) gy_out[((size_t)f * D + d) * T + t] = gys[d * kPsdBwdThreads + tid];
 }
 
 }  // namespace pbb

@@ -160,6 +160,47 @@ __global__ void __launch_bounds__(kSxrThreads) si_sdr_ratio_kernel(const double*
   if (threadIdx.x == 0) out[blockIdx.x] = db10(__ddiv_rn(v[0], v[1]));
 }
 
+// ---- SI-SDR backward (pbb_si_sdr_backward) ----
+// With p = alpha r, q = e - p (rounded as pass 2 forms them), P = sum p^2 and Q = sum q^2 of a row and c = 20 / ln 10:
+// ds/de = c (p / P - q / Q), ds/dr = c alpha (1 / P + 1 / Q) q.  Per row (one CTA): P, Q from the pass-2 partials,
+// then coef = (c g / P, c g / Q) for the incoming gradient g of the row.
+__global__ void __launch_bounds__(kSxrThreads) si_sdr_backward_row_kernel(const double* __restrict__ partial,
+                                                                          long long chunks,
+                                                                          const double* __restrict__ grad_out,
+                                                                          double* __restrict__ coef) {
+  double v[2];
+  row_totals<2>(partial, chunks, v);
+  if (threadIdx.x == 0) {
+    const double cg = 20.0 / log(10.0) * grad_out[blockIdx.x];
+    coef[2 * (size_t)blockIdx.x] = cg / v[0];
+    coef[2 * (size_t)blockIdx.x + 1] = cg / v[1];
+  }
+}
+
+// The gradient wrt one operand, one thread per element of its own (unbroadcast) rows: element (u, i) sums the rows
+// index[start[u]] .. index[start[u + 1] - 1] that read own row u, in that order.  WRT_E: estimation, else reference.
+template <bool WRT_E>
+__global__ void __launch_bounds__(kSxrThreads) si_sdr_backward_kernel(
+    const double* __restrict__ r, const double* __restrict__ e, const long long* __restrict__ roff,
+    const long long* __restrict__ eoff, long long n, const double* __restrict__ alpha, const double* __restrict__ coef,
+    long long own_rows, const long long* __restrict__ start, const long long* __restrict__ index,
+    double* __restrict__ out) {
+  const long long total = own_rows * n;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const long long u = idx / n, i = idx - u * n;
+    double s = 0.0;
+    for (long long j = start[u]; j < start[u + 1]; ++j) {
+      const long long row = index[j];
+      const double a = alpha[row], cp = coef[2 * row], cq = coef[2 * row + 1];
+      const double p = __dmul_rn(a, __ldg(r + roff[row] + i));
+      const double q = __dsub_rn(__ldg(e + eoff[row] + i), p);
+      s += WRT_E ? cp * p - cq * q : a * (cp + cq) * q;
+    }
+    out[idx] = s;
+  }
+}
+
 // np.sum of n values get(0) .. get(n - 1) (n <= 128 here): a left-to-right loop below 8 values, else NumPy's pairwise
 // block of 8 accumulators, their fixed combination, then the remainder in order.
 template <class F>

@@ -9,20 +9,24 @@ A broadcast operand is read in place through a row-offset table, never materiali
 and a pair's value does not depend on the rest of the batch.
 
 NumPy in gives NumPy out (an np.float64 for 1-D input); a CUDA tensor in gives a float64 CUDA tensor out, and the
-call only enqueues work on the current stream.  Documented difference: NumPy's divide-by-zero and invalid-value
+call only enqueues work on the current stream.  CUDA tensors that require grad get a graph: the backward runs
+pbb_si_sdr_backward, ds/de = (20 / ln 10)(p / P - q / Q) and ds/dr = (20 alpha / ln 10)(1 / P + 1 / Q) q with
+p = alpha r, q = e - p, P = |p|^2, Q = |q|^2; a broadcast operand's gradient sums the rows that share it.  Rows whose
+value is inf or nan (r = 0, e = 2 r, ...) give non-finite gradients.  Double backward raises.  Documented difference: NumPy's divide-by-zero and invalid-value
 RuntimeWarnings are not emitted; the inf / nan values are the same.
 """
 import math
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from .. import _device, _lib
 
 
 def _operand(x, shape):
-    """(data, offsets): x as a contiguous float64 CUDA tensor in its own (unbroadcast) shape, and the int64 element
-    offset of each of the broadcast shape's rows in it."""
+    """(data, offsets, host offsets): x as a contiguous float64 CUDA tensor in its own (unbroadcast) shape, and the
+    int64 element offset of each of the broadcast shape's rows in it (on the device and as a NumPy array)."""
     lead, n = shape[:-1], shape[-1]
     x = x.reshape((1,) * (len(shape) - x.dim()) + tuple(x.shape))
     if x.shape[-1] != n:                      # a broadcast last axis is materialised (one sample per row)
@@ -30,7 +34,8 @@ def _operand(x, shape):
     x = x.contiguous()
     own = tuple(x.shape[:-1])
     offsets = np.broadcast_to(np.arange(math.prod(own), dtype=np.int64).reshape(own) * n, lead).reshape(-1)
-    return x, _device.to_device(np.ascontiguousarray(offsets))
+    offsets = np.ascontiguousarray(offsets)
+    return x, _device.to_device(offsets), offsets
 
 
 def _is_float64(x):
@@ -56,19 +61,67 @@ def si_sdr(reference, estimation):
     assert _is_float64(e), e.dtype
     if len(shape) == 0:
         raise np.exceptions.AxisError(-1, 0)
-    lib = _lib.load()
+    _lib.load()
     lead, n = shape[:-1], shape[-1]
     rows = math.prod(lead)
-    out = _device.empty(lead, torch.float64)
     if rows:
-        rd, ro = _operand(_device.to_device(r), shape)
-        ed, eo = _operand(_device.to_device(e), shape)
+        rd, ro, ro_host = _operand(_device.to_device(r), shape)
+        ed, eo, eo_host = _operand(_device.to_device(e), shape)
+        out = _SiSdr.apply(rd, ed, ro, eo, ro_host, eo_host, lead, n)
+    else:
+        out = _device.empty(lead, torch.float64)
+    if not like_numpy:
+        return out
+    v = out.cpu().numpy()
+    return np.float64(v) if v.ndim == 0 else v
+
+
+def _row_table(offsets, n, own_rows):
+    """(start, index) on the device: the rows that read own row u of an operand are index[start[u]:start[u + 1]], in
+    increasing row order."""
+    own = offsets // n
+    index = np.argsort(own, kind='stable').astype(np.int64)
+    start = np.concatenate([[0], np.cumsum(np.bincount(own, minlength=own_rows))]).astype(np.int64)
+    return _device.to_device(start), _device.to_device(index)
+
+
+class _SiSdr(torch.autograd.Function):
+    """reference / estimation in their own shapes (float64 CUDA tensors) and their row offsets -> SI-SDR (lead) by
+    pbb_si_sdr; backward pbb_si_sdr_backward."""
+
+    @staticmethod
+    def forward(ctx, rd, ed, ro, eo, ro_host, eo_host, lead, n):
+        lib = _lib.load()
+        rows = math.prod(lead)
+        out = _device.empty(lead, torch.float64)
         nbytes = lib.pbb_si_sdr_workspace_bytes(rows, n)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
         _lib.check(lib.pbb_si_sdr(_device.ptr(rd) if n else None, _device.ptr(ed) if n else None, _device.ptr(ro),
                                   _device.ptr(eo), rows, n, _device.ptr(ws), nbytes, _device.ptr(out),
                                   _device.stream_ptr()), 'pbb_si_sdr')
-    if not like_numpy:
+        # the row tables of the backward are built here, where a host-to-device copy may synchronise
+        tables = [_row_table(off, n, x.numel() // n) if need and n else (None, None)
+                  for need, off, x in zip(ctx.needs_input_grad[:2], (ro_host, eo_host), (rd, ed))]
+        ctx.save_for_backward(rd, ed, ro, eo)
+        ctx.args = (rows, n, tables)
         return out
-    v = out.cpu().numpy()
-    return np.float64(v) if v.ndim == 0 else v
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        rd, ed, ro, eo = ctx.saved_tensors
+        rows, n, ((rs, ri), (es, ei)) = ctx.args
+        need_r, need_e = ctx.needs_input_grad[:2]
+        gr = torch.zeros_like(rd) if need_r else None
+        ge = torch.zeros_like(ed) if need_e else None
+        if n and (need_r or need_e):
+            lib = _lib.load()
+            g = grad.to(torch.float64).contiguous()
+            nbytes = lib.pbb_si_sdr_backward_workspace_bytes(rows, n)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=rd.device)
+            _lib.check(lib.pbb_si_sdr_backward(
+                _device.ptr(rd), _device.ptr(ed), _device.ptr(ro), _device.ptr(eo), rows, n, _device.ptr(g),
+                rd.numel() // n, _device.ptr(rs), _device.ptr(ri), ed.numel() // n, _device.ptr(es), _device.ptr(ei),
+                _device.ptr(ws), nbytes, _device.ptr(gr), _device.ptr(ge), _device.stream_ptr()),
+                'pbb_si_sdr_backward')
+        return gr, ge, None, None, None, None, None, None

@@ -3,9 +3,16 @@
 Shapes follow the reference (beamformer.py:1-12): X (F, D, T), mask (F, K, T),
 PSD (F, K, D, D); leading dims are independent.  numpy in -> numpy out, CUDA
 tensors in -> CUDA tensors out.  Small matrices are complex128 on the device.
+
+get_power_spectral_density_matrix, get_mvdr_vector_souden and
+apply_beamforming_vector are differentiable for CUDA tensors that require grad:
+their backward passes are the device kernels of pbb_*_backward (fp64, gradients
+in the input's dtype, double backward raises).  The other functions return
+outputs without a graph.
 """
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from .. import _device, _lib
 from .linalg import eigh
@@ -50,14 +57,13 @@ def get_power_spectral_density_matrix(observation, mask=None, sensor_dim=-2,
     (..., sources, sensors, sensors)."""
     like_numpy = not _device.is_tensor(observation)
     obs = _device.to_device(observation)
-    code = _device.complex_dtype_code(obs)
+    _device.complex_dtype_code(obs)
     nd = obs.dim()
     sensor_dim, source_dim, time_dim = (d % nd - nd for d in (sensor_dim, source_dim, time_dim))
     order = [i for i in range(-nd, 0) if i not in (sensor_dim, time_dim)] + [sensor_dim, time_dim]
     obs = obs.permute(*[i % nd for i in order])
     obs, lead = _flat(obs, 2)
     F, D, T = obs.shape
-    lib = _lib.load()
     single = False
     if mask is None:
         m, K = None, 1
@@ -73,13 +79,7 @@ def get_power_spectral_density_matrix(observation, mask=None, sensor_dim=-2,
             m = m.permute(*[i % nd for i in morder])
         K = m.shape[-2]
         m = m.expand(*lead, K, T).reshape(F, K, T).contiguous()
-    psd = _device.empty((F, K, D, D), torch.complex128)
-    nbytes = lib.pbb_psd_workspace_bytes(F, T, D, K)
-    ws = _device.workspace(nbytes)
-    _lib.check(lib.pbb_power_spectral_density(
-        _device.ptr(obs), code, F, D, T, _device.ptr(m), K, int(bool(normalize)),
-        _device.ptr(psd), _device.ptr(ws), nbytes, _device.stream_ptr()),
-        'pbb_power_spectral_density')
+    psd = _Psd.apply(obs, m, K, bool(normalize))
     if single:
         out = psd.reshape(*lead, D, D)
     else:
@@ -88,6 +88,43 @@ def get_power_spectral_density_matrix(observation, mask=None, sensor_dim=-2,
             # PSD shape (sources, ..., sensors, sensors), beamformer.py:156-158
             out = out.movedim(-3, source_dim % nd)
     return _device.to_host(out.contiguous(), like_numpy)
+
+
+class _Psd(torch.autograd.Function):
+    """observation (F, D, T) complex64 / complex128, mask (F, K, T) float64 or None -> PSD (F, K, D, D) by
+    pbb_power_spectral_density; backward pbb_power_spectral_density_backward."""
+
+    @staticmethod
+    def forward(ctx, obs, m, K, normalize):
+        F, D, T = obs.shape
+        code = _device.complex_dtype_code(obs)
+        lib = _lib.load()
+        psd = _device.empty((F, K, D, D), torch.complex128)
+        nbytes = lib.pbb_psd_workspace_bytes(F, T, D, K)
+        ws = _device.workspace(nbytes)
+        _lib.check(lib.pbb_power_spectral_density(
+            _device.ptr(obs), code, F, D, T, _device.ptr(m), K, int(normalize),
+            _device.ptr(psd), _device.ptr(ws), nbytes, _device.stream_ptr()),
+            'pbb_power_spectral_density')
+        ctx.save_for_backward(obs, m, psd)
+        ctx.args = (code, K, normalize)
+        return psd
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        obs, m, psd = ctx.saved_tensors
+        code, K, normalize = ctx.args
+        F, D, T = obs.shape
+        need_y, need_m = ctx.needs_input_grad[:2]
+        gy = _device.empty((F, D, T), torch.complex128) if need_y else None
+        gm = _device.empty((F, K, T), torch.float64) if need_m else None
+        if need_y or need_m:
+            g = grad.to(torch.complex128).contiguous()
+            _lib.check(_lib.load().pbb_power_spectral_density_backward(
+                _device.ptr(obs), code, F, D, T, _device.ptr(m), K, int(normalize), _device.ptr(psd), _device.ptr(g),
+                _device.ptr(gy), _device.ptr(gm), _device.stream_ptr()), 'pbb_power_spectral_density_backward')
+        return None if gy is None else gy.to(obs.dtype), gm, None, None
 
 
 def get_pca_vector(target_psd_matrix, scaling=None):
@@ -189,39 +226,71 @@ def get_mvdr_vector_souden(target_psd_matrix, noise_psd_matrix, ref_channel=None
     n = tf.shape[0]
     if eps is None:
         eps = np.finfo(np.float64).tiny
-    lib = _lib.load()
-    phi = _device.empty((n, D, D), torch.complex128)
-    status = _device.empty((1,), torch.int32)
-    status.zero_()
-    _lib.check(lib.pbb_solve_batched(_device.ptr(nf), _device.ptr(tf), n, D, D, 0, _device.ptr(phi),
-                                     _device.ptr(status), _device.stream_ptr()), 'pbb_solve_batched')
-    # stable_solve (math/solve.py:95-114): singular systems get the minimum-norm (lstsq) solution on the device
-    def on_error(s):
-        raise np.linalg.LinAlgError(f'get_mvdr_vector_souden: singular noise PSD matrix {s - 1} (D > 40: no lstsq fallback)')
-    _device.check_status(status, on_error)
-    mat = _device.empty((n, D, D), torch.complex128)
-    num = _device.empty((n, D), torch.complex128)
-    den = _device.empty((n, D), torch.complex128)
-    nsum = _device.empty((D,), torch.complex128)
-    dsum = _device.empty((D,), torch.complex128)
-    _lib.check(lib.pbb_souden(_device.ptr(phi), _device.ptr(tf), _device.ptr(nf), n, D, float(eps),
-                              _device.ptr(mat), _device.ptr(num), _device.ptr(den), _device.ptr(nsum),
-                              _device.ptr(dsum), _device.stream_ptr()), 'pbb_souden')
-    if ref_channel is None:
-        if len(lead) != 1:
-            raise ValueError(
-                'Estimating the ref_channel expects currently that the input '
-                'has 3 ndims (frequency x sensors x sensors). '
-                'Considering an independent dim in the SNR estimate is not unique.')
-        ns, ds = nsum.cpu().numpy(), dsum.cpu().numpy()
-        snr = ns / np.maximum(ds, eps)
-        assert np.all(np.isfinite(snr)), snr
-        ref_channel = int(np.argmax(snr.real))
-    assert np.isscalar(ref_channel), ref_channel
-    beamformer = _device.to_host(mat[..., ref_channel].reshape(*lead, D).contiguous(), like_numpy)
+    chosen = {}
+    w = _Souden.apply(tf, nf, ref_channel, float(eps), len(lead), chosen)
+    ref_channel = chosen['ref_channel']
+    beamformer = _device.to_host(w.reshape(*lead, D), like_numpy)
     if real_in:
         beamformer = np.ascontiguousarray(beamformer.real)
     return (beamformer, ref_channel) if return_ref_channel else beamformer
+
+
+class _Souden(torch.autograd.Function):
+    """target, noise (n, D, D) complex128 -> w = mat[:, ref_channel] (n, D) by pbb_solve_batched + pbb_souden, the
+    reference channel given or chosen by the SNR rule (written to chosen['ref_channel']; a constant of the backward,
+    pbb_souden_backward)."""
+
+    @staticmethod
+    def forward(ctx, tf, nf, ref_channel, eps, lead_dims, chosen):
+        n, D = tf.shape[0], tf.shape[-1]
+        lib = _lib.load()
+        phi = _device.empty((n, D, D), torch.complex128)
+        status = _device.empty((1,), torch.int32)
+        status.zero_()
+        _lib.check(lib.pbb_solve_batched(_device.ptr(nf), _device.ptr(tf), n, D, D, 0, _device.ptr(phi),
+                                         _device.ptr(status), _device.stream_ptr()), 'pbb_solve_batched')
+        # stable_solve (math/solve.py:95-114): singular systems get the minimum-norm (lstsq) solution on the device
+        def on_error(s):
+            raise np.linalg.LinAlgError(
+                f'get_mvdr_vector_souden: singular noise PSD matrix {s - 1} (D > 40: no lstsq fallback)')
+        _device.check_status(status, on_error)
+        mat = _device.empty((n, D, D), torch.complex128)
+        num = _device.empty((n, D), torch.complex128)
+        den = _device.empty((n, D), torch.complex128)
+        nsum = _device.empty((D,), torch.complex128)
+        dsum = _device.empty((D,), torch.complex128)
+        _lib.check(lib.pbb_souden(_device.ptr(phi), _device.ptr(tf), _device.ptr(nf), n, D, eps,
+                                  _device.ptr(mat), _device.ptr(num), _device.ptr(den), _device.ptr(nsum),
+                                  _device.ptr(dsum), _device.stream_ptr()), 'pbb_souden')
+        if ref_channel is None:
+            if lead_dims != 1:
+                raise ValueError(
+                    'Estimating the ref_channel expects currently that the input '
+                    'has 3 ndims (frequency x sensors x sensors). '
+                    'Considering an independent dim in the SNR estimate is not unique.')
+            ns, ds = nsum.cpu().numpy(), dsum.cpu().numpy()
+            snr = ns / np.maximum(ds, eps)
+            assert np.all(np.isfinite(snr)), snr
+            ref_channel = int(np.argmax(snr.real))
+        assert np.isscalar(ref_channel), ref_channel
+        chosen['ref_channel'] = ref_channel
+        ctx.save_for_backward(phi, nf)
+        ctx.args = (int(ref_channel) % D, eps)
+        return mat[..., ref_channel].contiguous()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        phi, nf = ctx.saved_tensors
+        ref, eps = ctx.args
+        n, D = phi.shape[0], phi.shape[-1]
+        g = grad.to(torch.complex128).contiguous()
+        gt = _device.empty((n, D, D), torch.complex128)
+        gn = _device.empty((n, D, D), torch.complex128)
+        _lib.check(_lib.load().pbb_souden_backward(_device.ptr(phi), _device.ptr(nf), _device.ptr(g), n, D, ref, eps,
+                                                   _device.ptr(gt), _device.ptr(gn), _device.stream_ptr()),
+                   'pbb_souden_backward')
+        return gt, gn, None, None, None, None
 
 
 def blind_analytic_normalization(vector, noise_psd_matrix):
@@ -246,7 +315,7 @@ def apply_beamforming_vector(vector, mix):
     like_numpy = not _device.is_tensor(mix)
     v = _device.to_device(vector, torch.complex128)
     y = _device.to_device(mix)
-    code = _device.complex_dtype_code(y)
+    _device.complex_dtype_code(y)
     assert v.shape[-1] < 30, (v.shape, y.shape)
     D, T = y.shape[-2], y.shape[-1]
     lead = tuple(torch.broadcast_shapes(v.shape[:-1], y.shape[:-2]))
@@ -261,24 +330,63 @@ def apply_beamforming_vector(vector, mix):
         B, F = int(np.prod(bshape)), int(np.prod(oshape)) if others else 1
         ve = v.expand(*lead, D).permute(*bdims, *others, len(lead)).reshape(B, F, D).contiguous()
         ysmall = ye[tuple(0 if i in bdims else slice(None) for i in range(len(lead)))].reshape(F, D, T).contiguous()
-        out = _device.empty((B, F, T), torch.complex128)
-        lib = _lib.load()
-        _lib.check(lib.pbb_apply_beamforming_vector_shared(_device.ptr(ve), _device.ptr(ysmall), code, B, F, D, T,
-                                                           _device.ptr(out), _device.stream_ptr()),
-                   'pbb_apply_beamforming_vector_shared')
+        out = _Apply.apply(ve, ysmall, True)
         out = out.reshape(*bshape, *oshape, T)
         if bdims != list(range(nb)):
             out = out.permute(*np.argsort(bdims + others).tolist(), len(lead)).contiguous()
         return _device.to_host(out, like_numpy)
     vf = v.expand(*lead, D).reshape(-1, D).contiguous()
     yf = ye.reshape(-1, D, T).contiguous()
-    F = vf.shape[0]
-    out = _device.empty((F, T), torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_apply_beamforming_vector(_device.ptr(vf), _device.ptr(yf), code, F, D, T,
-                                                _device.ptr(out), _device.stream_ptr()),
-               'pbb_apply_beamforming_vector')
+    out = _Apply.apply(vf, yf, False)
     return _device.to_host(out.reshape(*lead, T), like_numpy)
+
+
+class _Apply(torch.autograd.Function):
+    """vector (F, D) complex128, mix (F, D, T) complex64 / complex128 -> (F, T) by pbb_apply_beamforming_vector, or
+    (shared) vector (B, F, D) and one mix (F, D, T) -> (B, F, T) by pbb_apply_beamforming_vector_shared; backward
+    pbb_apply_beamforming_vector[_shared]_backward."""
+
+    @staticmethod
+    def forward(ctx, v, y, shared):
+        code = _device.complex_dtype_code(y)
+        F, D, T = y.shape
+        lib = _lib.load()
+        if shared:
+            B = v.shape[0]
+            out = _device.empty((B, F, T), torch.complex128)
+            _lib.check(lib.pbb_apply_beamforming_vector_shared(_device.ptr(v), _device.ptr(y), code, B, F, D, T,
+                                                               _device.ptr(out), _device.stream_ptr()),
+                       'pbb_apply_beamforming_vector_shared')
+        else:
+            out = _device.empty((F, T), torch.complex128)
+            _lib.check(lib.pbb_apply_beamforming_vector(_device.ptr(v), _device.ptr(y), code, F, D, T,
+                                                        _device.ptr(out), _device.stream_ptr()),
+                       'pbb_apply_beamforming_vector')
+        ctx.save_for_backward(v, y)
+        ctx.args = (code, shared)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        v, y = ctx.saved_tensors
+        code, shared = ctx.args
+        F, D, T = y.shape
+        need_v, need_y = ctx.needs_input_grad[:2]
+        gv = _device.empty(v.shape, torch.complex128) if need_v else None
+        gy = _device.empty((F, D, T), torch.complex128) if need_y else None
+        if need_v or need_y:
+            g = grad.to(torch.complex128).contiguous()
+            lib = _lib.load()
+            if shared:
+                _lib.check(lib.pbb_apply_beamforming_vector_shared_backward(
+                    _device.ptr(v), _device.ptr(y), code, v.shape[0], F, D, T, _device.ptr(g), _device.ptr(gv),
+                    _device.ptr(gy), _device.stream_ptr()), 'pbb_apply_beamforming_vector_shared_backward')
+            else:
+                _lib.check(lib.pbb_apply_beamforming_vector_backward(
+                    _device.ptr(v), _device.ptr(y), code, F, D, T, _device.ptr(g), _device.ptr(gv), _device.ptr(gy),
+                    _device.stream_ptr()), 'pbb_apply_beamforming_vector_backward')
+        return gv, None if gy is None else gy.to(y.dtype), None
 
 
 def _status():

@@ -4,10 +4,15 @@ pipeline (STFT -> fit -> predict -> alignment -> PSD -> beamformer -> iSTFT).
 The contract is restated in oracle/transform_oracle.py; it has not been checked against nara_wpe itself, which is not
 a dependency.  Every FFT runs in the hand-written fp64 kernels of csrc/fft.cuh (no cuFFT); ``size`` is a power of two
 in [64, 4096].  numpy in -> numpy out, CUDA tensors in -> CUDA tensors out.
+
+``stft`` and ``istft`` are differentiable: a CUDA tensor that requires grad gets a graph whose backward runs the
+device kernels of pbb_stft_backward / pbb_istft_backward (fp64, returned in the input's dtype).  Double backward
+raises.
 """
 import numpy as np
 import scipy.signal
 import torch
+from torch.autograd.function import once_differentiable
 
 from .. import _device, _lib
 
@@ -92,16 +97,9 @@ def stft(time_signal, size=1024, shift=256, axis=-1, window=scipy.signal.windows
         x = torch.movedim(x, axis, -1)
         x = x if x.dtype in (torch.float32, torch.float64) else x.to(torch.float64)
     xd = _device.to_device(x)
-    lead, n = tuple(xd.shape[:-1]), xd.shape[-1]
-    T = num_frames(n, size, shift, wl, fading, pad)
-    out = _device.empty(lead + (T, size // 2 + 1), torch.complex128)
-    rows = int(np.prod(lead, dtype=np.int64))
-    if out.numel():
-        dtype = _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64
-        lib = _lib.load()
-        _lib.check(lib.pbb_stft(_device.ptr(xd), dtype, rows, n, size, shift, wl, wl - shift if fading else 0, T,
-                                _device.ptr(_analysis_window(window, wl, symmetric_window)),
-                                _device.ptr(_twiddle(size)), _device.ptr(out), _device.stream_ptr()), 'pbb_stft')
+    T = num_frames(xd.shape[-1], size, shift, wl, fading, pad)
+    out = _Stft.apply(xd, size, shift, wl, wl - shift if fading else 0, T,
+                      _analysis_window(window, wl, symmetric_window))
     out = torch.movedim(out, (-2, -1), (axis, axis + 1))
     return _device.to_host(out, like_numpy) if like_numpy else out.contiguous()
 
@@ -116,22 +114,79 @@ def istft(stft_signal, size=1024, shift=256, window=scipy.signal.windows.blackma
     like_numpy = not _device.is_tensor(stft_signal)
     X = _device.to_device(stft_signal, torch.complex128)
     assert X.dim() >= 2 and X.shape[-1] == size // 2 + 1, tuple(X.shape)
-    lead, T = tuple(X.shape[:-2]), X.shape[-2]
-    crop = wl - shift if fading else 0
-    n_out = max(T * shift + wl - shift - 2 * crop, 0)
-    out = _device.empty(lead + (n_out,), torch.float64)
-    rows = int(np.prod(lead, dtype=np.int64))
-    if rows and T:
-        lib = _lib.load()
-        nbytes = lib.pbb_istft_workspace_bytes(rows, T, wl)
-        ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_istft(_device.ptr(X), rows, T, size, shift, wl, crop, n_out,
-                                 _device.ptr(_synthesis_window(window, wl, shift, symmetric_window)),
-                                 _device.ptr(_twiddle(size)), _device.ptr(ws), nbytes, _device.ptr(out),
-                                 _device.stream_ptr()), 'pbb_istft')
-    else:
-        out.zero_()
+    out = _Istft.apply(X, size, shift, wl, wl - shift if fading else 0,
+                       _synthesis_window(window, wl, shift, symmetric_window))
     return _device.to_host(out, like_numpy)
+
+
+class _Stft(torch.autograd.Function):
+    """(rows..., n) float32 / float64 -> (rows..., T, size // 2 + 1) complex128 by pbb_stft; backward pbb_stft_backward."""
+
+    @staticmethod
+    def forward(ctx, xd, size, shift, wl, offset, T, window):
+        lead, n = tuple(xd.shape[:-1]), xd.shape[-1]
+        out = _device.empty(lead + (T, size // 2 + 1), torch.complex128)
+        rows = int(np.prod(lead, dtype=np.int64))
+        if out.numel():
+            dtype = _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64
+            _lib.check(_lib.load().pbb_stft(_device.ptr(xd), dtype, rows, n, size, shift, wl, offset, T,
+                                            _device.ptr(window), _device.ptr(_twiddle(size)), _device.ptr(out),
+                                            _device.stream_ptr()), 'pbb_stft')
+        ctx.args = (lead, n, rows, size, shift, wl, offset, T, window, xd.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        lead, n, rows, size, shift, wl, offset, T, window, dtype = ctx.args
+        gx = _device.empty(lead + (n,), torch.float64)
+        if rows and T:
+            g = grad.to(torch.complex128).contiguous()
+            lib = _lib.load()
+            nbytes = lib.pbb_stft_backward_workspace_bytes(rows, T, wl)
+            ws = _device.workspace(nbytes)
+            _lib.check(lib.pbb_stft_backward(_device.ptr(g), rows, n, size, shift, wl, offset, T, _device.ptr(window),
+                                             _device.ptr(_twiddle(size)), _device.ptr(ws), nbytes, _device.ptr(gx),
+                                             _device.stream_ptr()), 'pbb_stft_backward')
+        else:
+            gx.zero_()
+        return gx.to(dtype), None, None, None, None, None, None
+
+
+class _Istft(torch.autograd.Function):
+    """(rows..., T, size // 2 + 1) complex128 -> (rows..., n_out) float64 by pbb_istft; backward pbb_istft_backward."""
+
+    @staticmethod
+    def forward(ctx, X, size, shift, wl, crop, synthesis):
+        lead, T = tuple(X.shape[:-2]), X.shape[-2]
+        n_out = max(T * shift + wl - shift - 2 * crop, 0)
+        out = _device.empty(lead + (n_out,), torch.float64)
+        rows = int(np.prod(lead, dtype=np.int64))
+        if rows and T:
+            lib = _lib.load()
+            nbytes = lib.pbb_istft_workspace_bytes(rows, T, wl)
+            ws = _device.workspace(nbytes)
+            _lib.check(lib.pbb_istft(_device.ptr(X), rows, T, size, shift, wl, crop, n_out, _device.ptr(synthesis),
+                                     _device.ptr(_twiddle(size)), _device.ptr(ws), nbytes, _device.ptr(out),
+                                     _device.stream_ptr()), 'pbb_istft')
+        else:
+            out.zero_()
+        ctx.args = (lead, T, rows, n_out, size, shift, wl, crop, synthesis)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        lead, T, rows, n_out, size, shift, wl, crop, synthesis = ctx.args
+        gX = _device.empty(lead + (T, size // 2 + 1), torch.complex128)
+        if rows and T:
+            g = grad.to(torch.float64).contiguous()
+            _lib.check(_lib.load().pbb_istft_backward(_device.ptr(g) if n_out else None, rows, T, size, shift, wl,
+                                                      crop, n_out, _device.ptr(synthesis), _device.ptr(_twiddle(size)),
+                                                      _device.ptr(gX), _device.stream_ptr()), 'pbb_istft_backward')
+        else:
+            gX.zero_()
+        return gX, None, None, None, None, None
 
 
 def griffin_lim_stft(x_hat, X, y, size, shift, fading):
