@@ -191,15 +191,10 @@ def _fft_shared(a, logM, DIR, tw):
     return a
 
 
-def model_stft(x, size, shift, window_length=None, fading=True, pad=True):
-    """stft_kernel's arithmetic in float64: (..., T, size // 2 + 1) complex128."""
-    wl = window_length or size
+def model_rfft(f, size):
+    """The forward body of stft_kernel in float64 on windowed real frames f (N, size): (N, size // 2 + 1) complex128."""
     M, logM = size // 2, int(np.log2(size)) - 1
     tw = twiddles(size)
-    fr = _frames(x, size, shift, wl, fading, pad)
-    lead, T = fr.shape[:-2], fr.shape[-2]
-    f = np.zeros((int(np.prod(lead, dtype=np.int64)) * T, size))
-    f[:, :wl] = fr.reshape(-1, wl) * TO.analysis_window(size, window_length=wl)
     z = _fft_shared(f[:, 0::2] + 1j * f[:, 1::2], logM, -1, tw)
     k = np.arange(1, M)
     a, b = z[:, k], z[:, M - k]
@@ -209,17 +204,24 @@ def model_stft(x, size, shift, window_length=None, fading=True, pad=True):
     out[:, 0] = z[:, 0].real + z[:, 0].imag
     out[:, M] = z[:, 0].real - z[:, 0].imag
     out[:, 1:M] = fe + np.conj(tw[k]) * fo
-    return out.reshape(lead + (T, M + 1))
+    return out
 
 
-def model_istft(X, size, shift, window_length=None, fading=True):
-    """istft_frames_kernel + overlap_add_kernel's arithmetic in float64."""
+def model_stft(x, size, shift, window_length=None, fading=True, pad=True):
+    """stft_kernel's arithmetic in float64: (..., T, size // 2 + 1) complex128."""
     wl = window_length or size
+    fr = _frames(x, size, shift, wl, fading, pad)
+    lead, T = fr.shape[:-2], fr.shape[-2]
+    f = np.zeros((int(np.prod(lead, dtype=np.int64)) * T, size))
+    f[:, :wl] = fr.reshape(-1, wl) * TO.analysis_window(size, window_length=wl)
+    return model_rfft(f, size).reshape(lead + (T, size // 2 + 1))
+
+
+def model_irfft(Xf, size):
+    """The inverse body of istft_frames_kernel in float64 on spectra Xf (N, size // 2 + 1): (N, size) real frames,
+    irfft(Xf, n=size)."""
     M, logM = size // 2, int(np.log2(size)) - 1
     tw = twiddles(size)
-    X = np.asarray(X, dtype=np.complex128)
-    lead, T = X.shape[:-2], X.shape[-2]
-    Xf = X.reshape(-1, M + 1)
     k = np.arange(1, M)
     a, b = Xf[:, k], Xf[:, M - k]
     fe = 0.5 * (a.real + b.real) + 1j * (0.5 * (a.imag - b.imag))
@@ -230,6 +232,15 @@ def model_istft(X, size, shift, window_length=None, fading=True):
     v = _fft_shared(z, logM, 1, tw)
     y = np.empty((Xf.shape[0], size))
     y[:, 0::2], y[:, 1::2] = v.real / M, v.imag / M
+    return y
+
+
+def model_istft(X, size, shift, window_length=None, fading=True):
+    """istft_frames_kernel + overlap_add_kernel's arithmetic in float64."""
+    wl = window_length or size
+    X = np.asarray(X, dtype=np.complex128)
+    lead, T = X.shape[:-2], X.shape[-2]
+    y = model_irfft(X.reshape(-1, size // 2 + 1), size)
     ws = TO.synthesis_window(TO.analysis_window(size, window_length=wl), shift)
     out = _overlap_add((ws * y[:, :wl]).reshape(lead + (T, wl)), shift)
     if fading:
