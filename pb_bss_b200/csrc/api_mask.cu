@@ -78,20 +78,21 @@ static int row_select_launch(const TI* x, int D, long long sD, const pbb_mask_la
   long long chunks = (264 + nrows - 1) / nrows;
   if (chunks > (n + 4095) / 4096) chunks = (n + 4095) / 4096;
   if (chunks < 1) chunks = 1;
-  const dim3 grid((unsigned)chunks, (unsigned)nrows);
+  // the row is blockIdx.x / chunks: rows < 2^31 and chunks * rows <= rows + 263, so the grid never exceeds grid.x
+  const unsigned grid = (unsigned)(chunks * nrows);
+  row_state_init_kernel<<<grid_for(nrows, 128), 128, 0, st>>>(nrows, n, p, state);
+  PBB_CUDA(cudaGetLastError());
   {
     LaunchScope ls("row_gather_kernel", st);
-    row_gather_kernel<TI><<<grid, 256, 0, st>>>(x, D, sD, *rows, *elems, n, p, vals);
+    row_gather_kernel<TI><<<grid, 256, 0, st>>>(x, D, sD, *rows, *elems, n, (int)chunks, p, vals, state);
     PBB_CUDA(cudaGetLastError());
   }
   const int queries = p.lorenz ? 1 : 2;
   for (int q = 0; q < queries; ++q) {
-    row_state_init_kernel<<<grid_for(nrows, 128), 128, 0, st>>>(nrows, n, q, p, state);
-    PBB_CUDA(cudaGetLastError());
     for (int pass = 0; pass < kSelPasses; ++pass) {
       {
         LaunchScope ls("row_hist_kernel", st);
-        row_hist_kernel<<<grid, 256, 0, st>>>(vals, n, pass, q, p.lorenz, state, hist);
+        row_hist_kernel<<<grid, 256, 0, st>>>(vals, n, (int)chunks, pass, q, p.lorenz, state, hist);
         PBB_CUDA(cudaGetLastError());
       }
       LaunchScope ls("row_decide_kernel", st);
@@ -100,7 +101,7 @@ static int row_select_launch(const TI* x, int D, long long sD, const pbb_mask_la
     }
   }
   LaunchScope ls("row_apply_kernel", st);
-  row_apply_kernel<TO><<<grid, 256, 0, st>>>(vals, *rows, *elems, n, p, state, out, status);
+  row_apply_kernel<TO><<<grid, 256, 0, st>>>(vals, *rows, *elems, n, (int)chunks, p, state, out, status);
   PBB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -42,15 +42,9 @@ __device__ __forceinline__ void st_elem(float* p, double2 v) { *p = (float)v.x; 
 __device__ __forceinline__ void st_elem(double2* p, double2 v) { *p = v; }
 __device__ __forceinline__ void st_elem(float2* p, double2 v) { *p = make_float2((float)v.x, (float)v.y); }
 
-// |s| rounded to nearest (np.abs = hypot): the square root of the exact sum of squares, corrected by one Newton step
-// on the residual; scaled by a power of two so that neither square over- or underflows
-__device__ __forceinline__ double abs_rn(double2 v) {
-  double a = fabs(v.x), b = fabs(v.y);
-  if (a < b) { const double t = a; a = b; b = t; }
-  if (b == 0.0 || !isfinite(a) || isnan(b)) return a + b;
-  // scale by 2^-e with e = exponent of a, so that a lies in [1, 2): exact, and b >= 2^-1022 or it is negligible
-  const int e = (int)((__double_as_longlong(a) >> 52) & 0x7ff) - 1023;
-  if (e < -1000 || e > 1000) return hypot(v.x, v.y);  // out of the scaled range: subnormal or huge
+// sqrt(a^2 + b^2) for a >= b > 0 with 2^e <= a < 2^(e+1), -1022 <= e <= 1000
+__device__ __forceinline__ double abs_rn_scaled(double a, double b, int e) {
+  // scale by 2^-e so that a lies in [1, 2): exact, and b >= 2^-1022 or it is negligible
   const double down = __longlong_as_double((long long)(1023 - e) << 52), up = __longlong_as_double((long long)(1023 + e) << 52);
   a = __dmul_rn(a, down);
   b = __dmul_rn(b, down);
@@ -62,6 +56,41 @@ __device__ __forceinline__ double abs_rn(double2 v) {
   const double r = __dadd_rn(fma(-h, h, s), sl);
   h = __dadd_rn(h, __dmul_rn(r, __dmul_rn(0.5, __drcp_rn(h))));
   return __dmul_rn(h, up);
+}
+
+// the exponent edges of abs_rn, out of line: |a| >= 2^1001, or |a| < 2^-1000
+__device__ __noinline__ double abs_rn_edge(double a, double b, int e) {
+  if (e == -1023) {  // subnormal: a = A 2^-1074, b = B 2^-1074, |s| = round(sqrt(A^2 + B^2)) 2^-1074
+    const unsigned long long A = (unsigned long long)__double_as_longlong(a), B = (unsigned long long)__double_as_longlong(b);
+    const unsigned __int128 N4 = ((unsigned __int128)A * A + (unsigned __int128)B * B) * 4;
+    unsigned long long k = (unsigned long long)__dsqrt_rn(__ull2double_rn(A) * (double)A + __ull2double_rn(B) * (double)B);
+    while ((unsigned __int128)(2 * k + 1) * (2 * k + 1) < N4) ++k;
+    while (k > 0 && (unsigned __int128)(2 * k - 1) * (2 * k - 1) > N4) --k;
+    return __longlong_as_double((long long)k);  // k < 2^53: the double with the bits of k is k 2^-1074
+  }
+  // one exact power-of-two step into the range of abs_rn_scaled: 2^-128 for huge a (b may underflow, but then
+  // b / a < 2^-1000 and b is negligible; the final product rounds to inf exactly when |s| does), 2^128 for small
+  // normal a (exact both ways: the result is at least a >= 2^-1022)
+  const double pre = e > 0 ? 0x1p-128 : 0x1p128, post = e > 0 ? 0x1p128 : 0x1p-128;
+  return __dmul_rn(abs_rn_scaled(__dmul_rn(a, pre), __dmul_rn(b, pre), e > 0 ? e - 128 : e + 128), post);
+}
+
+// |s| (np.abs = C's hypot: an infinite part gives +inf even next to a NaN).  Normal |a| >= |b|: the square root of
+// the sum of squares held exactly as a double-double, corrected by one Newton step on the residual, in a frame scaled
+// by powers of two so that neither square over- or underflows.  The corrected value is within 2^-48 ulp of the exact
+// one, so the result is the correctly rounded one unless |s| lies within that distance of a midpoint between two
+// doubles; midpoints are reached exactly (a Pythagorean triple with an odd 54-bit hypotenuse, scaled by a power of
+// two), and there the result is one of the two neighbours, not necessarily the even one.  Subnormal |a|: a and b are
+// integer multiples of 2^-1074, and round(sqrt(A^2 + B^2)) is exact in 128-bit integers (the square root of an
+// integer is never half way).
+__device__ __forceinline__ double abs_rn(double2 v) {
+  double a = fabs(v.x), b = fabs(v.y);
+  if (a < b) { const double t = a; a = b; b = t; }
+  if (b == 0.0 || !isfinite(a) || isnan(b))
+    return isinf(a) || isinf(b) ? __longlong_as_double(0x7ff0000000000000ll) : a + b;
+  const int e = (int)((__double_as_longlong(a) >> 52) & 0x7ff) - 1023;
+  if (e < -1000 || e > 1000) return abs_rn_edge(a, b, e);
+  return abs_rn_scaled(a, b, e);
 }
 
 // NumPy's complex division (umath loops: Smith's method, a zero divisor gives the inf / nan of the real divisions)
@@ -121,7 +150,8 @@ __global__ void __launch_bounds__(256) source_mask_kernel(const TI* __restrict__
       for (int k = 0; k < K; ++k) {
         double p = 0.0;
         for (int d = 0; d < D; ++d) p = __dadd_rn(p, abs2_rn(ld_elem(xr, k * sK + d * sD)));
-        if (k == 0 || p > best) { best = p; arg = k; }  // np.argmax: the first maximum
+        // np.argmax: the first maximum, and the first NaN over any number
+        if (k == 0 || p > best || (p != p && best == best)) { best = p; arg = k; }
         total = __dadd_rn(total, p);
       }
       if (kind == PBB_MASK_IDEAL_BINARY) {
@@ -172,7 +202,7 @@ struct SelState {
   double total;               // Lorenz: sum of the row
   long long rank;             // rank: 0-based position from the top among the elements matching the prefix
   int fail;
-  int pad;
+  int nan;                    // quantile, long rows: the row holds a NaN (set by row_gather_kernel in query 0's state)
 };
 
 struct RowSelParams {
@@ -273,7 +303,7 @@ __device__ __forceinline__ void sel_init(SelState& st, const RowSelParams& p, in
   st.above = 0.0;
   st.total = 0.0;
   st.fail = 0;
-  st.pad = 0;
+  st.nan = 0;
   // rank from the top of the k-th smallest element
   st.rank = p.lorenz ? 0 : n - 1 - (query == 0 ? p.k_lower : p.k_upper);
 }
@@ -338,7 +368,7 @@ __global__ void __launch_bounds__(kSelWarps * 32, 1) row_select_short_kernel(
     if (row0 + rl >= nrows) break;
     const double* v = vals + (size_t)rl * n;
     double sel_lo = 0.0, sel_hi = 0.0;
-    bool fail = false;
+    bool fail = false, nan = false;
     const int queries = p.lorenz ? 1 : 2;
 #pragma unroll 1
     for (int q = 0; q < queries; ++q) {
@@ -347,7 +377,11 @@ __global__ void __launch_bounds__(kSelWarps * 32, 1) row_select_short_kernel(
       for (int pass = 0; pass < kSelPasses && !st.fail; ++pass) {
         for (int b = lane; b < kSelBuckets; b += 32) { hcnt[b] = 0u; hsum[b] = 0.0; hmax[b] = 0ull; }
         __syncwarp();
-        for (int i = lane; i < n; i += 32) sel_count(hcnt, hsum, hmax, v[i], pass, st.prefix, p.lorenz);
+        for (int i = lane; i < n; i += 32) {
+          const double x = v[i];
+          nan |= x != x;
+          sel_count(hcnt, hsum, hmax, x, pass, st.prefix, p.lorenz);
+        }
         __syncwarp();
         warp_decide(hcnt, hsum, hmax, pass, p.lorenz, p.fraction, st, lane);
         __syncwarp();
@@ -355,7 +389,9 @@ __global__ void __launch_bounds__(kSelWarps * 32, 1) row_select_short_kernel(
       fail |= st.fail != 0;
       (q == 0 ? sel_lo : sel_hi) = __longlong_as_double((long long)st.prefix);
     }
+    // np.percentile of a row with a NaN is NaN, whatever the rank: no element compares true, every one is mask_low
     double t = p.lorenz ? sel_lo : quantile_lerp(sel_lo, sel_hi, p);
+    if (!p.lorenz && __any_sync(0xffffffffu, nan)) t = __longlong_as_double(0x7ff8000000000000ll);
     if (fail) {
       t = __longlong_as_double(0x7ff0000000000000ll);  // +inf: the mask is mask_low; the caller raises
       if (lane == 0 && status) report_first_row(status, row0 + rl);
@@ -373,32 +409,47 @@ __global__ void __launch_bounds__(kSelWarps * 32, 1) row_select_short_kernel(
   }
 }
 
-// Long rows, several CTAs per row (grid.y = row): the row values go to scratch once, then every digit is one
-// histogram launch (shared-memory histogram per CTA, merged into the row's global histogram with atomics) and one
-// decide launch (a warp per row, which also clears the histogram for the next digit).
+// Long rows, `chunks` CTAs per row (CTA c of row r is blockIdx.x = r chunks + c, so any number of rows fits the grid):
+// the row values go to scratch once, then every digit is one histogram launch (shared-memory histogram per CTA, merged
+// into the row's global histogram with atomics) and one decide launch (a warp per row, which also clears the histogram
+// for the next digit).
 template <class TI>
 __global__ void __launch_bounds__(256) row_gather_kernel(const TI* __restrict__ x, int D, long long sD,
                                                          pbb_mask_layout rows, pbb_mask_layout elems, long long n,
-                                                         RowSelParams p, double* __restrict__ vals) {
-  const long long row = blockIdx.y;
+                                                         int chunks, RowSelParams p, double* __restrict__ vals,
+                                                         SelState* __restrict__ state) {
+  const long long row = blockIdx.x / chunks, chunk = blockIdx.x - row * chunks;
   long long ri, ro;
   layout_offsets(rows, row, ri, ro);
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+  if (p.lorenz) {
+    for (long long i = chunk * blockDim.x + threadIdx.x; i < n; i += (long long)chunks * blockDim.x) {
+      long long ei, eo;
+      layout_offsets(elems, i, ei, eo);
+      vals[row * n + i] = row_value(x, ri + ei, D, sD, p);
+    }
+    return;
+  }
+  bool nan = false;
+  for (long long i = chunk * blockDim.x + threadIdx.x; i < n; i += (long long)chunks * blockDim.x) {
     long long ei, eo;
     layout_offsets(elems, i, ei, eo);
-    vals[row * n + i] = row_value(x, ri + ei, D, sD, p);
+    const double v = row_value(x, ri + ei, D, sD, p);
+    nan |= v != v;
+    vals[row * n + i] = v;
   }
+  if (nan) state[row * 2].nan = 1;
 }
 
-__global__ void __launch_bounds__(256) row_hist_kernel(const double* __restrict__ vals, long long n, int pass, int query,
-                                                       int lorenz, const SelState* __restrict__ state,
+__global__ void __launch_bounds__(256) row_hist_kernel(const double* __restrict__ vals, long long n, int chunks,
+                                                       int pass, int query, int lorenz,
+                                                       const SelState* __restrict__ state,
                                                        unsigned char* __restrict__ ghist) {
   // one sub-histogram per warp: the leading digits put almost every value into one or two buckets, and eight copies
   // cut the shared-memory atomic contention on them eightfold
   __shared__ unsigned cnt[8][kSelBuckets];
   __shared__ double sum[8][kSelBuckets];
   __shared__ unsigned long long mx[8][kSelBuckets];
-  const long long row = blockIdx.y;
+  const long long row = blockIdx.x / chunks, chunk = blockIdx.x - row * chunks;
   const SelState st = state[row * 2 + query];
   if (st.fail) return;
   for (int b = threadIdx.x; b < 8 * kSelBuckets; b += blockDim.x) {
@@ -409,7 +460,7 @@ __global__ void __launch_bounds__(256) row_hist_kernel(const double* __restrict_
   __syncthreads();
   const int w = threadIdx.x >> 5;
   const double* __restrict__ v = vals + row * n;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+  for (long long i = chunk * blockDim.x + threadIdx.x; i < n; i += (long long)chunks * blockDim.x)
     sel_count(cnt[w], sum[w], mx[w], v[i], pass, st.prefix, lorenz != 0);
   __syncthreads();
   unsigned char* h = ghist + row * kSelHistBytes;
@@ -449,29 +500,32 @@ __global__ void row_decide_kernel(long long n, int pass, int query, RowSelParams
   if (lane == 0) state[row * 2 + query] = st;
 }
 
-// pass 0 of the histogram needs the state of the query initialised before the decide launch runs it
-__global__ void row_state_init_kernel(long long rows, long long n, int query, RowSelParams p, SelState* state) {
+// both queries' states, before row_gather_kernel flags the NaN rows and before pass 0 of the histogram reads them
+__global__ void row_state_init_kernel(long long rows, long long n, RowSelParams p, SelState* state) {
   const long long row = blockIdx.x * (long long)blockDim.x + threadIdx.x;
   if (row >= rows) return;
-  SelState st;
-  sel_init(st, p, query, n);
-  state[row * 2 + query] = st;
+  for (int query = 0; query < 2; ++query) {
+    SelState st;
+    sel_init(st, p, query, n);
+    state[row * 2 + query] = st;
+  }
 }
 
 template <class TO>
 __global__ void __launch_bounds__(256) row_apply_kernel(const double* __restrict__ vals, pbb_mask_layout rows,
-                                                        pbb_mask_layout elems, long long n, RowSelParams p,
+                                                        pbb_mask_layout elems, long long n, int chunks, RowSelParams p,
                                                         const SelState* __restrict__ state, TO* __restrict__ out,
                                                         int* status) {
-  const long long row = blockIdx.y;
+  const long long row = blockIdx.x / chunks, chunk = blockIdx.x - row * chunks;
   const SelState s0 = state[row * 2], s1 = state[row * 2 + 1];
   const bool fail = s0.fail || (!p.lorenz && s1.fail);
   const double a = __longlong_as_double((long long)s0.prefix), b = __longlong_as_double((long long)s1.prefix);
-  const double thr = fail ? __longlong_as_double(0x7ff0000000000000ll) : (p.lorenz ? a : quantile_lerp(a, b, p));
-  if (fail && blockIdx.x == 0 && threadIdx.x == 0 && status) report_first_row(status, row);
+  double thr = fail ? __longlong_as_double(0x7ff0000000000000ll) : (p.lorenz ? a : quantile_lerp(a, b, p));
+  if (!p.lorenz && s0.nan) thr = __longlong_as_double(0x7ff8000000000000ll);  // np.percentile: NaN, all mask_low
+  if (fail && chunk == 0 && threadIdx.x == 0 && status) report_first_row(status, row);
   long long ri, ro;
   layout_offsets(rows, row, ri, ro);
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+  for (long long i = chunk * blockDim.x + threadIdx.x; i < n; i += (long long)chunks * blockDim.x) {
     long long ei, eo;
     layout_offsets(elems, i, ei, eo);
     store_mask(out, ro + eo, vals[row * n + i], thr, p);
