@@ -524,6 +524,58 @@ int pbb_souden_backward(const void* phi, const void* noise_psd, const void* grad
                         int ref_channel, double eps, void* grad_target_psd, void* grad_noise_psd,
                         void* stream);
 
+/* Differentiates the top eigenpair (lambda, w) of pbb_gev_batched (b = the noise PSD) and of pbb_heig_batched's last
+ * column (b NULL: B = I, the PCA vector and its eigenvalue).  A and B are the Hermitian parts of a and b, as the
+ * forwards read them; w (n, D) is the forward's output, w^H B w = 1.
+ *
+ * An eigenvector is defined up to a per-bin phase, which the forward's Jacobi solver picks by its rotation sequence.
+ * The derivative holds that phase fixed to first order, Im(w^H B dw) = 0 (torch.linalg.eigh's backward assumes the
+ * same).  With g = grad_w and g_lambda = grad_lambda (NULL: 0), u = sum_{j != top} w_j (w_j^H g) / (lambda - lambda_j):
+ *   grad_a = (G_A + G_A^H) / 2,  G_A = u w^H + g_lambda w w^H,
+ *   grad_b = (G_B + G_B^H) / 2,  G_B = -lambda u w^H - (Re(w^H g) / 2 + lambda g_lambda) w w^H   (b != NULL).
+ * The projector sum_{j != top} w_j w_j^H / (lambda - lambda_j) does not depend on the phase, so it is recomputed with
+ * the forward's own device code (the Cholesky and L^-1 A L^-H reduction of pbb_gev_batched, or the hermitisation of
+ * pbb_heig_batched, then the same Jacobi solver) rather than solved for with a bordered system; u w^H is formed with
+ * the saved w, whose phase a recomputed top vector must not replace.  For a loss that does not change under
+ * w -> e^{i theta} w per bin (w w^H, BAN's output power, the rank-1 estimates) this is the exact gradient; for one that
+ * does, it is the gradient with each bin's phase held fixed.
+ * A bin whose recomputed top eigenvalue is exactly tied with another, whose B is not positive definite, or which holds
+ * non-finite values gets NaN gradients; other bins are unaffected.  grad_a, grad_b (n, D, D); 0 < D <= 64. */
+int pbb_eigenvector_backward(const void* a, const void* b, const void* w, const void* grad_w,
+                             const double* grad_lambda, int n, int D, void* grad_a, void* grad_b,
+                             void* stream);
+
+/* Differentiates pbb_mvdr, w = x / s, x = N_h^-1 a, s = a^H x, N_h = (N + N^H) / 2.  x (n, D) is the forward's scratch
+ * (N_h^-1 a), w its output.  With t = w^H g:
+ *   q = (g - t a) / conj(s),  p = N_h^-1 q,  grad_atf = p - conj(t) w,  grad_noise_psd = -(p x^H + x p^H) / 2.
+ * The solve is pbb_solve_batched's elimination on N_h with a zero pivot giving NaN: a singular N (the forward's
+ * minimum-norm branch, which has no such derivative) or non-finite N gives NaN gradients in that bin only.
+ * grad_atf (n, D), grad_noise_psd (n, D, D); scratch: n * D complex128.  0 < D <= 64. */
+int pbb_mvdr_backward(const void* atf, const void* noise_psd, const void* x, const void* w, const void* grad_w,
+                      int n, int D, void* grad_atf, void* grad_noise_psd, void* scratch, void* stream);
+
+/* Differentiates pbb_blind_analytic_normalization, out = c w, c = sqrt|nu| / |delta|, nu = w^H N N w,
+ * delta = w^H N w, N read as given (not hermitised).  With r = N w, l = N^H w, rho = Re(w^H g),
+ * alpha = rho c conj(nu) / (2 |nu|^2), beta = -rho c conj(delta) / |delta|^2:
+ *   grad_vector = c g + alpha N r + conj(alpha) N^H l + beta r + conj(beta) l,
+ *   grad_noise_psd = conj(alpha) (w r^H + l w^H) + conj(beta) w w^H.
+ * delta = 0, where the forward's c is the constant 0: zero gradients.  nu = 0 with delta != 0 (sqrt|nu| has an
+ * infinite derivative there): NaN.  grad_vector (n, D), grad_noise_psd (n, D, D); 0 < D <= 1024. */
+int pbb_blind_analytic_normalization_backward(const void* vector, const void* noise_psd, const void* grad_out,
+                                              int n, int D, void* grad_vector, void* grad_noise_psd,
+                                              void* stream);
+
+/* Differentiates pbb_rank_one_estimate, out = a a^H t / nu, t = sum_d cov_dd (the complex trace), nu = |a|^2.  With
+ * G = grad_out and q = a^H G a:
+ *   grad_vector = (conj(t) G a + t G^H a) / nu - 2 Re(t conj(q)) / nu^2 a,   grad_covariance = (q / nu) I.
+ * |a| = 0 gives NaN in that bin.  grad_vector (n, D), grad_covariance (n, D, D); 0 < D <= 64. */
+int pbb_rank_one_estimate_backward(const void* vector, const void* covariance, const void* grad_out, int n,
+                                   int D, void* grad_vector, void* grad_covariance, void* stream);
+
+/* Differentiates pbb_matvec_batched, y = M x:  grad_matrix = g x^H,  grad_vector = M^H g.  0 < D <= 64. */
+int pbb_matvec_batched_backward(const void* matrix, const void* vector, const void* grad_out, int n, int D,
+                                void* grad_matrix, void* grad_vector, void* stream);
+
 /* get_lcmv_vector (beamformer.py:414-456): atf (K, F, D), response (K)
  * complex128 on the device, noise_psd (F, D, D) -> w (F, D).  X = solve(noise, H)
  * with the K ATFs as right-hand sides, y = solve(H^H X, r), w = X y; both solves

@@ -137,6 +137,11 @@ SIGNATURES = {
     'pbb_apply_beamforming_vector_shared_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_power_spectral_density_backward': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     'pbb_souden_backward': (_i, [_vp, _vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp]),
+    'pbb_eigenvector_backward': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    'pbb_mvdr_backward': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    'pbb_blind_analytic_normalization_backward': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    'pbb_rank_one_estimate_backward': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    'pbb_matvec_batched_backward': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     'pbb_solve_batched_strict': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     'pbb_lcmv': (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_wmwf': (_i, [_vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp]),

@@ -23,22 +23,10 @@ __global__ void heig_batched_kernel(const double2* __restrict__ a, int n, int D,
   double2* A = reinterpret_cast<double2*>(smem_raw + per * warp);
   double2* V = A + D * D;
   double* rot = reinterpret_cast<double*>(V + D * D);
-  const double2* __restrict__ am = a + (size_t)m * D * D;
-  bool bad = false;
-  double amax = 0.0;
-  // Hermitian part of the input, (A + A^H) / 2: LAPACK reads one triangle only
-  for (int i = lane; i < D * D; i += 32) {
-    const int r = i / D, c = i - r * D;
-    const double2 x = am[r * D + c], y = am[c * D + r];
-    const double2 h = make_double2(0.5 * (x.x + y.x), r == c ? 0.0 : 0.5 * (x.y - y.y));
-    bad |= !isfinite(h.x) || !isfinite(h.y);
-    A[i] = h;
-    amax = cabs_max(amax, h);
-  }
-  // diagonalise 2^-escale A (linalg_kernels.cuh: even_exponent): same V, eigenvalues times 2^escale
-  const int escale = even_exponent(amax);
-  for (int i = lane; i < D * D; i += 32) A[i] = cscalbn(A[i], -escale);
-  __syncwarp();
+  // Hermitian part of the input times 2^-escale (linalg_kernels.cuh: heig_prepare)
+  int escale;
+  bool bad;
+  heig_prepare(a + (size_t)m * D * D, D, lane, A, escale, bad);
   const int sweeps = warp_jacobi_any(A, V, rot, D, lane);
   if ((__any_sync(0xffffffffu, bad) || sweeps > kJacobiMaxSweeps) && lane == 0 && status) record_first(status, m + 1);
   for (int x = lane; x < D; x += 32) {
@@ -339,6 +327,109 @@ int pbb_souden_backward(const void* phi, const void* noise_psd, const void* grad
   souden_noise_backward_kernel<<<blocks_for((size_t)n * D * D, 128), 128, 0, st>>>(
       reinterpret_cast<const double2*>(grad_target_psd), reinterpret_cast<const double2*>(phi), n, D,
       reinterpret_cast<double2*>(grad_noise_psd));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// ---- backward passes of the get_bf_vector beamformers (linalg_kernels.cuh) ------------------------------------------
+
+int pbb_eigenvector_backward(const void* a, const void* b, const void* w, const void* grad_w, const double* grad_lambda,
+                             int n, int D, void* grad_a, void* grad_b, void* stream) {
+  PBB_CHECK_ARG(a != nullptr, 1, "a is null");
+  PBB_CHECK_ARG(w != nullptr, 3, "w is null");
+  PBB_CHECK_ARG(grad_w != nullptr, 4, "grad_w is null");
+  PBB_CHECK_ARG(n > 0, 6, "n must be positive");
+  PBB_CHECK_ARG(D > 0 && D <= 64, 7, "need 0 < D <= 64");
+  PBB_CHECK_ARG(grad_a != nullptr, 8, "grad_a is null");
+  PBB_CHECK_ARG(b == nullptr || grad_b != nullptr, 9, "grad_b is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const size_t per = eig_backward_smem_per_warp(D, b != nullptr);
+  const int warps = warps_for(per);
+  PBB_CUDA(cudaFuncSetAttribute(eig_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  LaunchScope ls("eig_backward_kernel", st);
+  eig_backward_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
+      reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), reinterpret_cast<const double2*>(w),
+      reinterpret_cast<const double2*>(grad_w), grad_lambda, n, D, reinterpret_cast<double2*>(grad_a),
+      reinterpret_cast<double2*>(grad_b), warps);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_mvdr_backward(const void* atf, const void* noise_psd, const void* x, const void* w, const void* grad_w, int n,
+                      int D, void* grad_atf, void* grad_noise_psd, void* scratch, void* stream) {
+  PBB_CHECK_ARG(atf && noise_psd && x && w && grad_w, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 6, "bad shape");
+  PBB_CHECK_ARG(grad_atf && grad_noise_psd, 8, "output is null");
+  PBB_CHECK_ARG(scratch != nullptr, 10, "scratch (n * D complex128) is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const double2* X = reinterpret_cast<const double2*>(x);
+  const double2* W = reinterpret_cast<const double2*>(w);
+  const double2* G = reinterpret_cast<const double2*>(grad_w);
+  double2* q = reinterpret_cast<double2*>(grad_atf);  // overwritten by the last kernel
+  double2* p = reinterpret_cast<double2*>(scratch);
+  {
+    LaunchScope ls("mvdr_backward_rhs_kernel", st);
+    mvdr_backward_rhs_kernel<<<blocks_for(n, 128), 128, 0, st>>>(reinterpret_cast<const double2*>(atf), X, W, G, n,
+                                                                  D, q);
+    PBB_CUDA(cudaGetLastError());
+  }
+  // p = N_h^-1 q; a zero pivot (the forward's minimum-norm branch, no derivative) or non-finite N gives NaN
+  const int rc = solve_launch(noise_psd, q, n, D, 1, 1, p, nullptr, 2, st);
+  if (rc) return rc;
+  LaunchScope ls("mvdr_backward_kernel", st);
+  mvdr_backward_kernel<<<blocks_for((size_t)n * D * D, 128), 128, 0, st>>>(
+      p, X, W, G, n, D, reinterpret_cast<double2*>(grad_atf), reinterpret_cast<double2*>(grad_noise_psd));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+constexpr int kBanBackwardMaxD = 1024;
+
+int pbb_blind_analytic_normalization_backward(const void* vector, const void* noise_psd, const void* grad_out, int n,
+                                              int D, void* grad_vector, void* grad_noise_psd, void* stream) {
+  PBB_CHECK_ARG(vector && noise_psd && grad_out, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= kBanBackwardMaxD, 4, "need n > 0 and 0 < D <= 1024");
+  PBB_CHECK_ARG(grad_vector && grad_noise_psd, 6, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const int warps = 4;
+  const size_t smem = (size_t)warps * 2 * D * sizeof(double2);
+  PBB_CUDA(cudaFuncSetAttribute(ban_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LaunchScope ls("ban_backward_kernel", st);
+  ban_backward_kernel<<<(n + warps - 1) / warps, 32 * warps, smem, st>>>(
+      reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(noise_psd),
+      reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_vector),
+      reinterpret_cast<double2*>(grad_noise_psd), warps);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_rank_one_estimate_backward(const void* vector, const void* covariance, const void* grad_out, int n, int D,
+                                   void* grad_vector, void* grad_covariance, void* stream) {
+  PBB_CHECK_ARG(vector && covariance && grad_out, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
+  PBB_CHECK_ARG(grad_vector && grad_covariance, 6, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("rank_one_backward_kernel", st);
+  rank_one_backward_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(vector),
+                                             reinterpret_cast<const double2*>(covariance),
+                                             reinterpret_cast<const double2*>(grad_out), n, D,
+                                             reinterpret_cast<double2*>(grad_vector),
+                                             reinterpret_cast<double2*>(grad_covariance));
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int pbb_matvec_batched_backward(const void* matrix, const void* vector, const void* grad_out, int n, int D,
+                                void* grad_matrix, void* grad_vector, void* stream) {
+  PBB_CHECK_ARG(matrix && vector && grad_out, 1, "input is null");
+  PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
+  PBB_CHECK_ARG(grad_matrix && grad_vector, 6, "output is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  LaunchScope ls("matvec_backward_kernel", st);
+  matvec_backward_kernel<<<blocks_for((size_t)n * D, 128), 128, 0, st>>>(
+      reinterpret_cast<const double2*>(matrix), reinterpret_cast<const double2*>(vector),
+      reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_matrix),
+      reinterpret_cast<double2*>(grad_vector));
   PBB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -89,21 +89,14 @@ __device__ inline void warp_trsm_lower_h(const double2* __restrict__ L, double2*
 // scipy.linalg.eigh(a, b) / LAPACK zhegvd ITYPE=1 (beamformer.py:367-411,
 // get_gev_vector.pyx:124-150): B = L L^H, C = L^{-1} A L^{-H}, C y = lambda y,
 // w = L^{-H} y, so w^H B w = 1.  out (n, D): eigenvector of the LARGEST eigenvalue.
-__global__ void gev_kernel(const double2* __restrict__ a, const double2* __restrict__ b, int n, int D,
-                           double2* __restrict__ out, int* status, int warps) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m = blockIdx.x * warps + warp;
-  if (m >= n) return;
-  const size_t per = ((size_t)3 * D * D * sizeof(double2) + (size_t)((D + 1) / 2) * 6 * sizeof(double) + 15) &
-                     ~(size_t)15;
-  double2* C = reinterpret_cast<double2*>(smem_raw + per * warp);  // A -> C (Jacobi input)
-  double2* V = C + D * D;
-  double2* L = V + D * D;
-  double* rot = reinterpret_cast<double*>(L + D * D);
-  const double2* __restrict__ am = a + (size_t)m * D * D;
-  const double2* __restrict__ bm = b + (size_t)m * D * D;
-  bool bad = false;
+//
+// gev_reduce is the part before the Jacobi solver, shared by gev_kernel and its backward (eig_backward_kernel):
+// C = the Hermitian part of 2^-ea A, L = the Cholesky factor of the Hermitian part of 2^-eb B, then C <- L^-1 C L^-H.
+// V is scratch.  Returns false if B is not positive definite; bad (per lane) flags non-finite input.
+__device__ __forceinline__ bool gev_reduce(const double2* __restrict__ am, const double2* __restrict__ bm, int D,
+                                           int lane, double2* __restrict__ C, double2* __restrict__ V,
+                                           double2* __restrict__ L, int& ea, int& eb, bool& bad) {
+  bad = false;
   double amax = 0.0, bmax = 0.0;
   // zhegvd reads the lower triangles (UPLO = 'L'); use the Hermitian parts
   for (int i = lane; i < D * D; i += 32) {
@@ -117,7 +110,8 @@ __global__ void gev_kernel(const double2* __restrict__ a, const double2* __restr
     bmax = cabs_max(bmax, L[i]);
   }
   // solve with 2^-ea A and 2^-eb B: y does not change, and w = 2^(-eb/2) times the w of the scaled pair
-  const int ea = even_exponent(amax), eb = even_exponent(bmax);
+  ea = even_exponent(amax);
+  eb = even_exponent(bmax);
   for (int i = lane; i < D * D; i += 32) {
     C[i] = cscalbn(C[i], -ea);
     L[i] = cscalbn(L[i], -eb);
@@ -139,13 +133,37 @@ __global__ void gev_kernel(const double2* __restrict__ a, const double2* __restr
     C[i] = make_double2(0.5 * (u.x + v.x), r == c ? 0.0 : 0.5 * (-u.y + v.y));
   }
   __syncwarp();
-  const int sweeps = warp_jacobi_any(C, V, rot, D, lane);
+  return pd;
+}
+
+// index of the largest eigenvalue on the diagonal of the diagonalised C, the last one of a tie (as eig_rank orders)
+__device__ __forceinline__ int top_eigen_index(const double2* __restrict__ C, int D) {
   int best = 0;
   double lmax = C[0].x;
   for (int d = 1; d < D; ++d) {
     const double l = C[d * D + d].x;
     if (l >= lmax) { lmax = l; best = d; }
   }
+  return best;
+}
+
+__global__ void gev_kernel(const double2* __restrict__ a, const double2* __restrict__ b, int n, int D,
+                           double2* __restrict__ out, int* status, int warps) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m = blockIdx.x * warps + warp;
+  if (m >= n) return;
+  const size_t per = ((size_t)3 * D * D * sizeof(double2) + (size_t)((D + 1) / 2) * 6 * sizeof(double) + 15) &
+                     ~(size_t)15;
+  double2* C = reinterpret_cast<double2*>(smem_raw + per * warp);  // A -> C (Jacobi input)
+  double2* V = C + D * D;
+  double2* L = V + D * D;
+  double* rot = reinterpret_cast<double*>(L + D * D);
+  int ea, eb;
+  bool bad;
+  const bool pd = gev_reduce(a + (size_t)m * D * D, b + (size_t)m * D * D, D, lane, C, V, L, ea, eb, bad);
+  const int sweeps = warp_jacobi_any(C, V, rot, D, lane);
+  const int best = top_eigen_index(C, D);
   // w = L^{-H} y
   double2* yv = C;                                // reuse C's first column block as the rhs (D x 1)
   __syncwarp();
@@ -155,6 +173,26 @@ __global__ void gev_kernel(const double2* __restrict__ a, const double2* __restr
   for (int d = lane; d < D; d += 32) out[(size_t)m * D + d] = cscalbn(yv[d], -eb / 2);
   if ((!pd || __any_sync(0xffffffffu, bad) || sweeps > kJacobiMaxSweeps) && lane == 0 && status)
     record_first(status, m + 1);
+}
+
+// The part of heig_batched_kernel (api_linalg.cu) before the Jacobi solver, shared with eig_backward_kernel: A = the
+// Hermitian part (a + a^H) / 2 (LAPACK reads one triangle only), times 2^-escale (even_exponent): the same V,
+// eigenvalues times 2^escale.  bad (per lane) flags non-finite input.
+__device__ __forceinline__ void heig_prepare(const double2* __restrict__ am, int D, int lane, double2* __restrict__ A,
+                                             int& escale, bool& bad) {
+  bad = false;
+  double amax = 0.0;
+  for (int i = lane; i < D * D; i += 32) {
+    const int r = i / D, c = i - r * D;
+    const double2 x = am[r * D + c], y = am[c * D + r];
+    const double2 h = make_double2(0.5 * (x.x + y.x), r == c ? 0.0 : 0.5 * (x.y - y.y));
+    bad |= !isfinite(h.x) || !isfinite(h.y);
+    A[i] = h;
+    amax = cabs_max(amax, h);
+  }
+  escale = even_exponent(amax);
+  for (int i = lane; i < D * D; i += 32) A[i] = cscalbn(A[i], -escale);
+  __syncwarp();
 }
 
 // shared memory of one warp of solve_kernel: A, X and -- when the minimum-norm fallback is available (D <= kLstsqMaxD)
@@ -701,6 +739,300 @@ __global__ void __launch_bounds__(kPsdBwdThreads) psd_backward_kernel(
   }
   if (live && gy_out)
     for (int d = 0; d < D; ++d) gy_out[((size_t)f * D + d) * T + t] = gys[d * kPsdBwdThreads + tid];
+}
+
+// ================================ backward passes of the get_bf_vector beamformers ================================
+
+// ---- top eigenpair (lambda, w) of the Hermitian parts of (A, B), w^H B w = 1 (pbb_eigenvector_backward) ----
+// Phase held fixed, Im(w^H B dw) = 0.  u = P g with P = sum_{j != top} w_j w_j^H / (lambda - lambda_j), recomputed
+// from the forward's own reduction and Jacobi solver (gev_reduce / heig_prepare, then warp_jacobi_any):
+//   P = 2^-ea L^-H (sum_{j != top} y_j y_j^H / (l - l_j)) L^-1 in the scaled pencil, l = eigenvalues of C.
+// P does not depend on the phase of the eigenvectors; u w^H is formed with the forward's saved w.
+//   grad A = (u w^H + w u^H) / 2 + g_lambda w w^H,
+//   grad B = -lambda (u w^H + w u^H) / 2 - (Re(w^H g) / 2 + lambda g_lambda) w w^H        (pencil only).
+// b == nullptr is the plain Hermitian case (B = I, PCA).  One warp per bin: C, V (and L) in shared memory like
+// gev_kernel, plus two D-vectors.  A tie of the top eigenvalue, a B that is not positive definite, non-finite input or
+// no convergence gives NaN in that bin only.
+__host__ __device__ inline size_t eig_backward_smem_per_warp(int D, bool pencil) {
+  return ((size_t)(pencil ? 3 : 2) * D * D * sizeof(double2) + (size_t)((D + 1) / 2) * 6 * sizeof(double) +
+          (size_t)2 * D * sizeof(double2) + 15) & ~(size_t)15;
+}
+
+__global__ void eig_backward_kernel(const double2* __restrict__ a, const double2* __restrict__ b,
+                                    const double2* __restrict__ w, const double2* __restrict__ g,
+                                    const double* __restrict__ glam, int n, int D, double2* __restrict__ ga,
+                                    double2* __restrict__ gb, int warps) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m = blockIdx.x * warps + warp;
+  if (m >= n) return;
+  const bool pencil = b != nullptr;
+  const size_t per = eig_backward_smem_per_warp(D, pencil);
+  double2* C = reinterpret_cast<double2*>(smem_raw + per * warp);
+  double2* V = C + D * D;
+  double2* L = V + D * D;  // pencil only
+  double* rot = reinterpret_cast<double*>(pencil ? L + D * D : L);
+  double2* h = reinterpret_cast<double2*>(rot + ((D + 1) / 2) * 6);
+  double2* z = h + D;
+  int ea, eb = 0;
+  bool bad, pd = true;
+  if (pencil) pd = gev_reduce(a + (size_t)m * D * D, b + (size_t)m * D * D, D, lane, C, V, L, ea, eb, bad);
+  else heig_prepare(a + (size_t)m * D * D, D, lane, C, ea, bad);
+  const int sweeps = warp_jacobi_any(C, V, rot, D, lane);
+  const int top = top_eigen_index(C, D);
+  const double lt = C[top * D + top].x;
+  bool tied = false;
+  for (int j = 0; j < D; ++j) tied |= j != top && C[j * D + j].x == lt;
+  const bool nan_bin = tied || !pd || __any_sync(0xffffffffu, bad) || sweeps > kJacobiMaxSweeps;
+  const double2* __restrict__ wm = w + (size_t)m * D;
+  const double2* __restrict__ gm = g + (size_t)m * D;
+  // h = L^-1 g (g in the pencil)
+  for (int d = lane; d < D; d += 32) h[d] = gm[d];
+  __syncwarp();
+  if (pencil) warp_trsm_lower(L, h, D, 1, lane);
+  // z_j = y_j^H h / (l - l_j), 0 at the top
+  for (int j = lane; j < D; j += 32) {
+    double2 s = make_double2(0.0, 0.0);
+    for (int k = 0; k < D; ++k) {
+      const double2 q = cmulc(h[k], V[k * D + j]);
+      s.x += q.x; s.y += q.y;
+    }
+    const double den = lt - C[j * D + j].x;
+    z[j] = j == top ? make_double2(0.0, 0.0) : make_double2(s.x / den, s.y / den);
+  }
+  __syncwarp();
+  // h <- Y z, then L^-H h: u = 2^-ea h
+  for (int k = lane; k < D; k += 32) {
+    double2 s = make_double2(0.0, 0.0);
+    for (int j = 0; j < D; ++j) {
+      const double2 q = cmul(V[k * D + j], z[j]);
+      s.x += q.x; s.y += q.y;
+    }
+    h[k] = s;
+  }
+  __syncwarp();
+  if (pencil) warp_trsm_lower_h(L, h, D, 1, lane);
+  double rho = 0.0;  // Re(w^H g), every lane in the same order
+  for (int k = 0; k < D; ++k) rho += wm[k].x * gm[k].x + wm[k].y * gm[k].y;
+  const double lam = scalbn(lt, ea - eb);
+  const double gl = glam ? glam[m] : 0.0;
+  const double cb = 0.5 * rho + lam * gl;
+  for (int idx = lane; idx < D * D; idx += 32) {
+    const int i = idx / D, k = idx - i * D;
+    double2 oa, ob;
+    if (nan_bin) {
+      oa = ob = make_double2(NAN, NAN);
+    } else {
+      const double2 ui = cscalbn(h[i], -ea), uk = cscalbn(h[k], -ea), wi = wm[i], wk = wm[k];
+      const double2 p = cmulc(ui, wk), q = cmulc(wi, uk), ww = cmulc(wi, wk);
+      const double2 sym = make_double2(0.5 * (p.x + q.x), 0.5 * (p.y + q.y));
+      oa = make_double2(sym.x + gl * ww.x, sym.y + gl * ww.y);
+      ob = make_double2(-lam * sym.x - cb * ww.x, -lam * sym.y - cb * ww.y);
+    }
+    ga[(size_t)m * D * D + idx] = oa;
+    if (pencil) gb[(size_t)m * D * D + idx] = ob;
+  }
+}
+
+// ---- MVDR, w = x / s, x = N_h^-1 a, s = a^H x, N_h = (N + N^H) / 2 (pbb_mvdr_backward) ----
+// With t = w^H g:  q = (g - t a) / conj(s),  p = N_h^-1 q (solve_kernel, strict = 2),
+//   grad a = p - conj(t) w,   grad N = -(p x^H + x p^H) / 2.
+// q, one thread per bin, s in mvdr_scale_kernel's order.
+__global__ void mvdr_backward_rhs_kernel(const double2* __restrict__ atf, const double2* __restrict__ x,
+                                         const double2* __restrict__ w, const double2* __restrict__ g, int n, int D,
+                                         double2* __restrict__ q) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= n) return;
+  double2 s = make_double2(0.0, 0.0), t = make_double2(0.0, 0.0);
+  for (int d = 0; d < D; ++d) {
+    const double2 a = atf[(size_t)m * D + d], v = x[(size_t)m * D + d];
+    const double2 p = cmul(make_double2(a.x, -a.y), v);
+    s.x += p.x; s.y += p.y;
+  }
+  for (int d = 0; d < D; ++d) {
+    const double2 u = cmulc(g[(size_t)m * D + d], w[(size_t)m * D + d]);  // conj(w_d) g_d
+    t.x += u.x; t.y += u.y;
+  }
+  const double2 sc = make_double2(s.x, -s.y);
+  for (int d = 0; d < D; ++d) {
+    const double2 ta = cmul(t, atf[(size_t)m * D + d]), gd = g[(size_t)m * D + d];
+    q[(size_t)m * D + d] = cdiv(make_double2(gd.x - ta.x, gd.y - ta.y), sc);
+  }
+}
+
+// grad N and grad a from p, one thread per entry of N; the threads of column 0 also write grad a
+__global__ void mvdr_backward_kernel(const double2* __restrict__ p, const double2* __restrict__ x,
+                                     const double2* __restrict__ w, const double2* __restrict__ g, int n, int D,
+                                     double2* __restrict__ ga, double2* __restrict__ gn) {
+  const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * D * D) return;
+  const long long m = idx / (D * D);
+  const int i = (int)(idx - m * D * D) / D, j = (int)(idx - m * D * D) % D;
+  const double2* __restrict__ pm = p + m * D;
+  const double2* __restrict__ xm = x + m * D;
+  const double2 a = cmulc(pm[i], xm[j]), b = cmulc(xm[i], pm[j]);
+  gn[idx] = make_double2(-0.5 * (a.x + b.x), -0.5 * (a.y + b.y));
+  if (j == 0) {
+    const double2* __restrict__ wm = w + m * D;
+    double2 t = make_double2(0.0, 0.0);
+    for (int d = 0; d < D; ++d) {
+      const double2 u = cmulc(g[m * D + d], wm[d]);
+      t.x += u.x; t.y += u.y;
+    }
+    const double2 tw = cmulc(wm[i], t);  // conj(t) w_i
+    ga[m * D + i] = make_double2(pm[i].x - tw.x, pm[i].y - tw.y);
+  }
+}
+
+// ---- blind analytic normalisation, out = c w, c = sqrt|nu| / |delta|, nu = w^H N N w, delta = w^H N w ----
+// (pbb_blind_analytic_normalization_backward; N as given, not hermitised).  With r = N w, l = N^H w, rho = Re(w^H g),
+// alpha = rho c conj(nu) / (2 |nu|^2) and beta = -rho c conj(delta) / |delta|^2:
+//   grad w = c g + alpha N r + conj(alpha) N^H l + beta r + conj(beta) l,
+//   grad N = conj(alpha) (w r^H + l w^H) + conj(beta) w w^H.
+// delta = 0 (c is the constant 0 there): zero gradients; nu = 0 with delta != 0 (infinite derivative of sqrt|nu|):
+// NaN.  One warp per bin; r and l (as ban_kernel forms them, so nu and delta are the forward's) in shared memory.
+__global__ void ban_backward_kernel(const double2* __restrict__ vec, const double2* __restrict__ noise,
+                                    const double2* __restrict__ g, int n, int D, double2* __restrict__ gv,
+                                    double2* __restrict__ gn, int warps) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m = blockIdx.x * warps + warp;
+  if (m >= n) return;
+  double2* left = reinterpret_cast<double2*>(smem_raw) + (size_t)2 * D * warp;  // w^H N = conj(l)^T
+  double2* right = left + D;                                                    // N w = r
+  const double2* __restrict__ N = noise + (size_t)m * D * D;
+  const double2* __restrict__ w = vec + (size_t)m * D;
+  const double2* __restrict__ gm = g + (size_t)m * D;
+  for (int a = lane; a < D; a += 32) {
+    double2 lf = make_double2(0.0, 0.0), rt = make_double2(0.0, 0.0);
+    for (int c = 0; c < D; ++c) {
+      const double2 p = cmul(make_double2(w[c].x, -w[c].y), N[c * D + a]);
+      lf.x += p.x; lf.y += p.y;
+      const double2 q = cmul(N[a * D + c], w[c]);
+      rt.x += q.x; rt.y += q.y;
+    }
+    left[a] = lf;
+    right[a] = rt;
+  }
+  __syncwarp();
+  double2 nom = make_double2(0.0, 0.0), den = make_double2(0.0, 0.0);
+  double rho = 0.0;
+  for (int a = 0; a < D; ++a) {  // ban_kernel's order, every lane
+    const double2 p = cmul(left[a], right[a]);
+    nom.x += p.x; nom.y += p.y;
+    const double2 q = cmul(make_double2(w[a].x, -w[a].y), right[a]);
+    den.x += q.x; den.y += q.y;
+    rho += w[a].x * gm[a].x + w[a].y * gm[a].y;
+  }
+  const double nmag = sqrt(sqrt(nom.x * nom.x + nom.y * nom.y));
+  const double dmag = sqrt(den.x * den.x + den.y * den.y);
+  const bool zero = !(dmag != 0.0), nan_bin = !zero && nom.x == 0.0 && nom.y == 0.0;
+  const double c = zero ? 0.0 : nmag / dmag;
+  const double n2 = nom.x * nom.x + nom.y * nom.y, d2 = den.x * den.x + den.y * den.y;
+  const double fa = zero || nan_bin ? 0.0 : 0.5 * rho * c / n2, fb = zero || nan_bin ? 0.0 : -rho * c / d2;
+  const double2 al = make_double2(fa * nom.x, -fa * nom.y), be = make_double2(fb * den.x, -fb * den.y);
+  const double2 alc = make_double2(al.x, -al.y), bec = make_double2(be.x, -be.y);
+  for (int i = lane; i < D; i += 32) {
+    double2 o;
+    if (nan_bin) {
+      o = make_double2(NAN, NAN);
+    } else {
+      double2 nr = make_double2(0.0, 0.0), nl = make_double2(0.0, 0.0);  // (N r)_i, (N^H l)_i
+      for (int k = 0; k < D; ++k) {
+        const double2 p = cmul(N[i * D + k], right[k]);
+        nr.x += p.x; nr.y += p.y;
+        const double2 q = cmul(N[k * D + i], left[k]);  // conj((N^H l)_i term)
+        nl.x += q.x; nl.y -= q.y;
+      }
+      const double2 t1 = cmul(al, nr), t2 = cmul(alc, nl), t3 = cmul(be, right[i]);
+      const double2 t4 = cmulc(bec, left[i]);  // conj(beta) l_i = conj(beta) conj(left_i)
+      o = make_double2(c * gm[i].x + t1.x + t2.x + t3.x + t4.x, c * gm[i].y + t1.y + t2.y + t3.y + t4.y);
+    }
+    gv[(size_t)m * D + i] = o;
+  }
+  for (int idx = lane; idx < D * D; idx += 32) {
+    const int i = idx / D, j = idx - i * D;
+    double2 o;
+    if (nan_bin) {
+      o = make_double2(NAN, NAN);
+    } else {
+      const double2 wr = cmulc(w[i], right[j]);                             // w_i conj(r_j)
+      const double2 lw = cmulc(make_double2(left[i].x, -left[i].y), w[j]);  // l_i conj(w_j)
+      const double2 ww = cmulc(w[i], w[j]);
+      const double2 s = cmul(alc, make_double2(wr.x + lw.x, wr.y + lw.y)), t = cmul(bec, ww);
+      o = make_double2(s.x + t.x, s.y + t.y);
+    }
+    gn[(size_t)m * D * D + idx] = o;
+  }
+}
+
+// ---- rank-1 estimate, out = a a^H t / nu, t = sum_d C_dd (complex), nu = |a|^2 (pbb_rank_one_estimate_backward) ----
+// With G = grad out and q = a^H G a:
+//   grad a = (conj(t) G a + t G^H a) / nu - 2 Re(t conj(q)) / nu^2 a,   grad C = (q / nu) I.
+// nu = 0 gives NaN.  One CTA of 64 threads per bin (D <= 64); G a and G^H a in shared memory.
+__global__ void rank_one_backward_kernel(const double2* __restrict__ a, const double2* __restrict__ cov,
+                                         const double2* __restrict__ gout, int n, int D, double2* __restrict__ ga,
+                                         double2* __restrict__ gc) {
+  __shared__ double2 Ga[64], GHa[64];
+  const int m = blockIdx.x, i = threadIdx.x;
+  if (m >= n) return;
+  const double2* __restrict__ am = a + (size_t)m * D;
+  const double2* __restrict__ G = gout + (size_t)m * D * D;
+  if (i < D) {
+    double2 s = make_double2(0.0, 0.0), sh = make_double2(0.0, 0.0);
+    for (int e = 0; e < D; ++e) {
+      const double2 p = cmul(G[i * D + e], am[e]);
+      s.x += p.x; s.y += p.y;
+      const double2 q = cmulc(am[e], G[e * D + i]);  // conj(G[e][i]) a_e
+      sh.x += q.x; sh.y += q.y;
+    }
+    Ga[i] = s;
+    GHa[i] = sh;
+  }
+  __syncthreads();
+  double2 tr = make_double2(0.0, 0.0), q = make_double2(0.0, 0.0);
+  double na = 0.0;
+  for (int d = 0; d < D; ++d) {  // rank_one_kernel's order for t and nu
+    const double2 c = cov[(size_t)m * D * D + d * D + d];
+    tr.x += c.x; tr.y += c.y;
+    na += am[d].x * am[d].x + am[d].y * am[d].y;
+    const double2 p = cmulc(Ga[d], am[d]);  // conj(a_d) (G a)_d
+    q.x += p.x; q.y += p.y;
+  }
+  const bool nan_bin = !(na > 0.0);
+  const double inv = 1.0 / na, k = 2.0 * (tr.x * q.x + tr.y * q.y) * inv * inv;
+  if (i < D) {
+    const double2 p = cmulc(Ga[i], tr), r = cmul(tr, GHa[i]);  // conj(t) G a, t G^H a
+    ga[(size_t)m * D + i] = nan_bin ? make_double2(NAN, NAN)
+                                    : make_double2((p.x + r.x) * inv - k * am[i].x, (p.y + r.y) * inv - k * am[i].y);
+  }
+  for (int idx = i; idx < D * D; idx += blockDim.x) {
+    const int d = idx / D, e = idx - d * D;
+    gc[(size_t)m * D * D + idx] = nan_bin ? make_double2(NAN, NAN)
+                                          : (d == e ? make_double2(q.x * inv, q.y * inv) : make_double2(0.0, 0.0));
+  }
+}
+
+// ---- y = M x per bin (pbb_matvec_batched_backward): grad M = g x^H, grad x = M^H g ----
+// One thread per (bin, row i): row i of grad M and entry i of grad x.
+__global__ void matvec_backward_kernel(const double2* __restrict__ M, const double2* __restrict__ x,
+                                       const double2* __restrict__ g, int n, int D, double2* __restrict__ gm,
+                                       double2* __restrict__ gx) {
+  const long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (idx >= (long long)n * D) return;
+  const long long m = idx / D;
+  const int i = (int)(idx - m * D);
+  const double2* __restrict__ Mm = M + m * D * D;
+  const double2* __restrict__ xm = x + m * D;
+  const double2* __restrict__ gv = g + m * D;
+  const double2 gi = gv[i];
+  double2 s = make_double2(0.0, 0.0);
+  for (int k = 0; k < D; ++k) {
+    gm[m * D * D + (size_t)i * D + k] = cmulc(gi, xm[k]);
+    const double2 q = cmulc(gv[k], Mm[k * D + i]);  // conj(M[k][i]) g_k
+    s.x += q.x; s.y += q.y;
+  }
+  gx[idx] = s;
 }
 
 }  // namespace pbb

@@ -4,11 +4,22 @@ Shapes follow the reference (beamformer.py:1-12): X (F, D, T), mask (F, K, T),
 PSD (F, K, D, D); leading dims are independent.  numpy in -> numpy out, CUDA
 tensors in -> CUDA tensors out.  Small matrices are complex128 on the device.
 
-get_power_spectral_density_matrix, get_mvdr_vector_souden and
-apply_beamforming_vector are differentiable for CUDA tensors that require grad:
-their backward passes are the device kernels of pbb_*_backward (fp64, gradients
-in the input's dtype, double backward raises).  The other functions return
-outputs without a graph.
+get_power_spectral_density_matrix, get_mvdr_vector_souden, get_gev_vector,
+get_pca_vector (every scaling), get_pca (return_all_vecs=False), get_mvdr_vector,
+blind_analytic_normalization and apply_beamforming_vector are differentiable for
+CUDA tensors that require grad: their backward passes are the device kernels of
+pbb_*_backward (fp64, gradients in the input's dtype, double backward raises).
+
+An eigenvector (GEV, PCA) is defined only up to a per-bin phase, which the
+device's Jacobi solver picks by its rotation sequence.  Its backward holds that
+phase fixed to first order, Im(w^H B dw) = 0, the convention torch.linalg.eigh's
+backward assumes.  For a loss that does not change under w -> e^{i theta} w per
+bin (w w^H, BAN's output power, a rank-1 estimate) the gradient is exact; for a
+phase-dependent loss such as gev+ban -> apply -> istft -> SI-SDR it is the
+gradient with each bin's phase held fixed.
+
+The other functions (get_pca(return_all_vecs=True), LCMV, WMWF, MERL and the
+vector post-processing) return outputs without a graph.
 """
 import numpy as np
 import torch
@@ -127,12 +138,57 @@ class _Psd(torch.autograd.Function):
         return None if gy is None else gy.to(obs.dtype), gm, None, None
 
 
+def _top_eig(psd):
+    """(eigenvalue (...), eigenvector (..., D)) of the largest eigenvalue of psd (..., D, D) complex128 on the device,
+    through _TopEig."""
+    D = psd.shape[-1]
+    af, lead = _flat(psd, 2)
+    val, vec = _TopEig.apply(af)
+    return val.reshape(lead), vec.reshape(*lead, D)
+
+
+class _TopEig(torch.autograd.Function):
+    """a (n, D, D) complex128 -> (the largest eigenvalue (n), its eigenvector (n, D)) of the Hermitian part: the last
+    column of pbb_heig_batched; backward pbb_eigenvector_backward without a second matrix (B = I), the phase held
+    fixed (include/pbb.h)."""
+
+    @staticmethod
+    def forward(ctx, af):
+        n, D = af.shape[0], af.shape[-1]
+        w = _device.empty((n, D), torch.float64)
+        v = _device.empty((n, D, D), torch.complex128)
+        status = _status()
+        _lib.check(_lib.load().pbb_heig_batched(_device.ptr(af), n, D, _device.ptr(w), _device.ptr(v),
+                                                _device.ptr(status), _device.stream_ptr()), 'pbb_heig_batched')
+
+        def on_error(s):
+            raise np.linalg.LinAlgError(f'eigh: non-finite input or no convergence in matrix {s - 1}')
+        _device.check_status(status, on_error)
+        val, vec = w[:, -1].contiguous(), v[:, :, -1].contiguous()
+        ctx.save_for_backward(af, vec)
+        return val, vec
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_val, grad_vec):
+        af, vec = ctx.saved_tensors
+        n, D = vec.shape
+        gv = grad_vec.to(torch.complex128).contiguous()
+        gl = grad_val.to(torch.float64).contiguous()
+        ga = _device.empty((n, D, D), torch.complex128)
+        _lib.check(_lib.load().pbb_eigenvector_backward(
+            _device.ptr(af), None, _device.ptr(vec), _device.ptr(gv), _device.ptr(gl), n, D, _device.ptr(ga), None,
+            _device.stream_ptr()), 'pbb_eigenvector_backward')
+        return ga
+
+
 def get_pca_vector(target_psd_matrix, scaling=None):
-    """Principal eigenvector of the target PSD, beamformer.py:197-224."""
+    """Principal eigenvector of the target PSD, beamformer.py:197-224.  Differentiable for CUDA tensors with respect to
+    the target PSD, with the eigenvector's arbitrary per-bin phase held fixed (_TopEig); the scalings are torch ops on
+    the eigenvalue and eigenvector."""
     like_numpy = not _device.is_tensor(target_psd_matrix)
     psd = _device.to_device(target_psd_matrix, torch.complex128)
-    w, v = eigh(psd)
-    vec, val = v[..., -1], w[..., -1]
+    val, vec = _top_eig(psd)
     if scaling is None:
         pass
     elif scaling == 'trace':
@@ -158,20 +214,44 @@ def get_mvdr_vector(atf_vector, noise_psd_matrix):
     lead = torch.broadcast_shapes(atf.shape[:-1], noise.shape[:-2])
     atf_f = atf.expand(*lead, D).reshape(-1, D).contiguous()
     noise_f = noise.expand(*lead, D, D).reshape(-1, D, D).contiguous()
-    n = atf_f.shape[0]
-    w = _device.empty((n, D), torch.complex128)
-    scratch = _device.empty((n, D), torch.complex128)
-    status = _device.empty((1,), torch.int32)
-    status.zero_()
-    lib = _lib.load()
-    _lib.check(lib.pbb_mvdr(_device.ptr(atf_f), _device.ptr(noise_f), n, D, _device.ptr(w),
-                            _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_mvdr')
-    # a singular noise PSD matrix takes the reference's np.linalg.lstsq fallback (beamformer.py:251-256) on the
-    # device (minimum-norm solution); the status word is only set where that fallback does not exist (D > 40)
-    def on_error(s):
-        raise np.linalg.LinAlgError(f'get_mvdr_vector: singular noise PSD matrix {s - 1} (D > 40: no lstsq fallback)')
-    _device.check_status(status, on_error)
+    w = _Mvdr.apply(atf_f, noise_f)
     return _device.to_host(w.reshape(*lead, D), like_numpy)
+
+
+class _Mvdr(torch.autograd.Function):
+    """atf (n, D), noise (n, D, D) complex128 -> w (n, D) by pbb_mvdr; backward pbb_mvdr_backward (a singular noise
+    matrix, the forward's minimum-norm branch, gives NaN gradients in its bin)."""
+
+    @staticmethod
+    def forward(ctx, atf_f, noise_f):
+        n, D = atf_f.shape
+        w = _device.empty((n, D), torch.complex128)
+        scratch = _device.empty((n, D), torch.complex128)
+        status = _status()
+        _lib.check(_lib.load().pbb_mvdr(_device.ptr(atf_f), _device.ptr(noise_f), n, D, _device.ptr(w),
+                                        _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_mvdr')
+        # a singular noise PSD matrix takes the reference's np.linalg.lstsq fallback (beamformer.py:251-256) on the
+        # device (minimum-norm solution); the status word is only set where that fallback does not exist (D > 40)
+        def on_error(s):
+            raise np.linalg.LinAlgError(
+                f'get_mvdr_vector: singular noise PSD matrix {s - 1} (D > 40: no lstsq fallback)')
+        _device.check_status(status, on_error)
+        ctx.save_for_backward(atf_f, noise_f, scratch, w)
+        return w
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        atf_f, noise_f, x, w = ctx.saved_tensors
+        n, D = atf_f.shape
+        g = grad.to(torch.complex128).contiguous()
+        ga = _device.empty((n, D), torch.complex128)
+        gn = _device.empty((n, D, D), torch.complex128)
+        scratch = _device.empty((n, D), torch.complex128)
+        _lib.check(_lib.load().pbb_mvdr_backward(
+            _device.ptr(atf_f), _device.ptr(noise_f), _device.ptr(x), _device.ptr(w), _device.ptr(g), n, D,
+            _device.ptr(ga), _device.ptr(gn), _device.ptr(scratch), _device.stream_ptr()), 'pbb_mvdr_backward')
+        return ga, gn
 
 
 def get_gev_vector(target_psd_matrix, noise_psd_matrix, force_cython=False,
@@ -191,18 +271,41 @@ def get_gev_vector(target_psd_matrix, noise_psd_matrix, force_cython=False,
     D = a.shape[-1]
     af, lead = _flat(a, 2)
     bf, _ = _flat(b, 2)
-    n = af.shape[0]
-    w = _device.empty((n, D), torch.complex128)
-    status = _device.empty((1,), torch.int32)
-    status.zero_()
-    lib = _lib.load()
-    _lib.check(lib.pbb_gev_batched(_device.ptr(af), _device.ptr(bf), n, D, _device.ptr(w),
-                                   _device.ptr(status), _device.stream_ptr()), 'pbb_gev_batched')
-    def on_error(s):
-        # get_gev_vector.pyx:130-147 / beamformer.py:398-408
-        raise ValueError(f'Error for frequency {s - 1}: noise PSD not positive definite or non-finite input')
-    _device.check_status(status, on_error)
+    w = _Gev.apply(af, bf)
     return _device.to_host(w.reshape(*lead, D), like_numpy)
+
+
+class _Gev(torch.autograd.Function):
+    """target, noise (n, D, D) complex128 -> the top generalised eigenvector w (n, D), w^H noise w = 1, by
+    pbb_gev_batched; backward pbb_eigenvector_backward with the phase held fixed (include/pbb.h)."""
+
+    @staticmethod
+    def forward(ctx, af, bf):
+        n, D = af.shape[0], af.shape[-1]
+        w = _device.empty((n, D), torch.complex128)
+        status = _status()
+        _lib.check(_lib.load().pbb_gev_batched(_device.ptr(af), _device.ptr(bf), n, D, _device.ptr(w),
+                                               _device.ptr(status), _device.stream_ptr()), 'pbb_gev_batched')
+
+        def on_error(s):
+            # get_gev_vector.pyx:130-147 / beamformer.py:398-408
+            raise ValueError(f'Error for frequency {s - 1}: noise PSD not positive definite or non-finite input')
+        _device.check_status(status, on_error)
+        ctx.save_for_backward(af, bf, w)
+        return w
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        af, bf, w = ctx.saved_tensors
+        n, D = w.shape
+        g = grad.to(torch.complex128).contiguous()
+        ga = _device.empty((n, D, D), torch.complex128)
+        gb = _device.empty((n, D, D), torch.complex128)
+        _lib.check(_lib.load().pbb_eigenvector_backward(
+            _device.ptr(af), _device.ptr(bf), _device.ptr(w), _device.ptr(g), None, n, D, _device.ptr(ga),
+            _device.ptr(gb), _device.stream_ptr()), 'pbb_eigenvector_backward')
+        return ga, gb
 
 
 def get_mvdr_vector_souden(target_psd_matrix, noise_psd_matrix, ref_channel=None,
@@ -302,12 +405,36 @@ def blind_analytic_normalization(vector, noise_psd_matrix):
     lead = torch.broadcast_shapes(v.shape[:-1], nz.shape[:-2])
     vf = v.expand(*lead, D).reshape(-1, D).contiguous()
     nf = nz.expand(*lead, D, D).reshape(-1, D, D).contiguous()
-    out = _device.empty(vf.shape, torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_blind_analytic_normalization(_device.ptr(vf), _device.ptr(nf), vf.shape[0], D,
-                                                    _device.ptr(out), _device.stream_ptr()),
-               'pbb_blind_analytic_normalization')
+    out = _Ban.apply(vf, nf)
     return _device.to_host(out.reshape(*lead, D), like_numpy)
+
+
+class _Ban(torch.autograd.Function):
+    """vector (n, D), noise (n, D, D) complex128 -> the normalised vector (n, D) by pbb_blind_analytic_normalization;
+    backward pbb_blind_analytic_normalization_backward."""
+
+    @staticmethod
+    def forward(ctx, vf, nf):
+        n, D = vf.shape
+        out = _device.empty((n, D), torch.complex128)
+        _lib.check(_lib.load().pbb_blind_analytic_normalization(_device.ptr(vf), _device.ptr(nf), n, D,
+                                                                _device.ptr(out), _device.stream_ptr()),
+                   'pbb_blind_analytic_normalization')
+        ctx.save_for_backward(vf, nf)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        vf, nf = ctx.saved_tensors
+        n, D = vf.shape
+        g = grad.to(torch.complex128).contiguous()
+        gv = _device.empty((n, D), torch.complex128)
+        gn = _device.empty((n, D, D), torch.complex128)
+        _lib.check(_lib.load().pbb_blind_analytic_normalization_backward(
+            _device.ptr(vf), _device.ptr(nf), _device.ptr(g), n, D, _device.ptr(gv), _device.ptr(gn),
+            _device.stream_ptr()), 'pbb_blind_analytic_normalization_backward')
+        return gv, gn
 
 
 def apply_beamforming_vector(vector, mix):
@@ -406,7 +533,12 @@ def _tiny(*arrays):
 
 def get_pca(target_psd_matrix, return_all_vecs=False):
     """All principal components and eigenvalues, beamformer.py:163-194: (eigenvectors, eigenvalues) with
-    return_all_vecs, else the eigenvector of the largest eigenvalue (..., D) and that eigenvalue (...)."""
+    return_all_vecs, else the eigenvector of the largest eigenvalue (..., D) and that eigenvalue (...).  Without
+    return_all_vecs a tensor input is differentiable in both outputs (_TopEig, the eigenvector's phase held fixed);
+    return_all_vecs=True returns outputs without a graph."""
+    if not return_all_vecs and _device.is_tensor(target_psd_matrix):
+        val, vec = _top_eig(_device.to_device(target_psd_matrix, torch.complex128))
+        return vec, val
     w, v = eigh(target_psd_matrix)
     if return_all_vecs:
         return v, w

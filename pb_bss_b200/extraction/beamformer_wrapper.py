@@ -3,9 +3,18 @@
 ``get_bf_vector('rank1_gev+mvdr_souden+ban', target_psd, noise_psd)`` chains the
 device kernels of ``beamformer.py``: an optional rank-1 approximation of the
 target PSD, the core beamformer, an optional blind analytic normalisation.
+
+Every string get_bf_vector accepts is differentiable for CUDA tensors that
+require grad, except ``chN`` (a constant vector) and ``wmwf`` (not built): the
+rank-1 estimates and the scaled GEV ATF have device backward passes here
+(pbb_rank_one_estimate_backward, pbb_matvec_batched_backward), the beamformers
+theirs in ``beamformer.py``.  Through a GEV or PCA vector the gradient holds each
+bin's eigenvector phase fixed (see ``beamformer.py``); the rank-1 estimates do
+not depend on that phase, so their gradients are exact.
 """
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from .. import _device, _lib
 from .beamformer import (
@@ -27,11 +36,35 @@ def _rank_one(vector, covariance):
     lead = tuple(c.shape[:-2])
     af = a.expand(*lead, D).reshape(-1, D).contiguous()
     cf = c.reshape(-1, D, D).contiguous()
-    out = _device.empty(cf.shape, torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_rank_one_estimate(_device.ptr(af), _device.ptr(cf), cf.shape[0], D, _device.ptr(out),
-                                         _device.stream_ptr()), 'pbb_rank_one_estimate')
+    out = _RankOne.apply(af, cf)
     return _device.to_host(out.reshape(*lead, D, D), like_numpy)
+
+
+class _RankOne(torch.autograd.Function):
+    """vector (n, D), covariance (n, D, D) complex128 -> a a^H tr(C) / |a|^2 (n, D, D) by pbb_rank_one_estimate;
+    backward pbb_rank_one_estimate_backward."""
+
+    @staticmethod
+    def forward(ctx, af, cf):
+        n, D = af.shape
+        out = _device.empty((n, D, D), torch.complex128)
+        _lib.check(_lib.load().pbb_rank_one_estimate(_device.ptr(af), _device.ptr(cf), n, D, _device.ptr(out),
+                                                     _device.stream_ptr()), 'pbb_rank_one_estimate')
+        ctx.save_for_backward(af, cf)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        af, cf = ctx.saved_tensors
+        n, D = af.shape
+        g = grad.to(torch.complex128).contiguous()
+        ga = _device.empty((n, D), torch.complex128)
+        gc = _device.empty((n, D, D), torch.complex128)
+        _lib.check(_lib.load().pbb_rank_one_estimate_backward(
+            _device.ptr(af), _device.ptr(cf), _device.ptr(g), n, D, _device.ptr(ga), _device.ptr(gc),
+            _device.stream_ptr()), 'pbb_rank_one_estimate_backward')
+        return ga, gc
 
 
 def _matvec(matrix, vector):
@@ -42,11 +75,35 @@ def _matvec(matrix, vector):
     lead = torch.broadcast_shapes(m.shape[:-2], v.shape[:-1])
     mf = m.expand(*lead, D, D).reshape(-1, D, D).contiguous()
     vf = v.expand(*lead, D).reshape(-1, D).contiguous()
-    out = _device.empty(vf.shape, torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_matvec_batched(_device.ptr(mf), _device.ptr(vf), mf.shape[0], D, _device.ptr(out),
-                                      _device.stream_ptr()), 'pbb_matvec_batched')
+    out = _Matvec.apply(mf, vf)
     return _device.to_host(out.reshape(*lead, D), like_numpy)
+
+
+class _Matvec(torch.autograd.Function):
+    """matrix (n, D, D), vector (n, D) complex128 -> matrix @ vector (n, D) by pbb_matvec_batched; backward
+    pbb_matvec_batched_backward."""
+
+    @staticmethod
+    def forward(ctx, mf, vf):
+        n, D = vf.shape
+        out = _device.empty((n, D), torch.complex128)
+        _lib.check(_lib.load().pbb_matvec_batched(_device.ptr(mf), _device.ptr(vf), n, D, _device.ptr(out),
+                                                  _device.stream_ptr()), 'pbb_matvec_batched')
+        ctx.save_for_backward(mf, vf)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        mf, vf = ctx.saved_tensors
+        n, D = vf.shape
+        g = grad.to(torch.complex128).contiguous()
+        gm = _device.empty((n, D, D), torch.complex128)
+        gv = _device.empty((n, D), torch.complex128)
+        _lib.check(_lib.load().pbb_matvec_batched_backward(
+            _device.ptr(mf), _device.ptr(vf), _device.ptr(g), n, D, _device.ptr(gm), _device.ptr(gv),
+            _device.stream_ptr()), 'pbb_matvec_batched_backward')
+        return gm, gv
 
 
 def get_pca_rank_one_estimate(covariance_matrix, **atf_kwargs):

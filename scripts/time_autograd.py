@@ -1,12 +1,15 @@
 """Time the differentiable mask-based beamforming chain on the device against the same chain restated in torch
-(oracle/autograd_oracle.py, cuFFT / cuBLAS / cuSOLVER through torch) on the same GPU, with the GPU name and power limit
-read in the same run.
+(oracle/autograd_oracle.py and oracle/bf_autograd_oracle.py, cuFFT / cuBLAS / cuSOLVER through torch) on the same
+GPU, with the GPU name and power limit read in the same run.
 
-    python scripts/time_autograd.py [--out result.json] [--trace-dir DIR]
+    python scripts/time_autograd.py [--beamformer souden|gev+ban|pca+mvdr|rank1_gev+mvdr_souden]
+                                    [--out result.json] [--trace-dir DIR]
 
 Shape: F = 257, D = 6, T = 1002 frames, size 512, shift 128 (an 8 s, 16 kHz six-channel STFT).  The chain is
-float32 mask logits -> sigmoid -> PSD (target, noise) -> Souden MVDR (automatic reference channel) -> apply -> istft ->
--si_sdr.  Forward and forward + backward times are medians of CUDA-event windows over several calls after a warm-up
+float32 mask logits -> sigmoid -> PSD (target, noise) -> beamformer -> apply -> istft -> -si_sdr.  The beamformer is
+the Souden MVDR (automatic reference channel; the default) or one of get_bf_vector's gev+ban, pca+mvdr and
+rank1_gev+mvdr_souden (reference channel 0); the torch side restates it with the eigenvectors' phase aligned to the
+device's.  Forward and forward + backward times are medians of CUDA-event windows over several calls after a warm-up
 (the forward synchronises once to pick the reference channel, on both sides).  A separate profiled run (torch.profiler,
 CUDA activity) gives each backward kernel's time; with the kernel's algorithmic bytes (each array it must read or
 write, once) it gives the achieved bandwidth and the share of the 3.35 TB/s HBM3 data-sheet figure of the H100 SXM.
@@ -23,8 +26,10 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import autograd_oracle as AO  # noqa: E402
+from oracle import bf_autograd_oracle as BO  # noqa: E402
 from pb_bss_b200.evaluation import si_sdr  # noqa: E402
 from pb_bss_b200.extraction import beamformer as B  # noqa: E402
+from pb_bss_b200.extraction import beamformer_wrapper as W  # noqa: E402
 from pb_bss_b200.transform import istft, stft  # noqa: E402
 from scripts.time_embedding_mm import gpu_info  # noqa: E402
 from scripts.time_extraction import device_seconds  # noqa: E402
@@ -34,22 +39,49 @@ SIZE, SHIFT, D = 512, 128, 6
 N = 999 * SHIFT - 3
 
 
-def chain(torch_side, y, logits, target, ref_channel=None):
+BEAMFORMERS = ('souden', 'gev+ban', 'pca+mvdr', 'rank1_gev+mvdr_souden')
+
+
+def torch_beamformer(name, pt, pn, phase):
+    """get_bf_vector(name) restated in torch; phase: the device's eigenvector (the GEV or PCA vector), whose per-bin
+    phase the restatement takes (oracle/bf_autograd_oracle.py: fix_phase)"""
+    if name == 'gev+ban':
+        return BO.blind_analytic_normalization(BO.gev_vector(pt, pn, phase)[0], pn)
+    if name == 'pca+mvdr':
+        return BO.mvdr_vector(BO.pca(pt, phase)[1], pn)
+    a = BO.matvec(pn, BO.gev_vector(pt, pn, phase)[0])  # rank1_gev+mvdr_souden
+    return AO.mvdr_vector_souden(BO.rank_one_estimate(a, pt), pn, 0)[0]
+
+
+def device_phase(name, pt, pn):
+    """the device's eigenvector of the chain, for the torch side's phase"""
+    with torch.no_grad():
+        return B.get_pca_vector(pt) if name == 'pca+mvdr' else B.get_gev_vector(pt, pn)
+
+
+def chain(torch_side, y, logits, target, ref_channel=None, beamformer='souden', phase=None):
     mask = torch.sigmoid(logits)
     if torch_side:
         pt = AO.power_spectral_density(y, mask[:, 0])
         pn = AO.power_spectral_density(y, mask[:, 1])
-        w, ref = AO.mvdr_vector_souden(pt, pn, ref_channel)
+        if beamformer == 'souden':
+            w, ref = AO.mvdr_vector_souden(pt, pn, ref_channel)
+        else:
+            w, ref = torch_beamformer(beamformer, pt, pn, phase), None
         x = AO.istft(AO.apply_beamforming_vector(w, y).transpose(0, 1), SIZE, SHIFT)
         return -AO.si_sdr(target, x[:target.shape[-1]]), ref
     pt = B.get_power_spectral_density_matrix(y, mask[:, 0])
     pn = B.get_power_spectral_density_matrix(y, mask[:, 1])
-    w, ref = B.get_mvdr_vector_souden(pt, pn, ref_channel, return_ref_channel=True)
+    if beamformer == 'souden':
+        w, ref = B.get_mvdr_vector_souden(pt, pn, ref_channel, return_ref_channel=True)
+    else:
+        kw = {'ref_channel': 0} if 'souden' in beamformer else {}
+        w, ref = W.get_bf_vector(beamformer, pt, pn, **kw), None
     x = istft(B.apply_beamforming_vector(w, y).transpose(0, 1), size=SIZE, shift=SHIFT)
     return -si_sdr(target, x[:target.shape[-1]]), ref
 
 
-def kernel_bytes(F, T, n_out, rows_stft, frames_stft):
+def kernel_bytes(F, T, n_out, rows_stft, frames_stft, pencil=True):
     """Algorithmic bytes of one call of each backward kernel at this shape (complex128 16 B, float64 8 B)."""
     c, r, wl, bins = 16, 8, SIZE, SIZE // 2 + 1
     return {
@@ -63,6 +95,13 @@ def kernel_bytes(F, T, n_out, rows_stft, frames_stft):
         'istft_backward_kernel': n_out * r + T * bins * c,
         'si_sdr_backward_kernel': 3 * N * r,
         'stft_backward_kernel': rows_stft * frames_stft * (bins * c + wl * r),
+        # the get_bf_vector backward kernels: A and B (or N) read, their gradients written, the vectors
+        'eig_backward_kernel': F * D * D * c * (4 if pencil else 2) + 2 * F * D * c,
+        'mvdr_backward_rhs_kernel': 4 * F * D * c + F * D * c,
+        'mvdr_backward_kernel': F * D * c * 4 + F * D * D * c + F * D * c,
+        'ban_backward_kernel': F * D * D * c * 2 + 3 * F * D * c,
+        'rank_one_backward_kernel': F * D * D * c * 3 + 2 * F * D * c,
+        'matvec_backward_kernel': F * D * D * c * 2 + 3 * F * D * c,
     }
 
 
@@ -70,7 +109,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', default=None)
     ap.add_argument('--trace-dir', default=None)
+    ap.add_argument('--beamformer', default='souden', choices=BEAMFORMERS)
     args = ap.parse_args()
+    bf = args.beamformer
     torch.cuda.set_device(0)
     rng = np.random.default_rng(0)
     sig = torch.tensor(rng.standard_normal((D, N)), device='cuda')
@@ -78,16 +119,23 @@ def main():
     F, _, T = y.shape
     logits = torch.tensor(rng.standard_normal((F, 2, T)), dtype=torch.float32, device='cuda', requires_grad=True)
     target = torch.tensor(rng.standard_normal(N), device='cuda')
-    _, ref = chain(False, y, logits, target)
-    result = {'gpu': gpu_info(), 'F': F, 'D': D, 'T': T, 'size': SIZE, 'shift': SHIFT, 'samples': N,
-              'reference_channel': ref, 'chain': {}}
+    _, ref = chain(False, y, logits, target, beamformer=bf)
+    phase = None
+    if bf in ('gev+ban', 'pca+mvdr', 'rank1_gev+mvdr_souden'):
+        with torch.no_grad():
+            mask = torch.sigmoid(logits)
+            phase = device_phase(bf, B.get_power_spectral_density_matrix(y, mask[:, 0]),
+                                 B.get_power_spectral_density_matrix(y, mask[:, 1]))
+    result = {'gpu': gpu_info(), 'beamformer': bf, 'F': F, 'D': D, 'T': T, 'size': SIZE, 'shift': SHIFT,
+              'samples': N, 'reference_channel': ref if bf == 'souden' else (0 if 'souden' in bf else None),
+              'chain': {}}
 
     def fwd(torch_side):
         with torch.no_grad():
-            chain(torch_side, y, logits, target, ref if torch_side else None)
+            chain(torch_side, y, logits, target, ref if torch_side else None, bf, phase)
 
     def fwd_bwd(torch_side):
-        loss, _ = chain(torch_side, y, logits, target, ref if torch_side else None)
+        loss, _ = chain(torch_side, y, logits, target, ref if torch_side else None, bf, phase)
         torch.autograd.grad(loss, logits)
 
     # alternate the two sides so that drift on the shared machine hits both
@@ -110,14 +158,14 @@ def main():
     steps = 10
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         for _ in range(steps):
-            loss, _ = chain(False, y, logits, target)
+            loss, _ = chain(False, y, logits, target, beamformer=bf)
             torch.autograd.grad(loss, logits)
             torch.autograd.grad(X, x, gX, retain_graph=True)
         torch.cuda.synchronize()
     if args.trace_dir:
         os.makedirs(args.trace_dir, exist_ok=True)
         prof.export_chrome_trace(os.path.join(args.trace_dir, 'time_autograd.pt.trace.json'))
-    nbytes = kernel_bytes(F, T, T * SHIFT - SHIFT - (SIZE - SHIFT), D, T)
+    nbytes = kernel_bytes(F, T, T * SHIFT - SHIFT - (SIZE - SHIFT), D, T, pencil=bf != 'pca+mvdr')
     kernels = {}
     for evt in prof.key_averages():
         name = evt.key
