@@ -1332,6 +1332,59 @@ int pbb_wpe(const void* y, int dtype, long long bins, int D, long long T, long l
             long long psd_context, int valid, long long group, void* workspace, size_t workspace_bytes, int* status,
             void* stream);
 
+/* pbb_wpe that also keeps, per iteration i < iterations, the filter G_i in G_save (iterations, bins, n, D)
+ * complex128 and the weights w_i in w_save (iterations, bins, T) float64, both contiguous (both null: pbb_wpe).  The
+ * launches and so the output are those of pbb_wpe; the copies are device-to-device on the stream. */
+int pbb_wpe_forward(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                    long long yst, void* out, long long osb, long long osd, long long ost, int taps, int delay,
+                    int iterations, long long psd_context, int valid, long long group, void* workspace,
+                    size_t workspace_bytes, int* status, void* G_save, double* w_save, void* stream);
+
+/* One WPE step with the caller's weights: R, P, G and X = Y - G^H Yt of pbb_wpe with w_t = weight[b wsb + t wst]
+ * (float64, element strides) in place of the power.  Workspace pbb_wpe_workspace_bytes; G_out (null: not kept)
+ * receives G (bins, n, D) complex128; *status as pbb_wpe. */
+int pbb_wpe_step(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                 long long yst, const double* weight, long long wsb, long long wst, void* out, long long osb,
+                 long long osd, long long ost, int taps, int delay, int valid, long long group, void* workspace,
+                 size_t workspace_bytes, int* status, void* G_out, void* stream);
+
+/* Backward of one WPE step, in torch's convention (the gradient of a real loss L is dL/dRe + i dL/dIm).  Per bin,
+ * n = taps D, yt_t the delayed stack (row k D + d is y_{d, t - delay - k}), m_t = 1 for t in S (else 0), the forward
+ * G = R^-1 P and x_t = y_t - G^H yt_t, and the incoming gradient xbar_t:
+ *   Gbar = -sum_t yt_t xbar_t^H (every frame); R Pbar = Gbar with the forward's pivots (R is Hermitian, so the
+ *     gradient of P is Pbar and that of R is -Pbar G^H);
+ *   c_t = Pbar^H yt_t, u_t = xbar_t + m_t w_t c_t, b_t = m_t w_t x_t;
+ *   ytbar_t = -G u_t + Pbar b_t (the R and P terms fold together through G^H yt_t = y_t - x_t);
+ *   ybar_t = u_t + sum_k ytbar_{k D + d, t + delay + k} (the shift-add of ytbar onto y, a gather);
+ *   wbar_t = m_t Re(c_t^H x_t).
+ * An empty S (valid, T <= delay + taps - 1) makes G = 0 for every input: ybar = xbar, wbar = 0.
+ * y as in pbb_wpe; weight (bins, T) float64 and G (bins, n, D) complex128 are the forward's (contiguous); xbar and
+ * ybar (bins, D, T) complex128 contiguous, ybar accumulated (+=); wbar (bins, T) float64 written.  R is recomputed
+ * with the forward's kernel and weights, so it is bit for bit the forward's.  A bin whose R has an exactly zero pivot
+ * (the forward took lstsq) or is not finite gets NaN gradients; other bins are unaffected. */
+size_t pbb_wpe_backward_workspace_bytes(long long group, int D, long long T, int taps, int delay, int valid);
+int pbb_wpe_backward(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                     long long yst, const double* weight, const void* G, const void* xbar, int taps, int delay,
+                     int valid, void* ybar, double* wbar, long long group, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
+/* Backward of the power chain lambda_t = mean_d |x_dt|^2, lambda_c = its psd_context mean over the frames that exist
+ * (psd_context < 0: inf), with x = y - G^H Yt (G (bins, taps D, D) complex128; null: x = y, taps and delay unused).
+ * mode PBB_WPE_GRAD_PLAIN: gin (bins, T) is lambda_c's gradient (get_power).  PBB_WPE_GRAD_INVERSE: gin is the
+ * gradient of w = 1 / max(lambda_c, 1e-10 M) with M the max per bin (wpe's weights); PBB_WPE_GRAD_INVERSE_ALL: the same
+ * with M the max over all bins (get_power_inverse).  With z = max(lambda_c, eps M): zbar = -wbar / z^2, split as
+ * torch.maximum does (all of it to the larger operand, half each on a tie); M's gradient eps sum(...) goes to the
+ * maxima of lambda_c in equal shares (amax).  Then lambdabar_t = sum_{s : |s - t| <= c} lambdabar_c,s / n_s with n_s
+ * the frames in s's window, and xbar_dt += (2 / D) lambdabar_t x_dt (xbar (bins, D, T) complex128 contiguous,
+ * accumulated).  lambda_c is recomputed with the forward's kernel, so the max and its ties are the forward's. */
+#define PBB_WPE_GRAD_INVERSE 0
+#define PBB_WPE_GRAD_PLAIN 1
+#define PBB_WPE_GRAD_INVERSE_ALL 2
+size_t pbb_wpe_power_backward_workspace_bytes(long long bins, long long T);
+int pbb_wpe_power_backward(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                           long long yst, const void* G, int taps, int delay, long long psd_context, int mode,
+                           const double* gin, void* xbar, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Workspace of pbb_wpe_power: bins * T doubles. */
 size_t pbb_wpe_power_workspace_bytes(long long bins, long long T);
 

@@ -222,6 +222,16 @@ SIGNATURES = {
     'pbb_wpe_workspace_bytes': (_sz, [_ll, _i, _ll, _i, _i, _i]),
     'pbb_wpe': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _i, _ll, _vp, _sz,
                      _vp, _vp]),
+    'pbb_wpe_forward': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _i, _ll, _vp,
+                             _sz, _vp, _vp, _vp, _vp]),
+    'pbb_wpe_step': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _vp,
+                          _sz, _vp, _vp, _vp]),
+    'pbb_wpe_backward_workspace_bytes': (_sz, [_ll, _i, _ll, _i, _i, _i]),
+    'pbb_wpe_backward': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _ll, _vp, _sz,
+                              _vp]),
+    'pbb_wpe_power_backward_workspace_bytes': (_sz, [_ll, _ll]),
+    'pbb_wpe_power_backward': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _i, _i, _ll, _i, _vp, _vp, _vp, _sz,
+                                    _vp]),
     'pbb_wpe_power_workspace_bytes': (_sz, [_ll, _ll]),
     'pbb_wpe_power': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _ll, _i, _vp, _vp, _sz, _vp]),
     'pbb_wpe_build_y_tilde': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _i, _i, _vp, _vp]),

@@ -88,9 +88,27 @@ static int wpe_corr(const TIn* y, WpeStrides ys, const WpeShape& s, long long bi
   return wpe_corr_launch<22>(y, ys, s, bins, w, part, st);
 }
 
+// R, P from the weights w of a group, G = stable_solve(R, P): wpe_corr, wpe_solve_kernel and wpe_lstsq_kernel
+template <class TIn>
+static int wpe_solve_group(const TIn* yg, WpeStrides ys, const WpeShape& s, long long g, const double* w, double* part,
+                           double2* G, int* lstsq, int* status, cudaStream_t st) {
+  int rc = wpe_corr<TIn>(yg, ys, s, g, w, part, st);
+  if (rc) return rc;
+  {
+    LaunchScope ls("wpe_solve_kernel", st);
+    wpe_solve_kernel<<<(unsigned)g, 256, wpe_solve_smem_bytes(s.n, s.D), st>>>(part, s, G, lstsq, status);
+    PBB_CUDA(cudaGetLastError());
+  }
+  LaunchScope ls("wpe_lstsq_kernel", st);
+  wpe_lstsq_kernel<<<(unsigned)g, 32, wpe_lstsq_smem_bytes(s.n, s.D), st>>>(part, s, lstsq, G);
+  PBB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 template <class TIn>
 static int wpe_run(const TIn* y, WpeStrides ys, long long bins, TIn* out, WpeStrides os, const WpeShape& s,
-                   int iterations, long long group, char* ws, int* status, cudaStream_t st) {
+                   int iterations, long long group, char* ws, int* status, cudaStream_t st, double2* G_save,
+                   double* w_save) {
   const WpeLayout l = wpe_layout(group, s);
   double* w = reinterpret_cast<double*>(ws + l.w);
   double* lam = reinterpret_cast<double*>(ws + l.lam);
@@ -109,23 +127,139 @@ static int wpe_run(const TIn* y, WpeStrides ys, long long bins, TIn* out, WpeStr
     if (rc) return rc;
     for (int it = 0; it < iterations; ++it) {
       const bool last = it == iterations - 1;
-      rc = wpe_corr<TIn>(yg, ys, s, g, w, part, st);
+      if (w_save != nullptr)
+        PBB_CUDA(cudaMemcpyAsync(w_save + (it * bins + b0) * s.T, w, (size_t)g * s.T * sizeof(double),
+                                 cudaMemcpyDeviceToDevice, st));
+      rc = wpe_solve_group<TIn>(yg, ys, s, g, w, part, G, lstsq, status, st);
       if (rc) return rc;
-      {
-        LaunchScope ls("wpe_solve_kernel", st);
-        wpe_solve_kernel<<<(unsigned)g, 256, solve_smem, st>>>(part, s, G, lstsq, status);
-        PBB_CUDA(cudaGetLastError());
-      }
-      {
-        LaunchScope ls("wpe_lstsq_kernel", st);
-        wpe_lstsq_kernel<<<(unsigned)g, 32, lstsq_smem, st>>>(part, s, lstsq, G);
-        PBB_CUDA(cudaGetLastError());
-      }
+      if (G_save != nullptr)
+        PBB_CUDA(cudaMemcpyAsync(G_save + (it * bins + b0) * s.n * s.D, G, (size_t)g * s.n * s.D * sizeof(double2),
+                                 cudaMemcpyDeviceToDevice, st));
       rc = wpe_filter_launch<TIn>(yg, ys, s, g, G, last ? og : nullptr, os, last ? kWpePowerNone : kWpePowerInverse,
                                   lam, w, status, st);
       if (rc) return rc;
     }
   }
+  return 0;
+}
+
+// one WPE step with the caller's weights wsrc (element (b, t) at b wsb + t wst), copied into the workspace's w:
+// pbb_wpe's launches with the copy in place of the power kernel; G_save (null: not kept) receives the filters
+template <class TIn>
+static int wpe_step_run(const TIn* y, WpeStrides ys, long long bins, const double* wsrc, long long wsb,
+                        long long wst, TIn* out, WpeStrides os, const WpeShape& s, long long group, char* ws,
+                        int* status, double2* G_save, cudaStream_t st) {
+  const WpeLayout l = wpe_layout(group, s);
+  double* w = reinterpret_cast<double*>(ws + l.w);
+  double* part = reinterpret_cast<double*>(ws + l.part);
+  double2* G = reinterpret_cast<double2*>(ws + l.G);
+  int* lstsq = reinterpret_cast<int*>(ws + l.lstsq);
+  const size_t solve_smem = wpe_solve_smem_bytes(s.n, s.D), lstsq_smem = wpe_lstsq_smem_bytes(s.n, s.D);
+  PBB_CUDA(cudaFuncSetAttribute(wpe_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem));
+  PBB_CUDA(cudaFuncSetAttribute(wpe_lstsq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lstsq_smem));
+  for (long long b0 = 0; b0 < bins; b0 += group) {
+    const long long g = bins - b0 < group ? bins - b0 : group;
+    {
+      LaunchScope ls("wpe_weight_copy_kernel", st);
+      const long long total = g * s.T;
+      wpe_weight_copy_kernel<<<(unsigned)(total / 256 + 1 < 65536 ? total / 256 + 1 : 65536), 256, 0, st>>>(
+          wsrc + b0 * wsb, wsb, wst, g, s.T, w);
+      PBB_CUDA(cudaGetLastError());
+    }
+    int rc = wpe_solve_group<TIn>(y + b0 * ys.b, ys, s, g, w, part, G, lstsq, status, st);
+    if (rc) return rc;
+    if (G_save != nullptr)
+      PBB_CUDA(cudaMemcpyAsync(G_save + b0 * s.n * s.D, G, (size_t)g * s.n * s.D * sizeof(double2),
+                               cudaMemcpyDeviceToDevice, st));
+    rc = wpe_filter_launch<TIn>(y + b0 * ys.b, ys, s, g, G, out + b0 * os.b, os, kWpePowerNone, nullptr, nullptr,
+                                status, st);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
+struct WpeBackLayout {
+  size_t part, Pbar, ub, total;  // byte offsets
+};
+
+static WpeBackLayout wpe_back_layout(long long group, const WpeShape& s) {
+  WpeBackLayout l;
+  l.part = 0;
+  l.Pbar = wpe_align(l.part + (size_t)group * s.parts * s.ntiles * 64 * sizeof(double));
+  l.ub = wpe_align(l.Pbar + (size_t)group * s.n * s.D * sizeof(double2));
+  l.total = l.ub + (size_t)group * 2 * s.D * s.T * sizeof(double2);
+  return l;
+}
+
+// one stage of the step backward: the forward's R again (wpe_corr with the same weights, bit for bit), Gbar, Pbar =
+// R^-1 Gbar, then the per-frame pass.  An empty S (valid, T <= delay + taps - 1) has G = 0 for every input: Pbar = 0.
+template <class TIn>
+static int wpe_backward_run(const TIn* y, WpeStrides ys, long long bins, const WpeShape& s, const double* w,
+                            const double2* G, const double2* xbar, double2* ybar, double* wbar, long long group,
+                            char* ws, cudaStream_t st) {
+  const WpeBackLayout l = wpe_back_layout(group, s);
+  double* part = reinterpret_cast<double*>(ws + l.part);
+  double2* Pbar = reinterpret_cast<double2*>(ws + l.Pbar);
+  double2* ub = reinterpret_cast<double2*>(ws + l.ub);
+  const size_t gbar_smem = wpe_gbar_smem_bytes(s.D, s.taps), solve_smem = wpe_solve_smem_bytes(s.n, s.D);
+  const size_t back_smem = wpe_step_backward_smem_bytes(s.D, s.taps);
+  PBB_CUDA(cudaFuncSetAttribute(wpe_gbar_kernel<TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gbar_smem));
+  PBB_CUDA(cudaFuncSetAttribute(wpe_solve_rhs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)solve_smem));
+  PBB_CUDA(cudaFuncSetAttribute(wpe_step_backward_kernel<TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)back_smem));
+  const long long per = (long long)s.D * s.T;
+  for (long long b0 = 0; b0 < bins; b0 += group) {
+    const long long g = bins - b0 < group ? bins - b0 : group;
+    const TIn* yg = y + b0 * ys.b;
+    if (s.tb < s.T) {
+      int rc = wpe_corr<TIn>(yg, ys, s, g, w + b0 * s.T, part, st);
+      if (rc) return rc;
+      {
+        LaunchScope ls("wpe_gbar_kernel", st);
+        wpe_gbar_kernel<TIn><<<(unsigned)g, 256, gbar_smem, st>>>(yg, ys, s, xbar + b0 * per, Pbar);
+        PBB_CUDA(cudaGetLastError());
+      }
+      {
+        LaunchScope ls("wpe_solve_rhs_kernel", st);
+        wpe_solve_rhs_kernel<<<(unsigned)g, 256, solve_smem, st>>>(part, s, Pbar);
+        PBB_CUDA(cudaGetLastError());
+      }
+    } else {
+      PBB_CUDA(cudaMemsetAsync(Pbar, 0, (size_t)g * s.n * s.D * sizeof(double2), st));
+    }
+    LaunchScope ls("wpe_step_backward_kernel", st);
+    wpe_step_backward_kernel<TIn><<<(unsigned)g, 256, back_smem, st>>>(
+        yg, ys, s, G + b0 * s.n * s.D, Pbar, w + b0 * s.T, xbar + b0 * per, ub, ybar + b0 * per, wbar + b0 * s.T);
+    PBB_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+// the power chain's backward over all bins; workspace: lambda, lambda_c and a gradient scratch, bins T doubles each
+template <class TIn>
+static int wpe_power_backward_run(const TIn* y, WpeStrides ys, long long bins, const WpeShape& s, const double2* G,
+                                  int mode, const double* gin, double2* xbar, double* ws, cudaStream_t st) {
+  double* lam = ws;
+  double* lamc = ws + bins * s.T;
+  double* pbar = lamc + bins * s.T;
+  if (mode != kWpeGradPlain) {
+    // lambda_c exactly as the forward computed it: the forward's own kernel and arguments
+    int rc = wpe_filter_launch<TIn>(y, ys, s, bins, G, nullptr, ys, kWpePowerPlain, lam, lamc, nullptr, st);
+    if (rc) return rc;
+  }
+  if (mode == kWpeGradInverseAll) {
+    LaunchScope ls("wpe_power_inverse_backward_kernel", st);
+    wpe_power_inverse_backward_kernel<<<1, 1024, 0, st>>>(lamc, gin, lam, bins * s.T);
+    PBB_CUDA(cudaGetLastError());
+    gin = lam;
+    mode = kWpeGradPlain;
+  }
+  const size_t smem = wpe_power_backward_smem_bytes(s.D, s.taps, G != nullptr);
+  PBB_CUDA(cudaFuncSetAttribute(wpe_power_backward_kernel<TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)smem));
+  LaunchScope ls("wpe_power_backward_kernel", st);
+  wpe_power_backward_kernel<TIn><<<(unsigned)bins, 256, smem, st>>>(y, ys, s, G, lamc, gin, mode, pbar, xbar);
+  PBB_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -176,6 +310,14 @@ int pbb_wpe(const void* y, int dtype, long long bins, int D, long long T, long l
             void* out, long long osb, long long osd, long long ost, int taps, int delay, int iterations,
             long long psd_context, int valid, long long group, void* workspace, size_t workspace_bytes, int* status,
             void* stream) {
+  return pbb_wpe_forward(y, dtype, bins, D, T, ysb, ysd, yst, out, osb, osd, ost, taps, delay, iterations,
+                         psd_context, valid, group, workspace, workspace_bytes, status, nullptr, nullptr, stream);
+}
+
+int pbb_wpe_forward(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                    long long yst, void* out, long long osb, long long osd, long long ost, int taps, int delay,
+                    int iterations, long long psd_context, int valid, long long group, void* workspace,
+                    size_t workspace_bytes, int* status, void* G_save, double* w_save, void* stream) {
   PBB_CHECK_ARG(y != nullptr, 1, "y is null");
   PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
   PBB_CHECK_ARG(bins > 0, 3, "bins must be positive");
@@ -190,16 +332,121 @@ int pbb_wpe(const void* y, int dtype, long long bins, int D, long long T, long l
   PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid),
                 19, "workspace too small (pbb_wpe_workspace_bytes)");
   PBB_CHECK_ARG(status != nullptr, 21, "status is null");
+  PBB_CHECK_ARG((G_save == nullptr) == (w_save == nullptr), 22, "G_save and w_save must both be given or both null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const WpeShape s = wpe_shape(D, T, taps, delay, valid, psd_context);
   const WpeStrides ys{ysb, ysd, yst}, os{osb, osd, ost};
   PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
   char* ws = static_cast<char*>(workspace);
+  double2* Gs = static_cast<double2*>(G_save);
   if (dtype == PBB_C64)
     return wpe_run<float2>(static_cast<const float2*>(y), ys, bins, static_cast<float2*>(out), os, s, iterations,
-                           group, ws, status, st);
+                           group, ws, status, st, Gs, w_save);
   return wpe_run<double2>(static_cast<const double2*>(y), ys, bins, static_cast<double2*>(out), os, s, iterations,
-                          group, ws, status, st);
+                          group, ws, status, st, Gs, w_save);
+}
+
+int pbb_wpe_step(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                 long long yst, const double* weight, long long wsb, long long wst, void* out, long long osb,
+                 long long osd, long long ost, int taps, int delay, int valid, long long group, void* workspace,
+                 size_t workspace_bytes, int* status, void* G_out, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0, 3, "bins must be positive");
+  PBB_CHECK_ARG(D >= 1 && D <= PBB_WPE_MAX_D, 4, "D must be in [1, PBB_WPE_MAX_D] (30)");
+  PBB_CHECK_ARG(T >= 1, 5, "T must be positive");
+  PBB_CHECK_ARG(weight != nullptr, 9, "weight is null");
+  PBB_CHECK_ARG(out != nullptr, 12, "out is null");
+  PBB_CHECK_ARG(taps >= 1, 16, "taps must be positive");
+  PBB_CHECK_ARG(delay >= 0, 17, "delay must be >= 0");
+  PBB_CHECK_ARG((long long)taps * D <= kWpeMaxN, 16, "taps * D must be <= PBB_WPE_MAX_N (96)");
+  PBB_CHECK_ARG(group > 0 && group <= PBB_WPE_MAX_GROUP, 19, "group must be in [1, PBB_WPE_MAX_GROUP]");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid),
+                20, "workspace too small (pbb_wpe_workspace_bytes)");
+  PBB_CHECK_ARG(status != nullptr, 22, "status is null");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const WpeShape s = wpe_shape(D, T, taps, delay, valid, 0);
+  const WpeStrides ys{ysb, ysd, yst}, os{osb, osd, ost};
+  PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
+  char* ws = static_cast<char*>(workspace);
+  double2* Go = static_cast<double2*>(G_out);
+  if (dtype == PBB_C64)
+    return wpe_step_run<float2>(static_cast<const float2*>(y), ys, bins, weight, wsb, wst, static_cast<float2*>(out),
+                                os, s, group, ws, status, Go, st);
+  return wpe_step_run<double2>(static_cast<const double2*>(y), ys, bins, weight, wsb, wst, static_cast<double2*>(out),
+                               os, s, group, ws, status, Go, st);
+}
+
+size_t pbb_wpe_backward_workspace_bytes(long long group, int D, long long T, int taps, int delay, int valid) {
+  if (group <= 0 || group > PBB_WPE_MAX_GROUP || !wpe_valid_shape(D, T, taps, delay)) return 0;
+  return wpe_back_layout(group, wpe_shape(D, T, taps, delay, valid, 0)).total;
+}
+
+int pbb_wpe_backward(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                     long long yst, const double* weight, const void* G, const void* xbar, int taps, int delay,
+                     int valid, void* ybar, double* wbar, long long group, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0, 3, "bins must be positive");
+  PBB_CHECK_ARG(D >= 1 && D <= PBB_WPE_MAX_D, 4, "D must be in [1, PBB_WPE_MAX_D] (30)");
+  PBB_CHECK_ARG(T >= 1, 5, "T must be positive");
+  PBB_CHECK_ARG(weight != nullptr, 9, "weight is null");
+  PBB_CHECK_ARG(G != nullptr, 10, "G is null");
+  PBB_CHECK_ARG(xbar != nullptr, 11, "xbar is null");
+  PBB_CHECK_ARG(taps >= 1, 12, "taps must be positive");
+  PBB_CHECK_ARG(delay >= 0, 13, "delay must be >= 0");
+  PBB_CHECK_ARG((long long)taps * D <= kWpeMaxN, 12, "taps * D must be <= PBB_WPE_MAX_N (96)");
+  PBB_CHECK_ARG(ybar != nullptr, 15, "ybar is null");
+  PBB_CHECK_ARG(wbar != nullptr, 16, "wbar is null");
+  PBB_CHECK_ARG(group > 0 && group <= PBB_WPE_MAX_GROUP, 17, "group must be in [1, PBB_WPE_MAX_GROUP]");
+  PBB_CHECK_ARG(workspace != nullptr &&
+                    workspace_bytes >= pbb_wpe_backward_workspace_bytes(group, D, T, taps, delay, valid),
+                18, "workspace too small (pbb_wpe_backward_workspace_bytes)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const WpeShape s = wpe_shape(D, T, taps, delay, valid, 0);
+  const WpeStrides ys{ysb, ysd, yst};
+  char* ws = static_cast<char*>(workspace);
+  const double2* g = static_cast<const double2*>(G);
+  const double2* xb = static_cast<const double2*>(xbar);
+  double2* yb = static_cast<double2*>(ybar);
+  if (dtype == PBB_C64)
+    return wpe_backward_run<float2>(static_cast<const float2*>(y), ys, bins, s, weight, g, xb, yb, wbar, group, ws,
+                                    st);
+  return wpe_backward_run<double2>(static_cast<const double2*>(y), ys, bins, s, weight, g, xb, yb, wbar, group, ws,
+                                   st);
+}
+
+size_t pbb_wpe_power_backward_workspace_bytes(long long bins, long long T) {
+  if (bins <= 0 || T <= 0) return 0;
+  return 3 * (size_t)bins * T * sizeof(double);
+}
+
+int pbb_wpe_power_backward(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
+                           long long yst, const void* G, int taps, int delay, long long psd_context, int mode,
+                           const double* gin, void* xbar, void* workspace, size_t workspace_bytes, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  PBB_CHECK_ARG(dtype == PBB_C64 || dtype == PBB_C128, 2, "dtype must be PBB_C64 or PBB_C128");
+  PBB_CHECK_ARG(bins > 0 && bins <= 0x7fffffffLL, 3, "bins must be in [1, 2^31 - 1]");
+  PBB_CHECK_ARG(D >= 1 && D <= PBB_WPE_MAX_D, 4, "D must be in [1, PBB_WPE_MAX_D] (30)");
+  PBB_CHECK_ARG(T >= 1, 5, "T must be positive");
+  PBB_CHECK_ARG(taps >= 1, 10, "taps must be positive");
+  PBB_CHECK_ARG(delay >= 0, 11, "delay must be >= 0");
+  PBB_CHECK_ARG(G == nullptr || (long long)taps * D <= kWpeMaxN, 10, "taps * D must be <= PBB_WPE_MAX_N (96)");
+  PBB_CHECK_ARG(mode >= PBB_WPE_GRAD_INVERSE && mode <= PBB_WPE_GRAD_INVERSE_ALL, 13, "mode must be a PBB_WPE_GRAD_*");
+  PBB_CHECK_ARG(gin != nullptr, 14, "gin is null");
+  PBB_CHECK_ARG(xbar != nullptr, 15, "xbar is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= pbb_wpe_power_backward_workspace_bytes(bins, T), 16,
+                "workspace too small (pbb_wpe_power_backward_workspace_bytes)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const WpeShape s = wpe_shape(D, T, G == nullptr ? 1 : taps, G == nullptr ? 0 : delay, 0, psd_context);
+  const WpeStrides ys{ysb, ysd, yst};
+  const double2* g = static_cast<const double2*>(G);
+  double2* xb = static_cast<double2*>(xbar);
+  double* ws = static_cast<double*>(workspace);
+  if (dtype == PBB_C64)
+    return wpe_power_backward_run<float2>(static_cast<const float2*>(y), ys, bins, s, g, mode, gin, xb, ws, st);
+  return wpe_power_backward_run<double2>(static_cast<const double2*>(y), ys, bins, s, g, mode, gin, xb, ws, st);
 }
 
 size_t pbb_wpe_power_workspace_bytes(long long bins, long long T) {

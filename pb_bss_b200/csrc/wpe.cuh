@@ -20,6 +20,9 @@
 //      psd_context mean and the per-bin max, giving w_t = 1 / max(lambda_t, 1e-10 max lambda).  X itself is only
 //      stored by the last iteration (in the output's dtype and strides); the statistics of the next iteration need
 //      Y and w only.  The first w comes from the same kernel with G = 0 (X = Y exactly).
+//   4. the backward passes of a step (pbb_wpe_backward: R again by wpe_corr_kernel, wpe_gbar_kernel,
+//      wpe_solve_rhs_kernel, wpe_step_backward_kernel) and of the power chain (wpe_power_backward_kernel,
+//      wpe_power_inverse_backward_kernel); the closed forms are in include/pbb.h.
 // Every sum runs in a fixed order and there are no float atomics: repeated calls are bitwise identical.  Status
 // bits (PBB_WPE_NONFINITE, PBB_WPE_LSTSQ) are set on the device and read by the caller after the last iteration.
 #pragma once
@@ -203,38 +206,12 @@ __device__ __forceinline__ double wpe_block_max(double v, double* red) {
   return v;
 }
 
-// one CTA (256 threads) per bin.  G (bins, n, D) complex; lstsq (bins) = 1 where the pivot was exactly zero.
-__global__ void __launch_bounds__(256) wpe_solve_kernel(const double* __restrict__ part, WpeShape s,
-                                                        double2* __restrict__ G, int* __restrict__ lstsq,
-                                                        int* __restrict__ status) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int n = s.n, D = s.D, tid = threadIdx.x, nt = blockDim.x;
-  double2* A = reinterpret_cast<double2*>(smem_raw);
-  double2* X = A + n * n;
-  double2* f = X + n * D;
-  double* red = reinterpret_cast<double*>(f + n);
-  __shared__ int piv_s, state_s;   // state: 0 running, 1 singular (zero pivot), 2 non-finite
-  const long long bin = blockIdx.x;
-  const double* pb = part + bin * s.parts * (long long)s.ntiles * 64;
-  double amax = 0.0;
-  bool bad = false;
-  for (int i = tid; i < n * (n + D); i += nt) {
-    const int row = i / (n + D), col = i - row * (n + D);
-    const double2 v = wpe_complex(pb, s, row, col);
-    if (col < n) {
-      A[row * n + col] = v;
-      amax = cabs_max(amax, v);
-      bad |= !isfinite(v.x) || !isfinite(v.y);
-    } else {
-      X[row * D + col - n] = v;
-    }
-  }
-  bad = __syncthreads_or(bad);
-  amax = wpe_block_max(amax, red);
-  // solve with 2^-escale R (exact), as solve_kernel does: G = 2^-escale times that solution
-  const int escale = !(amax > 0.0) || !isfinite(amax) ? 0 : ilogb(amax) & ~1;
-  for (int i = tid; i < n * n; i += nt) A[i] = cscalbn(A[i], -escale);
-  int state = bad ? 2 : 0;   // every thread's copy of state_s, read only after a barrier
+// LU with partial pivoting of A (n x n, shared) applied to the right-hand sides X (n x D, shared); f: n scratch.
+// state on entry: 0, or non-zero to skip the elimination.  Returns 1 on an exactly zero pivot (A, X then partly
+// eliminated), else the entry state.  Every thread of the CTA calls it.
+__device__ __forceinline__ int wpe_lu_eliminate(double2* A, double2* X, double2* f, int n, int D, int state,
+                                                int& piv_s, int& state_s) {
+  const int tid = threadIdx.x, nt = blockDim.x;
   for (int j = 0; j < n && state == 0; ++j) {
     if (tid < 32) {
       double best = -1.0;
@@ -288,16 +265,12 @@ __global__ void __launch_bounds__(256) wpe_solve_kernel(const double* __restrict
     }
     __syncthreads();
   }
-  double2* g = G + bin * (long long)n * D;
-  if (tid == 0) {
-    lstsq[bin] = state == 1;
-    if (state) atomicOr(status, state == 1 ? PBB_WPE_LSTSQ : PBB_WPE_NONFINITE);
-  }
-  if (state == 2) {
-    for (int i = tid; i < n * D; i += nt) g[i] = make_double2(CUDART_NAN, CUDART_NAN);
-    return;
-  }
-  if (state == 1) return;   // wpe_lstsq_kernel writes this bin's G
+  return state;
+}
+
+// back substitution of the eliminated system: X <- U^-1 X
+__device__ __forceinline__ void wpe_lu_back(const double2* A, double2* X, int n, int D) {
+  const int tid = threadIdx.x, nt = blockDim.x;
   for (int i = n - 1; i >= 0; --i) {
     if (tid < D) X[i * D + tid] = cdiv(X[i * D + tid], A[i * n + i]);
     __syncthreads();
@@ -308,7 +281,90 @@ __global__ void __launch_bounds__(256) wpe_solve_kernel(const double* __restrict
     }
     __syncthreads();
   }
+}
+
+// one CTA (256 threads) per bin.  G (bins, n, D) complex; lstsq (bins) = 1 where the pivot was exactly zero.
+__global__ void __launch_bounds__(256) wpe_solve_kernel(const double* __restrict__ part, WpeShape s,
+                                                        double2* __restrict__ G, int* __restrict__ lstsq,
+                                                        int* __restrict__ status) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int n = s.n, D = s.D, tid = threadIdx.x, nt = blockDim.x;
+  double2* A = reinterpret_cast<double2*>(smem_raw);
+  double2* X = A + n * n;
+  double2* f = X + n * D;
+  double* red = reinterpret_cast<double*>(f + n);
+  __shared__ int piv_s, state_s;   // state: 0 running, 1 singular (zero pivot), 2 non-finite
+  const long long bin = blockIdx.x;
+  const double* pb = part + bin * s.parts * (long long)s.ntiles * 64;
+  double amax = 0.0;
+  bool bad = false;
+  for (int i = tid; i < n * (n + D); i += nt) {
+    const int row = i / (n + D), col = i - row * (n + D);
+    const double2 v = wpe_complex(pb, s, row, col);
+    if (col < n) {
+      A[row * n + col] = v;
+      amax = cabs_max(amax, v);
+      bad |= !isfinite(v.x) || !isfinite(v.y);
+    } else {
+      X[row * D + col - n] = v;
+    }
+  }
+  bad = __syncthreads_or(bad);
+  amax = wpe_block_max(amax, red);
+  // solve with 2^-escale R (exact), as solve_kernel does: G = 2^-escale times that solution
+  const int escale = !(amax > 0.0) || !isfinite(amax) ? 0 : ilogb(amax) & ~1;
+  for (int i = tid; i < n * n; i += nt) A[i] = cscalbn(A[i], -escale);
+  int state = wpe_lu_eliminate(A, X, f, n, D, bad ? 2 : 0, piv_s, state_s);
+  double2* g = G + bin * (long long)n * D;
+  if (tid == 0) {
+    lstsq[bin] = state == 1;
+    if (state) atomicOr(status, state == 1 ? PBB_WPE_LSTSQ : PBB_WPE_NONFINITE);
+  }
+  if (state == 2) {
+    for (int i = tid; i < n * D; i += nt) g[i] = make_double2(CUDART_NAN, CUDART_NAN);
+    return;
+  }
+  if (state == 1) return;   // wpe_lstsq_kernel writes this bin's G
+  wpe_lu_back(A, X, n, D);
   for (int i = tid; i < n * D; i += nt) g[i] = cscalbn(X[i], -escale);
+}
+
+// The backward's solve: B <- R^-1 B in place (B (bins, n, D)), R assembled from the partial tiles exactly as
+// wpe_solve_kernel does (the same scaling and pivots).  A zero pivot or a non-finite R gives NaN in that bin: the
+// backward has no lstsq branch (the strict = 2 rule of solve_kernel).  One CTA (256 threads) per bin.
+__global__ void __launch_bounds__(256) wpe_solve_rhs_kernel(const double* __restrict__ part, WpeShape s,
+                                                            double2* __restrict__ B) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int n = s.n, D = s.D, tid = threadIdx.x, nt = blockDim.x;
+  double2* A = reinterpret_cast<double2*>(smem_raw);
+  double2* X = A + n * n;
+  double2* f = X + n * D;
+  double* red = reinterpret_cast<double*>(f + n);
+  __shared__ int piv_s, state_s;
+  const long long bin = blockIdx.x;
+  const double* pb = part + bin * s.parts * (long long)s.ntiles * 64;
+  double2* b = B + bin * (long long)n * D;
+  double amax = 0.0;
+  bool bad = false;
+  for (int i = tid; i < n * n; i += nt) {
+    const int row = i / n, col = i - row * n;
+    const double2 v = wpe_complex(pb, s, row, col);
+    A[i] = v;
+    amax = cabs_max(amax, v);
+    bad |= !isfinite(v.x) || !isfinite(v.y);
+  }
+  for (int i = tid; i < n * D; i += nt) X[i] = b[i];
+  bad = __syncthreads_or(bad);
+  amax = wpe_block_max(amax, red);
+  const int escale = !(amax > 0.0) || !isfinite(amax) ? 0 : ilogb(amax) & ~1;
+  for (int i = tid; i < n * n; i += nt) A[i] = cscalbn(A[i], -escale);
+  const int state = wpe_lu_eliminate(A, X, f, n, D, bad ? 2 : 0, piv_s, state_s);
+  if (state) {
+    for (int i = tid; i < n * D; i += nt) b[i] = make_double2(CUDART_NAN, CUDART_NAN);
+    return;
+  }
+  wpe_lu_back(A, X, n, D);
+  for (int i = tid; i < n * D; i += nt) b[i] = cscalbn(X[i], -escale);
 }
 
 __host__ __device__ inline size_t wpe_lstsq_smem_bytes(int n, int D) {
@@ -493,6 +549,314 @@ __global__ void __launch_bounds__(1024) wpe_power_inverse_kernel(double* __restr
   mx = wpe_block_max(mx, red);
   const double eps = 1e-10 * mx;
   for (long long i = threadIdx.x; i < count; i += blockDim.x) p[i] = 1.0 / fmax(p[i], eps);
+}
+
+// ---- 4. backward passes (pbb_wpe_backward, pbb_wpe_power_backward; the closed forms are in include/pbb.h) -------
+constexpr int kWpeBackChunk = 64;            // frames per chunk of the backward's per-bin kernels
+
+// caller weights (element (b, t) at b wsb + t wst) -> w (bins, T) contiguous
+__global__ void wpe_weight_copy_kernel(const double* __restrict__ src, long long wsb, long long wst, long long bins,
+                                       long long T, double* __restrict__ w) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < bins * T;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i / T, t = i - b * T;
+    w[i] = src[b * wsb + t * wst];
+  }
+}
+
+__host__ __device__ inline size_t wpe_gbar_smem_bytes(int D, int taps) {
+  return ((size_t)D * taps * D + (size_t)D * (kWpeBackChunk + taps - 1) + (size_t)D * kWpeBackChunk) *
+         sizeof(double2);
+}
+
+// Gbar = -sum_t Yt_t xbar_t^H over every frame: Gbar[k D + e][d] = -sum_t Y_{e, t - delay - k} conj(xbar_{d, t}).
+// One CTA (256 threads) per bin; each entry is owned by one thread and summed in frame order (the running sums stay
+// in shared memory between chunks).  xbar (bins, D, T) contiguous; Gbar (bins, n, D).
+template <class TIn>
+__global__ void __launch_bounds__(256) wpe_gbar_kernel(const TIn* __restrict__ y, WpeStrides ys, WpeShape s,
+                                                       const double2* __restrict__ xbar, double2* __restrict__ Gbar) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int D = s.D, taps = s.taps, n = s.n, tid = threadIdx.x, nt = blockDim.x;
+  const int lw = kWpeBackChunk + taps - 1;
+  const long long T = s.T, bin = blockIdx.x;
+  double2* acc = reinterpret_cast<double2*>(smem_raw);
+  double2* Yd = acc + n * D;                // delayed window (D, lw)
+  double2* Xb = Yd + D * lw;                // xbar chunk (D, chunk)
+  const TIn* yb = y + bin * ys.b;
+  const double2* xb = xbar + bin * D * T;
+  for (int i = tid; i < n * D; i += nt) acc[i] = make_double2(0.0, 0.0);
+  for (long long t0 = 0; t0 < T; t0 += kWpeBackChunk) {
+    const long long ws = t0 - s.delay - taps + 1;
+    __syncthreads();
+    for (int i = tid; i < D * lw; i += nt) {
+      const int d = i / lw, j = i - d * lw;
+      const long long f = ws + j;
+      Yd[i] = f >= 0 && f < T ? wpe_load(yb, d * ys.d + f * ys.t) : make_double2(0.0, 0.0);
+    }
+    for (int i = tid; i < D * kWpeBackChunk; i += nt) {
+      const int d = i / kWpeBackChunk, j = i - d * kWpeBackChunk;
+      Xb[i] = t0 + j < T ? xb[d * T + t0 + j] : make_double2(0.0, 0.0);
+    }
+    __syncthreads();
+    for (int i = tid; i < n * D; i += nt) {
+      const int row = i / D, d = i - row * D, k = row / D, e = row - k * D;
+      const double2* yr = Yd + e * lw + taps - 1 - k;
+      const double2* xr = Xb + d * kWpeBackChunk;
+      double2 a = acc[i];
+      for (int j = 0; j < kWpeBackChunk; ++j) {
+        const double2 qv = cmulc(yr[j], xr[j]);   // Y conj(xbar)
+        a.x += qv.x; a.y += qv.y;
+      }
+      acc[i] = a;
+    }
+  }
+  __syncthreads();
+  double2* g = Gbar + bin * (long long)n * D;
+  for (int i = tid; i < n * D; i += nt) g[i] = make_double2(-acc[i].x, -acc[i].y);
+}
+
+__host__ __device__ inline size_t wpe_step_backward_smem_bytes(int D, int taps) {
+  const int lw = kWpeBackChunk + taps - 1;
+  return (2 * (size_t)D * taps * D + 3 * (size_t)D * lw) * sizeof(double2) + (size_t)D * kWpeBackChunk * sizeof(double);
+}
+
+// One stage of the step backward for one bin per CTA (256 threads), given G, Pbar = R^-1 Gbar and w, per frame:
+//   x_t = y_t - G^H yt_t, c_t = Pbar^H yt_t, m_t = [t in S], u_t = xbar_t + m_t w_t c_t, b_t = m_t w_t x_t,
+//   wbar_t = m_t Re(c_t^H x_t), ybar_t += u_t + sum_k (-G_k u_{t + delay + k} + Pbar_k b_{t + delay + k})
+// with G_k, Pbar_k the D x D blocks of rows k D .. k D + D - 1.  The last term is the shift-add of
+// Ytbar_t = -G u_t + Pbar b_t back onto Y, written as a gather over later frames: chunks run from the last frame to
+// the first, u and b of every chunk go to ub (bins, 2, D, T) before the chunk gathers from it, and a chunk reads
+// only frames at or after its own.  ybar, xbar (bins, D, T) contiguous; ybar accumulated, wbar (bins, T) written.
+template <class TIn>
+__global__ void __launch_bounds__(256) wpe_step_backward_kernel(const TIn* __restrict__ y, WpeStrides ys, WpeShape s,
+                                                                const double2* __restrict__ G,
+                                                                const double2* __restrict__ Pbar,
+                                                                const double* __restrict__ w,
+                                                                const double2* __restrict__ xbar, double2* ub,
+                                                                double2* __restrict__ ybar,
+                                                                double* __restrict__ wbar) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int D = s.D, taps = s.taps, n = s.n, tid = threadIdx.x, nt = blockDim.x;
+  const int lw = kWpeBackChunk + taps - 1;
+  const long long T = s.T, bin = blockIdx.x;
+  double2* Gs = reinterpret_cast<double2*>(smem_raw);
+  double2* Ps = Gs + n * D;
+  double2* Yd = Ps + n * D;                 // delayed window of y (D, lw), frames from t0 - delay - taps + 1
+  double2* Uf = Yd + D * lw;                // u over frames t0 + delay .. (D, lw)
+  double2* Bf = Uf + D * lw;                // b likewise
+  double* pr = reinterpret_cast<double*>(Bf + D * lw);   // Re(c^H x) terms (D, chunk)
+  const TIn* yb = y + bin * ys.b;
+  const double2* xb = xbar + bin * D * T;
+  const double* wb = w + bin * T;
+  double2* ubu = ub + bin * 2 * D * T;
+  double2* ubb = ubu + D * T;
+  double2* yo = ybar + bin * D * T;
+  for (int i = tid; i < n * D; i += nt) {
+    Gs[i] = G[bin * n * D + i];
+    Ps[i] = Pbar[bin * n * D + i];
+  }
+  const long long nchunks = (T + kWpeBackChunk - 1) / kWpeBackChunk;
+  for (long long ci = nchunks - 1; ci >= 0; --ci) {
+    const long long t0 = ci * kWpeBackChunk, ws = t0 - s.delay - taps + 1;
+    __syncthreads();
+    for (int i = tid; i < D * lw; i += nt) {
+      const int d = i / lw, j = i - d * lw;
+      const long long f = ws + j;
+      Yd[i] = f >= 0 && f < T ? wpe_load(yb, d * ys.d + f * ys.t) : make_double2(0.0, 0.0);
+    }
+    __syncthreads();
+    for (int i = tid; i < D * kWpeBackChunk; i += nt) {
+      const int d = i / kWpeBackChunk, j = i - d * kWpeBackChunk;
+      const long long t = t0 + j;
+      if (t >= T) {
+        pr[i] = 0.0;
+        continue;
+      }
+      double2 x = wpe_load(yb, d * ys.d + t * ys.t), c = make_double2(0.0, 0.0);
+      for (int k = 0; k < taps; ++k)
+        for (int e = 0; e < D; ++e) {
+          const double2 yv = Yd[e * lw + j + taps - 1 - k];
+          const double2 qg = cmulc(yv, Gs[(k * D + e) * D + d]), qp = cmulc(yv, Ps[(k * D + e) * D + d]);
+          x.x -= qg.x; x.y -= qg.y;
+          c.x += qp.x; c.y += qp.y;
+        }
+      const double mw = t >= s.tb ? wb[t] : 0.0;
+      const double2 xv = xb[d * T + t];
+      ubu[d * T + t] = make_double2(xv.x + mw * c.x, xv.y + mw * c.y);
+      ubb[d * T + t] = make_double2(mw * x.x, mw * x.y);
+      pr[i] = t >= s.tb ? c.x * x.x + c.y * x.y : 0.0;
+    }
+    __syncthreads();
+    for (int j = tid; j < kWpeBackChunk; j += nt) {
+      if (t0 + j >= T) continue;
+      double v = 0.0;
+      for (int d = 0; d < D; ++d) v += pr[d * kWpeBackChunk + j];
+      wbar[bin * T + t0 + j] = v;
+    }
+    // u and b over the frames t0 + delay + j (j < lw) that exist; later chunks wrote theirs in earlier iterations
+    for (int i = tid; i < D * lw; i += nt) {
+      const int d = i / lw, j = i - d * lw;
+      const long long f = t0 + s.delay + j;
+      const bool in = f < T;
+      Uf[i] = in ? ubu[d * T + f] : make_double2(0.0, 0.0);
+      Bf[i] = in ? ubb[d * T + f] : make_double2(0.0, 0.0);
+    }
+    __syncthreads();
+    for (int i = tid; i < D * kWpeBackChunk; i += nt) {
+      const int d = i / kWpeBackChunk, j = i - d * kWpeBackChunk;
+      const long long t = t0 + j;
+      if (t >= T) continue;
+      double2 a = ubu[d * T + t];
+      for (int k = 0; k < taps; ++k)
+        for (int e = 0; e < D; ++e) {
+          const double2 qg = cmul(Gs[(k * D + d) * D + e], Uf[e * lw + j + k]);
+          const double2 qp = cmul(Ps[(k * D + d) * D + e], Bf[e * lw + j + k]);
+          a.x += qp.x - qg.x; a.y += qp.y - qg.y;
+        }
+      const double2 o = yo[d * T + t];
+      yo[d * T + t] = make_double2(o.x + a.x, o.y + a.y);
+    }
+  }
+}
+
+enum { kWpeGradInverse = PBB_WPE_GRAD_INVERSE, kWpeGradPlain = PBB_WPE_GRAD_PLAIN, kWpeGradInverseAll = PBB_WPE_GRAD_INVERSE_ALL };
+
+// the backward of w = 1 / max(p, 1e-10 M), M = max p (fmax from 0, as the forward), over p[0, count): the gradient of
+// p given wbar, torch.maximum's and amax's rule (ties split evenly).  Every thread of the CTA calls it; red holds
+// blockDim.x doubles.  Sums run per thread in index order, then over the threads in order.
+__device__ __forceinline__ void wpe_inverse_backward(const double* p, const double* wbar, double* pbar, long long count,
+                                                     double* red) {
+  const int tid = threadIdx.x, nt = blockDim.x;
+  double mx = 0.0;
+  for (long long t = tid; t < count; t += nt) mx = fmax(mx, p[t]);
+  mx = wpe_block_max(mx, red);
+  const double eps = 1e-10 * mx;
+  double gb = 0.0, ties = 0.0;
+  for (long long t = tid; t < count; t += nt) {
+    const double v = p[t], z = fmax(v, eps);
+    const double zb = -wbar[t] / (z * z);
+    pbar[t] = v > eps ? zb : v == eps ? 0.5 * zb : 0.0;
+    gb += v < eps ? zb : v == eps ? 0.5 * zb : 0.0;
+    ties += v == mx;
+  }
+  __syncthreads();
+  red[tid] = gb;
+  red[nt + tid] = ties;
+  __syncthreads();
+  gb = 0.0;
+  ties = 0.0;
+  for (int i = 0; i < nt; ++i) {
+    gb += red[i];
+    ties += red[nt + i];
+  }
+  const double share = 1e-10 * gb / ties;
+  for (long long t = tid; t < count; t += nt)
+    if (p[t] == mx) pbar[t] += share;
+  __syncthreads();
+}
+
+// get_power_inverse's max over the whole array: pbar from lamc and wbar over all `count` values (one CTA)
+__global__ void __launch_bounds__(1024) wpe_power_inverse_backward_kernel(const double* __restrict__ lamc,
+                                                                          const double* __restrict__ wbar,
+                                                                          double* __restrict__ pbar, long long count) {
+  __shared__ double red[2048];
+  wpe_inverse_backward(lamc, wbar, pbar, count, red);
+}
+
+__host__ __device__ inline size_t wpe_power_backward_smem_bytes(int D, int taps, bool filter) {
+  return filter ? ((size_t)taps * D * D + (size_t)D * (kWpeFilterChunk + taps - 1)) * sizeof(double2) +
+                      512 * sizeof(double)
+                : 512 * sizeof(double);
+}
+
+// The power chain's backward for one bin per CTA (256 threads): x = y - G^H Yt (G null: x = y), lamc (bins, T) the
+// forward's lambda_c.  mode kWpeGradInverse: gin is wbar of w = 1 / max(lambda_c, 1e-10 max_t lambda_c);
+// kWpeGradPlain: gin is lambda_c's gradient.  lambda_c's gradient goes through the adjoint of the psd_context mean,
+// lambdabar_t = sum_{s : |s - t| <= c} lambdabar_c,s / n_s (n_s the frames in s's window), and
+// xbar_dt += (2 / D) lambdabar_t x_dt (xbar (bins, D, T) contiguous, accumulated).  lamc and pbar are overwritten.
+template <class TIn>
+__global__ void __launch_bounds__(256) wpe_power_backward_kernel(const TIn* __restrict__ y, WpeStrides ys, WpeShape s,
+                                                                 const double2* __restrict__ G, double* lamc,
+                                                                 const double* __restrict__ gin, int mode,
+                                                                 double* pbar, double2* __restrict__ xbar) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int D = s.D, taps = s.taps, n = s.n, tid = threadIdx.x, nt = blockDim.x;
+  const int lw = kWpeFilterChunk + taps - 1;
+  const long long T = s.T, bin = blockIdx.x;
+  double* red = reinterpret_cast<double*>(smem_raw);
+  double2* Gs = reinterpret_cast<double2*>(red + 512);
+  double2* Yd = Gs + n * D;
+  double* lc = lamc + bin * T;
+  double* pb = pbar + bin * T;
+  const double* gb = gin + bin * T;
+  if (mode == kWpeGradInverse) {
+    wpe_inverse_backward(lc, gb, pb, T, red);
+  } else {
+    for (long long t = tid; t < T; t += nt) pb[t] = gb[t];
+    __syncthreads();
+  }
+  // lambdabar into lc
+  const long long c = s.psd_context;
+  if (c < 0) {
+    double v = 0.0;
+    for (long long t = tid; t < T; t += nt) v += pb[t];
+    __syncthreads();
+    red[tid] = v;
+    __syncthreads();
+    v = 0.0;
+    for (int i = 0; i < nt; ++i) v += red[i];
+    const double m = v / T;
+    for (long long t = tid; t < T; t += nt) lc[t] = m;
+  } else if (c == 0) {
+    for (long long t = tid; t < T; t += nt) lc[t] = pb[t];
+  } else {
+    for (long long t = tid; t < T; t += nt) {
+      const long long lo = t - c < 0 ? 0 : t - c, hi = t + c >= T ? T - 1 : t + c;
+      pb[t] /= (double)(hi - lo + 1);
+    }
+    __syncthreads();
+    for (long long t = tid; t < T; t += nt) {
+      const long long lo = t - c < 0 ? 0 : t - c, hi = t + c >= T ? T - 1 : t + c;
+      double v = 0.0;
+      for (long long u = lo; u <= hi; ++u) v += pb[u];
+      lc[t] = v;
+    }
+  }
+  const TIn* yb = y + bin * ys.b;
+  double2* xo = xbar + bin * D * T;
+  const double scale = 2.0 / D;
+  if (G != nullptr)
+    for (int i = tid; i < n * D; i += nt) Gs[i] = G[bin * n * D + i];
+  for (long long t0 = 0; t0 < T; t0 += kWpeFilterChunk) {
+    const long long ws = t0 - s.delay - taps + 1;
+    __syncthreads();
+    if (G != nullptr)
+      for (int i = tid; i < D * lw; i += nt) {
+        const int d = i / lw, j = i - d * lw;
+        const long long f = ws + j;
+        Yd[i] = f >= 0 && f < T ? wpe_load(yb, d * ys.d + f * ys.t) : make_double2(0.0, 0.0);
+      }
+    __syncthreads();
+    for (int i = tid; i < D * kWpeFilterChunk; i += nt) {
+      const int d = i / kWpeFilterChunk, j = i - d * kWpeFilterChunk;
+      const long long t = t0 + j;
+      if (t >= T) continue;
+      double2 x = wpe_load(yb, d * ys.d + t * ys.t);
+      if (G != nullptr) {
+        double2 acc = make_double2(0.0, 0.0);
+        for (int k = 0; k < taps; ++k)
+          for (int e = 0; e < D; ++e) {
+            const double2 qv = cmulc(Yd[e * lw + j + taps - 1 - k], Gs[(k * D + e) * D + d]);
+            acc.x += qv.x; acc.y += qv.y;
+          }
+        x.x -= acc.x;
+        x.y -= acc.y;
+      }
+      const double f = scale * lc[t];
+      const double2 o = xo[d * T + t];
+      xo[d * T + t] = make_double2(o.x + f * x.x, o.y + f * x.y);
+    }
+  }
 }
 
 // build_y_tilde: out (bins, taps D, T) contiguous, row k D + d at frame t = Y_{d, t - delay - k} (0 before frame 0)

@@ -13,6 +13,17 @@ so repeated calls are bitwise identical.
 NumPy in gives NumPy out; a CUDA tensor in gives a CUDA tensor out (in the input's strides where they are dense).
 Any strides are accepted: a view whose leading dims do not collapse to one stride is copied once on the device.
 
+``wpe_step`` is one WPE iteration with the caller's inverse power (nara_wpe's TensorFlow ``wpe_step`` and ESPnet's
+``wpe_one_iteration`` compute the same; the contract is restated in ``oracle/wpe_autograd_oracle.py``), the building
+block of DNN-WPE, where a network estimates the power.  ``wpe`` (through every iteration and its weights),
+``wpe_step`` (Y and the inverse power), ``get_power`` and ``get_power_inverse`` are differentiable for CUDA tensors
+that require grad: the forward runs the same kernels, so outputs are bitwise those of a call without grad, and the
+backward passes are the fp64 device kernels of pbb_wpe_backward and pbb_wpe_power_backward (closed forms in
+include/pbb.h; fixed-order sums, no atomics, no host synchronisation).  Gradients come back in the input's dtype,
+repeated backward calls are bitwise identical and double backward raises.  A bin whose R has an exactly zero pivot
+(the forward took lstsq) or holds a non-finite value gets NaN gradients in that bin only.  NumPy input and the online
+functions return results without a graph.
+
 Documented differences from nara_wpe:
   - real input raises TypeError (nara_wpe would compute in the real domain);
   - taps * D > 96 or D > 30 raises NotImplementedError (wpe, get_power, get_power_inverse);
@@ -32,6 +43,7 @@ import math
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _device, _lib
 
@@ -41,8 +53,10 @@ MAX_GROUP = 65535               # PBB_WPE_MAX_GROUP
 WORKSPACE_BYTES = 1 << 30       # bins run in groups whose workspace stays under this (one bin at least)
 NONFINITE, LSTSQ = 1, 2         # PBB_WPE_NONFINITE, PBB_WPE_LSTSQ
 
-__all__ = ['wpe', 'get_power', 'get_power_inverse', 'build_y_tilde', 'online_wpe_step', 'get_power_online',
-           'online_wpe', 'OnlineWPEState']
+GRAD_INVERSE, GRAD_PLAIN, GRAD_INVERSE_ALL = 0, 1, 2   # PBB_WPE_GRAD_*
+
+__all__ = ['wpe', 'wpe_step', 'get_power', 'get_power_inverse', 'build_y_tilde', 'online_wpe_step',
+           'get_power_online', 'online_wpe', 'OnlineWPEState']
 
 
 def _is_complex(x):
@@ -116,8 +130,7 @@ def _run(Y, taps, delay, iterations, psd_context, statistics_mode, inplace):
             out.copy_(y)
         return (Y if inplace else out), 0
     valid = int(statistics_mode == 'valid')
-    per_bin = lib.pbb_wpe_workspace_bytes(1, D, T, taps, delay, valid)
-    group = int(max(1, min(bins, MAX_GROUP, WORKSPACE_BYTES // per_bin)))
+    group = _group(lib.pbb_wpe_workspace_bytes(1, D, T, taps, delay, valid), bins)
     nbytes = lib.pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
     status = torch.zeros(1, dtype=torch.int32, device=y.device)
@@ -145,14 +158,112 @@ def _check_args(Y, taps, delay, iterations, psd_context, statistics_mode):
                                   f'D = {Y.shape[-2]}')
 
 
+def _needs_graph(*ts):
+    return torch.is_grad_enabled() and any(_device.is_tensor(t) and t.requires_grad for t in ts)
+
+
+def _group(per_bin, bins):
+    return int(max(1, min(bins, MAX_GROUP, WORKSPACE_BYTES // per_bin)))
+
+
+def _backward_workspace(bins, D, T, taps, delay, valid):
+    """(group, workspace) of pbb_wpe_backward"""
+    lib = _lib.load()
+    group = _group(lib.pbb_wpe_backward_workspace_bytes(1, D, T, taps, delay, valid), bins)
+    nbytes = lib.pbb_wpe_backward_workspace_bytes(group, D, T, taps, delay, valid)
+    return group, torch.empty(nbytes, dtype=torch.uint8, device=_device.device())
+
+
+def _power_backward(y, ys, G, taps, delay, c, mode, gin, xbar):
+    """pbb_wpe_power_backward: xbar (bins, D, T) complex128 += the power chain's gradient of y (G: x = y - G^H Yt)"""
+    bins, D, T = xbar.shape
+    lib = _lib.load()
+    nbytes = lib.pbb_wpe_power_backward_workspace_bytes(bins, T)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=xbar.device)
+    _lib.check(lib.pbb_wpe_power_backward(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys,
+                                          _device.ptr(G), taps, delay, c, mode, _device.ptr(gin), _device.ptr(xbar),
+                                          _device.ptr(ws), nbytes, _device.stream_ptr()), 'pbb_wpe_power_backward')
+
+
+def _step_backward(y, ys, w, G, xbar, ybar, taps, delay, valid):
+    """pbb_wpe_backward: ybar += Y's gradient of one step; returns the weights' gradient (bins, T) float64"""
+    bins, D, T = xbar.shape
+    group, ws = _backward_workspace(bins, D, T, taps, delay, valid)
+    wbar = torch.empty((bins, T), dtype=torch.float64, device=xbar.device)
+    _lib.check(_lib.load().pbb_wpe_backward(
+        _device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(w), _device.ptr(G),
+        _device.ptr(xbar), taps, delay, valid, _device.ptr(ybar), _device.ptr(wbar), group, _device.ptr(ws),
+        ws.numel(), _device.stream_ptr()), 'pbb_wpe_backward')
+    return wbar
+
+
+def _grad_in(grad, bins, D, T):
+    return grad.to(torch.complex128).contiguous().reshape(bins, D, T)
+
+
+class _Wpe(torch.autograd.Function):
+    """Y (..., D, T) complex on the device -> X by pbb_wpe_forward, which also keeps every iteration's G_i and w_i;
+    backward: pbb_wpe_backward per stage from the last to the first, each stage's weight gradient through
+    pbb_wpe_power_backward into the previous stage's output (into Y for the first stage)."""
+
+    @staticmethod
+    def forward(ctx, Y, taps, delay, iterations, c, valid):
+        D, T = Y.shape[-2], Y.shape[-1]
+        bins = int(np.prod(Y.shape[:-2], dtype=np.int64))
+        lib = _lib.load()
+        y, ys = _layout(Y)
+        out, os_ = _layout(torch.empty_like(y))
+        group = _group(lib.pbb_wpe_workspace_bytes(1, D, T, taps, delay, valid), bins)
+        nbytes = lib.pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
+        status = torch.zeros(1, dtype=torch.int32, device=y.device)
+        G = torch.empty((iterations, bins, taps * D, D), dtype=torch.complex128, device=y.device)
+        w = torch.empty((iterations, bins, T), dtype=torch.float64, device=y.device)
+        _lib.check(lib.pbb_wpe_forward(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(out),
+                                       *os_, taps, delay, iterations, c, valid, group, _device.ptr(ws), nbytes,
+                                       _device.ptr(status), _device.ptr(G) if iterations else None,
+                                       _device.ptr(w) if iterations else None, _device.stream_ptr()),
+                   'pbb_wpe_forward')
+        ctx.save_for_backward(y, G, w)
+        ctx.args = (ys, taps, delay, iterations, c, valid, Y.shape, Y.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        y, G, w = ctx.saved_tensors
+        ys, taps, delay, iterations, c, valid, shape, dtype = ctx.args
+        D, T = shape[-2], shape[-1]
+        bins = int(np.prod(shape[:-2], dtype=np.int64))
+        xbar = _grad_in(grad, bins, D, T)
+        if iterations == 0:
+            return xbar.reshape(shape).to(dtype), None, None, None, None, None
+        ybar = torch.zeros((bins, D, T), dtype=torch.complex128, device=y.device)
+        for i in range(iterations - 1, -1, -1):
+            wbar = _step_backward(y, ys, w[i], G[i], xbar, ybar, taps, delay, valid)
+            xprev = ybar if i == 0 else torch.zeros_like(ybar)
+            _power_backward(y, ys, G[i - 1] if i else None, taps, delay, c, GRAD_INVERSE, wbar, xprev)
+            xbar = xprev
+        return ybar.reshape(shape).to(dtype), None, None, None, None, None
+
+
 def wpe(Y, taps=10, delay=3, iterations=3, psd_context=0, statistics_mode='full', inplace=False):
     """nara_wpe.wpe.wpe (wpe_v8): the dereverberated (..., D, T) STFT of Y (..., D, T).
 
     taps: filter length in frames, delay: prediction delay, iterations: re-estimations of the power,
     psd_context: frames on each side of the power's moving mean (inf: the mean over all frames),
     statistics_mode: 'full' (every frame) or 'valid' (frames t >= delay + taps - 1) for the correlations,
-    inplace: write X into Y and return Y."""
+    inplace: write X into Y and return Y (raises for a tensor that requires grad).
+    Differentiable with respect to a CUDA tensor Y that requires grad (see the module's docstring)."""
     _check_args(Y, taps, delay, iterations, psd_context, statistics_mode)
+    if _needs_graph(Y):
+        if inplace:
+            raise RuntimeError('wpe(inplace=True) on a tensor that requires grad: an in-place operation would '
+                               'overwrite the input its gradient needs')
+        Yd, _ = _prepare(Y, 'wpe')
+        if Yd.numel() == 0:
+            return Yd.clone()
+        return _Wpe.apply(Yd, taps, delay, iterations, _context(psd_context), int(statistics_mode == 'valid'))
     Yd, like_numpy = _prepare(Y, 'wpe')
     if like_numpy:
         X, _ = _run(Yd, taps, delay, iterations, psd_context, statistics_mode, False)
@@ -168,15 +279,13 @@ def wpe(Y, taps=10, delay=3, iterations=3, psd_context=0, statistics_mode='full'
     return X
 
 
-def _power(signal, psd_context, inverse):
-    x, like_numpy = _prepare(signal, 'get_power_inverse' if inverse else 'get_power')
-    c = _context(psd_context)
+def _power_launch(x, c, inverse):
+    """(out (..., T) float64, x after _layout, its strides) by pbb_wpe_power"""
     D, T = x.shape[-2], x.shape[-1]
-    if D > MAX_D:
-        raise NotImplementedError(f'get_power supports D <= {MAX_D}, got D = {D}')
     lead = tuple(x.shape[:-2])
     bins = int(np.prod(lead, dtype=np.int64))
     out = _device.empty(lead + (T,), torch.float64)
+    xs = None
     if bins and T:
         lib = _lib.load()
         x, xs = _layout(x)
@@ -184,7 +293,110 @@ def _power(signal, psd_context, inverse):
         ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
         _lib.check(lib.pbb_wpe_power(_device.ptr(x), _device.complex_dtype_code(x), bins, D, T, *xs, c, int(inverse),
                                      _device.ptr(out), _device.ptr(ws), nbytes, _device.stream_ptr()), 'pbb_wpe_power')
-    return _device.to_host(out, like_numpy)
+    return out, x, xs
+
+
+class _Power(torch.autograd.Function):
+    """get_power / get_power_inverse of x (..., D, T) on the device by pbb_wpe_power; backward
+    pbb_wpe_power_backward (GRAD_PLAIN / GRAD_INVERSE_ALL)."""
+
+    @staticmethod
+    def forward(ctx, x, c, inverse):
+        out, xl, xs = _power_launch(x, c, inverse)
+        ctx.save_for_backward(xl)
+        ctx.args = (xs, c, inverse, x.shape, x.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        xl, = ctx.saved_tensors
+        xs, c, inverse, shape, dtype = ctx.args
+        D, T = shape[-2], shape[-1]
+        bins = int(np.prod(shape[:-2], dtype=np.int64))
+        xbar = torch.zeros((bins, D, T), dtype=torch.complex128, device=xl.device)
+        if bins and T:
+            g = grad.to(torch.float64).contiguous().reshape(bins, T)
+            _power_backward(xl, xs, None, 1, 0, c, GRAD_INVERSE_ALL if inverse else GRAD_PLAIN, g, xbar)
+        return xbar.reshape(shape).to(dtype), None, None
+
+
+class _WpeStep(torch.autograd.Function):
+    """Y (..., D, T) complex and w (bins, T) float64 on the device -> X by pbb_wpe_step, which also keeps G;
+    backward pbb_wpe_backward."""
+
+    @staticmethod
+    def forward(ctx, Y, w, taps, delay, valid):
+        D, T = Y.shape[-2], Y.shape[-1]
+        bins = w.shape[0]
+        lib = _lib.load()
+        y, ys = _layout(Y)
+        out, os_ = _layout(torch.empty_like(y))
+        group = _group(lib.pbb_wpe_workspace_bytes(1, D, T, taps, delay, valid), bins)
+        nbytes = lib.pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
+        status = torch.zeros(1, dtype=torch.int32, device=y.device)
+        G = torch.empty((bins, taps * D, D), dtype=torch.complex128, device=y.device)
+        _lib.check(lib.pbb_wpe_step(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(w),
+                                    w.stride(0), w.stride(1), _device.ptr(out), *os_, taps, delay, valid, group,
+                                    _device.ptr(ws), nbytes, _device.ptr(status), _device.ptr(G),
+                                    _device.stream_ptr()), 'pbb_wpe_step')
+        ctx.save_for_backward(y, w, G)
+        ctx.args = (ys, taps, delay, valid, Y.shape, Y.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        y, w, G = ctx.saved_tensors
+        ys, taps, delay, valid, shape, dtype = ctx.args
+        D, T = shape[-2], shape[-1]
+        bins = w.shape[0]
+        ybar = torch.zeros((bins, D, T), dtype=torch.complex128, device=y.device)
+        wc = w.contiguous()
+        wbar = _step_backward(y, ys, wc, G, _grad_in(grad, bins, D, T), ybar, taps, delay, valid)
+        return ybar.reshape(shape).to(dtype), wbar, None, None, None
+
+
+def wpe_step(Y, inverse_power, taps=10, delay=3, statistics_mode='full'):
+    """One WPE iteration with the caller's weights: X (..., D, T) for Y (..., D, T) complex and inverse_power
+    (..., T) real (float32 or float64, exactly Y's leading shape):
+        R = sum_S w_t Yt_t Yt_t^H, P = sum_S w_t Yt_t Y_t^H, G = stable_solve(R, P), X = Y - G^H Yt
+    with Yt = build_y_tilde(Y, taps, delay) and S as in ``wpe`` (the same limits and errors).  This is the step of
+    DNN-WPE, where a network estimates the power; differentiable with respect to Y and inverse_power for CUDA
+    tensors that require grad."""
+    _check_args(Y, taps, delay, 1, 0, statistics_mode)
+    if len(Y.shape) < 2:
+        raise ValueError(f'wpe_step needs shape (..., D, T), got {tuple(Y.shape)}')
+    want = tuple(Y.shape[:-2]) + (Y.shape[-1],)
+    if tuple(inverse_power.shape) != want:
+        raise ValueError(f'inverse_power must have shape {want}, got {tuple(inverse_power.shape)}')
+    if _device.is_tensor(inverse_power):
+        ok = inverse_power.dtype in (torch.float32, torch.float64)
+    else:
+        ok = np.asarray(inverse_power).dtype in (np.float32, np.float64)
+    if not ok:
+        raise ValueError(f'inverse_power must be float32 or float64, got {inverse_power.dtype}')
+    Yd, like_numpy = _prepare(Y, 'wpe_step')
+    w = inverse_power if _device.is_tensor(inverse_power) else torch.from_numpy(np.asarray(inverse_power))
+    w = w.to(device=Yd.device, dtype=torch.float64)
+    if Yd.numel() == 0:
+        X = Yd.clone()
+    else:
+        bins, T = int(np.prod(Yd.shape[:-2], dtype=np.int64)), Yd.shape[-1]
+        X = _WpeStep.apply(Yd, w.reshape(bins, T), taps, delay, int(statistics_mode == 'valid'))
+    return _device.to_host(X, like_numpy)
+
+
+def _power(signal, psd_context, inverse, graph=True):
+    x, like_numpy = _prepare(signal, 'get_power_inverse' if inverse else 'get_power')
+    c = _context(psd_context)
+    D = x.shape[-2]
+    if D > MAX_D:
+        raise NotImplementedError(f'get_power supports D <= {MAX_D}, got D = {D}')
+    if graph and _needs_graph(x):
+        return _Power.apply(x, c, inverse)
+    return _device.to_host(_power_launch(x, c, inverse)[0], like_numpy)
 
 
 def get_power(signal, psd_context=0):
@@ -231,7 +443,7 @@ def get_power_online(signal):
     get_power(signal, psd_context=inf)[..., 0]."""
     if signal.shape[-1] == 0:
         raise ValueError('get_power_online needs at least one frame')
-    return _power(signal, math.inf, False)[..., 0]
+    return _power(signal, math.inf, False, graph=False)[..., 0]
 
 
 def _check_online(taps, delay, alpha, D):
