@@ -999,6 +999,38 @@ int pbb_estoi(const void* x, const void* y, int dtype, long long rows, long long
               const double* twiddle, long long group, void* workspace, size_t workspace_bytes, double* out,
               long long* frames, double* resampled, double* energies, long long* status, void* stream);
 
+/* pbb_stoi_backward: the gradient of pbb_stoi's (extended = 0) or pbb_estoi's (extended = 1) out with respect to x
+ * and y.  x, y, dtype, rows, n, up, down, taps, taps_per_phase, pre_remove, window, bands, twiddle and group are
+ * pbb_stoi's; grad_out (rows) float64 is dL/dout; grad_x, grad_y (rows, n) float64 receive dL/dx, dL/dy (every
+ * element written; either may be null, and its chain is skipped).  The workspace is
+ * pbb_stoi_backward_workspace_bytes(group, n, up, down, extended) (0 for an invalid shape); nothing is kept from the
+ * forward: steps 1-3 run again with the forward's kernels, so the keep mask, the kept frames and the band energies
+ * are bitwise the forward's.  Only enqueues work (no status word, no host synchronisation); fp64, every sum a gather
+ * in a fixed order, no atomics: repeated calls are bitwise identical.
+ *
+ * The derivative, per row with M_r >= 30 (rows on the 1e-5 path, including a non-finite reference, get zeros):
+ *  - the keep mask is a constant (it depends on x only through a threshold): the gradient flows through the kept
+ *    frames into x and y; a dropped frame's samples get only what the kept frames over them pass;
+ *  - band energies e_b = sqrt(sum_k |X_k|^2): dL/dX_k = (dL/de_b / e_b) X_k, 0 where e_b = 0; the frame gradient is
+ *    Re sum_k (dL/dX_k) e^{+2 pi i j k / 512} (j < 256) times the window, then the overlap-add and the first window
+ *    are transposed, then the resampler (the polyphase filter's transpose; the identity at 10 kHz);
+ *  - STOI, per (segment, band) with g = grad_out / (15 J): c = ||x|| / (||y|| + eps), y' = min(c y, C x) with the
+ *    gradient to the operand the forward selected (x on a tie), a = y' - mean, e = x - mean,
+ *    d = <a, e> / ((||a|| + eps)(||e|| + eps)): dd/da = e / (Da De) - d a / (Da ||a||), dd/de symmetric, each
+ *    mean-removal's transpose, dc/dx = x / (||x|| (||y|| + eps)), dc/dy = -||x|| y / ((||y|| + eps)^2 ||y||); a zero
+ *    norm (||x||, ||y||, ||a||, ||e||) has a zero subgradient;
+ *  - ESTOI, per segment with g = grad_out / (30 J): z = v / ||v|| after centring, per band then per frame; the
+ *    transpose of each step is (I - z z^T) / ||v|| then the centring's; a row or column that the 2^-92 rule
+ *    normalises to zeros passes no gradient;
+ *  - a non-finite y with a finite x gives NaN gradients (in that row only).  Digital silence in y gives finite
+ *    gradients, large where c ~ ||x|| / eps. */
+size_t pbb_stoi_backward_workspace_bytes(long long group, long long n, int up, int down, int extended);
+int pbb_stoi_backward(const void* x, const void* y, int dtype, long long rows, long long n, int up, int down,
+                      const double* taps, int taps_per_phase, long long pre_remove, const double* window,
+                      const int* bands, const double* twiddle, long long group, void* workspace,
+                      size_t workspace_bytes, int extended, const double* grad_out, double* grad_x, double* grad_y,
+                      void* stream);
+
 /* ------------------------------------------------------------------------
  * SI-SDR (pb_bss/evaluation/module_si_sdr.py:4-56) and the invasive SxR (pb_bss/evaluation/sxr_module.py:17-274).
  * csrc/sxr.cuh.  fp64 throughout, no float atomics.  A row of n samples is summed in ceil(n / PBB_SXR_CHUNK) chunks,

@@ -189,6 +189,9 @@ SIGNATURES = {
                       _vp, _vp]),
     'pbb_estoi': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _vp, _vp, _vp, _vp,
                        _vp, _vp]),
+    'pbb_stoi_backward_workspace_bytes': (_sz, [_ll, _ll, _i, _i, _i]),
+    'pbb_stoi_backward': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _i, _vp,
+                               _vp, _vp, _vp]),
     'pbb_mean_square_workspace_bytes': (_sz, [_ll, _ll]),
     'pbb_mean_square': (_i, [_vp, _i, _ll, _ll, _vp, _sz, _vp, _vp]),
     'pbb_si_sdr_workspace_bytes': (_sz, [_ll, _ll]),

@@ -876,7 +876,7 @@ using namespace pbb;
 extern "C" {
 
 const char* pbb_last_error(void) { return g_err; }
-int pbb_version(void) { return 106; }
+int pbb_version(void) { return 107; }
 
 int pbb_normalize_observation(const void* y, void* z, int F, int T, int D, int dtype, int swap, void* stream) {
   PBB_CHECK_ARG(y != nullptr, 1, "y is null");

@@ -24,12 +24,28 @@ Documented differences from the reference:
     value of pystoi's random term there.  Digital silence in the estimate reaches this: its all-zero bands, and the
     segments with one non-zero frame at either end of a silent stretch, whose frames are constant over the bands
     after the first step in exact arithmetic.
+
+Gradients: STOI and ESTOI of CUDA tensors that require grad are differentiable with respect to both signals
+(pbb_stoi_backward, which runs the forward's stages again and then one fp64 kernel per adjoint step; fixed-order sums,
+no atomics, no host synchronisation).  The value is bitwise the same with or without a graph, gradients come back in
+the input's dtype, repeated backward calls are bitwise identical, and double backward raises.  A broadcast operand's
+gradient is torch's reduction of the broadcast.  The derivative's conventions:
+  - the silent-frame selection is a constant of the graph (it depends on the reference only through a threshold): the
+    gradient flows through the kept frames into both signals; a dropped frame's samples get only the contributions of
+    the kept frames that overlap them;
+  - the clipping min(c y, C x) passes the gradient to the operand the forward selected (x on a tie);
+  - a zero norm (a band energy, ||y|| in the scale c, a centred norm in the correlation) has a zero subgradient, as
+    torch.linalg.vector_norm: digital silence in the estimate gives finite, possibly very large, gradients;
+  - ESTOI's rows and columns that the 2^-92 rule normalises to zeros pass no gradient;
+  - rows on the 1e-5 path (fewer than 30 frames, including a non-finite reference) get zero gradients;
+  - a non-finite estimate sample with a finite reference gives NaN gradients in its row only.
 """
 import math
 import warnings
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from .. import _device, _lib
 
@@ -189,6 +205,48 @@ def _stages(x, y, sample_rate, stages=True, extended=False):
     return out
 
 
+def _backward(x, y, sample_rate, extended, grad, need_x, need_y):
+    """(grad_x, grad_y) float64 (rows, n), None where not needed, by pbb_stoi_backward; only enqueues work."""
+    lib = _lib.load()
+    rows, n = x.shape
+    up, down = rates(sample_rate)
+    taps, tpp, pre_remove, win, bands, tw = _device_tables(sample_rate)
+    per_row = lib.pbb_stoi_backward_workspace_bytes(1, n, up, down, int(extended))
+    group = int(max(1, min(rows, MAX_GROUP, WORKSPACE_BYTES // per_row)))
+    nbytes = lib.pbb_stoi_backward_workspace_bytes(group, n, up, down, int(extended))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    gx = torch.empty((rows, n), dtype=torch.float64, device=x.device) if need_x else None
+    gy = torch.empty((rows, n), dtype=torch.float64, device=x.device) if need_y else None
+    g = grad.to(torch.float64).contiguous()
+    _lib.check(lib.pbb_stoi_backward(_device.ptr(x), _device.ptr(y),
+                                     _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64, rows, n, up, down,
+                                     _device.ptr(taps), tpp, pre_remove, _device.ptr(win), _device.ptr(bands),
+                                     _device.ptr(tw), group, _device.ptr(ws), nbytes, int(extended), _device.ptr(g),
+                                     _device.ptr(gx), _device.ptr(gy), _device.stream_ptr()), 'pbb_stoi_backward')
+    return gx, gy
+
+
+class _Stoi(torch.autograd.Function):
+    """x, y (rows, n) contiguous CUDA tensors of one dtype -> STOI / ESTOI (rows,) float64 by pbb_stoi / pbb_estoi;
+    backward pbb_stoi_backward, which recomputes the forward's stages from x and y."""
+
+    @staticmethod
+    def forward(ctx, x, y, sample_rate, extended):
+        value = _stages(x, y, sample_rate, stages=False, extended=extended)['value']
+        ctx.save_for_backward(x, y)
+        ctx.args = (sample_rate, extended)
+        return value
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        x, y = ctx.saved_tensors
+        sample_rate, extended = ctx.args
+        need_x, need_y = ctx.needs_input_grad[:2]
+        gx, gy = _backward(x, y, sample_rate, extended, grad, need_x, need_y)
+        return (gx.to(x.dtype) if need_x else None, gy.to(y.dtype) if need_y else None, None, None)
+
+
 def stoi(reference, estimation, sample_rate, extended=False):
     """pb_bss.evaluation.stoi: the STOI of estimation against reference along the last axis, after broadcasting the
     two (NumPy's rules; ValueError if they do not broadcast).  1-D input gives an np.float64, n-D input an ndarray of
@@ -203,7 +261,10 @@ def stoi(reference, estimation, sample_rate, extended=False):
 
     A pair with fewer than 30 STFT frames after the silent-frame removal gives 1e-5 and a RuntimeWarning, as pystoi
     does.  float32 and integer input are computed in fp64; complex input raises TypeError; signals of more than 2^22
-    samples, more than 2^23 at 10 kHz, or without one 256-sample frame at 10 kHz raise ValueError."""
+    samples, more than 2^23 at 10 kHz, or without one 256-sample frame at 10 kHz raise ValueError.
+
+    CUDA tensors that require grad get a graph: the value is differentiable with respect to both signals (see the
+    module's docstring for the conventions at the keep mask, the clip, zero norms and the 1e-5 rows)."""
     shape = _check(reference, estimation, sample_rate)
     sample_rate = int(sample_rate)
     like_numpy = not (_device.is_tensor(reference) or _device.is_tensor(estimation))
@@ -212,7 +273,7 @@ def stoi(reference, estimation, sample_rate, extended=False):
         value = _device.empty(lead, torch.float64)
     else:
         x, y = _operands(reference, estimation, shape)
-        value = _stages(x, y, sample_rate, stages=False, extended=bool(extended))['value'].reshape(lead)
+        value = _Stoi.apply(x, y, sample_rate, bool(extended)).reshape(lead)
     if not like_numpy:
         return value
     v = value.cpu().numpy()
