@@ -69,7 +69,8 @@ const char* pbb_last_error(void);
 int pbb_version(void);
 
 /* Launch accounting and optional CUDA-event timing of the library's own kernels
- * (used by bench.py for `gpu_launches` and the roofline of the dominant kernel). */
+ * (used by bench.py for `gpu_launches` and the roofline of the dominant kernel).
+ * pbb_launch_count: the kernel launches so far; each launch also gets its own profile record. */
 long long pbb_launch_count(void);
 void pbb_profile_enable(int on);
 void pbb_profile_reset(void);

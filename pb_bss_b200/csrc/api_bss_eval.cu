@@ -49,35 +49,24 @@ static bool valid_shape(long long T, int K, int E) {
 // Blocked LU of `mats` augmented matrices, then the back substitution of their right-hand columns
 static int lu_solve(LuBatch b, long long mats, cudaStream_t st) {
   for (int k0 = 0; k0 < b.n; k0 += kPanel) {
-    {
-      LaunchScope ls("bss_lu_panel_kernel", st);
-      bss_lu_panel_kernel<<<(unsigned)mats, 512, 0, st>>>(b, k0);
-      PBB_CUDA(cudaGetLastError());
-    }
+    PBB_TRY(launch_kernel("bss_lu_panel_kernel", bss_lu_panel_kernel, (unsigned)mats, 512, 0, st, b, k0));
     const int cols = b.ncols - k0 - kPanel, rows = b.n - k0 - kPanel;
     if (cols > 0) {
-      LaunchScope ls("bss_lu_trsm_kernel", st);
-      bss_lu_trsm_kernel<<<dim3((cols + 127) / 128, (unsigned)mats), 128, 0, st>>>(b, k0);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("bss_lu_trsm_kernel", bss_lu_trsm_kernel, dim3((cols + 127) / 128, (unsigned)mats), 128, 0,
+                            st, b, k0));
     }
     if (cols > 0 && rows > 0) {
-      LaunchScope ls("bss_lu_update_kernel", st);
-      bss_lu_update_kernel<<<dim3((cols + 63) / 64, (rows + 63) / 64, (unsigned)mats), 128, 0, st>>>(b, k0);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("bss_lu_update_kernel", bss_lu_update_kernel,
+                            dim3((cols + 63) / 64, (rows + 63) / 64, (unsigned)mats), 128, 0, st, b, k0));
     }
   }
-  LaunchScope ls("bss_backsub_kernel", st);
-  bss_backsub_kernel<<<(unsigned)mats, 256, 0, st>>>(b);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("bss_backsub_kernel", bss_backsub_kernel, (unsigned)mats, 256, 0, st, b);
 }
 
 template <int NS>
 static int corr_launch(const double* x, const BssShape& s, long long g, double* part, cudaStream_t st) {
-  LaunchScope ls("bss_corr_kernel", st);
-  bss_corr_kernel<NS><<<dim3((unsigned)s.parts, (unsigned)s.K, (unsigned)g), 256, 0, st>>>(x, s, part);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("bss_corr_kernel", bss_corr_kernel<NS>, dim3((unsigned)s.parts, (unsigned)s.K, (unsigned)g), 256,
+                       0, st, x, s, part);
 }
 
 template <int NS>
@@ -85,10 +74,8 @@ static int project_launch(const double* x, const BssShape& s, long long g, const
                           double* sums, cudaStream_t st) {
   const size_t smem = sizeof(ProjSmem<NS>);
   PBB_CUDA(cudaFuncSetAttribute(bss_project_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchScope ls("bss_project_kernel", st);
-  bss_project_kernel<NS><<<dim3((unsigned)s.tiles, (unsigned)g), 256, smem, st>>>(x, s, G, Gb, sums);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("bss_project_kernel", bss_project_kernel<NS>, dim3((unsigned)s.tiles, (unsigned)g), 256, smem,
+                       st, x, s, G, Gb, sums);
 }
 
 }  // namespace pbb
@@ -132,26 +119,21 @@ int pbb_bss_eval(const double* x, long long items, int K, int E, long long T, in
     const long long g = items - i0 < group ? items - i0 : group;
     const double* xg = x + i0 * s.S * T;
     PBB_CUDA(cudaMemsetAsync(flags, 0, (size_t)g * sizeof(int), st));
-    {
-      LaunchScope ls("bss_check_kernel", st);
-      bss_check_kernel<<<dim3((unsigned)s.S, (unsigned)g), 256, 0, st>>>(xg, T, s.S, flags);
-      PBB_CUDA(cudaGetLastError());
-    }
+    PBB_TRY(launch_kernel("bss_check_kernel", bss_check_kernel, dim3((unsigned)s.S, (unsigned)g), 256, 0, st, xg, T,
+                          s.S, flags));
     const int ns = (s.S + 7) / 8;
     int rc = ns == 1 ? corr_launch<1>(xg, s, g, part, st)
                      : ns == 2 ? corr_launch<2>(xg, s, g, part, st) : corr_launch<3>(xg, s, g, part, st);
     if (rc) return rc;
     {
       const long long n = g * s.K * s.S * kBssL;
-      LaunchScope ls("bss_corr_reduce_kernel", st);
-      bss_corr_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(part, s, g, R);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("bss_corr_reduce_kernel", bss_corr_reduce_kernel, (unsigned)((n + 255) / 256), 256, 0, st,
+                            part, s, g, R));
     }
     {
       const long long n = g * s.N * (long long)(s.N + kRhsPad);
-      LaunchScope ls("bss_assemble_kernel", st);
-      bss_assemble_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(R, s, g, G, Gb);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("bss_assemble_kernel", bss_assemble_kernel, (unsigned)((n + 255) / 256), 256, 0, st, R, s,
+                            g, G, Gb));
     }
     rc = lu_solve(LuBatch{G, s.N, s.N + kRhsPad, s.N + E, 1, flags}, g, st);
     if (rc) return rc;
@@ -161,15 +143,9 @@ int pbb_bss_eval(const double* x, long long items, int K, int E, long long T, in
     }
     rc = E > 8 ? project_launch<2>(xg, s, g, G, Gb, sums, st) : project_launch<1>(xg, s, g, G, Gb, sums, st);
     if (rc) return rc;
-    {
-      LaunchScope ls("bss_ratio_kernel", st);
-      bss_ratio_kernel<<<(unsigned)g, 256, 0, st>>>(sums, s, compute_permutation, flags, i0, sdr, sir, sar, selection,
-                                                    pairs);
-      PBB_CUDA(cudaGetLastError());
-    }
-    LaunchScope ls("bss_status_kernel", st);
-    bss_status_kernel<<<1, 32, 0, st>>>(flags, g, i0, status);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("bss_ratio_kernel", bss_ratio_kernel, (unsigned)g, 256, 0, st, sums, s, compute_permutation,
+                          flags, i0, sdr, sir, sar, selection, pairs));
+    PBB_TRY(launch_kernel("bss_status_kernel", bss_status_kernel, 1, 32, 0, st, flags, g, i0, status));
   }
   return 0;
 }

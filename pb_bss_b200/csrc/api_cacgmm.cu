@@ -232,11 +232,6 @@ static int setup_frame_split(PersistArgs* p, const CacgmmWorkspace& ws, int F, i
 }
 
 // ---- shape / dtype dispatch ------------------------------------------------------
-// fn(ct) with a value of the storage type (double2 for PBB_C128, float2 for PBB_C64) standing for the type
-template <class Fn>
-static int with_ct(int dtype, Fn&& fn) {
-  return dtype == PBB_C128 ? fn(double2{}) : fn(float2{});
-}
 // fn(k, ct) with k = std::integral_constant<int, K> for the instantiated K in {2, 3, 4}
 template <class Fn>
 static int with_k_ct(int K, int dtype, Fn&& fn) {
@@ -268,16 +263,6 @@ static int with_bingham_d(int D, Fn&& fn) {
     case 6: return fn(std::integral_constant<int, 6>{});
     default: set_error("complex Bingham: D = %d, need 2 <= D <= 6", D); return -5;
   }
-}
-
-// ---- launches ------------------------------------------------------------------
-template <typename Kern, typename... Args>
-static int launch_kernel(const char* name, Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                         Args... args) {
-  LaunchScope ls(name, st);
-  kern<<<grid, block, smem, st>>>(args...);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
 }
 
 // The normalisation kernels put the bins on gridDim.y (at most 65535): more bins take one launch per 65535, with
@@ -596,10 +581,7 @@ static int launch_persistent_generic(Kern kern, int threads, size_t smem, int* c
   if (grid < 1) grid = 1;
   const long long tasks = (long long)a.iterations * a.F * (a.tsplit > 1 ? a.tsplit : 1);
   if (grid > tasks) grid = tasks;
-  LaunchScope ls(name, st);
-  kern<<<(unsigned)grid, threads, smem, st>>>(a);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel(name, kern, (unsigned)grid, threads, smem, st, a);
 }
 
 // The task kernel of a model: em_ws_kernel for the lean D = 8 model (the warp-specialised kernel), otherwise
@@ -654,9 +636,7 @@ static int launch_sticky(const PersistArgs& a, int K, int dtype, int S, cudaStre
   return with_k_ct(K, dtype, [&](auto k, auto ct) {
     const ClusterLaunch cl((unsigned)(a.F * S), 256, sizeof(WsSmem<8, decltype(k)::value, decltype(ct)>),
                            (unsigned)S, st);
-    LaunchScope ls("em_sticky_kernel", st);
-    PBB_CUDA(cudaLaunchKernelEx(&cl.cfg, em_sticky_kernel<decltype(k)::value, decltype(ct)>, a));
-    return 0;
+    return launch_ex("em_sticky_kernel", cl.cfg, em_sticky_kernel<decltype(k)::value, decltype(ct)>, a);
   });
 }
 
@@ -1003,12 +983,9 @@ int pbb_cacgmm_predict(const void* y, int dtype, int F, int T, int D, int K, con
   a.loglik_part = loglik ? ws.loglik_part : nullptr;
   int nch = launch_em(a, dtype, 0, st);
   if (nch <= 0) return nch ? nch : 1;
-  if (loglik) {
-    // per-bin sum of the chunk partials, fixed order
-    sum_rows_kernel<<<(F + 127) / 128, 128, 0, st>>>(ws.loglik_part, loglik, F, nch);
-    PBB_CUDA(cudaGetLastError());
-  }
-  return 0;
+  if (!loglik) return 0;
+  // per-bin sum of the chunk partials, fixed order
+  return launch_kernel("sum_rows_kernel", sum_rows_kernel, (F + 127) / 128, 128, 0, st, ws.loglik_part, loglik, F, nch);
 }
 
 int pbb_cacgmm_mstep(const void* y, int dtype, int F, int T, int D, int K, const double* affiliation,
@@ -1266,17 +1243,17 @@ int pbb_mixture_weight_over_bins(const double* affiliation, int F, int K, int T,
   PBB_CHECK_ARG(weight_kt != nullptr, 6, "weight (K, T) output is null");
   PBB_CHECK_ARG(!also_over_time || weight_k != nullptr, 7, "weight (K) output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("mean_over_bins_kernel", st);
-  mean_over_bins_kernel<<<(K * T + 255) / 256, 256, 0, st>>>(affiliation, F, K, T, weight_kt);
-  if (also_over_time) mean_over_time_kernel<<<K, 256, 0, st>>>(weight_kt, K, T, weight_k);
-  if (unit_norm) {
-    // the saliency form of estimate_mixture_weight (mixture_model_utils.py:192-203, used by CWMMTrainer):
-    // sums instead of means, then _unit_norm(ord=1, axis=-2, eps=1e-10, 'where') -- the 1/F (1/T) cancels
-    if (also_over_time) unit_norm_over_classes_kernel<<<1, 32, 0, st>>>(weight_k, K, 1);
-    else unit_norm_over_classes_kernel<<<(T + 127) / 128, 128, 0, st>>>(weight_kt, K, T);
-  }
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("mean_over_bins_kernel", mean_over_bins_kernel, (K * T + 255) / 256, 256, 0, st, affiliation, F,
+                        K, T, weight_kt));
+  if (also_over_time)
+    PBB_TRY(launch_kernel("mean_over_time_kernel", mean_over_time_kernel, K, 256, 0, st, weight_kt, K, T, weight_k));
+  if (!unit_norm) return 0;
+  // the saliency form of estimate_mixture_weight (mixture_model_utils.py:192-203, used by CWMMTrainer):
+  // sums instead of means, then _unit_norm(ord=1, axis=-2, eps=1e-10, 'where') -- the 1/F (1/T) cancels
+  if (also_over_time)
+    return launch_kernel("unit_norm_over_classes_kernel", unit_norm_over_classes_kernel, 1, 32, 0, st, weight_k, K, 1);
+  return launch_kernel("unit_norm_over_classes_kernel", unit_norm_over_classes_kernel, (T + 127) / 128, 128, 0, st,
+                       weight_kt, K, T);
 }
 
 }  // extern "C"

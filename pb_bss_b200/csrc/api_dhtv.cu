@@ -734,9 +734,8 @@ static int launch_dhtv_cluster(const DhtvCall& c, cudaStream_t st, bool* launche
       }
       cluster_ctas = C;
     }
-    LaunchScope ls("dhtv_cluster_kernel", st);
-    PBB_CUDA(cudaLaunchKernelEx(&cl.cfg, kern, c.features, c.plan_dev, c.nplan, c.K, c.F, c.T, c.mapping, c.metric,
-                                c.algorithm));
+    PBB_TRY(launch_ex("dhtv_cluster_kernel", cl.cfg, kern, c.features, c.plan_dev, c.nplan, c.K, c.F, c.T, c.mapping,
+                      c.metric, c.algorithm));
     *launched = true;
 #ifdef PBB_PHASE_TIMING
     print_dhtv_phases(st, "dhtv cluster", {"segment load (+store)", "partial sums", "barrier 1 + reduce-scatter",
@@ -753,7 +752,7 @@ static int launch_dhtv_cluster(const DhtvCall& c, cudaStream_t st, bool* launche
 }
 
 // dhtv_coop_kernel: one CTA per bin of the widest segment, as many as can be resident.
-static int launch_dhtv_coop(DhtvCall c, int dev, cudaStream_t st) {
+static int launch_dhtv_coop(const DhtvCall& c, int dev, cudaStream_t st) {
   const size_t smem = (size_t)c.K * c.T * sizeof(double);
   PBB_CUDA(cudaFuncSetAttribute(dhtv_coop_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   int per_sm = 0, sms = 0;
@@ -765,10 +764,9 @@ static int launch_dhtv_coop(DhtvCall c, int dev, cudaStream_t st) {
   int grid = c.widest;
   if (grid > per_sm * sms) grid = per_sm * sms;
   if (grid < 1) grid = 1;
-  void* args[] = {&c.features, &c.partial, &c.changed, &c.plan_dev, &c.nplan, &c.K,
-                  &c.F,        &c.T,       &c.mapping, &c.bar,      &c.metric, &c.algorithm};
-  LaunchScope ls("dhtv_coop_kernel", st);
-  PBB_CUDA(cudaLaunchCooperativeKernel((const void*)dhtv_coop_kernel, dim3(grid), dim3(threads), args, smem, st));
+  const CoopLaunch cl(grid, threads, smem, st);
+  PBB_TRY(launch_ex("dhtv_coop_kernel", cl.cfg, dhtv_coop_kernel, c.features, c.partial, c.changed, c.plan_dev, c.nplan,
+                    c.K, c.F, c.T, c.mapping, c.bar, c.metric, c.algorithm));
 #ifdef PBB_PHASE_TIMING
   print_dhtv_phases(st, "dhtv", {"phase A", "barrier 1", "centroid combine", "centroid norms", "scores", "assignment",
                                  "permute/rest", "barrier 2"});
@@ -802,13 +800,12 @@ int pbb_dhtv_mapping_ex(const double* mask, int K, int F, int T, const int* plan
   c.bar = reinterpret_cast<unsigned*>(c.changed + c.total_iters + 1);  // zeroed with the flags
   c.plan_dev = c.changed + c.total_iters + 2;
   PBB_CUDA(cudaMemsetAsync(c.changed, 0, (size_t)(c.total_iters + 2) * sizeof(int), st));
-  {
-    LaunchScope ls("dhtv_normalize_kernel", st);
-    if (metric == 1) dhtv_normalize_kernel<<<K * F, 128, 0, st>>>(mask, features, K * F, T);
-    else PBB_CUDA(cudaMemcpyAsync(features, mask, (size_t)K * F * T * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    dhtv_init_mapping_kernel<<<(K * F + 255) / 256, 256, 0, st>>>(mapping, K, F);
-    PBB_CUDA(cudaGetLastError());
-  }
+  if (metric == 1)
+    PBB_TRY(launch_kernel("dhtv_normalize_kernel", dhtv_normalize_kernel, K * F, 128, 0, st, mask, features, K * F, T));
+  else
+    PBB_CUDA(cudaMemcpyAsync(features, mask, (size_t)K * F * T * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  PBB_TRY(launch_kernel("dhtv_init_mapping_kernel", dhtv_init_mapping_kernel, (K * F + 255) / 256, 256, 0, st, mapping,
+                        K, F));
   PBB_CUDA(cudaMemcpyAsync(c.plan_dev, plan, (size_t)3 * nplan * sizeof(int), cudaMemcpyHostToDevice, st));
   // The reference's plans (~100-bin segments) fit a cluster.  PBB_DHTV_COOP=1 keeps the grid-barrier kernel (A/B).
   static const bool no_cluster = getenv("PBB_DHTV_COOP") != nullptr;
@@ -832,10 +829,7 @@ int pbb_apply_mapping(const double* mask, const long long* mapping, int K, int F
   PBB_CHECK_ARG(K > 0 && K < 20 && F > 0 && T > 0, 3, "bad shape (K < 20, permutation_alignment.py:102)");
   PBB_CHECK_ARG(out != nullptr, 6, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("apply_mapping_kernel", st);
-  apply_mapping_kernel<<<K * F, 128, 0, st>>>(mask, mapping, K, F, T, out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("apply_mapping_kernel", apply_mapping_kernel, K * F, 128, 0, st, mask, mapping, K, F, T, out);
 }
 
 int pbb_score_matrix(const double* mask, const double* reference, long long mask_source_stride,
@@ -848,11 +842,8 @@ int pbb_score_matrix(const double* mask, const double* reference, long long mask
   PBB_CHECK_ARG(metric >= 0 && metric <= 2, 8, "metric: 0 multiply, 1 cos, 2 euclidean");
   PBB_CHECK_ARG(scores != nullptr, 9, "scores is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("score_matrix_kernel", st);
-  score_matrix_kernel<<<(F + 3) / 4, 128, 0, st>>>(mask, reference, mask_source_stride, reference_source_stride, K,
-                                                   F, T, metric, scores);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("score_matrix_kernel", score_matrix_kernel, (F + 3) / 4, 128, 0, st, mask, reference,
+                       mask_source_stride, reference_source_stride, K, F, T, metric, scores);
 }
 
 int pbb_mapping_from_score_matrix(const double* scores, int F, int K, int algorithm, long long* mapping,
@@ -864,10 +855,8 @@ int pbb_mapping_from_score_matrix(const double* scores, int F, int K, int algori
   PBB_CHECK_ARG(mapping != nullptr, 5, "mapping is null");
   PBB_CHECK_ARG(status != nullptr, 6, "status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("mapping_from_score_kernel", st);
-  mapping_from_score_kernel<<<(F + 63) / 64, 64, 0, st>>>(scores, F, K, algorithm, mapping, status);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("mapping_from_score_kernel", mapping_from_score_kernel, (F + 63) / 64, 64, 0, st, scores, F, K,
+                       algorithm, mapping, status);
 }
 
 int pbb_chain_mapping(const long long* pair_mapping, int K, int F, long long* mapping, void* stream) {
@@ -876,10 +865,7 @@ int pbb_chain_mapping(const long long* pair_mapping, int K, int F, long long* ma
   PBB_CHECK_ARG(F > 0, 3, "F must be positive");
   PBB_CHECK_ARG(mapping != nullptr, 4, "mapping is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("chain_mapping_kernel", st);
-  chain_mapping_kernel<<<1, 32, 0, st>>>(pair_mapping, K, F, mapping);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("chain_mapping_kernel", chain_mapping_kernel, 1, 32, 0, st, pair_mapping, K, F, mapping);
 }
 
 }  // extern "C"

@@ -519,11 +519,8 @@ static int vmf_log_pdf_launch(const double* embedding, const double* mean, const
   PBB_CHECK_ARG(K > 0 && K <= kIntMaxK, 8, "need 0 < K <= 6");
   PBB_CHECK_ARG(out != nullptr, 9, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls(EXP ? "vmf_pdf_kernel" : "vmf_log_pdf_kernel", st);
-  vmf_log_pdf_kernel<EXP><<<dim3((N + 127) / 128, B), 128, 0, st>>>(embedding, mean, concentration, log_norm, N, E, K,
-                                                                     out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel(EXP ? "vmf_pdf_kernel" : "vmf_log_pdf_kernel", vmf_log_pdf_kernel<EXP>, dim3((N + 127) / 128, B),
+                       128, 0, st, embedding, mean, concentration, log_norm, N, E, K, out);
 }
 
 }  // namespace pbb
@@ -538,10 +535,8 @@ int pbb_cacg_log_pdf(const double* quadratic, const double* eigenvalues, int F, 
   PBB_CHECK_ARG(F > 0 && K > 0 && T > 0 && D > 0, 3, "bad shape");
   PBB_CHECK_ARG(log_pdf != nullptr, 7, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("cacg_log_pdf_kernel", st);
-  cacg_log_pdf_kernel<<<dim3((T + 127) / 128, F * K), 128, 0, st>>>(quadratic, eigenvalues, F, K, T, D, log_pdf);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("cacg_log_pdf_kernel", cacg_log_pdf_kernel, dim3((T + 127) / 128, F * K), 128, 0, st, quadratic,
+                       eigenvalues, F, K, T, D, log_pdf, kTiny, nullptr);
 }
 
 int pbb_cacg_log_pdf_floor(const double* quadratic, const double* eigenvalues, int F, int K, int T, int D,
@@ -551,11 +546,8 @@ int pbb_cacg_log_pdf_floor(const double* quadratic, const double* eigenvalues, i
   PBB_CHECK_ARG(quadratic_out != nullptr && quadratic_out != quadratic, 8, "quadratic_out is null or the input");
   PBB_CHECK_ARG(log_pdf != nullptr, 9, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("cacg_log_pdf_kernel", st);
-  cacg_log_pdf_kernel<<<dim3((T + 127) / 128, F * K), 128, 0, st>>>(quadratic, eigenvalues, F, K, T, D, log_pdf,
-                                                                      q_floor, quadratic_out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("cacg_log_pdf_kernel", cacg_log_pdf_kernel, dim3((T + 127) / 128, F * K), 128, 0, st, quadratic,
+                       eigenvalues, F, K, T, D, log_pdf, q_floor, quadratic_out);
 }
 
 int pbb_gaussian_log_pdf(const double* embedding, const double* mean, const double* precision_cholesky,
@@ -567,11 +559,9 @@ int pbb_gaussian_log_pdf(const double* embedding, const double* mean, const doub
   PBB_CHECK_ARG(K > 0 && K < kMaxK, 8, "bad K");
   PBB_CHECK_ARG(log_pdf != nullptr, 10, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("gaussian_log_pdf_kernel", st);
-  gaussian_log_pdf_kernel<<<dim3((T + 127) / 128, F), 128, (size_t)2 * K * E * sizeof(double), st>>>(
-      embedding, mean, precision_cholesky, log_det, F, T, E, K, diagonal, log_pdf);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("gaussian_log_pdf_kernel", gaussian_log_pdf_kernel, dim3((T + 127) / 128, F), 128,
+                       (size_t)2 * K * E * sizeof(double), st, embedding, mean, precision_cholesky, log_det, F, T, E, K,
+                       diagonal, log_pdf);
 }
 
 size_t pbb_gaussian_fit_scratch_doubles(int F, int E, int K) { return (size_t)F * K * (E + 1) + K; }
@@ -586,13 +576,14 @@ int pbb_gaussian_fit(const double* embedding, const double* weight, int F, int T
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   double* partial = scratch;
   double* denom = scratch + (size_t)F * K * (E + 1);
-  LaunchScope ls("gaussian_fit_kernels", st);
-  gaussian_fit_partial_kernel<<<dim3(F, K), 256, 0, st>>>(embedding, weight, mean, F, T, E, K, 0, partial);
-  gaussian_fit_mean_kernel<<<K, kIntMaxE + 1, 0, st>>>(partial, F, E, K, mean, denom);
-  gaussian_fit_partial_kernel<<<dim3(F, K), 256, 0, st>>>(embedding, weight, mean, F, T, E, K, 1, partial);
-  gaussian_fit_cov_kernel<<<K, kIntMaxE, 0, st>>>(partial, denom, F, E, K, spherical, covariance);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("gaussian_fit_partial_kernel", gaussian_fit_partial_kernel, dim3(F, K), 256, 0, st, embedding,
+                        weight, mean, F, T, E, K, 0, partial));
+  PBB_TRY(launch_kernel("gaussian_fit_mean_kernel", gaussian_fit_mean_kernel, K, kIntMaxE + 1, 0, st, partial, F, E, K,
+                        mean, denom));
+  PBB_TRY(launch_kernel("gaussian_fit_partial_kernel", gaussian_fit_partial_kernel, dim3(F, K), 256, 0, st, embedding,
+                        weight, mean, F, T, E, K, 1, partial));
+  return launch_kernel("gaussian_fit_cov_kernel", gaussian_fit_cov_kernel, K, kIntMaxE, 0, st, partial, denom, F, E, K,
+                       spherical, covariance);
 }
 
 int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b, double scale_a, double scale_b,
@@ -609,11 +600,9 @@ int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
   PBB_CHECK_ARG(!inline_pa || log_pdf_b != nullptr, 9, "the inline alignment pairs TWO log pdfs");
   PBB_CHECK_ARG(affiliation != nullptr, 13, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("log_pdf_to_affiliation_kernel", st);
-  log_pdf_to_affiliation_kernel<<<F, 256, 0, st>>>(log_pdf_a, log_pdf_b, scale_a, scale_b, weight, weight_mode, activity,
-                                                   affiliation_eps, inline_pa, F, K, T, affiliation, permutation);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("log_pdf_to_affiliation_kernel", log_pdf_to_affiliation_kernel, F, 256, 0, st, log_pdf_a,
+                       log_pdf_b, scale_a, scale_b, weight, weight_mode, activity, affiliation_eps, inline_pa, F, K, T,
+                       affiliation, permutation);
 }
 
 int pbb_class_weight(const double* masked_affiliation, int F, int K, int T, double* weight, void* stream) {
@@ -621,10 +610,7 @@ int pbb_class_weight(const double* masked_affiliation, int F, int K, int T, doub
   PBB_CHECK_ARG(F > 0 && K > 0 && K < kMaxK && T > 0, 2, "bad shape");
   PBB_CHECK_ARG(weight != nullptr, 5, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("class_weight_kernel", st);
-  class_weight_kernel<<<F, 256, 0, st>>>(masked_affiliation, F, K, T, weight);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("class_weight_kernel", class_weight_kernel, F, 256, 0, st, masked_affiliation, F, K, T, weight);
 }
 
 int pbb_gaussian_full_log_pdf(const double* embedding, const double* mean, const double* precision_cholesky,
@@ -637,17 +623,12 @@ int pbb_gaussian_full_log_pdf(const double* embedding, const double* mean, const
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const dim3 grid((N + 127) / 128, B);
   const size_t smem = (size_t)(E * E + E) * sizeof(double);
-  LaunchScope ls("gaussian_full_log_pdf_kernel", st);
-  if (E <= 8)
-    gaussian_full_log_pdf_kernel<8><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
-  else if (E <= 16)
-    gaussian_full_log_pdf_kernel<16><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
-  else if (E <= 32)
-    gaussian_full_log_pdf_kernel<32><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
-  else
-    gaussian_full_log_pdf_kernel<64><<<grid, 128, smem, st>>>(embedding, mean, precision_cholesky, log_det, N, E, K, log_pdf);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  const auto kern = E <= 8    ? gaussian_full_log_pdf_kernel<8>
+                    : E <= 16 ? gaussian_full_log_pdf_kernel<16>
+                    : E <= 32 ? gaussian_full_log_pdf_kernel<32>
+                              : gaussian_full_log_pdf_kernel<64>;
+  return launch_kernel("gaussian_full_log_pdf_kernel", kern, grid, 128, smem, st, embedding, mean, precision_cholesky,
+                       log_det, N, E, K, log_pdf);
 }
 
 size_t pbb_gaussian_full_fit_scratch_doubles(int B, int N, int E, int K) {
@@ -668,17 +649,14 @@ int pbb_gaussian_full_fit(const double* embedding, const double* weight, int B, 
   const int BK = B * K;
   double* partial = scratch;
   double* denom = scratch + (size_t)c.nchunks * BK * fit_entries(E);
-  LaunchScope ls("gaussian_full_fit_kernels", st);
-  gaussian_full_partial_kernel<<<dim3(c.nchunks, BK), kFitThreads, 0, st>>>(embedding, weight, nullptr, N, E, K,
-                                                                             c.chunk_len, 0, 0, partial);
-  gaussian_full_reduce_kernel<<<BK, kFitThreads, 0, st>>>(partial, c.nchunks, E, 0, denom, mean, nullptr, nullptr,
-                                                          nullptr);
-  gaussian_full_partial_kernel<<<dim3(c.nchunks, BK), kFitThreads, 0, st>>>(embedding, weight, mean, N, E, K,
-                                                                             c.chunk_len, 1, 0, partial);
-  gaussian_full_reduce_kernel<<<BK, kFitThreads, 0, st>>>(partial, c.nchunks, E, 1, denom, nullptr, nullptr, nullptr,
-                                                          covariance);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("gaussian_full_partial_kernel", gaussian_full_partial_kernel, dim3(c.nchunks, BK), kFitThreads,
+                        0, st, embedding, weight, nullptr, N, E, K, c.chunk_len, 0, 0, partial));
+  PBB_TRY(launch_kernel("gaussian_full_reduce_kernel", gaussian_full_reduce_kernel, BK, kFitThreads, 0, st, partial,
+                        c.nchunks, E, 0, denom, mean, nullptr, nullptr, nullptr));
+  PBB_TRY(launch_kernel("gaussian_full_partial_kernel", gaussian_full_partial_kernel, dim3(c.nchunks, BK), kFitThreads,
+                        0, st, embedding, weight, mean, N, E, K, c.chunk_len, 1, 0, partial));
+  return launch_kernel("gaussian_full_reduce_kernel", gaussian_full_reduce_kernel, BK, kFitThreads, 0, st, partial,
+                       c.nchunks, E, 1, denom, nullptr, nullptr, nullptr, covariance);
 }
 
 int pbb_precision_cholesky(const double* covariance, int M, int E, double* precision_cholesky, double* log_det,
@@ -688,12 +666,9 @@ int pbb_precision_cholesky(const double* covariance, int M, int E, double* preci
   PBB_CHECK_ARG(E > 0 && E <= kIntMaxE, 3, "need 0 < E <= 64");
   PBB_CHECK_ARG(precision_cholesky && log_det && status, 4, "output / status is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("precision_cholesky_kernel", st);
   PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
-  precision_cholesky_kernel<<<M, 32, (size_t)E * E * sizeof(double), st>>>(covariance, E, precision_cholesky, log_det,
-                                                                           status);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("precision_cholesky_kernel", precision_cholesky_kernel, M, 32, (size_t)E * E * sizeof(double),
+                       st, covariance, E, precision_cholesky, log_det, status);
 }
 
 int pbb_vmf_log_pdf(const double* embedding, const double* mean, const double* concentration, const double* log_norm,
@@ -718,13 +693,10 @@ int pbb_vmf_resultant(const double* embedding, const double* weight, int B, int 
   const int BK = B * K;
   double* partial = scratch;
   double* denom = scratch + (size_t)c.nchunks * BK * fit_entries(E);
-  LaunchScope ls("vmf_resultant_kernels", st);
-  gaussian_full_partial_kernel<<<dim3(c.nchunks, BK), kFitThreads, 0, st>>>(embedding, weight, nullptr, N, E, K,
-                                                                             c.chunk_len, 0, 1, partial);
-  gaussian_full_reduce_kernel<<<BK, kFitThreads, 0, st>>>(partial, c.nchunks, E, 0, denom, nullptr, resultant, total,
-                                                          nullptr);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("gaussian_full_partial_kernel", gaussian_full_partial_kernel, dim3(c.nchunks, BK), kFitThreads,
+                        0, st, embedding, weight, nullptr, N, E, K, c.chunk_len, 0, 1, partial));
+  return launch_kernel("gaussian_full_reduce_kernel", gaussian_full_reduce_kernel, BK, kFitThreads, 0, st, partial,
+                       c.nchunks, E, 0, denom, nullptr, resultant, total, nullptr);
 }
 
 int pbb_frame_weight(const double* masked_affiliation, int B, int K, int N, double* weight, void* stream) {
@@ -732,10 +704,8 @@ int pbb_frame_weight(const double* masked_affiliation, int B, int K, int N, doub
   PBB_CHECK_ARG(B > 0 && B <= 65535 && K > 0 && N > 0, 2, "bad shape");
   PBB_CHECK_ARG(weight != nullptr, 5, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("frame_weight_kernel", st);
-  frame_weight_kernel<<<dim3((N + 255) / 256, B), 256, 0, st>>>(masked_affiliation, K, N, weight);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("frame_weight_kernel", frame_weight_kernel, dim3((N + 255) / 256, B), 256, 0, st,
+                       masked_affiliation, K, N, weight);
 }
 
 }  // extern "C"

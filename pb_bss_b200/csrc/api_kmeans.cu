@@ -63,9 +63,8 @@ int pbb_kmeans_fit(const double* x, long long N, int E, int K, long long first, 
   {
     int grid = 0;
     if (int rc = km_grid((const void*)kmeans_init_kernel, 0, nch, max_ctas, &grid)) return rc;
-    void* args[] = {(void*)&x, &N, &E, &K, &first, (void*)&uniforms, (void*)&init, &w, &status};
-    LaunchScope ls("kmeans_init_kernel", st);
-    PBB_CUDA(cudaLaunchCooperativeKernel((const void*)kmeans_init_kernel, dim3(grid), dim3(kKmThreads), args, 0, st));
+    const CoopLaunch cl(grid, kKmThreads, 0, st);
+    PBB_TRY(launch_ex("kmeans_init_kernel", cl.cfg, kmeans_init_kernel, x, N, E, K, first, uniforms, init, w, status));
   }
   {
     const size_t smem = km_lloyd_smem(E, K);
@@ -74,10 +73,9 @@ int pbb_kmeans_fit(const double* x, long long N, int E, int K, long long first, 
     if (int rc = km_grid((const void*)kmeans_lloyd_kernel, smem, nch, max_ctas, &grid)) return rc;
     KmWork wl = w;
     wl.bar = w.bar + 1;
-    void* args[] = {&N, &E, &K, &max_iter, &wl, &centres, &labels, &inertia, &n_iter, &status};
-    LaunchScope ls("kmeans_lloyd_kernel", st);
-    PBB_CUDA(cudaLaunchCooperativeKernel((const void*)kmeans_lloyd_kernel, dim3(grid), dim3(kKmThreads), args, smem,
-                                         st));
+    const CoopLaunch cl(grid, kKmThreads, smem, st);
+    PBB_TRY(launch_ex("kmeans_lloyd_kernel", cl.cfg, kmeans_lloyd_kernel, N, E, K, max_iter, wl, centres, labels,
+                      inertia, n_iter, status));
   }
   return 0;
 }
@@ -92,11 +90,8 @@ int pbb_kmeans_predict(const double* x, long long N, int E, int K, const double*
   PBB_CHECK_ARG(labels != nullptr || one_hot != nullptr || N == 0, 6, "no output");
   if (N == 0) return 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("kmeans_predict_kernel", st);
-  kmeans_predict_kernel<<<(unsigned)((N + kKmThreads - 1) / kKmThreads), kKmThreads, 0, st>>>(x, N, E, K, centres,
-                                                                                             labels, one_hot);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("kmeans_predict_kernel", kmeans_predict_kernel, (unsigned)((N + kKmThreads - 1) / kKmThreads),
+                       kKmThreads, 0, st, x, N, E, K, centres, labels, one_hot);
 }
 
 }  // extern "C"

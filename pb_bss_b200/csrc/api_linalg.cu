@@ -57,12 +57,9 @@ static int solve_launch(const void* a, const void* b, int n, int D, int R, int h
   const size_t per = solve_smem_per_warp(D, R);
   const int warps = warps_for(per);
   PBB_CUDA(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  LaunchScope ls("solve_kernel", st);
-  solve_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
-      reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), n, D, R, hermitize,
-      reinterpret_cast<double2*>(x), status, warps, strict, fallback);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("solve_kernel", solve_kernel, (n + warps - 1) / warps, 32 * warps, per * warps, st,
+                       reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), n, D, R, hermitize,
+                       reinterpret_cast<double2*>(x), status, warps, strict, fallback);
 }
 
 static unsigned blocks_for(size_t count, int threads) { return (unsigned)((count + threads - 1) / threads); }
@@ -83,11 +80,8 @@ int pbb_heig_batched(const void* a, int n, int D, double* w, void* v, int* statu
   const size_t per = (jacobi_smem_bytes(D) + 15) & ~(size_t)15;
   const int warps = warps_for(per);
   PBB_CUDA(cudaFuncSetAttribute(heig_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  LaunchScope ls("heig_batched_kernel", st);
-  heig_batched_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
-      reinterpret_cast<const double2*>(a), n, D, w, reinterpret_cast<double2*>(v), status, warps);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("heig_batched_kernel", heig_batched_kernel, (n + warps - 1) / warps, 32 * warps, per * warps, st,
+                       reinterpret_cast<const double2*>(a), n, D, w, reinterpret_cast<double2*>(v), status, warps);
 }
 
 int pbb_gev_batched(const void* a, const void* b, int n, int D, void* w, int* status, void* stream) {
@@ -101,12 +95,9 @@ int pbb_gev_batched(const void* a, const void* b, int n, int D, void* w, int* st
                      ~(size_t)15;
   const int warps = warps_for(per);
   PBB_CUDA(cudaFuncSetAttribute(gev_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  LaunchScope ls("gev_kernel", st);
-  gev_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
-      reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), n, D,
-      reinterpret_cast<double2*>(w), status, warps);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("gev_kernel", gev_kernel, (n + warps - 1) / warps, 32 * warps, per * warps, st,
+                       reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), n, D,
+                       reinterpret_cast<double2*>(w), status, warps);
 }
 
 int pbb_solve_batched(const void* a, const void* b, int n, int D, int R, int hermitize, void* x, int* status,
@@ -140,12 +131,9 @@ int pbb_mvdr(const void* atf, const void* noise_psd, int n, int D, void* w, void
   int r = pbb_solve_batched(noise_psd, atf, n, D, 1, 1, scratch, status, stream);
   if (r) return r;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("mvdr_scale_kernel", st);
-  mvdr_scale_kernel<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<const double2*>(atf),
-                                                      reinterpret_cast<const double2*>(scratch), n, D,
-                                                      reinterpret_cast<double2*>(w));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("mvdr_scale_kernel", mvdr_scale_kernel, (n + 127) / 128, 128, 0, st,
+                       reinterpret_cast<const double2*>(atf), reinterpret_cast<const double2*>(scratch), n, D,
+                       reinterpret_cast<double2*>(w));
 }
 
 int pbb_souden(const void* phi, const void* target_psd, const void* noise_psd, int n, int D, double eps, void* mat,
@@ -154,20 +142,14 @@ int pbb_souden(const void* phi, const void* target_psd, const void* noise_psd, i
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
   PBB_CHECK_ARG(mat && num && den && num_sum && den_sum, 7, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  {
-    LaunchScope ls("souden_kernel", st);
-    souden_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(phi),
-                                    reinterpret_cast<const double2*>(target_psd),
-                                    reinterpret_cast<const double2*>(noise_psd), n, D, eps,
-                                    reinterpret_cast<double2*>(mat), reinterpret_cast<double2*>(num),
-                                    reinterpret_cast<double2*>(den));
-    PBB_CUDA(cudaGetLastError());
-  }
-  LaunchScope ls("colsum_kernel", st);
-  colsum_kernel<<<1, 128, 0, st>>>(reinterpret_cast<const double*>(num), reinterpret_cast<double*>(num_sum), n, 2 * D);
-  colsum_kernel<<<1, 128, 0, st>>>(reinterpret_cast<const double*>(den), reinterpret_cast<double*>(den_sum), n, 2 * D);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("souden_kernel", souden_kernel, n, 64, 0, st, reinterpret_cast<const double2*>(phi),
+                        reinterpret_cast<const double2*>(target_psd), reinterpret_cast<const double2*>(noise_psd), n, D,
+                        eps, reinterpret_cast<double2*>(mat), reinterpret_cast<double2*>(num),
+                        reinterpret_cast<double2*>(den)));
+  PBB_TRY(launch_kernel("colsum_kernel", colsum_kernel, 1, 128, 0, st, reinterpret_cast<const double*>(num),
+                        reinterpret_cast<double*>(num_sum), n, 2 * D));
+  return launch_kernel("colsum_kernel", colsum_kernel, 1, 128, 0, st, reinterpret_cast<const double*>(den),
+                       reinterpret_cast<double*>(den_sum), n, 2 * D);
 }
 
 int pbb_blind_analytic_normalization(const void* vector, const void* noise_psd, int n, int D, void* out,
@@ -176,12 +158,8 @@ int pbb_blind_analytic_normalization(const void* vector, const void* noise_psd, 
   PBB_CHECK_ARG(n > 0 && D > 0, 3, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 5, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("ban_kernel", st);
-  ban_kernel<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<const double2*>(vector),
-                                              reinterpret_cast<const double2*>(noise_psd), n, D,
-                                              reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("ban_kernel", ban_kernel, (n + 127) / 128, 128, 0, st, reinterpret_cast<const double2*>(vector),
+                       reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
 }
 
 static int apply_bf_launch(const void* vector, const void* mix, int dtype, int B, int F, int D, int T, void* out,
@@ -192,17 +170,12 @@ static int apply_bf_launch(const void* vector, const void* mix, int dtype, int B
   PBB_CHECK_ARG(out != nullptr, 7, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   dim3 grid((T + 255) / 256, F < 65535 ? F : 65535, B);
-  LaunchScope ls("apply_bf_kernel", st);
-  if (dtype == PBB_C128)
-    apply_bf_kernel<double2><<<grid, 256, 0, st>>>(reinterpret_cast<const double2*>(vector),
-                                                    reinterpret_cast<const double2*>(mix), F, D, T,
-                                                    reinterpret_cast<double2*>(out));
-  else
-    apply_bf_kernel<float2><<<grid, 256, 0, st>>>(reinterpret_cast<const double2*>(vector),
-                                                   reinterpret_cast<const float2*>(mix), F, D, T,
-                                                   reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_kernel("apply_bf_kernel", apply_bf_kernel<CT>, grid, 256, 0, st,
+                         reinterpret_cast<const double2*>(vector), reinterpret_cast<const CT*>(mix), F, D, T,
+                         reinterpret_cast<double2*>(out));
+  });
 }
 
 int pbb_apply_beamforming_vector(const void* vector, const void* mix, int dtype, int F, int D, int T, void* out,
@@ -220,12 +193,8 @@ int pbb_rank_one_estimate(const void* vector, const void* covariance, int n, int
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 3, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 5, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("rank_one_kernel", st);
-  rank_one_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(vector),
-                                    reinterpret_cast<const double2*>(covariance), n, D,
-                                    reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("rank_one_kernel", rank_one_kernel, n, 64, 0, st, reinterpret_cast<const double2*>(vector),
+                       reinterpret_cast<const double2*>(covariance), n, D, reinterpret_cast<double2*>(out));
 }
 
 int pbb_matvec_batched(const void* matrix, const void* vector, int n, int D, void* out, void* stream) {
@@ -233,12 +202,9 @@ int pbb_matvec_batched(const void* matrix, const void* vector, int n, int D, voi
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 3, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 5, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("matvec_kernel", st);
-  matvec_kernel<<<(n + 127) / 128, 128, 0, st>>>(reinterpret_cast<const double2*>(matrix),
-                                                 reinterpret_cast<const double2*>(vector), n, D,
-                                                 reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("matvec_kernel", matvec_kernel, (n + 127) / 128, 128, 0, st,
+                       reinterpret_cast<const double2*>(matrix), reinterpret_cast<const double2*>(vector), n, D,
+                       reinterpret_cast<double2*>(out));
 }
 
 size_t pbb_psd_workspace_bytes(int F, int T, int D, int K) {
@@ -264,10 +230,8 @@ int pbb_power_spectral_density(const void* observation, int dtype, int F, int D,
   const int nch = launch_em(a, dtype, 0, st);
   if (nch <= 0) return nch ? nch : 1;
   const int scale = mask == nullptr ? 2 : (normalize ? 1 : 0);
-  LaunchScope ls("psd_finalize_kernel", st);
-  psd_finalize_kernel<<<dim3(F, K), 64, 0, st>>>(a.part, nch, F, K, D, T, scale, reinterpret_cast<double2*>(psd));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("psd_finalize_kernel", psd_finalize_kernel, dim3(F, K), 64, 0, st, a.part, nch, F, K, D, T,
+                       scale, reinterpret_cast<double2*>(psd));
 }
 
 // ---- backward passes of the mask-based beamforming chain (linalg_kernels.cuh) --------------------------------------
@@ -291,18 +255,12 @@ int pbb_power_spectral_density_backward(const void* observation, int dtype, int 
   const double2* P = reinterpret_cast<const double2*>(psd);
   const double2* G = reinterpret_cast<const double2*>(grad_psd);
   double2* gy = reinterpret_cast<double2*>(grad_observation);
-  LaunchScope ls("psd_backward_kernel", st);
-  if (dtype == PBB_C128) {
-    PBB_CUDA(cudaFuncSetAttribute(psd_backward_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    psd_backward_kernel<double2><<<grid, kPsdBwdThreads, smem, st>>>(
-        reinterpret_cast<const double2*>(observation), mask, P, G, F, D, T, K, normalize, gy, grad_mask);
-  } else {
-    PBB_CUDA(cudaFuncSetAttribute(psd_backward_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    psd_backward_kernel<float2><<<grid, kPsdBwdThreads, smem, st>>>(
-        reinterpret_cast<const float2*>(observation), mask, P, G, F, D, T, K, normalize, gy, grad_mask);
-  }
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    PBB_CUDA(cudaFuncSetAttribute(psd_backward_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return launch_kernel("psd_backward_kernel", psd_backward_kernel<CT>, grid, kPsdBwdThreads, smem, st,
+                         reinterpret_cast<const CT*>(observation), mask, P, G, F, D, T, K, normalize, gy, grad_mask);
+  });
 }
 
 int pbb_souden_backward(const void* phi, const void* noise_psd, const void* grad_w, int n, int D, int ref_channel,
@@ -314,21 +272,16 @@ int pbb_souden_backward(const void* phi, const void* noise_psd, const void* grad
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   {
     // grad Phi goes to grad_noise_psd, which the last kernel overwrites
-    LaunchScope ls("souden_backward_kernel", st);
-    souden_backward_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(phi),
-                                             reinterpret_cast<const double2*>(grad_w), n, D, ref_channel, eps,
-                                             reinterpret_cast<double2*>(grad_noise_psd));
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("souden_backward_kernel", souden_backward_kernel, n, 64, 0, st,
+                          reinterpret_cast<const double2*>(phi), reinterpret_cast<const double2*>(grad_w), n, D,
+                          ref_channel, eps, reinterpret_cast<double2*>(grad_noise_psd)));
   }
   // grad X = N^-H grad Phi; a zero pivot (no derivative: the forward's minimum-norm branch) or non-finite N gives NaN
   const int rc = solve_launch(noise_psd, grad_noise_psd, n, D, D, 2, grad_target_psd, nullptr, 2, st);
   if (rc) return rc;
-  LaunchScope ls("souden_noise_backward_kernel", st);
-  souden_noise_backward_kernel<<<blocks_for((size_t)n * D * D, 128), 128, 0, st>>>(
-      reinterpret_cast<const double2*>(grad_target_psd), reinterpret_cast<const double2*>(phi), n, D,
-      reinterpret_cast<double2*>(grad_noise_psd));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("souden_noise_backward_kernel", souden_noise_backward_kernel, blocks_for((size_t)n * D * D, 128),
+                       128, 0, st, reinterpret_cast<const double2*>(grad_target_psd),
+                       reinterpret_cast<const double2*>(phi), n, D, reinterpret_cast<double2*>(grad_noise_psd));
 }
 
 // ---- backward passes of the get_bf_vector beamformers (linalg_kernels.cuh) ------------------------------------------
@@ -346,13 +299,10 @@ int pbb_eigenvector_backward(const void* a, const void* b, const void* w, const 
   const size_t per = eig_backward_smem_per_warp(D, b != nullptr);
   const int warps = warps_for(per);
   PBB_CUDA(cudaFuncSetAttribute(eig_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  LaunchScope ls("eig_backward_kernel", st);
-  eig_backward_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
-      reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b), reinterpret_cast<const double2*>(w),
-      reinterpret_cast<const double2*>(grad_w), grad_lambda, n, D, reinterpret_cast<double2*>(grad_a),
-      reinterpret_cast<double2*>(grad_b), warps);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("eig_backward_kernel", eig_backward_kernel, (n + warps - 1) / warps, 32 * warps, per * warps, st,
+                       reinterpret_cast<const double2*>(a), reinterpret_cast<const double2*>(b),
+                       reinterpret_cast<const double2*>(w), reinterpret_cast<const double2*>(grad_w), grad_lambda, n, D,
+                       reinterpret_cast<double2*>(grad_a), reinterpret_cast<double2*>(grad_b), warps);
 }
 
 int pbb_mvdr_backward(const void* atf, const void* noise_psd, const void* x, const void* w, const void* grad_w, int n,
@@ -367,20 +317,13 @@ int pbb_mvdr_backward(const void* atf, const void* noise_psd, const void* x, con
   const double2* G = reinterpret_cast<const double2*>(grad_w);
   double2* q = reinterpret_cast<double2*>(grad_atf);  // overwritten by the last kernel
   double2* p = reinterpret_cast<double2*>(scratch);
-  {
-    LaunchScope ls("mvdr_backward_rhs_kernel", st);
-    mvdr_backward_rhs_kernel<<<blocks_for(n, 128), 128, 0, st>>>(reinterpret_cast<const double2*>(atf), X, W, G, n,
-                                                                  D, q);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("mvdr_backward_rhs_kernel", mvdr_backward_rhs_kernel, blocks_for(n, 128), 128, 0, st,
+                        reinterpret_cast<const double2*>(atf), X, W, G, n, D, q));
   // p = N_h^-1 q; a zero pivot (the forward's minimum-norm branch, no derivative) or non-finite N gives NaN
   const int rc = solve_launch(noise_psd, q, n, D, 1, 1, p, nullptr, 2, st);
   if (rc) return rc;
-  LaunchScope ls("mvdr_backward_kernel", st);
-  mvdr_backward_kernel<<<blocks_for((size_t)n * D * D, 128), 128, 0, st>>>(
-      p, X, W, G, n, D, reinterpret_cast<double2*>(grad_atf), reinterpret_cast<double2*>(grad_noise_psd));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("mvdr_backward_kernel", mvdr_backward_kernel, blocks_for((size_t)n * D * D, 128), 128, 0, st, p,
+                       X, W, G, n, D, reinterpret_cast<double2*>(grad_atf), reinterpret_cast<double2*>(grad_noise_psd));
 }
 
 constexpr int kBanBackwardMaxD = 1024;
@@ -394,13 +337,10 @@ int pbb_blind_analytic_normalization_backward(const void* vector, const void* no
   const int warps = 4;
   const size_t smem = (size_t)warps * 2 * D * sizeof(double2);
   PBB_CUDA(cudaFuncSetAttribute(ban_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchScope ls("ban_backward_kernel", st);
-  ban_backward_kernel<<<(n + warps - 1) / warps, 32 * warps, smem, st>>>(
-      reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(noise_psd),
-      reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_vector),
-      reinterpret_cast<double2*>(grad_noise_psd), warps);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("ban_backward_kernel", ban_backward_kernel, (n + warps - 1) / warps, 32 * warps, smem, st,
+                       reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(noise_psd),
+                       reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_vector),
+                       reinterpret_cast<double2*>(grad_noise_psd), warps);
 }
 
 int pbb_rank_one_estimate_backward(const void* vector, const void* covariance, const void* grad_out, int n, int D,
@@ -409,14 +349,10 @@ int pbb_rank_one_estimate_backward(const void* vector, const void* covariance, c
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
   PBB_CHECK_ARG(grad_vector && grad_covariance, 6, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("rank_one_backward_kernel", st);
-  rank_one_backward_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(vector),
-                                             reinterpret_cast<const double2*>(covariance),
-                                             reinterpret_cast<const double2*>(grad_out), n, D,
-                                             reinterpret_cast<double2*>(grad_vector),
-                                             reinterpret_cast<double2*>(grad_covariance));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("rank_one_backward_kernel", rank_one_backward_kernel, n, 64, 0, st,
+                       reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(covariance),
+                       reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_vector),
+                       reinterpret_cast<double2*>(grad_covariance));
 }
 
 int pbb_matvec_batched_backward(const void* matrix, const void* vector, const void* grad_out, int n, int D,
@@ -425,13 +361,10 @@ int pbb_matvec_batched_backward(const void* matrix, const void* vector, const vo
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
   PBB_CHECK_ARG(grad_matrix && grad_vector, 6, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("matvec_backward_kernel", st);
-  matvec_backward_kernel<<<blocks_for((size_t)n * D, 128), 128, 0, st>>>(
-      reinterpret_cast<const double2*>(matrix), reinterpret_cast<const double2*>(vector),
-      reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_matrix),
-      reinterpret_cast<double2*>(grad_vector));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("matvec_backward_kernel", matvec_backward_kernel, blocks_for((size_t)n * D, 128), 128, 0, st,
+                       reinterpret_cast<const double2*>(matrix), reinterpret_cast<const double2*>(vector),
+                       reinterpret_cast<const double2*>(grad_out), n, D, reinterpret_cast<double2*>(grad_matrix),
+                       reinterpret_cast<double2*>(grad_vector));
 }
 
 static int apply_bf_backward_launch(const void* vector, const void* mix, int dtype, int B, int F, int D, int T,
@@ -443,21 +376,18 @@ static int apply_bf_backward_launch(const void* vector, const void* mix, int dty
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const double2* g = reinterpret_cast<const double2*>(grad_out);
   if (grad_vector) {
-    LaunchScope ls("apply_bf_vector_backward_kernel", st);
     const unsigned blocks = blocks_for((size_t)B * F * D * 32, 256);
-    if (dtype == PBB_C128)
-      apply_bf_vector_backward_kernel<double2><<<blocks, 256, 0, st>>>(
-          reinterpret_cast<const double2*>(mix), g, B, F, D, T, reinterpret_cast<double2*>(grad_vector));
-    else
-      apply_bf_vector_backward_kernel<float2><<<blocks, 256, 0, st>>>(
-          reinterpret_cast<const float2*>(mix), g, B, F, D, T, reinterpret_cast<double2*>(grad_vector));
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(with_ct(dtype, [&](auto ct) {
+      using CT = decltype(ct);
+      return launch_kernel("apply_bf_vector_backward_kernel", apply_bf_vector_backward_kernel<CT>, blocks, 256, 0, st,
+                           reinterpret_cast<const CT*>(mix), g, B, F, D, T, reinterpret_cast<double2*>(grad_vector));
+    }));
   }
   if (grad_mix) {
-    LaunchScope ls("apply_bf_mix_backward_kernel", st);
-    apply_bf_mix_backward_kernel<<<dim3((T + 255) / 256, F < 65535 ? F : 65535), 256, 0, st>>>(
-        reinterpret_cast<const double2*>(vector), g, B, F, D, T, reinterpret_cast<double2*>(grad_mix));
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("apply_bf_mix_backward_kernel", apply_bf_mix_backward_kernel,
+                          dim3((T + 255) / 256, F < 65535 ? F : 65535), 256, 0, st,
+                          reinterpret_cast<const double2*>(vector), g, B, F, D, T,
+                          reinterpret_cast<double2*>(grad_mix)));
   }
   return 0;
 }
@@ -493,27 +423,17 @@ int pbb_lcmv(const void* atf, const void* response, const void* noise_psd, int K
   double2* y = rhs + (size_t)F * K;
   int* fallback = reinterpret_cast<int*>(y + (size_t)F * K);
   PBB_CUDA(cudaMemsetAsync(fallback, 0, sizeof(int), st));
-  {
-    LaunchScope ls("lcmv_rhs_kernel", st);
-    lcmv_rhs_kernel<<<blocks_for((size_t)K * F * D, 256), 256, 0, st>>>(reinterpret_cast<const double2*>(atf), K, F,
-                                                                        D, H);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("lcmv_rhs_kernel", lcmv_rhs_kernel, blocks_for((size_t)K * F * D, 256), 256, 0, st,
+                        reinterpret_cast<const double2*>(atf), K, F, D, H));
   int r = solve_launch(noise_psd, H, F, D, K, 0, X, status, 0, st);  // Phi_N X = H, stable_solve (:432-435)
   if (r) return r;
-  {
-    LaunchScope ls("lcmv_gram_kernel", st);
-    lcmv_gram_kernel<<<blocks_for((size_t)F * K * K, 128), 128, 0, st>>>(
-        reinterpret_cast<const double2*>(atf), X, reinterpret_cast<const double2*>(response), K, F, D, G, rhs);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("lcmv_gram_kernel", lcmv_gram_kernel, blocks_for((size_t)F * K * K, 128), 128, 0, st,
+                        reinterpret_cast<const double2*>(atf), X, reinterpret_cast<const double2*>(response), K, F, D,
+                        G, rhs));
   r = solve_launch(G, rhs, F, K, 1, 0, y, status, 0, st, fallback);  // (H^H Phi_N^-1 H) y = r (:446-449)
   if (r) return r;
-  LaunchScope ls("lcmv_combine_kernel", st);
-  lcmv_combine_kernel<<<blocks_for((size_t)F * D, 128), 128, 0, st>>>(X, y, fallback, K, F, D,
-                                                                      reinterpret_cast<double2*>(w));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("lcmv_combine_kernel", lcmv_combine_kernel, blocks_for((size_t)F * D, 128), 128, 0, st, X, y,
+                       fallback, K, F, D, reinterpret_cast<double2*>(w));
 }
 
 int pbb_wmwf(const void* target_psd, const void* noise_psd, int n, int D, int frequency_dependent,
@@ -527,12 +447,9 @@ int pbb_wmwf(const void* target_psd, const void* noise_psd, int n, int D, int fr
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int r = solve_launch(noise_psd, target_psd, n, D, D, 0, scratch, status, 0, st);  // phi, stable_solve (:735)
   if (r) return r;
-  LaunchScope ls("wmwf_filter_kernel", st);
-  wmwf_filter_kernel<<<blocks_for((size_t)n * D * D, 256), 256, 0, st>>>(
-      reinterpret_cast<const double2*>(scratch), reinterpret_cast<const double2*>(target_psd), n, D,
-      frequency_dependent, distortion_weight, reinterpret_cast<double2*>(filter));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("wmwf_filter_kernel", wmwf_filter_kernel, blocks_for((size_t)n * D * D, 256), 256, 0, st,
+                       reinterpret_cast<const double2*>(scratch), reinterpret_cast<const double2*>(target_psd), n, D,
+                       frequency_dependent, distortion_weight, reinterpret_cast<double2*>(filter));
 }
 
 int pbb_weighted_channel_sum(const void* filter, const void* weight, int n, int D, void* out, void* stream) {
@@ -541,12 +458,9 @@ int pbb_weighted_channel_sum(const void* filter, const void* weight, int n, int 
   PBB_CHECK_ARG(n > 0 && D > 0, 3, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 5, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("weighted_channel_sum_kernel", st);
-  weighted_channel_sum_kernel<<<blocks_for((size_t)n * D, 256), 256, 0, st>>>(
-      reinterpret_cast<const double2*>(filter), reinterpret_cast<const double2*>(weight), n, D,
-      reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("weighted_channel_sum_kernel", weighted_channel_sum_kernel, blocks_for((size_t)n * D, 256), 256,
+                       0, st, reinterpret_cast<const double2*>(filter), reinterpret_cast<const double2*>(weight), n, D,
+                       reinterpret_cast<double2*>(out));
 }
 
 int pbb_reference_channel_snr(const void* w_mat, const void* target_psd, const void* noise_psd, int n, int D,
@@ -555,19 +469,14 @@ int pbb_reference_channel_snr(const void* w_mat, const void* target_psd, const v
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
   PBB_CHECK_ARG(num && den && num_sum && den_sum, 6, "output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  {
-    LaunchScope ls("reference_snr_kernel", st);
-    reference_snr_kernel<<<n, 64, 0, st>>>(reinterpret_cast<const double2*>(w_mat),
-                                           reinterpret_cast<const double2*>(target_psd),
-                                           reinterpret_cast<const double2*>(noise_psd), n, D,
-                                           reinterpret_cast<double2*>(num), reinterpret_cast<double2*>(den));
-    PBB_CUDA(cudaGetLastError());
-  }
-  LaunchScope ls("colsum_kernel", st);
-  colsum_kernel<<<1, 128, 0, st>>>(reinterpret_cast<const double*>(num), reinterpret_cast<double*>(num_sum), n, 2 * D);
-  colsum_kernel<<<1, 128, 0, st>>>(reinterpret_cast<const double*>(den), reinterpret_cast<double*>(den_sum), n, 2 * D);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("reference_snr_kernel", reference_snr_kernel, n, 64, 0, st,
+                        reinterpret_cast<const double2*>(w_mat), reinterpret_cast<const double2*>(target_psd),
+                        reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(num),
+                        reinterpret_cast<double2*>(den)));
+  PBB_TRY(launch_kernel("colsum_kernel", colsum_kernel, 1, 128, 0, st, reinterpret_cast<const double*>(num),
+                        reinterpret_cast<double*>(num_sum), n, 2 * D));
+  return launch_kernel("colsum_kernel", colsum_kernel, 1, 128, 0, st, reinterpret_cast<const double*>(den),
+                       reinterpret_cast<double*>(den_sum), n, 2 * D);
 }
 
 int pbb_mvdr_merl(const void* target_psd, const void* noise_psd, int n, int D, void* w, void* scratch, int* status,
@@ -582,11 +491,8 @@ int pbb_mvdr_merl(const void* target_psd, const void* noise_psd, int n, int D, v
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   int r = solve_launch(noise_psd, target_psd, n, D, D, 0, scratch, status, 1, st);  // np.linalg.solve (:277)
   if (r) return r;
-  LaunchScope ls("merl_kernel", st);
-  merl_kernel<<<blocks_for(n, 128), 128, 0, st>>>(reinterpret_cast<const double2*>(scratch), n, D,
-                                                  reinterpret_cast<double2*>(w));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("merl_kernel", merl_kernel, blocks_for(n, 128), 128, 0, st,
+                       reinterpret_cast<const double2*>(scratch), n, D, reinterpret_cast<double2*>(w));
 }
 
 int pbb_condition_covariance(const void* x, int n, int D, double gamma, void* out, void* stream) {
@@ -594,11 +500,8 @@ int pbb_condition_covariance(const void* x, int n, int D, double gamma, void* ou
   PBB_CHECK_ARG(n > 0 && D > 0, 2, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 5, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("condition_covariance_kernel", st);
-  condition_covariance_kernel<<<blocks_for((size_t)n * D * D, 256), 256, 0, st>>>(
-      reinterpret_cast<const double2*>(x), n, D, gamma, reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("condition_covariance_kernel", condition_covariance_kernel, blocks_for((size_t)n * D * D, 256),
+                       256, 0, st, reinterpret_cast<const double2*>(x), n, D, gamma, reinterpret_cast<double2*>(out));
 }
 
 int pbb_distortionless_normalization(const void* vector, const void* atf, const void* noise_psd, int n, int D,
@@ -607,12 +510,9 @@ int pbb_distortionless_normalization(const void* vector, const void* atf, const 
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 6, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("distortionless_kernel", st);
-  distortionless_kernel<<<blocks_for(n, 128), 128, 0, st>>>(
-      reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(atf),
-      reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("distortionless_kernel", distortionless_kernel, blocks_for(n, 128), 128, 0, st,
+                       reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(atf),
+                       reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
 }
 
 int pbb_mvdr_snr_postfilter(const void* vector, const void* target_psd, const void* noise_psd, int n, int D,
@@ -621,12 +521,9 @@ int pbb_mvdr_snr_postfilter(const void* vector, const void* target_psd, const vo
   PBB_CHECK_ARG(n > 0 && D > 0 && D <= 64, 4, "bad shape");
   PBB_CHECK_ARG(out != nullptr, 6, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("snr_postfilter_kernel", st);
-  snr_postfilter_kernel<<<blocks_for(n, 128), 128, 0, st>>>(
-      reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(target_psd),
-      reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("snr_postfilter_kernel", snr_postfilter_kernel, blocks_for(n, 128), 128, 0, st,
+                       reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(target_psd),
+                       reinterpret_cast<const double2*>(noise_psd), n, D, reinterpret_cast<double2*>(out));
 }
 
 int pbb_zero_degree_normalization(const void* vector, int n, int D, int reference_channel, void* out, void* stream) {
@@ -635,12 +532,9 @@ int pbb_zero_degree_normalization(const void* vector, int n, int D, int referenc
   PBB_CHECK_ARG(reference_channel >= 0 && reference_channel < D, 4, "need 0 <= reference_channel < D");
   PBB_CHECK_ARG(out != nullptr, 5, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("zero_degree_kernel", st);
-  zero_degree_kernel<<<blocks_for((size_t)n * D, 256), 256, 0, st>>>(reinterpret_cast<const double2*>(vector), n, D,
-                                                                      reference_channel,
-                                                                      reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("zero_degree_kernel", zero_degree_kernel, blocks_for((size_t)n * D, 256), 256, 0, st,
+                       reinterpret_cast<const double2*>(vector), n, D, reference_channel,
+                       reinterpret_cast<double2*>(out));
 }
 
 int pbb_phase_correction(const void* vector, int A, int M, int F, int D, int scan_bins, void* out, void* stream) {
@@ -650,12 +544,10 @@ int pbb_phase_correction(const void* vector, int A, int M, int F, int D, int sca
   PBB_CHECK_ARG(out != nullptr, 7, "out is null");
   PBB_CHECK_ARG(out != vector, 7, "out must not alias vector");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("phase_correction_kernel", st);
   const size_t threads = scan_bins ? 1 : (size_t)M * F;
-  phase_correction_kernel<<<blocks_for(threads, 128), 128, 0, st>>>(reinterpret_cast<const double2*>(vector), A, M, F,
-                                                                    D, scan_bins, reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("phase_correction_kernel", phase_correction_kernel, blocks_for(threads, 128), 128, 0, st,
+                       reinterpret_cast<const double2*>(vector), A, M, F, D, scan_bins,
+                       reinterpret_cast<double2*>(out));
 }
 
 int pbb_apply_online_beamforming_vector(const void* vector, const void* mix, int dtype, int B, int F, int D, int T,
@@ -670,17 +562,13 @@ int pbb_apply_online_beamforming_vector(const void* vector, const void* mix, int
   PBB_CHECK_ARG(out != nullptr, 12, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   dim3 grid((T + 127) / 128, F);
-  LaunchScope ls("apply_online_kernel", st);
-  if (dtype == PBB_C128)
-    apply_online_kernel<double2><<<grid, 128, 0, st>>>(
-        reinterpret_cast<const double2*>(vector), reinterpret_cast<const double2*>(mix), B, F, D, T,
-        vector_frame_stride, vector_bin_stride, mix_batch_stride, mix_bin_stride, reinterpret_cast<double2*>(out));
-  else
-    apply_online_kernel<float2><<<grid, 128, 0, st>>>(
-        reinterpret_cast<const double2*>(vector), reinterpret_cast<const float2*>(mix), B, F, D, T,
-        vector_frame_stride, vector_bin_stride, mix_batch_stride, mix_bin_stride, reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_kernel("apply_online_kernel", apply_online_kernel<CT>, grid, 128, 0, st,
+                         reinterpret_cast<const double2*>(vector), reinterpret_cast<const CT*>(mix), B, F, D, T,
+                         vector_frame_stride, vector_bin_stride, mix_batch_stride, mix_bin_stride,
+                         reinterpret_cast<double2*>(out));
+  });
 }
 
 // ---- single distributions of pb_bss/distribution (csrc/distribution.cuh) -----------------------------------------
@@ -697,12 +585,9 @@ int pbb_cacg_from_covariance(const void* covariance, int n, int D, int covarianc
   const int warps = warps_for(per);
   if (status) PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
   PBB_CUDA(cudaFuncSetAttribute(cacg_from_covariance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  LaunchScope ls("cacg_from_covariance_kernel", st);
-  cacg_from_covariance_kernel<<<(n + warps - 1) / warps, 32 * warps, per * warps, st>>>(
-      reinterpret_cast<const double2*>(covariance), n, D, covariance_norm, eigenvalue_floor,
-      reinterpret_cast<double2*>(eigenvectors), eigenvalues, status, warps);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("cacg_from_covariance_kernel", cacg_from_covariance_kernel, (n + warps - 1) / warps, 32 * warps,
+                       per * warps, st, reinterpret_cast<const double2*>(covariance), n, D, covariance_norm,
+                       eigenvalue_floor, reinterpret_cast<double2*>(eigenvectors), eigenvalues, status, warps);
 }
 
 int pbb_cw_log_norm(const double* kappa, long long n, int D, int variant, double* log_norm, void* stream) {
@@ -712,10 +597,8 @@ int pbb_cw_log_norm(const double* kappa, long long n, int D, int variant, double
   PBB_CHECK_ARG(variant >= PBB_CW_NORM_1F1 && variant <= PBB_CW_NORM_TRAN_VU, 4, "bad variant");
   PBB_CHECK_ARG(log_norm != nullptr, 5, "log_norm is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("cw_log_norm_kernel", st);
-  cw_log_norm_kernel<<<blocks_for((size_t)n, 256), 256, 0, st>>>(kappa, n, D, variant, log_norm);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("cw_log_norm_kernel", cw_log_norm_kernel, blocks_for((size_t)n, 256), 256, 0, st, kappa, n, D,
+                       variant, log_norm);
 }
 
 int pbb_cw_log_pdf(const void* y, int dtype, long long y_stride, int M, int N, int D, const void* mode,
@@ -728,15 +611,11 @@ int pbb_cw_log_pdf(const void* y, int dtype, long long y_stride, int M, int N, i
   PBB_CHECK_ARG(log_pdf != nullptr, 9, "log_pdf is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const dim3 grid(blocks_for((size_t)N, 256), std::min(M, kDistMaxGridY));
-  LaunchScope ls("cw_log_pdf_kernel", st);
-  if (dtype == PBB_C128)
-    cw_log_pdf_kernel<double2><<<grid, 256, 0, st>>>(reinterpret_cast<const double2*>(y), y_stride, M, N, D,
-                                                     reinterpret_cast<const double2*>(mode), concentration, log_pdf);
-  else
-    cw_log_pdf_kernel<float2><<<grid, 256, 0, st>>>(reinterpret_cast<const float2*>(y), y_stride, M, N, D,
-                                                    reinterpret_cast<const double2*>(mode), concentration, log_pdf);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_kernel("cw_log_pdf_kernel", cw_log_pdf_kernel<CT>, grid, 256, 0, st, reinterpret_cast<const CT*>(y),
+                         y_stride, M, N, D, reinterpret_cast<const double2*>(mode), concentration, log_pdf);
+  });
 }
 
 // workspace of pbb_ccsg_log_pdf (LU (M, D, D) | perm (M, D) | logdet (M)) and of pbb_ccsg_sample (L (M, D, D))
@@ -769,26 +648,16 @@ int pbb_ccsg_log_pdf(const void* y, int dtype, long long y_stride, int M, int N,
   const int warps = warps_for(lu_per_warp);
   const size_t lu_smem = (size_t)warps * lu_per_warp;
   PBB_CUDA(cudaFuncSetAttribute(ccsg_lu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-  {
-    LaunchScope ls("ccsg_lu_kernel", st);
-    ccsg_lu_kernel<<<(M + warps - 1) / warps, 32 * warps, lu_smem, st>>>(
-        reinterpret_cast<const double2*>(covariance), M, D, lu, perm, logdet, status, warps);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("ccsg_lu_kernel", ccsg_lu_kernel, (M + warps - 1) / warps, 32 * warps, lu_smem, st,
+                        reinterpret_cast<const double2*>(covariance), M, D, lu, perm, logdet, status, warps));
   const size_t smem = ccsg_log_pdf_smem(D);
   const dim3 grid(blocks_for((size_t)N, kCcsgThreads), std::min(M, kDistMaxGridY));
-  LaunchScope ls("ccsg_log_pdf_kernel", st);
-  if (dtype == PBB_C128) {
-    PBB_CUDA(cudaFuncSetAttribute(ccsg_log_pdf_kernel<double2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    ccsg_log_pdf_kernel<double2><<<grid, kCcsgThreads, smem, st>>>(reinterpret_cast<const double2*>(y), y_stride, M,
-                                                                   N, D, lu, perm, logdet, log_pdf);
-  } else {
-    PBB_CUDA(cudaFuncSetAttribute(ccsg_log_pdf_kernel<float2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    ccsg_log_pdf_kernel<float2><<<grid, kCcsgThreads, smem, st>>>(reinterpret_cast<const float2*>(y), y_stride, M,
-                                                                  N, D, lu, perm, logdet, log_pdf);
-  }
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    PBB_CUDA(cudaFuncSetAttribute(ccsg_log_pdf_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    return launch_kernel("ccsg_log_pdf_kernel", ccsg_log_pdf_kernel<CT>, grid, kCcsgThreads, smem, st,
+                         reinterpret_cast<const CT*>(y), y_stride, M, N, D, lu, perm, logdet, log_pdf);
+  });
 }
 
 int pbb_ccsg_sample(const void* a, const double* eigenvalues, int C, int D, const double* normals,
@@ -806,19 +675,13 @@ int pbb_ccsg_sample(const void* a, const double* eigenvalues, int C, int D, cons
   PBB_CUDA(cudaMemsetAsync(status, 0, sizeof(int), st));
   const size_t chol_per_warp = (size_t)D * D * sizeof(double2);
   const int warps = warps_for(chol_per_warp);
-  {
-    LaunchScope ls("ccsg_cholesky_kernel", st);
-    PBB_CUDA(cudaFuncSetAttribute(ccsg_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
-    ccsg_cholesky_kernel<<<(C + warps - 1) / warps, 32 * warps, (size_t)warps * chol_per_warp, st>>>(
-        reinterpret_cast<const double2*>(a), eigenvalues, C, D, L, status, warps);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_CUDA(cudaFuncSetAttribute(ccsg_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  PBB_TRY(launch_kernel("ccsg_cholesky_kernel", ccsg_cholesky_kernel, (C + warps - 1) / warps, 32 * warps,
+                        (size_t)warps * chol_per_warp, st, reinterpret_cast<const double2*>(a), eigenvalues, C, D, L,
+                        status, warps));
   if (S == 0) return 0;
-  LaunchScope ls("ccsg_sample_kernel", st);
-  ccsg_sample_kernel<<<blocks_for((size_t)S, 128), 128, 0, st>>>(L, C, D, normals, offsets, dest, S, unit_norm,
-                                                                reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("ccsg_sample_kernel", ccsg_sample_kernel, blocks_for((size_t)S, 128), 128, 0, st, L, C, D,
+                       normals, offsets, dest, S, unit_norm, reinterpret_cast<double2*>(out));
 }
 
 int pbb_ccsg_fit(const void* observation, int dtype, int F, int D, int N, const double* saliency,
@@ -827,11 +690,8 @@ int pbb_ccsg_fit(const void* observation, int dtype, int F, int D, int N, const 
                                      workspace_bytes, stream);
   if (r || saliency == nullptr) return r;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("ccsg_fit_scale_kernel", st);
-  ccsg_fit_scale_kernel<<<F, 256, 0, st>>>(saliency, N, D, denominator_floor,
-                                           reinterpret_cast<double2*>(covariance));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("ccsg_fit_scale_kernel", ccsg_fit_scale_kernel, F, 256, 0, st, saliency, N, D, denominator_floor,
+                       reinterpret_cast<double2*>(covariance));
 }
 
 }  // extern "C"

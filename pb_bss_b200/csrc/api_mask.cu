@@ -29,14 +29,14 @@ static bool dtype_ok(int dtype) {
   return dtype == PBB_C64 || dtype == PBB_C128 || dtype == PBB_F32 || dtype == PBB_F64;
 }
 
-// calls fn(TI*) with the signal pointer cast to its element type
+// returns fn(TI*) with the signal pointer cast to its element type
 template <class Fn>
-static void with_input(int dtype, const void* p, Fn&& fn) {
+static int with_input(int dtype, const void* p, Fn&& fn) {
   switch (dtype) {
-    case PBB_C128: fn(reinterpret_cast<const double2*>(p)); break;
-    case PBB_C64: fn(reinterpret_cast<const float2*>(p)); break;
-    case PBB_F64: fn(reinterpret_cast<const double*>(p)); break;
-    default: fn(reinterpret_cast<const float*>(p)); break;
+    case PBB_C128: return fn(reinterpret_cast<const double2*>(p));
+    case PBB_C64: return fn(reinterpret_cast<const float2*>(p));
+    case PBB_F64: return fn(reinterpret_cast<const double*>(p));
+    default: return fn(reinterpret_cast<const float*>(p));
   }
 }
 
@@ -60,11 +60,8 @@ static int row_select_launch(const TI* x, int D, long long sD, const pbb_mask_la
     const size_t smem = (size_t)R * n * sizeof(double) + R * sizeof(double) + (size_t)kSelWarps * kSelHistBytes;
     PBB_CUDA(cudaFuncSetAttribute(row_select_short_kernel<TI, TO>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   (int)smem));
-    LaunchScope ls("row_select_short_kernel", st);
-    row_select_short_kernel<TI, TO><<<(unsigned)((nrows + R - 1) / R), kSelWarps * 32, smem, st>>>(
-        x, D, sD, *rows, nrows, *elems, (int)n, R, rowfast, p, out, status);
-    PBB_CUDA(cudaGetLastError());
-    return 0;
+    return launch_kernel("row_select_short_kernel", row_select_short_kernel<TI, TO>, (unsigned)((nrows + R - 1) / R),
+                         kSelWarps * 32, smem, st, x, D, sD, *rows, nrows, *elems, (int)n, R, rowfast, p, out, status);
   }
   if (scratch == nullptr || scratch_bytes < pbb_row_select_scratch_bytes(nrows, n)) {
     set_error("argument: scratch too small for rows of %lld elements (pbb_row_select_scratch_bytes)", n);
@@ -80,30 +77,21 @@ static int row_select_launch(const TI* x, int D, long long sD, const pbb_mask_la
   if (chunks < 1) chunks = 1;
   // the row is blockIdx.x / chunks: rows < 2^31 and chunks * rows <= rows + 263, so the grid never exceeds grid.x
   const unsigned grid = (unsigned)(chunks * nrows);
-  row_state_init_kernel<<<grid_for(nrows, 128), 128, 0, st>>>(nrows, n, p, state);
-  PBB_CUDA(cudaGetLastError());
-  {
-    LaunchScope ls("row_gather_kernel", st);
-    row_gather_kernel<TI><<<grid, 256, 0, st>>>(x, D, sD, *rows, *elems, n, (int)chunks, p, vals, state);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("row_state_init_kernel", row_state_init_kernel, grid_for(nrows, 128), 128, 0, st, nrows, n, p,
+                        state));
+  PBB_TRY(launch_kernel("row_gather_kernel", row_gather_kernel<TI>, grid, 256, 0, st, x, D, sD, *rows, *elems, n,
+                        (int)chunks, p, vals, state));
   const int queries = p.lorenz ? 1 : 2;
   for (int q = 0; q < queries; ++q) {
     for (int pass = 0; pass < kSelPasses; ++pass) {
-      {
-        LaunchScope ls("row_hist_kernel", st);
-        row_hist_kernel<<<grid, 256, 0, st>>>(vals, n, (int)chunks, pass, q, p.lorenz, state, hist);
-        PBB_CUDA(cudaGetLastError());
-      }
-      LaunchScope ls("row_decide_kernel", st);
-      row_decide_kernel<<<(unsigned)nrows, 32, 0, st>>>(n, pass, q, p, state, hist);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("row_hist_kernel", row_hist_kernel, grid, 256, 0, st, vals, n, (int)chunks, pass, q,
+                            p.lorenz, state, hist));
+      PBB_TRY(launch_kernel("row_decide_kernel", row_decide_kernel, (unsigned)nrows, 32, 0, st, n, pass, q, p, state,
+                            hist));
     }
   }
-  LaunchScope ls("row_apply_kernel", st);
-  row_apply_kernel<TO><<<grid, 256, 0, st>>>(vals, *rows, *elems, n, (int)chunks, p, state, out, status);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("row_apply_kernel", row_apply_kernel<TO>, grid, 256, 0, st, vals, *rows, *elems, n, (int)chunks,
+                       p, state, out, status);
 }
 
 template <class TI>
@@ -137,29 +125,25 @@ int pbb_source_mask(const void* signal, int dtype, int kind, int K, int D, long 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long n = layout_count(rest);
   const unsigned grid = grid_for(n, 256);
-  LaunchScope ls("source_mask_kernel", st);
-  with_input(dtype, signal, [&](auto x) {
+  return with_input(dtype, signal, [&](auto x) {
     using TI = std::remove_const_t<std::remove_pointer_t<decltype(x)>>;
     const bool complex_out = kind == PBB_MASK_IDEAL_COMPLEX && IsComplex<TI>::value;
     if (complex_out && is32(dtype))
-      source_mask_kernel<TI, float2><<<grid, 256, 0, st>>>(x, kind, K, D, source_stride, sensor_stride,
-                                                           out_source_stride, *rest, n, eps,
-                                                           reinterpret_cast<float2*>(out));
-    else if (complex_out)
-      source_mask_kernel<TI, double2><<<grid, 256, 0, st>>>(x, kind, K, D, source_stride, sensor_stride,
-                                                            out_source_stride, *rest, n, eps,
-                                                            reinterpret_cast<double2*>(out));
-    else if (is32(dtype))
-      source_mask_kernel<TI, float><<<grid, 256, 0, st>>>(x, kind, K, D, source_stride, sensor_stride,
-                                                          out_source_stride, *rest, n, eps,
-                                                          reinterpret_cast<float*>(out));
-    else
-      source_mask_kernel<TI, double><<<grid, 256, 0, st>>>(x, kind, K, D, source_stride, sensor_stride,
-                                                           out_source_stride, *rest, n, eps,
-                                                           reinterpret_cast<double*>(out));
+      return launch_kernel("source_mask_kernel", source_mask_kernel<TI, float2>, grid, 256, 0, st, x, kind, K, D,
+                           source_stride, sensor_stride, out_source_stride, *rest, n, eps,
+                           reinterpret_cast<float2*>(out));
+    if (complex_out)
+      return launch_kernel("source_mask_kernel", source_mask_kernel<TI, double2>, grid, 256, 0, st, x, kind, K, D,
+                           source_stride, sensor_stride, out_source_stride, *rest, n, eps,
+                           reinterpret_cast<double2*>(out));
+    if (is32(dtype))
+      return launch_kernel("source_mask_kernel", source_mask_kernel<TI, float>, grid, 256, 0, st, x, kind, K, D,
+                           source_stride, sensor_stride, out_source_stride, *rest, n, eps,
+                           reinterpret_cast<float*>(out));
+    return launch_kernel("source_mask_kernel", source_mask_kernel<TI, double>, grid, 256, 0, st, x, kind, K, D,
+                         source_stride, sensor_stride, out_source_stride, *rest, n, eps,
+                         reinterpret_cast<double*>(out));
   });
-  PBB_CUDA(cudaGetLastError());
-  return 0;
 }
 
 size_t pbb_row_select_scratch_bytes(long long rows, long long n) {
@@ -183,9 +167,8 @@ int pbb_lorenz_mask(const void* signal, int dtype, int D, long long sensor_strid
   p.mask_low = mask_low;
   p.mask_high = mask_high;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = 0;
-  with_input(dtype, signal, [&](auto x) {
-    rc = row_select_dispatch(dtype, x, D, sensor_stride, rows, elems, p, out, scratch, scratch_bytes, status, st);
+  const int rc = with_input(dtype, signal, [&](auto x) {
+    return row_select_dispatch(dtype, x, D, sensor_stride, rows, elems, p, out, scratch, scratch_bytes, status, st);
   });
   if (rc == -1) return -11;
   return rc;
@@ -214,9 +197,8 @@ int pbb_quantile_mask(const void* signal, int dtype, const pbb_mask_layout* rows
   p.mask_low = mask_low;
   p.mask_high = mask_high;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  int rc = 0;
-  with_input(dtype, signal, [&](auto x) {
-    rc = row_select_dispatch(dtype, x, 1, 0, rows, elems, p, out, scratch, scratch_bytes, nullptr, st);
+  const int rc = with_input(dtype, signal, [&](auto x) {
+    return row_select_dispatch(dtype, x, 1, 0, rows, elems, p, out, scratch, scratch_bytes, nullptr, st);
   });
   if (rc == -1) return -13;
   return rc;
@@ -233,15 +215,12 @@ int pbb_biased_binary_mask(const void* signal, int dtype, long long component_st
   PBB_CHECK_ARG(out != nullptr, 10, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long n = layout_count(rest);
-  LaunchScope ls("biased_binary_kernel", st);
-  with_input(dtype, signal, [&](auto x) {
+  return with_input(dtype, signal, [&](auto x) {
     using TI = std::remove_const_t<std::remove_pointer_t<decltype(x)>>;
-    biased_binary_kernel<TI><<<grid_for(n, 256), 256, 0, st>>>(x, component_stride, out_component_stride, *rest, n, L,
-                                                               speech_div, noise_div, force,
-                                                               reinterpret_cast<unsigned char*>(out));
+    return launch_kernel("biased_binary_kernel", biased_binary_kernel<TI>, grid_for(n, 256), 256, 0, st, x,
+                         component_stride, out_component_stride, *rest, n, L, speech_div, noise_div, force,
+                         reinterpret_cast<unsigned char*>(out));
   });
-  PBB_CUDA(cudaGetLastError());
-  return 0;
 }
 
 int pbb_steering_vector(const double* tdoa, int A, int M, const double* freq, int F, int normalize, void* out,
@@ -252,11 +231,8 @@ int pbb_steering_vector(const double* tdoa, int A, int M, const double* freq, in
   PBB_CHECK_ARG(F > 0, 5, "F must be positive");
   PBB_CHECK_ARG(out != nullptr, 7, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("steering_vector_kernel", st);
-  steering_vector_kernel<<<grid_for((long long)A * F, 128), 128, 0, st>>>(tdoa, A, M, freq, F, normalize,
-                                                                          reinterpret_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("steering_vector_kernel", steering_vector_kernel, grid_for((long long)A * F, 128), 128, 0, st,
+                       tdoa, A, M, freq, F, normalize, reinterpret_cast<double2*>(out));
 }
 
 int pbb_diffuse_noise_coherence(const double* distances, int D, const double* freq, int F, double sound_velocity,
@@ -267,11 +243,8 @@ int pbb_diffuse_noise_coherence(const double* distances, int D, const double* fr
   PBB_CHECK_ARG(F > 0, 4, "F must be positive");
   PBB_CHECK_ARG(out != nullptr, 6, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("diffuse_coherence_kernel", st);
-  diffuse_coherence_kernel<<<grid_for((long long)F * D * D, 256), 256, 0, st>>>(distances, D, freq, F, sound_velocity,
-                                                                                out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("diffuse_coherence_kernel", diffuse_coherence_kernel, grid_for((long long)F * D * D, 256), 256,
+                       0, st, distances, D, freq, F, sound_velocity, out);
 }
 
 int pbb_array_geometry(int mode, const double* points, int S, const double* sensor, int M, int reference_channel,
@@ -284,11 +257,8 @@ int pbb_array_geometry(int mode, const double* points, int S, const double* sens
   PBB_CHECK_ARG(mode == 0 || (reference_channel >= 0 && reference_channel < M), 6, "reference_channel out of range");
   PBB_CHECK_ARG(out != nullptr, 8, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("array_geometry_kernel", st);
-  array_geometry_kernel<<<grid_for((long long)S * M, 128), 128, 0, st>>>(mode, points, S, sensor, M, reference_channel,
-                                                                         sound_velocity, out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("array_geometry_kernel", array_geometry_kernel, grid_for((long long)S * M, 128), 128, 0, st,
+                       mode, points, S, sensor, M, reference_channel, sound_velocity, out);
 }
 
 }  // extern "C"

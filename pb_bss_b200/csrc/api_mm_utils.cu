@@ -43,19 +43,12 @@ static int reduce_launch(const void* x, const double* mul, const pbb_nd_layout& 
   const long long len = red_chunk_len(outs, n), chunks = red_chunks(outs, n);
   const bool warp = len >= 32;
   const long long threads = outs * chunks * (warp ? 32 : 1);
-  LaunchScope ls(warp ? "reduce_kernel<warp>" : "reduce_kernel", st);
-  if (warp)
-    reduce_kernel<T, CPLX, TO, true><<<blocks_for(threads), kNdThreads, 0, st>>>(
-        static_cast<const T*>(x), mul, O, R, outs, n, len, chunks, op, partial, static_cast<TO*>(out));
-  else
-    reduce_kernel<T, CPLX, TO, false><<<blocks_for(threads), kNdThreads, 0, st>>>(
-        static_cast<const T*>(x), mul, O, R, outs, n, len, chunks, op, partial, static_cast<TO*>(out));
-  PBB_CUDA(cudaGetLastError());
-  if (chunks > 1) {
-    red_finish_kernel<TO><<<blocks_for(outs * 32), kNdThreads, 0, st>>>(partial, O, outs, chunks, op,
-                                                                        static_cast<TO*>(out));
-    PBB_CUDA(cudaGetLastError());
-  }
+  const auto kern = warp ? reduce_kernel<T, CPLX, TO, true> : reduce_kernel<T, CPLX, TO, false>;
+  PBB_TRY(launch_kernel(warp ? "reduce_kernel<warp>" : "reduce_kernel", kern, blocks_for(threads), kNdThreads, 0, st,
+                        static_cast<const T*>(x), mul, O, R, outs, n, len, chunks, op, partial, static_cast<TO*>(out)));
+  if (chunks > 1)
+    PBB_TRY(launch_kernel("red_finish_kernel", red_finish_kernel<TO>, blocks_for(outs * 32), kNdThreads, 0, st, partial,
+                          O, outs, chunks, op, static_cast<TO*>(out)));
   return 0;
 }
 
@@ -74,28 +67,20 @@ static int reduce_dispatch(const void* x, int dtype, const double* mul, const pb
 template <class T, bool CPLX>
 static int divide_launch(const void* x, const double* norm, const pbb_nd_layout& L, long long total, void* out,
                          cudaStream_t st) {
-  LaunchScope ls("scale_nd_kernel<divide>", st);
-  scale_nd_kernel<T, CPLX, true><<<blocks_for(total), kNdThreads, 0, st>>>(static_cast<const T*>(x), norm, L, total,
-                                                                           static_cast<T*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("scale_nd_kernel<divide>", scale_nd_kernel<T, CPLX, true>, blocks_for(total), kNdThreads, 0, st,
+                       static_cast<const T*>(x), norm, L, total, static_cast<T*>(out));
 }
 
 template <class T, bool CPLX>
 static int force_hermitian_launch(const void* a, long long total, int D, void* out, cudaStream_t st) {
-  LaunchScope ls("force_hermitian_kernel", st);
-  force_hermitian_kernel<T, CPLX><<<blocks_for(total), kNdThreads, 0, st>>>(static_cast<const T*>(a), total, D,
-                                                                            static_cast<T*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("force_hermitian_kernel", force_hermitian_kernel<T, CPLX>, blocks_for(total), kNdThreads, 0, st,
+                       static_cast<const T*>(a), total, D, static_cast<T*>(out));
 }
 
 template <class T, bool CPLX>
 static int abs_square_launch(const void* x, long long n, void* out, cudaStream_t st) {
-  LaunchScope ls("abs_square_kernel", st);
-  abs_square_kernel<T, CPLX><<<blocks_for(n), kNdThreads, 0, st>>>(static_cast<const T*>(x), n, static_cast<T*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("abs_square_kernel", abs_square_kernel<T, CPLX>, blocks_for(n), kNdThreads, 0, st,
+                       static_cast<const T*>(x), n, static_cast<T*>(out));
 }
 
 template <class E>
@@ -103,21 +88,15 @@ static int one_hot_launch(const long long* labels, long long outer, long long in
                           void* out, int* status, cudaStream_t st) {
   E v;
   std::memcpy(&v, one, sizeof(E));
-  LaunchScope ls("one_hot_kernel", st);
-  one_hot_kernel<E><<<blocks_for(outer * C * inner), kNdThreads, 0, st>>>(labels, outer, inner, C, v,
-                                                                          static_cast<E*>(out), status);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("one_hot_kernel", one_hot_kernel<E>, blocks_for(outer * C * inner), kNdThreads, 0, st, labels,
+                       outer, inner, C, v, static_cast<E*>(out), status);
 }
 
 template <class T, bool CPLX>
 static int scale_launch(const void* x, const double* f, const pbb_nd_layout& L, long long total, void* out,
                         cudaStream_t st) {
-  LaunchScope ls("scale_nd_kernel", st);
-  scale_nd_kernel<T, CPLX, false><<<blocks_for(total), kNdThreads, 0, st>>>(static_cast<const T*>(x), f, L, total,
-                                                                     static_cast<T*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("scale_nd_kernel", scale_nd_kernel<T, CPLX, false>, blocks_for(total), kNdThreads, 0, st,
+                       static_cast<const T*>(x), f, L, total, static_cast<T*>(out));
 }
 
 }  // namespace pbb
@@ -138,17 +117,13 @@ int pbb_affiliation_nd(const void* log_pdf, int dtype, const double* weight, con
   if (cols == 0 || K == 0) return 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const long long* cs = class_stride;
-  LaunchScope ls("affiliation_nd_kernel", st);
   if (dtype == PBB_F64)
-    affiliation_nd_kernel<double><<<blocks_for(cols), kNdThreads, 0, st>>>(
-        static_cast<const double*>(log_pdf), weight, mask, *columns, cols, K, cs[0], cs[1], cs[2], cs[3], DBL_MIN,
-        affiliation_eps, static_cast<double*>(out));
-  else
-    affiliation_nd_kernel<float><<<blocks_for(cols), kNdThreads, 0, st>>>(
-        static_cast<const float*>(log_pdf), weight, mask, *columns, cols, K, cs[0], cs[1], cs[2], cs[3],
-        (double)FLT_MIN, affiliation_eps, static_cast<float*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+    return launch_kernel("affiliation_nd_kernel", affiliation_nd_kernel<double>, blocks_for(cols), kNdThreads, 0, st,
+                         static_cast<const double*>(log_pdf), weight, mask, *columns, cols, K, cs[0], cs[1], cs[2],
+                         cs[3], DBL_MIN, affiliation_eps, static_cast<double*>(out));
+  return launch_kernel("affiliation_nd_kernel", affiliation_nd_kernel<float>, blocks_for(cols), kNdThreads, 0, st,
+                       static_cast<const float*>(log_pdf), weight, mask, *columns, cols, K, cs[0], cs[1], cs[2], cs[3],
+                       (double)FLT_MIN, affiliation_eps, static_cast<float*>(out));
 }
 
 size_t pbb_reduce_workspace_bytes(long long outs, long long n) {

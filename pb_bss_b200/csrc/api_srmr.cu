@@ -13,40 +13,19 @@ static int vad_tiles(long long N) { return (int)((N + kVadTile - 1) / kVadTile);
 template <class T>
 static int vad_launch(VadParams p, int normalise, cudaStream_t st) {
   const unsigned ctas = (unsigned)(p.rows * p.tiles), rows = (unsigned)p.rows;
-#define PBB_VAD_TILE(PH, NAME)                                                \
-  {                                                                           \
-    LaunchScope ls(NAME, st);                                                 \
-    vad_tile_kernel<T, PH><<<ctas, kVadThreads, 0, st>>>(p);                  \
-    PBB_CUDA(cudaGetLastError());                                             \
-  }
-#define PBB_VAD_NORM(PH, NAME)                                                \
-  {                                                                           \
-    LaunchScope ls(NAME, st);                                                 \
-    vad_norm_kernel<PH><<<ctas, kVadThreads, 0, st>>>(p);                     \
-    PBB_CUDA(cudaGetLastError());                                             \
-  }
-#define PBB_VAD_ROW(PH, NAME)                                                 \
-  {                                                                           \
-    LaunchScope ls(NAME, st);                                                 \
-    vad_row_kernel<T, PH><<<rows, kVadRowThreads, 0, st>>>(p);                \
-    PBB_CUDA(cudaGetLastError());                                             \
-  }
-  PBB_VAD_TILE(VAD_MAX, "srmr_vad_max_kernel")
-  PBB_VAD_ROW(ROW_THRESHOLD, "srmr_vad_threshold_kernel")
-  PBB_VAD_TILE(VAD_EDGES, "srmr_vad_edges_kernel")
-  PBB_VAD_ROW(ROW_EDGES, "srmr_vad_row_edges_kernel")
-  PBB_VAD_TILE(VAD_COUNT, "srmr_vad_count_kernel")
-  PBB_VAD_ROW(ROW_OFFSETS, "srmr_vad_offsets_kernel")
-  PBB_VAD_TILE(VAD_COMPACT, "srmr_vad_compact_kernel")
-  PBB_VAD_ROW(ROW_MEAN, "srmr_vad_mean_kernel")
+  PBB_TRY(launch_kernel("srmr_vad_max_kernel", vad_tile_kernel<T, VAD_MAX>, ctas, kVadThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_threshold_kernel", vad_row_kernel<T, ROW_THRESHOLD>, rows, kVadRowThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_edges_kernel", vad_tile_kernel<T, VAD_EDGES>, ctas, kVadThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_row_edges_kernel", vad_row_kernel<T, ROW_EDGES>, rows, kVadRowThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_count_kernel", vad_tile_kernel<T, VAD_COUNT>, ctas, kVadThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_offsets_kernel", vad_row_kernel<T, ROW_OFFSETS>, rows, kVadRowThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_compact_kernel", vad_tile_kernel<T, VAD_COMPACT>, ctas, kVadThreads, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_vad_mean_kernel", vad_row_kernel<T, ROW_MEAN>, rows, kVadRowThreads, 0, st, p));
   if (normalise) {
-    PBB_VAD_NORM(VAD_MOMENTS, "srmr_vad_moments_kernel")
-    PBB_VAD_ROW(ROW_STD, "srmr_vad_std_kernel")
-    PBB_VAD_NORM(VAD_NORMALISE, "srmr_vad_normalise_kernel")
+    PBB_TRY(launch_kernel("srmr_vad_moments_kernel", vad_norm_kernel<VAD_MOMENTS>, ctas, kVadThreads, 0, st, p));
+    PBB_TRY(launch_kernel("srmr_vad_std_kernel", vad_row_kernel<T, ROW_STD>, rows, kVadRowThreads, 0, st, p));
+    PBB_TRY(launch_kernel("srmr_vad_normalise_kernel", vad_norm_kernel<VAD_NORMALISE>, ctas, kVadThreads, 0, st, p));
   }
-#undef PBB_VAD_TILE
-#undef PBB_VAD_ROW
-#undef PBB_VAD_NORM
   return 0;
 }
 
@@ -73,10 +52,7 @@ static int smem_launch(K kernel, const char* name, long long ctas, size_t smem, 
     return -1;
   }
   PBB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchScope ls(name, st);
-  kernel<<<(unsigned)ctas, kFlThreads, smem, st>>>(args...);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel(name, kernel, (unsigned)ctas, kFlThreads, smem, st, args...);
 }
 
 }  // namespace pbb
@@ -152,12 +128,10 @@ int pbb_srmr_hilbert(double* y, long long rows, long long N, int n, const long l
   double2* tw2 = reinterpret_cast<double2*>(w + l.tw2);
   double* ks = reinterpret_cast<double*>(w + l.ks);
   double2* ws = reinterpret_cast<double2*>(w + l.fft);
-  {
-    LaunchScope ls("fl_stage_table_kernel", st);
-    fl_stage_table_kernel<<<(2 * sh.P1() + 255) / 256, 256, 0, st>>>(tw1, sh.logP1 + 1);
-    fl_stage_table_kernel<<<(2 * sh.P2() + 255) / 256, 256, 0, st>>>(tw2, sh.logP2 + 1);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("fl_stage_table_kernel", fl_stage_table_kernel, (2 * sh.P1() + 255) / 256, 256, 0, st, tw1,
+                        sh.logP1 + 1));
+  PBB_TRY(launch_kernel("fl_stage_table_kernel", fl_stage_table_kernel, (2 * sh.P2() + 255) / 256, 256, 0, st, tw2,
+                        sh.logP2 + 1));
   const size_t col_smem = 2 * (size_t)sh.cols * sh.P1() * sizeof(double2);
   const size_t row_smem = 4 * (size_t)sh.P2() * sizeof(double2);
   const FlForwardStore fwd{ws, sh.logP, sh.logP2};
@@ -231,25 +205,12 @@ int pbb_srmr_means(const double* env, long long rows, long long N, int n, const 
     set_error("argument: %lld blocks exceed the grid", units);
     return -1;
   }
-  {
-    LaunchScope ls("srmr_block_state_kernel", st);
-    srmr_block_kernel<false><<<(unsigned)((units + 255) / 256), 256, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
-  }
-  {
-    LaunchScope ls("srmr_carry_kernel", st);
-    srmr_carry_kernel<<<(unsigned)((filters + 255) / 256), 256, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
-  }
-  {
-    LaunchScope ls("srmr_block_energy_kernel", st);
-    srmr_block_kernel<true><<<(unsigned)((units + 255) / 256), 256, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
-  }
-  LaunchScope ls("srmr_mean_kernel", st);
-  srmr_mean_kernel<<<(unsigned)((filters + 255) / 256), 256, 0, st>>>(p);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("srmr_block_state_kernel", srmr_block_kernel<false>, (unsigned)((units + 255) / 256), 256, 0,
+                        st, p));
+  PBB_TRY(launch_kernel("srmr_carry_kernel", srmr_carry_kernel, (unsigned)((filters + 255) / 256), 256, 0, st, p));
+  PBB_TRY(launch_kernel("srmr_block_energy_kernel", srmr_block_kernel<true>, (unsigned)((units + 255) / 256), 256, 0,
+                        st, p));
+  return launch_kernel("srmr_mean_kernel", srmr_mean_kernel, (unsigned)((filters + 255) / 256), 256, 0, st, p);
 }
 
 int pbb_srmr_ratio(const double* means, long long rows, int n, const double* erb, const double* cutoff, double* out,
@@ -260,10 +221,8 @@ int pbb_srmr_ratio(const double* means, long long rows, int n, const double* erb
   PBB_CHECK_ARG(erb != nullptr && cutoff != nullptr, 4, "erb or cutoff is null");
   PBB_CHECK_ARG(out != nullptr, 6, "out is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("srmr_ratio_kernel", st);
-  srmr_ratio_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(means, rows, n, erb, cutoff, out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("srmr_ratio_kernel", srmr_ratio_kernel, (unsigned)((rows + 127) / 128), 128, 0, st, means, rows,
+                       n, erb, cutoff, out);
 }
 
 }  // extern "C"

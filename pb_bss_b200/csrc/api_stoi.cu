@@ -61,9 +61,7 @@ static int stoi_resample(const StoiParams& p, const StoiShape& s, cudaStream_t s
   if (s.resample) {
     const long long total = p.rows * 2 * p.L;
     const long long ctas = std::min<long long>((total + kStoiThreads - 1) / kStoiThreads, 1ll << 20);
-    LaunchScope ls("stoi_resample_kernel", st);
-    stoi_resample_kernel<T><<<(unsigned)ctas, kStoiThreads, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("stoi_resample_kernel", stoi_resample_kernel<T>, (unsigned)ctas, kStoiThreads, 0, st, p));
   }
   return 0;
 }
@@ -74,20 +72,13 @@ template <class U>
 static int stoi_envelopes(const StoiParams& p, cudaStream_t st) {
   {
     const long long warps = p.rows * p.F;
-    LaunchScope ls("stoi_energy_kernel", st);
-    stoi_energy_kernel<U><<<(unsigned)((warps * 32 + kStoiThreads - 1) / kStoiThreads), kStoiThreads, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("stoi_energy_kernel", stoi_energy_kernel<U>,
+                          (unsigned)((warps * 32 + kStoiThreads - 1) / kStoiThreads), kStoiThreads, 0, st, p));
   }
-  {
-    LaunchScope ls("stoi_compact_kernel", st);
-    stoi_compact_kernel<<<(unsigned)p.rows, kStoiCompactThreads, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("stoi_compact_kernel", stoi_compact_kernel, (unsigned)p.rows, kStoiCompactThreads, 0, st, p));
   if (p.Mmax > 0) {
     const long long ctas = p.rows * 2 * ((p.Mmax + kStoiFpc - 1) / kStoiFpc);
-    LaunchScope ls("stoi_bands_kernel", st);
-    stoi_bands_kernel<U><<<(unsigned)ctas, kStoiThreads, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("stoi_bands_kernel", stoi_bands_kernel<U>, (unsigned)ctas, kStoiThreads, 0, st, p));
   }
   return 0;
 }
@@ -103,18 +94,13 @@ static int stoi_group(StoiParams p, const StoiShape& s, bool extended, cudaStrea
     if (extended) {
       PBB_CUDA(cudaFuncSetAttribute(estoi_segment_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)kEstoiSmemBytes));
-      LaunchScope ls("estoi_segment_kernel", st);
-      estoi_segment_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, kEstoiSmemBytes, st>>>(p);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("estoi_segment_kernel", estoi_segment_kernel, (unsigned)(p.rows * p.blocks), kStoiThreads,
+                            kEstoiSmemBytes, st, p));
     } else {
-      LaunchScope ls("stoi_segment_kernel", st);
-      stoi_segment_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, 0, st>>>(p);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("stoi_segment_kernel", stoi_segment_kernel, (unsigned)(p.rows * p.blocks), kStoiThreads, 0,
+                            st, p));
     }
-    LaunchScope ls("stoi_value_kernel", st);
-    stoi_value_kernel<<<1, kStoiThreads, 0, st>>>(p);
-    PBB_CUDA(cudaGetLastError());
-    return 0;
+    return launch_kernel("stoi_value_kernel", stoi_value_kernel, 1, kStoiThreads, 0, st, p);
   };
   if (s.resample) return run(double{});
   return run(T{});
@@ -220,48 +206,32 @@ static int stoi_backward_group(StoiParams p, StoiGrad q, const StoiShape& s, boo
     using U = decltype(tag);
     if (int rc = stoi_envelopes<U>(p, st)) return rc;
     PBB_CUDA(cudaMemsetAsync(q.rank, 0xff, (size_t)p.rows * p.F * sizeof(int), st));
-    {
-      LaunchScope ls("stoi_rank_kernel", st);
-      stoi_rank_kernel<<<stoi_ctas(p.rows * p.F), kStoiThreads, 0, st>>>(p, q);
-      PBB_CUDA(cudaGetLastError());
-    }
+    PBB_TRY(launch_kernel("stoi_rank_kernel", stoi_rank_kernel, stoi_ctas(p.rows * p.F), kStoiThreads, 0, st, p, q));
     if (p.Mmax >= kStoiSeg) {
       if (extended) {
         PBB_CUDA(cudaFuncSetAttribute(estoi_segment_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)kEstoiSmemBytes));
-        LaunchScope ls("estoi_segment_prep_kernel", st);
-        estoi_segment_prep_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, kEstoiSmemBytes, st>>>(p, q);
-        PBB_CUDA(cudaGetLastError());
+        PBB_TRY(launch_kernel("estoi_segment_prep_kernel", estoi_segment_prep_kernel, (unsigned)(p.rows * p.blocks),
+                              kStoiThreads, kEstoiSmemBytes, st, p, q));
       } else {
-        LaunchScope ls("stoi_segment_prep_kernel", st);
-        stoi_segment_prep_kernel<<<(unsigned)(p.rows * p.blocks), kStoiThreads, 0, st>>>(p, q);
-        PBB_CUDA(cudaGetLastError());
+        PBB_TRY(launch_kernel("stoi_segment_prep_kernel", stoi_segment_prep_kernel, (unsigned)(p.rows * p.blocks),
+                              kStoiThreads, 0, st, p, q));
       }
       const unsigned ctas = stoi_ctas(p.rows * kStoiBands * p.Mmax);
       if (extended) {
-        LaunchScope ls("estoi_segment_grad_kernel", st);
-        estoi_segment_grad_kernel<<<ctas, kStoiThreads, 0, st>>>(p, q);
-        PBB_CUDA(cudaGetLastError());
+        PBB_TRY(launch_kernel("estoi_segment_grad_kernel", estoi_segment_grad_kernel, ctas, kStoiThreads, 0, st, p, q));
       } else {
-        LaunchScope ls("stoi_segment_grad_kernel", st);
-        stoi_segment_grad_kernel<<<ctas, kStoiThreads, 0, st>>>(p, q);
-        PBB_CUDA(cudaGetLastError());
+        PBB_TRY(launch_kernel("stoi_segment_grad_kernel", stoi_segment_grad_kernel, ctas, kStoiThreads, 0, st, p, q));
       }
-      LaunchScope ls("stoi_spectral_grad_kernel", st);
-      stoi_spectral_grad_kernel<U>
-          <<<(unsigned)(p.rows * 2 * ((p.Mmax + kStoiFpc - 1) / kStoiFpc)), kStoiThreads, 0, st>>>(p, q);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("stoi_spectral_grad_kernel", stoi_spectral_grad_kernel<U>,
+                            (unsigned)(p.rows * 2 * ((p.Mmax + kStoiFpc - 1) / kStoiFpc)), kStoiThreads, 0, st, p, q));
     }
     // below 30 STFT frames in every row the kernel only writes zeros
-    {
-      LaunchScope ls("stoi_removal_grad_kernel", st);
-      stoi_removal_grad_kernel<<<stoi_ctas(p.rows * 2 * p.L), kStoiThreads, 0, st>>>(p, q);
-      PBB_CUDA(cudaGetLastError());
-    }
+    PBB_TRY(launch_kernel("stoi_removal_grad_kernel", stoi_removal_grad_kernel, stoi_ctas(p.rows * 2 * p.L),
+                          kStoiThreads, 0, st, p, q));
     if (s.resample) {
-      LaunchScope ls("stoi_resample_grad_kernel", st);
-      stoi_resample_grad_kernel<<<stoi_ctas(p.rows * 2 * p.n), kStoiThreads, 0, st>>>(p, q);
-      PBB_CUDA(cudaGetLastError());
+      PBB_TRY(launch_kernel("stoi_resample_grad_kernel", stoi_resample_grad_kernel, stoi_ctas(p.rows * 2 * p.n),
+                            kStoiThreads, 0, st, p, q));
     }
     return 0;
   };

@@ -17,15 +17,11 @@ static int mean_square_launch(const void* x, long long rows, long long n, double
                               cudaStream_t st) {
   const long long chunks = sxr_chunks(n);
   if (chunks > 0) {
-    LaunchScope ls("mean_square_chunk_kernel", st);
-    mean_square_chunk_kernel<T><<<(unsigned)(rows * chunks), kSxrThreads, 0, st>>>(static_cast<const T*>(x), n, chunks,
-                                                                                     partial);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("mean_square_chunk_kernel", mean_square_chunk_kernel<T>, (unsigned)(rows * chunks),
+                          kSxrThreads, 0, st, static_cast<const T*>(x), n, chunks, partial));
   }
-  LaunchScope ls("mean_square_row_kernel", st);
-  mean_square_row_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(partial, n, chunks, out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("mean_square_row_kernel", mean_square_row_kernel, (unsigned)rows, kSxrThreads, 0, st, partial, n,
+                       chunks, out);
 }
 
 }  // namespace pbb
@@ -87,26 +83,16 @@ int pbb_si_sdr(const double* reference, const double* estimation, const long lon
   double* alpha = p2 + rows * chunks * 2;
   const unsigned grid = (unsigned)(rows * chunks);
   if (chunks > 0) {
-    LaunchScope ls("si_sdr_pass1_kernel", st);
-    si_sdr_pass1_kernel<<<grid, kSxrThreads, 0, st>>>(reference, estimation, reference_offsets, estimation_offsets, n,
-                                                      chunks, p1);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("si_sdr_pass1_kernel", si_sdr_pass1_kernel, grid, kSxrThreads, 0, st, reference, estimation,
+                          reference_offsets, estimation_offsets, n, chunks, p1));
   }
-  {
-    LaunchScope ls("si_sdr_alpha_kernel", st);
-    si_sdr_alpha_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(p1, chunks, alpha);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("si_sdr_alpha_kernel", si_sdr_alpha_kernel, (unsigned)rows, kSxrThreads, 0, st, p1, chunks,
+                        alpha));
   if (chunks > 0) {
-    LaunchScope ls("si_sdr_pass2_kernel", st);
-    si_sdr_pass2_kernel<<<grid, kSxrThreads, 0, st>>>(reference, estimation, reference_offsets, estimation_offsets, n,
-                                                      chunks, alpha, p2);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("si_sdr_pass2_kernel", si_sdr_pass2_kernel, grid, kSxrThreads, 0, st, reference, estimation,
+                          reference_offsets, estimation_offsets, n, chunks, alpha, p2));
   }
-  LaunchScope ls("si_sdr_ratio_kernel", st);
-  si_sdr_ratio_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(p2, chunks, out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("si_sdr_ratio_kernel", si_sdr_ratio_kernel, (unsigned)rows, kSxrThreads, 0, st, p2, chunks, out);
 }
 
 size_t pbb_si_sdr_backward_workspace_bytes(long long rows, long long n) {
@@ -142,44 +128,26 @@ int pbb_si_sdr_backward(const double* reference, const double* estimation, const
   double* coef = alpha + rows;
   const unsigned grid = (unsigned)(rows * chunks);
   // alpha, P and Q exactly as pbb_si_sdr forms them
-  {
-    LaunchScope ls("si_sdr_pass1_kernel", st);
-    si_sdr_pass1_kernel<<<grid, kSxrThreads, 0, st>>>(reference, estimation, reference_offsets, estimation_offsets, n,
-                                                      chunks, p1);
-    PBB_CUDA(cudaGetLastError());
-  }
-  {
-    LaunchScope ls("si_sdr_alpha_kernel", st);
-    si_sdr_alpha_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(p1, chunks, alpha);
-    PBB_CUDA(cudaGetLastError());
-  }
-  {
-    LaunchScope ls("si_sdr_pass2_kernel", st);
-    si_sdr_pass2_kernel<<<grid, kSxrThreads, 0, st>>>(reference, estimation, reference_offsets, estimation_offsets, n,
-                                                      chunks, alpha, p2);
-    PBB_CUDA(cudaGetLastError());
-  }
-  {
-    LaunchScope ls("si_sdr_backward_row_kernel", st);
-    si_sdr_backward_row_kernel<<<(unsigned)rows, kSxrThreads, 0, st>>>(p2, chunks, grad_out, coef);
-    PBB_CUDA(cudaGetLastError());
-  }
+  PBB_TRY(launch_kernel("si_sdr_pass1_kernel", si_sdr_pass1_kernel, grid, kSxrThreads, 0, st, reference, estimation,
+                        reference_offsets, estimation_offsets, n, chunks, p1));
+  PBB_TRY(launch_kernel("si_sdr_alpha_kernel", si_sdr_alpha_kernel, (unsigned)rows, kSxrThreads, 0, st, p1, chunks,
+                        alpha));
+  PBB_TRY(launch_kernel("si_sdr_pass2_kernel", si_sdr_pass2_kernel, grid, kSxrThreads, 0, st, reference, estimation,
+                        reference_offsets, estimation_offsets, n, chunks, alpha, p2));
+  PBB_TRY(launch_kernel("si_sdr_backward_row_kernel", si_sdr_backward_row_kernel, (unsigned)rows, kSxrThreads, 0, st,
+                        p2, chunks, grad_out, coef));
   const auto blocks = [](long long count) {
     return (unsigned)std::min<long long>((count + kSxrThreads - 1) / kSxrThreads, 1ll << 20);
   };
   if (grad_estimation && estimation_rows > 0) {
-    LaunchScope ls("si_sdr_backward_kernel", st);
-    si_sdr_backward_kernel<true><<<blocks(estimation_rows * n), kSxrThreads, 0, st>>>(
-        reference, estimation, reference_offsets, estimation_offsets, n, alpha, coef, estimation_rows,
-        estimation_row_start, estimation_row_index, grad_estimation);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("si_sdr_backward_kernel", si_sdr_backward_kernel<true>, blocks(estimation_rows * n),
+                          kSxrThreads, 0, st, reference, estimation, reference_offsets, estimation_offsets, n, alpha,
+                          coef, estimation_rows, estimation_row_start, estimation_row_index, grad_estimation));
   }
   if (grad_reference && reference_rows > 0) {
-    LaunchScope ls("si_sdr_backward_kernel", st);
-    si_sdr_backward_kernel<false><<<blocks(reference_rows * n), kSxrThreads, 0, st>>>(
-        reference, estimation, reference_offsets, estimation_offsets, n, alpha, coef, reference_rows,
-        reference_row_start, reference_row_index, grad_reference);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("si_sdr_backward_kernel", si_sdr_backward_kernel<false>, blocks(reference_rows * n),
+                          kSxrThreads, 0, st, reference, estimation, reference_offsets, estimation_offsets, n, alpha,
+                          coef, reference_rows, reference_row_start, reference_row_index, grad_reference));
   }
   return 0;
 }
@@ -192,10 +160,8 @@ int pbb_input_sxr(const double* S, const double* N, int K, int D, int average_so
   PBB_CHECK_ARG(D >= 1 && D <= PBB_SXR_MAX_D, 4, "D must be in [1, PBB_SXR_MAX_D]");
   PBB_CHECK_ARG(sdr != nullptr && sir != nullptr && snr != nullptr, 7, "an output is null");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  LaunchScope ls("input_sxr_kernel", st);
-  input_sxr_kernel<<<1, 1, 0, st>>>(S, N, K, D, average_sources != 0, average_channels != 0, sdr, sir, snr);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("input_sxr_kernel", input_sxr_kernel, 1, 1, 0, st, S, N, K, D, average_sources != 0,
+                       average_channels != 0, sdr, sir, snr);
 }
 
 static int output_sxr_ctas(int K_source, int K_target) {
@@ -221,17 +187,10 @@ int pbb_output_sxr(const double* S, const double* N, int K_source, int K_target,
   const int ctas = output_sxr_ctas(K_source, K_target);
   double* best = static_cast<double*>(workspace);
   long long* best_idx = reinterpret_cast<long long*>(best + ctas);
-  {
-    LaunchScope ls("output_sxr_search_kernel", st);
-    output_sxr_search_kernel<<<ctas, kSxrThreads, 0, st>>>(S, K_source, K_target,
-                                                           sxr_perm_count(K_target, K_source), best, best_idx);
-    PBB_CUDA(cudaGetLastError());
-  }
-  LaunchScope ls("output_sxr_kernel", st);
-  output_sxr_kernel<<<1, 1, 0, st>>>(S, N, K_source, K_target, best, best_idx, ctas, average_sources != 0, sdr, sir,
-                                     snr, selection);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("output_sxr_search_kernel", output_sxr_search_kernel, ctas, kSxrThreads, 0, st, S, K_source,
+                        K_target, sxr_perm_count(K_target, K_source), best, best_idx));
+  return launch_kernel("output_sxr_kernel", output_sxr_kernel, 1, 1, 0, st, S, N, K_source, K_target, best, best_idx,
+                       ctas, average_sources != 0, sdr, sir, snr, selection);
 }
 
 }  // extern "C"

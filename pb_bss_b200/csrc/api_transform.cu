@@ -29,8 +29,8 @@ static int frames_per_cta(int size, long long rows, int frames) {
   return pbb_stft_frames_per_cta(size, rows, frames, sm_count());
 }
 
-template <class K>
-static int fft_launch(K kernel, const char* name, long long rows, int frames, int fpc, int size, void* params_ptr,
+template <class P>
+static int fft_launch(void (*kernel)(P), const char* name, long long rows, int frames, int fpc, int size, const P& p,
                       cudaStream_t st) {
   const size_t smem = (size_t)fpc * size * sizeof(double2);  // two buffers of fpc * size / 2 points
   PBB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -39,10 +39,7 @@ static int fft_launch(K kernel, const char* name, long long rows, int frames, in
     set_error("argument: %lld CTAs exceed the grid", ctas);
     return -1;
   }
-  LaunchScope ls(name, st);
-  void* args[] = {params_ptr};
-  PBB_CUDA(cudaLaunchKernel((const void*)kernel, dim3((unsigned)ctas), dim3(kFftThreads), args, smem, st));
-  return 0;
+  return launch_kernel(name, kernel, (unsigned)ctas, kFftThreads, smem, st, p);
 }
 
 struct GtShape {
@@ -63,20 +60,14 @@ static int gammatone_launch(const GtParams& p, cudaStream_t st) {
   }
   GtParams q = p;
   if (p.chunks > 1) {
-    {
-      LaunchScope ls("gammatone_chunk_state_kernel", st);
-      gammatone_chunk_kernel<T, false><<<(unsigned)ctas, kGtThreads, 0, st>>>(q);
-      PBB_CUDA(cudaGetLastError());
-    }
+    PBB_TRY(launch_kernel("gammatone_chunk_state_kernel", gammatone_chunk_kernel<T, false>, (unsigned)ctas, kGtThreads,
+                          0, st, q));
     const long long units = p.groups < kGtGroup ? p.groups : kGtGroup;
-    LaunchScope ls("gammatone_carry_kernel", st);
-    gammatone_carry_kernel<<<(unsigned)(p.rows * p.n), (unsigned)((units * 8 + 31) / 32 * 32), 0, st>>>(q);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("gammatone_carry_kernel", gammatone_carry_kernel, (unsigned)(p.rows * p.n),
+                          (unsigned)((units * 8 + 31) / 32 * 32), 0, st, q));
   }
-  LaunchScope ls("gammatone_output_kernel", st);
-  gammatone_chunk_kernel<T, true><<<(unsigned)ctas, kGtThreads, 0, st>>>(q);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("gammatone_output_kernel", gammatone_chunk_kernel<T, true>, (unsigned)ctas, kGtThreads, 0, st,
+                       q);
 }
 
 }  // namespace pbb
@@ -128,8 +119,8 @@ int pbb_stft(const void* x, int dtype, long long rows, long long n, int size, in
   p.tw = reinterpret_cast<const double2*>(twiddle);
   p.out = reinterpret_cast<double2*>(out);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (dtype == PBB_F32) return fft_launch(stft_kernel<float, STFT_PLAIN>, "stft_kernel", rows, frames, p.fpc, size, &p, st);
-  return fft_launch(stft_kernel<double, STFT_PLAIN>, "stft_kernel", rows, frames, p.fpc, size, &p, st);
+  if (dtype == PBB_F32) return fft_launch(stft_kernel<float, STFT_PLAIN>, "stft_kernel", rows, frames, p.fpc, size, p, st);
+  return fft_launch(stft_kernel<double, STFT_PLAIN>, "stft_kernel", rows, frames, p.fpc, size, p, st);
 }
 
 int pbb_griffin_lim_stft(const double* x_hat, int K, long long n, const double* y, const void* X, int size, int shift,
@@ -168,8 +159,8 @@ int pbb_griffin_lim_stft(const double* x_hat, int K, long long n, const double* 
   p.out_dash = reinterpret_cast<double2*>(X_dash);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (y != nullptr)
-    return fft_launch(stft_kernel<double, STFT_MISI>, "stft_misi_kernel", K, frames, p.fpc, size, &p, st);
-  return fft_launch(stft_kernel<double, STFT_GRIFFIN_LIM>, "stft_griffin_lim_kernel", K, frames, p.fpc, size, &p, st);
+    return fft_launch(stft_kernel<double, STFT_MISI>, "stft_misi_kernel", K, frames, p.fpc, size, p, st);
+  return fft_launch(stft_kernel<double, STFT_GRIFFIN_LIM>, "stft_griffin_lim_kernel", K, frames, p.fpc, size, p, st);
 }
 
 size_t pbb_istft_workspace_bytes(long long rows, int frames, int window_length) {
@@ -207,15 +198,12 @@ int pbb_istft(const void* X, long long rows, int frames, int size, int shift, in
   p.synthesis = synthesis_window;
   p.tw = reinterpret_cast<const double2*>(twiddle);
   p.framebuf = reinterpret_cast<double*>(workspace);
-  const int rc = fft_launch(istft_frames_kernel, "istft_frames_kernel", rows, frames, p.fpc, size, &p, st);
+  const int rc = fft_launch(istft_frames_kernel, "istft_frames_kernel", rows, frames, p.fpc, size, p, st);
   if (rc != 0 || n_out == 0) return rc;
   long long blocks = (rows * n_out + 255) / 256;
   if (blocks > 4ll * 32 * sm_count()) blocks = 4ll * 32 * sm_count();
-  LaunchScope ls("overlap_add_kernel", st);
-  overlap_add_kernel<<<(unsigned)blocks, 256, 0, st>>>(p.framebuf, rows, frames, window_length, shift, crop, n_out,
-                                                       out);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("overlap_add_kernel", overlap_add_kernel, (unsigned)blocks, 256, 0, st, p.framebuf, rows, frames,
+                       window_length, shift, crop, n_out, out);
 }
 
 int pbb_istft_backward(const double* grad_out, long long rows, int frames, int size, int shift, int window_length,
@@ -248,7 +236,7 @@ int pbb_istft_backward(const double* grad_out, long long rows, int frames, int s
   p.window = synthesis_window;
   p.tw = reinterpret_cast<const double2*>(twiddle);
   p.out = reinterpret_cast<double2*>(grad_X);
-  return fft_launch(istft_backward_kernel, "istft_backward_kernel", rows, frames, p.fpc, size, &p,
+  return fft_launch(istft_backward_kernel, "istft_backward_kernel", rows, frames, p.fpc, size, p,
                     reinterpret_cast<cudaStream_t>(stream));
 }
 
@@ -285,17 +273,13 @@ int pbb_stft_backward(const void* grad_X, long long rows, long long n, int size,
   p.synthesis = window;
   p.tw = reinterpret_cast<const double2*>(twiddle);
   p.framebuf = reinterpret_cast<double*>(workspace);
-  const int rc = fft_launch(stft_backward_kernel, "stft_backward_kernel", rows, frames, p.fpc,
-                            size, &p, st);
+  const int rc = fft_launch(stft_backward_kernel, "stft_backward_kernel", rows, frames, p.fpc, size, p, st);
   if (rc != 0 || n == 0) return rc;
   // sample s of row r sums the frames t covering padded position s + offset; samples no frame covers get 0
   long long blocks = (rows * n + 255) / 256;
   if (blocks > 4ll * 32 * sm_count()) blocks = 4ll * 32 * sm_count();
-  LaunchScope ls("overlap_add_kernel", st);
-  overlap_add_kernel<<<(unsigned)blocks, 256, 0, st>>>(p.framebuf, rows, frames, window_length, shift, offset, n,
-                                                       grad_x);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("overlap_add_kernel", overlap_add_kernel, (unsigned)blocks, 256, 0, st, p.framebuf, rows, frames,
+                       window_length, shift, offset, n, grad_x);
 }
 
 int pbb_gammatone_chunk_length(long long rows, int n, long long N) {

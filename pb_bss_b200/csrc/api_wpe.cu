@@ -56,10 +56,8 @@ static int wpe_filter_launch(const TIn* y, WpeStrides ys, const WpeShape& s, lon
                              cudaStream_t st) {
   const size_t smem = wpe_filter_smem_bytes(s.D, s.taps);
   PBB_CUDA(cudaFuncSetAttribute(wpe_filter_kernel<TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchScope ls("wpe_filter_kernel", st);
-  wpe_filter_kernel<TIn><<<(unsigned)bins, 256, smem, st>>>(y, ys, s, G, out, os, power, lam, pw, status);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("wpe_filter_kernel", wpe_filter_kernel<TIn>, (unsigned)bins, 256, smem, st, y, ys, s, G, out, os,
+                       power, lam, pw, status);
 }
 
 template <int TPW, class TIn>
@@ -68,11 +66,8 @@ static int wpe_corr_launch(const TIn* y, WpeStrides ys, const WpeShape& s, long 
   const size_t smem = wpe_corr_smem_doubles(s.D, s.taps) * sizeof(double);
   const unsigned passes = (unsigned)((s.ntiles + kWpeCorrWarps * TPW - 1) / (kWpeCorrWarps * TPW));
   PBB_CUDA(cudaFuncSetAttribute(wpe_corr_kernel<TPW, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchScope ls("wpe_corr_kernel", st);
-  wpe_corr_kernel<TPW, TIn><<<dim3((unsigned)s.parts, (unsigned)bins, passes), 32 * kWpeCorrWarps, smem, st>>>(
-      y, ys, s, w, part);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("wpe_corr_kernel", wpe_corr_kernel<TPW, TIn>, dim3((unsigned)s.parts, (unsigned)bins, passes),
+                       32 * kWpeCorrWarps, smem, st, y, ys, s, w, part);
 }
 
 // tiles per warp: the smallest instantiated slot count that covers every lower-triangle tile in one pass; more than
@@ -94,15 +89,10 @@ static int wpe_solve_group(const TIn* yg, WpeStrides ys, const WpeShape& s, long
                            double2* G, int* lstsq, int* status, cudaStream_t st) {
   int rc = wpe_corr<TIn>(yg, ys, s, g, w, part, st);
   if (rc) return rc;
-  {
-    LaunchScope ls("wpe_solve_kernel", st);
-    wpe_solve_kernel<<<(unsigned)g, 256, wpe_solve_smem_bytes(s.n, s.D), st>>>(part, s, G, lstsq, status);
-    PBB_CUDA(cudaGetLastError());
-  }
-  LaunchScope ls("wpe_lstsq_kernel", st);
-  wpe_lstsq_kernel<<<(unsigned)g, 32, wpe_lstsq_smem_bytes(s.n, s.D), st>>>(part, s, lstsq, G);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  PBB_TRY(launch_kernel("wpe_solve_kernel", wpe_solve_kernel, (unsigned)g, 256, wpe_solve_smem_bytes(s.n, s.D), st,
+                        part, s, G, lstsq, status));
+  return launch_kernel("wpe_lstsq_kernel", wpe_lstsq_kernel, (unsigned)g, 32, wpe_lstsq_smem_bytes(s.n, s.D), st, part,
+                       s, lstsq, G);
 }
 
 template <class TIn>
@@ -159,13 +149,10 @@ static int wpe_step_run(const TIn* y, WpeStrides ys, long long bins, const doubl
   PBB_CUDA(cudaFuncSetAttribute(wpe_lstsq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lstsq_smem));
   for (long long b0 = 0; b0 < bins; b0 += group) {
     const long long g = bins - b0 < group ? bins - b0 : group;
-    {
-      LaunchScope ls("wpe_weight_copy_kernel", st);
-      const long long total = g * s.T;
-      wpe_weight_copy_kernel<<<(unsigned)(total / 256 + 1 < 65536 ? total / 256 + 1 : 65536), 256, 0, st>>>(
-          wsrc + b0 * wsb, wsb, wst, g, s.T, w);
-      PBB_CUDA(cudaGetLastError());
-    }
+    const long long total = g * s.T;
+    PBB_TRY(launch_kernel("wpe_weight_copy_kernel", wpe_weight_copy_kernel,
+                          (unsigned)(total / 256 + 1 < 65536 ? total / 256 + 1 : 65536), 256, 0, st, wsrc + b0 * wsb,
+                          wsb, wst, g, s.T, w));
     int rc = wpe_solve_group<TIn>(y + b0 * ys.b, ys, s, g, w, part, G, lstsq, status, st);
     if (rc) return rc;
     if (G_save != nullptr)
@@ -214,23 +201,16 @@ static int wpe_backward_run(const TIn* y, WpeStrides ys, long long bins, const W
     if (s.tb < s.T) {
       int rc = wpe_corr<TIn>(yg, ys, s, g, w + b0 * s.T, part, st);
       if (rc) return rc;
-      {
-        LaunchScope ls("wpe_gbar_kernel", st);
-        wpe_gbar_kernel<TIn><<<(unsigned)g, 256, gbar_smem, st>>>(yg, ys, s, xbar + b0 * per, Pbar);
-        PBB_CUDA(cudaGetLastError());
-      }
-      {
-        LaunchScope ls("wpe_solve_rhs_kernel", st);
-        wpe_solve_rhs_kernel<<<(unsigned)g, 256, solve_smem, st>>>(part, s, Pbar);
-        PBB_CUDA(cudaGetLastError());
-      }
+      PBB_TRY(launch_kernel("wpe_gbar_kernel", wpe_gbar_kernel<TIn>, (unsigned)g, 256, gbar_smem, st, yg, ys, s,
+                            xbar + b0 * per, Pbar));
+      PBB_TRY(launch_kernel("wpe_solve_rhs_kernel", wpe_solve_rhs_kernel, (unsigned)g, 256, solve_smem, st, part, s,
+                            Pbar));
     } else {
       PBB_CUDA(cudaMemsetAsync(Pbar, 0, (size_t)g * s.n * s.D * sizeof(double2), st));
     }
-    LaunchScope ls("wpe_step_backward_kernel", st);
-    wpe_step_backward_kernel<TIn><<<(unsigned)g, 256, back_smem, st>>>(
-        yg, ys, s, G + b0 * s.n * s.D, Pbar, w + b0 * s.T, xbar + b0 * per, ub, ybar + b0 * per, wbar + b0 * s.T);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("wpe_step_backward_kernel", wpe_step_backward_kernel<TIn>, (unsigned)g, 256, back_smem, st,
+                          yg, ys, s, G + b0 * s.n * s.D, Pbar, w + b0 * s.T, xbar + b0 * per, ub, ybar + b0 * per,
+                          wbar + b0 * s.T));
   }
   return 0;
 }
@@ -248,19 +228,16 @@ static int wpe_power_backward_run(const TIn* y, WpeStrides ys, long long bins, c
     if (rc) return rc;
   }
   if (mode == kWpeGradInverseAll) {
-    LaunchScope ls("wpe_power_inverse_backward_kernel", st);
-    wpe_power_inverse_backward_kernel<<<1, 1024, 0, st>>>(lamc, gin, lam, bins * s.T);
-    PBB_CUDA(cudaGetLastError());
+    PBB_TRY(launch_kernel("wpe_power_inverse_backward_kernel", wpe_power_inverse_backward_kernel, 1, 1024, 0, st, lamc,
+                          gin, lam, bins * s.T));
     gin = lam;
     mode = kWpeGradPlain;
   }
   const size_t smem = wpe_power_backward_smem_bytes(s.D, s.taps, G != nullptr);
   PBB_CUDA(cudaFuncSetAttribute(wpe_power_backward_kernel<TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 (int)smem));
-  LaunchScope ls("wpe_power_backward_kernel", st);
-  wpe_power_backward_kernel<TIn><<<(unsigned)bins, 256, smem, st>>>(y, ys, s, G, lamc, gin, mode, pbar, xbar);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("wpe_power_backward_kernel", wpe_power_backward_kernel<TIn>, (unsigned)bins, 256, smem, st, y,
+                       ys, s, G, lamc, gin, mode, pbar, xbar);
 }
 
 template <int R, class TIn>
@@ -269,11 +246,8 @@ static int wpe_online_launch(const TIn* y, WpeStrides ys, const TIn* hist, WpeSt
                              double2* Gout, long long bins, const WpeOnlineShape& s, cudaStream_t st) {
   const size_t smem = wpe_online_smem_bytes(s.D, s.taps, s.delay);
   PBB_CUDA(cudaFuncSetAttribute(wpe_online_kernel<R, TIn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  LaunchScope ls("wpe_online_kernel", st);
-  wpe_online_kernel<R, TIn><<<(unsigned)bins, kWpeOnlineThreads, smem, st>>>(y, ys, hist, hs, power, Qin, Gin, z,
-                                                                              zs, Qout, Gout, s);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("wpe_online_kernel", wpe_online_kernel<R, TIn>, (unsigned)bins, kWpeOnlineThreads, smem, st, y,
+                       ys, hist, hs, power, Qin, Gin, z, zs, Qout, Gout, s);
 }
 
 // R = ceil(n / 16): each of the 16 x 16 threads holds R x R entries of Q
@@ -475,10 +449,7 @@ int pbb_wpe_power(const void* y, int dtype, long long bins, int D, long long T, 
                : wpe_filter_launch<double2>(static_cast<const double2*>(y), ys, s, bins, nullptr, nullptr, ys,
                                             kWpePowerPlain, lam, out, nullptr, st);
   if (rc || !inverse) return rc;
-  LaunchScope ls("wpe_power_inverse_kernel", st);
-  wpe_power_inverse_kernel<<<1, 1024, 0, st>>>(out, bins * T);
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return launch_kernel("wpe_power_inverse_kernel", wpe_power_inverse_kernel, 1, 1024, 0, st, out, bins * T);
 }
 
 int pbb_wpe_build_y_tilde(const void* y, int dtype, long long bins, int D, long long T, long long ysb, long long ysd,
@@ -495,15 +466,11 @@ int pbb_wpe_build_y_tilde(const void* y, int dtype, long long bins, int D, long 
   const WpeStrides ys{ysb, ysd, yst};
   const long long total = bins * taps * D * T;
   const unsigned blocks = (unsigned)(total / 256 + 1 < 65536 ? total / 256 + 1 : 65536);
-  LaunchScope ls("wpe_y_tilde_kernel", st);
-  if (dtype == PBB_C64)
-    wpe_y_tilde_kernel<float2><<<blocks, 256, 0, st>>>(static_cast<const float2*>(y), ys, bins, D, T, taps, delay,
-                                                       static_cast<float2*>(out));
-  else
-    wpe_y_tilde_kernel<double2><<<blocks, 256, 0, st>>>(static_cast<const double2*>(y), ys, bins, D, T, taps, delay,
-                                                        static_cast<double2*>(out));
-  PBB_CUDA(cudaGetLastError());
-  return 0;
+  return with_ct(dtype, [&](auto ct) {
+    using CT = decltype(ct);
+    return launch_kernel("wpe_y_tilde_kernel", wpe_y_tilde_kernel<CT>, blocks, 256, 0, st, static_cast<const CT*>(y),
+                         ys, bins, D, T, taps, delay, static_cast<CT*>(out));
+  });
 }
 
 size_t pbb_wpe_online_smem_bytes(int D, int taps, int delay) {

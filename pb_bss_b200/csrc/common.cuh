@@ -31,27 +31,55 @@ int cuda_fail(cudaError_t e, const char* what);
     if (_e != cudaSuccess) return ::pbb::cuda_fail(_e, #call);\
   } while (0)
 
-// ---- thread-block cluster launch (host) ----------------------------------------
-// Configuration of a 1-D grid launched in clusters of `cluster` CTAs, for cudaLaunchKernelEx and
+// propagates a nonzero status (a launch_kernel result, say) to the caller
+#define PBB_TRY(...)                                          \
+  do {                                                        \
+    if (int _r = (__VA_ARGS__)) return _r;                    \
+  } while (0)
+
+// ---- launches with one attribute (host) ------------------------------------------
+// Configuration of a launch with one launch attribute, for launch_ex (prof.cuh) and
 // cudaOccupancyMaxActiveClusters.  cfg points at attr, so the object is not copied.
-struct ClusterLaunch {
+struct AttrLaunch {
   cudaLaunchConfig_t cfg{};
   cudaLaunchAttribute attr{};
-  ClusterLaunch(unsigned ctas, unsigned threads, size_t smem, unsigned cluster, cudaStream_t st) {
-    cfg.gridDim = dim3(ctas);
-    cfg.blockDim = dim3(threads);
+  AttrLaunch(dim3 grid, dim3 block, size_t smem, cudaStream_t st) {
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+  }
+  AttrLaunch(const AttrLaunch&) = delete;
+  AttrLaunch& operator=(const AttrLaunch&) = delete;
+};
+
+// a 1-D grid launched in clusters of `cluster` CTAs
+struct ClusterLaunch : AttrLaunch {
+  ClusterLaunch(unsigned ctas, unsigned threads, size_t smem, unsigned cluster, cudaStream_t st)
+      : AttrLaunch(dim3(ctas), dim3(threads), smem, st) {
     attr.id = cudaLaunchAttributeClusterDimension;
     attr.val.clusterDim.x = cluster;
     attr.val.clusterDim.y = 1;
     attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
   }
-  ClusterLaunch(const ClusterLaunch&) = delete;
-  ClusterLaunch& operator=(const ClusterLaunch&) = delete;
 };
+
+// a cooperative launch: all CTAs co-resident (grid_barrier), or the launch fails
+struct CoopLaunch : AttrLaunch {
+  CoopLaunch(dim3 grid, dim3 block, size_t smem, cudaStream_t st) : AttrLaunch(grid, block, smem, st) {
+    attr.id = cudaLaunchAttributeCooperative;
+    attr.val.cooperative = 1;
+  }
+};
+
+// ---- dtype dispatch (host) ---------------------------------------------------------
+// fn(ct) with a value of the storage type (double2 for PBB_C128, float2 for PBB_C64) standing for the type
+template <class Fn>
+static int with_ct(int dtype, Fn&& fn) {
+  return dtype == PBB_C128 ? fn(double2{}) : fn(float2{});
+}
 
 // ---- compile-time loop -----------------------------------------------------
 template <class F, int... I>
