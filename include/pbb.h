@@ -189,6 +189,75 @@ int pbb_cacgmm_mstep(const void* y, int dtype, int F, int T, int D, int K,
                      void* workspace, size_t workspace_bytes, int* status,
                      void* stream);
 
+/* ---- Backward passes of the cACGMM (torch.autograd in pb_bss_b200.distribution.cacgmm).  Conventions as for the
+ * beamforming chain below: grad z = dL/dRe z + i dL/dIm z for a real loss L, <A, B> = sum conj(A_ij) B_ij, fp64,
+ * fixed-order sums and no atomics (repeated calls are bitwise identical), no status word, enqueue only.  Gradients
+ * are written as complex128 / float64; shapes and limits are those of the forward (D < 35, K < 20, any T).
+ *
+ * Notation: z_t = y_t / |y_t| (a zero frame stays zero), s_t the saliency (1 without), tiny = DBL_MIN.
+ * M-step (pbb_cacgmm_mstep):
+ *   g_kt = gamma_kt s_t,  S_k = sum_t g_kt,  c_kt = g_kt / max(q_kt, 10 tiny),  Psi_k = sum_t c_kt z_t z_t^H,
+ *   C_k = D Psi_k / max(S_k, tiny);  'trace': C'_k = C_k / max(tr C_k, tiny), otherwise C'_k = C_k;
+ *   C'_k = V diag(mu) V^H;  'eigenvalue': lam_i = max(mu_i / max(mu_max, tiny), floor), else lam_i = max(mu_i,
+ *   mu_max floor);  w_k = S_k / T (no saliency), S_k / sum_j |S_j| (saliency; a zero sum counts as 1e-10), 1 / K (-2).
+ * E-step (pbb_cacgmm_predict), with B^-1 = V diag(1 / lam) V^H and ld = sum log lam:
+ *   q_kt = max(|z_t^H B_k^-1 z_t|, tiny),  lp_kt = -D log q_kt - ld_k,  a_kt = exp(lp_kt - max_j lp_jt) w_k act_kt,
+ *   gamma_kt = clip(a_kt / max(sum_j a_jt, tiny), eps, 1 - eps) (no clip for eps = 0),
+ *   loglik_f = sum_t logsumexp_k lp_kt (without the weights).
+ * Backward of the E-step, per frame (gb = grad gamma where the clip is not active, else 0):
+ *   abar_k = (gb_k - sum_j gb_j gamma_j) / den (den = sum_j a_j > tiny; gb_k / tiny otherwise),
+ *   lpbar_k = abar_k w_k act_k e_k + grad_loglik e_k / sum_j e_j (e_k = exp(lp_k - max lp)),
+ *   qbar_k = grad_q_k - D lpbar_k / q_k,  qbar_raw_k = qbar_k sign(z^H B_k^-1 z) where q_k > tiny, else 0;
+ *   grad z = sum_k 2 qbar_raw_k B_k^-1 z,  Bbar_k = sum_t qbar_raw_kt z_t z_t^H,  ldbar_k = -sum_t lpbar_kt,
+ *   grad V_k = 2 Bbar_k V_k diag(1 / lam),  grad lam_ki = -v_i^H Bbar_k v_i / lam_i^2 + ldbar_k / lam_i,
+ *   grad w_k = sum_t abar_kt e_kt act_kt.
+ * Backward of the M-step, per (bin, class), from V (the forward's output) and the raw eigenvalues
+ * mu_i = v_i^H C' v_i of the recomputed scatter (no second eigensolve):
+ *   mubar_i = lambar_i / m (pass_i), plus, on the top eigenvector (the forward's last), -sum_i pass_i lambar_i mu_i / m^2
+ *   while mu_max > tiny ('eigenvalue', m = max(mu_max, tiny), pass_i: lam_i > floor); mubar_i = lambar_i (pass_i) and
+ *   floor lambar_i onto the top otherwise (pass_i: lam_i > lam_max floor).  The floors pass no gradient.
+ *   M_ii = mubar_i; M_ij = G_ij / (mu_j - mu_i) with G = V^H Vbar, but exactly 0 where lam_i == lam_j: B^-1 does not
+ *   change under rotations inside a block of equal model eigenvalues, and every floored block is such a block, so a
+ *   rank-deficient scatter gives finite gradients.  Cbar' = V (M + M^H) / 2 V^H.  This is exact for every loss that
+ *   sees the model through B^-1 and ld only (E-step, predict, log_likelihood); for a loss on V itself it is the
+ *   gradient with the phase and the in-block rotations held fixed.
+ *   'trace': Cbar = Cbar' / tau - Re<Cbar', C'> / tau I (tau = tr C > tiny; Cbar' / tiny otherwise).
+ *   Psibar_k = D Cbar_k / S_k,  Sbar_k = -Re<Cbar_k, C_k> / S_k + the weight's share (wbar_k / T, or
+ *   wbar_k / n - sum_j wbar_j S_j / n^2 with n = sum_j |S_j|); a class with S_k <= tiny passes no gradient;
+ *   cbar_kt = z_t^H Psibar_k z_t,  grad z_t = sum_k 2 c_kt Psibar_k z_t,  gbar_kt = cbar_kt / max(q_kt, 10 tiny) + Sbar_k,
+ *   grad gamma_kt = gbar_kt s_t,  grad q_kt = -cbar_kt g_kt / q_kt^2 (q_kt > 10 tiny, else 0),
+ *   grad s_t = sum_k gbar_kt gamma_kt.
+ * Both: grad y_t = (grad z_t - z_t Re(z_t^H grad z_t)) / |y_t|, zero for an all-zero frame.  A bin with a zero model
+ * eigenvalue (eigenvalue_floor = 0) or a non-finite sample gets NaN gradients in that bin only. */
+size_t pbb_cacgmm_predict_backward_workspace_bytes(int F, int T, int D, int K);
+
+/* Differentiates pbb_cacgmm_predict with a per-bin weight (F, K) (PBB_WEIGHT_TIME; pass 1 / K for _CONST).
+ * affiliation / quadratic: the forward's outputs (F, K, T), so the forward's softmax variant does not matter;
+ * grad_affiliation, grad_quadratic (F, K, T) and grad_loglik (F) may each be NULL (zero).  Writes grad_y (F, T, D)
+ * complex128, grad_eigenvectors (F, K, D, D) complex128, grad_eigenvalues (F, K, D) and grad_weight (F, K). */
+int pbb_cacgmm_predict_backward(const void* y, int dtype, int F, int T, int D, int K,
+                                const void* eigenvectors, const double* eigenvalues, const double* weight,
+                                const uint8_t* activity, double affiliation_eps,
+                                const double* affiliation, const double* quadratic,
+                                const double* grad_affiliation, const double* grad_quadratic,
+                                const double* grad_loglik, void* grad_y, void* grad_eigenvectors,
+                                double* grad_eigenvalues, double* grad_weight, void* workspace,
+                                size_t workspace_bytes, void* stream);
+
+size_t pbb_cacgmm_mstep_backward_workspace_bytes(int F, int T, int D, int K);
+
+/* Differentiates pbb_cacgmm_mstep (opt: the forward's options, weight_mode PBB_WEIGHT_TIME or _CONST).
+ * eigenvectors / eigenvalues: the forward's outputs; grad_eigenvectors (F, K, D, D), grad_eigenvalues (F, K, D) and
+ * grad_weight (F, K) may each be NULL (zero).  Writes grad_y (F, T, D) complex128, grad_affiliation (F, K, T),
+ * grad_quadratic (F, K, T; NULL iff quadratic is NULL) and grad_saliency (F, T; NULL iff saliency is NULL). */
+int pbb_cacgmm_mstep_backward(const void* y, int dtype, int F, int T, int D, int K,
+                              const double* affiliation, const double* quadratic, const double* saliency,
+                              const pbb_cacgmm_options* opt, const void* eigenvectors,
+                              const double* eigenvalues, const void* grad_eigenvectors,
+                              const double* grad_eigenvalues, const double* grad_weight, void* grad_y,
+                              double* grad_affiliation, double* grad_quadratic, double* grad_saliency,
+                              void* workspace, size_t workspace_bytes, void* stream);
+
 /* estimate_mixture_weight with weight_constant_axis=(-3,) / (-3, -1)
  * (mixture_model_utils.py:133-203): weight_kt[k][t] = mean over bins of
  * affiliation[f][k][t]; flags bit 0: additionally weight_k[k] = mean over t; flags bit 1:

@@ -89,6 +89,12 @@ SIGNATURES = {
     'pbb_cacgmm_mstep': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp,
                               ctypes.POINTER(CacgmmOptions), _vp, _vp, _vp,
                               _vp, _sz, _vp, _vp]),
+    'pbb_cacgmm_predict_backward_workspace_bytes': (_sz, [_i, _i, _i, _i]),
+    'pbb_cacgmm_predict_backward': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _d, _vp, _vp, _vp, _vp, _vp,
+                                         _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    'pbb_cacgmm_mstep_backward_workspace_bytes': (_sz, [_i, _i, _i, _i]),
+    'pbb_cacgmm_mstep_backward': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(CacgmmOptions), _vp,
+                                       _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     'pbb_mixture_weight_over_bins': (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'pbb_cwmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'pbb_cwmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _d,

@@ -10,6 +10,7 @@
 
 #include <cuda.h>
 
+#include "em_backward.cuh"
 #include "em_kernels.cuh"
 #include "em_persistent.cuh"
 #include "em_ws.cuh"
@@ -849,6 +850,41 @@ static int run_iterative_fit(const FitCall& c, bool fast_sm) {
   return 0;
 }
 
+// ---- backward passes (em_backward.cuh) ------------------------------------------------
+// The forward's workspace (carve), then the backward's own arrays.
+struct CacgmmBwdWorkspace {
+  CacgmmWorkspace em;
+  double* qcoef;   // (F, K, T) coefficients of the E-step adjoint's scatter
+  double* wpart;   // (F, nchb, 2K) chunk sums of the weight and log det gradients
+  double2* gpsi;   // (F, K, D, D) Psibar of the M-step adjoint
+  double* gS;      // (F, K) Sbar
+  size_t bytes;
+};
+
+static int bwd_chunks(int T) { return (T + kBwdFrames - 1) / kBwdFrames; }
+
+static CacgmmBwdWorkspace carve_bwd(void* base, int F, int T, int D, int K) {
+  CacgmmBwdWorkspace b;
+  b.em = carve(base, F, T, D, K);
+  char* p = reinterpret_cast<char*>(base);
+  size_t off = align_up(b.em.bytes);
+  auto take = [&](size_t n) { char* q = p + off; off += align_up(n); return q; };
+  b.qcoef = reinterpret_cast<double*>(take((size_t)F * K * T * sizeof(double)));
+  b.wpart = reinterpret_cast<double*>(take((size_t)F * bwd_chunks(T) * 2 * K * sizeof(double)));
+  b.gpsi = reinterpret_cast<double2*>(take((size_t)F * K * D * D * sizeof(double2)));
+  b.gS = reinterpret_cast<double*>(take((size_t)F * K * sizeof(double)));
+  b.bytes = off;
+  return b;
+}
+
+// one CTA per (bin, frame chunk) (per_frame) or per (bin, class)
+template <typename Kern, typename Args>
+static int launch_bwd(const char* name, Kern kern, dim3 grid, int threads, size_t smem, const Args& a,
+                      cudaStream_t st) {
+  PBB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  return launch_kernel(name, kern, grid, threads, smem, st, a);
+}
+
 }  // namespace pbb
 
 using namespace pbb;
@@ -856,7 +892,7 @@ using namespace pbb;
 extern "C" {
 
 const char* pbb_last_error(void) { return g_err; }
-int pbb_version(void) { return 107; }
+int pbb_version(void) { return 108; }
 
 int pbb_normalize_observation(const void* y, void* z, int F, int T, int D, int dtype, int swap, void* stream) {
   PBB_CHECK_ARG(y != nullptr, 1, "y is null");
@@ -1010,6 +1046,106 @@ int pbb_cacgmm_mstep(const void* y, int dtype, int F, int T, int D, int K, const
   UpdArgs u = upd_args(ws, F, T, D, K, opt, saliency != nullptr, eigenvectors, eigenvalues, weight, status);
   u.nch = nch;
   return launch_update(cacg_update_kernel, "cacg_update_kernel", u, st);
+}
+
+size_t pbb_cacgmm_predict_backward_workspace_bytes(int F, int T, int D, int K) {
+  if (F <= 0 || T <= 0 || D <= 0 || K <= 0) return 0;
+  return carve_bwd(nullptr, F, T, D, K).bytes;
+}
+
+size_t pbb_cacgmm_mstep_backward_workspace_bytes(int F, int T, int D, int K) {
+  return pbb_cacgmm_predict_backward_workspace_bytes(F, T, D, K);
+}
+
+int pbb_cacgmm_predict_backward(const void* y, int dtype, int F, int T, int D, int K, const void* eigenvectors,
+                                const double* eigenvalues, const double* weight, const uint8_t* activity,
+                                double affiliation_eps, const double* affiliation, const double* quadratic,
+                                const double* grad_affiliation, const double* grad_quadratic,
+                                const double* grad_loglik, void* grad_y, void* grad_eigenvectors,
+                                double* grad_eigenvalues, double* grad_weight, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  if (int r = check_shape(F, T, D, K, dtype)) return r;
+  PBB_CHECK_ARG(eigenvectors && eigenvalues && weight, 7, "model is null");
+  PBB_CHECK_ARG(affiliation && quadratic, 12, "the forward's affiliation / quadratic form is null");
+  PBB_CHECK_ARG(grad_y && grad_eigenvectors && grad_eigenvalues && grad_weight, 17, "gradient output is null");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= carve_bwd(nullptr, F, T, D, K).bytes, 21,
+                "workspace too small (pbb_cacgmm_predict_backward_workspace_bytes)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const CacgmmBwdWorkspace ws = carve_bwd(workspace, F, T, D, K);
+  int r;
+  if ((r = normalize(y, dtype, ws.em, F, T, D, false, st))) return r;
+  if ((r = launch_from_eig(ws.em, F, D, K, eigenvectors, eigenvalues, weight, st))) return r;
+  const int nchb = bwd_chunks(T);
+  EstepBwdArgs e;
+  e.y = y; e.F = F; e.T = T; e.D = D; e.K = K; e.nch = nchb;
+  e.coef = ws.em.coef; e.ld = ws.em.ld; e.w = ws.em.w; e.activity = activity; e.eps = affiliation_eps;
+  e.aff = affiliation; e.q = quadratic; e.gaff = grad_affiliation; e.gq = grad_quadratic; e.gll = grad_loglik;
+  e.qcoef = ws.qcoef; e.part = ws.wpart; e.ybar = static_cast<double2*>(grad_y);
+  if ((r = with_ct(dtype, [&](auto ct) {
+         return launch_bwd("cacgmm_estep_bwd_kernel", cacgmm_estep_bwd_kernel<decltype(ct)>, dim3(F, nchb),
+                           kBwdFrames, bwd_frame_smem(D, 3 * K), e, st);
+       })))
+    return r;
+  // Bbar^-1 = sum_t qbar_raw z z^H: the forward's scatter kernel with the coefficients as affiliations
+  EmArgs a = em_args(ws.em, F, T, D, K);
+  a.mode = kModeM; a.aff_in = ws.qcoef; a.q_in = nullptr;
+  const int nch = launch_em(a, dtype, 0, st);
+  if (nch <= 0) return nch ? nch : 1;
+  PredictSpecBwdArgs p;
+  p.F = F; p.D = D; p.K = K; p.nch = nch; p.nchb = nchb; p.part = ws.em.part; p.wpart = ws.wpart;
+  p.V = static_cast<const double2*>(eigenvectors); p.lam = eigenvalues;
+  p.gV = static_cast<double2*>(grad_eigenvectors); p.glam = grad_eigenvalues; p.gw = grad_weight;
+  const size_t smem = (size_t)2 * D * D * sizeof(double2) + (size_t)D * D * sizeof(double);
+  return launch_bwd("cacgmm_predict_spec_bwd_kernel", cacgmm_predict_spec_bwd_kernel, dim3(F, K), 32, smem, p, st);
+}
+
+int pbb_cacgmm_mstep_backward(const void* y, int dtype, int F, int T, int D, int K, const double* affiliation,
+                              const double* quadratic, const double* saliency, const pbb_cacgmm_options* opt,
+                              const void* eigenvectors, const double* eigenvalues, const void* grad_eigenvectors,
+                              const double* grad_eigenvalues, const double* grad_weight, void* grad_y,
+                              double* grad_affiliation, double* grad_quadratic, double* grad_saliency,
+                              void* workspace, size_t workspace_bytes, void* stream) {
+  PBB_CHECK_ARG(y != nullptr, 1, "y is null");
+  if (int r = check_shape(F, T, D, K, dtype)) return r;
+  PBB_CHECK_ARG(affiliation != nullptr, 7, "affiliation is null");
+  PBB_CHECK_ARG(opt != nullptr, 10, "options are null");
+  PBB_CHECK_ARG(opt->covariance_norm >= 0 && opt->covariance_norm <= 2, 10, "bad covariance_norm");
+  PBB_CHECK_ARG(opt->weight_mode == PBB_WEIGHT_TIME || opt->weight_mode == PBB_WEIGHT_CONST, 10,
+                "weight_mode: PBB_WEIGHT_TIME or PBB_WEIGHT_CONST");
+  PBB_CHECK_ARG(eigenvectors && eigenvalues, 11, "the forward's model is null");
+  PBB_CHECK_ARG(grad_y && grad_affiliation, 16, "gradient output is null");
+  PBB_CHECK_ARG((grad_quadratic != nullptr) == (quadratic != nullptr), 18, "grad_quadratic iff quadratic");
+  PBB_CHECK_ARG((grad_saliency != nullptr) == (saliency != nullptr), 19, "grad_saliency iff saliency");
+  PBB_CHECK_ARG(workspace != nullptr && workspace_bytes >= carve_bwd(nullptr, F, T, D, K).bytes, 20,
+                "workspace too small (pbb_cacgmm_mstep_backward_workspace_bytes)");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  const CacgmmBwdWorkspace ws = carve_bwd(workspace, F, T, D, K);
+  int r;
+  if ((r = normalize(y, dtype, ws.em, F, T, D, false, st))) return r;
+  // the forward's scatter sums, recomputed by the forward's launch
+  EmArgs a = em_args(ws.em, F, T, D, K);
+  a.mode = kModeM; a.aff_in = affiliation; a.q_in = quadratic; a.saliency = saliency;
+  const int nch = launch_em(a, dtype, opt->frames_per_block, st);
+  if (nch <= 0) return nch ? nch : 1;
+  MstepSpecBwdArgs m;
+  m.F = F; m.T = T; m.D = D; m.K = K; m.nch = nch; m.part = ws.em.part;
+  m.covariance_norm = opt->covariance_norm; m.weight_mode = opt->weight_mode; m.has_saliency = saliency != nullptr;
+  m.eigenvalue_floor = opt->eigenvalue_floor;
+  m.V = static_cast<const double2*>(eigenvectors); m.lam = eigenvalues;
+  m.gV = static_cast<const double2*>(grad_eigenvectors); m.glam = grad_eigenvalues; m.gw = grad_weight;
+  m.gpsi = ws.gpsi; m.gS = ws.gS;
+  if ((r = launch_bwd("cacgmm_mstep_spec_bwd_kernel", cacgmm_mstep_spec_bwd_kernel, dim3(F, K), 32,
+                      mstep_spec_bwd_smem(D), m, st)))
+    return r;
+  MstepBwdArgs b;
+  b.y = y; b.F = F; b.T = T; b.D = D; b.K = K; b.nch = bwd_chunks(T);
+  b.aff = affiliation; b.q = quadratic; b.saliency = saliency; b.gpsi = ws.gpsi; b.gS = ws.gS;
+  b.gaff = grad_affiliation; b.gq = grad_quadratic; b.gsal = grad_saliency; b.ybar = static_cast<double2*>(grad_y);
+  return with_ct(dtype, [&](auto ct) {
+    return launch_bwd("cacgmm_mstep_bwd_kernel", cacgmm_mstep_bwd_kernel<decltype(ct)>, dim3(F, b.nch), kBwdFrames,
+                      bwd_frame_smem(D, 0), b, st);
+  });
 }
 
 size_t pbb_cwmm_workspace_bytes(int F, int T, int D, int K) { return pbb_cacgmm_workspace_bytes(F, T, D, K); }

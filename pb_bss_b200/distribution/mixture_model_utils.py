@@ -148,7 +148,7 @@ def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, a
                 saliency_form, total_bins=None, bin_group=None):
     """EM whose bins couple in every iteration: frequency-tied mixture weights (``weight_constant_axis`` (-3,) /
     (-3, -1), mixture_model_utils.py:187-190) and / or the inline permutation alignment
-    (mixture_model_utils.py:264-306).  The loop is the reference's (cacgmm.py:252-278, cwmm.py:152-184,
+    (mixture_model_utils.py:264-306); with per-bin weights (the cACGMM fit with a graph) the model is the M-step's.  The loop is the reference's (cacgmm.py:252-278, cwmm.py:152-184,
     cbmm.py:186-203); every step runs on the device and the status words are read once, after the last iteration.
 
     yd: (F, N, D) device observation; affiliation: initial (F, K, N) device affiliations, or ``model`` to start from;
@@ -190,6 +190,8 @@ def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, a
                         quadratic_form = apply_mapping(quadratic_form.permute(1, 0, 2).contiguous(),
                                                        mapping).permute(1, 0, 2).contiguous()
             model = m_step(affiliation, quadratic_form)
+            if mode not in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED):
+                continue  # per-bin weights (the cACGMM fit with a graph): the M-step's own
             # the tied weight: with a saliency, the sum of affiliation * saliency (mixture_model_utils.py:192-203)
             K = affiliation.shape[1]
             masked = masked_affiliation(affiliation, sal).contiguous()
