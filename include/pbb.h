@@ -216,14 +216,19 @@ int pbb_cacgmm_mstep(const void* y, int dtype, int F, int T, int D, int K,
  *   mubar_i = lambar_i / m (pass_i), plus, on the top eigenvector (the forward's last), -sum_i pass_i lambar_i mu_i / m^2
  *   while mu_max > tiny ('eigenvalue', m = max(mu_max, tiny), pass_i: lam_i > floor); mubar_i = lambar_i (pass_i) and
  *   floor lambar_i onto the top otherwise (pass_i: lam_i > lam_max floor).  The floors pass no gradient.
- *   M_ii = mubar_i; M_ij = G_ij / (mu_j - mu_i) with G = V^H Vbar, but exactly 0 where lam_i == lam_j: B^-1 does not
- *   change under rotations inside a block of equal model eigenvalues, and every floored block is such a block, so a
- *   rank-deficient scatter gives finite gradients.  Cbar' = V (M + M^H) / 2 V^H.  This is exact for every loss that
- *   sees the model through B^-1 and ld only (E-step, predict, log_likelihood); for a loss on V itself it is the
- *   gradient with the phase and the in-block rotations held fixed.
+ *   M_ii = mubar_i; M_ij = G_ij / (mu_j - mu_i) with G = V^H Vbar, except where |mu_j - mu_i| <= 2^-26 mu_max (a tie):
+ *   there M_ij = -lam' (G_ij + conj G_ji) / (2 (lam_i + lam_j)) if neither eigenvalue is floored (lam' = d lam / d mu:
+ *   1 / m for 'eigenvalue', else 1), the Daleckii-Krein limit -lam' P_ij / lam^2 of a B^-1 consumer, whose
+ *   G = 2 P diag(1 / lam) with P = V^H Bbar V.  Every pair of floored eigenvalues gives 0 (1 / lam is constant on the
+ *   floor), so a rank-deficient scatter gives finite gradients; a floored and an unfloored eigenvalue take the divided
+ *   difference, but 0 where |mu_j - mu_i| <= 64 u D mu_max (both at the floor's kink, within the rounding of mu).  Cbar' = V (M + M^H) / 2 V^H.  This is
+ *   exact for every loss that sees the model through B^-1 and ld only (E-step, predict, log_likelihood); for a loss on
+ *   V itself it is the gradient with the phase held fixed, and at a tie a convention.  At a tied top eigenvalue m is
+ *   the Rayleigh quotient of the forward's last eigenvector, held fixed.
  *   'trace': Cbar = Cbar' / tau - Re<Cbar', C'> / tau I (tau = tr C > tiny; Cbar' / tiny otherwise).
  *   Psibar_k = D Cbar_k / S_k,  Sbar_k = -Re<Cbar_k, C_k> / S_k + the weight's share (wbar_k / T, or
- *   wbar_k / n - sum_j wbar_j S_j / n^2 with n = sum_j |S_j|); a class with S_k <= tiny passes no gradient;
+ *   wbar_k / n - sum_j wbar_j S_j / n^2 with n = sum_j |S_j|); a class with S_k <= tiny passes no gradient (the
+ *   forward forms its covariance as D Psi_k / tiny, a finite model: C_k = 0 at S_k = 0);
  *   cbar_kt = z_t^H Psibar_k z_t,  grad z_t = sum_k 2 c_kt Psibar_k z_t,  gbar_kt = cbar_kt / max(q_kt, 10 tiny) + Sbar_k,
  *   grad gamma_kt = gbar_kt s_t,  grad q_kt = -cbar_kt g_kt / q_kt^2 (q_kt > 10 tiny, else 0),
  *   grad s_t = sum_k gbar_kt gamma_kt.

@@ -15,6 +15,13 @@
 namespace pbb {
 
 constexpr int kBwdFrames = 64;  // frames per CTA of the per-frame backward kernels
+// Two unfloored eigenvalues of the M-step backward count as tied where |mu_i - mu_j| <= kTieGap mu_max (= sqrt(u)):
+// past it the divided difference loses at most ~u D mu_max / gap <= sqrt(u) D; below it the eigenvectors themselves
+// are not determined to better than that.  A floored and an unfloored eigenvalue (both at the floor's kink, where the
+// divided difference lies between 0 and -lam' / lam^2) take the divided difference unless their gap is within the
+// rounding of the Rayleigh quotients, kKinkGap D mu_max, where they give 0.
+constexpr double kTieGap = 0x1p-26;
+constexpr double kKinkGap = 64.0 * 0x1p-52;
 
 // Shared memory of the per-frame kernels: z and zbar as [D][kBwdFrames], one D x D class matrix, nk rows of
 // per-frame scalars, then the per-frame norm and projection.
@@ -395,7 +402,14 @@ __global__ void __launch_bounds__(32) cacgmm_mstep_spec_bwd_kernel(const MstepSp
     mub[top] += topb;
   }
   __syncwarp();
-  // G = V^H Vbar; M = diag(mubar) + (Vbar-term / (mu_j - mu_i)), zero between equal model eigenvalues
+  // G = V^H Vbar; M = diag(mubar) + the Vbar term of each pair (pbb.h): the divided difference over mu_c - mu_r, or
+  // the tie limit for two unfloored eigenvalues within kTieGap mu_max, or 0 for two floored ones and for a floored and
+  // an unfloored one within kKinkGap D mu_max.  Every test is on the divisor itself, so no rounding of lam can send a
+  // zero gap into the division.
+  const bool eig = a.covariance_norm == PBB_NORM_EIGENVALUE;
+  const double thr = eig ? a.eigenvalue_floor : lam[D - 1] * a.eigenvalue_floor;  // unfloored: lam > thr
+  const double dl = eig ? 1.0 / fmax(mu[D - 1], kTiny) : 1.0;                  // d lam / d mu where unfloored
+  const double tie = kTieGap * mu[D - 1], kink = kKinkGap * D * mu[D - 1];
   for (int j = lane; j < NS; j += 32) {
     const int r = j / D, c = j - r * D;
     double re = 0.0, im = 0.0;
@@ -414,11 +428,20 @@ __global__ void __launch_bounds__(32) cacgmm_mstep_spec_bwd_kernel(const MstepSp
     double2 v = make_double2(0.0, 0.0);
     if (r == c) {
       v.x = mub[r];
-    } else if (lam[r] != lam[c]) {
-      // (M + M^H) / 2 with M_rc = G_rc / (mu_c - mu_r)
+    } else {
       const double2 g1 = G[r * D + c], g2 = G[c * D + r];
-      const double inv = 0.5 / (mu[c] - mu[r]);
-      v = make_double2((g1.x - g2.x) * inv, (g1.y + g2.y) * inv);
+      const bool pr = lam[r] > thr, pc = lam[c] > thr;
+      const double gap = fabs(mu[c] - mu[r]);
+      if (pr && pc && !(gap > tie)) {
+        // tie limit -lam' P_rc / lam^2, P = V^H Bbar V, from G = 2 P diag(1 / lam):
+        // M_rc = -lam' (G_rc + conj G_cr) / (2 (lam_r + lam_c)), Hermitian
+        const double s = -dl / (2.0 * (lam[r] + lam[c]));
+        v = make_double2((g1.x + g2.x) * s, (g1.y - g2.y) * s);
+      } else if ((pr && pc) || ((pr || pc) && gap > kink)) {
+        // (M + M^H) / 2 with M_rc = G_rc / (mu_c - mu_r)
+        const double inv = 0.5 / (mu[c] - mu[r]);
+        v = make_double2((g1.x - g2.x) * inv, (g1.y + g2.y) * inv);
+      }
     }
     M[j] = v;
   }

@@ -535,14 +535,16 @@ __global__ void cacg_update_kernel(const UpdArgs u) {
       if (s < NS) S[s] = sum; else sumg[k] = sum;
     }
     __syncwarp();
-    // 2. covariance = D * S / max(sum gamma, tiny)      (cacg.py:316-330)
+    // 2. covariance = D * S / max(sum gamma, tiny)      (cacg.py:316-330); for sum gamma <= tiny as D S / tiny,
+    // since D / tiny overflows for D >= 4 (2^-1022 is tiny, so the division is an exact power-of-two scaling)
+    const bool live = sumg[k] > kTiny;
     const double scale = (double)D / fmax(sumg[k], kTiny);
     bool bad = false;
     double* Ad = reinterpret_cast<double*>(A);
     for (int s = lane; s < NS; s += 32) {
       const int pk = tab[s];
       const int d = pk & 255, e = (pk >> 8) & 255, kind = pk >> 16;
-      const double v = S[s] * scale;
+      const double v = live ? S[s] * scale : ((double)D * S[s]) * 0x1p1022;
       bad |= !isfinite(v);
       if (kind == 0) { Ad[2 * (d * D + d)] = v; Ad[2 * (d * D + d) + 1] = 0.0; }
       else if (kind == 1) { Ad[2 * (d * D + e)] = v; Ad[2 * (e * D + d)] = v; }

@@ -14,11 +14,12 @@ saliency and a warm-start model's tensors.  The backward passes are pbb_cacgmm_m
 pbb_cacgmm_predict_backward (closed forms in include/pbb.h): gradients come back in the input's dtype, repeated
 backward calls are bitwise identical, the backward only enqueues work, and double backward raises.  The floors and
 clips pass no gradient where they are active, a zero frame has a zero gradient, the source activity mask is a
-constant, a class whose affiliations sum to at most tiny passes no gradient, and a pair of equal model eigenvalues (a
-floored block) contributes nothing through the eigenvectors, so rank-deficient scatter matrices give finite
-gradients.  The eigenvector gradient is exact for every loss that sees the model through B^-1 and log det B (predict,
-log_likelihood, the next E-step); for a loss on the eigenvectors themselves it holds their phase and the rotations
-inside a block of equal eigenvalues fixed.  A bin with a zero model eigenvalue or a non-finite sample gets NaN
+constant, a class whose affiliations sum to at most tiny passes no gradient, and a pair of floored model eigenvalues
+contributes nothing through the eigenvectors, so rank-deficient scatter matrices give finite gradients.  Tied
+unfloored eigenvalues take the Daleckii-Krein limit, and a floored and an unfloored eigenvalue within rounding of
+each other (at the floor's kink) contribute nothing.  The eigenvector gradient is exact for every loss that sees the
+model through B^-1 and log det B (predict, log_likelihood, the next E-step); for a loss on the eigenvectors
+themselves it holds their phase fixed, and at a tie it is that convention.  A bin with a zero model eigenvalue or a non-finite sample gets NaN
 gradients in that bin only.
 
 The M-step, predict and log_likelihood with a graph launch what they launch without one, so their outputs are

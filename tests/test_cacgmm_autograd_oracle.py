@@ -124,3 +124,203 @@ def test_loewner_backward_matches_central_differences_at_a_floored_bin():
         num = (loss(C + h * E) - loss(C - h * E)).item() / (2 * h)
         ana = (Cg.grad.conj() * E).real.sum().item()
         assert abs(num - ana) <= 1e-5 * max(1.0, abs(num)), (i, j, part, num, ana)
+
+
+# ---- the restatement's gradients against mpmath directional derivatives ----------------------------------------------
+U = np.finfo(np.float64).eps
+
+
+def _dirs(rng, inputs):
+    return {k: (rng.standard_normal(v.shape) + 1j * rng.standard_normal(v.shape)) if np.iscomplexobj(v)
+            else rng.standard_normal(v.shape) for k, v in inputs.items()}
+
+
+def _check_mp(grads, inputs, rng, bound, n_dirs=2, **kw):
+    """Re <grad, dir> against mpmath's directional derivative along random directions: |err| <= bound * sum |grad|
+    |dir| (the derivative's own scale); returns the worst err / bound"""
+    worst = 0.0
+    for _ in range(n_dirs):
+        dirs = _dirs(rng, inputs)
+        ref = A.mp_directional(inputs, dirs, **kw)
+        got = A.directional(grads, dirs)
+        scale = sum(float(np.sum(np.abs(grads[k]) * np.abs(dirs[k]))) for k in dirs)
+        ratio = abs(got - ref) / (bound * scale)
+        assert ratio <= 1, (got, ref, scale)
+        worst = max(worst, ratio)
+    return worst
+
+
+def _m_step_grads(y, init, q, sal, R, probe=None, mask=None, iterations=1, **kw):
+    """gradients of sum R * predict(probe) + 0.1 log_likelihood(probe) through the restatement's m_step / fit"""
+    inputs = dict(y=y, init=init)
+    if q is not None:
+        inputs['q'] = q
+    if sal is not None:
+        inputs['saliency'] = sal
+    ts = {k: _t(v).requires_grad_() for k, v in inputs.items()}
+    if iterations == 1:
+        m = A.m_step(ts['y'], ts.get('q'), ts['init'], ts.get('saliency'), **kw)
+    else:
+        m = A.fit(ts['y'], ts['init'], iterations, saliency=ts.get('saliency'),
+                  source_activity_mask=None if mask is None else _t(mask), **kw)
+    yp = ts['y'] if probe is None else _t(probe)
+    loss = (_t(R) * A.predict(yp, m)).sum() + 0.1 * A.log_likelihood(yp, m)
+    g = torch.autograd.grad(loss, list(ts.values()))
+    return {k: v.numpy() for k, v in zip(ts, g)}, inputs, m
+
+
+MP_CASES = [
+    # norm, options
+    ('eigenvalue', {}),
+    ('trace', {}),
+    (False, {}),
+    ('eigenvalue', {'saliency': True}),
+    ('trace', {'saliency': True, 'q': True}),
+    ('eigenvalue', {'weight_constant_axis': -2, 'q': True}),
+    ('eigenvalue', {'iterations': 2, 'mask': True}),
+    ('trace', {'iterations': 3, 'affiliation_eps': 0.}),
+    (False, {'iterations': 2, 'saliency': True}),
+]
+
+
+@pytest.mark.parametrize('norm,opts', MP_CASES)
+def test_m_step_and_fit_gradients_match_mpmath(norm, opts):
+    F, T, D, K = 1, 10, 4, 2
+    y, _ = synth.structured_stft(F, T, D, K, seed=21)
+    init = synth.init_affiliation(F, K, T, seed=22)
+    rng = np.random.RandomState(23)
+    q = rng.uniform(0.5, 2.0, (F, K, T)) if opts.get('q') else None
+    sal = rng.uniform(0.2, 1.0, (F, T)) if opts.get('saliency') else None
+    mask = rng.uniform(size=(F, K, T)) > 0.25 if opts.get('mask') else None
+    R = rng.standard_normal((F, K, T))
+    it = opts.get('iterations', 1)
+    kw = dict(covariance_norm=norm)
+    mp_kw = dict(covariance_norm=norm, iterations=it, R=R, mask=mask)
+    if 'weight_constant_axis' in opts:
+        kw['weight_constant_axis'] = mp_kw['weight_constant_axis'] = opts['weight_constant_axis']
+    if it > 1:
+        kw['affiliation_eps'] = mp_kw['affiliation_eps'] = opts.get('affiliation_eps', 1e-10)
+    grads, inputs, _ = _m_step_grads(y, init, q, sal, R, mask=mask, iterations=it, **kw)
+    worst = _check_mp(grads, inputs, rng, 1e-11, **mp_kw)
+    print(f'\nrestatement vs mpmath {norm} {opts}: worst err / bound {worst:.2e}')
+
+
+def test_predict_and_log_likelihood_gradients_match_mpmath():
+    F, T, D, K = 2, 12, 4, 3
+    y, _ = synth.structured_stft(F, T, D, K, seed=24)
+    init = synth.init_affiliation(F, K, T, seed=25)
+    m0 = A.m_step(_t(y), None, _t(init))
+    inputs = dict(y=y, V=m0['eigenvectors'].numpy(), lam=m0['eigenvalues'].numpy(), w=m0['weight'][..., 0].numpy())
+    rng = np.random.RandomState(26)
+    R = rng.standard_normal((F, K, T))
+    ts = {k: _t(v).requires_grad_() for k, v in inputs.items()}
+    m = A.from_eig(ts['V'], ts['lam'], ts['w'][..., None])
+    loss = (_t(R) * A.predict(ts['y'], m)).sum() + 0.1 * A.log_likelihood(ts['y'], m)
+    g = dict(zip(ts, (v.numpy() for v in torch.autograd.grad(loss, list(ts.values())))))
+    _check_mp(g, inputs, rng, 1e-11, iterations=0, R=R)
+
+
+# ---- ties, near ties, floored blocks and the top eigenvalue ----------------------------------------------------------
+@pytest.mark.parametrize('norm', ['eigenvalue', 'trace', False])
+def test_spectral_model_at_an_exact_unfloored_tie_matches_central_differences(norm):
+    """C = diag(0.5, 0.5, 1): a perturbation that splits the tied pair changes B^-1 at first order (the divided
+    difference tends to -lam' / lam^2, not to 0)"""
+    C = _t(np.diag([0.5, 0.5, 1.0]).astype(np.complex128))
+    G = _t(np.random.RandomState(13).randn(3, 3) + 1j * np.random.RandomState(14).randn(3, 3))
+
+    def loss(c):
+        c = (c + c.mH) / 2
+        with torch.no_grad():
+            top = torch.linalg.eigh(c)[1][..., -1:]
+        m = (top.mH @ c @ top).real[..., 0]
+        binv, ld = A.SpectralModel.apply(c, m, 1e-3, norm)
+        return (G.conj() * binv).real.sum() + 0.3 * ld
+
+    Cg = C.clone().requires_grad_()
+    loss(Cg).backward()
+    h = 1e-6
+    for i, j, part in [(0, 1, 1), (0, 1, 1j), (0, 0, 1), (1, 2, 1), (0, 2, 1j)]:
+        E = torch.zeros(3, 3, dtype=torch.complex128)
+        E[i, j] = part
+        E[j, i] += np.conj(part) if i != j else 0
+        num = (loss(C + h * E) - loss(C - h * E)).item() / (2 * h)
+        ana = (Cg.grad.conj() * E).real.sum().item()
+        assert abs(num - ana) <= 1e-6 * max(1.0, abs(num)), (i, j, part, num, ana)
+
+
+@pytest.mark.parametrize('norm', ['eigenvalue', 'trace', False])
+@pytest.mark.parametrize('D', [3, 5])
+def test_exact_ties_below_the_top_match_mpmath(norm, D):
+    # class 0: a pair tied below the top; class 1: one pair (D = 3) or two pairs (D = 5) tied below a simple top
+    w0 = [0.3, 0.3] + [0.5 + 0.1 * d for d in range(D - 2)]
+    w1 = [0.2, 0.2] + [0.45] * (D - 3) + [0.8]
+    y, init, probe, R = A.tie_data(D, [w0, w1])
+    grads, inputs, m = _m_step_grads(y, init, None, None, R, probe=probe, covariance_norm=norm)
+    lam = m['eigenvalues'].numpy()[0]
+    assert lam[0, 0] == lam[0, 1] and lam[1, 0] == lam[1, 1] and np.all(lam > 1e-10)
+    _check_mp(grads, inputs, np.random.RandomState(D), 1e-11, n_dirs=3, covariance_norm=norm, R=R, probe=probe)
+
+
+@pytest.mark.parametrize('gap', [1e-2, 1e-4, 1e-6, 1e-8, 1e-10, 1e-12])
+@pytest.mark.parametrize('norm', ['eigenvalue', False])
+def test_near_ties_match_mpmath(gap, norm):
+    """a relative gap between two unfloored eigenvalues: the closed form has no cancellation, so the error stays far
+    below u D / gap (the loss of a divided difference of computed eigenvalues)"""
+    D = 4
+    y, init, probe, R = A.tie_data(D, [[0.3, 0.3 * (1 + gap), 0.5, 0.9], [0.7, 0.2, 0.2 * (1 + gap), 0.4]], seed=1)
+    grads, inputs, _ = _m_step_grads(y, init, None, None, R, probe=probe, covariance_norm=norm)
+    rng = np.random.RandomState(2)
+    worst = _check_mp(grads, inputs, rng, max(1e-11, U * D / gap), n_dirs=2, covariance_norm=norm, R=R, probe=probe)
+    # and the closed form is accurate to ~1e-11 at every gap, not only within u D / gap
+    _check_mp(grads, inputs, rng, 1e-11, n_dirs=1, covariance_norm=norm, R=R, probe=probe)
+    print(f'\nnear tie gap {gap:.0e} {norm}: worst err / (u D / gap) {worst:.2e}')
+
+
+@pytest.mark.parametrize('norm', ['eigenvalue', 'trace', False])
+@pytest.mark.parametrize('rank', [1, 2, 3])
+def test_floored_blocks_match_mpmath(norm, rank):
+    """observations in a rank-r subspace of D = 4: D - r floored eigenvalues (multiplicity 3, 2, 1), whose block of
+    B^-1 is 1 / floor and passes no gradient through the floor"""
+    F, T, D, K = 1, 10, 4, 2
+    rng = np.random.RandomState(30 + rank)
+    basis = rng.randn(rank, D) + 1j * rng.randn(rank, D)
+    y = ((rng.randn(T, rank) + 1j * rng.randn(T, rank)) @ basis)[None]
+    init = synth.init_affiliation(F, K, T, seed=rank)
+    probe = rng.randn(1, 5, D) + 1j * rng.randn(1, 5, D)
+    R = rng.standard_normal((F, K, 5))
+    floor = 1e-3
+    grads, inputs, m = _m_step_grads(y, init, None, None, R, probe=probe, covariance_norm=norm, eigenvalue_floor=floor)
+    lam = m['eigenvalues'].numpy()[0]
+    assert np.sum(lam[0] == lam[0, 0]) == D - rank
+    _check_mp(grads, inputs, rng, 1e-10, n_dirs=2, covariance_norm=norm, eigenvalue_floor=floor, R=R, probe=probe)
+
+
+@pytest.mark.parametrize('norm', ['eigenvalue', 'trace', False])
+def test_tied_top_eigenvalue_follows_the_forwards_top_eigenvector(norm):
+    """At a tie at the top, mu_max is not differentiable.  The convention: m is the Rayleigh quotient of the forward's
+    top eigenvector, held fixed (the derivative of mu_max wherever the top is simple).  A floored eigenvalue makes m
+    matter for every norm."""
+    D = 4
+    y, init, probe, R = A.tie_data(D, [[0.0, 0.4, 0.7, 0.7], [0.5, 0.0, 0.9, 0.9]], seed=3)
+    grads, inputs, m = _m_step_grads(y, init, None, None, R, probe=probe, covariance_norm=norm, eigenvalue_floor=1e-3)
+    lam = m['eigenvalues'].numpy()[0]
+    assert lam[0, -1] == lam[0, -2] and lam[1, -1] == lam[1, -2]
+    _check_mp(grads, inputs, np.random.RandomState(4), 1e-11, n_dirs=3, covariance_norm=norm, eigenvalue_floor=1e-3,
+              R=R, probe=probe, top=m['eigenvectors'].numpy())
+
+
+@pytest.mark.parametrize('dead', [0.0, 1e-310])
+def test_dead_class_passes_no_gradient_and_no_nan(dead):
+    """S_k <= tiny: exactly 0 (C_k = 0) or subnormal (C_k = D Psi_k / tiny, an O(1) covariance that depends on y)"""
+    F, T, D, K = 1, 20, 4, 3
+    y, _ = synth.structured_stft(F, T, D, K, seed=40)
+    init = synth.init_affiliation(F, K, T, seed=41)
+    init[0, 2] = dead
+    probe = np.random.RandomState(42).randn(1, 5, D) + 1j * np.random.RandomState(43).randn(1, 5, D)
+    R = np.random.RandomState(44).standard_normal((F, K, 5))
+    q = np.random.RandomState(45).uniform(0.5, 2.0, (F, K, T))
+    grads, _, m = _m_step_grads(y, init, q, None, R, probe=probe)
+    assert np.all(np.isfinite(m['eigenvalues'].numpy()))
+    for k, v in grads.items():
+        assert np.all(np.isfinite(v)), k
+    assert not np.any(grads['init'][0, 2]) and not np.any(grads['q'][0, 2])
