@@ -126,6 +126,25 @@ def lu_solve(A, B):
     return B
 
 
+def lstsq_solve(R, P):
+    """np.linalg.lstsq's minimum-norm R^-1 P for an R whose singular part is exactly zero rows and columns (a dead
+    channel of Y zeroes its taps rows of Yt, so those rows and columns of R and those rows of P are 0): the live
+    block solved by lu_solve, zeros in the dead rows.  Any dtype, long double included."""
+    live = np.flatnonzero(np.any(R != 0, axis=1))
+    dead = np.setdiff1d(np.arange(R.shape[0]), live)
+    assert not np.any(R[:, dead]) and not np.any(P[dead]), 'the singular part of R is not exactly zero rows'
+    G = np.zeros(P.shape, np.result_type(R, P))
+    if live.size:
+        G[live] = lu_solve(R[np.ix_(live, live)], P[live])
+    return G
+
+
+def live_kappa(R):
+    """kappa (1-norm) of the block of R that lstsq_solve solves"""
+    live = np.flatnonzero(np.any(R != 0, axis=1))
+    return kappa(R[np.ix_(live, live)])
+
+
 def y_tilde(Y, taps, delay):
     D, T = Y.shape
     out = np.zeros((taps * D, T), dtype=Y.dtype)
@@ -144,14 +163,17 @@ def _m(T, taps, delay, statistics_mode):
 
 
 def step_forward(Y, w, taps, delay, statistics_mode='full'):
-    """one bin: (X, G, R); G = 0 and R = 0 for an empty S"""
+    """one bin: (X, G, R); G = 0 and R = 0 for an empty S; an exactly zero pivot takes lstsq_solve"""
     D, T = Y.shape
     Yt = y_tilde(Y, taps, delay)
     wm = w * _m(T, taps, delay, statistics_mode).astype(w.dtype)
     R = (Yt * wm) @ Yt.conj().T
     if not wm.any():
         return Y.copy(), np.zeros((taps * D, D), Y.dtype), R
-    G = lu_solve(R, (Yt * wm) @ Y.conj().T)
+    P = (Yt * wm) @ Y.conj().T
+    G = lu_solve(R, P)
+    if G is None:
+        G = lstsq_solve(R, P)
     return Y - G.conj().T @ Yt, G, R
 
 

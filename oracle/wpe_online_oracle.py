@@ -52,25 +52,31 @@ def get_power_online(signal):
 
 
 def initial_state(F, D, taps, delay, dtype=np.complex128):
+    """zeros, Q = I, G = 0; Q and G in complex128, or in dtype where that is wider (np.clongdouble)"""
     n = taps * D
+    cd = np.result_type(dtype, np.complex128)
     return OnlineState(np.zeros((taps + delay, F, D), dtype),
-                       np.broadcast_to(np.eye(n, dtype=np.complex128), (F, n, n)).copy(),
-                       np.zeros((F, n, D), np.complex128))
+                       np.broadcast_to(np.eye(n, dtype=cd), (F, n, n)).copy(),
+                       np.zeros((F, n, D), cd))
 
 
 def online_wpe(Y, taps, delay, alpha, state=None, details=False):
     """Y (T, F, D) -> (Z (T, F, D), state); every frame is one online_wpe_step with lambda = get_power_online of its
-    buffer.  details: also kappa(Q_t) per bin and frame (Q_t = R_t^-1, so this is kappa(R_t)), shape (T, F)."""
+    buffer.  The recursion runs in complex128, or in Y's dtype where that is wider (np.clongdouble: the long-double
+    reference).  details: also kappa(Q_t) per bin and frame (Q_t = R_t^-1, so this is kappa(R_t)), shape (T, F),
+    the ratio of the extreme eigenvalue moduli of a complex128 copy of the Hermitian Q_t (its 2-norm condition
+    number)."""
     Y = np.asarray(Y)
     T, F, D = Y.shape
+    cd = np.result_type(Y.dtype, np.complex128)
     if state is None:
         state = initial_state(F, D, taps, delay, Y.dtype)
-    hist = np.asarray(state.history, dtype=np.complex128)
-    Q = np.asarray(state.inv_cov, dtype=np.complex128)
-    G = np.asarray(state.filter_taps, dtype=np.complex128)
-    stream = np.concatenate([hist, Y.astype(np.complex128)])
+    hist = np.asarray(state.history, dtype=cd)
+    Q = np.asarray(state.inv_cov, dtype=cd)
+    G = np.asarray(state.filter_taps, dtype=cd)
+    stream = np.concatenate([hist, Y.astype(cd)])
     L = taps + delay + 1
-    Z = np.empty((T, F, D), np.complex128)
+    Z = np.empty((T, F, D), cd)
     kappa = np.empty((T, F))
     with np.errstate(invalid='ignore', divide='ignore'):
         for t in range(T):
@@ -78,7 +84,8 @@ def online_wpe(Y, taps, delay, alpha, state=None, details=False):
             power = get_power_online(buf.transpose(1, 2, 0))
             Z[t], Q, G = online_wpe_step(buf, power, Q, G, alpha, taps, delay)
             if details:
-                kappa[t] = np.linalg.cond(Q)
+                lam = np.abs(np.linalg.eigvalsh(Q.astype(np.complex128)))
+                kappa[t] = lam.max(axis=-1) / lam.min(axis=-1)
     out = OnlineState(stream[T:].astype(Y.dtype), Q, G)
     Z = Z.astype(Y.dtype)
     return (Z, out, kappa) if details else (Z, out)
