@@ -263,19 +263,11 @@ int pbb_cacgmm_mstep_backward(const void* y, int dtype, int F, int T, int D, int
                               double* grad_affiliation, double* grad_quadratic, double* grad_saliency,
                               void* workspace, size_t workspace_bytes, void* stream);
 
-/* estimate_mixture_weight with weight_constant_axis=(-3,) / (-3, -1)
- * (mixture_model_utils.py:133-203): weight_kt[k][t] = mean over bins of
- * affiliation[f][k][t]; flags bit 0: additionally weight_k[k] = mean over t; flags bit 1:
- * the saliency form (:192-203, what CWMMTrainer uses, cwmm.py:129-130): the result is
- * L1-normalised over the classes (zero norm -> 1e-10). */
-int pbb_mixture_weight_over_bins(const double* affiliation, int F, int K, int T,
-                                 int flags, double* weight_kt,
-                                 double* weight_k, void* stream);
-
 /* ------------------------------------------------------------------------
  * Integrated spatial + spectral model (pb_bss/distribution/gcacgmm.py): cACG of the observation combined with a
  * Gaussian over per-(bin, frame) embeddings (F, T, E).  The spatial part reuses pbb_cacgmm_predict (quadratic form)
- * and pbb_cacgmm_mstep; these entries are the pieces around them.
+ * and pbb_cacgmm_mstep; these entries are the pieces around them.  The mixture weights are pbb_axis_sum and
+ * pbb_unit_norm.
  * ------------------------------------------------------------------------ */
 
 /* ComplexAngularCentralGaussian._log_pdf (cacg.py:198-201) from the quadratic form: log_pdf = -D log max(|q|, tiny)
@@ -316,15 +308,11 @@ int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
                                double affiliation_eps, int inline_pa, int F, int K, int T,
                                double* affiliation, int* permutation, void* stream);
 
-/* Per-bin class weights of the integrated models (gcacgmm.py:286-291, weight_constant_axis (-1,)):
- * weight[f][k] = sum_t m[f][k][t] / sum_k sum_t m[f][k][t]. */
-int pbb_class_weight(const double* masked_affiliation, int F, int K, int T, double* weight,
-                     void* stream);
-
 /* ------------------------------------------------------------------------
  * Embedding mixture models with independent leading dims (pb_bss/distribution/gmm.py, vmfmm.py): B independent
  * models of K classes over N embeddings of dimension E each.  embedding (B, N, E), weights / log pdfs (B, K, N).
- * E <= 64, K <= 6 (the posterior, pbb_log_pdf_to_affiliation with F = B, T = N). */
+ * E <= 64, K <= 6 (the posterior, pbb_log_pdf_to_affiliation with F = B, T = N).  The mixture weights are
+ * pbb_axis_sum and pbb_unit_norm. */
 
 /* Gaussian.log_pdf (gaussian.py:36-56) with full covariance: mean (B, K, E), precision_cholesky U (B, K, E, E) (only
  * the upper triangle is read), log_det (B, K) -> log_pdf (B, K, N).  The reference contracts sklearn's
@@ -359,12 +347,6 @@ int pbb_vmf_log_pdf(const double* embedding, const double* mean, const double* c
  * reduction and scratch size as pbb_gaussian_full_fit. */
 int pbb_vmf_resultant(const double* embedding, const double* weight, int B, int N, int E, int K, double* resultant,
                       double* total, double* scratch, void* stream);
-
-/* estimate_mixture_weight with weight_constant_axis (-2,) and a saliency (mixture_model_utils.py:178-201): the tuple
- * is not caught by the reference's int test, so the masked affiliations (B, K, N) are summed over the classes and
- * L1-normalised over that singleton axis: weight (B, N) = s / |s|, 0 where s == 0.  Feed it to
- * pbb_log_pdf_to_affiliation as PBB_WEIGHT_FRAME. */
-int pbb_frame_weight(const double* masked_affiliation, int B, int K, int N, double* weight, void* stream);
 
 /* ------------------------------------------------------------------------
  * Complex Watson mixture model (pb_bss/distribution/cwmm.py, complex_watson.py).

@@ -95,7 +95,6 @@ SIGNATURES = {
     'pbb_cacgmm_mstep_backward_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'pbb_cacgmm_mstep_backward': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(CacgmmOptions), _vp,
                                        _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    'pbb_mixture_weight_over_bins': (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'pbb_cwmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
     'pbb_cwmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _d,
                           _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
@@ -121,14 +120,12 @@ SIGNATURES = {
     'pbb_gaussian_fit_scratch_doubles': (ctypes.c_size_t, [_i, _i, _i]),
     'pbb_gaussian_fit': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_log_pdf_to_affiliation': (_i, [_vp, _vp, _d, _d, _vp, _i, _vp, _d, _i, _i, _i, _i, _vp, _vp, _vp]),
-    'pbb_class_weight': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'pbb_gaussian_full_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'pbb_gaussian_full_fit_scratch_doubles': (_sz, [_i, _i, _i, _i]),
     'pbb_gaussian_full_fit': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_precision_cholesky': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
     'pbb_vmf_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'pbb_vmf_resultant': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_frame_weight': (_i, [_vp, _i, _i, _i, _vp, _vp]),
     'pbb_dhtv_mapping': (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i), _i, _vp, _vp, _vp, _vp]),
     'pbb_dhtv_mapping_ex': (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i), _i, _vp, _vp, _vp, _i, _i, _vp]),
     'pbb_apply_mapping': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),

@@ -45,40 +45,6 @@ __global__ void sum_rows_kernel(const double* in, double* out, int rows, int n) 
   out[r] = s;
 }
 
-// out[k][t] = mean over f of aff[f][k][t]   (estimate_mixture_weight, axis -3)
-__global__ void mean_over_bins_kernel(const double* __restrict__ aff, int F, int K, int T, double* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= K * T) return;
-  double s = 0.0;
-  for (int f = 0; f < F; ++f) s += aff[(size_t)f * K * T + i];
-  out[i] = s / (double)F;
-}
-// out[k] = mean over t of in[k][t]
-__global__ void mean_over_time_kernel(const double* __restrict__ in, int K, int T, double* __restrict__ out) {
-  const int k = blockIdx.x;
-  __shared__ double red[32];
-  double s = 0.0;
-  for (int t = threadIdx.x; t < T; t += blockDim.x) s += in[(size_t)k * T + t];
-  s = warp_sum(s);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double tot = 0.0;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) tot += red[i];
-    out[k] = tot / (double)T;
-  }
-}
-
-// w[k][t] /= sum_k |w[k][t]|  (a zero norm counts as 1e-10)
-__global__ void unit_norm_over_classes_kernel(double* __restrict__ w, int K, int T) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= T) return;
-  double n = 0.0;
-  for (int k = 0; k < K; ++k) n += fabs(w[(size_t)k * T + t]);
-  if (n == 0.0) n = 1e-10;
-  for (int k = 0; k < K; ++k) w[(size_t)k * T + t] /= n;
-}
-
 // ---- workspace carving -------------------------------------------------------
 // Control block of the persistent fits, cleared by one memset (control_bytes) before the launch: flags (F) and the
 // ticket, then, 8-byte aligned, the PBB_PHASE_TIMING cycle sums (kPhaseWords; the kernels write 0..11) and the
@@ -892,7 +858,7 @@ using namespace pbb;
 extern "C" {
 
 const char* pbb_last_error(void) { return g_err; }
-int pbb_version(void) { return 108; }
+int pbb_version(void) { return 109; }
 
 int pbb_normalize_observation(const void* y, void* z, int F, int T, int D, int dtype, int swap, void* stream) {
   PBB_CHECK_ARG(y != nullptr, 1, "y is null");
@@ -1369,27 +1335,6 @@ int pbb_bingham_log_pdf(const void* y, int dtype, int M, int T, int D, const voi
     return launch_kernel("bingham_log_pdf_kernel", bingham_log_pdf_kernel<CT>, blocks, 128, 0, st,
                          static_cast<const CT*>(y), V, eigenvalues, log_norm, M, T, D, log_pdf);
   });
-}
-
-int pbb_mixture_weight_over_bins(const double* affiliation, int F, int K, int T, int flags, double* weight_kt,
-                                 double* weight_k, void* stream) {
-  const int also_over_time = flags & 1, unit_norm = flags & 2;
-  PBB_CHECK_ARG(affiliation != nullptr, 1, "affiliation is null");
-  PBB_CHECK_ARG(F > 0 && K > 0 && K < kMaxK && T > 0, 2, "bad shape");
-  PBB_CHECK_ARG(weight_kt != nullptr, 6, "weight (K, T) output is null");
-  PBB_CHECK_ARG(!also_over_time || weight_k != nullptr, 7, "weight (K) output is null");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  PBB_TRY(launch_kernel("mean_over_bins_kernel", mean_over_bins_kernel, (K * T + 255) / 256, 256, 0, st, affiliation, F,
-                        K, T, weight_kt));
-  if (also_over_time)
-    PBB_TRY(launch_kernel("mean_over_time_kernel", mean_over_time_kernel, K, 256, 0, st, weight_kt, K, T, weight_k));
-  if (!unit_norm) return 0;
-  // the saliency form of estimate_mixture_weight (mixture_model_utils.py:192-203, used by CWMMTrainer):
-  // sums instead of means, then _unit_norm(ord=1, axis=-2, eps=1e-10, 'where') -- the 1/F (1/T) cancels
-  if (also_over_time)
-    return launch_kernel("unit_norm_over_classes_kernel", unit_norm_over_classes_kernel, 1, 32, 0, st, weight_k, K, 1);
-  return launch_kernel("unit_norm_over_classes_kernel", unit_norm_over_classes_kernel, (T + 127) / 128, 128, 0, st,
-                       weight_kt, K, T);
 }
 
 }  // extern "C"

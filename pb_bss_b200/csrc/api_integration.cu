@@ -7,12 +7,11 @@
 //   pbb_gaussian_fit              weighted mean + variance, two passes           (gaussian.py:155-193)
 //   pbb_log_pdf_to_affiliation    softmax * weight, clip (mixture_model_utils.py:7-55), optionally after the
 //                                 per-bin search over the K! pairings of spatial and spectral classes (:58-130)
-//   pbb_class_weight              L1-normalised sums of the masked affiliations  (gcacgmm.py:283-291)
 // and the batched pieces of the embedding mixture models GMM / VMFMM (gmm.py, vmfmm.py), B independent models:
 //   pbb_gaussian_full_log_pdf     full-covariance Gaussian, the reference's U d form (gaussian.py:36-56)
 //   pbb_gaussian_full_fit         weighted mean + full scatter, N split over CTAs (gaussian.py:152-193)
 //   pbb_precision_cholesky        sklearn's precision Cholesky + log det, one warp per matrix
-//   pbb_vmf_log_pdf / pbb_vmf_resultant / pbb_frame_weight
+//   pbb_vmf_log_pdf / pbb_vmf_resultant
 // All reductions run in a fixed order (bit-reproducible).
 #include <cstring>
 
@@ -22,7 +21,6 @@
 
 namespace pbb {
 
-constexpr int kMaxKInt = kMaxK;
 constexpr int kIntMaxK = 6;    // K! permutations are enumerated per bin
 constexpr int kIntMaxE = 64;   // embedding dimension held in registers / shared memory
 
@@ -226,25 +224,6 @@ __global__ void __launch_bounds__(256) log_pdf_to_affiliation_kernel(
       if (eps != 0.0) v = fmin(fmax(v, eps), 1.0 - eps);
       out[((size_t)f * K + k) * T + t] = v;
     }
-  }
-}
-
-// per-bin class weights: w[f][k] = sum_t m[f][k][t] / sum_k sum_t m[f][k][t]   (gcacgmm.py:286-291, axis (-1,))
-__global__ void class_weight_kernel(const double* __restrict__ m, int F, int K, int T, double* __restrict__ w) {
-  __shared__ double red[8];
-  __shared__ double s[kMaxKInt];
-  const int f = blockIdx.x;
-  for (int k = 0; k < K; ++k) {
-    double v = 0.0;
-    for (int t = threadIdx.x; t < T; t += blockDim.x) v += m[((size_t)f * K + k) * T + t];
-    v = block_sum_256(v, red);
-    if (threadIdx.x == 0) s[k] = v;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double tot = 0.0;
-    for (int k = 0; k < K; ++k) tot += s[k];
-    for (int k = 0; k < K; ++k) w[(size_t)f * K + k] = s[k] / tot;
   }
 }
 
@@ -485,17 +464,6 @@ __global__ void __launch_bounds__(128) vmf_log_pdf_kernel(const double* __restri
     }
 }
 
-// Mixture weight of weight_constant_axis=(-2,) with a saliency (mixture_model_utils.py:191-201): the sum over the
-// classes, L1-normalised over its singleton class axis -> s / |s|, and 0 where s == 0 (eps_style 'where').
-__global__ void frame_weight_kernel(const double* __restrict__ m, int K, int N, double* __restrict__ w) {
-  const int b = blockIdx.y, n = blockIdx.x * blockDim.x + threadIdx.x;
-  if (n >= N) return;
-  double s = 0.0;
-  for (int k = 0; k < K; ++k) s += m[((size_t)b * K + k) * N + n];
-  const double nrm = fabs(s);
-  w[(size_t)b * N + n] = s / (nrm == 0.0 ? 1e-10 : nrm);
-}
-
 struct FullFitChunks { int nchunks, chunk_len; };
 inline FullFitChunks full_fit_chunks(int B, int N, int K) {
   const long long BK = (long long)B * K;
@@ -605,14 +573,6 @@ int pbb_log_pdf_to_affiliation(const double* log_pdf_a, const double* log_pdf_b,
                        affiliation, permutation);
 }
 
-int pbb_class_weight(const double* masked_affiliation, int F, int K, int T, double* weight, void* stream) {
-  PBB_CHECK_ARG(masked_affiliation != nullptr, 1, "input is null");
-  PBB_CHECK_ARG(F > 0 && K > 0 && K < kMaxK && T > 0, 2, "bad shape");
-  PBB_CHECK_ARG(weight != nullptr, 5, "output is null");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return launch_kernel("class_weight_kernel", class_weight_kernel, F, 256, 0, st, masked_affiliation, F, K, T, weight);
-}
-
 int pbb_gaussian_full_log_pdf(const double* embedding, const double* mean, const double* precision_cholesky,
                               const double* log_det, int B, int N, int E, int K, double* log_pdf, void* stream) {
   PBB_CHECK_ARG(embedding && mean && precision_cholesky && log_det, 1, "input is null");
@@ -697,15 +657,6 @@ int pbb_vmf_resultant(const double* embedding, const double* weight, int B, int 
                         0, st, embedding, weight, nullptr, N, E, K, c.chunk_len, 0, 1, partial));
   return launch_kernel("gaussian_full_reduce_kernel", gaussian_full_reduce_kernel, BK, kFitThreads, 0, st, partial,
                        c.nchunks, E, 0, denom, nullptr, resultant, total, nullptr);
-}
-
-int pbb_frame_weight(const double* masked_affiliation, int B, int K, int N, double* weight, void* stream) {
-  PBB_CHECK_ARG(masked_affiliation != nullptr, 1, "input is null");
-  PBB_CHECK_ARG(B > 0 && B <= 65535 && K > 0 && N > 0, 2, "bad shape");
-  PBB_CHECK_ARG(weight != nullptr, 5, "output is null");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  return launch_kernel("frame_weight_kernel", frame_weight_kernel, dim3((N + 255) / 256, B), 256, 0, st,
-                       masked_affiliation, K, N, weight);
 }
 
 }  // extern "C"

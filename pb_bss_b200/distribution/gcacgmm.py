@@ -3,8 +3,9 @@ spatial model [Drude2019Integration] (pb_bss/distribution/gcacgmm.py:38-333).
 
 Same class / argument names and defaults as the reference.  Every array of size F*T lives on the device: the spatial
 quadratic form and the cACG M-step are the cACGMM kernels (``pbb_cacgmm_predict`` / ``pbb_cacgmm_mstep``), the
-spectral log pdf, the Gaussian fit, the posterior (with the optional per-bin pairing of spatial and spectral classes)
-and the class weights are the kernels of ``csrc/api_integration.cu``.  The Gaussians are tied over all bins, so the
+spectral log pdf, the Gaussian fit and the posterior (with the optional per-bin pairing of spatial and spectral
+classes) are the kernels of ``csrc/api_integration.cu``, the class weights the axis sums and unit norms of
+``estimate_mixture_weight`` (``pbb_axis_sum`` / ``pbb_unit_norm``).  The Gaussians are tied over all bins, so the
 EM loop is a per-iteration sequence of launches like the frequency-tied cACGMM (``mixture_model_utils.coupled_fit``)."""
 import ctypes
 from dataclasses import dataclass
@@ -17,8 +18,8 @@ from .. import _device, _lib
 from .cacgmm import CACGMM, _NORMS
 from .complex_angular_central_gaussian import ComplexAngularCentralGaussian
 from .gaussian import gaussian_fit_fkt
-from .mixture_model_utils import (check_initialization, initial_affiliation, masked_affiliation, model_to_host,
-                                  saliency_bn, status_check)
+from .mixture_model_utils import (check_initialization, class_weight, initial_affiliation, masked_affiliation,
+                                  model_to_host, saliency_bn, status_check, tied_weight)
 from .utils import _ProbabilisticModel
 
 
@@ -90,23 +91,16 @@ def integrated_posterior(model, spectral, od, affiliation_eps, inline_permutatio
 
 
 def class_weights(masked, weight_constant_axis):
-    """Mixture weights of an integrated model from the masked affiliations (F, K, T) (gcacgmm.py:283-291)."""
-    F, K, T = masked.shape
-    lib = _lib.load()
+    """Mixture weights of an integrated model from the masked affiliations (F, K, T) (gcacgmm.py:283-291), sums
+    L1-normalised over the classes: per bin (F, K), NaN for a bin without weight as in the reference, or the
+    frequency-tied (K, T) / (K,), 0 for a frame without weight."""
     mode = _weight_layout(weight_constant_axis)
     if mode == _lib.WEIGHT_CONST:
-        return 1 / K
+        return 1 / masked.shape[1]
     if mode == _lib.WEIGHT_TIME:
-        weight = _device.empty((F, K), torch.float64)
-        _lib.check(lib.pbb_class_weight(_device.ptr(masked), F, K, T, _device.ptr(weight), _device.stream_ptr()),
-                   'pbb_class_weight')
-        return weight
-    w_kt = _device.empty((K, T), torch.float64)
-    w_k = _device.empty((K,), torch.float64)
-    _lib.check(lib.pbb_mixture_weight_over_bins(
-        _device.ptr(masked), F, K, T, int(mode == _lib.WEIGHT_TIED) | 2, _device.ptr(w_kt), _device.ptr(w_k),
-        _device.stream_ptr()), 'pbb_mixture_weight_over_bins')
-    return w_kt if mode == _lib.WEIGHT_TIED_TIME else w_k
+        return class_weight(masked)
+    weight = tied_weight(masked, None, mode, saliency_form=True)
+    return weight[0] if mode == _lib.WEIGHT_TIED_TIME else weight[0, :, 0]
 
 
 def cacg_m_step(od, affiliation, quadratic_form, sal, hermitize, covariance_norm, eigenvalue_floor, what):

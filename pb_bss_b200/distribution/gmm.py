@@ -2,8 +2,8 @@
 leading dims: y (..., N, E), affiliations (..., K, N), one model (K, E[, E]) per leading index.
 
 Same class / argument names, defaults and error types as the reference.  The EM loop is a per-iteration sequence of
-launches on the caller's stream without a host synchronisation: class weights (``pbb_class_weight`` /
-``pbb_frame_weight``), the Gaussian fit (``pbb_gaussian_full_fit``, or ``pbb_gaussian_fit`` for the diagonal /
+launches on the caller's stream without a host synchronisation: class weights (``pbb_axis_sum`` /
+``pbb_unit_norm``), the Gaussian fit (``pbb_gaussian_full_fit``, or ``pbb_gaussian_fit`` for the diagonal /
 spherical model, which the reference only accepts without a leading dim > 1), the precision Cholesky factors
 (``pbb_precision_cholesky``, status words read when the loop ends) and the posterior (``pbb_log_pdf_to_affiliation``
 with the leading dims as its bin axis).  All arithmetic is float64.  NumPy in gives NumPy out, a CUDA tensor in gives
@@ -19,11 +19,12 @@ from typing import Any
 import numpy as np
 import torch
 
-from .. import _device, _lib
+from .. import _device, _lib, _nd
 from .gaussian import (_ILL_DEFINED, MAX_K, DiagonalGaussian, Gaussian, SphericalGaussian, _dev, _is_real,
                        check_embedding_dim, full_fit_bkn, full_log_pdf_bkn, precision_cholesky, small_log_pdf_kn)
-from .mixture_model_utils import check_initialization, initial_affiliation, masked_affiliation, saliency_bn
-from .utils import _ProbabilisticModel
+from .mixture_model_utils import (check_initialization, class_weight, initial_affiliation, masked_affiliation,
+                                  saliency_bn)
+from .utils import _ProbabilisticModel, _unit_norm
 
 
 def weight_kind(weight_constant_axis):
@@ -49,19 +50,14 @@ def check_classes(K):
 
 def mixture_weight(masked, kind):
     """masked affiliations (B, K, N) device -> (posterior weight mode, device weight or None)."""
-    B, K, N = masked.shape
-    lib = _lib.load()
     if kind == 'const':
         return _lib.WEIGHT_CONST, None
     if kind == 'class':
-        w = _device.empty((B, K), torch.float64)
-        _lib.check(lib.pbb_class_weight(_device.ptr(masked), B, K, N, _device.ptr(w), _device.stream_ptr()),
-                   'pbb_class_weight')
-        return _lib.WEIGHT_TIME, w
-    w = _device.empty((B, N), torch.float64)
-    _lib.check(lib.pbb_frame_weight(_device.ptr(masked), B, K, N, _device.ptr(w), _device.stream_ptr()),
-               'pbb_frame_weight')
-    return _lib.WEIGHT_FRAME, w
+        return _lib.WEIGHT_TIME, class_weight(masked)
+    # weight_constant_axis (-2,) with a saliency (mixture_model_utils.py:191-201): the sum over the classes,
+    # L1-normalised over its singleton class axis -> s / |s|, and 0 where s == 0
+    total = _nd.axis_sum(masked, (1,), True)
+    return _lib.WEIGHT_FRAME, _unit_norm(total, ord=1, axis=-2, eps=1e-10, eps_style='where')[:, 0]
 
 
 def weight_to_public(mode, w, lead, K, N, like_numpy):

@@ -86,6 +86,25 @@ def masked_affiliation(aff, sal):
     return aff if sal is None else (aff * sal[:, None, :]).contiguous()
 
 
+def class_weight(masked):
+    """Per-row class weights of masked affiliations (B, K, N) (gcacgmm.py:286-291): the sum over N divided by its
+    sum over the classes -> (B, K).  The sums are non-negative, so that divisor is their L1 norm; with eps = 0 a row
+    without weight stays 0 / 0 = NaN, as in the reference."""
+    return _unit_norm(_nd.axis_sum(masked, (2,), False), ord=1, axis=-1, eps=0.)
+
+
+def tied_weight(affiliation, sal, mode, saliency_form):
+    """The frequency-tied weight of (F, K, T) affiliations (estimate_mixture_weight, mixture_model_utils.py:187-203)
+    -> (1, K, T) for WEIGHT_TIED_TIME, (1, K, 1) for WEIGHT_TIED, float64: the mean over the bins (and frames), or,
+    with saliency_form, the sum of affiliation * saliency L1-normalised over the classes.  sal: (F, T) or None."""
+    axes = (0,) if mode == _lib.WEIGHT_TIED_TIME else (0, 2)
+    weight = _nd.axis_sum(affiliation, axes, True, multiplier=None if sal is None else sal[:, None, :],
+                          divide_by_count=not saliency_form, out_dtype=torch.float64)
+    if saliency_form:
+        weight = _unit_norm(weight, ord=1, axis=-2, eps=1e-10, eps_style='where')
+    return weight
+
+
 def weight_to_device(weight, independent, F, K, N):
     """A model's weight -> (device weight, mode) for the predict kernels: (..., K, 1) -> (F, K) WEIGHT_TIME; the
     time-varying weight (..., K, T) of weight_constant_axis=(-3,), shared by every bin -> (K, T) WEIGHT_TIED_TIME."""
@@ -154,12 +173,12 @@ def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, a
     yd: (F, N, D) device observation; affiliation: initial (F, K, N) device affiliations, or ``model`` to start from;
     sal: (F, N) device saliency or None.  ``predict(model)`` -> (affiliation (F, K, N), quadratic form or None);
     ``m_step(affiliation, quadratic_form)`` -> model with per-bin weights, which then get the tied weight.
-    saliency_form: L1-normalise the tied weight over the classes (flag bit 1 of ``pbb_mixture_weight_over_bins``).
+    saliency_form: the tied weight is the sum of affiliation * saliency L1-normalised over the classes (tied_weight).
     total_bins, bin_group: ``yd`` holds this rank's slice of ``total_bins`` bins (pb_bss_b200.parallel).
     Returns the model of device tensors."""
     from .. import parallel
     from ..permutation_alignment import apply_mapping
-    independent, F, N, _ = flatten_obs(yd)
+    independent, F, _, _ = flatten_obs(yd)
     mode = weight_mode(weight_constant_axis, len(independent) + 2)
     if aligner is not None:
         message = ('Inline permutation alignment reduces mismatch between frequency independent '
@@ -172,7 +191,6 @@ def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, a
     assert hi - lo == F, ('this rank holds bins', (lo, hi), 'but y has', F)
     if sal is not None and F_all != F:
         raise NotImplementedError('saliency with frequency-tied weights is single-rank only')
-    lib = _lib.load()
     quadratic_form = None
     with _device.deferred_status():
         for _ in range(iterations):
@@ -192,19 +210,10 @@ def coupled_fit(yd, affiliation, model, iterations, weight_constant_axis, sal, a
             model = m_step(affiliation, quadratic_form)
             if mode not in (_lib.WEIGHT_TIED_TIME, _lib.WEIGHT_TIED):
                 continue  # per-bin weights (the cACGMM fit with a graph): the M-step's own
-            # the tied weight: with a saliency, the sum of affiliation * saliency (mixture_model_utils.py:192-203)
-            K = affiliation.shape[1]
-            masked = masked_affiliation(affiliation, sal).contiguous()
-            w_kt = _device.empty((K, N), torch.float64)
-            w_k = _device.empty((K,), torch.float64)
-            flags = int(mode == _lib.WEIGHT_TIED) | (2 if saliency_form else 0)
-            _lib.check(lib.pbb_mixture_weight_over_bins(
-                _device.ptr(masked), F, K, N, flags, _device.ptr(w_kt), _device.ptr(w_k),
-                _device.stream_ptr()), 'pbb_mixture_weight_over_bins')
+            weight = tied_weight(affiliation, sal, mode, saliency_form)
             if F_all != F:  # sum over the other ranks' bins
-                w_kt = parallel.mean_over_all_bins(w_kt, F, F_all, bin_group)
-                w_k = parallel.mean_over_all_bins(w_k, F, F_all, bin_group)
-            model.weight = w_kt[None] if mode == _lib.WEIGHT_TIED_TIME else w_k[None, :, None]
+                weight = parallel.mean_over_all_bins(weight, F, F_all, bin_group)
+            model.weight = weight
     return model
 
 

@@ -74,18 +74,15 @@ def _souden(ref_channel):
     return make
 
 
-def _mixture_weight(flags):
+def _tied_weight(flags):
+    """The frequency-tied weight of the coupled EM loop: flags bit 0 ties the frames too, bit 1 the saliency form."""
     def make():
-        import torch
-        from pb_bss_b200 import _device, _lib
+        from pb_bss_b200 import _lib
+        from pb_bss_b200.distribution.mixture_model_utils import tied_weight
         F, K, T = 7, 3, 50
         aff = _cuda(_rng(6).random((F, K, T)))
-        w_kt = torch.empty((K, T), dtype=torch.float64, device='cuda')
-        w_k = torch.empty((K,), dtype=torch.float64, device='cuda')
-        lib = _lib.load()
-        return lambda: _lib.check(lib.pbb_mixture_weight_over_bins(
-            _device.ptr(aff), F, K, T, flags, _device.ptr(w_kt), _device.ptr(w_k), _device.stream_ptr()),
-            'pbb_mixture_weight_over_bins')
+        mode = _lib.WEIGHT_TIED if flags & 1 else _lib.WEIGHT_TIED_TIME
+        return lambda: tied_weight(aff, None, mode, bool(flags & 2))
     return make
 
 
@@ -189,11 +186,11 @@ CASES = {
     'vmf_resultant': (_vmf_resultant, ['gaussian_full_partial_kernel', 'gaussian_full_reduce_kernel']),
     'souden_ref_channel': (_souden(1), ['souden_kernel', 'colsum_kernel']),
     'souden_chosen_channel': (_souden(None), ['souden_kernel', 'colsum_kernel']),
-    'mixture_weight': (_mixture_weight(0), ['mean_over_bins_kernel']),
-    'mixture_weight_over_time': (_mixture_weight(1), ['mean_over_bins_kernel', 'mean_over_time_kernel']),
-    'mixture_weight_unit_norm': (_mixture_weight(2), ['mean_over_bins_kernel', 'unit_norm_over_classes_kernel']),
-    'mixture_weight_over_time_unit_norm': (_mixture_weight(3), ['mean_over_time_kernel',
-                                                                'unit_norm_over_classes_kernel']),
+    'tied_weight': (_tied_weight(0), ['reduce_kernel']),
+    'tied_weight_over_time': (_tied_weight(1), ['reduce_kernel<warp>', 'red_finish_kernel']),
+    'tied_weight_unit_norm': (_tied_weight(2), ['reduce_kernel', 'scale_nd_kernel<divide>']),
+    'tied_weight_over_time_unit_norm': (_tied_weight(3), ['reduce_kernel<warp>', 'red_finish_kernel', 'reduce_kernel',
+                                                          'scale_nd_kernel<divide>']),
     'axis_sum_chunks': (_axis_sum_chunks, ['red_finish_kernel']),
     'dhtv_cos': (_dhtv('cos'), ['dhtv_normalize_kernel', 'dhtv_init_mapping_kernel']),
     'dhtv_multiply': (_dhtv('multiply'), ['dhtv_init_mapping_kernel']),
