@@ -1,7 +1,7 @@
 """torch tensors as device-memory containers for the C ABI.
 
 Nothing here computes: tensors are allocated, copied host<->device and handed
-to the library as raw pointers on torch's current CUDA stream.
+to the library as raw pointers on torch's current CUDA stream (``call``).
 """
 import threading
 
@@ -107,6 +107,77 @@ def ptr(t):
 
 def stream_ptr():
     return torch.cuda.current_stream().cuda_stream
+
+
+_DTYPES = {'double': (torch.float64,), 'float': (torch.float32,), 'int': (torch.int32,), 'long long': (torch.int64,),
+           'uint8_t': (torch.uint8, torch.bool), 'unsigned char': (torch.uint8, torch.bool), 'void': None}
+_Tensor = torch.Tensor
+_NUMBERS = frozenset((int, float, bool))  # isinstance(x, torch.Tensor) is slow for a non-tensor x; these skip it
+_entries = {}
+
+
+def _entry(name):
+    """(function, arity, scalar positions, (position, dtypes) of each pointer) of a device entry point; dtypes are
+    the ones a tensor may have there (None: any; an empty tuple for a struct, which takes no tensor)."""
+    lib = _lib.load()
+    decl = _lib.DECLARATIONS.get(name)
+    if decl is None:
+        raise TypeError(f'{name} is not declared in include/pbb.h')
+    if not decl.streamed:
+        raise TypeError(f'{name} does not take a stream; call it through _lib.load() directly')
+    params = decl.params[:-1]
+    scalars = tuple(i for i, p in enumerate(params) if p.pointee is None)
+    pointers = tuple((i, _DTYPES.get(p.pointee, ())) for i, p in enumerate(params) if p.pointee is not None)
+    _entries[name] = entry = (getattr(lib, name), len(params), scalars, pointers)
+    return entry
+
+
+def _placement(name, i, t, dev):
+    """The current device index (looked up once per call, on the first CUDA tensor; None before) if tensor argument
+    i may be passed, else raises: it must be on the current device or in pinned host memory."""
+    d = t.get_device()
+    if d < 0:
+        if not t.is_pinned():
+            raise ValueError(f'{name}: argument {i + 1} is in pageable host memory; the device cannot read it')
+        return dev
+    if dev is None:
+        dev = torch.cuda.current_device()
+    if d != dev:
+        raise ValueError(f'{name}: argument {i + 1} is on cuda:{d}, the current device is cuda:{dev}')
+    return dev
+
+
+def call(name, *args):
+    """Calls the device entry point ``name`` of include/pbb.h on the current stream and raises through _lib.check.
+
+    ``args`` are its parameters without the stream.  A pointer takes None (NULL), a ctypes object, or a tensor
+    whose dtype matches the pointee (float64 for double, float32 for float, int32 for int, int64 for long long,
+    uint8 or bool for uint8_t, any for void) and that is on the current CUDA device or in pinned host memory.  A
+    Python int for a pointer, or a tensor for a scalar, is a TypeError.  Contiguity is the caller's business: some
+    entry points take strides.  Everything is checked before the stream is read or the library is called."""
+    fn, arity, scalars, pointers = _entries.get(name) or _entry(name)
+    if len(args) != arity:
+        raise TypeError(f'{name} takes {arity} arguments besides the stream, got {len(args)}')
+    for i in scalars:
+        a = args[i]
+        if type(a) not in _NUMBERS and isinstance(a, _Tensor):
+            raise TypeError(f'{name}: argument {i + 1} is a scalar, got a tensor')
+    cargs = list(args)
+    dev = None
+    for i, want in pointers:
+        a = args[i]
+        if a is None:
+            continue
+        if isinstance(a, _Tensor):
+            if want is not None and a.dtype not in want:
+                raise TypeError(f'{name}: argument {i + 1} wants {" or ".join(map(str, want)) or "no tensor"}, '
+                                f'got {a.dtype}')
+            if a.get_device() != dev:
+                dev = _placement(name, i, a, dev)
+            cargs[i] = a.data_ptr()
+        elif isinstance(a, int):
+            raise TypeError(f'{name}: argument {i + 1} is a pointer; pass a tensor, None or a ctypes object')
+    _lib.check(fn(*cargs, torch.cuda.current_stream().cuda_stream), name)
 
 
 def empty(shape, dtype):

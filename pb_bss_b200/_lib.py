@@ -5,6 +5,8 @@ absent this module raises -- there is no CPU fallback anywhere in the package.
 """
 import ctypes
 import os
+import re
+from typing import NamedTuple, Optional, Tuple
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # PBB_LIB selects an alternative build of the same ABI (kernel-variant experiments)
@@ -63,195 +65,79 @@ class NdLayout(ctypes.Structure):
     ]
 
 
-_vp, _i, _d, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_size_t
-_ll, _lay = ctypes.c_longlong, ctypes.POINTER(MaskLayout)
-_nd = ctypes.POINTER(NdLayout)
+HEADER = os.path.join(os.path.dirname(_HERE), 'include', 'pbb.h')
 
-# name -> (restype, argtypes); mirrors include/pbb.h one to one
-SIGNATURES = {
-    'pbb_last_error': (ctypes.c_char_p, []),
-    'pbb_version': (_i, []),
-    'pbb_launch_count': (ctypes.c_longlong, []),
-    'pbb_profile_enable': (None, [_i]),
-    'pbb_profile_reset': (None, []),
-    'pbb_profile_dump': (None, []),
-    'pbb_profile_dominant': (_i, [ctypes.c_char_p, _i, ctypes.POINTER(_d), ctypes.POINTER(_i)]),
-    'pbb_normalize_observation': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp]),
-    'pbb_streamed_task_order': (_i, [_i, _i, _i, _i, ctypes.POINTER(_i)]),
-    'pbb_em_dispatch': (_i, [_i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_i), ctypes.POINTER(_i)]),
-    'pbb_em_last_plan': (_i, [ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i)]),
-    'pbb_cacgmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'pbb_cacgmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp,
-                            ctypes.POINTER(CacgmmOptions), _vp, _vp, _vp,
-                            _vp, _sz, _vp, _vp]),
-    'pbb_cacgmm_predict': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i,
-                                _vp, _d, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_cacgmm_mstep': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp,
-                              ctypes.POINTER(CacgmmOptions), _vp, _vp, _vp,
-                              _vp, _sz, _vp, _vp]),
-    'pbb_cacgmm_predict_backward_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'pbb_cacgmm_predict_backward': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _d, _vp, _vp, _vp, _vp, _vp,
-                                         _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    'pbb_cacgmm_mstep_backward_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'pbb_cacgmm_mstep_backward': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, ctypes.POINTER(CacgmmOptions), _vp,
-                                       _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    'pbb_cwmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'pbb_cwmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, _vp, _i, _d,
-                          _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_cwmm_predict': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_cbmm_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'pbb_cbmm_fit': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _d, _d, _d,
-                          _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_cbmm_predict': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i, _d, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_bingham_parameters': (_i, [_vp, _i, _i, _d, _d, _vp, _vp, _vp]),
-    'pbb_bingham_log_norm': (_i, [_vp, _i, _i, _d, _vp, _vp]),
-    'pbb_bingham_log_pdf': (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_heig_batched': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_psd_workspace_bytes': (_sz, [_i, _i, _i, _i]),
-    'pbb_power_spectral_density': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _sz, _vp]),
-    'pbb_gev_batched': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp]),
-    'pbb_solve_batched': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
-    'pbb_mvdr': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_souden': (_i, [_vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_blind_analytic_normalization': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
-    'pbb_dhtv_scratch_doubles': (_sz, [_i, _i, ctypes.POINTER(_i), _i]),
-    'pbb_cacg_log_pdf': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_gaussian_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_gaussian_fit_scratch_doubles': (ctypes.c_size_t, [_i, _i, _i]),
-    'pbb_gaussian_fit': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_log_pdf_to_affiliation': (_i, [_vp, _vp, _d, _d, _vp, _i, _vp, _d, _i, _i, _i, _i, _vp, _vp, _vp]),
-    'pbb_gaussian_full_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_gaussian_full_fit_scratch_doubles': (_sz, [_i, _i, _i, _i]),
-    'pbb_gaussian_full_fit': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_precision_cholesky': (_i, [_vp, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_vmf_log_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_vmf_resultant': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_dhtv_mapping': (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i), _i, _vp, _vp, _vp, _vp]),
-    'pbb_dhtv_mapping_ex': (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i), _i, _vp, _vp, _vp, _i, _i, _vp]),
-    'pbb_apply_mapping': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
-    'pbb_score_matrix': (_i, [_vp, _vp, ctypes.c_longlong, ctypes.c_longlong, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_mapping_from_score_matrix': (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
-    'pbb_chain_mapping': (_i, [_vp, _i, _i, _vp, _vp]),
-    'pbb_rank_one_estimate': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
-    'pbb_matvec_batched': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
-    'pbb_apply_beamforming_vector': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_apply_beamforming_vector_shared': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_apply_beamforming_vector_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_apply_beamforming_vector_shared_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_power_spectral_density_backward': (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_souden_backward': (_i, [_vp, _vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp]),
-    'pbb_eigenvector_backward': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
-    'pbb_mvdr_backward': (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_blind_analytic_normalization_backward': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
-    'pbb_rank_one_estimate_backward': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
-    'pbb_matvec_batched_backward': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
-    'pbb_solve_batched_strict': (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
-    'pbb_lcmv': (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_wmwf': (_i, [_vp, _vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp]),
-    'pbb_weighted_channel_sum': (_i, [_vp, _vp, _i, _i, _vp, _vp]),
-    'pbb_reference_channel_snr': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_mvdr_merl': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_condition_covariance': (_i, [_vp, _i, _i, _d, _vp, _vp]),
-    'pbb_distortionless_normalization': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
-    'pbb_mvdr_snr_postfilter': (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp]),
-    'pbb_zero_degree_normalization': (_i, [_vp, _i, _i, _i, _vp, _vp]),
-    'pbb_phase_correction': (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_apply_online_beamforming_vector': (_i, [_vp, _vp, _i, _i, _i, _i, _i, ctypes.c_longlong, ctypes.c_longlong,
-                                                 ctypes.c_longlong, ctypes.c_longlong, _vp, _vp]),
-    'pbb_source_mask': (_i, [_vp, _i, _i, _i, _i, _ll, _ll, _ll, _lay, _d, _vp, _vp]),
-    'pbb_row_select_scratch_bytes': (_sz, [_ll, _ll]),
-    'pbb_lorenz_mask': (_i, [_vp, _i, _i, _ll, _lay, _lay, _d, _d, _d, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_quantile_mask': (_i, [_vp, _i, _lay, _lay, _ll, _ll, _d, _d, _i, _d, _d, _vp, _vp, _sz, _vp]),
-    'pbb_biased_binary_mask': (_i, [_vp, _i, _ll, _ll, _lay, _i, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_steering_vector': (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp]),
-    'pbb_diffuse_noise_coherence': (_i, [_vp, _i, _vp, _i, _d, _vp, _vp]),
-    'pbb_array_geometry': (_i, [_i, _vp, _i, _vp, _i, _i, _d, _vp, _vp]),
-    'pbb_stft_frames_per_cta': (_i, [_i, _ll, _i, _i]),
-    'pbb_stft': (_i, [_vp, _i, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_griffin_lim_stft': (_i, [_vp, _i, _ll, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_istft_workspace_bytes': (_sz, [_ll, _i, _i]),
-    'pbb_istft': (_i, [_vp, _ll, _i, _i, _i, _i, _i, _ll, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_stft_backward_workspace_bytes': (_sz, [_ll, _i, _i]),
-    'pbb_stft_backward': (_i, [_vp, _ll, _ll, _i, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_istft_backward': (_i, [_vp, _ll, _i, _i, _i, _i, _i, _ll, _vp, _vp, _vp, _vp]),
-    'pbb_gammatone_chunk_length': (_i, [_ll, _i, _ll]),
-    'pbb_gammatone_workspace_bytes': (_sz, [_ll, _i, _ll]),
-    'pbb_gammatone': (_i, [_vp, _i, _ll, _ll, _i, _vp, _vp, _i, _vp, _sz, _vp, _vp]),
-    'pbb_srmr_vad_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_srmr_vad': (_i, [_vp, _i, _ll, _ll, _d, _i, _vp, _sz, _vp, _vp, _vp, _vp]),
-    'pbb_srmr_fft_log2': (_i, [_ll]),
-    'pbb_srmr_hilbert_workspace_bytes': (_sz, [_ll, _ll, _ll]),
-    'pbb_srmr_hilbert': (_i, [_vp, _ll, _ll, _i, _vp, _ll, _vp, _sz, _vp]),
-    'pbb_srmr_means_workspace_bytes': (_sz, [_ll, _ll, _i, _i]),
-    'pbb_srmr_means': (_i, [_vp, _ll, _ll, _i, _vp, _i, _vp, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_srmr_ratio': (_i, [_vp, _ll, _i, _vp, _vp, _vp, _vp]),
-    'pbb_bss_eval_workspace_bytes': (_sz, [_ll, _i, _i, _ll]),
-    'pbb_bss_eval': (_i, [_vp, _ll, _i, _i, _ll, _i, _ll, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_stoi_workspace_bytes': (_sz, [_ll, _ll, _i, _i]),
-    'pbb_stoi': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _vp, _vp, _vp, _vp,
-                      _vp, _vp]),
-    'pbb_estoi': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _vp, _vp, _vp, _vp,
-                       _vp, _vp]),
-    'pbb_stoi_backward_workspace_bytes': (_sz, [_ll, _ll, _i, _i, _i]),
-    'pbb_stoi_backward': (_i, [_vp, _vp, _i, _ll, _ll, _i, _i, _vp, _i, _ll, _vp, _vp, _vp, _ll, _vp, _sz, _i, _vp,
-                               _vp, _vp, _vp]),
-    'pbb_mean_square_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_mean_square': (_i, [_vp, _i, _ll, _ll, _vp, _sz, _vp, _vp]),
-    'pbb_si_sdr_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_si_sdr': (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp, _sz, _vp, _vp]),
-    'pbb_si_sdr_backward_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_si_sdr_backward': (_i, [_vp, _vp, _vp, _vp, _ll, _ll, _vp, _ll, _vp, _vp, _ll, _vp, _vp, _vp, _sz, _vp, _vp,
-                                 _vp]),
-    'pbb_input_sxr': (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_output_sxr_workspace_bytes': (_sz, [_i, _i]),
-    'pbb_output_sxr': (_i, [_vp, _vp, _i, _i, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp]),
-    'pbb_kmeans_workspace_bytes': (_sz, [_ll, _i, _i]),
-    'pbb_kmeans_fit': (_i, [_vp, _ll, _i, _i, _ll, _vp, _vp, _i, _vp, _sz, _vp, _vp, _vp, _vp, _vp, _i, _vp]),
-    'pbb_kmeans_predict': (_i, [_vp, _ll, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_cacg_from_covariance': (_i, [_vp, _i, _i, _i, _d, _vp, _vp, _vp, _vp]),
-    'pbb_cacg_log_pdf_floor': (_i, [_vp, _vp, _i, _i, _i, _i, _d, _vp, _vp, _vp]),
-    'pbb_cw_log_norm': (_i, [_vp, _ll, _i, _i, _vp, _vp]),
-    'pbb_cw_log_pdf': (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_ccsg_workspace_bytes': (_sz, [_i, _i]),
-    'pbb_ccsg_log_pdf': (_i, [_vp, _i, _ll, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_ccsg_sample': (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _ll, _i, _vp, _vp, _sz, _vp, _vp]),
-    'pbb_ccsg_fit': (_i, [_vp, _i, _i, _i, _i, _vp, _d, _vp, _vp, _sz, _vp]),
-    'pbb_affiliation_nd': (_i, [_vp, _i, _vp, _vp, _nd, _i, ctypes.POINTER(_ll), _d, _vp, _vp]),
-    'pbb_reduce_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_axis_sum': (_i, [_vp, _i, _vp, _nd, _nd, _i, _d, _vp, _i, _vp, _sz, _vp]),
-    'pbb_unit_norm': (_i, [_vp, _i, _nd, _ll, _ll, _ll, _d, _d, _i, _vp, _vp, _sz, _vp]),
-    'pbb_force_hermitian': (_i, [_vp, _i, _ll, _i, _vp, _vp]),
-    'pbb_abs_square': (_i, [_vp, _i, _ll, _vp, _vp]),
-    'pbb_labels_to_one_hot': (_i, [_vp, _ll, _ll, _i, _i, _vp, _vp, _vp, _vp]),
-    'pbb_scale_nd': (_i, [_vp, _i, _vp, _nd, _vp, _vp]),
-    'pbb_vmf_pdf': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
-    'pbb_wpe_workspace_bytes': (_sz, [_ll, _i, _ll, _i, _i, _i]),
-    'pbb_wpe': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _i, _ll, _vp, _sz,
-                     _vp, _vp]),
-    'pbb_wpe_forward': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _i, _ll, _vp,
-                             _sz, _vp, _vp, _vp, _vp]),
-    'pbb_wpe_step': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _ll, _ll, _i, _i, _i, _ll, _vp,
-                          _sz, _vp, _vp, _vp]),
-    'pbb_wpe_backward_workspace_bytes': (_sz, [_ll, _i, _ll, _i, _i, _i]),
-    'pbb_wpe_backward': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _ll, _vp, _sz,
-                              _vp]),
-    'pbb_wpe_power_backward_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_wpe_power_backward': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _i, _i, _ll, _i, _vp, _vp, _vp, _sz,
-                                    _vp]),
-    'pbb_wpe_power_workspace_bytes': (_sz, [_ll, _ll]),
-    'pbb_wpe_power': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _ll, _i, _vp, _vp, _sz, _vp]),
-    'pbb_wpe_build_y_tilde': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _i, _i, _vp, _vp]),
-    'pbb_wpe_online_smem_bytes': (_sz, [_i, _i, _i]),
-    'pbb_wpe_online': (_i, [_vp, _i, _ll, _i, _ll, _ll, _ll, _ll, _vp, _ll, _ll, _ll, _vp, _vp, _vp, _vp, _ll, _ll,
-                            _ll, _vp, _vp, _i, _i, _d, _vp]),
-}
+_SCALARS = {'int': ctypes.c_int, 'double': ctypes.c_double, 'size_t': ctypes.c_size_t,
+            'long long': ctypes.c_longlong}
+_STRUCTS = {'pbb_cacgmm_options': CacgmmOptions, 'pbb_mask_layout': MaskLayout, 'pbb_nd_layout': NdLayout}
+# pointees passed as c_void_p; _device.call matches tensors to them by dtype
+_POINTEES = ('double', 'float', 'int', 'long long', 'uint8_t', 'unsigned char', 'char', 'void')
 
+
+class Param(NamedTuple):
+    name: str
+    ctype: object
+    pointee: Optional[str]  # None for a scalar, else the C type pointed to
+
+
+class Declaration(NamedTuple):
+    restype: object
+    params: Tuple[Param, ...]
+    streamed: bool  # the last parameter is `void* stream`: a device entry point
+
+
+def _c_type(spec, where):
+    """'const double *' -> (ctype, pointee); ImportError for a type this binding does not know."""
+    words = spec.replace('*', ' * ').split()
+    stars = words.count('*')
+    base = ' '.join(w for w in words if w not in ('const', '*'))
+    if stars == 0 and base in _SCALARS:
+        return _SCALARS[base], None
+    if stars == 1 and base in _STRUCTS:
+        return ctypes.POINTER(_STRUCTS[base]), base
+    if stars == 1 and base in _POINTEES:
+        return ctypes.c_void_p, base
+    raise ImportError(f'{HEADER}: unknown C type {spec!r} in {where}')
+
+
+def parse_header(path=HEADER):
+    """name -> Declaration for every pbb_* function declared in include/pbb.h."""
+    with open(path) as f:
+        text = f.read()
+    text = re.sub(r'/\*.*?\*/|//[^\n]*', ' ', text, flags=re.S)
+    text = re.sub(r'^\s*#[^\n]*', ' ', text, flags=re.M)
+    decls = {}
+    for ret, name, args in re.findall(r'([A-Za-z_][\w\s*]*?)\s*\b(pbb_\w+)\s*\(([^()]*)\)\s*;', text):
+        where = f'{" ".join(ret.split())} {name}({" ".join(args.split())})'
+        ret = ' '.join(ret.replace('*', ' * ').split())
+        if ret == 'void':
+            restype = None
+        elif ret == 'const char *':
+            restype = ctypes.c_char_p
+        else:
+            restype, pointee = _c_type(ret, where)
+            if pointee is not None:
+                raise ImportError(f'{HEADER}: unknown return type in {where}')
+        params = []
+        if args.strip() != 'void':
+            for arg in args.split(','):
+                m = re.fullmatch(r'\s*(.*?)\b(\w+)\s*', arg, flags=re.S)
+                if m is None or not m.group(1).strip():
+                    raise ImportError(f'{HEADER}: unnamed or malformed parameter {arg.strip()!r} in {where}')
+                params.append(Param(m.group(2), *_c_type(m.group(1), where)))
+        streamed = bool(params) and params[-1].name == 'stream' and params[-1].pointee == 'void'
+        decls[name] = Declaration(restype, tuple(params), streamed)
+    return decls
+
+
+DECLARATIONS = {}
 _lib = None
 
 
 def load():
-    """Loads libpbb.so (once) and attaches the signatures.  Raises ImportError
-    with build instructions if the library or any declared symbol is missing."""
+    """Loads libpbb.so (once) and attaches the signatures parsed from include/pbb.h.  Raises ImportError with
+    build instructions if the library or any declared symbol is missing, and names any declaration whose
+    types it does not know."""
     global _lib
     if _lib is not None:
         return _lib
@@ -260,14 +146,16 @@ def load():
             f'{LIB_PATH} not found: the CUDA library is not built. Run '
             '`python -c "import __graft_entry__ as g; g.build()"` or '
             '`pb_bss_b200/csrc/build.sh`. There is no CPU fallback.')
+    decls = parse_header()
     lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, decl in decls.items():
         try:
             fn = getattr(lib, name)
         except AttributeError as e:
             raise ImportError(f'{LIB_PATH} does not export {name}; rebuild it') from e
-        fn.restype = res
-        fn.argtypes = args
+        fn.restype = decl.restype
+        fn.argtypes = [p.ctype for p in decl.params]
+    DECLARATIONS.update(decls)
     _lib = lib
     return lib
 

@@ -79,11 +79,8 @@ def axis_sum(x, axes, keepdims, multiplier=None, square=False, divide_by_count=F
     outs = int(np.prod(out_shape))
     nbytes = lib.pbb_reduce_workspace_bytes(outs, count)
     ws = _device.workspace(max(nbytes, 1))
-    _lib.check(lib.pbb_axis_sum(_device.ptr(x) if x.numel() else None, CODES[x.dtype], _device.ptr(multiplier),
-                                outer, red, int(square), float(count) if divide_by_count else 1.0,
-                                _device.ptr(out) if out.numel() else None, CODES[out_dtype], _device.ptr(ws), nbytes,
-                                _device.stream_ptr()),
-               'pbb_axis_sum')
+    _device.call('pbb_axis_sum', x if x.numel() else None, CODES[x.dtype], multiplier, outer, red, int(square),
+                 float(count) if divide_by_count else 1.0, out if out.numel() else None, CODES[out_dtype], ws, nbytes)
     if not keepdims:
         out = out.reshape(tuple(shape[a] for a in kept))
     return out

@@ -72,12 +72,8 @@ def _predict_launch(yd, V, lam, w, wmode, act, affiliation_eps, aff, q, ll):
     lib = _lib.load()
     nbytes = lib.pbb_cacgmm_workspace_bytes(F, N, D, K)
     ws = _device.workspace(nbytes)
-    _lib.check(lib.pbb_cacgmm_predict(
-        _device.ptr(yd), _device.complex_dtype_code(yd), F, N, D, K, _device.ptr(V), _device.ptr(lam),
-        _device.ptr(w), wmode, _device.ptr(act),
-        float(affiliation_eps), _device.ptr(aff), _device.ptr(q),
-        _device.ptr(ll), _device.ptr(ws), nbytes, _device.ptr(status),
-        _device.stream_ptr()), 'pbb_cacgmm_predict')
+    _device.call('pbb_cacgmm_predict', yd, _device.complex_dtype_code(yd), F, N, D, K, V, lam, w, wmode, act,
+                 float(affiliation_eps), aff, q, ll, ws, nbytes, status)
     status_check(status, 'CACGMM.predict')
 
 
@@ -92,11 +88,8 @@ def _mstep_launch(yd, aff, q, sal, opts):
     lib = _lib.load()
     nbytes = lib.pbb_cacgmm_workspace_bytes(F, N, D, K)
     ws = _device.workspace(nbytes)
-    _lib.check(lib.pbb_cacgmm_mstep(
-        _device.ptr(yd), _device.complex_dtype_code(yd), F, N, D, K, _device.ptr(aff), _device.ptr(q),
-        _device.ptr(sal), ctypes.byref(opts), _device.ptr(V), _device.ptr(lam),
-        _device.ptr(w), _device.ptr(ws), nbytes, _device.ptr(status),
-        _device.stream_ptr()), 'pbb_cacgmm_mstep')
+    _device.call('pbb_cacgmm_mstep', yd, _device.complex_dtype_code(yd), F, N, D, K, aff, q, sal, ctypes.byref(opts), V,
+                 lam, w, ws, nbytes, status)
     status_check(status, 'cacgmm_m_step')
     return V, lam, w
 
@@ -136,12 +129,9 @@ class _Predict(torch.autograd.Function):
         lib = _lib.load()
         nbytes = lib.pbb_cacgmm_predict_backward_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_cacgmm_predict_backward(
-            _device.ptr(y), _device.complex_dtype_code(y), F, N, D, K, _device.ptr(V), _device.ptr(lam),
-            _device.ptr(w), _device.ptr(act), float(ctx.affiliation_eps), _device.ptr(aff), _device.ptr(q),
-            _device.ptr(_flat(gaff, F, K, N)), _device.ptr(_flat(gq, F, K, N)), _device.ptr(_flat(gll, F)),
-            _device.ptr(gy), _device.ptr(gV), _device.ptr(glam), _device.ptr(gw), _device.ptr(ws), nbytes,
-            _device.stream_ptr()), 'pbb_cacgmm_predict_backward')
+        _device.call('pbb_cacgmm_predict_backward', y, _device.complex_dtype_code(y), F, N, D, K, V, lam, w, act,
+                     float(ctx.affiliation_eps), aff, q, _flat(gaff, F, K, N), _flat(gq, F, K, N), _flat(gll, F), gy,
+                     gV, glam, gw, ws, nbytes)
         return gy.to(y.dtype), gV.to(V.dtype), glam, gw, None, None, None
 
 
@@ -169,12 +159,9 @@ class _MStep(torch.autograd.Function):
         lib = _lib.load()
         nbytes = lib.pbb_cacgmm_mstep_backward_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_cacgmm_mstep_backward(
-            _device.ptr(y), _device.complex_dtype_code(y), F, N, D, K, _device.ptr(aff), _device.ptr(q),
-            _device.ptr(sal), ctypes.byref(ctx.opts), _device.ptr(V), _device.ptr(lam),
-            _device.ptr(_flat(gV, F, K, D, D)), _device.ptr(_flat(glam, F, K, D)), _device.ptr(_flat(gw, F, K)),
-            _device.ptr(gy), _device.ptr(gaff), _device.ptr(gq), _device.ptr(gsal), _device.ptr(ws), nbytes,
-            _device.stream_ptr()), 'pbb_cacgmm_mstep_backward')
+        _device.call('pbb_cacgmm_mstep_backward', y, _device.complex_dtype_code(y), F, N, D, K, aff, q, sal,
+                     ctypes.byref(ctx.opts), V, lam, _flat(gV, F, K, D, D), _flat(glam, F, K, D), _flat(gw, F, K), gy,
+                     gaff, gq, gsal, ws, nbytes)
         return gy.to(y.dtype), gaff, gq, gsal, None
 
 
@@ -417,11 +404,8 @@ class CACGMMTrainer:
         lib = _lib.load()
         nbytes = lib.pbb_cacgmm_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_cacgmm_fit(
-            _device.ptr(yd), code, F, N, D, K, _device.ptr(init_dev),
-            _device.ptr(sal), _device.ptr(act), ctypes.byref(opts),
-            _device.ptr(V), _device.ptr(lam), _device.ptr(w), _device.ptr(ws),
-            nbytes, _device.ptr(status), _device.stream_ptr()), 'pbb_cacgmm_fit')
+        _device.call('pbb_cacgmm_fit', yd, code, F, N, D, K, init_dev, sal, act, ctypes.byref(opts), V, lam, w, ws,
+                     nbytes, status)
         status_check(status, 'CACGMMTrainer.fit')
         return CACGMM(
             weight=weight_to_host(mode, w, independent, K, like_numpy),

@@ -41,10 +41,8 @@ class CBMM(_ProbabilisticModel):
         lib = _lib.load()
         nbytes = lib.pbb_cbmm_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_cbmm_predict(
-            _device.ptr(yd), code, F, N, D, K, _device.ptr(V), _device.ptr(lam), _device.ptr(w), wmode,
-            float(affiliation_eps), _device.ptr(aff), _device.ptr(ws), nbytes, _device.ptr(status),
-            _device.stream_ptr()), 'pbb_cbmm_predict')
+        _device.call('pbb_cbmm_predict', yd, code, F, N, D, K, V, lam, w, wmode, float(affiliation_eps), aff, ws,
+                     nbytes, status)
         _device.check_status(status, _status_error('CBMM.predict', K))
         return _device.to_host(aff.reshape(*independent, K, N), like_numpy)
 

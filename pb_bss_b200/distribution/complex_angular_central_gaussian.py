@@ -56,10 +56,7 @@ def normalize_observation(observation):
     *independent, N, D = y.shape
     F = int(np.prod(independent)) if independent else 1
     z = torch.empty((*independent, D, N), dtype=y.dtype, device=y.device)
-    lib = _lib.load()
-    _lib.check(lib.pbb_normalize_observation(
-        _device.ptr(y), _device.ptr(z), F, N, D, code, 1,
-        _device.stream_ptr()), 'pbb_normalize_observation')
+    _device.call('pbb_normalize_observation', y, z, F, N, D, code, 1)
     return _device.to_host(z, like_numpy)
 
 
@@ -102,9 +99,8 @@ class ComplexAngularCentralGaussian(_ProbabilisticModel):
         lam = _device.empty((n, D), torch.float64)
         if n:
             status = _device.empty((1,), torch.int32)
-            _lib.check(_lib.load().pbb_cacg_from_covariance(
-                _device.ptr(c), n, D, _NORMS[covariance_norm], float(eigenvalue_floor), _device.ptr(V),
-                _device.ptr(lam), _device.ptr(status), _device.stream_ptr()), 'pbb_cacg_from_covariance')
+            _device.call('pbb_cacg_from_covariance', c, n, D, _NORMS[covariance_norm], float(eigenvalue_floor), V, lam,
+                         status)
 
             def on_error(s):
                 if torch.isfinite(torch.view_as_real(c[s - 1])).all():
@@ -190,17 +186,14 @@ class ComplexAngularCentralGaussian(_ProbabilisticModel):
             lib = _lib.load()
             nbytes = lib.pbb_cacgmm_workspace_bytes(F, N, D, K)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_cacgmm_predict(
-                _device.ptr(yf), _device.complex_dtype_code(yf), F, N, D, K, _device.ptr(Vf), _device.ptr(lamf),
-                None, _lib.WEIGHT_CONST, None, 0., None, _device.ptr(q_raw), None, _device.ptr(ws), nbytes,
-                _device.ptr(status), _device.stream_ptr()), 'pbb_cacgmm_predict')
+            _device.call('pbb_cacgmm_predict', yf, _device.complex_dtype_code(yf), F, N, D, K, Vf, lamf, None,
+                         _lib.WEIGHT_CONST, None, 0., None, q_raw, None, ws, nbytes, status)
             status_check(status, 'ComplexAngularCentralGaussian.log_pdf')
             step = max(1, _MAX_GRID_Y // K)
             for f0 in range(0, F, step):
                 f1 = min(F, f0 + step)
-                _lib.check(lib.pbb_cacg_log_pdf_floor(
-                    _device.ptr(q_raw[f0:f1]), _device.ptr(lamf[f0:f1]), f1 - f0, K, N, D, tiny,
-                    _device.ptr(q[f0:f1]), _device.ptr(out[f0:f1]), _device.stream_ptr()), 'pbb_cacg_log_pdf_floor')
+                _device.call('pbb_cacg_log_pdf_floor', q_raw[f0:f1], lamf[f0:f1], f1 - f0, K, N, D, tiny, q[f0:f1],
+                             out[f0:f1])
         shape = (*lead, N)
         return (_device.to_host(out.reshape(shape), like_numpy), _device.to_host(q.reshape(shape), like_numpy))
 
@@ -240,10 +233,8 @@ class ComplexAngularCentralGaussianTrainer:
             lib = _lib.load()
             nbytes = lib.pbb_cacgmm_workspace_bytes(F, N, D, 1)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_cacgmm_fit(
-                _device.ptr(yd), _device.complex_dtype_code(yd), F, N, D, 1, _device.ptr(init), None, None,
-                ctypes.byref(opts), _device.ptr(V), _device.ptr(lam), _device.ptr(w), _device.ptr(ws), nbytes,
-                _device.ptr(status), _device.stream_ptr()), 'pbb_cacgmm_fit')
+            _device.call('pbb_cacgmm_fit', yd, _device.complex_dtype_code(yd), F, N, D, 1, init, None, None,
+                         ctypes.byref(opts), V, lam, w, ws, nbytes, status)
             status_check(status, 'ComplexAngularCentralGaussianTrainer.fit')
         return ComplexAngularCentralGaussian(
             covariance_eigenvectors=_device.to_host(V.reshape(*independent, D, D), like_numpy),

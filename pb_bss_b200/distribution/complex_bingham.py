@@ -92,10 +92,7 @@ class ComplexBingham(_ProbabilisticModel):
         lam = lam.expand(*lead, D).reshape(M, D).contiguous()
         ld = self._log_norm_device(lam, 1e-8)
         out = _device.empty((M, T), torch.float64)
-        lib = _lib.load()
-        _lib.check(lib.pbb_bingham_log_pdf(
-            _device.ptr(yd), _device.complex_dtype_code(yd), M, T, D, _device.ptr(V), _device.ptr(lam),
-            _device.ptr(ld), _device.ptr(out), _device.stream_ptr()), 'pbb_bingham_log_pdf')
+        _device.call('pbb_bingham_log_pdf', yd, _device.complex_dtype_code(yd), M, T, D, V, lam, ld, out)
         return _device.to_host(out.reshape(*lead, T), like_numpy)
 
     @staticmethod
@@ -104,8 +101,7 @@ class ComplexBingham(_ProbabilisticModel):
         _check_dimension(D)
         n = lam.numel() // D
         out = _device.empty((n,), torch.float64)
-        _lib.check(_lib.load().pbb_bingham_log_norm(
-            _device.ptr(lam), n, D, float(eps), _device.ptr(out), _device.stream_ptr()), 'pbb_bingham_log_norm')
+        _device.call('pbb_bingham_log_norm', lam, n, D, float(eps), out)
         return out
 
     def log_norm(self, remove_duplicate_eigenvalues=True):
@@ -146,9 +142,7 @@ class ComplexBinghamTrainer:
         n = s.numel() // D
         lam = _device.empty(tuple(s.shape), torch.float64)
         status = _device.empty((1,), torch.int32)
-        _lib.check(_lib.load().pbb_bingham_parameters(
-            _device.ptr(s), n, D, float(eps), float(max_concentration), _device.ptr(lam), _device.ptr(status),
-            _device.stream_ptr()), 'pbb_bingham_parameters')
+        _device.call('pbb_bingham_parameters', s, n, D, float(eps), float(max_concentration), lam, status)
         _device.check_status(status, _status_error('find_eigenvalues_v3'))
         return _device.to_host(lam, like_numpy)
 
@@ -207,9 +201,7 @@ def _cbmm_fit_device(yd, init, sal, K, iterations, weight_mode, affiliation_eps,
     lib = _lib.load()
     nbytes = lib.pbb_cbmm_workspace_bytes(F, N, D, K)
     ws = _device.workspace(nbytes)
-    _lib.check(lib.pbb_cbmm_fit(
-        _device.ptr(yd), code, F, N, D, K, _device.ptr(init), _device.ptr(sal), int(iterations), weight_mode,
-        float(affiliation_eps), float(eigenvalue_eps), float(max_concentration), _device.ptr(V), _device.ptr(lam),
-        _device.ptr(w), _device.ptr(ws), nbytes, _device.ptr(status), _device.stream_ptr()), 'pbb_cbmm_fit')
+    _device.call('pbb_cbmm_fit', yd, code, F, N, D, K, init, sal, int(iterations), weight_mode, float(affiliation_eps),
+                 float(eigenvalue_eps), float(max_concentration), V, lam, w, ws, nbytes, status)
     _device.check_status(status, _status_error(what, K))
     return V, lam, w

@@ -79,10 +79,8 @@ def sample_classes(a, eigenvalues, draws, unit_norm, like_numpy, dest=None):
     lib = _lib.load()
     nbytes = lib.pbb_ccsg_workspace_bytes(C, D)
     ws = _device.workspace(nbytes)
-    _lib.check(lib.pbb_ccsg_sample(
-        _device.ptr(a.contiguous()), _device.ptr(lam), C, D, _device.ptr(normals), _device.ptr(off),
-        _device.ptr(dst), S, int(bool(unit_norm)), _device.ptr(out), _device.ptr(ws), nbytes, _device.ptr(status),
-        _device.stream_ptr()), 'pbb_ccsg_sample')
+    _device.call('pbb_ccsg_sample', a.contiguous(), lam, C, D, normals, off, dst, S, int(bool(unit_norm)), out, ws,
+                 nbytes, status)
     _device.check_status(status, _linalg_error('Matrix is not positive definite'))
     return _device.to_host(out, like_numpy)
 
@@ -126,10 +124,8 @@ class ComplexCircularSymmetricGaussian(_ProbabilisticModel):
             lib = _lib.load()
             nbytes = lib.pbb_ccsg_workspace_bytes(M, D)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_ccsg_log_pdf(
-                _device.ptr(frames), _device.complex_dtype_code(frames), stride, M, N, D, _device.ptr(S),
-                _device.ptr(out), _device.ptr(ws), nbytes, _device.ptr(status), _device.stream_ptr()),
-                'pbb_ccsg_log_pdf')
+            _device.call('pbb_ccsg_log_pdf', frames, _device.complex_dtype_code(frames), stride, M, N, D, S, out, ws,
+                         nbytes, status)
             _device.check_status(status, _linalg_error('Singular matrix'))
         return _device.to_host(out.reshape(*lead, N), like_numpy)
 
@@ -178,8 +174,7 @@ class ComplexCircularSymmetricGaussianTrainer:
             lib = _lib.load()
             nbytes = lib.pbb_psd_workspace_bytes(F, N, D, 1)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_ccsg_fit(
-                _device.ptr(obs), _device.complex_dtype_code(obs), F, D, N, _device.ptr(sal),
-                float(np.finfo(np.float32 if yd.dtype == torch.complex64 else np.float64).tiny), _device.ptr(cov),
-                _device.ptr(ws), nbytes, _device.stream_ptr()), 'pbb_ccsg_fit')
+            _device.call('pbb_ccsg_fit', obs, _device.complex_dtype_code(obs), F, D, N, sal,
+                         float(np.finfo(np.float32 if yd.dtype == torch.complex64 else np.float64).tiny), cov, ws,
+                         nbytes)
         return ComplexCircularSymmetricGaussian(covariance=_device.to_host(cov.reshape(*lead, D, D), like_numpy))

@@ -40,9 +40,7 @@ def normalize_observation(observation):
     *independent, N, D = y.shape
     z = torch.empty(tuple(y.shape), dtype=y.dtype, device=y.device)
     if z.numel():
-        lib = _lib.load()
-        _lib.check(lib.pbb_normalize_observation(_device.ptr(y), _device.ptr(z), math.prod(independent), N, D, code,
-                                                 0, _device.stream_ptr()), 'pbb_normalize_observation')
+        _device.call('pbb_normalize_observation', y, z, math.prod(independent), N, D, code, 0)
     return _device.to_host(z, like_numpy)
 
 
@@ -75,9 +73,8 @@ class ComplexWatson(_ProbabilisticModel):
             frames, stride = _frames(yd, lead)
             mode = mode.expand(*lead, D).reshape(M, D).contiguous()
             kappa = kappa.expand(lead).reshape(M).contiguous()
-            _lib.check(_lib.load().pbb_cw_log_pdf(
-                _device.ptr(frames), _device.complex_dtype_code(frames), stride, M, N, D, _device.ptr(mode),
-                _device.ptr(kappa), _device.ptr(out), _device.stream_ptr()), 'pbb_cw_log_pdf')
+            _device.call('pbb_cw_log_pdf', frames, _device.complex_dtype_code(frames), stride, M, N, D, mode, kappa,
+                         out)
         return _device.to_host(out.reshape(*lead, N), like_numpy)
 
     @staticmethod
@@ -116,8 +113,7 @@ def _log_norm(scale, dimension, variant):
     k = _as_device(scale if not like_numpy else np.asarray(scale, dtype=float), torch.float64).contiguous()
     out = _device.empty(tuple(k.shape), torch.float64)
     if k.numel():
-        _lib.check(_lib.load().pbb_cw_log_norm(_device.ptr(k), k.numel(), int(dimension), variant,
-                                               _device.ptr(out), _device.stream_ptr()), 'pbb_cw_log_norm')
+        _device.call('pbb_cw_log_norm', k, k.numel(), int(dimension), variant, out)
     out = _device.to_host(out, like_numpy)
     if like_numpy and variant == _lib.CW_NORM_1F1 and out.ndim == 0:
         return out[()]
@@ -209,11 +205,9 @@ class ComplexWatsonTrainer:
             lib = _lib.load()
             nbytes = lib.pbb_cwmm_workspace_bytes(F, N, D, 1)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_cwmm_fit(
-                _device.ptr(yf), _device.complex_dtype_code(yf), F, N, D, 1, _device.ptr(init), None, 1,
-                _lib.WEIGHT_TIME, _device.ptr(t_dev), _device.ptr(c_dev), int(c_dev.numel()),
-                float(self.max_concentration), _device.ptr(mode), _device.ptr(kappa), _device.ptr(w),
-                _device.ptr(ws), nbytes, _device.ptr(status), _device.stream_ptr()), 'pbb_cwmm_fit')
+            _device.call('pbb_cwmm_fit', yf, _device.complex_dtype_code(yf), F, N, D, 1, init, None, 1,
+                         _lib.WEIGHT_TIME, t_dev, c_dev, int(c_dev.numel()), float(self.max_concentration), mode, kappa,
+                         w, ws, nbytes, status)
             status_check(status, 'ComplexWatsonTrainer.fit')
         return ComplexWatson(mode=_device.to_host(mode.reshape(*lead, D), like_numpy),
                              concentration=_device.to_host(kappa.reshape(lead), like_numpy))

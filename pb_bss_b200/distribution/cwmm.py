@@ -40,11 +40,7 @@ class CWMM(_ProbabilisticModel):
         lib = _lib.load()
         nbytes = lib.pbb_cwmm_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_cwmm_predict(
-            _device.ptr(yd), code, F, N, D, K, _device.ptr(mode),
-            _device.ptr(kappa), _device.ptr(w), wmode, _device.ptr(aff),
-            _device.ptr(ws), nbytes, _device.ptr(status),
-            _device.stream_ptr()), 'pbb_cwmm_predict')
+        _device.call('pbb_cwmm_predict', yd, code, F, N, D, K, mode, kappa, w, wmode, aff, ws, nbytes, status)
         status_check(status, 'CWMM.predict')
         return _device.to_host(aff.reshape(*independent, K, N), like_numpy)
 
@@ -119,13 +115,8 @@ class CWMMTrainer:
         lib = _lib.load()
         nbytes = lib.pbb_cwmm_workspace_bytes(F, N, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_cwmm_fit(
-            _device.ptr(yd), code, F, N, D, K, _device.ptr(init),
-            _device.ptr(sal), int(iterations), weight_mode, _device.ptr(t_dev),
-            _device.ptr(c_dev), int(c_dev.numel()),
-            float(self.max_concentration), _device.ptr(mode),
-            _device.ptr(kappa), _device.ptr(w), _device.ptr(ws), nbytes,
-            _device.ptr(status), _device.stream_ptr()), 'pbb_cwmm_fit')
+        _device.call('pbb_cwmm_fit', yd, code, F, N, D, K, init, sal, int(iterations), weight_mode, t_dev, c_dev,
+                     int(c_dev.numel()), float(self.max_concentration), mode, kappa, w, ws, nbytes, status)
         status_check(status, 'CWMMTrainer.fit')
         return CWMM(
             weight=weight_to_host(weight_mode, w, independent, K, like_numpy),

@@ -64,9 +64,7 @@ def precision_cholesky(cov):
     pc = _device.empty(cov.shape, torch.float64)
     ld = _device.empty(cov.shape[:-2], torch.float64)
     status = _device.empty((1,), torch.int32)
-    lib = _lib.load()
-    _lib.check(lib.pbb_precision_cholesky(_device.ptr(cov), M, E, _device.ptr(pc), _device.ptr(ld),
-                                          _device.ptr(status), _device.stream_ptr()), 'pbb_precision_cholesky')
+    _device.call('pbb_precision_cholesky', cov, M, E, pc, ld, status)
 
     def on_error(s):
         raise ValueError(_ILL_DEFINED)
@@ -79,10 +77,7 @@ def full_log_pdf_bkn(x, mean, pc, ld):
     B, N, E = x.shape
     K = mean.shape[1]
     out = _device.empty((B, K, N), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_gaussian_full_log_pdf(_device.ptr(x), _device.ptr(mean), _device.ptr(pc), _device.ptr(ld),
-                                             B, N, E, K, _device.ptr(out), _device.stream_ptr()),
-               'pbb_gaussian_full_log_pdf')
+    _device.call('pbb_gaussian_full_log_pdf', x, mean, pc, ld, B, N, E, K, out)
     return out
 
 
@@ -96,9 +91,7 @@ def full_fit_bkn(x, weight):
     mean = _device.empty((B, K, E), torch.float64)
     cov = _device.empty((B, K, E, E), torch.float64)
     scratch = _device.empty((int(lib.pbb_gaussian_full_fit_scratch_doubles(B, N, E, K)),), torch.float64)
-    _lib.check(lib.pbb_gaussian_full_fit(_device.ptr(x), _device.ptr(weight), B, N, E, K, _device.ptr(mean),
-                                         _device.ptr(cov), _device.ptr(scratch), _device.stream_ptr()),
-               'pbb_gaussian_full_fit')
+    _device.call('pbb_gaussian_full_fit', x, weight, B, N, E, K, mean, cov, scratch)
     return mean, cov
 
 
@@ -202,11 +195,9 @@ def _gaussian_log_pdf(model, embedding):
     mean, pc, ld = model._device_params(E)
     K = mean.shape[0]
     out = _device.empty((F, K, T), torch.float64)
-    lib = _lib.load()
     # DiagonalGaussian: the reference's einsum quirk (gaussian.py:79-87) is reproduced by the kernel, see include/pbb.h
-    _lib.check(lib.pbb_gaussian_log_pdf(_device.ptr(embedding), _device.ptr(mean), _device.ptr(pc), _device.ptr(ld),
-                                        F, T, E, K, int(isinstance(model, DiagonalGaussian)), _device.ptr(out),
-                                        _device.stream_ptr()), 'pbb_gaussian_log_pdf')
+    _device.call('pbb_gaussian_log_pdf', embedding, mean, pc, ld, F, T, E, K, int(isinstance(model, DiagonalGaussian)),
+                 out)
     return out
 
 
@@ -220,10 +211,7 @@ def small_log_pdf_kn(model, x):
     pc = pc.reshape(K, E) if diagonal else pc.reshape(K, 1).expand(K, E).contiguous()
     ld = _dev(model.log_det_precision_cholesky).reshape(K).contiguous()
     out = _device.empty((1, K, N), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_gaussian_log_pdf(_device.ptr(x), _device.ptr(mean), _device.ptr(pc), _device.ptr(ld),
-                                        1, N, E, K, int(diagonal), _device.ptr(out), _device.stream_ptr()),
-               'pbb_gaussian_log_pdf')
+    _device.call('pbb_gaussian_log_pdf', x, mean, pc, ld, 1, N, E, K, int(diagonal), out)
     return out[0]
 
 
@@ -274,9 +262,7 @@ class GaussianTrainer:
         cov = _device.empty((B,) if spherical else (B, E), torch.float64)
         scratch = _device.empty((int(lib.pbb_gaussian_fit_scratch_doubles(1, E, 1)),), torch.float64)
         for b in range(B):   # one tied model per leading index: the kernels of the integrated model with F = K = 1
-            _lib.check(lib.pbb_gaussian_fit(_device.ptr(x[b]), _device.ptr(w[b]), 1, N, E, 1, int(spherical),
-                                            _device.ptr(mean[b]), _device.ptr(cov[b]), _device.ptr(scratch),
-                                            _device.stream_ptr()), 'pbb_gaussian_fit')
+            _device.call('pbb_gaussian_fit', x[b], w[b], 1, N, E, 1, int(spherical), mean[b], cov[b], scratch)
         cls = SphericalGaussian if spherical else DiagonalGaussian
         return cls(mean=mean.reshape(lead + (E,)).cpu().numpy(),
                    covariance=cov.reshape(lead + (() if spherical else (E,))).cpu().numpy())
@@ -295,8 +281,6 @@ def gaussian_fit_fkt(embedding, weight_fkt, covariance_type):
     cov = _device.empty((K,) if spherical else (K, E), torch.float64)
     lib = _lib.load()
     scratch = _device.empty((int(lib.pbb_gaussian_fit_scratch_doubles(F, E, K)),), torch.float64)
-    _lib.check(lib.pbb_gaussian_fit(_device.ptr(embedding), _device.ptr(weight_fkt), F, T, E, K, int(spherical),
-                                    _device.ptr(mean), _device.ptr(cov), _device.ptr(scratch),
-                                    _device.stream_ptr()), 'pbb_gaussian_fit')
+    _device.call('pbb_gaussian_fit', embedding, weight_fkt, F, T, E, K, int(spherical), mean, cov, scratch)
     cls = SphericalGaussian if spherical else DiagonalGaussian
     return cls(mean=mean.cpu().numpy(), covariance=cov.cpu().numpy())

@@ -60,9 +60,7 @@ def spatial_log_pdf(cacg, od):
     lam = _device.to_device(cacg.covariance_eigenvalues, torch.float64).contiguous()
     K = lam.shape[-2]
     lp = _device.empty((F, K, T), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_cacg_log_pdf(_device.ptr(q.contiguous()), _device.ptr(lam), F, K, T, D, _device.ptr(lp),
-                                    _device.stream_ptr()), 'pbb_cacg_log_pdf')
+    _device.call('pbb_cacg_log_pdf', q.contiguous(), lam, F, K, T, D, lp)
     return q, lp
 
 
@@ -82,11 +80,9 @@ def integrated_posterior(model, spectral, od, affiliation_eps, inline_permutatio
             raise IndexError((), [], model.weight_constant_axis)
     w = None if mode == _lib.WEIGHT_CONST else _device.to_device(model.weight, torch.float64).contiguous()
     aff = _device.empty((F, K, T), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_log_pdf_to_affiliation(
-        _device.ptr(spatial), _device.ptr(spectral), float(model.spatial_weight), float(model.spectral_weight),
-        _device.ptr(w), mode, None, float(affiliation_eps), int(bool(inline_permutation_alignment)), F, K, T,
-        _device.ptr(aff), None, _device.stream_ptr()), 'pbb_log_pdf_to_affiliation')
+    _device.call('pbb_log_pdf_to_affiliation', spatial, spectral, float(model.spatial_weight),
+                 float(model.spectral_weight), w, mode, None, float(affiliation_eps),
+                 int(bool(inline_permutation_alignment)), F, K, T, aff, None)
     return aff, quadratic_form
 
 
@@ -118,11 +114,8 @@ def cacg_m_step(od, affiliation, quadratic_form, sal, hermitize, covariance_norm
         frames_per_block=0, reserved=0)
     nbytes = lib.pbb_cacgmm_workspace_bytes(F, T, D, K)
     ws = _device.workspace(nbytes)
-    _lib.check(lib.pbb_cacgmm_mstep(
-        _device.ptr(od), _device.complex_dtype_code(od), F, T, D, K, _device.ptr(affiliation.contiguous()),
-        _device.ptr(quadratic_form), _device.ptr(sal), ctypes.byref(opts), _device.ptr(V), _device.ptr(lam),
-        _device.ptr(w_unused), _device.ptr(ws), nbytes, _device.ptr(status), _device.stream_ptr()),
-        'pbb_cacgmm_mstep')
+    _device.call('pbb_cacgmm_mstep', od, _device.complex_dtype_code(od), F, T, D, K, affiliation.contiguous(),
+                 quadratic_form, sal, ctypes.byref(opts), V, lam, w_unused, ws, nbytes, status)
     status_check(status, what)
     return ComplexAngularCentralGaussian(covariance_eigenvectors=V, covariance_eigenvalues=lam)
 

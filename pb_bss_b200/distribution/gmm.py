@@ -84,10 +84,7 @@ def posterior(log_pdf, mode, w):
     """log_pdf_to_affiliation (mixture_model_utils.py:7-55), affiliation_eps = 0: (B, K, N) -> (B, K, N)."""
     B, K, N = log_pdf.shape
     aff = _device.empty((B, K, N), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_log_pdf_to_affiliation(
-        _device.ptr(log_pdf), None, 1.0, 0.0, _device.ptr(w), mode, None, 0.0, 0, B, K, N, _device.ptr(aff), None,
-        _device.stream_ptr()), 'pbb_log_pdf_to_affiliation')
+    _device.call('pbb_log_pdf_to_affiliation', log_pdf, None, 1.0, 0.0, w, mode, None, 0.0, 0, B, K, N, aff, None)
     return aff
 
 
@@ -202,9 +199,7 @@ class GMMTrainer:
         mean = _device.empty((K, E), torch.float64)
         cov = _device.empty((K,) if spherical else (K, E), torch.float64)
         scratch = _device.empty((int(lib.pbb_gaussian_fit_scratch_doubles(1, E, K)),), torch.float64)
-        _lib.check(lib.pbb_gaussian_fit(_device.ptr(x), _device.ptr(masked), 1, N, E, K, int(spherical),
-                                        _device.ptr(mean), _device.ptr(cov), _device.ptr(scratch),
-                                        _device.stream_ptr()), 'pbb_gaussian_fit')
+        _device.call('pbb_gaussian_fit', x, masked, 1, N, E, K, int(spherical), mean, cov, scratch)
         if fixed is not None:
             cov = fixed.reshape(cov.shape)
         # sklearn's _compute_precision_cholesky(cov, 'diag') on the K x E parameters (gaussian.py:66-71, 103-108)
@@ -224,11 +219,8 @@ class GMMTrainer:
         K, E = state['mean'].shape
         pc = state['pc'] if state['type'] == 'diagonal' else state['pc'][:, None].expand(K, E).contiguous()
         out = _device.empty((1, K, x.shape[1]), torch.float64)
-        lib = _lib.load()
-        _lib.check(lib.pbb_gaussian_log_pdf(_device.ptr(x), _device.ptr(state['mean']), _device.ptr(pc),
-                                            _device.ptr(state['ld']), 1, x.shape[1], E, K,
-                                            int(state['type'] == 'diagonal'), _device.ptr(out),
-                                            _device.stream_ptr()), 'pbb_gaussian_log_pdf')
+        _device.call('pbb_gaussian_log_pdf', x, state['mean'], pc, state['ld'], 1, x.shape[1], E, K,
+                     int(state['type'] == 'diagonal'), out)
         return out
 
     @staticmethod
@@ -300,10 +292,8 @@ def _kmeans_fit(x, K, init=None, max_ctas=0):
     inertia = _device.empty((), torch.float64)
     n_iter = _device.empty((), torch.int32)
     status = _device.empty((1,), torch.int32)
-    _lib.check(lib.pbb_kmeans_fit(_device.ptr(xd), N, E, K, first, _device.ptr(uniforms), _device.ptr(dev_init),
-                                  _KMEANS_MAX_ITER, _device.ptr(ws), ws.numel(), _device.ptr(centres),
-                                  _device.ptr(labels), _device.ptr(inertia), _device.ptr(n_iter), _device.ptr(status),
-                                  max_ctas, _device.stream_ptr()), 'pbb_kmeans_fit')
+    _device.call('pbb_kmeans_fit', xd, N, E, K, first, uniforms, dev_init, _KMEANS_MAX_ITER, ws, ws.numel(), centres,
+                 labels, inertia, n_iter, status, max_ctas)
 
     def on_status(s):
         if s & 1:
@@ -334,12 +324,9 @@ class KMeans:
             raise ValueError(f'X has {E} features, but KMeans is expecting {self.cluster_centers_.shape[1]} features '
                              'as input.')
         xd = _dev(x)
-        lib = _lib.load()
         labels = None if one_hot else _device.empty((N,), torch.int32)
         oh = _device.empty((K, N), torch.float64) if one_hot else None
-        _lib.check(lib.pbb_kmeans_predict(_device.ptr(xd), N, E, K, _device.ptr(_dev(self.cluster_centers_)),
-                                          _device.ptr(labels), _device.ptr(oh), _device.stream_ptr()),
-                   'pbb_kmeans_predict')
+        _device.call('pbb_kmeans_predict', xd, N, E, K, _dev(self.cluster_centers_), labels, oh)
         return oh if one_hot else labels
 
     def predict(self, x):

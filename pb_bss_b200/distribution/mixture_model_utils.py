@@ -262,11 +262,8 @@ def log_pdf_to_affiliation(weight, log_pdf, source_activity_mask=None, affiliati
     lay = _nd.layout([shape[a] for a in cols], *[[s[a] for a in cols] for s in (ls, ws, ms, os_)])
     cs = (ctypes.c_longlong * 4)(ls[-2], ws[-2], ms[-2], os_[-2])
     if out.numel():
-        lib = _lib.load()
-        _lib.check(lib.pbb_affiliation_nd(_device.ptr(lp), _nd.CODES[lp.dtype], _device.ptr(w),
-                                          _device.ptr(m.view(torch.uint8)) if m is not None else None, lay, shape[-2],
-                                          cs, float(affiliation_eps), _device.ptr(out), _device.stream_ptr()),
-                   'pbb_affiliation_nd')
+        _device.call('pbb_affiliation_nd', lp, _nd.CODES[lp.dtype], w, m.view(torch.uint8) if m is not None else None,
+                     lay, shape[-2], cs, float(affiliation_eps), out)
     return _device.to_host(out, like)
 
 
@@ -296,10 +293,8 @@ def log_pdf_to_affiliation_for_integration_models_with_inline_pa(weight, spatial
     if source_activity_mask is not None:
         act = _device.to_device(source_activity_mask, torch.bool).expand(F, K, T).contiguous().view(torch.uint8)
     out = _device.empty((F, K, T), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_log_pdf_to_affiliation(
-        _device.ptr(a), _device.ptr(b), 1.0, 1.0, _device.ptr(w3), mode, _device.ptr(act), float(affiliation_eps), 1,
-        F, K, T, _device.ptr(out), None, _device.stream_ptr()), 'pbb_log_pdf_to_affiliation')
+    _device.call('pbb_log_pdf_to_affiliation', a, b, 1.0, 1.0, w3, mode, act, float(affiliation_eps), 1, F, K, T, out,
+                 None)
     return _device.to_host(out, like)
 
 

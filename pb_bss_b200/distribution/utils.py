@@ -79,10 +79,8 @@ def _unit_norm(signal, *, axis=-1, eps=1e-4, eps_style='plus', ord=None):
     lib = _lib.load()
     nbytes = lib.pbb_reduce_workspace_bytes(math.prod(x.shape[a] for a in rows), x.shape[ax])
     ws = _device.workspace(max(nbytes, 1))
-    _lib.check(lib.pbb_unit_norm(_device.ptr(x) if x.numel() else None, _nd.CODES[x.dtype], lay, x.shape[ax],
-                                 xs[ax], os_[ax], p, float(eps), _EPS_STYLES[eps_style],
-                                 _device.ptr(out) if out.numel() else None, _device.ptr(ws), nbytes,
-                                 _device.stream_ptr()), 'pbb_unit_norm')
+    _device.call('pbb_unit_norm', x if x.numel() else None, _nd.CODES[x.dtype], lay, x.shape[ax], xs[ax], os_[ax], p,
+                 float(eps), _EPS_STYLES[eps_style], out if out.numel() else None, ws, nbytes)
     return _device.to_host(out, like)
 
 
@@ -122,8 +120,6 @@ def force_hermitian(matrix):
     a = a.contiguous()
     out = _device.empty(tuple(a.shape), a.dtype)
     batch = math.prod(a.shape[:-2])
-    lib = _lib.load()
-    _lib.check(lib.pbb_force_hermitian(_device.ptr(a) if a.numel() else None, _nd.CODES[a.dtype], batch, D,
-                                       _device.ptr(out) if out.numel() else None, _device.stream_ptr()),
-               'pbb_force_hermitian')
+    _device.call('pbb_force_hermitian', a if a.numel() else None, _nd.CODES[a.dtype], batch, D,
+                 out if out.numel() else None)
     return _device.to_host(out, like)

@@ -68,10 +68,7 @@ class VonMisesFisher(_ProbabilisticModel):
                                 torch.float64)
         ln = _device.to_device(np.ascontiguousarray(self.log_norm()), torch.float64)
         out = _device.empty((F, K, T), torch.float64)
-        lib = _lib.load()
-        _lib.check(lib.pbb_gaussian_log_pdf(_device.ptr(embedding), _device.ptr(mean), _device.ptr(kap),
-                                            _device.ptr(ln), F, T, E, K, 2, _device.ptr(out), _device.stream_ptr()),
-                   'pbb_gaussian_log_pdf')
+        _device.call('pbb_gaussian_log_pdf', embedding, mean, kap, ln, F, T, E, K, 2, out)
         return out
 
 
@@ -84,8 +81,7 @@ def vmf_fit_fkt(embedding, weight_fkt, min_concentration, max_concentration):
     cov = _device.empty((K,), torch.float64)
     lib = _lib.load()
     scratch = _device.empty((int(lib.pbb_gaussian_fit_scratch_doubles(F, E, K)),), torch.float64)
-    _lib.check(lib.pbb_gaussian_fit(_device.ptr(embedding), _device.ptr(weight_fkt), F, T, E, K, 1, _device.ptr(mean),
-                                    _device.ptr(cov), _device.ptr(scratch), _device.stream_ptr()), 'pbb_gaussian_fit')
+    _device.call('pbb_gaussian_fit', embedding, weight_fkt, F, T, E, K, 1, mean, cov, scratch)
     total = scratch[F * K * (E + 1):F * K * (E + 1) + K].cpu().numpy()        # sum of the weights per class
     r = mean.cpu().numpy() * total[:, None]                                   # Banerjee2005vMF eq. 2.4
     norm = np.linalg.norm(r, axis=-1)
@@ -101,10 +97,8 @@ def vmf_log_pdf_bkn(x, mean, concentration, log_norm, exp=False):
     B, N, E = x.shape
     K = mean.shape[1]
     out = _device.empty((B, K, N), torch.float64)
-    lib = _lib.load()
     name = 'pbb_vmf_pdf' if exp else 'pbb_vmf_log_pdf'
-    _lib.check(getattr(lib, name)(_device.ptr(x), _device.ptr(mean), _device.ptr(concentration),
-                                  _device.ptr(log_norm), B, N, E, K, _device.ptr(out), _device.stream_ptr()), name)
+    _device.call(name, x, mean, concentration, log_norm, B, N, E, K, out)
     return out
 
 
@@ -118,9 +112,7 @@ def vmf_fit_bkn(x, weight, min_concentration, max_concentration):
     r = _device.empty((B, K, E), torch.float64)
     total = _device.empty((B, K), torch.float64)
     scratch = _device.empty((int(lib.pbb_gaussian_full_fit_scratch_doubles(B, N, E, K)),), torch.float64)
-    _lib.check(lib.pbb_vmf_resultant(_device.ptr(x), _device.ptr(weight), B, N, E, K, _device.ptr(r),
-                                     _device.ptr(total), _device.ptr(scratch), _device.stream_ptr()),
-               'pbb_vmf_resultant')
+    _device.call('pbb_vmf_resultant', x, weight, B, N, E, K, r, total, scratch)
     r, total = r.cpu().numpy(), total.cpu().numpy()
     norm = np.linalg.norm(r, axis=-1)                                                 # Banerjee2005vMF eq. 2.4
     mean = r / np.maximum(norm, np.finfo(np.float64).tiny)[..., None]

@@ -90,10 +90,8 @@ def _evaluate(x, K, E, T, compute_permutation, pairs=False):
     selection = _device.empty((items, K), torch.int64) if compute_permutation else None
     pm = _device.empty((items, 3, E, K), torch.float64) if pairs else None
     status = torch.zeros(1, dtype=torch.int64, device=x.device)
-    _lib.check(lib.pbb_bss_eval(_device.ptr(x), items, K, E, T, int(bool(compute_permutation)), group,
-                                _device.ptr(ws), nbytes, _device.ptr(sdr), _device.ptr(sir), _device.ptr(sar),
-                                _device.ptr(selection), _device.ptr(pm), _device.ptr(status), _device.stream_ptr()),
-               'pbb_bss_eval')
+    _device.call('pbb_bss_eval', x, items, K, E, T, int(bool(compute_permutation)), group, ws, nbytes, sdr, sir, sar,
+                 selection, pm, status)
     _device.check_status(status, _status_error)
     return sdr, sir, sar, selection, pm
 

@@ -96,9 +96,7 @@ class _SiSdr(torch.autograd.Function):
         out = _device.empty(lead, torch.float64)
         nbytes = lib.pbb_si_sdr_workspace_bytes(rows, n)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=out.device)
-        _lib.check(lib.pbb_si_sdr(_device.ptr(rd) if n else None, _device.ptr(ed) if n else None, _device.ptr(ro),
-                                  _device.ptr(eo), rows, n, _device.ptr(ws), nbytes, _device.ptr(out),
-                                  _device.stream_ptr()), 'pbb_si_sdr')
+        _device.call('pbb_si_sdr', rd if n else None, ed if n else None, ro, eo, rows, n, ws, nbytes, out)
         # the row tables of the backward are built here, where a host-to-device copy may synchronise
         tables = [_row_table(off, n, x.numel() // n) if need and n else (None, None)
                   for need, off, x in zip(ctx.needs_input_grad[:2], (ro_host, eo_host), (rd, ed))]
@@ -119,9 +117,6 @@ class _SiSdr(torch.autograd.Function):
             g = grad.to(torch.float64).contiguous()
             nbytes = lib.pbb_si_sdr_backward_workspace_bytes(rows, n)
             ws = torch.empty(nbytes, dtype=torch.uint8, device=rd.device)
-            _lib.check(lib.pbb_si_sdr_backward(
-                _device.ptr(rd), _device.ptr(ed), _device.ptr(ro), _device.ptr(eo), rows, n, _device.ptr(g),
-                rd.numel() // n, _device.ptr(rs), _device.ptr(ri), ed.numel() // n, _device.ptr(es), _device.ptr(ei),
-                _device.ptr(ws), nbytes, _device.ptr(gr), _device.ptr(ge), _device.stream_ptr()),
-                'pbb_si_sdr_backward')
+            _device.call('pbb_si_sdr_backward', rd, ed, ro, eo, rows, n, g, rd.numel() // n, rs, ri, ed.numel() // n,
+                         es, ei, ws, nbytes, gr, ge)
         return gr, ge, None, None, None, None, None, None

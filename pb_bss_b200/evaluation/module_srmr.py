@@ -111,9 +111,8 @@ def _vad(xd, sample_rate, normalise):
     out = _device.empty((rows, N), torch.float64)
     nr = _device.empty((rows,), torch.int64)
     stats = _device.empty((rows, 2), torch.float64)
-    _lib.check(lib.pbb_srmr_vad(_device.ptr(xd), _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64, rows,
-                                N, 0.05 * sample_rate, int(normalise), _device.ptr(ws), nbytes, _device.ptr(out),
-                                _device.ptr(nr), _device.ptr(stats), _device.stream_ptr()), 'pbb_srmr_vad')
+    _device.call('pbb_srmr_vad', xd, _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64, rows, N,
+                 0.05 * sample_rate, int(normalise), ws, nbytes, out, nr, stats)
     return out, nr
 
 
@@ -125,8 +124,7 @@ def _hilbert_envelopes(y, nr):
     group = max(1, min(n * rows, HILBERT_WORKSPACE_BYTES // (16 * P)))
     nbytes = lib.pbb_srmr_hilbert_workspace_bytes(rows, N, group)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
-    _lib.check(lib.pbb_srmr_hilbert(_device.ptr(y), rows, N, n, _device.ptr(nr), group, _device.ptr(ws), nbytes,
-                                    _device.stream_ptr()), 'pbb_srmr_hilbert')
+    _device.call('pbb_srmr_hilbert', y, rows, N, n, nr, group, ws, nbytes)
     return y
 
 
@@ -142,12 +140,9 @@ def _stages(xd, sample_rate, n, low_freq):
     nbytes = lib.pbb_srmr_means_workspace_bytes(rows, N, n, hop)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=xd.device)
     means = _device.empty((rows, n, 8), torch.float64)
-    _lib.check(lib.pbb_srmr_means(_device.ptr(env), rows, N, n, _device.ptr(nr), hop, _device.ptr(coef),
-                                  _device.ptr(trans), _device.ptr(window), _device.ptr(ws), nbytes, _device.ptr(means),
-                                  _device.stream_ptr()), 'pbb_srmr_means')
+    _device.call('pbb_srmr_means', env, rows, N, n, nr, hop, coef, trans, window, ws, nbytes, means)
     value = _device.empty((rows,), torch.float64)
-    _lib.check(lib.pbb_srmr_ratio(_device.ptr(means), rows, n, _device.ptr(erb), _device.ptr(cut),
-                                  _device.ptr(value), _device.stream_ptr()), 'pbb_srmr_ratio')
+    _device.call('pbb_srmr_ratio', means, rows, n, erb, cut, value)
     return dict(nr=nr, normalised=x, envelopes=env, means=means, value=value)
 
 

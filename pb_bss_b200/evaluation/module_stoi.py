@@ -195,12 +195,9 @@ def _stages(x, y, sample_rate, stages=True, extended=False):
         out['resampled'] = _device.empty((rows, 2, L), torch.float64) if (up, down) != (1, 1) else None
         out['energies'] = torch.zeros((rows, 2, BANDS, m_max), dtype=torch.float64, device=x.device)
     name = 'pbb_estoi' if extended else 'pbb_stoi'
-    _lib.check(getattr(lib, name)(_device.ptr(x), _device.ptr(y),
-                                  _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64, rows, n, up, down,
-                                  _device.ptr(taps), tpp, pre_remove, _device.ptr(win), _device.ptr(bands),
-                                  _device.ptr(tw), group, _device.ptr(ws), nbytes, _device.ptr(value),
-                                  _device.ptr(out.get('frames')), _device.ptr(out.get('resampled')),
-                                  _device.ptr(out.get('energies')), _device.ptr(status), _device.stream_ptr()), name)
+    _device.call(name, x, y, _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64, rows, n, up, down, taps, tpp,
+                 pre_remove, win, bands, tw, group, ws, nbytes, value, out.get('frames'), out.get('resampled'),
+                 out.get('energies'), status)
     _device.check_status(status[:1], _warn(status))
     return out
 
@@ -218,11 +215,8 @@ def _backward(x, y, sample_rate, extended, grad, need_x, need_y):
     gx = torch.empty((rows, n), dtype=torch.float64, device=x.device) if need_x else None
     gy = torch.empty((rows, n), dtype=torch.float64, device=x.device) if need_y else None
     g = grad.to(torch.float64).contiguous()
-    _lib.check(lib.pbb_stoi_backward(_device.ptr(x), _device.ptr(y),
-                                     _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64, rows, n, up, down,
-                                     _device.ptr(taps), tpp, pre_remove, _device.ptr(win), _device.ptr(bands),
-                                     _device.ptr(tw), group, _device.ptr(ws), nbytes, int(extended), _device.ptr(g),
-                                     _device.ptr(gx), _device.ptr(gy), _device.stream_ptr()), 'pbb_stoi_backward')
+    _device.call('pbb_stoi_backward', x, y, _lib.PBB_F32 if x.dtype == torch.float32 else _lib.PBB_F64, rows, n, up,
+                 down, taps, tpp, pre_remove, win, bands, tw, group, ws, nbytes, int(extended), g, gx, gy)
     return gx, gy
 
 

@@ -59,8 +59,7 @@ def mean_square(x):
     nbytes = lib.pbb_mean_square_workspace_bytes(rows, n)
     ws = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=x.device)
     out = torch.empty(rows, dtype=torch.float64, device=x.device)
-    _lib.check(lib.pbb_mean_square(_device.ptr(x) if x.numel() else None, _DTYPES[x.dtype], rows, n, _device.ptr(ws),
-                                   nbytes, _device.ptr(out), _device.stream_ptr()), 'pbb_mean_square')
+    _device.call('pbb_mean_square', x if x.numel() else None, _DTYPES[x.dtype], rows, n, ws, nbytes, out)
     return out
 
 
@@ -156,9 +155,7 @@ def set_snr(X, N, snr, current_snr=None, *, axis=None, inplace=True):
                          f'shape {shape}')
     out = x if inplace and n_tensor else _device.empty(shape, x.dtype)
     lay = _nd.layout(shape, x.stride(), _nd.broadcast_strides(f, shape), out.stride())
-    lib = _lib.load()
-    _lib.check(lib.pbb_scale_nd(_device.ptr(x) if x.numel() else None, _nd.CODES[x.dtype], _device.ptr(f), lay,
-                                _device.ptr(out) if out.numel() else None, _device.stream_ptr()), 'pbb_scale_nd')
+    _device.call('pbb_scale_nd', x if x.numel() else None, _nd.CODES[x.dtype], f, lay, out if out.numel() else None)
     if inplace:
         if not n_tensor:
             N[...] = out.cpu().numpy()
@@ -178,15 +175,12 @@ def _result(values, return_dict, strict):
 
 def input_sxr_from_powers(S, N, average_sources=True, average_channels=True):
     """SDR, SIR, SNR (float64 CUDA tensors) of input_sxr from the powers S (K, D) and N (D), float64 CUDA tensors."""
-    lib = _lib.load()
     K, D = S.shape
     shape = {(True, True): (), (False, True): (K,), (True, False): (D,), (False, False): (K, D)}[
         (bool(average_sources), bool(average_channels))]
     out = [_device.empty(shape, torch.float64) for _ in range(3)]
     S, N = S.contiguous(), N.contiguous()
-    _lib.check(lib.pbb_input_sxr(_device.ptr(S), _device.ptr(N), K, D, int(bool(average_sources)),
-                                 int(bool(average_channels)), *(_device.ptr(v) for v in out), _device.stream_ptr()),
-               'pbb_input_sxr')
+    _device.call('pbb_input_sxr', S, N, K, D, int(bool(average_sources)), int(bool(average_channels)), *out)
     return out
 
 
@@ -219,9 +213,7 @@ def output_sxr_from_powers(S, N, average_sources=True):
     nbytes = lib.pbb_output_sxr_workspace_bytes(K_source, K_target)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=S.device)
     S, N = S.contiguous(), N.contiguous()
-    _lib.check(lib.pbb_output_sxr(_device.ptr(S), _device.ptr(N), K_source, K_target, int(bool(average_sources)),
-                                  _device.ptr(ws), nbytes, *(_device.ptr(v) for v in out), _device.ptr(selection),
-                                  _device.stream_ptr()), 'pbb_output_sxr')
+    _device.call('pbb_output_sxr', S, N, K_source, K_target, int(bool(average_sources)), ws, nbytes, *out, selection)
     return out + [selection]
 
 

@@ -6,7 +6,7 @@ import numpy as np
 import torch
 from numpy.exceptions import AxisError
 
-from .. import _device, _lib
+from .. import _device
 
 
 def get_stft_center_frequencies(size=1024, sample_rate=16000):
@@ -36,9 +36,7 @@ def get_steering_vector(
     A = tdoa.numel() // M if M else 0
     out = _device.empty((*tdoa.shape, F), torch.complex128)
     if out.numel():
-        lib = _lib.load()
-        _lib.check(lib.pbb_steering_vector(_device.ptr(tdoa), A, M, _device.ptr(freq), F, int(bool(normalize)),
-                                           _device.ptr(out), _device.stream_ptr()), 'pbb_steering_vector')
+        _device.call('pbb_steering_vector', tdoa, A, M, freq, F, int(bool(normalize)), out)
     return _device.to_host(out, like_numpy)
 
 
@@ -56,10 +54,7 @@ def get_diffuse_noise_psd(
     F, D = freq.shape[0], dist.shape[0]
     out = _device.empty((F, D, D), torch.float64)
     if out.numel():
-        lib = _lib.load()
-        _lib.check(lib.pbb_diffuse_noise_coherence(_device.ptr(dist), D, _device.ptr(freq), F, float(sound_velocity),
-                                                   _device.ptr(out), _device.stream_ptr()),
-                   'pbb_diffuse_noise_coherence')
+        _device.call('pbb_diffuse_noise_coherence', dist, D, freq, F, float(sound_velocity), out)
     return _device.to_host(out, like_numpy)
 
 
@@ -75,9 +70,7 @@ def get_nearfield_time_of_flight(source_positions, sensor_positions,
     S, M = src.shape[1], sen.shape[1]
     out = _device.empty((S, M), torch.float64)
     if out.numel():
-        lib = _lib.load()
-        _lib.check(lib.pbb_array_geometry(0, _device.ptr(src), S, _device.ptr(sen), M, 0, float(sound_velocity),
-                                          _device.ptr(out), _device.stream_ptr()), 'pbb_array_geometry')
+        _device.call('pbb_array_geometry', 0, src, S, sen, M, 0, float(sound_velocity), out)
     return _device.to_host(out, like_numpy)
 
 
@@ -96,8 +89,5 @@ def get_farfield_time_difference_of_arrival(
         raise IndexError(f'index {reference_channel} is out of bounds for axis 1 with size {M}')
     out = _device.empty((M, K), torch.float64)
     if out.numel():
-        lib = _lib.load()
-        _lib.check(lib.pbb_array_geometry(1, _device.ptr(ang), K, _device.ptr(sen), M, reference_channel % M,
-                                          float(sound_velocity), _device.ptr(out), _device.stream_ptr()),
-                   'pbb_array_geometry')
+        _device.call('pbb_array_geometry', 1, ang, K, sen, M, reference_channel % M, float(sound_velocity), out)
     return _device.to_host(out, like_numpy)

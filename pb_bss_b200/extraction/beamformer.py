@@ -113,10 +113,7 @@ class _Psd(torch.autograd.Function):
         psd = _device.empty((F, K, D, D), torch.complex128)
         nbytes = lib.pbb_psd_workspace_bytes(F, T, D, K)
         ws = _device.workspace(nbytes)
-        _lib.check(lib.pbb_power_spectral_density(
-            _device.ptr(obs), code, F, D, T, _device.ptr(m), K, int(normalize),
-            _device.ptr(psd), _device.ptr(ws), nbytes, _device.stream_ptr()),
-            'pbb_power_spectral_density')
+        _device.call('pbb_power_spectral_density', obs, code, F, D, T, m, K, int(normalize), psd, ws, nbytes)
         ctx.save_for_backward(obs, m, psd)
         ctx.args = (code, K, normalize)
         return psd
@@ -132,9 +129,8 @@ class _Psd(torch.autograd.Function):
         gm = _device.empty((F, K, T), torch.float64) if need_m else None
         if need_y or need_m:
             g = grad.to(torch.complex128).contiguous()
-            _lib.check(_lib.load().pbb_power_spectral_density_backward(
-                _device.ptr(obs), code, F, D, T, _device.ptr(m), K, int(normalize), _device.ptr(psd), _device.ptr(g),
-                _device.ptr(gy), _device.ptr(gm), _device.stream_ptr()), 'pbb_power_spectral_density_backward')
+            _device.call('pbb_power_spectral_density_backward', obs, code, F, D, T, m, K, int(normalize), psd, g, gy,
+                         gm)
         return None if gy is None else gy.to(obs.dtype), gm, None, None
 
 
@@ -158,8 +154,7 @@ class _TopEig(torch.autograd.Function):
         w = _device.empty((n, D), torch.float64)
         v = _device.empty((n, D, D), torch.complex128)
         status = _status()
-        _lib.check(_lib.load().pbb_heig_batched(_device.ptr(af), n, D, _device.ptr(w), _device.ptr(v),
-                                                _device.ptr(status), _device.stream_ptr()), 'pbb_heig_batched')
+        _device.call('pbb_heig_batched', af, n, D, w, v, status)
 
         def on_error(s):
             raise np.linalg.LinAlgError(f'eigh: non-finite input or no convergence in matrix {s - 1}')
@@ -176,9 +171,7 @@ class _TopEig(torch.autograd.Function):
         gv = grad_vec.to(torch.complex128).contiguous()
         gl = grad_val.to(torch.float64).contiguous()
         ga = _device.empty((n, D, D), torch.complex128)
-        _lib.check(_lib.load().pbb_eigenvector_backward(
-            _device.ptr(af), None, _device.ptr(vec), _device.ptr(gv), _device.ptr(gl), n, D, _device.ptr(ga), None,
-            _device.stream_ptr()), 'pbb_eigenvector_backward')
+        _device.call('pbb_eigenvector_backward', af, None, vec, gv, gl, n, D, ga, None)
         return ga
 
 
@@ -228,8 +221,7 @@ class _Mvdr(torch.autograd.Function):
         w = _device.empty((n, D), torch.complex128)
         scratch = _device.empty((n, D), torch.complex128)
         status = _status()
-        _lib.check(_lib.load().pbb_mvdr(_device.ptr(atf_f), _device.ptr(noise_f), n, D, _device.ptr(w),
-                                        _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_mvdr')
+        _device.call('pbb_mvdr', atf_f, noise_f, n, D, w, scratch, status)
         # a singular noise PSD matrix takes the reference's np.linalg.lstsq fallback (beamformer.py:251-256) on the
         # device (minimum-norm solution); the status word is only set where that fallback does not exist (D > 40)
         def on_error(s):
@@ -248,9 +240,7 @@ class _Mvdr(torch.autograd.Function):
         ga = _device.empty((n, D), torch.complex128)
         gn = _device.empty((n, D, D), torch.complex128)
         scratch = _device.empty((n, D), torch.complex128)
-        _lib.check(_lib.load().pbb_mvdr_backward(
-            _device.ptr(atf_f), _device.ptr(noise_f), _device.ptr(x), _device.ptr(w), _device.ptr(g), n, D,
-            _device.ptr(ga), _device.ptr(gn), _device.ptr(scratch), _device.stream_ptr()), 'pbb_mvdr_backward')
+        _device.call('pbb_mvdr_backward', atf_f, noise_f, x, w, g, n, D, ga, gn, scratch)
         return ga, gn
 
 
@@ -284,8 +274,7 @@ class _Gev(torch.autograd.Function):
         n, D = af.shape[0], af.shape[-1]
         w = _device.empty((n, D), torch.complex128)
         status = _status()
-        _lib.check(_lib.load().pbb_gev_batched(_device.ptr(af), _device.ptr(bf), n, D, _device.ptr(w),
-                                               _device.ptr(status), _device.stream_ptr()), 'pbb_gev_batched')
+        _device.call('pbb_gev_batched', af, bf, n, D, w, status)
 
         def on_error(s):
             # get_gev_vector.pyx:130-147 / beamformer.py:398-408
@@ -302,9 +291,7 @@ class _Gev(torch.autograd.Function):
         g = grad.to(torch.complex128).contiguous()
         ga = _device.empty((n, D, D), torch.complex128)
         gb = _device.empty((n, D, D), torch.complex128)
-        _lib.check(_lib.load().pbb_eigenvector_backward(
-            _device.ptr(af), _device.ptr(bf), _device.ptr(w), _device.ptr(g), None, n, D, _device.ptr(ga),
-            _device.ptr(gb), _device.stream_ptr()), 'pbb_eigenvector_backward')
+        _device.call('pbb_eigenvector_backward', af, bf, w, g, None, n, D, ga, gb)
         return ga, gb
 
 
@@ -346,12 +333,10 @@ class _Souden(torch.autograd.Function):
     @staticmethod
     def forward(ctx, tf, nf, ref_channel, eps, lead_dims, chosen):
         n, D = tf.shape[0], tf.shape[-1]
-        lib = _lib.load()
         phi = _device.empty((n, D, D), torch.complex128)
         status = _device.empty((1,), torch.int32)
         status.zero_()
-        _lib.check(lib.pbb_solve_batched(_device.ptr(nf), _device.ptr(tf), n, D, D, 0, _device.ptr(phi),
-                                         _device.ptr(status), _device.stream_ptr()), 'pbb_solve_batched')
+        _device.call('pbb_solve_batched', nf, tf, n, D, D, 0, phi, status)
         # stable_solve (math/solve.py:95-114): singular systems get the minimum-norm (lstsq) solution on the device
         def on_error(s):
             raise np.linalg.LinAlgError(
@@ -362,9 +347,7 @@ class _Souden(torch.autograd.Function):
         den = _device.empty((n, D), torch.complex128)
         nsum = _device.empty((D,), torch.complex128)
         dsum = _device.empty((D,), torch.complex128)
-        _lib.check(lib.pbb_souden(_device.ptr(phi), _device.ptr(tf), _device.ptr(nf), n, D, eps,
-                                  _device.ptr(mat), _device.ptr(num), _device.ptr(den), _device.ptr(nsum),
-                                  _device.ptr(dsum), _device.stream_ptr()), 'pbb_souden')
+        _device.call('pbb_souden', phi, tf, nf, n, D, eps, mat, num, den, nsum, dsum)
         if ref_channel is None:
             if lead_dims != 1:
                 raise ValueError(
@@ -390,9 +373,7 @@ class _Souden(torch.autograd.Function):
         g = grad.to(torch.complex128).contiguous()
         gt = _device.empty((n, D, D), torch.complex128)
         gn = _device.empty((n, D, D), torch.complex128)
-        _lib.check(_lib.load().pbb_souden_backward(_device.ptr(phi), _device.ptr(nf), _device.ptr(g), n, D, ref, eps,
-                                                   _device.ptr(gt), _device.ptr(gn), _device.stream_ptr()),
-                   'pbb_souden_backward')
+        _device.call('pbb_souden_backward', phi, nf, g, n, D, ref, eps, gt, gn)
         return gt, gn, None, None, None, None
 
 
@@ -417,9 +398,7 @@ class _Ban(torch.autograd.Function):
     def forward(ctx, vf, nf):
         n, D = vf.shape
         out = _device.empty((n, D), torch.complex128)
-        _lib.check(_lib.load().pbb_blind_analytic_normalization(_device.ptr(vf), _device.ptr(nf), n, D,
-                                                                _device.ptr(out), _device.stream_ptr()),
-                   'pbb_blind_analytic_normalization')
+        _device.call('pbb_blind_analytic_normalization', vf, nf, n, D, out)
         ctx.save_for_backward(vf, nf)
         return out
 
@@ -431,9 +410,7 @@ class _Ban(torch.autograd.Function):
         g = grad.to(torch.complex128).contiguous()
         gv = _device.empty((n, D), torch.complex128)
         gn = _device.empty((n, D, D), torch.complex128)
-        _lib.check(_lib.load().pbb_blind_analytic_normalization_backward(
-            _device.ptr(vf), _device.ptr(nf), _device.ptr(g), n, D, _device.ptr(gv), _device.ptr(gn),
-            _device.stream_ptr()), 'pbb_blind_analytic_normalization_backward')
+        _device.call('pbb_blind_analytic_normalization_backward', vf, nf, g, n, D, gv, gn)
         return gv, gn
 
 
@@ -477,18 +454,13 @@ class _Apply(torch.autograd.Function):
     def forward(ctx, v, y, shared):
         code = _device.complex_dtype_code(y)
         F, D, T = y.shape
-        lib = _lib.load()
         if shared:
             B = v.shape[0]
             out = _device.empty((B, F, T), torch.complex128)
-            _lib.check(lib.pbb_apply_beamforming_vector_shared(_device.ptr(v), _device.ptr(y), code, B, F, D, T,
-                                                               _device.ptr(out), _device.stream_ptr()),
-                       'pbb_apply_beamforming_vector_shared')
+            _device.call('pbb_apply_beamforming_vector_shared', v, y, code, B, F, D, T, out)
         else:
             out = _device.empty((F, T), torch.complex128)
-            _lib.check(lib.pbb_apply_beamforming_vector(_device.ptr(v), _device.ptr(y), code, F, D, T,
-                                                        _device.ptr(out), _device.stream_ptr()),
-                       'pbb_apply_beamforming_vector')
+            _device.call('pbb_apply_beamforming_vector', v, y, code, F, D, T, out)
         ctx.save_for_backward(v, y)
         ctx.args = (code, shared)
         return out
@@ -504,15 +476,10 @@ class _Apply(torch.autograd.Function):
         gy = _device.empty((F, D, T), torch.complex128) if need_y else None
         if need_v or need_y:
             g = grad.to(torch.complex128).contiguous()
-            lib = _lib.load()
             if shared:
-                _lib.check(lib.pbb_apply_beamforming_vector_shared_backward(
-                    _device.ptr(v), _device.ptr(y), code, v.shape[0], F, D, T, _device.ptr(g), _device.ptr(gv),
-                    _device.ptr(gy), _device.stream_ptr()), 'pbb_apply_beamforming_vector_shared_backward')
+                _device.call('pbb_apply_beamforming_vector_shared_backward', v, y, code, v.shape[0], F, D, T, g, gv, gy)
             else:
-                _lib.check(lib.pbb_apply_beamforming_vector_backward(
-                    _device.ptr(v), _device.ptr(y), code, F, D, T, _device.ptr(g), _device.ptr(gv), _device.ptr(gy),
-                    _device.stream_ptr()), 'pbb_apply_beamforming_vector_backward')
+                _device.call('pbb_apply_beamforming_vector_backward', v, y, code, F, D, T, g, gv, gy)
         return gv, None if gy is None else gy.to(y.dtype), None
 
 
@@ -568,10 +535,7 @@ def get_optimal_reference_channel(w_mat, target_psd_matrix, noise_psd_matrix, ep
     den = _device.empty((n, D), torch.complex128)
     nsum = _device.empty((D,), torch.complex128)
     dsum = _device.empty((D,), torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_reference_channel_snr(_device.ptr(w), _device.ptr(t), _device.ptr(nz), n, D, _device.ptr(num),
-                                             _device.ptr(den), _device.ptr(nsum), _device.ptr(dsum),
-                                             _device.stream_ptr()), 'pbb_reference_channel_snr')
+    _device.call('pbb_reference_channel_snr', w, t, nz, n, D, num, den, nsum, dsum)
     ns, ds = nsum.cpu().numpy(), dsum.cpu().numpy()
     snr = ns / np.maximum(ds, eps)
     assert np.all(np.isfinite(snr)), snr
@@ -598,9 +562,7 @@ def get_mvdr_vector_merl(target_psd_matrix, noise_psd_matrix):
     w = _device.empty((n, D), torch.complex128)
     scratch = _device.empty((n, D, D), torch.complex128)
     status = _status()
-    lib = _lib.load()
-    _lib.check(lib.pbb_mvdr_merl(_device.ptr(t), _device.ptr(nz), n, D, _device.ptr(w), _device.ptr(scratch),
-                                 _device.ptr(status), _device.stream_ptr()), 'pbb_mvdr_merl')
+    _device.call('pbb_mvdr_merl', t, nz, n, D, w, scratch, status)
 
     def on_error(s):
         raise np.linalg.LinAlgError(f'Singular matrix (get_mvdr_vector_merl: noise PSD matrix of bin {s - 1})')
@@ -628,9 +590,7 @@ def get_lcmv_vector(atf_vectors, response_vector, noise_psd_matrix):
     w = _device.empty((F, D), torch.complex128)
     scratch = _device.empty((F * (2 * D * K + K * K + 2 * K) + 1,), torch.complex128)
     status = _status()
-    lib = _lib.load()
-    _lib.check(lib.pbb_lcmv(_device.ptr(a), _device.ptr(r), _device.ptr(nz), K, F, D, _device.ptr(w),
-                            _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_lcmv')
+    _device.call('pbb_lcmv', a, r, nz, K, F, D, w, scratch, status)
 
     def on_error(s):
         raise np.linalg.LinAlgError(f'get_lcmv_vector: singular system in bin {s - 1} (D or K > 40: no lstsq fallback)')
@@ -670,9 +630,7 @@ def get_wmwf_vector(target_psd_matrix, noise_psd_matrix, reference_channel=None,
     filt = _device.empty((n, D, D), torch.complex128)
     scratch = _device.empty((n, D, D), torch.complex128)
     status = _status()
-    lib = _lib.load()
-    _lib.check(lib.pbb_wmwf(_device.ptr(tf), _device.ptr(nf), n, D, int(frequency_dependent), mu, _device.ptr(filt),
-                            _device.ptr(scratch), _device.ptr(status), _device.stream_ptr()), 'pbb_wmwf')
+    _device.call('pbb_wmwf', tf, nf, n, D, int(frequency_dependent), mu, filt, scratch, status)
 
     def on_error(s):
         raise np.linalg.LinAlgError(f'get_wmwf_vector: singular noise PSD matrix {s - 1} (D > 40: no lstsq fallback)')
@@ -684,8 +642,7 @@ def get_wmwf_vector(target_psd_matrix, noise_psd_matrix, reference_channel=None,
         ff = filt.expand(shape).reshape(-1, D, D).contiguous()
         sf = sel.expand(shape).reshape(-1, D, D).contiguous()
         out = _device.empty((ff.shape[0], D), torch.complex128)
-        _lib.check(lib.pbb_weighted_channel_sum(_device.ptr(ff), _device.ptr(sf), ff.shape[0], D, _device.ptr(out),
-                                                _device.stream_ptr()), 'pbb_weighted_channel_sum')
+        _device.call('pbb_weighted_channel_sum', ff, sf, ff.shape[0], D, out)
         return _device.to_host(out.reshape(shape[:-1]), like_numpy)
     if reference_channel is None:
         reference_channel = get_optimal_reference_channel(filt, tf.reshape(*lead, D, D), nf.reshape(*lead, D, D),
@@ -701,9 +658,7 @@ def condition_covariance(x, gamma):
     D = xd.shape[-1]
     xf, lead = _flat(xd, 2)
     out = _device.empty(xf.shape, torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_condition_covariance(_device.ptr(xf), xf.shape[0], D, float(gamma), _device.ptr(out),
-                                            _device.stream_ptr()), 'pbb_condition_covariance')
+    _device.call('pbb_condition_covariance', xf, xf.shape[0], D, float(gamma), out)
     return _device.to_host(out.reshape(*lead, D, D), like_numpy)
 
 
@@ -724,10 +679,7 @@ def distortionless_normalization(vector, atf_vector, noise_psd_matrix):
     if a.shape != v.shape or tuple(nz.shape) != (F, D, D):
         raise ValueError(f'shape mismatch: {tuple(v.shape)}, {tuple(a.shape)}, {tuple(nz.shape)}')
     out = _device.empty((F, D), torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_distortionless_normalization(_device.ptr(v), _device.ptr(a), _device.ptr(nz), F, D,
-                                                    _device.ptr(out), _device.stream_ptr()),
-               'pbb_distortionless_normalization')
+    _device.call('pbb_distortionless_normalization', v, a, nz, F, D, out)
     return _device.to_host(out, like_numpy)
 
 
@@ -741,9 +693,7 @@ def mvdr_snr_postfilter(vector, target_psd_matrix, noise_psd_matrix):
     if tuple(t.shape) != (F, D, D) or tuple(nz.shape) != (F, D, D):
         raise ValueError(f'shape mismatch: {tuple(v.shape)}, {tuple(t.shape)}, {tuple(nz.shape)}')
     out = _device.empty((F, 1), torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_mvdr_snr_postfilter(_device.ptr(v), _device.ptr(t), _device.ptr(nz), F, D, _device.ptr(out),
-                                           _device.stream_ptr()), 'pbb_mvdr_snr_postfilter')
+    _device.call('pbb_mvdr_snr_postfilter', v, t, nz, F, D, out)
     return _device.to_host(out, like_numpy)
 
 
@@ -757,9 +707,7 @@ def zero_degree_normalization(vector, reference_channel):
         raise IndexError(f'index {ref} is out of bounds for axis {v.dim() - 1} with size {D}')
     vf, lead = _flat(v, 1)
     out = _device.empty(vf.shape, torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_zero_degree_normalization(_device.ptr(vf), vf.shape[0], D, ref % D, _device.ptr(out),
-                                                 _device.stream_ptr()), 'pbb_zero_degree_normalization')
+    _device.call('pbb_zero_degree_normalization', vf, vf.shape[0], D, ref % D, out)
     return _device.to_host(out.reshape(*lead, D), like_numpy)
 
 
@@ -790,9 +738,7 @@ def phase_correction(vector):
     out = _device.empty(tuple(v.shape), torch.complex128)
     if out.numel() == 0:
         return _device.to_host(out, like_numpy)
-    lib = _lib.load()
-    _lib.check(lib.pbb_phase_correction(_device.ptr(v), A, M, F, D, scan, _device.ptr(out), _device.stream_ptr()),
-               'pbb_phase_correction')
+    _device.call('pbb_phase_correction', v, A, M, F, D, scan, out)
     return _device.to_host(out, like_numpy)
 
 
@@ -818,8 +764,6 @@ def apply_online_beamforming_vector(vector, mix):
     if ye.stride(2) != T or ye.stride(3) != 1:
         ye = ye.contiguous()
     out = _device.empty((B, F, T), torch.complex128)
-    lib = _lib.load()
-    _lib.check(lib.pbb_apply_online_beamforming_vector(
-        _device.ptr(v), _device.ptr(ye), code, B, F, D, T, Fv * D, D if Fv == F else 0, ye.stride(0), ye.stride(1),
-        _device.ptr(out), _device.stream_ptr()), 'pbb_apply_online_beamforming_vector')
+    _device.call('pbb_apply_online_beamforming_vector', v, ye, code, B, F, D, T, Fv * D, D if Fv == F else 0,
+                 ye.stride(0), ye.stride(1), out)
     return _device.to_host(out.reshape(*lead, T), like_numpy)

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
 
-from .. import _device, _lib
+from .. import _device
 from .beamformer import (
     blind_analytic_normalization,
     get_gev_vector,
@@ -48,8 +48,7 @@ class _RankOne(torch.autograd.Function):
     def forward(ctx, af, cf):
         n, D = af.shape
         out = _device.empty((n, D, D), torch.complex128)
-        _lib.check(_lib.load().pbb_rank_one_estimate(_device.ptr(af), _device.ptr(cf), n, D, _device.ptr(out),
-                                                     _device.stream_ptr()), 'pbb_rank_one_estimate')
+        _device.call('pbb_rank_one_estimate', af, cf, n, D, out)
         ctx.save_for_backward(af, cf)
         return out
 
@@ -61,9 +60,7 @@ class _RankOne(torch.autograd.Function):
         g = grad.to(torch.complex128).contiguous()
         ga = _device.empty((n, D), torch.complex128)
         gc = _device.empty((n, D, D), torch.complex128)
-        _lib.check(_lib.load().pbb_rank_one_estimate_backward(
-            _device.ptr(af), _device.ptr(cf), _device.ptr(g), n, D, _device.ptr(ga), _device.ptr(gc),
-            _device.stream_ptr()), 'pbb_rank_one_estimate_backward')
+        _device.call('pbb_rank_one_estimate_backward', af, cf, g, n, D, ga, gc)
         return ga, gc
 
 
@@ -87,8 +84,7 @@ class _Matvec(torch.autograd.Function):
     def forward(ctx, mf, vf):
         n, D = vf.shape
         out = _device.empty((n, D), torch.complex128)
-        _lib.check(_lib.load().pbb_matvec_batched(_device.ptr(mf), _device.ptr(vf), n, D, _device.ptr(out),
-                                                  _device.stream_ptr()), 'pbb_matvec_batched')
+        _device.call('pbb_matvec_batched', mf, vf, n, D, out)
         ctx.save_for_backward(mf, vf)
         return out
 
@@ -100,9 +96,7 @@ class _Matvec(torch.autograd.Function):
         g = grad.to(torch.complex128).contiguous()
         gm = _device.empty((n, D, D), torch.complex128)
         gv = _device.empty((n, D), torch.complex128)
-        _lib.check(_lib.load().pbb_matvec_batched_backward(
-            _device.ptr(mf), _device.ptr(vf), _device.ptr(g), n, D, _device.ptr(gm), _device.ptr(gv),
-            _device.stream_ptr()), 'pbb_matvec_batched_backward')
+        _device.call('pbb_matvec_batched_backward', mf, vf, g, n, D, gm, gv)
         return gm, gv
 
 

@@ -2,7 +2,7 @@
 import numpy as np
 import torch
 
-from .. import _device, _lib
+from .. import _device
 
 
 def eigh(a):
@@ -17,10 +17,7 @@ def eigh(a):
     w = _device.empty((n, D), torch.float64)
     v = _device.empty((n, D, D), torch.complex128)
     status = torch.zeros(1, dtype=torch.int32, device=ad.device)
-    lib = _lib.load()
-    _lib.check(lib.pbb_heig_batched(
-        _device.ptr(ad), n, D, _device.ptr(w), _device.ptr(v),
-        _device.ptr(status), _device.stream_ptr()), 'pbb_heig_batched')
+    _device.call('pbb_heig_batched', ad, n, D, w, v, status)
     def on_error(s):
         raise np.linalg.LinAlgError(f'eigh: non-finite input or no convergence in matrix {s - 1}')
     _device.check_status(status, on_error)
@@ -43,10 +40,8 @@ def stable_solve(A, B, hermitize=False):
     n = int(np.prod(lead)) if lead else 1
     x = _device.empty((n, D, R), torch.complex128)
     status = torch.zeros(1, dtype=torch.int32, device=ad.device)
-    lib = _lib.load()
-    _lib.check(lib.pbb_solve_batched(
-        _device.ptr(ad.reshape(n, D, D).contiguous()), _device.ptr(bd.reshape(n, D, R).contiguous()), n, D, R,
-        1 if hermitize else 0, _device.ptr(x), _device.ptr(status), _device.stream_ptr()), 'pbb_solve_batched')
+    _device.call('pbb_solve_batched', ad.reshape(n, D, D).contiguous(), bd.reshape(n, D, R).contiguous(), n, D, R,
+                 1 if hermitize else 0, x, status)
     def on_error(s):
         raise np.linalg.LinAlgError(f'stable_solve: singular matrix {s - 1} (D > 40: no lstsq fallback)')
     _device.check_status(status, on_error)

@@ -106,11 +106,8 @@ def _source_mask(kind, signal, source_axis, sensor_axis, keepdims, eps):
     if out.numel():
         ostr = _contiguous_strides(keep_shape)
         rest = _layout([(shape[a], x.stride(a), ostr[a]) for a in range(nd) if a not in (sa, se)])
-        lib = _lib.load()
-        _lib.check(lib.pbb_source_mask(
-            _device.ptr(x), _CODES[x.dtype], kind, shape[sa], 1 if se is None else shape[se], x.stride(sa),
-            0 if se is None else x.stride(se), ostr[sa], rest, eps, _device.ptr(out), _device.stream_ptr()),
-            'pbb_source_mask')
+        _device.call('pbb_source_mask', x, _CODES[x.dtype], kind, shape[sa], 1 if se is None else shape[se],
+                     x.stride(sa), 0 if se is None else x.stride(se), ostr[sa], rest, eps, out)
     if se is not None and not keepdims:
         out = out.squeeze(se)
     return _device.to_host(out, like_numpy)
@@ -211,11 +208,11 @@ def _row_geometry(x, elem_axes, pooled_axis, out_shape):
     return rows, elems, n_rows, n
 
 
-def _scratch(lib, n_rows, n):
+def _scratch(n_rows, n):
     if n <= _lib.ROW_SELECT_SHORT_MAX:
         return None, 0
-    nbytes = lib.pbb_row_select_scratch_bytes(n_rows, n)
-    return _device.ptr(_device.workspace(nbytes)), nbytes
+    nbytes = _lib.load().pbb_row_select_scratch_bytes(n_rows, n)
+    return _device.workspace(nbytes), nbytes
 
 
 def lorenz_mask(
@@ -247,13 +244,11 @@ def lorenz_mask(
     out = _device.empty(out_shape, rdt)
     if out.numel():
         rows, elems, n_rows, n = _row_geometry(x, elem_axes, se, out_shape)
-        lib = _lib.load()
-        scratch, nbytes = _scratch(lib, n_rows, n)
+        scratch, nbytes = _scratch(n_rows, n)
         status = torch.zeros(1, dtype=torch.int32, device=x.device)
-        _lib.check(lib.pbb_lorenz_mask(
-            _device.ptr(x), _CODES[x.dtype], 1 if se is None else x.shape[se], 0 if se is None else x.stride(se),
-            rows, elems, float(lorenz_fraction), lo, hi, _device.ptr(out), scratch, nbytes, _device.ptr(status),
-            _device.stream_ptr()), 'pbb_lorenz_mask')
+        _device.call('pbb_lorenz_mask', x, _CODES[x.dtype], 1 if se is None else x.shape[se],
+                     0 if se is None else x.stride(se), rows, elems, float(lorenz_fraction), lo, hi, out, scratch,
+                     nbytes, status)
 
         def on_error(s):
             raise ValueError(f'lorenz_mask: no value of row {s - 1} has a Lorenz value below lorenz_fraction='
@@ -315,11 +310,9 @@ def quantile_mask(
         rows, elems, n_rows, n = _row_geometry(x, elem_axes, None, list(x.shape))
         percent = (1 - quantile) * 100 if quantile >= 0 else abs(quantile) * 100
         k_lower, k_upper, gamma, one_minus_gamma = _percentile_terms(n, percent, np_dtype)
-        lib = _lib.load()
-        scratch, nbytes = _scratch(lib, n_rows, n)
-        _lib.check(lib.pbb_quantile_mask(
-            _device.ptr(x), _CODES[x.dtype], rows, elems, k_lower, k_upper, gamma, one_minus_gamma,
-            int(quantile < 0), lo, hi, _device.ptr(out), scratch, nbytes, _device.stream_ptr()), 'pbb_quantile_mask')
+        scratch, nbytes = _scratch(n_rows, n)
+        _device.call('pbb_quantile_mask', x, _CODES[x.dtype], rows, elems, k_lower, k_upper, gamma, one_minus_gamma,
+                     int(quantile < 0), lo, hi, out, scratch, nbytes)
     return _device.to_host(out, like_numpy)
 
 
@@ -363,8 +356,5 @@ def biased_binary_mask(
         ostr = _contiguous_strides(list(x.shape))
         rest = _layout([(x.shape[a], x.stride(a), ostr[a]) for a in range(nd) if a != ca])
         sd, nd_, fc = (_device.to_device(a) for a in (speech_div, noise_div, force))
-        lib = _lib.load()
-        _lib.check(lib.pbb_biased_binary_mask(
-            _device.ptr(x), _CODES[x.dtype], x.stride(ca), ostr[ca], rest, L, _device.ptr(sd), _device.ptr(nd_),
-            _device.ptr(fc), _device.ptr(out), _device.stream_ptr()), 'pbb_biased_binary_mask')
+        _device.call('pbb_biased_binary_mask', x, _CODES[x.dtype], x.stride(ca), ostr[ca], rest, L, sd, nd_, fc, out)
     return _device.to_host(out, like_numpy)

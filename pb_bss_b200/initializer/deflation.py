@@ -8,7 +8,7 @@ similarity |z^H m|^2).  torch only selects the frames around the saliency maximu
 import numpy as np
 import torch
 
-from .. import _device, _lib
+from .. import _device
 from ..extraction import (apply_beamforming_vector, get_pca_vector,
                           get_power_spectral_density_matrix)
 
@@ -17,9 +17,7 @@ def _unit_norm(Y):
     """_parameterized_vector_norm over the last axis (permutation_alignment.py:358-377) of (F, T, D)."""
     F, T, D = Y.shape
     z = torch.empty_like(Y)
-    lib = _lib.load()
-    _lib.check(lib.pbb_normalize_observation(_device.ptr(Y), _device.ptr(z), F, T, D, _device.complex_dtype_code(Y), 0,
-                                             _device.stream_ptr()), 'pbb_normalize_observation')
+    _device.call('pbb_normalize_observation', Y, z, F, T, D, _device.complex_dtype_code(Y), 0)
     return z
 
 

@@ -46,9 +46,7 @@ def apply_mapping(mask, mapping):
     T = int(np.prod(md.shape[2:])) if md.dim() > 2 else 1
     md = md.reshape(K, F, T).contiguous()
     out = _device.empty((K, F, T), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_apply_mapping(_device.ptr(md), _device.ptr(mp), K, F, T, _device.ptr(out),
-                                     _device.stream_ptr()), 'pbb_apply_mapping')
+    _device.call('pbb_apply_mapping', md, mp, K, F, T, out)
     out = out.reshape(m.shape).to(out_dtype)
     return _device.to_host(out, like_numpy)
 
@@ -142,10 +140,8 @@ class DHTVPermutationAlignment(_PermutationAlignment):
         mapping = _device.empty((K, F), torch.int64)
         if self.algorithm not in _ALGORITHMS:
             raise ValueError(self.algorithm)   # _mapping_from_score_matrix (:588-589)
-        _lib.check(lib.pbb_dhtv_mapping_ex(_device.ptr(m), K, F, T, plan_p, int(plan.shape[0]),
-                                           _device.ptr(feat), _device.ptr(cent), _device.ptr(mapping),
-                                           self._metric, _ALGORITHMS[self.algorithm],
-                                           _device.stream_ptr()), 'pbb_dhtv_mapping_ex')
+        _device.call('pbb_dhtv_mapping_ex', m, K, F, T, plan_p, int(plan.shape[0]), feat, cent, mapping, self._metric,
+                     _ALGORITHMS[self.algorithm])
         return _device.to_host(mapping, like_numpy)
 
 
@@ -172,9 +168,7 @@ def _score_matrix(mask, reference_mask, metric, F, source_strides=None):
     K, _, T = mask.shape
     ms, rs = source_strides or (mask.shape[1] * T, reference_mask.shape[1] * T)
     scores = _device.empty((F, K, K), torch.float64)
-    lib = _lib.load()
-    _lib.check(lib.pbb_score_matrix(_device.ptr(mask), _device.ptr(reference_mask), ms, rs, K, F, T, metric,
-                                    _device.ptr(scores), _device.stream_ptr()), 'pbb_score_matrix')
+    _device.call('pbb_score_matrix', mask, reference_mask, ms, rs, K, F, T, metric, scores)
     return scores
 
 
@@ -190,10 +184,7 @@ def _mapping_from_score_matrix(score_matrix, algorithm='optimal'):
     sc = sc.reshape(n, K, K).contiguous()
     mapping = _device.empty((K, n), torch.int64)
     status = torch.zeros(1, dtype=torch.int32, device=sc.device)
-    lib = _lib.load()
-    _lib.check(lib.pbb_mapping_from_score_matrix(_device.ptr(sc), n, K, _ALGORITHMS[algorithm],
-                                                 _device.ptr(mapping), _device.ptr(status),
-                                                 _device.stream_ptr()), 'pbb_mapping_from_score_matrix')
+    _device.call('pbb_mapping_from_score_matrix', sc, n, K, _ALGORITHMS[algorithm], mapping, status)
     def on_error(s):
         # message of scipy.optimize.linear_sum_assignment, like the reference (:511-513)
         raise ValueError('score matrix is infeasible')
@@ -223,18 +214,14 @@ class GreedyPermutationAlignment(_PermutationAlignment):
         K, F, T = m.shape
         assert K < 10, (K, 'Sure?')
         assert F % 2 == 1, (F, 'Sure? Usually F is odd.', tuple(m.shape))
-        lib = _lib.load()
         mapping = _device.empty((K, F), torch.int64)
         pair = None
         if F > 1:
             # scores between mask[:, 1:] and mask[:, :-1]: two views of the same array
             scores = _device.empty((F - 1, K, K), torch.float64)
-            _lib.check(lib.pbb_score_matrix(_device.ptr(m) + T * 8, _device.ptr(m), F * T, F * T, K, F - 1, T,
-                                            self._metric, _device.ptr(scores), _device.stream_ptr()),
-                       'pbb_score_matrix')
+            _device.call('pbb_score_matrix', m[:, 1:], m, F * T, F * T, K, F - 1, T, self._metric, scores)
             pair = _mapping_from_score_matrix(scores, 'greedy')
-        _lib.check(lib.pbb_chain_mapping(_device.ptr(pair), K, F, _device.ptr(mapping), _device.stream_ptr()),
-                   'pbb_chain_mapping')
+        _device.call('pbb_chain_mapping', pair, K, F, mapping)
         return _device.to_host(mapping, like_numpy)
 
 

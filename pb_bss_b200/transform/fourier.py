@@ -129,9 +129,7 @@ class _Stft(torch.autograd.Function):
         rows = int(np.prod(lead, dtype=np.int64))
         if out.numel():
             dtype = _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64
-            _lib.check(_lib.load().pbb_stft(_device.ptr(xd), dtype, rows, n, size, shift, wl, offset, T,
-                                            _device.ptr(window), _device.ptr(_twiddle(size)), _device.ptr(out),
-                                            _device.stream_ptr()), 'pbb_stft')
+            _device.call('pbb_stft', xd, dtype, rows, n, size, shift, wl, offset, T, window, _twiddle(size), out)
         ctx.args = (lead, n, rows, size, shift, wl, offset, T, window, xd.dtype)
         return out
 
@@ -145,9 +143,8 @@ class _Stft(torch.autograd.Function):
             lib = _lib.load()
             nbytes = lib.pbb_stft_backward_workspace_bytes(rows, T, wl)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_stft_backward(_device.ptr(g), rows, n, size, shift, wl, offset, T, _device.ptr(window),
-                                             _device.ptr(_twiddle(size)), _device.ptr(ws), nbytes, _device.ptr(gx),
-                                             _device.stream_ptr()), 'pbb_stft_backward')
+            _device.call('pbb_stft_backward', g, rows, n, size, shift, wl, offset, T, window, _twiddle(size), ws,
+                         nbytes, gx)
         else:
             gx.zero_()
         return gx.to(dtype), None, None, None, None, None, None
@@ -166,9 +163,8 @@ class _Istft(torch.autograd.Function):
             lib = _lib.load()
             nbytes = lib.pbb_istft_workspace_bytes(rows, T, wl)
             ws = _device.workspace(nbytes)
-            _lib.check(lib.pbb_istft(_device.ptr(X), rows, T, size, shift, wl, crop, n_out, _device.ptr(synthesis),
-                                     _device.ptr(_twiddle(size)), _device.ptr(ws), nbytes, _device.ptr(out),
-                                     _device.stream_ptr()), 'pbb_istft')
+            _device.call('pbb_istft', X, rows, T, size, shift, wl, crop, n_out, synthesis, _twiddle(size), ws, nbytes,
+                         out)
         else:
             out.zero_()
         ctx.args = (lead, T, rows, n_out, size, shift, wl, crop, synthesis)
@@ -181,9 +177,8 @@ class _Istft(torch.autograd.Function):
         gX = _device.empty(lead + (T, size // 2 + 1), torch.complex128)
         if rows and T:
             g = grad.to(torch.float64).contiguous()
-            _lib.check(_lib.load().pbb_istft_backward(_device.ptr(g) if n_out else None, rows, T, size, shift, wl,
-                                                      crop, n_out, _device.ptr(synthesis), _device.ptr(_twiddle(size)),
-                                                      _device.ptr(gX), _device.stream_ptr()), 'pbb_istft_backward')
+            _device.call('pbb_istft_backward', g if n_out else None, rows, T, size, shift, wl, crop, n_out, synthesis,
+                         _twiddle(size), gX)
         else:
             gX.zero_()
         return gX, None, None, None, None, None
@@ -202,10 +197,6 @@ def griffin_lim_stft(x_hat, X, y, size, shift, fading):
                          f'({K},{T},{size // 2 + 1})')
     Xdd = _device.empty((K, T, size // 2 + 1), torch.complex128)
     Xd = torch.empty_like(Xdd)
-    lib = _lib.load()
-    _lib.check(lib.pbb_griffin_lim_stft(_device.ptr(x_hat), K, n, _device.ptr(y), _device.ptr(X), size, shift, wl,
-                                        wl - shift if fading else 0, T,
-                                        _device.ptr(_analysis_window(window, wl, False)), _device.ptr(_twiddle(size)),
-                                        _device.ptr(Xdd), _device.ptr(Xd), _device.stream_ptr()),
-               'pbb_griffin_lim_stft')
+    _device.call('pbb_griffin_lim_stft', x_hat, K, n, y, X, size, shift, wl, wl - shift if fading else 0, T,
+                 _analysis_window(window, wl, False), _twiddle(size), Xdd, Xd)
     return Xdd, Xd

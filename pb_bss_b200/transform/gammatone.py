@@ -162,7 +162,6 @@ def filterbank_tensor(xd, sample_rate, n, low_freq, high_freq):
         coef, trans = _device_tables(sample_rate, n, low_freq, high_freq, L)
         nbytes = lib.pbb_gammatone_workspace_bytes(rows, n, N)
         ws = _device.workspace(nbytes) if nbytes else None
-        _lib.check(lib.pbb_gammatone(_device.ptr(xd), _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64,
-                                     rows, N, n, _device.ptr(coef), _device.ptr(trans), L, _device.ptr(ws), nbytes,
-                                     _device.ptr(out), _device.stream_ptr()), 'pbb_gammatone')
+        _device.call('pbb_gammatone', xd, _lib.PBB_F32 if xd.dtype == torch.float32 else _lib.PBB_F64, rows, N, n, coef,
+                     trans, L, ws, nbytes, out)
     return out

@@ -137,10 +137,8 @@ def labels_to_one_hot(labels, categories: int, axis: int = 0, keepdims=False, dt
         lab = lab.to(torch.int64).contiguous()
         out = torch.empty(out_shape, dtype=_TORCH_DTYPES[np_dtype], device=_device.device())
     status = torch.zeros((), dtype=torch.int32, device=_device.device())
-    lib = _lib.load()
-    _lib.check(lib.pbb_labels_to_one_hot(_device.ptr(lab) if lab.numel() else None, outer, inner, int(categories),
-                                         np_dtype.itemsize, one, _device.ptr(out) if out.numel() else None,
-                                         _device.ptr(status), _device.stream_ptr()), 'pbb_labels_to_one_hot')
+    _device.call('pbb_labels_to_one_hot', lab if lab.numel() else None, outer, inner, int(categories),
+                 np_dtype.itemsize, one, out if out.numel() else None, status)
 
     def on_error(s):
         raise IndexError(f'index {int(lab.reshape(-1)[s - 1])} is out of bounds for axis 0 with size {categories}')
@@ -174,9 +172,8 @@ def abs_square(x):
         dtype = torch.float64
     t = t.contiguous()
     out = _device.empty(tuple(t.shape), _nd.REAL.get(t.dtype, t.dtype))
-    lib = _lib.load()
-    _lib.check(lib.pbb_abs_square(_device.ptr(t) if t.numel() else None, _ABS_SQUARE_CODES[t.dtype], t.numel(),
-                                  _device.ptr(out) if out.numel() else None, _device.stream_ptr()), 'pbb_abs_square')
+    _device.call('pbb_abs_square', t if t.numel() else None, _ABS_SQUARE_CODES[t.dtype], t.numel(),
+                 out if out.numel() else None)
     if out.dtype != _nd.REAL.get(dtype, dtype):
         out = out.to(_nd.REAL.get(dtype, dtype))
     return _device.to_host(out, like)

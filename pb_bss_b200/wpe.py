@@ -134,9 +134,8 @@ def _run(Y, taps, delay, iterations, psd_context, statistics_mode, inplace):
     nbytes = lib.pbb_wpe_workspace_bytes(group, D, T, taps, delay, valid)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
     status = torch.zeros(1, dtype=torch.int32, device=y.device)
-    _lib.check(lib.pbb_wpe(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(out), *os_,
-                           taps, delay, iterations, _context(psd_context), valid, group, _device.ptr(ws), nbytes,
-                           _device.ptr(status), _device.stream_ptr()), 'pbb_wpe')
+    _device.call('pbb_wpe', y, _device.complex_dtype_code(y), bins, D, T, *ys, out, *os_, taps, delay, iterations,
+                 _context(psd_context), valid, group, ws, nbytes, status)
     if inplace and out.data_ptr() != Y.data_ptr():
         Y.copy_(out)
         out = Y
@@ -180,9 +179,8 @@ def _power_backward(y, ys, G, taps, delay, c, mode, gin, xbar):
     lib = _lib.load()
     nbytes = lib.pbb_wpe_power_backward_workspace_bytes(bins, T)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=xbar.device)
-    _lib.check(lib.pbb_wpe_power_backward(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys,
-                                          _device.ptr(G), taps, delay, c, mode, _device.ptr(gin), _device.ptr(xbar),
-                                          _device.ptr(ws), nbytes, _device.stream_ptr()), 'pbb_wpe_power_backward')
+    _device.call('pbb_wpe_power_backward', y, _device.complex_dtype_code(y), bins, D, T, *ys, G, taps, delay, c, mode,
+                 gin, xbar, ws, nbytes)
 
 
 def _step_backward(y, ys, w, G, xbar, ybar, taps, delay, valid):
@@ -190,10 +188,8 @@ def _step_backward(y, ys, w, G, xbar, ybar, taps, delay, valid):
     bins, D, T = xbar.shape
     group, ws = _backward_workspace(bins, D, T, taps, delay, valid)
     wbar = torch.empty((bins, T), dtype=torch.float64, device=xbar.device)
-    _lib.check(_lib.load().pbb_wpe_backward(
-        _device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(w), _device.ptr(G),
-        _device.ptr(xbar), taps, delay, valid, _device.ptr(ybar), _device.ptr(wbar), group, _device.ptr(ws),
-        ws.numel(), _device.stream_ptr()), 'pbb_wpe_backward')
+    _device.call('pbb_wpe_backward', y, _device.complex_dtype_code(y), bins, D, T, *ys, w, G, xbar, taps, delay, valid,
+                 ybar, wbar, group, ws, ws.numel())
     return wbar
 
 
@@ -219,11 +215,9 @@ class _Wpe(torch.autograd.Function):
         status = torch.zeros(1, dtype=torch.int32, device=y.device)
         G = torch.empty((iterations, bins, taps * D, D), dtype=torch.complex128, device=y.device)
         w = torch.empty((iterations, bins, T), dtype=torch.float64, device=y.device)
-        _lib.check(lib.pbb_wpe_forward(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(out),
-                                       *os_, taps, delay, iterations, c, valid, group, _device.ptr(ws), nbytes,
-                                       _device.ptr(status), _device.ptr(G) if iterations else None,
-                                       _device.ptr(w) if iterations else None, _device.stream_ptr()),
-                   'pbb_wpe_forward')
+        _device.call('pbb_wpe_forward', y, _device.complex_dtype_code(y), bins, D, T, *ys, out, *os_, taps, delay,
+                     iterations, c, valid, group, ws, nbytes, status, G if iterations else None,
+                     w if iterations else None)
         ctx.save_for_backward(y, G, w)
         ctx.args = (ys, taps, delay, iterations, c, valid, Y.shape, Y.dtype)
         return out
@@ -291,8 +285,8 @@ def _power_launch(x, c, inverse):
         x, xs = _layout(x)
         nbytes = lib.pbb_wpe_power_workspace_bytes(bins, T)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-        _lib.check(lib.pbb_wpe_power(_device.ptr(x), _device.complex_dtype_code(x), bins, D, T, *xs, c, int(inverse),
-                                     _device.ptr(out), _device.ptr(ws), nbytes, _device.stream_ptr()), 'pbb_wpe_power')
+        _device.call('pbb_wpe_power', x, _device.complex_dtype_code(x), bins, D, T, *xs, c, int(inverse), out, ws,
+                     nbytes)
     return out, x, xs
 
 
@@ -337,10 +331,8 @@ class _WpeStep(torch.autograd.Function):
         ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device)
         status = torch.zeros(1, dtype=torch.int32, device=y.device)
         G = torch.empty((bins, taps * D, D), dtype=torch.complex128, device=y.device)
-        _lib.check(lib.pbb_wpe_step(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(w),
-                                    w.stride(0), w.stride(1), _device.ptr(out), *os_, taps, delay, valid, group,
-                                    _device.ptr(ws), nbytes, _device.ptr(status), _device.ptr(G),
-                                    _device.stream_ptr()), 'pbb_wpe_step')
+        _device.call('pbb_wpe_step', y, _device.complex_dtype_code(y), bins, D, T, *ys, w, w.stride(0), w.stride(1),
+                     out, *os_, taps, delay, valid, group, ws, nbytes, status, G)
         ctx.save_for_backward(y, w, G)
         ctx.args = (ys, taps, delay, valid, Y.shape, Y.dtype)
         return out
@@ -425,9 +417,7 @@ def build_y_tilde(Y, taps, delay):
     out = _device.empty(lead + (taps * D, T), y.dtype)
     if bins and T:
         y, ys = _layout(y)
-        _lib.check(_lib.load().pbb_wpe_build_y_tilde(_device.ptr(y), _device.complex_dtype_code(y), bins, D, T, *ys,
-                                                     taps, delay, _device.ptr(out), _device.stream_ptr()),
-                   'pbb_wpe_build_y_tilde')
+        _device.call('pbb_wpe_build_y_tilde', y, _device.complex_dtype_code(y), bins, D, T, *ys, taps, delay, out)
     return _device.to_host(out, like_numpy)
 
 
@@ -487,10 +477,8 @@ def _online(y, hist, power, Q, G, taps, delay, alpha):
     yv, ys = _frames(y) if T else (y, (0, 0, 0))
     zv, zs = _frames(Z) if T else (Z, (0, 0, 0))
     hv, hs = _frames(hist) if hist is not None else (None, (0, 0, 0))
-    _lib.check(_lib.load().pbb_wpe_online(
-        _device.ptr(yv) if T else None, _device.complex_dtype_code(y), bins, D, T, *ys, _device.ptr(hv), *hs,
-        _device.ptr(power), _device.ptr(Q), _device.ptr(G), _device.ptr(zv) if T else None, *zs, _device.ptr(Qo),
-        _device.ptr(Go), taps, delay, float(alpha), _device.stream_ptr()), 'pbb_wpe_online')
+    _device.call('pbb_wpe_online', yv if T else None, _device.complex_dtype_code(y), bins, D, T, *ys, hv, *hs, power, Q,
+                 G, zv if T else None, *zs, Qo, Go, taps, delay, float(alpha))
     return Z, Qo, Go
 
 

@@ -16,15 +16,20 @@ def _declared_symbols():
     return sorted(set(re.findall(r'\b(pbb_[a-z0-9_]+)\s*\(', text)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_every_declared_symbol_is_exported_and_parsed():
+    """Every pbb_* declaration of include/pbb.h is exported by the library and bound with the argtypes and restype
+    parsed from the header."""
     from pb_bss_b200 import _lib
     lib = _lib.load()
     names = _declared_symbols()
     assert len(names) >= 6, names
     for n in names:
         assert hasattr(lib, n), f'{n} declared in include/pbb.h but not exported'
-        assert n in _lib.SIGNATURES, f'{n} has no ctypes signature in _lib.py'
-    assert set(_lib.SIGNATURES) == set(names)
+        assert n in _lib.DECLARATIONS, f'{n} is not parsed from include/pbb.h'
+        decl = _lib.DECLARATIONS[n]
+        assert getattr(lib, n).argtypes == [p.ctype for p in decl.params], n
+        assert getattr(lib, n).restype is decl.restype, n
+    assert set(_lib.DECLARATIONS) == set(names)
 
 
 def test_version_error_string_and_workspace_size():
@@ -189,3 +194,136 @@ def test_deferred_status_scope_host_logic():
     _device.check_status(ok, raiser('a'))                       # and the scope is gone afterwards
     with pytest.raises(ValueError, match='b:3'):
         _device.check_status(bad3, raiser('b'))
+
+
+def _header_code():
+    text = open(os.path.join(ROOT, 'include', 'pbb.h')).read()
+    return re.sub(r'/\*.*?\*/|//[^\n]*', ' ', text, flags=re.S)
+
+
+def test_parsed_signatures():
+    """Spot checks of the ctypes signatures _lib reads from include/pbb.h."""
+    from pb_bss_b200 import _lib
+    decls = _lib.parse_header()
+    fit = decls['pbb_cacgmm_fit']
+    assert len(fit.params) == 17 and fit.streamed
+    assert fit.params[9].ctype is ctypes.POINTER(_lib.CacgmmOptions)
+    assert [p.pointee for p in fit.params if p.name == 'eigenvalues'] == ['double']
+    assert [p.pointee for p in fit.params if p.name == 'y'] == ['void']
+    assert fit.params[4].ctype is ctypes.c_int and fit.params[4].pointee is None
+    assert decls['pbb_cacgmm_workspace_bytes'].restype is ctypes.c_size_t
+    assert decls['pbb_last_error'].restype is ctypes.c_char_p and decls['pbb_last_error'].params == ()
+    assert decls['pbb_profile_reset'].restype is None
+    assert decls['pbb_launch_count'].restype is ctypes.c_longlong
+    host_only = {'pbb_last_error', 'pbb_version', 'pbb_launch_count', 'pbb_profile_enable', 'pbb_profile_reset',
+                 'pbb_profile_dominant', 'pbb_profile_dump', 'pbb_streamed_task_order', 'pbb_em_dispatch',
+                 'pbb_em_last_plan', 'pbb_stft_frames_per_cta', 'pbb_gammatone_chunk_length', 'pbb_srmr_fft_log2'}
+    for name, decl in decls.items():
+        names = [p.name for p in decl.params]
+        if name in host_only or name.endswith(('_bytes', '_doubles')):
+            assert not decl.streamed and 'stream' not in names, name
+        else:  # every device entry point returns a status and takes the stream last
+            assert decl.streamed and decl.restype is ctypes.c_int and names.count('stream') == 1, name
+    assert sum(d.streamed for d in decls.values()) >= 100
+
+
+def test_unknown_c_type_is_an_import_error(tmp_path):
+    from pb_bss_b200 import _lib
+    header = tmp_path / 'pbb.h'
+    header.write_text('int pbb_ok(const double* x, long long n, void* stream);\n')
+    assert _lib.parse_header(str(header))['pbb_ok'].params[1].ctype is ctypes.c_longlong
+    for decl in ('int pbb_bad(float x, void* stream);', 'int pbb_bad(const double** x, void* stream);',
+                 'unsigned pbb_bad(void);', 'double* pbb_bad(void);', 'int pbb_bad(int, void* stream);'):
+        header.write_text(decl + '\n')
+        with pytest.raises(ImportError, match='pbb_bad'):
+            _lib.parse_header(str(header))
+
+
+def test_mirrored_constants_match_the_header():
+    """The integer constants and the three structs of _lib.py are hand-mirrored; they must equal include/pbb.h."""
+    from pb_bss_b200 import _lib
+    code = _header_code()
+    consts = {n: int(v) for n, v in re.findall(r'#define\s+(PBB_\w+)\s+(-?\d+)\b', code)}
+    for body in re.findall(r'\benum\s*\{(.*?)\}', code, flags=re.S):
+        consts.update((n, int(v)) for n, v in re.findall(r'\b(PBB_\w+)\s*=\s*(-?\d+)', body))
+    mirrored = {n: v for n, v in vars(_lib).items() if n.isupper() and type(v) is int}
+    assert len(mirrored) >= 30
+    for name, value in mirrored.items():
+        c_name = name if name.startswith('PBB_') else 'PBB_' + name
+        assert c_name in consts, f'_lib.{name} has no counterpart in include/pbb.h'
+        assert value == consts[c_name], (name, value, consts[c_name])
+
+    scalars = {'int': ctypes.c_int, 'double': ctypes.c_double, 'long long': ctypes.c_longlong}
+    for c_name, cls in (('pbb_cacgmm_options', _lib.CacgmmOptions), ('pbb_mask_layout', _lib.MaskLayout),
+                        ('pbb_nd_layout', _lib.NdLayout)):
+        body = re.search(r'typedef\s+struct\s+%s\s*\{(.*?)\}\s*%s\s*;' % (c_name, c_name), code, flags=re.S).group(1)
+        fields = []
+        for ctype, name, dims in re.findall(r'([A-Za-z_][\w ]*?)\s+(\w+)\s*((?:\[\w+\])*)\s*;', body):
+            t = scalars[' '.join(ctype.split())]
+            for dim in reversed(re.findall(r'\[(\w+)\]', dims)):
+                t = t * (int(dim) if dim.isdigit() else consts[dim])
+            fields.append((name, t))
+        assert cls._fields_ == fields, c_name
+        assert ctypes.sizeof(cls) == sum(ctypes.sizeof(t) for _, t in fields), c_name  # no padding to disagree on
+
+
+@pytest.fixture
+def no_device_work(monkeypatch):
+    """_device.call without a GPU: reading the stream fails the test, and the library function is replaced by a
+    recorder, so a check that passed would be seen."""
+    import torch
+    from pb_bss_b200 import _device
+
+    calls = []
+
+    def stream():
+        raise AssertionError('the stream was read')
+
+    def stub(*args):
+        calls.append(args)
+        return 0
+    monkeypatch.setattr(torch.cuda, 'current_stream', stream)
+    for name in ('pbb_apply_mapping', 'pbb_mapping_from_score_matrix', 'pbb_cacgmm_fit'):
+        monkeypatch.setitem(_device._entries, name, (stub,) + _device._entry(name)[1:])
+    yield calls
+    assert calls == []
+
+
+def test_device_call_rejects_bad_arguments_before_any_device_work(no_device_work):
+    import torch
+    from pb_bss_b200 import _device
+    f64 = torch.zeros(4, dtype=torch.float64)
+    with pytest.raises(TypeError, match='not declared'):
+        _device.call('pbb_no_such_function', None)
+    with pytest.raises(TypeError, match='does not take a stream'):
+        _device.call('pbb_cacgmm_workspace_bytes', 1, 1, 1, 1)
+    with pytest.raises(TypeError, match='takes 6 arguments'):
+        _device.call('pbb_apply_mapping', None, None, 1, 1, 1)
+    with pytest.raises(TypeError, match='argument 1 wants torch.float64, got torch.float32'):
+        _device.call('pbb_apply_mapping', torch.zeros(4, dtype=torch.float32), None, 1, 1, 1, None)
+    with pytest.raises(TypeError, match='argument 6 wants torch.int32, got torch.int64'):
+        _device.call('pbb_mapping_from_score_matrix', None, 1, 1, 0, None, torch.zeros(1, dtype=torch.int64))
+    with pytest.raises(TypeError, match='argument 5 wants torch.int64, got torch.int32'):
+        _device.call('pbb_mapping_from_score_matrix', None, 1, 1, 0, torch.zeros(1, dtype=torch.int32), None)
+    with pytest.raises(ValueError, match='argument 1 is in pageable host memory'):
+        _device.call('pbb_apply_mapping', f64, None, 1, 1, 1, None)
+    with pytest.raises(TypeError, match='argument 2 is a pointer'):
+        _device.call('pbb_apply_mapping', None, f64.data_ptr(), 1, 1, 1, None)
+    with pytest.raises(TypeError, match='argument 3 is a scalar'):
+        _device.call('pbb_apply_mapping', None, None, torch.tensor(1), 1, 1, None)
+    with pytest.raises(TypeError, match='argument 10 wants no tensor'):
+        _device.call('pbb_cacgmm_fit', None, 1, 1, 1, 4, 2, None, None, None, torch.zeros(1), None, None, None, None,
+                     0, None)
+
+
+def test_device_call_passes_null_ctypes_objects_and_the_stream(no_device_work, monkeypatch):
+    import torch
+    from pb_bss_b200 import _device, _lib
+
+    class Stream:
+        cuda_stream = 1234
+    monkeypatch.setattr(torch.cuda, 'current_stream', lambda: Stream)
+    opts = ctypes.byref(_lib.CacgmmOptions())
+    _device.call('pbb_cacgmm_fit', None, 1, 1, 1, 4, 2, None, None, None, opts, None, None, None, None, 0, None)
+    assert no_device_work == [(None, 1, 1, 1, 4, 2, None, None, None, opts, None, None, None, None, 0, None, 1234)]
+    no_device_work.clear()
